@@ -1,11 +1,11 @@
 #!/usr/bin/env python3
 """bench.py — PageRank GTEPS (edges/sec/iter) on synthetic RMAT, the headline metric of BASELINE.json.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--scale S] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--scale S] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one graph: `page_rank` with 20 forced sweeps
 (tolerance 0, damping 0.85) on the RMAT scale-S graph (default 26 = the configuration the metric is
-quoted on; it fits one B200).  One JSON line is printed by rank 0.
+quoted on; it fits one 80 GB H100).  One JSON line is printed by rank 0.
 
   value        m * sweeps * K / device time of K steps, graph resident in HBM, result left in HBM
   e2e          same metric through the C ABI with HOST buffers (gb_page_rank_csr_u32): every step uploads
@@ -16,6 +16,9 @@ quoted on; it fits one B200).  One JSON line is printed by rank 0.
   cpu_baseline the reference's multi-threaded in-place sweep (oracle.page_rank_mt, the C restatement
                of crates/algos/src/page_rank.rs:113-168) on the same graph, bounded sample
   --impl reference   times that CPU path alone, all host threads, same metric / config
+  --dump-outputs DIR writes what the timed path returned in its last step as DIR/<name>.npy (float32 or
+               float64; an output of more than DUMP_SAMPLE entries is stored as a fixed seeded sample,
+               with the sampled positions in DIR/<name>_index.npy), so two builds can be compared
 """
 from __future__ import annotations
 
@@ -35,7 +38,6 @@ ROOT = Path(__file__).resolve().parent
 sys.path.insert(0, str(ROOT))
 
 SWEEPS = 20
-PR_KERNEL_VERSION = "r02-cb16"   # bump with every change of the sweep kernels / layout (keys profiles/pr_traffic.json)
 DAMPING = 0.85
 SEED = 42
 EDGE_FACTOR = 16
@@ -48,7 +50,7 @@ def peaks():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 class ClockSampler:
@@ -112,6 +114,26 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": self.max_mhz, "reasons": [], "samples": 0}
         return {"sm_mhz": float(np.median(self.samples)), "sm_max_mhz": self.max_mhz,
                 "reasons": sorted(self.reasons), "samples": len(self.samples)}
+
+
+DUMP_SAMPLE = 1 << 21   # entries kept of a larger output (seeded, sorted positions): <= 48 MB per dump
+
+
+def dump_outputs(dirname, arrays):
+    """--dump-outputs: name -> host array, written as float32 (f32 outputs) or float64 (everything else,
+    exact for integer ids); outputs longer than DUMP_SAMPLE are sampled at fixed seeded positions."""
+    if not dirname:
+        return
+    out = Path(dirname)
+    out.mkdir(parents=True, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a).reshape(-1)
+        a = a.astype(np.float32 if a.dtype == np.float32 else np.float64)
+        if a.size > DUMP_SAMPLE:
+            idx = np.unique(np.random.default_rng(SEED).integers(0, a.size, DUMP_SAMPLE))
+            np.save(out / f"{name}_index.npy", idx.astype(np.float64))
+            a = a[idx]
+        np.save(out / f"{name}.npy", a)
 
 
 def pinned_empty(count: int, dtype):
@@ -215,8 +237,11 @@ def run_reference(args):
         oracle.page_rank_mt(in_off, in_tgt, out_off, 1, 0.0, DAMPING, 0)
     t0 = time.perf_counter()
     for _ in range(args.steps):
-        oracle.page_rank_mt(in_off, in_tgt, out_off, sample_sweeps, 0.0, DAMPING, 0)
+        res = oracle.page_rank_mt(in_off, in_tgt, out_off, sample_sweeps, 0.0, DAMPING, 0)
     dt = time.perf_counter() - t0
+    if args.steps:
+        scores, it, err = res
+        dump_outputs(args.dump_outputs, {"scores": scores, "ran_iterations": [it], "error": [err]})
     gteps = m * sample_sweeps * args.steps / dt / 1e9
     sample = f"{sample_sweeps} of {SWEEPS} sweeps per step on the full RMAT scale-{scale} graph; input prep: {prep}"
     line = {
@@ -275,6 +300,8 @@ def run_single(args):
         torch.cuda.synchronize()
     ms = ev0.elapsed_time(ev1)
     assert it.value == SWEEPS
+    dump_outputs(args.dump_outputs, {"scores": d_scores.cpu().numpy(), "ran_iterations": [it.value],
+                                     "error": [err.value]})
     gteps = m * SWEEPS * args.steps / (ms * 1e-3) / 1e9
 
     # dominant kernel, timed live with CUDA events around every launch (separate pass)
@@ -288,17 +315,7 @@ def run_single(args):
     peak, peak_src = peaks()
     bytes_per_launch = algorithmic_bytes(n, m)
     achieved = bytes_per_launch / (hot_ms / hot_n * 1e-3) / 1e9 if hot_n else 0.0
-    # DRAM bytes per sweep from the committed ncu capture of THIS kernel version and layout (else null)
-    traffic, traffic_src = None, None
-    tp = ROOT / "profiles" / "pr_traffic.json"
-    if tp.exists():
-        try:
-            rec = json.loads(tp.read_text())
-            if rec.get("kernel_version") == PR_KERNEL_VERSION:
-                traffic = rec.get(f"scale{scale}")
-                traffic_src = rec.get("source")
-        except Exception:
-            traffic = None
+    traffic, traffic_src = None, None  # DRAM bytes per sweep: not measured
     roofline = {"bound": "hbm", "kernel": "k_pr_cb + k_pr_sell + k_pr_finish (one sweep)", "achieved": achieved,
                 "peak": peak, "unit": "GB/s",
                 "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
@@ -394,6 +411,8 @@ def run_multi(args):
     stats = spr.backend.stats
     # untimed verification: the sharded ranks against a single-GPU run of the same graph on rank 0
     sharded = spr.scores_host()
+    if rank == 0:
+        dump_outputs(args.dump_outputs, {"scores": sharded, "ran_iterations": [SWEEPS]})
     verified, verification = None, None
     if rank == 0:
         single = g.page_rank(max_iterations=SWEEPS, tolerance=0.0, damping_factor=DAMPING, mode="jacobi").scores()
@@ -477,13 +496,14 @@ def run_algo(args):
     torch.cuda.set_device(0)
     gb.set_device(0)
     peak, peak_src = peaks()
-    reps = max(args.steps, 3)
+    reps = args.steps
 
     def timed(fn):
         for _ in range(max(args.warmup, 1)):
             fn()
         dev, wall, launches = [], [], 0
         res = None
+        assert reps >= 1, "--steps must be >= 1"
         for _ in range(reps):
             t0 = time.perf_counter()
             res = fn()
@@ -499,6 +519,7 @@ def run_algo(args):
         g = gb.DiGraph.rmat(scale, EDGE_FACTOR, SEED, gb.Layout.Sorted)
         with ClockSampler(0) as clocks:
             res, dev_ms, wall_ms, launches = timed(lambda: g.wcc())
+        dump_outputs(args.dump_outputs, {"components": res.components()})
         byts = 8 * m + 16 * n + 8
         comp = res.components()
         oo, ot = g.csr("out")
@@ -533,6 +554,7 @@ def run_algo(args):
             g.make_degree_ordered()
             relabel_ms = (time.perf_counter() - t0) * 1e3
             res, dev_ms, wall_ms, launches = timed(lambda: g.global_triangle_count())
+        dump_outputs(args.dump_outputs, {"triangles": [res.triangles]})
         launches += l0
         byts = 8 * m + 4 * (n + 1)
         cpu, verified = None, None
@@ -564,6 +586,7 @@ def run_algo(args):
         delta = 0.05
         with ClockSampler(0) as clocks:
             res, dev_ms, wall_ms, launches = timed(lambda: g.delta_stepping(start_node=start, delta=delta))
+        dump_outputs(args.dump_outputs, {"distances": res.distances()})
         d = res.distances()
         byts = 8 * m + 4 * (n + 1) + 8 * n
         cpu, verified = None, None
@@ -609,6 +632,8 @@ def main():
     ap.add_argument("--exchange", default="auto", choices=["auto", "peer", "allgather"])
     ap.add_argument("--no-multicast", action="store_true", help="multi-GPU: unicast peer stores instead of multimem.st")
     ap.add_argument("--diag", action="store_true", help="multi-GPU: print per-rank kernel / exchange ms per sweep")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32/float64, <= 64 MB)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """The reference's end-to-end walk-through (crates/algos/examples/usage-demo.rs and
 crates/mate/notebooks/usage-demo.ipynb) against graph_b200: load a Graph500 file, PageRank, WCC,
-to_undirected, make_degree_ordered, triangle count.  Needs a B200.
+to_undirected, make_degree_ordered, triangle count.  Needs an H100.
 
   python examples/usage_demo.py [path.graph500]      # default: synthetic RMAT scale-20 written to /tmp
 """

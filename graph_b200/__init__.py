@@ -1,4 +1,4 @@
-"""graph_b200 — B200-native drop-in for the CSR hot path of neo4j-labs/graph.
+"""graph_b200 — H100-native drop-in for the CSR hot path of neo4j-labs/graph.
 
 The public names mirror the reference's Python module ``graph_mate`` (crates/mate/graph_mate.pyi:
 ``DiGraph``, ``Graph``, ``Layout``, ``FileFormat``, ``PageRankResult``, ``WccResult``,

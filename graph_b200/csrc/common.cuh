@@ -185,7 +185,9 @@ gb_status new_graph(int device, gb_graph_kind kind, uint32_t n, gb_graph** out);
 gb_status upload_host_csr(cudaStream_t s, uint32_t n, const uint32_t* off, const uint32_t* tgt, const float* w,
                           DevCsr* csr, const char* what);
 
-inline unsigned grid_for(uint64_t items, unsigned block, unsigned max_blocks = 148u * 16u) {
+constexpr unsigned H100_SMS = 132;  // streaming multiprocessors of an H100 SXM: sizes the grid-stride grids
+
+inline unsigned grid_for(uint64_t items, unsigned block, unsigned max_blocks = H100_SMS * 16u) {
   uint64_t b = (items + block - 1) / block;
   if (b < 1) b = 1;
   if (b > max_blocks) b = max_blocks;

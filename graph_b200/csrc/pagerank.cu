@@ -9,10 +9,10 @@
 //            reference wherever the reference is deterministic (n <= 16384 = one chunk).
 //   JACOBI — the throughput path (double-buffered, deterministic).
 //
-// JACOBI design (round 2).  A pull sweep issues one 4-byte gather per edge, and divergent gathers
-// that miss L1 are limited to ~1 per clock per SM by the L1TEX->XBAR request port
-// (profiles/r01_gather_ceiling_microbench.txt) — 27 % of the HBM roofline, whatever the layout of the
-// index stream.  Shared memory serves ~9 random 4-byte reads per clock.  So the sweep is COLUMN
+// JACOBI design.  A pull sweep issues one 4-byte gather per edge, and divergent gathers that miss L1
+// are limited by the L1TEX->XBAR request rate (profiles/microbench/gather_ceiling.cu), whatever the
+// layout of the index stream, far below the HBM roofline.  Shared memory serves several random 4-byte
+// reads per clock.  So the sweep is COLUMN
 // BLOCKED: vertices are renumbered by in-degree descending, then out-degree descending (hot sources
 // first); the source vector is cut into blocks of B entries that fit in shared memory, and every
 // (row, block) pair that is expected to hold at least tau edges gets a SEGMENT of 16-bit block-local
@@ -21,7 +21,7 @@
 // shared memory, and reduce lanes that belong to the same row with a segmented warp scan; one f32
 // partial per (row, block) pair goes back to HBM.  Edges of pairs below the threshold (and all edges
 // of short rows) stay in a SELL-32 layout with 32-bit ids: one lane per row, gathers through L1/L2
-// (no shared memory: the whole 228 KB serve as L1); that kernel also completes every row whose
+// (no shared memory: the whole L1 / shared-memory array serves as L1); that kernel also completes every row whose
 // segments lie in at most 4 blocks.  A finish kernel adds the hub rows' partials in a fixed order
 // (f64), applies the update of page_rank.rs:148-158 and reduces the sweep error.
 // Everything is deterministic: bit-identical run to run for a given shard count; across shard counts the
@@ -706,11 +706,10 @@ struct PrArgs {
   uint32_t sweep_no;  // 1-based global sweep number
 };
 
-// 8 gathers per lane in straight-line predicated code (padding id ~0 reads nothing).  Measured in round 1
-// (profiles/r01_sweep_hot_head.txt): per-target if/else made every load wait for a scoreboard slot of
-// the previous one, and every pending miss holds an L1 line — so this kernel uses NO shared memory at
-// all and leaves the whole 228 KB to L1 (a 128 KB shared-memory mirror of the hottest sources was
-// slower than two mirror-less CTAs per SM: profiles/r02_sweep_breakdown.txt).
+// 8 gathers per lane in straight-line predicated code (padding id ~0 reads nothing): per-target if/else
+// makes every load wait for a scoreboard slot of the previous one, and every pending miss holds an L1
+// line — so this kernel uses NO shared memory at all and leaves the whole L1 / shared-memory array to L1
+// (a 128 KB shared-memory mirror of the hottest sources was slower than two mirror-less CTAs per SM).
 __device__ __forceinline__ void pr_gather(const float* x, const uint4& ta, const uint4& tb, float (&v)[8]) {
   const uint32_t t[8] = {ta.x, ta.y, ta.z, ta.w, tb.x, tb.y, tb.z, tb.w};
 #pragma unroll
@@ -875,8 +874,8 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
 // is split into one contiguous RANGE per CTA, each with its own atomic cursor: a CTA first drains its own
 // range — consecutive tasks of one block, so the 192 KB block is loaded once, not once per task — and then
 // steals from the other ranges' cursors.  Self-balancing whatever else shares the SM and however uneven the
-// thin blocks are (a purely static split ran 2.4x slower, one global cursor reloads the block for every
-// task: profiles/r02_sweep_breakdown.txt).  Claiming the next task one task ahead (to hide the atomic's
+// thin blocks are (a purely static split leaves thin blocks at single-warp latency, one global cursor reloads the
+// block for every task).  Claiming the next task one task ahead (to hide the atomic's
 // round trip) was measured and dropped: a claimed task cannot be stolen, which costs more at the tail.
 template <int NT>
 __device__ __forceinline__ void pr_cb_body(const PrArgs& a) {
@@ -1386,7 +1385,7 @@ static gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan
   DevBufStreamScope scope(s);
   const TargetFeed* feed = g->feed;
   gb_status st = [&]() -> gb_status {
-    int dev_sms = 148;
+    int dev_sms = H100_SMS;
     GB_CUDA(cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, g->device));
     // knobs (experiments; defaults are the measured optima)
     uint32_t B = env_u32("GB_PR_BLOCK", CB_BLOCK_DEFAULT);
@@ -1748,9 +1747,9 @@ static gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan
     p->smem_cb = ((size_t)B + 4) * sizeof(float);
     GB_CUDA(cudaFuncSetAttribute(k_pr_cb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cb));
     GB_CUDA(cudaFuncSetAttribute(k_pr_cb_half, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cb));
-    // GB_PR_DUAL=1 (experiment): k_pr_cb_half and k_pr_sell at the same time on two streams.  Measured
-    // (profiles/r02_sweep_breakdown.txt): both kernels load the same LSU data pipe, so the overlap buys
-    // <= 5 % at a 128 KB block and loses with larger blocks (k_pr_sell then starves for L1); default off.
+    // GB_PR_DUAL=1 (experiment): k_pr_cb_half and k_pr_sell at the same time on two streams.  Both kernels
+    // load the same LSU data pipe and k_pr_sell starves for L1 next to a large block: on an H100 at RMAT-26
+    // the overlap is slower than the sequential sweep (4.98 vs 4.56-4.77 ms); default off.
     p->dual = p->grid_cb > 0 && p->num_slices > 0 && env_u32("GB_PR_DUAL", 0) != 0;
     if (p->dual) {
       GB_CUDA(cudaStreamCreateWithFlags(&p->s2, cudaStreamNonBlocking));
@@ -1776,9 +1775,9 @@ static gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan
     // Role split of the finish CTAs: when every CTA has at most one pass of each kind to do (the grid is not
     // capped) and the hub chain is long (hundreds of blocks per row), CTAs [0, hub groups) take one hub
     // group each and the others the remaining rows — the two latency chains then run side by side instead
-    // of one after the other in every CTA.  Measured (profiles/r02_sweep_breakdown.txt): -20 % on an
-    // eighth-shard of RMAT-26; no gain when the grid is capped (RMAT-26 on one GPU) or the hub chain is
-    // short (RMAT-22), where every CTA keeps doing both parts.
+    // of one after the other in every CTA.  It pays on a shard of a large graph; there is nothing to gain
+    // when the grid is capped (RMAT-26 on one GPU) or the hub chain is short (RMAT-22), where every CTA keeps
+    // doing both parts.
     p->fin_hub_ctas = 0;
     if (want_fin <= (uint64_t)dev_sms * 8 && p->KB > 4 * FIN_CTA_BLOCKS && p->n_fin_warp && p->n_fin > p->n_fin_warp &&
         p->grid_fin > p->n_fin_warp / 32)

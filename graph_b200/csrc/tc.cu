@@ -130,7 +130,7 @@ extern "C" gb_status gb_triangle_count(const gb_graph* g, uint64_t* triangles) {
   GB_CUDA(cudaEventRecord(g->ev_begin, s));
   GB_CUDA(cudaMemsetAsync(total.p, 0, 8, s));
   if (g->out.len) {
-    k_tc<<<grid_for(g->out.len, 256, 148u * 32u), 256, 0, s>>>(g->out.off.p, g->out.tgt.p, g->n, g->out.len, total.p);
+    k_tc<<<grid_for(g->out.len, 256, H100_SMS * 32u), 256, 0, s>>>(g->out.off.p, g->out.tgt.p, g->n, g->out.len, total.p);
     g->timing.kernel_launches += 1;
   }
   GB_CUDA(cudaGetLastError());

@@ -1,4 +1,4 @@
-"""graph_b200.flight — the Arrow Flight front end of the reference (crates/server) over the B200 hot path.
+"""graph_b200.flight — the Arrow Flight front end of the reference (crates/server) over the H100 hot path.
 
 What a client of the reference's server sees is kept: the six JSON actions of actions.rs:28-55
 (`create`, `list`, `remove`, `compute`, `to_relabeled`, `to_undirected`), `do_put` with a
@@ -297,7 +297,7 @@ class GraphFlightServer(fl.FlightServerBase):
 
 def main(argv=None) -> None:
     import argparse
-    ap = argparse.ArgumentParser(description="Graph Arrow Server (B200)")
+    ap = argparse.ArgumentParser(description="Graph Arrow Server (H100)")
     ap.add_argument("host", nargs="?", default="127.0.0.1")
     ap.add_argument("port", nargs="?", type=int, default=50051)
     a = ap.parse_args(argv)

@@ -1,7 +1,7 @@
-// gather_ceiling.cu — what does a B200 SM sustain for divergent 4-byte gathers?
+// gather_ceiling.cu — what does an H100 SM sustain for divergent 4-byte gathers?
 // Measures random gathers from an f32 table (16 MiB: L2 resident; 256 MiB: larger than L2) through
 // (a) ld.global.nc, (b) tex1Dfetch, (c) half/half, (d) cp.async 4-byte global->shared, at several
-// occupancies.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o gather_ceiling gather_ceiling.cu
+// occupancies.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o gather_ceiling gather_ceiling.cu
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
@@ -53,7 +53,7 @@ __global__ void k_gather(const float* __restrict__ table, cudaTextureObject_t te
 template <int MODE>
 void run(const char* name, const float* table, cudaTextureObject_t tex, const uint32_t* idx, uint64_t count, float* out,
          int threads, int blocks_per_sm) {
-  int sms = 148;
+  int sms = 132;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   const int grid = sms * blocks_per_sm;
   size_t smem = (MODE == 3) ? (size_t)threads * 8 * 4 : 0;
@@ -86,7 +86,7 @@ int main() {
   for (int log_n : {22, 26}) {
     const uint64_t n = 1ull << log_n;
     float* table; CK(cudaMalloc(&table, n * 4)); CK(cudaMemset(table, 0, n * 4));
-    k_fill_idx<<<148 * 8, 256>>>(idx, count, (uint32_t)(n - 1));
+    k_fill_idx<<<132 * 8, 256>>>(idx, count, (uint32_t)(n - 1));
     cudaResourceDesc rd{}; rd.resType = cudaResourceTypeLinear; rd.res.linear.devPtr = table;
     rd.res.linear.desc = cudaCreateChannelDesc<float>(); rd.res.linear.sizeInBytes = n * 4;
     cudaTextureDesc td{}; td.readMode = cudaReadModeElementType;

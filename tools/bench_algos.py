@@ -9,7 +9,7 @@ ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
 import graph_b200 as gb
 
-PEAK = 6487.4
+PEAK = 3350.0  # GB/s, H100 SXM data sheet
 try:
     PEAK = float(json.loads((ROOT / "MEASURED_PEAKS.json").read_text())["hbm_gbs"])
 except Exception:
