@@ -497,6 +497,12 @@ class DiGraph(_Handle):
         check(lib.gb_page_rank_plan_info(self._g, C.byref(st)))
         return st.as_dict()
 
+    def page_rank_plan_shape(self) -> dict:
+        """Diagnostics: the launch shape of the JACOBI sweep kernels (built on first use)."""
+        sh = _capi.PrPlanShape()
+        check(lib.gb_page_rank_plan_shape(self._g, C.byref(sh)))
+        return sh.as_dict()
+
     # -- algorithms --
     def page_rank(self, *, max_iterations: int = PageRankConfig.DEFAULT_MAX_ITERATIONS,
                   tolerance: float = PageRankConfig.DEFAULT_TOLERANCE,

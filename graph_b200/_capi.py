@@ -53,6 +53,17 @@ class PrShardStats(C.Structure):
         return {k: int(getattr(self, k)) for k, _ in self._fields_}
 
 
+class PrPlanShape(C.Structure):
+    _fields_ = [("hot_blocks", C.c_uint32), ("n_cb", C.c_uint32), ("n_fin", C.c_uint32),
+                ("n_fin_warp", C.c_uint32), ("fin_u", C.c_uint32), ("fin_hub_ctas", C.c_uint32),
+                ("grid_cb", C.c_uint32), ("grid_sell", C.c_uint32), ("grid_fin", C.c_uint32),
+                ("n_mega", C.c_uint32), ("n_fix", C.c_uint32), ("fix_in_sell", C.c_uint32), ("dual", C.c_uint32),
+                ("last_hot_block", C.c_uint32)]
+
+    def as_dict(self):
+        return {k: int(getattr(self, k)) for k, _ in self._fields_}
+
+
 class GraphB200Error(RuntimeError):
     """CUDA / allocation failure inside libgraph_b200."""
 
@@ -100,9 +111,11 @@ SIGNATURES = {
     "gb_triangle_count": (C.c_int, [_P, C.POINTER(C.c_uint64)]),
     "gb_in_degree_partition": (C.c_int, [_P, C.c_uint32, _P]),
     "gb_page_rank_plan_info": (C.c_int, [_P, C.POINTER(PrShardStats)]),
+    "gb_page_rank_plan_shape": (C.c_int, [_P, C.POINTER(PrPlanShape)]),
     "gb_page_rank_plan_reset": (C.c_int, [_P]),
     "gb_pr_shard_create": (C.c_int, [_P, C.c_uint32, C.c_uint32, C.POINTER(_P)]),
     "gb_pr_shard_info": (C.c_int, [_P, C.POINTER(PrShardStats)]),
+    "gb_pr_shard_plan_shape": (C.c_int, [_P, C.POINTER(PrPlanShape)]),
     "gb_pr_shard_init": (C.c_int, [_P, C.c_float, _P, _P, _P, _P]),
     "gb_pr_shard_step": (C.c_int, [_P, C.c_float, C.c_uint64, _P, _P, _P, C.c_uint32, _P, _P, _P, _P]),
     "gb_pr_shard_sync": (C.c_int, [_P, C.c_uint64, _P, _P, _P, _P, C.c_uint32, _P]),

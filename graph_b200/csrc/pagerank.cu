@@ -98,6 +98,8 @@ struct PrPlan {
   uint64_t NG = 0;              // groups in all block streams
   uint32_t chunk_groups = 0, n_chunks = 0, n_tasks = 0, n_fix = 0;
   uint32_t fix_max_row = 0;     // largest local row that owns a segment cut by a chunk boundary
+  uint32_t n_mega = 0;          // local rows [0, n_mega) went through the sort path of the layout build
+  uint32_t last_hot_block = CB_NONE;  // largest source block index among the hot blocks
   DevBuf<uint32_t> blk;         // [KB] source block of hot rank j
   DevBuf<uint32_t> nrows;       // [KB] local rows [0, nrows[j]) have a segment in block j (non-increasing)
   DevBuf<uint32_t> poff;        // [KB+1] staircase offsets
@@ -1507,6 +1509,7 @@ static gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan
       p->S = S;
     }
     p->KB = (uint32_t)h_blk.size();
+    if (p->KB) p->last_hot_block = *std::max_element(h_blk.begin(), h_blk.end());
     p->n_cb = p->KB ? h_nrows[0] : 0;
     if (h_poff.empty()) h_poff.push_back(0);
     DevBuf<uint32_t> hot_of_blk;
@@ -1547,6 +1550,7 @@ static gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan
       if (M) GB_TRY(upload(s, &mega_off, h_moff));
       else n_mega = 0;
     }
+    p->n_mega = n_mega;
     // all other rows that own segments: one record per in-edge (consumed by the fill pass)
     DevBuf<uint2> rec;
     if (p->n_cb > n_mega) {
@@ -1769,6 +1773,9 @@ static gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan
     const uint64_t fin_warps2 = (uint64_t)p->n_fin_warp / 32 * (PR_FIN_THREADS / 32) + (p->n_fin - p->n_fin_warp + 63) / 64;
     const uint64_t fin_warps4 = (uint64_t)p->n_fin_warp / 32 * (PR_FIN_THREADS / 32) + (p->n_fin - p->n_fin_warp + 127) / 128;
     p->fin_u = (fin_warps2 + PR_FIN_THREADS / 32 - 1) / (PR_FIN_THREADS / 32) <= (uint64_t)dev_sms * 8 ? 2 : 4;
+    // GB_PR_FIN_U (experiment / tests): 2 or 4 forces that instantiation of k_pr_finish; anything else = automatic
+    const uint32_t force_u = env_u32("GB_PR_FIN_U", 0);
+    if (force_u == 2 || force_u == 4) p->fin_u = force_u;
     const uint64_t fin_tasks = p->fin_u == 2 ? fin_warps2 : fin_warps4;
     const uint64_t want_fin = (fin_tasks + PR_FIN_THREADS / 32 - 1) / (PR_FIN_THREADS / 32);
     p->grid_fin = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(want_fin, (uint64_t)dev_sms * 8));
@@ -1778,9 +1785,15 @@ static gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan
     // of one after the other in every CTA.  It pays on a shard of a large graph; there is nothing to gain
     // when the grid is capped (RMAT-26 on one GPU) or the hub chain is short (RMAT-22), where every CTA keeps
     // doing both parts.
+    // GB_PR_FIN_SPLIT (experiment / tests): 1 forces the split, 2 never splits, 0 = automatic.  Forcing waives
+    // only the two conditions above that decide whether it pays; the structural ones stay (a hub group to
+    // take, rows left for the others, and at least one CTA beyond the hub CTAs: else no CTA would update
+    // the tail rows).
     p->fin_hub_ctas = 0;
-    if (want_fin <= (uint64_t)dev_sms * 8 && p->KB > 4 * FIN_CTA_BLOCKS && p->n_fin_warp && p->n_fin > p->n_fin_warp &&
-        p->grid_fin > p->n_fin_warp / 32)
+    const uint32_t split = env_u32("GB_PR_FIN_SPLIT", 0);
+    const bool split_pays = want_fin <= (uint64_t)dev_sms * 8 && p->KB > 4 * FIN_CTA_BLOCKS;
+    if (p->n_fin_warp && p->n_fin > p->n_fin_warp && p->grid_fin > p->n_fin_warp / 32 &&
+        (split == 1 || (split == 0 && split_pays)))
       p->fin_hub_ctas = p->n_fin_warp / 32;
     const size_t nerr = (size_t)p->grid_sell + p->grid_fin;
     GB_TRY(p->block_err.alloc(nerr));
@@ -2228,6 +2241,38 @@ gb_status gb_page_rank_plan_info(const gb_graph* g, gb_pr_shard_stats* stats) {
   tmp.graph = g;
   tmp.plan = g->pr_plan;
   return gb_pr_shard_info(&tmp, stats);
+}
+
+gb_status gb_pr_shard_plan_shape(const gb_pr_shard* shard, gb_pr_plan_shape* shape) {
+  GB_REQUIRE(shard && shape, "NULL argument");
+  const gb::PrPlan* p = shard->plan;
+  shape->hot_blocks = p->KB;
+  shape->n_cb = p->n_cb;
+  shape->n_fin = p->n_fin;
+  shape->n_fin_warp = p->n_fin_warp;
+  shape->fin_u = p->fin_u;
+  shape->fin_hub_ctas = p->fin_hub_ctas;
+  shape->grid_cb = p->grid_cb;
+  shape->grid_sell = p->grid_sell;
+  shape->grid_fin = p->grid_fin;
+  shape->n_mega = p->n_mega;
+  shape->n_fix = p->n_fix;
+  shape->fix_in_sell = gb::fix_in_sell(p) ? 1u : 0u;
+  shape->dual = p->dual ? 1u : 0u;
+  shape->last_hot_block = p->last_hot_block;
+  return GB_OK;
+}
+
+gb_status gb_page_rank_plan_shape(const gb_graph* g, gb_pr_plan_shape* shape) {
+  GB_REQUIRE(g && shape, "NULL argument");
+  if (g->kind != GB_KIND_DIRECTED) return gb::fail(GB_ERR_UNSUPPORTED, "page rank needs a directed graph");
+  gb::DeviceGuard guard(g->device);
+  std::lock_guard<std::mutex> lock(g->mu);
+  if (!g->pr_plan) GB_TRY(gb::build_pr_plan(g, gb::PrDeal{}, &g->pr_plan));
+  gb_pr_shard tmp;
+  tmp.graph = g;
+  tmp.plan = g->pr_plan;
+  return gb_pr_shard_plan_shape(&tmp, shape);
 }
 
 gb_status gb_page_rank_plan_reset(const gb_graph* g) {

@@ -13,6 +13,7 @@
 #include <cfloat>
 
 #include "common.cuh"
+#include "sssp_bucket.h"
 
 namespace gb {
 
@@ -194,11 +195,9 @@ static gb_status sssp_impl(const gb_graph* g, const gb_sssp_config* cfg, float* 
   uint32_t* far_out = fb.p;
   uint32_t near_count = 1, far_count = 0;
   const float delta = cfg->delta;
-  double bucket = 0.0;  // current bucket index; bounds are delta * bucket in f32 like sssp.rs:126
+  float lower = 0.0f, upper = delta;  // the current bucket (sssp_bucket.h)
   uint32_t h_counts[4];
   for (;;) {
-    const float lower = delta * (float)bucket;
-    const float upper = delta * (float)(bucket + 1.0);
     // drain the near queue of this bucket
     while (near_count > 0) {
       const uint32_t zero2[2] = {0u, far_count};
@@ -228,20 +227,15 @@ static gb_status sssp_impl(const gb_graph* g, const gb_sssp_config* cfg, float* 
     if (h_min == inf) break;  // everything left in the pile is stale
     float dmin;
     memcpy(&dmin, &h_min, 4);
-    double next_bucket = floor((double)(dmin / delta));  // dest_bin = (nd / delta) as usize, sssp.rs:190
-    if (next_bucket <= bucket) next_bucket = bucket + 1.0;
-    // guard against f32 rounding at the bucket edge: make sure dmin < upper of the chosen bucket
-    while (!(dmin < delta * (float)(next_bucket + 1.0))) next_bucket += 1.0;
-    while (next_bucket > bucket + 1.0 && dmin < delta * (float)next_bucket) next_bucket -= 1.0;
-    bucket = next_bucket;
+    const SsspBucket next = sssp_next_bucket(dmin, delta, upper);
+    lower = next.lower;
+    upper = next.upper;
     st.epoch += 1;  // entries appended to the pile from now on are tracked under the new epoch
-    const float lo2 = delta * (float)bucket, up2 = delta * (float)(bucket + 1.0);
     const uint32_t zero3[3] = {0u, 0u, 0u};
     GB_CUDA(cudaMemcpyAsync(counts.p, zero3, 12, cudaMemcpyHostToDevice, s));
-    // anything below lo2 in the pile was settled (its distance was final when its bucket drained)
-    k_sssp_split_far<<<grid_for(far_count, blk), blk, 0, s>>>(dist, far, far_count, 0.0f, up2, near_in, far_out,
+    // anything below lower in the pile was settled (its distance was final when its bucket drained)
+    k_sssp_split_far<<<grid_for(far_count, blk), blk, 0, s>>>(dist, far, far_count, 0.0f, upper, near_in, far_out,
                                                              counts.p, cap);
-    (void)lo2;
     g->timing.kernel_launches += 1;
     GB_CUDA(cudaMemcpyAsync(h_counts, counts.p, 12, cudaMemcpyDeviceToHost, s));
     GB_CUDA(cudaStreamSynchronize(s));

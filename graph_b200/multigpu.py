@@ -55,6 +55,12 @@ class CudaShardBackend:
         check(lib.gb_pr_shard_info(self._shard, C.byref(st)))
         return st.as_dict()
 
+    def plan_shape(self) -> dict:
+        """Diagnostics: the launch shape of this shard's sweep kernels."""
+        sh = _capi.PrPlanShape()
+        check(lib.gb_pr_shard_plan_shape(self._shard, C.byref(sh)))
+        return sh.as_dict()
+
     def __del__(self):
         sh, self._shard = getattr(self, "_shard", None), None
         if sh:

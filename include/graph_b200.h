@@ -298,6 +298,25 @@ gb_status gb_page_rank_plan_reset(const gb_graph* graph);
 /* builds the layout of shard `rank` of `world` on the graph's device */
 gb_status gb_pr_shard_create(const gb_graph* graph, uint32_t rank, uint32_t world, gb_pr_shard** shard);
 gb_status gb_pr_shard_info(const gb_pr_shard* shard, gb_pr_shard_stats* stats);
+/* Diagnostics: the launch shape the layout chose for the sweep kernels (k_pr_cb, k_pr_fixup, k_pr_sell,
+ * k_pr_finish), so that tests can tell which variant of each a graph reaches.  Not part of the stable
+ * statistics above; fields may be added. */
+typedef struct gb_pr_plan_shape {
+  uint32_t hot_blocks;         /* column blocks that own segments (KB) */
+  uint32_t n_cb;               /* local rows [0, n_cb) own at least one segment */
+  uint32_t n_fin;              /* local rows [0, n_fin) are completed by k_pr_finish */
+  uint32_t n_fin_warp;         /* of which [0, n_fin_warp) are hub groups (one finish CTA per 32 rows) */
+  uint32_t fin_u;              /* 32-row groups per warp iteration of k_pr_finish (2 or 4) */
+  uint32_t fin_hub_ctas;       /* finish CTAs reserved for the hub groups (0 = no role split) */
+  uint32_t grid_cb, grid_sell, grid_fin;
+  uint32_t n_mega;             /* local rows laid out through the sort path of the layout build */
+  uint32_t n_fix;              /* chunks whose last segment continues in the next chunk */
+  uint32_t fix_in_sell;        /* 1: those parts are added by k_pr_sell, 0: by k_pr_fixup */
+  uint32_t dual;               /* 1: k_pr_cb_half and k_pr_sell on two streams (GB_PR_DUAL) */
+  uint32_t last_hot_block;     /* largest source block index among the hot blocks (0xFFFFFFFF: none) */
+} gb_pr_plan_shape;
+gb_status gb_page_rank_plan_shape(const gb_graph* graph, gb_pr_plan_shape* shape);
+gb_status gb_pr_shard_plan_shape(const gb_pr_shard* shard, gb_pr_plan_shape* shape);
 /* fills the full initial vectors (n floats each, internal order) on this rank: d_x0 = init/outdeg,
  * the constant part of d_x1; d_scores = init for own rows, 0 for the others (rows without in-edges:
  * base on rank 0), so that the ranks' score vectors can be summed into the full one */

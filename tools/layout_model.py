@@ -14,6 +14,16 @@ import numpy as np
 CB_G = 4
 REC_SEG = 0x80000000
 NONE = 0xFFFFFFFF
+CB_BLOCK_DEFAULT = 49152
+CB_BLOCK_MAX = 56 * 1024
+CB_TAU_DEFAULT = 1.5
+CB_MAX_BLOCKS = 8192
+CB_MEGA_DEG = 32768
+CB_MEGA_JBITS = 14
+SELL_FEW = 4
+FIN_CTA_BLOCKS = 64
+PR_FIN_WARPS = 8          # PR_FIN_THREADS / 32
+H100_SMS = 132
 
 
 def deal_global(l, P, p):
@@ -37,8 +47,15 @@ def deal_count(R, P, p):
     return c
 
 
-def make_plan(in_off, in_tgt, out_deg, B, tau, P=1, p=0):
-    """Renumbering + staircase, like steps 1-3 of build_pr_plan (host side, no edge data needed)."""
+def clamp_block(B):
+    """GB_PR_BLOCK as build_pr_plan applies it: a multiple of 1024 in [1024, CB_BLOCK_MAX]"""
+    return min(max(B & ~1023, 1024), CB_BLOCK_MAX)
+
+
+def make_plan(in_off, in_tgt, out_deg, B, tau, P=1, p=0, mega=CB_MEGA_DEG):
+    """Renumbering + staircase, like steps 1-3 of build_pr_plan (host side, no edge data needed).
+    B is used as given (see clamp_block); `mega` is GB_PR_MEGA, the in-degree above which a row takes the
+    sort path of the layout build."""
     n = len(in_off) - 1
     indeg = np.diff(in_off).astype(np.int64)
     # in-degree descending, then out-degree descending, then id
@@ -60,6 +77,7 @@ def make_plan(in_off, in_tgt, out_deg, B, tau, P=1, p=0):
         rows_ge.append(int((indeg_int[:n_active] >= dmin).sum()))
     hot = [b for b in range(nblk) if deal_count(rows_ge[b], P, p) > 0]
     hot.sort(key=lambda b: (-rows_ge[b], b))
+    hot = hot[:CB_MAX_BLOCKS]
     hot_of_blk = np.full(nblk, -1, np.int64)
     nrows, poff, S = [], [0], 0
     for j, b in enumerate(hot):
@@ -68,9 +86,59 @@ def make_plan(in_off, in_tgt, out_deg, B, tau, P=1, p=0):
         S += nrows[-1]
         poff.append(S)
     n_loc = deal_count(n_active, P, p)
+    n_cb = nrows[0] if nrows else 0
+    # rows on the sort path: in-degree > mega, a prefix of the rows with segments (the 32-bit prefix trim of
+    # the sort index needs graphs beyond any test)
+    n_mega = deal_count(int((indeg_int[:n_active] >= mega + 1).sum()), P, p) if m else 0
+    n_mega = min(n_mega, n_cb, (1 << (32 - CB_MEGA_JBITS)) - 1)
+    if len(hot) >= (1 << CB_MEGA_JBITS) - 1:
+        n_mega = 0
     return dict(n=n, order=order, new_id=new_id, n_active=n_active, n_loc=n_loc, blk=np.array(hot, np.int64),
                 hot_of_blk=hot_of_blk, nrows=np.array(nrows, np.int64), poff=np.array(poff, np.int64), S=S,
-                n_cb=nrows[0] if nrows else 0, B=B, P=P, p=p)
+                n_cb=n_cb, KB=len(hot), n_mega=n_mega, last_hot_block=max(hot) if hot else NONE, nblk=nblk,
+                B=B, P=P, p=p)
+
+
+def launch_shape(plan, sms=H100_SMS, fin_u=0, fin_split=0, dual=False):
+    """Step 8 of build_pr_plan: which rows k_pr_finish completes and how (fin_u, grid, role split).
+    fin_u / fin_split are GB_PR_FIN_U / GB_PR_FIN_SPLIT; dual is GB_PR_DUAL=1 (taken when there are hot
+    blocks and active rows)."""
+    KB, n_cb, nr = plan["KB"], plan["n_cb"], plan["nrows"]
+    dual = bool(dual) and KB > 0 and plan["n_loc"] > 0
+    ceil32 = lambda x: (int(x) + 31) // 32 * 32
+    n_fin = n_cb if dual else (min(n_cb, ceil32(nr[SELL_FEW])) if KB > SELL_FEW else 0)
+    n_fin_warp = min(n_fin, ceil32(nr[FIN_CTA_BLOCKS])) if KB > FIN_CTA_BLOCKS else 0
+    warps2 = n_fin_warp // 32 * PR_FIN_WARPS + (n_fin - n_fin_warp + 63) // 64
+    warps4 = n_fin_warp // 32 * PR_FIN_WARPS + (n_fin - n_fin_warp + 127) // 128
+    u = 2 if (warps2 + PR_FIN_WARPS - 1) // PR_FIN_WARPS <= sms * 8 else 4
+    if fin_u in (2, 4):
+        u = fin_u
+    want_fin = ((warps2 if u == 2 else warps4) + PR_FIN_WARPS - 1) // PR_FIN_WARPS
+    grid_fin = max(1, min(want_fin, sms * 8))
+    pays = want_fin <= sms * 8 and KB > 4 * FIN_CTA_BLOCKS
+    structural = n_fin_warp > 0 and n_fin > n_fin_warp and grid_fin > n_fin_warp // 32
+    split = structural and (fin_split == 1 or (fin_split == 0 and pays))
+    return dict(hot_blocks=KB, n_cb=n_cb, n_fin=n_fin, n_fin_warp=n_fin_warp, fin_u=u, grid_fin=grid_fin,
+                fin_hub_ctas=n_fin_warp // 32 if split else 0, grid_capped=want_fin > sms * 8,
+                n_mega=plan["n_mega"], dual=int(dual), last_hot_block=plan["last_hot_block"])
+
+
+def layout_counts(plan, in_off, in_tgt):
+    """Staircase pairs, 4-id groups and edges served from column blocks (k_cb_count + k_cb_groups),
+    vectorised: the statistics gb_pr_shard_stats reports as segments / groups / block_edges."""
+    n, B, P, p = plan["n"], plan["B"], plan["P"], plan["p"]
+    in_off = np.asarray(in_off, np.int64)
+    row = np.repeat(np.arange(n, dtype=np.int64), np.diff(in_off))   # original row of every in-edge
+    g = plan["new_id"][row]
+    sl = g >> 5
+    l = ((sl // P) << 5) | (g & 31)
+    j = plan["hot_of_blk"][plan["new_id"][np.asarray(in_tgt, np.int64)] // B]
+    nrows = plan["nrows"] if len(plan["nrows"]) else np.zeros(1, np.int64)
+    seg = (sl % P == p) & (g < plan["n_active"]) & (j >= 0)
+    seg &= l < nrows[np.maximum(j, 0)]
+    cnt = np.bincount(plan["poff"][j[seg]] + l[seg], minlength=plan["S"])[:plan["S"]]
+    groups = int(np.where(cnt > 0, (cnt + CB_G - 1) // CB_G, 1).sum())
+    return dict(segments=int(plan["S"]), groups=groups, block_edges=int(seg.sum()))
 
 
 def classify_row(plan, l, tgt_row, cnt, rec_out):
