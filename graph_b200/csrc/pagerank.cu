@@ -2077,6 +2077,7 @@ static gb_status page_rank_impl(const gb_graph* g, const gb_page_rank_config* cf
 // ---- multi-GPU shard (1-D edge-cut by destination, 32-row slices dealt round-robin) ----------------
 struct gb_pr_shard {
   const gb_graph* graph = nullptr;
+  int device = 0;                     // the graph's device: gb_pr_shard_free must not read a freed graph
   gb::PrPlan* plan = nullptr;
   gb::DevBuf<void*> sync_table;       // device copy of the ranks' control-block pointers (gb_pr_shard_sync)
   void* sync_table_host[8] = {nullptr};
@@ -2093,6 +2094,7 @@ gb_status gb_pr_shard_create(const gb_graph* g, uint32_t rank, uint32_t world, g
   gb_pr_shard* sh = new (std::nothrow) gb_pr_shard();
   if (!sh) return gb::fail(GB_ERR_OOM, "host allocation failed");
   sh->graph = g;
+  sh->device = g->device;
   gb::PrDeal deal;
   deal.P = world;
   deal.p = rank;
@@ -2107,7 +2109,8 @@ gb_status gb_pr_shard_create(const gb_graph* g, uint32_t rank, uint32_t world, g
 
 gb_status gb_pr_shard_free(gb_pr_shard* shard) {
   if (!shard) return GB_OK;
-  gb::DeviceGuard guard(shard->graph->device);
+  // the plan owns all its memory: freeing it needs the device, not the graph, which may be gone already
+  gb::DeviceGuard guard(shard->device);
   gb::free_pr_plan(shard->plan);
   delete shard;
   return GB_OK;

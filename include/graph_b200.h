@@ -344,6 +344,7 @@ gb_status gb_pr_shard_sync(const gb_pr_shard* shard, uint64_t sweep_no, const do
 /* internal order -> original ids: d_scores_out[v] = d_scores_internal[new_id[v]] */
 gb_status gb_pr_shard_finish(const gb_pr_shard* shard, const float* d_scores_internal,
                              float* d_scores_out, void* cuda_stream);
+/* the graph must outlive every other call on its shards; the free may come before or after gb_graph_free */
 gb_status gb_pr_shard_free(gb_pr_shard* shard);
 
 /* ---- single-process multi-GPU PageRank ------------------------------------------------------------

@@ -16,6 +16,9 @@ import layout_model as lm  # noqa: E402
 import oracle  # noqa: E402
 
 TAIL_R = (1, 2, 3, 5, 33)
+# every environment knob of the plan build and the sweep (graph_b200/csrc/pagerank.cu)
+KNOBS = ("GB_PR_BLOCK", "GB_PR_TAU", "GB_PR_MIN_BLOCK", "GB_PR_MEGA", "GB_PR_CHUNK", "GB_PR_TASK_CHUNKS",
+         "GB_PR_DUAL", "GB_PR_DEBUG", "GB_PR_FIN_U", "GB_PR_FIN_SPLIT", "GB_PR_FEED_CHUNKS", "GB_PR_FEED_MIN_EDGES")
 
 
 def tail_block(r):
@@ -99,6 +102,17 @@ FIXTURES = {
 }
 
 _CACHE: dict = {}
+
+
+def set_knobs(monkeypatch, name, **env):
+    """every knob unset except the fixture's GB_PR_BLOCK and `env`"""
+    for k in KNOBS:
+        monkeypatch.delenv(k, raising=False)
+    block = FIXTURES[name][1] if name in FIXTURES else None
+    if block:
+        monkeypatch.setenv("GB_PR_BLOCK", str(block))
+    for k, v in env.items():
+        monkeypatch.setenv(k, str(v))
 
 
 def graph(name):

@@ -510,37 +510,15 @@ def test_invalid_host_csr_is_rejected(gb):
 # ---- shard API on one GPU: several virtual ranks, dealt slices exchanged by plain copies ----------
 @pytest.mark.parametrize("world", [2, 3, 8])
 def test_shard_api_virtual_ranks_match_single_gpu(gb, world):
-    import torch
-    from graph_b200.multigpu import CudaShardBackend, owner_of_rows
+    from virtual_ranks import VirtualRanks
     g = gb.DiGraph.rmat(15, seed=11, layout=gb.Layout.Sorted)
-    n = g.node_count()
     sweeps, damping = 6, 0.85
     want = g.page_rank(max_iterations=sweeps, tolerance=0.0, damping_factor=damping, mode="jacobi")
-    ranks = [CudaShardBackend(g, r, world) for r in range(world)]
-    n_active = ranks[0].n_active
-    assert sum(b.stats["local_rows"] for b in ranks) == n_active
-    assert sum(b.stats["local_edges"] for b in ranks) == g.edge_count()
-    dev = ranks[0].device
-    owner = torch.from_numpy(owner_of_rows(np.arange(n), world)).to(dev)
-    mine = [owner == r for r in range(world)]
-    x = [[torch.zeros(n, dtype=torch.float32, device=dev) for _ in range(2)] for _ in range(world)]
-    scores = [torch.empty(n, dtype=torch.float32, device=dev) for _ in range(world)]
-    err = [torch.zeros(1, dtype=torch.float64, device=dev) for _ in range(world)]
-    for r, b in enumerate(ranks):
-        b.init(damping, x[r][0], x[r][1], scores[r])
-    total = 0.0
-    for sweep in range(1, sweeps + 1):
-        cur, nxt = (sweep - 1) & 1, sweep & 1
-        for r, b in enumerate(ranks):
-            b.step(damping, sweep, x[r][cur], x[r][nxt], None, scores[r], err[r])
-        torch.cuda.synchronize()
-        for r in range(world):  # the all-gather: every rank's rows go to every other rank
-            for q in range(world):
-                if q != r:
-                    x[q][nxt][mine[r]] = x[r][nxt][mine[r]]
-        total = sum(float(e.item()) for e in err)
-    full = torch.stack(scores).sum(dim=0)   # own rows + zeros elsewhere (rows without in-edges: rank 0)
-    got = ranks[0].finish(full).cpu().numpy()
+    vr = VirtualRanks(g, world, damping)
+    assert sum(b.stats["local_rows"] for b in vr.ranks) == vr.n_active
+    assert sum(b.stats["local_edges"] for b in vr.ranks) == g.edge_count()
+    total = vr.run(sweeps)                  # host-copy exchange
+    got = vr.scores_host()
     # every (row, block) partial is the same set of addends on every shard count; only the tree that
     # adds a pair's 4-id groups depends on where the pair sits in its 32-group step: <= 1 ulp per partial
     assert np.max(np.abs(got - want.scores()) / want.scores()) <= 5e-7
@@ -551,33 +529,11 @@ def test_shard_api_virtual_ranks_match_single_gpu(gb, world):
 def test_wcc_shard_phases_virtual_ranks_bit_exact(gb, world):
     """Multi-GPU WCC on one GPU: every virtual rank runs the phases on its vertex range over its own
     full parent array; the all-gather is a list of tensors.  Labels must equal the single-GPU run."""
-    from graph_b200 import _capi
-    from graph_b200.multigpu import CudaWccBackend, vertex_ranges
+    from virtual_ranks import wcc_virtual_ranks
     g = gb.DiGraph.rmat(16, seed=3, layout=gb.Layout.Sorted)
     want = g.wcc().components()
-    b = CudaWccBackend(g)
-    ranges = vertex_ranges(g.node_count(), world)
-    parents = [b.new_parent() for _ in range(world)]
-
-    def merge_all():
-        snap = [p.clone() for p in parents]
-        for r, p in enumerate(parents):
-            for q in range(world):
-                if q != r:
-                    b.phase(_capi.WCC_MERGE, p, other=snap[q])
-            b.phase(_capi.WCC_COMPRESS, p)
-
-    for r, p in enumerate(parents):
-        b.phase(_capi.WCC_INIT, p)
-        b.phase(_capi.WCC_SAMPLE, p, *ranges[r])
-        b.phase(_capi.WCC_COMPRESS, p)
-    merge_all()
-    labels = [b.sample_label(p) for p in parents]
+    parents, labels = wcc_virtual_ranks(g, world)
     assert len(set(labels)) == 1                      # same forest, same seed -> same giant component
-    for r, p in enumerate(parents):
-        b.phase(_capi.WCC_LINK_REMAINING, p, *ranges[r], labels[r][0], labels[r][1])
-        b.phase(_capi.WCC_COMPRESS, p)
-    merge_all()
     for p in parents:
         assert (p.cpu().numpy().view(np.uint32) == want).all()
 

@@ -18,8 +18,7 @@ pytestmark = pytest.mark.gpu
 PR_RTOL = 1e-6
 ERR_ATOL = 2e-6          # as test_gpu_parity.py
 SWEEPS = 10
-KNOBS = ("GB_PR_BLOCK", "GB_PR_TAU", "GB_PR_MIN_BLOCK", "GB_PR_MEGA", "GB_PR_CHUNK", "GB_PR_TASK_CHUNKS",
-         "GB_PR_DUAL", "GB_PR_DEBUG", "GB_PR_FIN_U", "GB_PR_FIN_SPLIT", "GB_PR_FEED_CHUNKS", "GB_PR_FEED_MIN_EDGES")
+set_knobs = fx.set_knobs
 SHAPE_KEYS = ("hot_blocks", "n_cb", "n_fin", "n_fin_warp", "fin_u", "grid_fin", "fin_hub_ctas", "n_mega", "dual",
               "last_hot_block")
 
@@ -34,16 +33,6 @@ def gb():
 def sms():
     import torch
     return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def set_knobs(monkeypatch, name, **env):
-    for k in KNOBS:
-        monkeypatch.delenv(k, raising=False)
-    block = fx.FIXTURES[name][1]
-    if block:
-        monkeypatch.setenv("GB_PR_BLOCK", str(block))
-    for k, v in env.items():
-        monkeypatch.setenv(k, str(v))
 
 
 def oracle_pr(name, sweeps, tol):
@@ -202,40 +191,19 @@ def test_capped_finish_grid(gb, sms, monkeypatch):
 def test_split_on_virtual_rank_shards(gb, sms, monkeypatch, world):
     """the harness of test_shard_api_virtual_ranks_match_single_gpu with the role split forced on every
     shard of RMAT-18 (where production uses the split: a shard of a large graph)"""
-    import torch
-    from graph_b200.multigpu import CudaShardBackend, owner_of_rows
+    from virtual_ranks import VirtualRanks
     set_knobs(monkeypatch, "rmat18")
     g = device_graph(gb, "rmat18")
-    n = g.node_count()
     sweeps, damping = 6, 0.85
     want = g.page_rank(max_iterations=sweeps, tolerance=0.0, damping_factor=damping, mode="jacobi")
     monkeypatch.setenv("GB_PR_FIN_SPLIT", "1")
-    ranks = [CudaShardBackend(g, r, world) for r in range(world)]
-    for r, b in enumerate(ranks):
+    vr = VirtualRanks(g, world, damping)
+    for r, b in enumerate(vr.ranks):
         shape = b.plan_shape()
         _, model, _ = fx.model("rmat18", P=world, p=r, sms=sms, fin_split=1)
         assert {k: shape[k] for k in SHAPE_KEYS} == {k: model[k] for k in SHAPE_KEYS}
         assert shape["fin_hub_ctas"] > 0
-    dev = ranks[0].device
-    owner = torch.from_numpy(owner_of_rows(np.arange(n), world)).to(dev)
-    mine = [owner == r for r in range(world)]
-    x = [[torch.zeros(n, dtype=torch.float32, device=dev) for _ in range(2)] for _ in range(world)]
-    scores = [torch.empty(n, dtype=torch.float32, device=dev) for _ in range(world)]
-    err = [torch.zeros(1, dtype=torch.float64, device=dev) for _ in range(world)]
-    for r, b in enumerate(ranks):
-        b.init(damping, x[r][0], x[r][1], scores[r])
-    total = 0.0
-    for sweep in range(1, sweeps + 1):
-        cur, nxt = (sweep - 1) & 1, sweep & 1
-        for r, b in enumerate(ranks):
-            b.step(damping, sweep, x[r][cur], x[r][nxt], None, scores[r], err[r])
-        torch.cuda.synchronize()
-        for r in range(world):
-            for q in range(world):
-                if q != r:
-                    x[q][nxt][mine[r]] = x[r][nxt][mine[r]]
-        total = sum(float(e.item()) for e in err)
-    full = torch.stack(scores).sum(dim=0)
-    got = ranks[0].finish(full).cpu().numpy()
+    total = vr.run(sweeps)
+    got = vr.scores_host()
     assert np.max(np.abs(got - want.scores()) / want.scores()) <= 5e-7
     assert abs(total - want.error) <= 1e-7 + 1e-6 * want.error

@@ -29,6 +29,18 @@ def test_records_reproduce_the_direct_layout(seed, world):
     assert segments > 0
 
 
+def test_deal_count_matches_the_row_owners_on_tiny_graphs():
+    """deal_count (what every shard's local_rows must be) against the owner of each row as the multi-GPU
+    driver assigns it, for every world and every active-row count up to a bit more than one slice per rank:
+    ranks that own nothing, a partial last slice, a partial slice on a later rank"""
+    from graph_b200.multigpu import owner_of_rows
+    for P in range(1, 9):
+        for n_active in range(0, 32 * P + 41):
+            owner = owner_of_rows(range(n_active), P)
+            for p in range(P):
+                assert lm.deal_count(n_active, P, p) == int((owner == p).sum()), (P, n_active, p)
+
+
 def test_cyclic_deal_is_a_partition():
     for P in (1, 2, 3, 8):
         for R in (0, 1, 31, 32, 33, 1000, 1024):

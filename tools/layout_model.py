@@ -23,6 +23,7 @@ CB_MEGA_JBITS = 14
 SELL_FEW = 4
 FIN_CTA_BLOCKS = 64
 PR_FIN_WARPS = 8          # PR_FIN_THREADS / 32
+PR_SELL_WARPS = 16        # PR_SELL_THREADS / 32
 H100_SMS = 132
 
 
@@ -100,12 +101,15 @@ def make_plan(in_off, in_tgt, out_deg, B, tau, P=1, p=0, mega=CB_MEGA_DEG):
 
 
 def launch_shape(plan, sms=H100_SMS, fin_u=0, fin_split=0, dual=False):
-    """Step 8 of build_pr_plan: which rows k_pr_finish completes and how (fin_u, grid, role split).
+    """Step 8 of build_pr_plan: the SELL grid (one warp per 32-row slice, no launch for a shard without
+    rows) and which rows k_pr_finish completes and how (fin_u, grid, role split).
     fin_u / fin_split are GB_PR_FIN_U / GB_PR_FIN_SPLIT; dual is GB_PR_DUAL=1 (taken when there are hot
     blocks and active rows)."""
     KB, n_cb, nr = plan["KB"], plan["n_cb"], plan["nrows"]
     dual = bool(dual) and KB > 0 and plan["n_loc"] > 0
     ceil32 = lambda x: (int(x) + 31) // 32 * 32
+    num_slices = (plan["n_loc"] + 31) // 32
+    grid_sell = min((num_slices + PR_SELL_WARPS - 1) // PR_SELL_WARPS, sms * 2)
     n_fin = n_cb if dual else (min(n_cb, ceil32(nr[SELL_FEW])) if KB > SELL_FEW else 0)
     n_fin_warp = min(n_fin, ceil32(nr[FIN_CTA_BLOCKS])) if KB > FIN_CTA_BLOCKS else 0
     warps2 = n_fin_warp // 32 * PR_FIN_WARPS + (n_fin - n_fin_warp + 63) // 64
@@ -118,7 +122,8 @@ def launch_shape(plan, sms=H100_SMS, fin_u=0, fin_split=0, dual=False):
     pays = want_fin <= sms * 8 and KB > 4 * FIN_CTA_BLOCKS
     structural = n_fin_warp > 0 and n_fin > n_fin_warp and grid_fin > n_fin_warp // 32
     split = structural and (fin_split == 1 or (fin_split == 0 and pays))
-    return dict(hot_blocks=KB, n_cb=n_cb, n_fin=n_fin, n_fin_warp=n_fin_warp, fin_u=u, grid_fin=grid_fin,
+    return dict(hot_blocks=KB, n_cb=n_cb, n_fin=n_fin, n_fin_warp=n_fin_warp, fin_u=u, grid_sell=grid_sell,
+                grid_fin=grid_fin,
                 fin_hub_ctas=n_fin_warp // 32 if split else 0, grid_capped=want_fin > sms * 8,
                 n_mega=plan["n_mega"], dual=int(dual), last_hot_block=plan["last_hot_block"])
 
