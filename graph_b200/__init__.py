@@ -9,6 +9,7 @@ package.  Every algorithm call goes through the C ABI of ``libgraph_b200.so``
 from __future__ import annotations
 
 import ctypes as C
+import os
 import sys
 import time
 from pathlib import Path
@@ -191,7 +192,22 @@ class SsspResult:
 
 
 # ---- input files (crates/builder/src/input/{graph500,edgelist}.rs) --------------------------------
-# parsed by the library's native multi-threaded readers (csrc/io.cu)
+# DiGraph.load / Graph.load stream the file to the device and parse it there (csrc/load.cu).  The host
+# readers below (csrc/io.cu) give the same edges; they serve the Flight server's weighted undirected graphs
+# and are the reference the device loader is tested against.
+def _load_args(path, file_format, layout):
+    """(path bytes, format value, layout value) for gb_*_load_u32; raises what opening the file raises."""
+    if file_format is FileFormat.Graph500:
+        fmt = 0
+    elif file_format is FileFormat.EdgeList:
+        fmt = 1
+    else:
+        raise TypeError(f"unknown file format {file_format!r}")
+    path = os.fspath(path)
+    open(path, "rb").close()  # FileNotFoundError / IsADirectoryError / PermissionError as before
+    return os.fsencode(path), fmt, _layout_value(layout)
+
+
 def _read_graph500(path) -> tuple[np.ndarray, np.ndarray, int]:
     """Packed 12-byte edges {v0_low, v1_low, high} (graph500.rs:111-127); node_count = edges/16 (:74)."""
     raw = np.fromfile(path, dtype=np.uint8)
@@ -250,6 +266,42 @@ def _edges_from_numpy(arr) -> tuple[np.ndarray, np.ndarray]:
 
 def _ptr(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def _torch_edges(src, dst, weights):
+    """Device u32 id tensors (narrowed and range-checked on the device), the weights, and torch's current
+    stream on the graph's device, for gb_*_from_device_edges_u32."""
+    import torch  # only this constructor needs torch
+
+    dev = torch.device("cuda", _device)
+
+    def check_tensor(t, what, dtypes):
+        if not isinstance(t, torch.Tensor) or t.device != dev:
+            raise ValueError(f"{what} must be a tensor on {dev}")
+        if t.dim() != 1 or not t.is_contiguous():
+            raise ValueError(f"{what} must be a contiguous 1-D tensor")
+        if t.dtype not in dtypes:
+            raise TypeError(f"{what} must be a tensor of {' or '.join(map(str, dtypes))}")
+
+    check_tensor(src, "src", (torch.int32, torch.int64))
+    check_tensor(dst, "dst", (torch.int32, torch.int64))
+    m = src.numel()
+    if dst.numel() != m:
+        raise ValueError("src and dst must have the same length")
+    if weights is not None:
+        check_tensor(weights, "weights", (torch.float32,))
+        if weights.numel() != m:
+            raise ValueError("weights must have one entry per edge")
+    stream = torch.cuda.current_stream(dev)
+    ids = []
+    for t in (src, dst):
+        u = torch.empty(m, dtype=torch.int32, device=dev)  # holds the u32 bit patterns
+        try:
+            check(lib.gb_ids_to_u32(_device, t.data_ptr(), t.element_size(), m, u.data_ptr(), stream.cuda_stream))
+        except ValueError:
+            raise TypeError("node ids must be 32-bit unsigned integers") from None
+        ids.append(u)
+    return ids[0], ids[1], weights, m, stream
 
 
 # ---- graph handles ---------------------------------------------------------------------------
@@ -329,6 +381,13 @@ class _Handle:
     def cuda_stream(self) -> int:
         return int(lib.gb_graph_stream(self._g) or 0)
 
+    def load_info(self) -> dict:
+        """Statistics of the file load that created this graph (zeros for graphs made otherwise):
+        file_bytes, chunks, edges, fallback_lines (values re-parsed on the host), h2d_bytes."""
+        info = _capi.LoadInfo()
+        check(lib.gb_graph_load_info(self._g, C.byref(info)))
+        return info.as_dict()
+
     def __repr__(self):
         return (f"{type(self).__name__} {{ node_count: {self.node_count()}, edge_count: {self.edge_count()}, "
                 f"load_took: {_took(self.load_micros)} }}")
@@ -360,25 +419,36 @@ class DiGraph(_Handle):
 
     @staticmethod
     def load(path, layout=None, file_format=FileFormat.Graph500) -> "DiGraph":
-        """Load a graph from the provided format (crates/mate/src/graphs/digraph.rs:35-44)."""
+        """Load a graph from the provided format (crates/mate/src/graphs/digraph.rs:35-44); the file is
+        parsed on the device."""
         t0 = time.perf_counter()
-        if file_format is FileFormat.Graph500:
-            src, dst, n = _read_graph500(path)
-            w = None
-        elif file_format is FileFormat.EdgeList:
-            src, dst = _read_edge_list(path)
-            n, w = 0, None
-        else:
-            raise TypeError(f"unknown file format {file_format!r}")
-        g = DiGraph._from_edges(src, dst, w, n, layout)
-        g.load_micros = max(1, int((time.perf_counter() - t0) * 1e6))
-        return g
+        p, fmt, lay = _load_args(path, file_format, layout)
+        out = C.c_void_p()
+        check(lib.gb_digraph_load_u32(_device, p, fmt, lay, 0, C.byref(out)))
+        return DiGraph(out, max(1, int((time.perf_counter() - t0) * 1e6)))
 
     @staticmethod
     def load_weighted(path, layout=None) -> "DiGraph":
         """Weighted text edge list `<src> <dst> <f32>` (DirectedCsrGraph<u32, (), f32>, for sssp)."""
-        src, dst, w = _read_edge_list(path, with_values=True)
-        return DiGraph._from_edges(src, dst, w, 0, layout)
+        t0 = time.perf_counter()
+        p, fmt, lay = _load_args(path, FileFormat.EdgeList, layout)
+        out = C.c_void_p()
+        check(lib.gb_digraph_load_u32(_device, p, fmt, lay, 1, C.byref(out)))
+        return DiGraph(out, max(1, int((time.perf_counter() - t0) * 1e6)))
+
+    @staticmethod
+    def from_torch(src, dst, weights=None, node_count: int = 0, layout=None) -> "DiGraph":
+        """From contiguous 1-D CUDA tensors on the graph's device (ids int32 or int64, weights float32),
+        without a host copy.  node_count 0 means max id + 1."""
+        s, d, w, m, stream = _torch_edges(src, dst, weights)
+        out = C.c_void_p()
+
+        def go():
+            check(lib.gb_digraph_from_device_edges_u32(_device, s.data_ptr(), d.data_ptr(),
+                                                       None if w is None else w.data_ptr(), m, int(node_count),
+                                                       _layout_value(layout), stream.cuda_stream, C.byref(out)))
+        _, micros = _timed(go)
+        return DiGraph(out, micros)
 
     @staticmethod
     def from_numpy(arr, layout=None, weights=None, node_count: int = 0) -> "DiGraph":
@@ -573,16 +643,22 @@ class Graph(_Handle):
     @staticmethod
     def load(path, layout=None, file_format=FileFormat.Graph500) -> "Graph":
         t0 = time.perf_counter()
-        if file_format is FileFormat.Graph500:
-            src, dst, n = _read_graph500(path)
-        elif file_format is FileFormat.EdgeList:
-            src, dst = _read_edge_list(path)
-            n = 0
-        else:
-            raise TypeError(f"unknown file format {file_format!r}")
-        g = Graph._from_edges(src, dst, n, layout)
-        g.load_micros = max(1, int((time.perf_counter() - t0) * 1e6))
-        return g
+        p, fmt, lay = _load_args(path, file_format, layout)
+        out = C.c_void_p()
+        check(lib.gb_graph_load_u32(_device, p, fmt, lay, C.byref(out)))
+        return Graph(out, max(1, int((time.perf_counter() - t0) * 1e6)))
+
+    @staticmethod
+    def from_torch(src, dst, node_count: int = 0, layout=None) -> "Graph":
+        """From contiguous 1-D int32 / int64 CUDA tensors on the graph's device, without a host copy."""
+        s, d, _, m, stream = _torch_edges(src, dst, None)
+        out = C.c_void_p()
+
+        def go():
+            check(lib.gb_graph_from_device_edges_u32(_device, s.data_ptr(), d.data_ptr(), m, int(node_count),
+                                                     _layout_value(layout), stream.cuda_stream, C.byref(out)))
+        _, micros = _timed(go)
+        return Graph(out, micros)
 
     @staticmethod
     def from_numpy(arr, layout=None, node_count: int = 0) -> "Graph":

@@ -64,6 +64,14 @@ class PrPlanShape(C.Structure):
         return {k: int(getattr(self, k)) for k, _ in self._fields_}
 
 
+class LoadInfo(C.Structure):
+    _fields_ = [("file_bytes", C.c_uint64), ("chunks", C.c_uint64), ("edges", C.c_uint64),
+                ("fallback_lines", C.c_uint64), ("h2d_bytes", C.c_uint64)]
+
+    def as_dict(self):
+        return {k: int(getattr(self, k)) for k, _ in self._fields_}
+
+
 class GraphB200Error(RuntimeError):
     """CUDA / allocation failure inside libgraph_b200."""
 
@@ -88,6 +96,14 @@ SIGNATURES = {
     "gb_graph500_decode": (C.c_int, [_P, C.c_uint64, _P, _P, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]),
     "gb_graph500_encode": (C.c_int, [_P, _P, C.c_uint64, _P]),
     "gb_edge_list_parse": (C.c_int, [C.c_char_p, C.c_uint64, _P, _P, _P, C.POINTER(C.c_uint64)]),
+    "gb_digraph_load_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
+    "gb_graph_load_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.c_int, C.POINTER(_P)]),
+    "gb_graph_load_info": (C.c_int, [_P, C.POINTER(LoadInfo)]),
+    "gb_digraph_from_device_edges_u32": (C.c_int, [C.c_int, _P, _P, _P, C.c_uint64, C.c_uint32, C.c_int, _P,
+                                                   C.POINTER(_P)]),
+    "gb_graph_from_device_edges_u32": (C.c_int, [C.c_int, _P, _P, C.c_uint64, C.c_uint32, C.c_int, _P,
+                                                 C.POINTER(_P)]),
+    "gb_ids_to_u32": (C.c_int, [C.c_int, _P, C.c_int, C.c_uint64, _P, _P]),
     "gb_graph_free": (C.c_int, [_P]),
     "gb_graph_get_info": (C.c_int, [_P, C.POINTER(GraphInfo)]),
     "gb_graph_copy_csr": (C.c_int, [_P, C.c_int, _P, _P, _P]),

@@ -155,6 +155,7 @@ struct gb_graph {
   mutable const gb::TargetFeed* feed = nullptr;  // set only while gb_page_rank_csr_u32 streams the targets in
   mutable gb_timing timing{};
   uint64_t extra_bytes = 0;
+  gb_load_info load{};  // filled by gb_[di]graph_load_u32 (load.cu)
 };
 
 namespace gb {
@@ -184,6 +185,10 @@ gb_status new_graph(int device, gb_graph_kind kind, uint32_t n, gb_graph** out);
 // uploads a host CSR (offsets always, targets/weights when non-null) and validates it on the device
 gb_status upload_host_csr(cudaStream_t s, uint32_t n, const uint32_t* off, const uint32_t* tgt, const float* w,
                           DevCsr* csr, const char* what);
+// builds a graph from device edge arrays (graph.cu; behind gb_[di]graph_from_device_edges_u32)
+gb_status graph_from_device_arrays(int device, gb_graph_kind kind, const uint32_t* d_src, const uint32_t* d_dst,
+                                   const float* d_w, uint64_t m, uint32_t n, gb_layout layout, cudaStream_t caller,
+                                   gb_graph** out);
 
 constexpr unsigned H100_SMS = 132;  // streaming multiprocessors of an H100 SXM: sizes the grid-stride grids
 

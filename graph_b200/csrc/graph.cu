@@ -460,6 +460,96 @@ static gb_status graph_from_host_edges(int device, gb_graph_kind kind, const uin
   return GB_OK;
 }
 
+__global__ void k_max_ids(const uint32_t* __restrict__ a, const uint32_t* __restrict__ b, uint64_t count,
+                          unsigned int* __restrict__ mx) {
+  uint32_t v = 0;
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
+       i += (uint64_t)gridDim.x * blockDim.x)
+    v = max(v, max(a[i], b[i]));
+  for (int o = 16; o; o >>= 1) v = max(v, __shfl_xor_sync(0xFFFFFFFFu, v, o));
+  if ((threadIdx.x & 31) == 0) atomicMax(mx, v);
+}
+
+static gb_status require_device_array(const void* p, int device, const char* what) {
+  cudaPointerAttributes a{};
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(GB_ERR_INVALID, "%s is not a device pointer", what);
+  }
+  GB_REQUIRE((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == device,
+             "%s is not device memory of device %d", what, device);
+  return GB_OK;
+}
+
+gb_status graph_from_device_arrays(int device, gb_graph_kind kind, const uint32_t* d_src, const uint32_t* d_dst,
+                                   const float* d_w, uint64_t m, uint32_t n, gb_layout layout, cudaStream_t caller,
+                                   gb_graph** out) {
+  GB_REQUIRE(out != nullptr, "graph out-pointer is NULL");
+  GB_REQUIRE(m == 0 || (d_src && d_dst), "edge arrays are NULL");
+  GB_REQUIRE((int)layout >= 0 && (int)layout <= 2, "bad layout %d", (int)layout);
+  uint64_t cap = (kind == GB_KIND_UNDIRECTED) ? 2 * m : m;
+  GB_REQUIRE(cap < 0xFFFFFFFFull, "edge count %llu does not fit u32 offsets", (unsigned long long)m);
+  GB_REQUIRE(n != 0 || m > 0, "cannot infer node_count from an empty edge list");
+  gb_graph* g = nullptr;
+  GB_TRY(new_graph(device, kind, n, &g));
+  gb_status st = [&]() -> gb_status {
+    if (m) {
+      GB_TRY(require_device_array(d_src, device, "d_src"));
+      GB_TRY(require_device_array(d_dst, device, "d_dst"));
+      if (d_w && kind == GB_KIND_DIRECTED) GB_TRY(require_device_array(d_w, device, "d_weights"));
+    }
+    // the caller's producer work comes first
+    cudaEvent_t ready;
+    GB_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
+    cudaError_t e = cudaEventRecord(ready, caller);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(g->stream, ready, 0);
+    cudaEventDestroy(ready);
+    GB_CUDA(e);
+    DevBuf<unsigned int> scratch;
+    GB_TRY(scratch.alloc(1));
+    GB_CUDA(cudaMemsetAsync(scratch.p, 0, 4, g->stream));
+    unsigned int h = 0;
+    if (n == 0) {  // Edges::max_node_id + 1, edgelist.rs:84-90
+      k_max_ids<<<grid_for(m, 256), 256, 0, g->stream>>>(d_src, d_dst, m, scratch.p);
+      GB_CUDA(cudaMemcpyAsync(&h, scratch.p, 4, cudaMemcpyDeviceToHost, g->stream));
+      GB_CUDA(cudaStreamSynchronize(g->stream));
+      GB_REQUIRE(h < 0xFFFFFFFFu, "node id 2^32-1 leaves no room for node_count");
+      g->n = h + 1;
+    } else {
+      if (m) {
+        k_check_ids<<<grid_for(m, 256), 256, 0, g->stream>>>(d_src, m, n, scratch.p);
+        k_check_ids<<<grid_for(m, 256), 256, 0, g->stream>>>(d_dst, m, n, scratch.p);
+      }
+      GB_CUDA(cudaMemcpyAsync(&h, scratch.p, 4, cudaMemcpyDeviceToHost, g->stream));
+      GB_CUDA(cudaStreamSynchronize(g->stream));
+      GB_REQUIRE(h == 0, "%u edge endpoints are >= node_count %u", h, n);
+    }
+    GB_CUDA(cudaGetLastError());
+    // build_csr_device only reads the edge arrays
+    return graph_from_device_edges(g, const_cast<uint32_t*>(d_src), const_cast<uint32_t*>(d_dst),
+                                   kind == GB_KIND_DIRECTED ? const_cast<float*>(d_w) : nullptr, m, layout);
+  }();
+  if (st != GB_OK) {
+    gb_graph_free(g);
+    return st;
+  }
+  *out = g;
+  return GB_OK;
+}
+
+template <typename T>
+__global__ void k_ids_to_u32(const T* __restrict__ in, uint64_t count, uint32_t* __restrict__ out,
+                             unsigned int* __restrict__ bad) {
+  bool b = false;
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
+       i += (uint64_t)gridDim.x * blockDim.x) {
+    const long long v = (long long)in[i];
+    b |= v < 0 || v > 0xFFFFFFFFll;
+    out[i] = (uint32_t)v;
+  }
+  if (__any_sync(0xFFFFFFFFu, b) && (threadIdx.x & 31) == 0) atomicOr(bad, 1u);
+}
+
 static gb_status rmat_graph(int device, gb_graph_kind kind, uint32_t scale, uint32_t edge_factor,
                             uint64_t seed, gb_layout layout, int weights, gb_graph** out) {
   GB_REQUIRE(out != nullptr, "graph out-pointer is NULL");
@@ -562,6 +652,46 @@ gb_status gb_digraph_from_edges_u32(int device, const uint32_t* src, const uint3
 gb_status gb_graph_from_edges_u32(int device, const uint32_t* src, const uint32_t* dst, uint64_t m,
                                   uint32_t n, gb_layout layout, gb_graph** graph) {
   return graph_from_host_edges(device, GB_KIND_UNDIRECTED, src, dst, nullptr, m, n, layout, graph);
+}
+
+gb_status gb_digraph_from_device_edges_u32(int device, const uint32_t* d_src, const uint32_t* d_dst,
+                                           const float* d_weights, uint64_t m, uint32_t n, gb_layout layout,
+                                           void* stream, gb_graph** graph) {
+  return graph_from_device_arrays(device, GB_KIND_DIRECTED, d_src, d_dst, d_weights, m, n, layout,
+                                  static_cast<cudaStream_t>(stream), graph);
+}
+
+gb_status gb_graph_from_device_edges_u32(int device, const uint32_t* d_src, const uint32_t* d_dst, uint64_t m,
+                                         uint32_t n, gb_layout layout, void* stream, gb_graph** graph) {
+  return graph_from_device_arrays(device, GB_KIND_UNDIRECTED, d_src, d_dst, nullptr, m, n, layout,
+                                  static_cast<cudaStream_t>(stream), graph);
+}
+
+gb_status gb_ids_to_u32(int device, const void* d_ids, int id_bytes, uint64_t count, uint32_t* d_out,
+                        void* stream) {
+  GB_REQUIRE(id_bytes == 4 || id_bytes == 8, "ids must be 4 or 8 bytes wide, not %d", id_bytes);
+  if (count == 0) return GB_OK;
+  GB_REQUIRE(d_ids && d_out, "NULL argument");
+  int devs = gb_device_count();
+  if (devs <= 0) return fail(GB_ERR_CUDA, "no CUDA device available: libgraph_b200 has no CPU fallback");
+  GB_REQUIRE(device >= 0 && device < devs, "device %d out of range", device);
+  DeviceGuard guard(device);
+  GB_TRY(require_device_array(d_ids, device, "ids"));
+  GB_TRY(require_device_array(d_out, device, "output ids"));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  DevBuf<unsigned int> bad;
+  GB_TRY(bad.alloc(1));
+  GB_CUDA(cudaMemsetAsync(bad.p, 0, 4, s));
+  if (id_bytes == 4)
+    k_ids_to_u32<int32_t><<<grid_for(count, 256), 256, 0, s>>>(static_cast<const int32_t*>(d_ids), count, d_out, bad.p);
+  else
+    k_ids_to_u32<int64_t><<<grid_for(count, 256), 256, 0, s>>>(static_cast<const int64_t*>(d_ids), count, d_out, bad.p);
+  GB_CUDA(cudaGetLastError());
+  unsigned int h = 0;
+  GB_CUDA(cudaMemcpyAsync(&h, bad.p, 4, cudaMemcpyDeviceToHost, s));
+  GB_CUDA(cudaStreamSynchronize(s));
+  GB_REQUIRE(h == 0, "node ids must be 32-bit unsigned integers");
+  return GB_OK;
 }
 
 gb_status gb_digraph_rmat(int device, uint32_t scale, uint32_t edge_factor, uint64_t seed,

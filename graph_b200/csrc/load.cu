@@ -1,0 +1,655 @@
+// load.cu — Graph500 and text edge-list files read straight into device edge arrays.
+//
+// The host readers (io.cu) decode the whole file in pageable memory, and the edges then cross PCIe.  Here
+// the file is streamed through a ring of pinned buffers: one thread per buffer preads the chunks that map
+// to it, the chunk goes to the device on a copy stream, and kernels on a second stream decode it into the
+// edge arrays.  A buffer is refilled only after its copy has completed, and a device buffer only after the
+// kernel that read it has.  The graph is then built from the device arrays (graph_from_device_arrays), so
+// it is the one the host readers followed by gb_[di]graph_from_edges_u32 give.
+//
+//   Graph500: records never straddle a chunk (chunks are a multiple of 48 bytes = 4 records), m = len / 12 is
+//   known up front, and k_load_graph500 decodes 4 records per thread with three 128-bit loads.
+//   Text: a chunk ends at its last '\n'; the bytes after it are carried into the next chunk.  The edge index
+//   of a line is the number of '\n' before it, so edges come out in file order: k_load_count_lines counts
+//   the '\n' of each 4 KB tile, a CUB scan turns the counts into tile bases, and k_load_parse_text finds the
+//   line starts of a tile from 128-bit loads (a block scan ranks them) and parses one line per start
+//   (edgelist_scan.h).  m is unknown until the end, so the edge arrays grow; values the device parser
+//   declines are listed (file offset, edge index) and re-parsed on the host with gb::parse_line.
+#include <fcntl.h>
+#include <sys/stat.h>
+#include <unistd.h>
+
+#include <algorithm>
+#include <cerrno>
+#include <condition_variable>
+#include <cstdlib>
+#include <memory>
+#include <thread>
+
+#include <cub/cub.cuh>
+
+#include "common.cuh"
+#include "edgelist_line.h"
+#include "edgelist_scan.h"
+
+namespace gb {
+
+constexpr unsigned LOAD_BLOCK = 256;                    // threads per CTA of the text kernels
+constexpr unsigned LOAD_TILE = LOAD_BLOCK * 16;         // bytes per CTA: one 128-bit load per thread
+constexpr uint64_t LOAD_DEFAULT_CHUNK = 64ull << 20;    // bytes per pinned buffer
+constexpr uint64_t LOAD_MIN_CHUNK = 64ull << 10;        // smallest buffer chosen for a small file
+constexpr uint64_t LOAD_CARRY_RESERVE = 4096;           // pinned bytes in front of a chunk for the carried line
+constexpr unsigned LOAD_RING = 4;                       // pinned buffers (and reader threads)
+
+struct LoadCounters {
+  unsigned int declined;  // text values re-parsed on the host
+  unsigned int wide;      // an id above 32 bits was seen
+};
+
+// bit j set = byte pos + j is '\n' and lies before len
+__device__ __forceinline__ uint32_t newline_mask(uint4 v, uint64_t pos, uint64_t len) {
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+  uint32_t m = 0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const uint32_t eq = __vcmpeq4(w[k], 0x0A0A0A0Au);  // 0xFF in every byte that is '\n'
+#pragma unroll
+    for (int b = 0; b < 4; ++b) m |= ((eq >> (8 * b + 7)) & 1u) << (4 * k + b);
+  }
+  if (pos >= len) return 0;
+  if (len - pos < 16) m &= (1u << (len - pos)) - 1u;
+  return m;
+}
+
+__global__ void __launch_bounds__(LOAD_BLOCK) k_load_count_lines(const uint4* __restrict__ buf, uint64_t len,
+                                                                 uint32_t* __restrict__ counts) {
+  using Reduce = cub::BlockReduce<uint32_t, LOAD_BLOCK>;
+  __shared__ typename Reduce::TempStorage tmp;
+  const uint64_t i = (uint64_t)blockIdx.x * LOAD_BLOCK + threadIdx.x;
+  const uint32_t c = __popc(newline_mask(buf[i], 16 * i, len));
+  const uint32_t total = Reduce(tmp).Sum(c);
+  if (threadIdx.x == 0) counts[blockIdx.x] = total;
+}
+
+// incl[t] = '\n' in tiles 0..t of the chunk; edge_base = edges of the earlier chunks; file_off = file
+// position of buf[0].  Lines start at 0 and after every '\n' that is not the chunk's last byte.
+__global__ void __launch_bounds__(LOAD_BLOCK) k_load_parse_text(const uint4* __restrict__ buf, uint64_t len,
+                                                                const uint32_t* __restrict__ incl,
+                                                                uint64_t edge_base, uint64_t file_off,
+                                                                int want_value, uint32_t* __restrict__ src,
+                                                                uint32_t* __restrict__ dst, float* __restrict__ w,
+                                                                LoadCounters* __restrict__ ctr,
+                                                                uint64_t* __restrict__ declined_off,
+                                                                uint32_t* __restrict__ declined_edge) {
+  using Scan = cub::BlockScan<uint32_t, LOAD_BLOCK>;
+  __shared__ typename Scan::TempStorage tmp;
+  const uint64_t i = (uint64_t)blockIdx.x * LOAD_BLOCK + threadIdx.x;
+  const uint64_t pos = 16 * i;
+  uint32_t m = newline_mask(buf[i], pos, len);
+  uint32_t before;
+  Scan(tmp).ExclusiveSum((uint32_t)__popc(m), before);
+  uint64_t e = edge_base + (blockIdx.x ? incl[blockIdx.x - 1] : 0u) + before;  // '\n' before this segment
+  const char* text = reinterpret_cast<const char*>(buf);
+  bool wide = false;
+  auto parse = [&](uint64_t start, uint64_t edge) {
+    ScannedLine sl;
+    scan_line(text, start, len, want_value != 0, &sl);
+    wide |= (sl.src | sl.dst) > 0xFFFFFFFFull;
+    src[edge] = (uint32_t)sl.src;
+    dst[edge] = (uint32_t)sl.dst;
+    if (want_value) {
+      w[edge] = sl.value;
+      if (sl.declined) {
+        const unsigned int k = atomicAdd(&ctr->declined, 1u);
+        declined_off[k] = file_off + start;
+        declined_edge[k] = (uint32_t)edge;
+      }
+    }
+  };
+  if (i == 0 && len > 0) parse(0, edge_base);
+  while (m) {
+    const int j = __ffs(m) - 1;
+    m &= m - 1;
+    ++e;  // this '\n' is before the line it ends
+    if (pos + j + 1 < len) parse(pos + j + 1, e);
+  }
+  if (__syncthreads_or(wide) && threadIdx.x == 0) atomicOr(&ctr->wide, 1u);
+}
+
+// PackedEdge{v0_low, v1_low, high} (graph500.rs:111-127): 4 records = 48 bytes = three 128-bit loads per
+// thread; edge_base is a multiple of 4, so the src / dst stores are 128-bit too.
+__global__ void k_load_graph500(const uint4* __restrict__ buf, uint64_t nrec, uint64_t edge_base,
+                                uint32_t* __restrict__ src, uint32_t* __restrict__ dst,
+                                LoadCounters* __restrict__ ctr) {
+  uint32_t high = 0;
+  const uint64_t groups = (nrec + 3) / 4;
+  for (uint64_t g = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; g < groups;
+       g += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t r0 = 4 * g;
+    if (r0 + 4 <= nrec) {
+      const uint4 a = buf[3 * g], b = buf[3 * g + 1], c = buf[3 * g + 2];
+      *reinterpret_cast<uint4*>(src + edge_base + r0) = make_uint4(a.x, a.w, b.z, c.y);
+      *reinterpret_cast<uint4*>(dst + edge_base + r0) = make_uint4(a.y, b.x, b.w, c.z);
+      high |= a.z | b.y | c.x | c.w;
+    } else {
+      const uint32_t* words = reinterpret_cast<const uint32_t*>(buf);
+      for (uint64_t r = r0; r < nrec; ++r) {
+        src[edge_base + r] = words[3 * r];
+        dst[edge_base + r] = words[3 * r + 1];
+        high |= words[3 * r + 2];
+      }
+    }
+  }
+  if (__any_sync(0xFFFFFFFFu, high != 0) && (threadIdx.x & 31) == 0) atomicOr(&ctr->wide, 1u);
+}
+
+__global__ void k_load_patch(const uint32_t* __restrict__ edge, const float* __restrict__ val, uint64_t count,
+                             float* __restrict__ w) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
+       i += (uint64_t)gridDim.x * blockDim.x)
+    w[edge[i]] = val[i];
+}
+
+// ---- host side ---------------------------------------------------------------------------------------
+static uint64_t env_chunk_bytes() {
+  const char* s = std::getenv("GB_LOAD_CHUNK_BYTES");
+  if (!s || !*s) return 0;
+  const unsigned long long v = std::strtoull(s, nullptr, 10);
+  return v;
+}
+
+static bool pread_all(int fd, char* dst, uint64_t bytes, uint64_t off) {
+  while (bytes) {
+    const ssize_t r = ::pread(fd, dst, bytes, (off_t)off);
+    if (r < 0 && errno == EINTR) continue;
+    if (r <= 0) return false;
+    dst += r;
+    off += (uint64_t)r;
+    bytes -= (uint64_t)r;
+  }
+  return true;
+}
+
+struct FileHandle {
+  int fd = -1;
+  ~FileHandle() {
+    if (fd >= 0) ::close(fd);
+  }
+};
+
+struct PinnedBuf {
+  char* p = nullptr;
+  ~PinnedBuf() {
+    if (p) cudaFreeHost(p);
+  }
+};
+
+// Pinning host memory costs about as much as reading it from the page cache, so the ring is kept for the
+// next load (at most LOAD_RING buffers of one default chunk each).  A load that finds it in use allocates
+// its own ring and frees it.
+struct PinnedRingCache {
+  std::mutex mu;
+  bool busy = false;
+  std::vector<char*> bufs;
+  uint64_t bytes = 0;  // of each buffer
+};
+static PinnedRingCache& pinned_ring_cache() {
+  static PinnedRingCache* c = new PinnedRingCache();  // never destroyed: no CUDA call at process exit
+  return *c;
+}
+
+// The ring of pinned buffers and the reader threads that fill it.  Thread r reads chunks r, r + R, ... into
+// buffer r, each after the consumer has released the buffer for it and the copy out of it has completed.
+struct ChunkReader {
+  int fd = -1, device = 0;
+  uint64_t chunk = 0, read_end = 0, nchunks = 0;
+  unsigned ring = 0;
+  std::vector<PinnedBuf> host;          // [ring]: LOAD_CARRY_RESERVE bytes, then the chunk
+  bool cached = false;                  // host[] belongs to the pinned ring cache
+  std::vector<cudaEvent_t> copied;      // [ring]: recorded behind the last copy out of the buffer
+  std::vector<uint64_t> filled;         // [ring]: chunk index + 1 the buffer holds (0: none yet)
+  std::vector<uint64_t> released_for;   // [ring]: the buffer may be filled with this chunk
+  std::vector<std::thread> threads;
+  std::mutex mu;
+  std::condition_variable cv;
+  bool stop = false, failed = false;
+  std::string error;
+
+  uint64_t chunk_bytes(uint64_t k) const { return std::min(chunk, read_end - k * chunk); }
+  char* data(unsigned r) { return host[r].p + LOAD_CARRY_RESERVE; }
+
+  gb_status start() {
+    host.resize(ring);
+    copied.assign(ring, nullptr);
+    filled.assign(ring, 0);
+    released_for.resize(ring);
+    const uint64_t bytes = LOAD_CARRY_RESERVE + chunk;
+    PinnedRingCache& pc = pinned_ring_cache();
+    {
+      std::lock_guard<std::mutex> lock(pc.mu);
+      if (!pc.busy && bytes <= LOAD_CARRY_RESERVE + LOAD_DEFAULT_CHUNK) {
+        pc.busy = cached = true;
+        if (pc.bytes < bytes || pc.bufs.size() < ring) {
+          for (char* p : pc.bufs) cudaFreeHost(p);
+          pc.bufs.clear();
+          pc.bytes = std::max(pc.bytes, bytes);
+          for (unsigned r = 0; r < ring; ++r) {
+            char* p = nullptr;
+            if (cudaHostAlloc(reinterpret_cast<void**>(&p), pc.bytes, cudaHostAllocDefault) != cudaSuccess) {
+              cudaGetLastError();
+              for (char* q : pc.bufs) cudaFreeHost(q);
+              pc.bufs.clear();
+              pc.bytes = 0;
+              pc.busy = cached = false;
+              break;
+            }
+            pc.bufs.push_back(p);
+          }
+        }
+        for (unsigned r = 0; cached && r < ring; ++r) host[r].p = pc.bufs[r];
+      }
+    }
+    for (unsigned r = 0; r < ring; ++r) {
+      released_for[r] = r;
+      if (!cached) GB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&host[r].p), bytes, cudaHostAllocDefault));
+      GB_CUDA(cudaEventCreateWithFlags(&copied[r], cudaEventDisableTiming));
+    }
+    for (unsigned r = 0; r < ring; ++r) threads.emplace_back([this, r] { run(r); });
+    return GB_OK;
+  }
+
+  void run(unsigned r) {
+    cudaSetDevice(device);
+    for (uint64_t k = r; k < nchunks; k += ring) {
+      {
+        std::unique_lock<std::mutex> lock(mu);
+        cv.wait(lock, [&] { return stop || released_for[r] == k; });
+        if (stop) return;
+      }
+      const bool ok = cudaEventSynchronize(copied[r]) == cudaSuccess &&
+                      pread_all(fd, data(r), chunk_bytes(k), k * chunk);
+      std::lock_guard<std::mutex> lock(mu);
+      if (!ok) {
+        failed = true;
+        error = "reading the file failed";
+        cv.notify_all();
+        return;
+      }
+      filled[r] = k + 1;
+      cv.notify_all();
+    }
+  }
+
+  gb_status wait_filled(uint64_t k) {
+    const unsigned r = (unsigned)(k % ring);
+    std::unique_lock<std::mutex> lock(mu);
+    cv.wait(lock, [&] { return failed || filled[r] == k + 1; });
+    if (failed) return fail(GB_ERR_INVALID, "%s", error.c_str());
+    return GB_OK;
+  }
+
+  void release(uint64_t k) {
+    std::lock_guard<std::mutex> lock(mu);
+    released_for[k % ring] = k + ring;
+    cv.notify_all();
+  }
+
+  ~ChunkReader() {
+    {
+      std::lock_guard<std::mutex> lock(mu);
+      stop = true;
+    }
+    cv.notify_all();
+    for (auto& t : threads) t.join();
+    for (cudaEvent_t e : copied) {
+      if (e) cudaEventSynchronize(e), cudaEventDestroy(e);  // no copy may still read a buffer
+    }
+    if (cached) {
+      for (auto& h : host) h.p = nullptr;  // back to the cache, not freed
+      PinnedRingCache& pc = pinned_ring_cache();
+      std::lock_guard<std::mutex> lock(pc.mu);
+      pc.busy = false;
+    }
+  }
+};
+
+struct StreamPair {
+  cudaStream_t copy = nullptr, work = nullptr;
+  ~StreamPair() {
+    if (copy) cudaStreamSynchronize(copy), cudaStreamDestroy(copy);
+    if (work) cudaStreamSynchronize(work), cudaStreamDestroy(work);
+  }
+};
+
+// grows a device array to hold at least `need` entries, keeping the first `keep`
+template <typename T>
+static gb_status grow(DevBuf<T>& b, uint64_t need, uint64_t want, uint64_t keep, cudaStream_t s) {
+  if (b.p && b.n >= need) return GB_OK;
+  DevBuf<T> nb;
+  GB_TRY(nb.alloc(std::max(need, want)));
+  if (keep) GB_CUDA(cudaMemcpyAsync(nb.p, b.p, keep * sizeof(T), cudaMemcpyDeviceToDevice, s));
+  b = std::move(nb);  // the old array is released once s has finished with it (DevBufStreamScope)
+  return GB_OK;
+}
+
+struct LoadedEdges {
+  DevBuf<uint32_t> src, dst;
+  DevBuf<float> w;
+  uint64_t m = 0;
+  uint32_t n = 0;  // 0: max id + 1
+};
+
+static gb_status load_file(int device, const char* path, gb_file_format format, bool want_value,
+                           LoadedEdges* out, gb_load_info* info) {
+  FileHandle f;
+  f.fd = ::open(path, O_RDONLY | O_CLOEXEC);
+  if (f.fd < 0) return fail(GB_ERR_INVALID, "cannot open %s: %s", path, std::strerror(errno));
+  struct stat st {};
+  if (::fstat(f.fd, &st) != 0 || !S_ISREG(st.st_mode)) return fail(GB_ERR_INVALID, "%s is not a regular file", path);
+  const uint64_t file_bytes = (uint64_t)st.st_size;
+  const bool g500 = format == GB_FORMAT_GRAPH500;
+  info->file_bytes = file_bytes;
+
+  ChunkReader rd;
+  rd.fd = f.fd;
+  rd.device = device;
+  const uint64_t m500 = file_bytes / 12;
+  rd.read_end = g500 ? 12 * m500 : file_bytes;  // a Graph500 tail shorter than a record is ignored
+  uint64_t chunk = env_chunk_bytes();
+  if (chunk == 0) {
+    const uint64_t quarter = (rd.read_end / LOAD_RING + 4095) & ~(uint64_t)4095;  // small files: all buffers busy
+    chunk = std::min(LOAD_DEFAULT_CHUNK, std::max(LOAD_MIN_CHUNK, quarter));
+  }
+  if (g500) chunk = std::max<uint64_t>(48, chunk / 48 * 48);  // whole 4-record groups
+  chunk = std::max<uint64_t>(chunk, 16);
+  rd.chunk = chunk;
+  rd.nchunks = (rd.read_end + chunk - 1) / chunk;
+  rd.ring = (unsigned)std::min<uint64_t>(LOAD_RING, std::max<uint64_t>(rd.nchunks, 1));
+  info->chunks = rd.nchunks;
+  if (rd.nchunks == 0) return GB_OK;  // empty: gb_*_from_device_edges reports it
+
+  StreamPair sp;
+  GB_CUDA(cudaStreamCreateWithFlags(&sp.copy, cudaStreamNonBlocking));
+  GB_CUDA(cudaStreamCreateWithFlags(&sp.work, cudaStreamNonBlocking));
+  GB_TRY(rd.start());
+  DevBufStreamScope scope(sp.work);
+
+  const unsigned R = rd.ring;
+  std::vector<DevBuf<uint8_t>> dbuf(R);
+  std::vector<cudaEvent_t> parsed(R, nullptr);
+  struct Events {
+    std::vector<cudaEvent_t>* v;
+    ~Events() {
+      for (cudaEvent_t e : *v)
+        if (e) cudaEventDestroy(e);
+    }
+  } parsed_guard{&parsed};
+  for (unsigned r = 0; r < R; ++r) GB_CUDA(cudaEventCreateWithFlags(&parsed[r], cudaEventDisableTiming));
+  DevBuf<LoadCounters> ctr;
+  GB_TRY(ctr.alloc(1));
+  GB_CUDA(cudaMemsetAsync(ctr.p, 0, sizeof(LoadCounters), sp.work));
+  PinnedBuf small;  // [0] = '\n' in the chunk, [1] = declined so far
+  GB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&small.p), 64, cudaHostAllocDefault));
+  uint32_t* hsmall = reinterpret_cast<uint32_t*>(small.p);
+
+  DevBuf<uint32_t> counts;  // per-tile '\n' counts, scanned in place
+  DevBuf<uint8_t> scan_tmp;
+  DevBuf<uint64_t> dec_off;
+  DevBuf<uint32_t> dec_edge;
+  // on every exit, nothing may still be copying into the buffers above when they are released
+  struct Drain {
+    StreamPair* sp;
+    ~Drain() { cudaStreamSynchronize(sp->copy); }
+  } drain{&sp};
+  uint64_t h2d = 0, m = 0;
+  if (g500) {
+    GB_TRY(out->src.alloc(m500));
+    GB_TRY(out->dst.alloc(m500));
+  }
+
+  // what prepare() leaves for run(): the device chunk and where it starts in the file
+  struct Staged {
+    uint64_t len = 0, file_off = 0;
+    bool ends_with_newline = true;
+  };
+  std::vector<Staged> staged(R);
+  std::string carry;  // text: the bytes after the last '\n' so far
+
+  // waits for chunk k's bytes, moves them (with the carried line in front) to the device on the copy stream
+  auto prepare = [&](uint64_t k) -> gb_status {
+    const unsigned r = (unsigned)(k % R);
+    GB_TRY(rd.wait_filled(k));
+    char* data = rd.data(r);
+    const uint64_t n = rd.chunk_bytes(k);
+    const bool last = k + 1 == rd.nchunks;
+    uint64_t body = n;  // bytes of this chunk that go to the device now
+    std::string next_carry;
+    if (!g500 && !last) {
+      const void* nl = memrchr(data, '\n', n);
+      body = nl ? (uint64_t)(static_cast<const char*>(nl) - data) + 1 : 0;
+      if (!nl) next_carry = carry;
+      next_carry.append(data + body, n - body);
+    }
+    const uint64_t cl = (!g500 && (body || last)) ? carry.size() : 0;  // carried bytes that go in front
+    Staged& sg = staged[r];
+    sg.len = cl + body;
+    sg.file_off = k * rd.chunk - cl;
+    sg.ends_with_newline = sg.len == 0 || (body ? data[body - 1] == '\n' : carry.back() == '\n');
+    if (sg.len) {
+      if (dbuf[r].n < sg.len + LOAD_TILE) {
+        GB_CUDA(cudaEventSynchronize(parsed[r]));
+        DevBuf<uint8_t> nb;
+        GB_TRY(nb.alloc(std::max<uint64_t>(sg.len, rd.chunk + LOAD_CARRY_RESERVE) + LOAD_TILE));
+        dbuf[r] = std::move(nb);
+      }
+      GB_CUDA(cudaStreamWaitEvent(sp.copy, parsed[r], 0));  // the kernel that read this device buffer is done
+      if (cl <= LOAD_CARRY_RESERVE) {
+        std::memcpy(data - cl, carry.data(), cl);
+        GB_CUDA(cudaMemcpyAsync(dbuf[r].p, data - cl, sg.len, cudaMemcpyHostToDevice, sp.copy));
+      } else {  // a line longer than the reserve: its head goes from pageable memory
+        GB_CUDA(cudaMemcpyAsync(dbuf[r].p, carry.data(), cl, cudaMemcpyHostToDevice, sp.copy));
+        if (body) GB_CUDA(cudaMemcpyAsync(dbuf[r].p + cl, data, body, cudaMemcpyHostToDevice, sp.copy));
+      }
+      h2d += sg.len;
+      GB_CUDA(cudaEventRecord(rd.copied[r], sp.copy));
+    }
+    rd.release(k);
+    if (sg.len) GB_CUDA(cudaStreamWaitEvent(sp.work, rd.copied[r], 0));
+    if (!g500) carry.swap(next_carry);
+    return GB_OK;
+  };
+
+  GB_TRY(prepare(0));
+  for (uint64_t k = 0; k < rd.nchunks; ++k) {
+    const unsigned r = (unsigned)(k % R);
+    const Staged sg = staged[r];
+    const uint4* d = reinterpret_cast<const uint4*>(dbuf[r].p);
+    if (g500) {
+      if (k + 1 < rd.nchunks) GB_TRY(prepare(k + 1));
+      const uint64_t nrec = sg.len / 12;
+      if (nrec) {
+        k_load_graph500<<<grid_for((nrec + 3) / 4, 256), 256, 0, sp.work>>>(d, nrec, k * rd.chunk / 12, out->src.p,
+                                                                             out->dst.p, ctr.p);
+        GB_CUDA(cudaGetLastError());
+      }
+      GB_CUDA(cudaEventRecord(parsed[r], sp.work));
+      continue;
+    }
+    const uint64_t tiles = (sg.len + LOAD_TILE - 1) / LOAD_TILE;
+    if (tiles) {
+      GB_TRY(grow(counts, tiles, 2 * tiles, 0, sp.work));
+      k_load_count_lines<<<(unsigned)tiles, LOAD_BLOCK, 0, sp.work>>>(d, sg.len, counts.p);
+      size_t tb = 0;
+      GB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, counts.p, counts.p, (int)tiles, sp.work));
+      GB_TRY(grow(scan_tmp, tb, 2 * tb, 0, sp.work));
+      GB_CUDA(cub::DeviceScan::InclusiveSum(scan_tmp.p, tb, counts.p, counts.p, (int)tiles, sp.work));
+      GB_CUDA(cudaMemcpyAsync(hsmall, counts.p + tiles - 1, 4, cudaMemcpyDeviceToHost, sp.work));
+      GB_CUDA(cudaMemcpyAsync(hsmall + 1, &ctr.p->declined, 4, cudaMemcpyDeviceToHost, sp.work));
+    }
+    if (k + 1 < rd.nchunks) GB_TRY(prepare(k + 1));  // the next chunk crosses the bus meanwhile
+    if (tiles) {
+      GB_CUDA(cudaStreamSynchronize(sp.work));
+      const uint64_t lines = hsmall[0] + (sg.ends_with_newline ? 0 : 1);
+      // size the arrays for the whole file from the lines per byte seen so far
+      const uint64_t through = std::min(rd.read_end, (k + 1) * rd.chunk);
+      const uint64_t est = (uint64_t)((double)(m + lines) * (double)rd.read_end / (double)through * 1.02) + 1024;
+      const uint64_t want = std::max(est, out->src.n + out->src.n / 2);
+      GB_TRY(grow(out->src, m + lines, want, m, sp.work));
+      GB_TRY(grow(out->dst, m + lines, want, m, sp.work));
+      if (want_value) {
+        GB_TRY(grow(out->w, m + lines, want, m, sp.work));
+        const uint64_t declined = hsmall[1];
+        GB_TRY(grow(dec_off, declined + lines, 2 * (declined + lines), declined, sp.work));
+        GB_TRY(grow(dec_edge, declined + lines, 2 * (declined + lines), declined, sp.work));
+      }
+      k_load_parse_text<<<(unsigned)tiles, LOAD_BLOCK, 0, sp.work>>>(d, sg.len, counts.p, m, sg.file_off,
+                                                                    want_value ? 1 : 0, out->src.p, out->dst.p,
+                                                                    out->w.p, ctr.p, dec_off.p, dec_edge.p);
+      GB_CUDA(cudaGetLastError());
+      m += lines;
+    }
+    GB_CUDA(cudaEventRecord(parsed[r], sp.work));
+  }
+  LoadCounters hc{};
+  GB_CUDA(cudaMemcpyAsync(&hc, ctr.p, sizeof hc, cudaMemcpyDeviceToHost, sp.work));
+  GB_CUDA(cudaStreamSynchronize(sp.work));
+  GB_REQUIRE(hc.wide == 0, g500 ? "Graph500 node id does not fit 32 bits" : "edge list node id does not fit 32 bits");
+  if (g500) m = m500;
+
+  // declined values: re-read each line and parse it with the host reader's own function
+  if (hc.declined) {
+    std::vector<uint64_t> off(hc.declined);
+    std::vector<uint32_t> edge(hc.declined);
+    GB_CUDA(cudaMemcpyAsync(off.data(), dec_off.p, hc.declined * 8ull, cudaMemcpyDeviceToHost, sp.work));
+    GB_CUDA(cudaMemcpyAsync(edge.data(), dec_edge.p, hc.declined * 4ull, cudaMemcpyDeviceToHost, sp.work));
+    GB_CUDA(cudaStreamSynchronize(sp.work));
+    std::vector<float> val(hc.declined);
+    std::string line;
+    for (uint64_t i = 0; i < hc.declined; ++i) {
+      uint64_t want = 256;
+      for (;;) {
+        const uint64_t n = std::min(want, file_bytes - off[i]);
+        line.resize(n);
+        if (!pread_all(f.fd, &line[0], n, off[i])) return fail(GB_ERR_INVALID, "reading %s failed", path);
+        if (n == file_bytes - off[i] || std::memchr(line.data(), '\n', n)) break;
+        want *= 2;
+      }
+      uint64_t s, t;
+      gb::parse_line(line.data(), 0, line.size(), 1, &s, &t, &val[i]);
+    }
+    DevBuf<float> dval;
+    GB_TRY(dval.alloc(hc.declined));
+    GB_CUDA(cudaMemcpyAsync(dval.p, val.data(), hc.declined * 4ull, cudaMemcpyHostToDevice, sp.work));
+    k_load_patch<<<grid_for(hc.declined, 256), 256, 0, sp.work>>>(dec_edge.p, dval.p, hc.declined, out->w.p);
+    GB_CUDA(cudaGetLastError());
+    GB_CUDA(cudaStreamSynchronize(sp.work));
+    h2d += hc.declined * 4ull;
+  }
+  out->m = m;
+  out->n = g500 ? (uint32_t)std::min<uint64_t>(m500 / 16, 0xFFFFFFFFull) : 0;  // graph500.rs:74
+  info->edges = m;
+  info->fallback_lines = hc.declined;
+  info->h2d_bytes = h2d;
+  GB_CUDA(cudaStreamSynchronize(sp.copy));
+  return GB_OK;
+}
+
+// Below these sizes the fixed costs of the pipeline (threads, streams, pinned ring) exceed what it saves, and
+// the host readers are faster (H100 80GB HBM3, 400 W; tools/bench_load.py).  GB_LOAD_CHUNK_BYTES, when
+// set, selects the device path whatever the size.
+static uint64_t load_device_min_bytes(gb_file_format format) {
+  (void)format;
+  return 64ull << 20;
+}
+
+// the host readers of io.cu and the upload of gb_[di]graph_from_edges_u32
+static gb_status load_on_host(int device, gb_graph_kind kind, const char* path, gb_file_format format,
+                              gb_layout layout, bool want_value, gb_graph** graph, gb_load_info* info) {
+  FileHandle f;
+  f.fd = ::open(path, O_RDONLY | O_CLOEXEC);
+  if (f.fd < 0) return fail(GB_ERR_INVALID, "cannot open %s: %s", path, std::strerror(errno));
+  struct stat st {};
+  if (::fstat(f.fd, &st) != 0 || !S_ISREG(st.st_mode)) return fail(GB_ERR_INVALID, "%s is not a regular file", path);
+  const uint64_t len = (uint64_t)st.st_size;
+  std::unique_ptr<char[]> bytes(new (std::nothrow) char[len ? len : 1]);  // not zero-filled
+  if (!bytes) return fail(GB_ERR_OOM, "host allocation of %llu bytes failed", (unsigned long long)len);
+  if (len && !pread_all(f.fd, bytes.get(), len, 0)) return fail(GB_ERR_INVALID, "reading %s failed", path);
+  std::vector<uint32_t> src, dst;
+  std::vector<float> w;
+  uint64_t m = 0;
+  uint32_t n = 0;
+  if (format == GB_FORMAT_GRAPH500) {
+    src.resize(len / 12);
+    dst.resize(len / 12);
+    GB_TRY(gb_graph500_decode(bytes.get(), len, src.data(), dst.data(), &m, &n));
+  } else {
+    GB_TRY(gb_edge_list_parse(bytes.get(), len, nullptr, nullptr, nullptr, &m));
+    src.resize(m);
+    dst.resize(m);
+    if (want_value) w.resize(m);
+    GB_TRY(gb_edge_list_parse(bytes.get(), len, src.data(), dst.data(), want_value ? w.data() : nullptr, &m));
+  }
+  if (kind == GB_KIND_DIRECTED)
+    GB_TRY(gb_digraph_from_edges_u32(device, src.data(), dst.data(), want_value ? w.data() : nullptr, m, n, layout,
+                                     graph));
+  else
+    GB_TRY(gb_graph_from_edges_u32(device, src.data(), dst.data(), m, n, layout, graph));
+  info->file_bytes = len;
+  info->edges = m;
+  info->h2d_bytes = m * (want_value ? 12 : 8);
+  return GB_OK;
+}
+
+static gb_status load_graph(int device, gb_graph_kind kind, const char* path, gb_file_format format,
+                            gb_layout layout, int with_values, gb_graph** graph) {
+  GB_REQUIRE(graph != nullptr, "graph out-pointer is NULL");
+  GB_REQUIRE(path != nullptr, "path is NULL");
+  GB_REQUIRE(format == GB_FORMAT_GRAPH500 || format == GB_FORMAT_EDGE_LIST, "unknown file format %d", (int)format);
+  GB_REQUIRE(!with_values || format == GB_FORMAT_EDGE_LIST, "only edge lists carry edge values");
+  GB_REQUIRE((int)layout >= 0 && (int)layout <= 2, "bad layout %d", (int)layout);
+  int count = 0;
+  if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0) {
+    cudaGetLastError();
+    return fail(GB_ERR_CUDA, "no CUDA device available: libgraph_b200 has no CPU fallback");
+  }
+  GB_REQUIRE(device >= 0 && device < count, "device %d out of range (have %d)", device, count);
+  DeviceGuard guard(device);
+  struct stat st {};
+  if (::stat(path, &st) != 0) return fail(GB_ERR_INVALID, "cannot open %s: %s", path, std::strerror(errno));
+  gb_load_info info{};
+  if (env_chunk_bytes() == 0 && (uint64_t)st.st_size < load_device_min_bytes(format)) {
+    GB_TRY(load_on_host(device, kind, path, format, layout, with_values != 0, graph, &info));
+    (*graph)->load = info;
+    return GB_OK;
+  }
+  LoadedEdges e;
+  GB_TRY(load_file(device, path, format, with_values != 0, &e, &info));
+  gb_graph* g = nullptr;
+  GB_TRY(graph_from_device_arrays(device, kind, e.src.p, e.dst.p, with_values ? e.w.p : nullptr, e.m, e.n, layout,
+                                  nullptr, &g));
+  g->load = info;
+  *graph = g;
+  return GB_OK;
+}
+
+}  // namespace gb
+
+extern "C" {
+
+gb_status gb_digraph_load_u32(int device, const char* path, gb_file_format format, gb_layout layout,
+                              int with_values, gb_graph** graph) {
+  return gb::load_graph(device, GB_KIND_DIRECTED, path, format, layout, with_values, graph);
+}
+
+gb_status gb_graph_load_u32(int device, const char* path, gb_file_format format, gb_layout layout,
+                            gb_graph** graph) {
+  return gb::load_graph(device, GB_KIND_UNDIRECTED, path, format, layout, 0, graph);
+}
+
+gb_status gb_graph_load_info(const gb_graph* g, gb_load_info* info) {
+  GB_REQUIRE(g && info, "NULL argument");
+  *info = g->load;
+  return GB_OK;
+}
+
+}  // extern "C"

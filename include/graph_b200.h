@@ -175,6 +175,48 @@ gb_status gb_graph500_encode(const uint32_t* src, const uint32_t* dst, uint64_t 
 gb_status gb_edge_list_parse(const char* text, uint64_t len, uint32_t* src, uint32_t* dst,
                              float* values, uint64_t* edge_count);
 
+/* ---- loading files on the device ----------------------------------------------------------------
+ * The file is streamed through a ring of pinned buffers (pread on several threads, copy stream, parse
+ * kernels); no host edge array exists.  The graph is the one the host readers above followed by
+ * gb_[di]graph_from_edges_u32 give, byte for byte, with the same errors and messages.  Text values that
+ * the device parser declines (inf, nan, long or exotic spellings) are re-parsed on the host.  Files below
+ * 64 MiB are read by the host readers, whose fixed costs are lower; the
+ * pinned ring (at most 4 x 64 MiB) is kept for the next load.
+ * GB_LOAD_CHUNK_BYTES (environment, read per call) sets the buffer size and selects the device path at
+ * any file size, for tests. */
+typedef enum gb_file_format {
+  GB_FORMAT_GRAPH500 = 0, /* packed 12-byte records; node_count = edges / 16 */
+  GB_FORMAT_EDGE_LIST = 1 /* text "<src> <dst>[ <f32>]"; node_count = max id + 1 */
+} gb_file_format;
+/* with_values: read the third column of an edge list as f32 edge values (Graph500 has none) */
+gb_status gb_digraph_load_u32(int device, const char* path, gb_file_format format, gb_layout layout,
+                              int with_values, gb_graph** graph);
+gb_status gb_graph_load_u32(int device, const char* path, gb_file_format format, gb_layout layout,
+                            gb_graph** graph);
+/* Statistics of the load that created the graph (all zero for graphs made otherwise). */
+typedef struct gb_load_info {
+  uint64_t file_bytes;     /* size of the file */
+  uint64_t chunks;         /* pinned buffers the file was streamed through */
+  uint64_t edges;          /* edges read */
+  uint64_t fallback_lines; /* lines whose value was re-parsed on the host */
+  uint64_t h2d_bytes;      /* bytes copied host -> device */
+} gb_load_info;
+gb_status gb_graph_load_info(const gb_graph* graph, gb_load_info* info);
+
+/* From DEVICE edge arrays on `device` (not modified, not kept): like gb_[di]graph_from_edges_u32 without the
+ * upload.  node_count == 0 means max id + 1, found on the device.  Work already enqueued on `stream`
+ * (a cudaStream_t; NULL = the legacy default stream) is waited for before the arrays are read. */
+gb_status gb_digraph_from_device_edges_u32(int device, const uint32_t* d_src, const uint32_t* d_dst,
+                                           const float* d_weights, uint64_t edge_count, uint32_t node_count,
+                                           gb_layout layout, void* stream, gb_graph** graph);
+gb_status gb_graph_from_device_edges_u32(int device, const uint32_t* d_src, const uint32_t* d_dst,
+                                         uint64_t edge_count, uint32_t node_count, gb_layout layout,
+                                         void* stream, gb_graph** graph);
+/* Narrows device ids (int32 when id_bytes == 4, int64 when 8) to uint32 on the device; any id outside
+ * [0, 2^32) is GB_ERR_INVALID.  Enqueued on `stream`, waited for before returning. */
+gb_status gb_ids_to_u32(int device, const void* d_ids, int id_bytes, uint64_t count, uint32_t* d_out,
+                        void* stream);
+
 gb_status gb_graph_free(gb_graph* graph);
 gb_status gb_graph_get_info(const gb_graph* graph, gb_graph_info* info);
 /* copy a CSR back to the host (neighbour views of the host mirror: csr.rs:97-117).
