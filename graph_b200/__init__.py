@@ -399,6 +399,13 @@ def _timed(fn):
     return out, max(1, int((time.perf_counter() - t0) * 1e6))
 
 
+def _construct(cls, fn, *args):
+    """cls around the graph the C constructor fn(*args, &graph) makes, with the call's time as load_micros."""
+    out = C.c_void_p()
+    _, micros = _timed(lambda: check(fn(*args, C.byref(out))))
+    return cls(out, micros)
+
+
 _PR_MODES = {"auto": _capi.PR_AUTO, "exact": _capi.PR_EXACT, "jacobi": _capi.PR_JACOBI}
 
 
@@ -409,46 +416,28 @@ class DiGraph(_Handle):
     # -- construction --
     @staticmethod
     def _from_edges(src, dst, weights, node_count, layout) -> "DiGraph":
-        out = C.c_void_p()
-
-        def go():
-            check(lib.gb_digraph_from_edges_u32(_device, _ptr(src), _ptr(dst), _ptr(weights), len(src),
-                                                node_count, _layout_value(layout), C.byref(out)))
-        _, micros = _timed(go)
-        return DiGraph(out, micros)
+        return _construct(DiGraph, lib.gb_digraph_from_edges_u32, _device, _ptr(src), _ptr(dst), _ptr(weights),
+                          len(src), node_count, _layout_value(layout))
 
     @staticmethod
     def load(path, layout=None, file_format=FileFormat.Graph500) -> "DiGraph":
         """Load a graph from the provided format (crates/mate/src/graphs/digraph.rs:35-44); the file is
         parsed on the device."""
-        t0 = time.perf_counter()
-        p, fmt, lay = _load_args(path, file_format, layout)
-        out = C.c_void_p()
-        check(lib.gb_digraph_load_u32(_device, p, fmt, lay, 0, C.byref(out)))
-        return DiGraph(out, max(1, int((time.perf_counter() - t0) * 1e6)))
+        return _construct(DiGraph, lib.gb_digraph_load_u32, _device, *_load_args(path, file_format, layout), 0)
 
     @staticmethod
     def load_weighted(path, layout=None) -> "DiGraph":
         """Weighted text edge list `<src> <dst> <f32>` (DirectedCsrGraph<u32, (), f32>, for sssp)."""
-        t0 = time.perf_counter()
-        p, fmt, lay = _load_args(path, FileFormat.EdgeList, layout)
-        out = C.c_void_p()
-        check(lib.gb_digraph_load_u32(_device, p, fmt, lay, 1, C.byref(out)))
-        return DiGraph(out, max(1, int((time.perf_counter() - t0) * 1e6)))
+        return _construct(DiGraph, lib.gb_digraph_load_u32, _device, *_load_args(path, FileFormat.EdgeList, layout), 1)
 
     @staticmethod
     def from_torch(src, dst, weights=None, node_count: int = 0, layout=None) -> "DiGraph":
         """From contiguous 1-D CUDA tensors on the graph's device (ids int32 or int64, weights float32),
         without a host copy.  node_count 0 means max id + 1."""
         s, d, w, m, stream = _torch_edges(src, dst, weights)
-        out = C.c_void_p()
-
-        def go():
-            check(lib.gb_digraph_from_device_edges_u32(_device, s.data_ptr(), d.data_ptr(),
-                                                       None if w is None else w.data_ptr(), m, int(node_count),
-                                                       _layout_value(layout), stream.cuda_stream, C.byref(out)))
-        _, micros = _timed(go)
-        return DiGraph(out, micros)
+        return _construct(DiGraph, lib.gb_digraph_from_device_edges_u32, _device, s.data_ptr(), d.data_ptr(),
+                          None if w is None else w.data_ptr(), m, int(node_count), _layout_value(layout),
+                          stream.cuda_stream)
 
     @staticmethod
     def from_numpy(arr, layout=None, weights=None, node_count: int = 0) -> "DiGraph":
@@ -476,13 +465,8 @@ class DiGraph(_Handle):
             raise ValueError("in and out offsets must have the same length (node_count + 1)")
         if ow is not None and len(ow) != len(ot):
             raise ValueError("out_weights must have one entry per out target")
-        out = C.c_void_p()
-
-        def go():
-            check(lib.gb_digraph_from_csr_u32(_device, len(oo) - 1, _ptr(oo), _ptr(ot), _ptr(ow), _ptr(io),
-                                              _ptr(it), C.byref(out)))
-        _, micros = _timed(go)
-        return DiGraph(out, micros)
+        return _construct(DiGraph, lib.gb_digraph_from_csr_u32, _device, len(oo) - 1, _ptr(oo), _ptr(ot), _ptr(ow),
+                          _ptr(io), _ptr(it))
 
     @staticmethod
     def for_page_rank(in_offsets, in_targets, out_offsets) -> "DiGraph":
@@ -495,23 +479,14 @@ class DiGraph(_Handle):
         _check_host_csr(io, it, "in")
         if len(oo) != len(io):
             raise ValueError("in and out offsets must have the same length (node_count + 1)")
-        out = C.c_void_p()
-
-        def go():
-            check(lib.gb_digraph_for_page_rank_u32(_device, len(io) - 1, _ptr(io), _ptr(it), _ptr(oo), C.byref(out)))
-        _, micros = _timed(go)
-        return DiGraph(out, micros)
+        return _construct(DiGraph, lib.gb_digraph_for_page_rank_u32, _device, len(io) - 1, _ptr(io), _ptr(it),
+                          _ptr(oo))
 
     @staticmethod
     def rmat(scale: int, edge_factor: int = 16, seed: int = 42, layout=Layout.Sorted, weights=False) -> "DiGraph":
         """Synthetic R-MAT graph generated and built on device (the BASELINE.json workload)."""
-        out = C.c_void_p()
-
-        def go():
-            check(lib.gb_digraph_rmat(_device, scale, edge_factor, seed, _layout_value(layout), int(bool(weights)),
-                                      C.byref(out)))
-        _, micros = _timed(go)
-        return DiGraph(out, micros)
+        return _construct(DiGraph, lib.gb_digraph_rmat, _device, scale, edge_factor, seed, _layout_value(layout),
+                          int(bool(weights)))
 
     # -- accessors --
     def out_degree(self, node: int) -> int:
@@ -547,12 +522,7 @@ class DiGraph(_Handle):
 
     def to_undirected(self, layout=None) -> "Graph":
         """New, unrelated undirected graph (graph_ops.rs:229; csr.rs:391-464)."""
-        out = C.c_void_p()
-
-        def go():
-            check(lib.gb_to_undirected(self._g, _layout_value(layout), C.byref(out)))
-        _, micros = _timed(go)
-        return Graph(out, micros)
+        return _construct(Graph, lib.gb_to_undirected, self._g, _layout_value(layout))
 
     def in_degree_partition(self, parts: int) -> list:
         """graph_ops.rs:431-439 — ranges as [(start, end), ...]"""
@@ -632,33 +602,19 @@ class Graph(_Handle):
 
     @staticmethod
     def _from_edges(src, dst, node_count, layout) -> "Graph":
-        out = C.c_void_p()
-
-        def go():
-            check(lib.gb_graph_from_edges_u32(_device, _ptr(src), _ptr(dst), len(src), node_count,
-                                              _layout_value(layout), C.byref(out)))
-        _, micros = _timed(go)
-        return Graph(out, micros)
+        return _construct(Graph, lib.gb_graph_from_edges_u32, _device, _ptr(src), _ptr(dst), len(src), node_count,
+                          _layout_value(layout))
 
     @staticmethod
     def load(path, layout=None, file_format=FileFormat.Graph500) -> "Graph":
-        t0 = time.perf_counter()
-        p, fmt, lay = _load_args(path, file_format, layout)
-        out = C.c_void_p()
-        check(lib.gb_graph_load_u32(_device, p, fmt, lay, C.byref(out)))
-        return Graph(out, max(1, int((time.perf_counter() - t0) * 1e6)))
+        return _construct(Graph, lib.gb_graph_load_u32, _device, *_load_args(path, file_format, layout))
 
     @staticmethod
     def from_torch(src, dst, node_count: int = 0, layout=None) -> "Graph":
         """From contiguous 1-D int32 / int64 CUDA tensors on the graph's device, without a host copy."""
         s, d, _, m, stream = _torch_edges(src, dst, None)
-        out = C.c_void_p()
-
-        def go():
-            check(lib.gb_graph_from_device_edges_u32(_device, s.data_ptr(), d.data_ptr(), m, int(node_count),
-                                                     _layout_value(layout), stream.cuda_stream, C.byref(out)))
-        _, micros = _timed(go)
-        return Graph(out, micros)
+        return _construct(Graph, lib.gb_graph_from_device_edges_u32, _device, s.data_ptr(), d.data_ptr(), m,
+                          int(node_count), _layout_value(layout), stream.cuda_stream)
 
     @staticmethod
     def from_numpy(arr, layout=None, node_count: int = 0) -> "Graph":
@@ -674,21 +630,11 @@ class Graph(_Handle):
         off = np.ascontiguousarray(offsets, np.uint32)
         tgt = np.ascontiguousarray(targets, np.uint32)
         _check_host_csr(off, tgt, "undirected")
-        out = C.c_void_p()
-
-        def go():
-            check(lib.gb_graph_from_csr_u32(_device, len(off) - 1, _ptr(off), _ptr(tgt), C.byref(out)))
-        _, micros = _timed(go)
-        return Graph(out, micros)
+        return _construct(Graph, lib.gb_graph_from_csr_u32, _device, len(off) - 1, _ptr(off), _ptr(tgt))
 
     @staticmethod
     def rmat(scale: int, edge_factor: int = 16, seed: int = 42, layout=Layout.Sorted) -> "Graph":
-        out = C.c_void_p()
-
-        def go():
-            check(lib.gb_graph_rmat(_device, scale, edge_factor, seed, _layout_value(layout), C.byref(out)))
-        _, micros = _timed(go)
-        return Graph(out, micros)
+        return _construct(Graph, lib.gb_graph_rmat, _device, scale, edge_factor, seed, _layout_value(layout))
 
     def degree(self, node: int) -> int:
         return self._degree(_capi.CSR_UNDIRECTED, node)

@@ -6,6 +6,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <string>
@@ -122,7 +123,6 @@ struct DevCsr {
   DevBuf<uint32_t> tgt;
   DevBuf<float> w;
   uint64_t len = 0;
-  bool present() const { return off.p != nullptr; }
   uint64_t bytes() const { return off.bytes() + tgt.bytes() + w.bytes(); }
 };
 
@@ -154,7 +154,6 @@ struct gb_graph {
   mutable gb::PrPlan* pr_plan = nullptr;  // lazily built PageRank layout (pagerank.cu)
   mutable const gb::TargetFeed* feed = nullptr;  // set only while gb_page_rank_csr_u32 streams the targets in
   mutable gb_timing timing{};
-  uint64_t extra_bytes = 0;
   gb_load_info load{};  // filled by gb_[di]graph_load_u32 (load.cu)
 };
 
@@ -176,15 +175,31 @@ struct DeviceGuard {
   }
 };
 
+// owning graph handle: a constructor that fails part-way releases the graph by returning
+struct GraphFree {
+  void operator()(gb_graph* g) const { gb_graph_free(g); }
+};
+using GraphPtr = std::unique_ptr<gb_graph, GraphFree>;
+
+// GB_ERR_CUDA when there is no CUDA device, GB_ERR_INVALID when `device` is not one of them
+gb_status require_device(int device);
+gb_status check_layout(gb_layout layout);
+
 // CSR construction on device (graph.cu)
-// rows/cols: device arrays of `count` entries (consumed / overwritten). Builds `csr` with the
-// given layout; n rows.  w may be null.
-gb_status build_csr_device(cudaStream_t s, uint32_t n, uint32_t* d_rows, uint32_t* d_cols, float* d_w,
-                           uint64_t count, gb_layout layout, DevCsr* csr);
-gb_status new_graph(int device, gb_graph_kind kind, uint32_t n, gb_graph** out);
-// uploads a host CSR (offsets always, targets/weights when non-null) and validates it on the device
+// rows/cols: device arrays of `count` entries, only read. Builds `csr` with the given layout; n rows.
+// w may be null.
+gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, const uint32_t* d_cols,
+                           const float* d_w, uint64_t count, gb_layout layout, DevCsr* csr);
+gb_status new_graph(int device, gb_graph_kind kind, uint32_t n, GraphPtr* out);
+// Uploads a host CSR on stream s and checks it: offsets[0] == 0 on the host, the offsets monotone and the
+// targets below n on the device.  offsets_only uploads the offsets alone (degrees); otherwise tgt must
+// be non-NULL when the CSR has entries, and w may be NULL.  Returns with s synchronised.
 gb_status upload_host_csr(cudaStream_t s, uint32_t n, const uint32_t* off, const uint32_t* tgt, const float* w,
-                          DevCsr* csr, const char* what);
+                          DevCsr* csr, const char* what, bool offsets_only = false);
+// enqueue on s: *bad += the number of ids in a[0, count) that are >= n
+void check_ids_async(cudaStream_t s, const uint32_t* a, uint64_t count, uint32_t n, unsigned int* bad);
+// enqueue on s: *bad += the number of rows v < n with off[v] > off[v + 1]
+void check_monotone_async(cudaStream_t s, const uint32_t* off, uint32_t n, unsigned int* bad);
 // builds a graph from device edge arrays (graph.cu; behind gb_[di]graph_from_device_edges_u32)
 gb_status graph_from_device_arrays(int device, gb_graph_kind kind, const uint32_t* d_src, const uint32_t* d_dst,
                                    const float* d_w, uint64_t m, uint32_t n, gb_layout layout, cudaStream_t caller,

@@ -121,8 +121,7 @@ __global__ void k_dedup_flags(const uint64_t* __restrict__ keys, uint64_t count,
 }
 
 // expands CSR offsets into one row id per entry: one warp per row (coalesced stores, no searches)
-__global__ void k_expand_rows(const uint32_t* __restrict__ off, uint32_t n, uint64_t count,
-                              uint32_t* __restrict__ rows) {
+__global__ void k_expand_rows(const uint32_t* __restrict__ off, uint32_t n, uint32_t* __restrict__ rows) {
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
@@ -130,7 +129,6 @@ __global__ void k_expand_rows(const uint32_t* __restrict__ off, uint32_t n, uint
     const uint32_t b = off[v], e = off[v + 1];
     for (uint32_t i = b + lane; i < e; i += 32) rows[i] = v;
   }
-  (void)count;
 }
 
 __global__ void k_check_ids(const uint32_t* __restrict__ a, uint64_t count, uint32_t n,
@@ -180,8 +178,8 @@ __global__ void k_relabel_keys(const uint32_t* __restrict__ rows, const uint32_t
 }
 
 // ---- CSR build -----------------------------------------------------------------------------
-gb_status build_csr_device(cudaStream_t s, uint32_t n, uint32_t* d_rows, uint32_t* d_cols, float* d_w,
-                           uint64_t count, gb_layout layout, DevCsr* csr) {
+gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, const uint32_t* d_cols,
+                           const float* d_w, uint64_t count, gb_layout layout, DevCsr* csr) {
   GB_REQUIRE(count < 0xFFFFFFFFull, "CSR with %llu entries does not fit u32 offsets (csr.rs:124)",
              (unsigned long long)count);
   const uint32_t bits = bits_for(n);
@@ -303,13 +301,25 @@ gb_status build_csr_device(cudaStream_t s, uint32_t n, uint32_t* d_rows, uint32_
   return GB_OK;
 }
 
-gb_status new_graph(int device, gb_graph_kind kind, uint32_t n, gb_graph** out) {
+gb_status require_device(int device) {
   int count = 0;
-  if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0)
+  if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0) {
+    cudaGetLastError();
     return fail(GB_ERR_CUDA, "no CUDA device available: libgraph_b200 has no CPU fallback");
+  }
   GB_REQUIRE(device >= 0 && device < count, "device %d out of range (have %d)", device, count);
+  return GB_OK;
+}
+
+gb_status check_layout(gb_layout layout) {
+  GB_REQUIRE((int)layout >= 0 && (int)layout <= 2, "bad layout %d", (int)layout);
+  return GB_OK;
+}
+
+gb_status new_graph(int device, gb_graph_kind kind, uint32_t n, GraphPtr* out) {
+  GB_TRY(require_device(device));
   GB_CUDA(cudaSetDevice(device));
-  gb_graph* g = new (std::nothrow) gb_graph();
+  GraphPtr g(new (std::nothrow) gb_graph());
   if (!g) return fail(GB_ERR_OOM, "host allocation failed");
   g->device = device;
   g->kind = kind;
@@ -317,36 +327,8 @@ gb_status new_graph(int device, gb_graph_kind kind, uint32_t n, gb_graph** out) 
   cudaError_t e = cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking);
   if (e == cudaSuccess) e = cudaEventCreate(&g->ev_begin);
   if (e == cudaSuccess) e = cudaEventCreate(&g->ev_end);
-  if (e != cudaSuccess) {
-    delete g;
-    return fail(GB_ERR_CUDA, "stream/event creation failed: %s", cudaGetErrorString(e));
-  }
-  *out = g;
-  return GB_OK;
-}
-
-static gb_status upload_csr(cudaStream_t s, uint32_t n, const uint32_t* off, const uint32_t* tgt,
-                            const float* w, DevCsr* csr) {
-  uint64_t len = off[n];
-  csr->len = len;
-  GB_TRY(csr->off.alloc((size_t)n + 1));
-  GB_TRY(csr->tgt.alloc(len, 8));
-  GB_CUDA(cudaMemcpyAsync(csr->off.p, off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, s));
-  if (len) GB_CUDA(cudaMemcpyAsync(csr->tgt.p, tgt, len * 4, cudaMemcpyHostToDevice, s));
-  GB_CUDA(cudaMemsetAsync(csr->tgt.p + len, 0, 8 * 4, s));
-  if (w) {
-    GB_TRY(csr->w.alloc(len, 8));
-    if (len) GB_CUDA(cudaMemcpyAsync(csr->w.p, w, len * 4, cudaMemcpyHostToDevice, s));
-  }
-  return GB_OK;
-}
-
-// Host-side sanity of the offsets (O(n)); the O(m) target range check runs on the device after
-// the upload (k_check_ids) so that a billion-edge twin is not validated by one CPU thread.
-static gb_status validate_host_csr(uint32_t n, const uint32_t* off, const uint32_t* tgt, const char* what) {
-  GB_REQUIRE(off != nullptr, "%s offsets is NULL", what);
-  GB_REQUIRE(off[0] == 0, "%s offsets[0] must be 0", what);
-  GB_REQUIRE(off[n] == 0 || tgt != nullptr, "%s targets is NULL", what);
+  if (e != cudaSuccess) return fail(GB_ERR_CUDA, "stream/event creation failed: %s", cudaGetErrorString(e));
+  *out = std::move(g);
   return GB_OK;
 }
 
@@ -355,12 +337,39 @@ __global__ void k_check_monotone(const uint32_t* __restrict__ off, uint32_t n, u
     if (off[v] > off[v + 1]) atomicAdd(bad, 1u);
 }
 
-static gb_status validate_device_targets(cudaStream_t s, uint32_t n, const DevCsr& c, const char* what) {
-  DevBuf<unsigned int> bad;
+void check_ids_async(cudaStream_t s, const uint32_t* a, uint64_t count, uint32_t n, unsigned int* bad) {
+  if (count) k_check_ids<<<grid_for(count, 256), 256, 0, s>>>(a, count, n, bad);
+}
+
+void check_monotone_async(cudaStream_t s, const uint32_t* off, uint32_t n, unsigned int* bad) {
+  k_check_monotone<<<grid_for(n, 256), 256, 0, s>>>(off, n, bad);
+}
+
+// Only O(1) checks read the host arrays; the O(n + m) ones run on the device after the upload, so that a
+// billion-edge twin is not validated by one CPU thread.
+gb_status upload_host_csr(cudaStream_t s, uint32_t n, const uint32_t* off, const uint32_t* tgt, const float* w,
+                          DevCsr* csr, const char* what, bool offsets_only) {
+  GB_REQUIRE(off != nullptr, "%s offsets is NULL", what);
+  GB_REQUIRE(off[0] == 0, "%s offsets[0] must be 0", what);
+  const uint64_t len = off[n];
+  GB_REQUIRE(offsets_only || len == 0 || tgt != nullptr, "%s targets is NULL", what);
+  DevBuf<unsigned int> bad;  // [0] targets >= n, [1] rows whose offsets decrease
   GB_TRY(bad.alloc(2));
   GB_CUDA(cudaMemsetAsync(bad.p, 0, 8, s));
-  if (c.len) k_check_ids<<<grid_for(c.len, 256), 256, 0, s>>>(c.tgt.p, c.len, n, bad.p);
-  k_check_monotone<<<grid_for(n, 256), 256, 0, s>>>(c.off.p, n, bad.p + 1);
+  csr->len = len;
+  GB_TRY(csr->off.alloc((size_t)n + 1));
+  GB_CUDA(cudaMemcpyAsync(csr->off.p, off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, s));
+  check_monotone_async(s, csr->off.p, n, bad.p + 1);
+  if (!offsets_only) {
+    GB_TRY(csr->tgt.alloc(len, 8));
+    if (len) GB_CUDA(cudaMemcpyAsync(csr->tgt.p, tgt, len * 4, cudaMemcpyHostToDevice, s));
+    GB_CUDA(cudaMemsetAsync(csr->tgt.p + len, 0, 8 * 4, s));
+    if (w) {
+      GB_TRY(csr->w.alloc(len, 8));
+      if (len) GB_CUDA(cudaMemcpyAsync(csr->w.p, w, len * 4, cudaMemcpyHostToDevice, s));
+    }
+    check_ids_async(s, csr->tgt.p, len, n, bad.p);
+  }
   unsigned int nbad[2] = {0, 0};
   GB_CUDA(cudaMemcpyAsync(nbad, bad.p, 8, cudaMemcpyDeviceToHost, s));
   GB_CUDA(cudaStreamSynchronize(s));
@@ -369,25 +378,9 @@ static gb_status validate_device_targets(cudaStream_t s, uint32_t n, const DevCs
   return GB_OK;
 }
 
-gb_status upload_host_csr(cudaStream_t s, uint32_t n, const uint32_t* off, const uint32_t* tgt, const float* w,
-                          DevCsr* csr, const char* what) {
-  GB_TRY(validate_host_csr(n, off, tgt ? tgt : off, what));
-  if (tgt) {
-    GB_TRY(upload_csr(s, n, off, tgt, w, csr));
-    return validate_device_targets(s, n, *csr, what);
-  }
-  // offsets only (degrees): no target array on the device
-  csr->len = off[n];
-  GB_TRY(csr->off.alloc((size_t)n + 1));
-  GB_CUDA(cudaMemcpyAsync(csr->off.p, off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, s));
-  DevCsr none;
-  (void)none;
-  return GB_OK;
-}
-
-// builds a directed or undirected graph from DEVICE edge arrays
-static gb_status graph_from_device_edges(gb_graph* g, uint32_t* d_src, uint32_t* d_dst, float* d_w,
-                                         uint64_t m, gb_layout layout) {
+// builds a directed or undirected graph's CSRs from DEVICE edge arrays
+static gb_status build_graph_csrs(gb_graph* g, const uint32_t* d_src, const uint32_t* d_dst, const float* d_w,
+                                  uint64_t m, gb_layout layout) {
   cudaStream_t s = g->stream;
   if (g->kind == GB_KIND_DIRECTED) {
     GB_TRY(build_csr_device(s, g->n, d_src, d_dst, d_w, m, layout, &g->out));
@@ -408,58 +401,6 @@ static gb_status graph_from_device_edges(gb_graph* g, uint32_t* d_src, uint32_t*
   return GB_OK;
 }
 
-static gb_status graph_from_host_edges(int device, gb_graph_kind kind, const uint32_t* src,
-                                       const uint32_t* dst, const float* w, uint64_t m, uint32_t n,
-                                       gb_layout layout, gb_graph** out) {
-  GB_REQUIRE(out != nullptr, "graph out-pointer is NULL");
-  GB_REQUIRE(m == 0 || (src && dst), "edge arrays are NULL");
-  GB_REQUIRE((int)layout >= 0 && (int)layout <= 2, "bad layout %d", (int)layout);
-  uint64_t cap = (kind == GB_KIND_UNDIRECTED) ? 2 * m : m;
-  GB_REQUIRE(cap < 0xFFFFFFFFull, "edge count %llu does not fit u32 offsets", (unsigned long long)m);
-  if (n == 0) {  // Edges::max_node_id + 1, edgelist.rs:84-90
-    uint32_t mx = 0;
-    for (uint64_t i = 0; i < m; ++i) {
-      if (src[i] > mx) mx = src[i];
-      if (dst[i] > mx) mx = dst[i];
-    }
-    GB_REQUIRE(m > 0, "cannot infer node_count from an empty edge list");
-    GB_REQUIRE(mx < 0xFFFFFFFFu, "node id 2^32-1 leaves no room for node_count");
-    n = mx + 1;
-  }
-  gb_graph* g = nullptr;
-  GB_TRY(new_graph(device, kind, n, &g));
-  gb_status st = [&]() -> gb_status {
-    DevBuf<uint32_t> d_src, d_dst;
-    DevBuf<float> d_w;
-    DevBuf<unsigned int> bad;
-    GB_TRY(d_src.alloc(m));
-    GB_TRY(d_dst.alloc(m));
-    GB_TRY(bad.alloc(1));
-    GB_CUDA(cudaMemsetAsync(bad.p, 0, 4, g->stream));
-    if (m) {
-      GB_CUDA(cudaMemcpyAsync(d_src.p, src, m * 4, cudaMemcpyHostToDevice, g->stream));
-      GB_CUDA(cudaMemcpyAsync(d_dst.p, dst, m * 4, cudaMemcpyHostToDevice, g->stream));
-      k_check_ids<<<grid_for(m, 256), 256, 0, g->stream>>>(d_src.p, m, n, bad.p);
-      k_check_ids<<<grid_for(m, 256), 256, 0, g->stream>>>(d_dst.p, m, n, bad.p);
-    }
-    if (w && kind == GB_KIND_DIRECTED) {
-      GB_TRY(d_w.alloc(m));
-      if (m) GB_CUDA(cudaMemcpyAsync(d_w.p, w, m * 4, cudaMemcpyHostToDevice, g->stream));
-    }
-    unsigned int nbad = 0;
-    GB_CUDA(cudaMemcpyAsync(&nbad, bad.p, 4, cudaMemcpyDeviceToHost, g->stream));
-    GB_CUDA(cudaStreamSynchronize(g->stream));
-    GB_REQUIRE(nbad == 0, "%u edge endpoints are >= node_count %u", nbad, n);
-    return graph_from_device_edges(g, d_src.p, d_dst.p, d_w.p, m, layout);
-  }();
-  if (st != GB_OK) {
-    gb_graph_free(g);
-    return st;
-  }
-  *out = g;
-  return GB_OK;
-}
-
 __global__ void k_max_ids(const uint32_t* __restrict__ a, const uint32_t* __restrict__ b, uint64_t count,
                           unsigned int* __restrict__ mx) {
   uint32_t v = 0;
@@ -468,6 +409,67 @@ __global__ void k_max_ids(const uint32_t* __restrict__ a, const uint32_t* __rest
     v = max(v, max(a[i], b[i]));
   for (int o = 16; o; o >>= 1) v = max(v, __shfl_xor_sync(0xFFFFFFFFu, v, o));
   if ((threadIdx.x & 31) == 0) atomicMax(mx, v);
+}
+
+// the argument checks of the host and the device edge paths
+static gb_status check_edge_args(gb_graph_kind kind, const uint32_t* src, const uint32_t* dst, uint64_t m,
+                                 uint32_t n, gb_layout layout, gb_graph** out) {
+  GB_REQUIRE(out != nullptr, "graph out-pointer is NULL");
+  GB_REQUIRE(m == 0 || (src && dst), "edge arrays are NULL");
+  GB_TRY(check_layout(layout));
+  uint64_t cap = (kind == GB_KIND_UNDIRECTED) ? 2 * m : m;
+  GB_REQUIRE(cap < 0xFFFFFFFFull, "edge count %llu does not fit u32 offsets", (unsigned long long)m);
+  GB_REQUIRE(n != 0 || m > 0, "cannot infer node_count from an empty edge list");
+  return GB_OK;
+}
+
+// Checks device edge arrays on g's stream, then builds g's CSRs from them.  g->n == 0 is inferred as the
+// largest id + 1 (Edges::max_node_id + 1, edgelist.rs:84-90); otherwise every id must be below g->n.
+static gb_status build_from_edges(gb_graph* g, const uint32_t* d_src, const uint32_t* d_dst, const float* d_w,
+                                  uint64_t m, gb_layout layout) {
+  cudaStream_t s = g->stream;
+  const bool infer = g->n == 0;
+  DevBuf<unsigned int> scratch;
+  GB_TRY(scratch.alloc(1));
+  GB_CUDA(cudaMemsetAsync(scratch.p, 0, 4, s));
+  if (infer) {
+    k_max_ids<<<grid_for(m, 256), 256, 0, s>>>(d_src, d_dst, m, scratch.p);
+  } else {
+    check_ids_async(s, d_src, m, g->n, scratch.p);
+    check_ids_async(s, d_dst, m, g->n, scratch.p);
+  }
+  unsigned int h = 0;
+  GB_CUDA(cudaMemcpyAsync(&h, scratch.p, 4, cudaMemcpyDeviceToHost, s));
+  GB_CUDA(cudaStreamSynchronize(s));
+  GB_CUDA(cudaGetLastError());
+  if (infer) {
+    GB_REQUIRE(h < 0xFFFFFFFFu, "node id 2^32-1 leaves no room for node_count");
+    g->n = h + 1;
+  } else {
+    GB_REQUIRE(h == 0, "%u edge endpoints are >= node_count %u", h, g->n);
+  }
+  return build_graph_csrs(g, d_src, d_dst, d_w, m, layout);
+}
+
+static gb_status graph_from_host_edges(int device, gb_graph_kind kind, const uint32_t* src,
+                                       const uint32_t* dst, const float* w, uint64_t m, uint32_t n,
+                                       gb_layout layout, gb_graph** out) {
+  GB_TRY(check_edge_args(kind, src, dst, m, n, layout, out));
+  GraphPtr g;
+  GB_TRY(new_graph(device, kind, n, &g));
+  DevBuf<uint32_t> d_src, d_dst;
+  DevBuf<float> d_w;
+  GB_TRY(d_src.alloc(m));
+  GB_TRY(d_dst.alloc(m));
+  if (w) GB_TRY(d_w.alloc(m));
+  if (m) {
+    GB_CUDA(cudaMemcpyAsync(d_src.p, src, m * 4, cudaMemcpyHostToDevice, g->stream));
+    GB_CUDA(cudaMemcpyAsync(d_dst.p, dst, m * 4, cudaMemcpyHostToDevice, g->stream));
+    if (w) GB_CUDA(cudaMemcpyAsync(d_w.p, w, m * 4, cudaMemcpyHostToDevice, g->stream));
+  }
+  GB_TRY(build_from_edges(g.get(), d_src.p, d_dst.p, d_w.p, m, layout));
+  *out = g.release();
+  return GB_OK;
 }
 
 static gb_status require_device_array(const void* p, int device, const char* what) {
@@ -484,56 +486,23 @@ static gb_status require_device_array(const void* p, int device, const char* wha
 gb_status graph_from_device_arrays(int device, gb_graph_kind kind, const uint32_t* d_src, const uint32_t* d_dst,
                                    const float* d_w, uint64_t m, uint32_t n, gb_layout layout, cudaStream_t caller,
                                    gb_graph** out) {
-  GB_REQUIRE(out != nullptr, "graph out-pointer is NULL");
-  GB_REQUIRE(m == 0 || (d_src && d_dst), "edge arrays are NULL");
-  GB_REQUIRE((int)layout >= 0 && (int)layout <= 2, "bad layout %d", (int)layout);
-  uint64_t cap = (kind == GB_KIND_UNDIRECTED) ? 2 * m : m;
-  GB_REQUIRE(cap < 0xFFFFFFFFull, "edge count %llu does not fit u32 offsets", (unsigned long long)m);
-  GB_REQUIRE(n != 0 || m > 0, "cannot infer node_count from an empty edge list");
-  gb_graph* g = nullptr;
+  GB_TRY(check_edge_args(kind, d_src, d_dst, m, n, layout, out));
+  GraphPtr g;
   GB_TRY(new_graph(device, kind, n, &g));
-  gb_status st = [&]() -> gb_status {
-    if (m) {
-      GB_TRY(require_device_array(d_src, device, "d_src"));
-      GB_TRY(require_device_array(d_dst, device, "d_dst"));
-      if (d_w && kind == GB_KIND_DIRECTED) GB_TRY(require_device_array(d_w, device, "d_weights"));
-    }
-    // the caller's producer work comes first
-    cudaEvent_t ready;
-    GB_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
-    cudaError_t e = cudaEventRecord(ready, caller);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(g->stream, ready, 0);
-    cudaEventDestroy(ready);
-    GB_CUDA(e);
-    DevBuf<unsigned int> scratch;
-    GB_TRY(scratch.alloc(1));
-    GB_CUDA(cudaMemsetAsync(scratch.p, 0, 4, g->stream));
-    unsigned int h = 0;
-    if (n == 0) {  // Edges::max_node_id + 1, edgelist.rs:84-90
-      k_max_ids<<<grid_for(m, 256), 256, 0, g->stream>>>(d_src, d_dst, m, scratch.p);
-      GB_CUDA(cudaMemcpyAsync(&h, scratch.p, 4, cudaMemcpyDeviceToHost, g->stream));
-      GB_CUDA(cudaStreamSynchronize(g->stream));
-      GB_REQUIRE(h < 0xFFFFFFFFu, "node id 2^32-1 leaves no room for node_count");
-      g->n = h + 1;
-    } else {
-      if (m) {
-        k_check_ids<<<grid_for(m, 256), 256, 0, g->stream>>>(d_src, m, n, scratch.p);
-        k_check_ids<<<grid_for(m, 256), 256, 0, g->stream>>>(d_dst, m, n, scratch.p);
-      }
-      GB_CUDA(cudaMemcpyAsync(&h, scratch.p, 4, cudaMemcpyDeviceToHost, g->stream));
-      GB_CUDA(cudaStreamSynchronize(g->stream));
-      GB_REQUIRE(h == 0, "%u edge endpoints are >= node_count %u", h, n);
-    }
-    GB_CUDA(cudaGetLastError());
-    // build_csr_device only reads the edge arrays
-    return graph_from_device_edges(g, const_cast<uint32_t*>(d_src), const_cast<uint32_t*>(d_dst),
-                                   kind == GB_KIND_DIRECTED ? const_cast<float*>(d_w) : nullptr, m, layout);
-  }();
-  if (st != GB_OK) {
-    gb_graph_free(g);
-    return st;
+  if (m) {
+    GB_TRY(require_device_array(d_src, device, "d_src"));
+    GB_TRY(require_device_array(d_dst, device, "d_dst"));
+    if (d_w) GB_TRY(require_device_array(d_w, device, "d_weights"));
   }
-  *out = g;
+  // the caller's producer work comes first
+  cudaEvent_t ready;
+  GB_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
+  cudaError_t e = cudaEventRecord(ready, caller);
+  if (e == cudaSuccess) e = cudaStreamWaitEvent(g->stream, ready, 0);
+  cudaEventDestroy(ready);
+  GB_CUDA(e);
+  GB_TRY(build_from_edges(g.get(), d_src, d_dst, d_w, m, layout));
+  *out = g.release();
   return GB_OK;
 }
 
@@ -558,26 +527,20 @@ static gb_status rmat_graph(int device, gb_graph_kind kind, uint32_t scale, uint
   uint64_t m = (uint64_t)edge_factor << scale;
   uint64_t cap = (kind == GB_KIND_UNDIRECTED) ? 2 * m : m;
   GB_REQUIRE(cap < 0xFFFFFFFFull, "2^%u * %u edges do not fit u32 offsets", scale, edge_factor);
-  gb_graph* g = nullptr;
+  GraphPtr g;
   GB_TRY(new_graph(device, kind, 1u << scale, &g));
-  gb_status st = [&]() -> gb_status {
-    DevBuf<uint32_t> d_src, d_dst;
-    DevBuf<float> d_w;
-    GB_TRY(d_src.alloc(m));
-    GB_TRY(d_dst.alloc(m));
-    k_rmat<<<grid_for(m, 256), 256, 0, g->stream>>>(scale, seed, 0, m, d_src.p, d_dst.p);
-    if (weights && kind == GB_KIND_DIRECTED) {
-      GB_TRY(d_w.alloc(m));
-      k_rmat_weights<<<grid_for(m, 256), 256, 0, g->stream>>>(seed, m, d_w.p);
-    }
-    GB_CUDA(cudaGetLastError());
-    return graph_from_device_edges(g, d_src.p, d_dst.p, d_w.p, m, layout);
-  }();
-  if (st != GB_OK) {
-    gb_graph_free(g);
-    return st;
+  DevBuf<uint32_t> d_src, d_dst;
+  DevBuf<float> d_w;
+  GB_TRY(d_src.alloc(m));
+  GB_TRY(d_dst.alloc(m));
+  k_rmat<<<grid_for(m, 256), 256, 0, g->stream>>>(scale, seed, 0, m, d_src.p, d_dst.p);
+  if (weights && kind == GB_KIND_DIRECTED) {
+    GB_TRY(d_w.alloc(m));
+    k_rmat_weights<<<grid_for(m, 256), 256, 0, g->stream>>>(seed, m, d_w.p);
   }
-  *out = g;
+  GB_CUDA(cudaGetLastError());
+  GB_TRY(build_graph_csrs(g.get(), d_src.p, d_dst.p, d_w.p, m, layout));
+  *out = g.release();
   return GB_OK;
 }
 
@@ -605,22 +568,12 @@ gb_status gb_digraph_from_csr_u32(int device, uint32_t n, const uint32_t* out_of
                                   const uint32_t* in_tgt, gb_graph** graph) {
   GB_REQUIRE(graph != nullptr, "graph out-pointer is NULL");
   GB_REQUIRE(n > 0, "node_count must be > 0");
-  GB_TRY(validate_host_csr(n, out_off, out_tgt, "out"));
-  GB_TRY(validate_host_csr(n, in_off, in_tgt, "in"));
-  GB_REQUIRE(out_off[n] == in_off[n], "out and in CSR disagree on the edge count");
-  gb_graph* g = nullptr;
+  GraphPtr g;
   GB_TRY(new_graph(device, GB_KIND_DIRECTED, n, &g));
-  gb_status st = upload_csr(g->stream, n, out_off, out_tgt, out_w, &g->out);
-  if (st == GB_OK) st = upload_csr(g->stream, n, in_off, in_tgt, nullptr, &g->in);
-  if (st == GB_OK) st = validate_device_targets(g->stream, n, g->out, "out");
-  if (st == GB_OK) st = validate_device_targets(g->stream, n, g->in, "in");
-  if (st == GB_OK && cudaStreamSynchronize(g->stream) != cudaSuccess)
-    st = fail(GB_ERR_CUDA, "upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-  if (st != GB_OK) {
-    gb_graph_free(g);
-    return st;
-  }
-  *graph = g;
+  GB_TRY(upload_host_csr(g->stream, n, out_off, out_tgt, out_w, &g->out, "out"));
+  GB_TRY(upload_host_csr(g->stream, n, in_off, in_tgt, nullptr, &g->in, "in"));
+  GB_REQUIRE(g->out.len == g->in.len, "out and in CSR disagree on the edge count");
+  *graph = g.release();
   return GB_OK;
 }
 
@@ -628,18 +581,10 @@ gb_status gb_graph_from_csr_u32(int device, uint32_t n, const uint32_t* off, con
                                 gb_graph** graph) {
   GB_REQUIRE(graph != nullptr, "graph out-pointer is NULL");
   GB_REQUIRE(n > 0, "node_count must be > 0");
-  GB_TRY(validate_host_csr(n, off, tgt, "undirected"));
-  gb_graph* g = nullptr;
+  GraphPtr g;
   GB_TRY(new_graph(device, GB_KIND_UNDIRECTED, n, &g));
-  gb_status st = upload_csr(g->stream, n, off, tgt, nullptr, &g->out);
-  if (st == GB_OK) st = validate_device_targets(g->stream, n, g->out, "undirected");
-  if (st == GB_OK && cudaStreamSynchronize(g->stream) != cudaSuccess)
-    st = fail(GB_ERR_CUDA, "upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-  if (st != GB_OK) {
-    gb_graph_free(g);
-    return st;
-  }
-  *graph = g;
+  GB_TRY(upload_host_csr(g->stream, n, off, tgt, nullptr, &g->out, "undirected"));
+  *graph = g.release();
   return GB_OK;
 }
 
@@ -672,9 +617,7 @@ gb_status gb_ids_to_u32(int device, const void* d_ids, int id_bytes, uint64_t co
   GB_REQUIRE(id_bytes == 4 || id_bytes == 8, "ids must be 4 or 8 bytes wide, not %d", id_bytes);
   if (count == 0) return GB_OK;
   GB_REQUIRE(d_ids && d_out, "NULL argument");
-  int devs = gb_device_count();
-  if (devs <= 0) return fail(GB_ERR_CUDA, "no CUDA device available: libgraph_b200 has no CPU fallback");
-  GB_REQUIRE(device >= 0 && device < devs, "device %d out of range", device);
+  GB_TRY(require_device(device));
   DeviceGuard guard(device);
   GB_TRY(require_device_array(d_ids, device, "ids"));
   GB_TRY(require_device_array(d_out, device, "output ids"));
@@ -707,9 +650,7 @@ gb_status gb_rmat_edges(int device, uint32_t scale, uint64_t seed, uint64_t firs
                         uint32_t* src, uint32_t* dst) {
   GB_REQUIRE(scale >= 1 && scale <= 31, "scale %u out of range [1,31]", scale);
   GB_REQUIRE(count == 0 || (src && dst), "output arrays are NULL");
-  int devs = gb_device_count();
-  if (devs <= 0) return fail(GB_ERR_CUDA, "no CUDA device available: libgraph_b200 has no CPU fallback");
-  GB_REQUIRE(device >= 0 && device < devs, "device %d out of range", device);
+  GB_TRY(require_device(device));
   DeviceGuard guard(device);
   DevBuf<uint32_t> d_src, d_dst;
   GB_TRY(d_src.alloc(count));
@@ -799,26 +740,20 @@ gb_status gb_graph_last_timing(const gb_graph* g, gb_timing* t) {
 gb_status gb_to_undirected(const gb_graph* dg, gb_layout layout, gb_graph** graph) {
   GB_REQUIRE(dg && graph, "NULL argument");
   if (dg->kind != GB_KIND_DIRECTED) return fail(GB_ERR_UNSUPPORTED, "to_undirected needs a directed graph");
-  GB_REQUIRE((int)layout >= 0 && (int)layout <= 2, "bad layout %d", (int)layout);
+  GB_TRY(check_layout(layout));
   uint64_t m = dg->out.len;
   GB_REQUIRE(m == 0 || dg->out.tgt.p != nullptr, "this handle holds no out targets (page-rank-only twin)");
   GB_REQUIRE(2 * m < 0xFFFFFFFFull, "undirected twin would exceed u32 offsets");
   DeviceGuard guard(dg->device);
-  gb_graph* g = nullptr;
+  GraphPtr g;
   GB_TRY(new_graph(dg->device, GB_KIND_UNDIRECTED, dg->n, &g));
-  gb_status st = [&]() -> gb_status {
-    std::lock_guard<std::mutex> lock(dg->mu);
-    DevBuf<uint32_t> rows;
-    GB_TRY(rows.alloc(m));
-    if (m) k_expand_rows<<<grid_for((uint64_t)dg->n * 32, 256), 256, 0, g->stream>>>(dg->out.off.p, dg->n, m, rows.p);
-    GB_CUDA(cudaGetLastError());
-    return graph_from_device_edges(g, rows.p, dg->out.tgt.p, nullptr, m, layout);
-  }();
-  if (st != GB_OK) {
-    gb_graph_free(g);
-    return st;
-  }
-  *graph = g;
+  std::lock_guard<std::mutex> lock(dg->mu);
+  DevBuf<uint32_t> rows;
+  GB_TRY(rows.alloc(m));
+  if (m) k_expand_rows<<<grid_for((uint64_t)dg->n * 32, 256), 256, 0, g->stream>>>(dg->out.off.p, dg->n, rows.p);
+  GB_CUDA(cudaGetLastError());
+  GB_TRY(build_graph_csrs(g.get(), rows.p, dg->out.tgt.p, nullptr, m, layout));
+  *graph = g.release();
   return GB_OK;
 }
 
@@ -855,7 +790,7 @@ gb_status gb_make_degree_ordered(gb_graph* g) {
   GB_CUDA(cudaMemsetAsync(fresh.tgt.p + len, 0, 8 * 4, s));
   if (len) {
     GB_TRY(rows.alloc(len));
-    k_expand_rows<<<grid_for((uint64_t)n * 32, 256), 256, 0, s>>>(g->out.off.p, n, len, rows.p);
+    k_expand_rows<<<grid_for((uint64_t)n * 32, 256), 256, 0, s>>>(g->out.off.p, n, rows.p);
     DevBuf<uint64_t> keys, keys_alt;
     GB_TRY(keys.alloc(len));
     GB_TRY(keys_alt.alloc(len));

@@ -557,10 +557,7 @@ static gb_status load_file(int device, const char* path, gb_file_format format, 
 // Below these sizes the fixed costs of the pipeline (threads, streams, pinned ring) exceed what it saves, and
 // the host readers are faster (H100 80GB HBM3, 400 W; tools/bench_load.py).  GB_LOAD_CHUNK_BYTES, when
 // set, selects the device path whatever the size.
-static uint64_t load_device_min_bytes(gb_file_format format) {
-  (void)format;
-  return 64ull << 20;
-}
+constexpr uint64_t LOAD_DEVICE_MIN_BYTES = 64ull << 20;
 
 // the host readers of io.cu and the upload of gb_[di]graph_from_edges_u32
 static gb_status load_on_host(int device, gb_graph_kind kind, const char* path, gb_file_format format,
@@ -606,29 +603,21 @@ static gb_status load_graph(int device, gb_graph_kind kind, const char* path, gb
   GB_REQUIRE(path != nullptr, "path is NULL");
   GB_REQUIRE(format == GB_FORMAT_GRAPH500 || format == GB_FORMAT_EDGE_LIST, "unknown file format %d", (int)format);
   GB_REQUIRE(!with_values || format == GB_FORMAT_EDGE_LIST, "only edge lists carry edge values");
-  GB_REQUIRE((int)layout >= 0 && (int)layout <= 2, "bad layout %d", (int)layout);
-  int count = 0;
-  if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0) {
-    cudaGetLastError();
-    return fail(GB_ERR_CUDA, "no CUDA device available: libgraph_b200 has no CPU fallback");
-  }
-  GB_REQUIRE(device >= 0 && device < count, "device %d out of range (have %d)", device, count);
+  GB_TRY(check_layout(layout));
+  GB_TRY(require_device(device));
   DeviceGuard guard(device);
   struct stat st {};
   if (::stat(path, &st) != 0) return fail(GB_ERR_INVALID, "cannot open %s: %s", path, std::strerror(errno));
   gb_load_info info{};
-  if (env_chunk_bytes() == 0 && (uint64_t)st.st_size < load_device_min_bytes(format)) {
+  if (env_chunk_bytes() == 0 && (uint64_t)st.st_size < LOAD_DEVICE_MIN_BYTES) {
     GB_TRY(load_on_host(device, kind, path, format, layout, with_values != 0, graph, &info));
-    (*graph)->load = info;
-    return GB_OK;
+  } else {
+    LoadedEdges e;
+    GB_TRY(load_file(device, path, format, with_values != 0, &e, &info));
+    GB_TRY(graph_from_device_arrays(device, kind, e.src.p, e.dst.p, with_values ? e.w.p : nullptr, e.m, e.n, layout,
+                                    nullptr, graph));
   }
-  LoadedEdges e;
-  GB_TRY(load_file(device, path, format, with_values != 0, &e, &info));
-  gb_graph* g = nullptr;
-  GB_TRY(graph_from_device_arrays(device, kind, e.src.p, e.dst.p, with_values ? e.w.p : nullptr, e.m, e.n, layout,
-                                  nullptr, &g));
-  g->load = info;
-  *graph = g;
+  (*graph)->load = info;
   return GB_OK;
 }
 

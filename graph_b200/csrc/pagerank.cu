@@ -304,7 +304,7 @@ __device__ __forceinline__ uint32_t cb_classify_row(uint32_t l, uint32_t b0, uin
       src[u] = 0;
       if (valid[u]) {
         uint32_t t = in_tgt[b0 + k];
-        if (CHECK && t >= n) t = 0;  // reported by k_feed_check; keep the lookups in range meanwhile
+        if (CHECK && t >= n) t = 0;  // reported by the chunk's id check; keep the lookups in range meanwhile
         src[u] = new_id[t];
       }
     }
@@ -400,18 +400,6 @@ __global__ void k_cb_count_rows(const uint32_t* __restrict__ in_off, const uint3
     }
   }
   if (lane == 0 && in_cb) atomicAdd(cb_edges, in_cb);
-}
-// range check of a chunk of targets and of the offsets of its rows (what validate_device_targets does
-// for a resident CSR)
-__global__ void k_feed_check(const uint32_t* __restrict__ tgt, uint64_t count, uint32_t n, unsigned int* __restrict__ bad) {
-  unsigned int mine = 0;
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count; i += (uint64_t)gridDim.x * blockDim.x)
-    mine += tgt[i] >= n;
-  if (mine) atomicAdd(bad, mine);
-}
-__global__ void k_feed_monotone(const uint32_t* __restrict__ off, uint32_t n, unsigned int* __restrict__ bad) {
-  for (uint32_t v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += gridDim.x * blockDim.x)
-    if (off[v] > off[v + 1]) atomicAdd(bad, 1u);
 }
 // ---- the longest rows (a prefix of the local rows) go through ONE stable radix sort -----------------
 // A row's warp walks it 128 edges at a time, ~3 us per step: a million-edge hub would take tens of
@@ -1569,7 +1557,7 @@ static gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan
         const uint32_t v0 = feed->row_begin[k], v1 = feed->row_begin[k + 1];
         const uint64_t e0 = feed->edge_begin[k], e1 = feed->edge_begin[k + 1];
         GB_CUDA(cudaStreamWaitEvent(s, feed->ready[k], 0));
-        if (e1 > e0) k_feed_check<<<grid_for(e1 - e0, 256), 256, 0, s>>>(g->in.tgt.p + e0, e1 - e0, n, bad.p);
+        check_ids_async(s, g->in.tgt.p + e0, e1 - e0, n, bad.p);
         if (p->n_cb > n_mega && v1 > v0)
           k_cb_count_rows<<<grid_for((uint64_t)(v1 - v0), 256), 256, 0, s>>>(
               g->in.off.p, g->in.tgt.p, p->new_id.p, hot_of_blk.p, p->nrows.p, p->poff.p, p->blk.p, B, v0, v1, n, n_mega,
@@ -2311,14 +2299,12 @@ gb_status gb_page_rank_csr_u32(int device, uint32_t n, const uint32_t* in_off, c
   if (m < gb::env_u32("GB_PR_FEED_MIN_EDGES", 1u << 22)) chunks = 0;
   // the single-warp EXACT mode (small graphs) reads the CSR directly: nothing to overlap
   if (!config || config->mode == GB_PR_EXACT || (config->mode == GB_PR_AUTO && n <= 16384)) chunks = 0;
-  gb_graph* g = nullptr;
+  gb::GraphPtr g;
   GB_TRY(gb::new_graph(device, GB_KIND_DIRECTED, n, &g));
   if (chunks == 0) {
-    gb_status st = gb::upload_host_csr(g->stream, n, in_off, in_tgt, nullptr, &g->in, "in");
-    if (st == GB_OK) st = gb::upload_host_csr(g->stream, n, out_off, nullptr, nullptr, &g->out, "out");
-    if (st == GB_OK) st = gb::page_rank_impl(g, config, nullptr, scores, ran_iterations, error);
-    gb_graph_free(g);
-    return st;
+    GB_TRY(gb::upload_host_csr(g->stream, n, in_off, in_tgt, nullptr, &g->in, "in"));
+    GB_TRY(gb::upload_host_csr(g->stream, n, out_off, nullptr, nullptr, &g->out, "out", true));
+    return gb::page_rank_impl(g.get(), config, nullptr, scores, ran_iterations, error);
   }
   gb::TargetFeed feed;
   cudaStream_t copy = nullptr;
@@ -2368,8 +2354,8 @@ gb_status gb_page_rank_csr_u32(int device, uint32_t n, const uint32_t* in_off, c
     gb::DevBuf<unsigned int> bad;
     GB_TRY(bad.alloc(2));
     GB_CUDA(cudaMemsetAsync(bad.p, 0, 8, g->stream));
-    gb::k_feed_monotone<<<gb::grid_for(n, 256), 256, 0, g->stream>>>(g->in.off.p, n, bad.p);
-    gb::k_feed_monotone<<<gb::grid_for(n, 256), 256, 0, g->stream>>>(g->out.off.p, n, bad.p + 1);
+    gb::check_monotone_async(g->stream, g->in.off.p, n, bad.p);
+    gb::check_monotone_async(g->stream, g->out.off.p, n, bad.p + 1);
     unsigned int nbad[2] = {0, 0};
     GB_CUDA(cudaMemcpyAsync(nbad, bad.p, 8, cudaMemcpyDeviceToHost, g->stream));
     GB_CUDA(cudaStreamSynchronize(g->stream));
@@ -2380,13 +2366,11 @@ gb_status gb_page_rank_csr_u32(int device, uint32_t n, const uint32_t* in_off, c
     GB_REQUIRE(nbad[0] == 0, "in offsets are not monotone (%u rows)", nbad[0]);
     GB_REQUIRE(nbad[1] == 0, "out offsets are not monotone (%u rows)", nbad[1]);
     g->feed = &feed;
-    gb_status r = gb::page_rank_impl(g, config, nullptr, scores, ran_iterations, error);
-    g->feed = nullptr;
-    return r;
+    return gb::page_rank_impl(g.get(), config, nullptr, scores, ran_iterations, error);
   }();
   g->feed = nullptr;
   if (copy) cudaStreamSynchronize(copy);  // an early error must not free buffers under a running copy
-  gb_graph_free(g);
+  g.reset();
   for (cudaEvent_t ev : feed.ready) cudaEventDestroy(ev);
   if (offsets_in) cudaEventDestroy(offsets_in);
   if (copy) cudaStreamDestroy(copy);
@@ -2399,15 +2383,11 @@ gb_status gb_digraph_for_page_rank_u32(int device, uint32_t n, const uint32_t* i
   GB_REQUIRE(n > 0, "node_count must be > 0");
   GB_REQUIRE(in_off && out_off, "offset arrays are NULL");
   GB_REQUIRE(in_off[n] == out_off[n], "in and out offsets disagree on the edge count");
-  gb_graph* g = nullptr;
+  gb::GraphPtr g;
   GB_TRY(gb::new_graph(device, GB_KIND_DIRECTED, n, &g));
-  gb_status st = gb::upload_host_csr(g->stream, n, in_off, in_tgt, nullptr, &g->in, "in");
-  if (st == GB_OK) st = gb::upload_host_csr(g->stream, n, out_off, nullptr, nullptr, &g->out, "out");
-  if (st != GB_OK) {
-    gb_graph_free(g);
-    return st;
-  }
-  *graph = g;
+  GB_TRY(gb::upload_host_csr(g->stream, n, in_off, in_tgt, nullptr, &g->in, "in"));
+  GB_TRY(gb::upload_host_csr(g->stream, n, out_off, nullptr, nullptr, &g->out, "out", true));
+  *graph = g.release();
   return GB_OK;
 }
 

@@ -50,6 +50,24 @@ def test_no_cpu_fallback_without_gpu():
         gb.Graph.rmat(4)
 
 
+def test_every_constructor_reports_the_missing_device(golden_dir):
+    """Valid input to each constructor that needs no device to be called fails on the device check."""
+    import torch
+    if torch.cuda.is_available():
+        pytest.skip("this box has a GPU")
+    import graph_b200 as gb
+    off = np.array([0, 1, 2], np.uint32)
+    tgt = np.array([1, 0], np.uint32)
+    for make in (lambda: gb.DiGraph.from_numpy(np.array([[0, 1], [1, 0]], np.uint32)),
+                 lambda: gb.DiGraph.from_csr(off, tgt, off, tgt),
+                 lambda: gb.DiGraph.for_page_rank(off, tgt, off),
+                 lambda: gb.DiGraph.rmat(4),
+                 lambda: gb.DiGraph.load(golden_dir / "scale_8.graph500"),
+                 lambda: gb.Graph.from_csr(off, tgt)):
+        with pytest.raises(gb.GraphB200Error, match="no CUDA device"):
+            make()
+
+
 def test_product_never_imports_the_oracle():
     for path in (ROOT / "graph_b200").rglob("*.py"):
         src = path.read_text()
