@@ -49,12 +49,14 @@ __device__ __forceinline__ uint32_t sssp_reserve(uint32_t* counter) {
 }
 
 // A vertex whose distance improves several times in one pass (or several times while it waits in the far
-// pile) is queued once: near_stamp[t] holds the last pass, far_stamp[t] the last bucket epoch, in which t
-// was appended.  This bounds the near queue by n and the far pile by 2n whatever delta is.
+// pile) is queued once: near_stamp[t] holds the last pass in which t was appended to the near queue, and
+// in_pile[t] is 1 while t has an entry in the far pile (set by the append here, cleared by k_sssp_split_far
+// when the entry leaves the pile).  The pile never holds a vertex twice, however many buckets pass while t
+// waits in it, and every queue is bounded by n whatever delta is.
 struct SsspStamps {
   uint32_t* near_stamp;
-  uint32_t* far_stamp;
-  uint32_t pass, epoch;
+  uint32_t* in_pile;
+  uint32_t pass;
 };
 __device__ __forceinline__ void sssp_relax_edge(const uint32_t* __restrict__ tgt, const float* __restrict__ w,
                                                 uint32_t* dist, uint32_t i, float du, float upper,
@@ -71,7 +73,7 @@ __device__ __forceinline__ void sssp_relax_edge(const uint32_t* __restrict__ tgt
         if (pos < cap) near_out[pos] = t;
       }
     } else {
-      if (atomicMax(st.far_stamp + t, st.epoch) < st.epoch) {
+      if (atomicExch(st.in_pile + t, 1u) == 0u) {
         const uint32_t pos = sssp_reserve(counts + 1);
         if (pos < cap) far[pos] = t;
       }
@@ -116,13 +118,17 @@ __global__ void k_sssp_relax(const uint32_t* __restrict__ off, const uint32_t* _
 }
 
 // splits the far pile at the new bucket bound; entries whose distance dropped below `lower` were
-// settled already and are discarded
+// settled already and are discarded.  An entry that leaves the pile clears in_pile; one that stays keeps it,
+// so k_sssp_relax does not append the vertex a second time while it waits (a vertex improved in k buckets
+// while it stayed far used to have k entries).  Carried entries cost no write.
 __global__ void k_sssp_split_far(const uint32_t* __restrict__ dist, const uint32_t* __restrict__ far_in,
                                  uint32_t count, float lower, float upper, uint32_t* __restrict__ near_out,
-                                 uint32_t* __restrict__ far_out, uint32_t* counts, uint32_t cap) {
+                                 uint32_t* __restrict__ far_out, uint32_t* counts, uint32_t cap,
+                                 uint32_t* __restrict__ in_pile) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) {
     const uint32_t t = far_in[i];
     const float d = __uint_as_float(dist[t]);
+    if (d < upper) in_pile[t] = 0u;
     if (d < lower) continue;
     if (d < upper) {
       uint32_t pos = sssp_reserve(counts + 0);
@@ -164,18 +170,17 @@ static gb_status sssp_impl(const gb_graph* g, const gb_sssp_config* cfg, float* 
     d_dist = tmp.p;
   }
   uint32_t* dist = reinterpret_cast<uint32_t*>(d_dist);
-  // a vertex is appended at most once per pass to the near queue and once per bucket epoch to the far pile
-  // (stamps), and the pile carried over a bucket change holds each vertex at most once more: 2n bounds
-  // every queue for every delta (the overflow check below is an internal-error guard only)
+  // a vertex is appended at most once per pass to the near queue (near stamps), and the far pile holds it
+  // at most once (in_pile): n bounds every queue for every delta (the overflow check below is an
+  // internal-error guard only)
   (void)m;
-  const uint64_t cap64 = std::min<uint64_t>(2ull * n + 1024, 0xFFFFFFF0ull);
-  const uint32_t cap = (uint32_t)cap64;
-  DevBuf<uint32_t> qa, qb, fa, fb, counts, minb, near_stamp, far_stamp;
+  const uint32_t cap = n;
+  DevBuf<uint32_t> qa, qb, fa, fb, counts, minb, near_stamp, in_pile;
   GB_TRY(near_stamp.alloc(n));
-  GB_TRY(far_stamp.alloc(n));
+  GB_TRY(in_pile.alloc(n));
   GB_CUDA(cudaMemsetAsync(near_stamp.p, 0, (size_t)n * 4, s));
-  GB_CUDA(cudaMemsetAsync(far_stamp.p, 0, (size_t)n * 4, s));
-  SsspStamps st{near_stamp.p, far_stamp.p, 0u, 1u};
+  GB_CUDA(cudaMemsetAsync(in_pile.p, 0, (size_t)n * 4, s));
+  SsspStamps st{near_stamp.p, in_pile.p, 0u};
   GB_TRY(qa.alloc(cap));
   GB_TRY(qb.alloc(cap));
   GB_TRY(fa.alloc(cap));
@@ -230,12 +235,11 @@ static gb_status sssp_impl(const gb_graph* g, const gb_sssp_config* cfg, float* 
     const SsspBucket next = sssp_next_bucket(dmin, delta, upper);
     lower = next.lower;
     upper = next.upper;
-    st.epoch += 1;  // entries appended to the pile from now on are tracked under the new epoch
     const uint32_t zero3[3] = {0u, 0u, 0u};
     GB_CUDA(cudaMemcpyAsync(counts.p, zero3, 12, cudaMemcpyHostToDevice, s));
     // anything below lower in the pile was settled (its distance was final when its bucket drained)
     k_sssp_split_far<<<grid_for(far_count, blk), blk, 0, s>>>(dist, far, far_count, 0.0f, upper, near_in, far_out,
-                                                             counts.p, cap);
+                                                             counts.p, cap, st.in_pile);
     g->timing.kernel_launches += 1;
     GB_CUDA(cudaMemcpyAsync(h_counts, counts.p, 12, cudaMemcpyDeviceToHost, s));
     GB_CUDA(cudaStreamSynchronize(s));
