@@ -56,6 +56,7 @@ constexpr uint32_t CB_BLOCK_MAX = 56 * 1024;
 constexpr double CB_TAU_DEFAULT = 1.5;       // a (row, block) pair gets a segment if it expects >= tau edges
 constexpr uint32_t CB_MAX_BLOCKS = 8192;     // hot blocks kept (the staircase rarely needs more than ~1000)
 constexpr uint32_t CB_TASK_CHUNKS = 32;      // chunks per task (one per warp)
+constexpr uint32_t CB_WIDE_MIN = 128;        // chunks of at least this many groups take k_pr_cb's 128-group step
 constexpr uint32_t SELL_FEW = 4;             // rows with segments in at most this many blocks are finished by k_pr_sell itself
 constexpr uint32_t FIN_CTA_BLOCKS = 64;      // finish: 32-row groups with segments in more blocks get a CTA each
 constexpr uint32_t CB_NONE = 0xFFFFFFFFu;
@@ -104,7 +105,7 @@ struct PrPlan {
   DevBuf<uint32_t> nrows;       // [KB] local rows [0, nrows[j]) have a segment in block j (non-increasing)
   DevBuf<uint32_t> poff;        // [KB+1] staircase offsets
   DevBuf<uint2> cb_ids;         // [NG] groups of 4 block-local 16-bit ids (pad id = B)
-  DevBuf<uint32_t> cb_bits;     // [NG/32 + 4] bit g set <=> group g starts a segment
+  DevBuf<uint32_t> cb_bits;     // [NG/32 + 8] bit g set <=> group g starts a segment
   DevBuf<float> partial;        // [S] one partial sum per (block, row) pair
   DevBuf<uint4> chunks;         // [n_chunks] (g_begin, g_end, row_before, j | flags << 24)
   DevBuf<uint32_t> tail_slot;   // [n_chunks] staircase slot of the segment cut by the chunk end
@@ -642,6 +643,97 @@ __global__ void k_cb_chunks(const uint32_t* __restrict__ goff, const uint32_t* _
   }
 }
 
+// Bank-aware order of the ids inside each group (tools/cb_bank_model.py restates it).  A step of k_pr_cb
+// reads a WINDOW of 32 G groups (G = 2, or 4 in chunks of at least CB_WIDE_MIN groups): lane L's groups
+// G L + i (i < G) feed its shared-memory reads 4i..4i+3, and each of those read instructions takes as many
+// wavefronts as its most crowded bank (id & 31) holds words.  The 4 ids of a group belong to one (row,
+// block) pair, so their order only changes the rounding of the group's sum.  One thread per SET i of a
+// window: lanes 0..31 in turn put the 4 ids of their group G L + i into the 4 read slots in the order (of
+// 24) that lands them on the least loaded banks so far; padding ids (all lanes read the same word, a
+// broadcast) are free.  A set keeps its old order unless the new one lowers the sum over its slots of the
+// largest bank count.  Windows are the kernel's steps: chunk c steps from g0 & ~1 by 32 G and reads groups
+// outside [g0, g1) as padding (they are ordered by their own chunk), so every group is ordered by exactly
+// one thread and the result does not depend on thread timing.
+constexpr int CB_BANK_THREADS = 128;
+__global__ void __launch_bounds__(CB_BANK_THREADS) k_cb_bank_order(const uint4* __restrict__ chunks, uint32_t n_chunks,
+                                                                   uint32_t B, uint2* __restrict__ ids) {
+  __shared__ uint8_t hist[4 * 32][CB_BANK_THREADS];  // [slot * 32 + bank][thread]: no two threads share a byte
+  uint8_t(*h)[CB_BANK_THREADS] = hist;
+  const uint32_t t = threadIdx.x, lane = t & 31;
+  const uint32_t warp = (blockIdx.x * blockDim.x + t) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
+  // the 24 orders, slot -> id index, two bits per slot; the identity first, so ties keep the old order
+  constexpr uint8_t perms[24] = {0xE4, 0xB4, 0xD8, 0x78, 0x9C, 0x6C, 0xE1, 0xB1, 0xC9, 0x39, 0x8D, 0x2D,
+                                 0xD2, 0x72, 0xC6, 0x36, 0x4E, 0x1E, 0x93, 0x63, 0x87, 0x27, 0x4B, 0x1B};
+  const auto clear = [&]() {
+    for (int i = 0; i < 4 * 32; ++i) h[i][t] = 0;
+  };
+  const auto bound = [&]() {  // sum over the slots of max(1, the largest bank count)
+    uint32_t tot = 0;
+    for (int s = 0; s < 4; ++s) {
+      uint32_t mx = 1;
+      for (int b = 0; b < 32; ++b) mx = max(mx, (uint32_t)h[s * 32 + b][t]);
+      tot += mx;
+    }
+    return tot;
+  };
+  uint2 out[32];
+  for (uint32_t c = warp; c < n_chunks; c += nwarps) {
+    const uint4 ch = chunks[c];
+    const uint32_t g0 = ch.x, g1 = ch.y;
+    if (g0 >= g1) continue;
+    const uint32_t G = g1 - g0 >= CB_WIDE_MIN ? 4u : 2u;  // groups per lane in the chunk's steps
+    const uint32_t set = lane % G;
+    for (uint32_t gw = (g0 & ~1u) + 32 * G * (lane / G); gw < g1; gw += 32 * 32) {
+      clear();
+      for (uint32_t L = 0; L < 32; ++L) {
+        const uint32_t g = gw + G * L + set;
+        if (g < g0 || g >= g1) continue;
+        const uint2 v = ids[g];
+        const uint32_t id[4] = {v.x & 0xFFFFu, v.x >> 16, v.y & 0xFFFFu, v.y >> 16};
+        for (int s = 0; s < 4; ++s)
+          if (id[s] != B) ++h[s * 32 + (id[s] & 31u)][t];
+      }
+      const uint32_t before = bound();
+      clear();
+      for (uint32_t L = 0; L < 32; ++L) {
+        const uint32_t g = gw + G * L + set;
+        if (g < g0 || g >= g1) continue;
+        const uint2 v = ids[g];
+        const uint32_t id[4] = {v.x & 0xFFFFu, v.x >> 16, v.y & 0xFFFFu, v.y >> 16};
+        uint32_t cost[4][4];  // [slot][id index]: load of the id's bank in that slot so far
+#pragma unroll
+        for (int s = 0; s < 4; ++s)
+#pragma unroll
+          for (int k = 0; k < 4; ++k) cost[s][k] = id[k] == B ? 0u : h[s * 32 + (id[k] & 31u)][t];
+        uint32_t best = 0, best_cost = 0xFFFFFFFFu;
+#pragma unroll
+        for (int p = 0; p < 24; ++p) {
+          uint32_t sum = 0;
+#pragma unroll
+          for (int s = 0; s < 4; ++s) sum += cost[s][(perms[p] >> (2 * s)) & 3u];
+          if (sum < best_cost) {
+            best_cost = sum;
+            best = perms[p];
+          }
+        }
+        uint32_t o[4];
+#pragma unroll
+        for (int s = 0; s < 4; ++s) {
+          const uint32_t k = (best >> (2 * s)) & 3u;
+          o[s] = k == 0 ? id[0] : k == 1 ? id[1] : k == 2 ? id[2] : id[3];
+          if (o[s] != B) ++h[s * 32 + (o[s] & 31u)][t];
+        }
+        out[L] = make_uint2(o[0] | (o[1] << 16), o[2] | (o[3] << 16));
+      }
+      if (bound() >= before) continue;
+      for (uint32_t L = 0; L < 32; ++L) {
+        const uint32_t g = gw + G * L + set;
+        if (g >= g0 && g < g1) ids[g] = out[L];
+      }
+    }
+  }
+}
+
 // ---- sweep kernels (JACOBI) ------------------------------------------------------------------
 struct PrArgs {
   const uint32_t* outdeg;
@@ -736,7 +828,8 @@ __device__ __forceinline__ double pr_update(uint32_t gr, float sum, float old, u
 }
 
 // ---- column blocks ------------------------------------------------------------------------------------
-// One warp, one chunk: groups [g0, g1) of block j's stream, 64 groups (256 ids) per step.  Lane L owns
+// One warp, one chunk: groups [g0, g1) of block j's stream.  Chunks shorter than CB_WIDE_MIN groups (thin
+// blocks) take this 64-group step, longer ones the 128-group step of cb_chunk_wide below.  Lane L owns
 // the ADJACENT groups 2L and 2L+1 of the even-aligned window (one 128-bit load).  Inside a lane the two
 // group sums are combined when they belong to the same row; across lanes the value of the run that is
 // open at the end of each lane goes through a segmented inclusive scan (5 shuffles per 256 ids); a run
@@ -822,11 +915,109 @@ __device__ __forceinline__ void cb_chunk_impl(const PrArgs& a, const float* xs, 
     ids = nids;
   }
 }
+// The 128-group step (512 ids) of chunks with at least CB_WIDE_MIN groups: lane L owns groups 4L..4L+3
+// (two 128-bit loads), adds the runs inside the lane in f32 and ends up to four of them, and the warp
+// runs ONE segmented scan, one ballot and one read of the start bits per 512 ids instead of two.
+__device__ __forceinline__ uint4 ld_ids_u4(const uint4* p) {
+  uint4 r;  // the lane's second load reads the other half of the sectors of its first one: keep them in L1
+  asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
+  return r;
+}
+__device__ __forceinline__ float cb_group_sum(const float* xs, uint32_t lo, uint32_t hi) {
+  return xs[lo & 0xFFFFu] + xs[lo >> 16] + (xs[hi & 0xFFFFu] + xs[hi >> 16]);
+}
+template <bool SPECIAL>
+__device__ __forceinline__ void cb_chunk_wide(const PrArgs& a, const float* xs, uint32_t c, const uint4 ch,
+                                              uint32_t lane, uint32_t pad2) {
+  const uint32_t g0 = ch.x, g1 = ch.y;
+  const uint32_t j = ch.w & 0xFFFFFFu, fl = ch.w >> 24;
+  const bool head_cont = SPECIAL && (fl & CB_HEAD_CONT), tail_cont = SPECIAL && (fl & CB_TAIL_CONT);
+  uint32_t slot0 = a.poff[j] + ch.z;
+  bool in_head = head_cont;
+  double carry = 0.0;
+  const uint32_t le_mask = 0xFFFFFFFFu >> (31u - lane);
+  const uint32_t q0 = 4 * lane;  // the lane's first position in the step
+  const uint4* ids16 = reinterpret_cast<const uint4*>(a.cb_ids);
+  const uint4 padv = make_uint4(pad2, pad2, pad2, pad2);
+  const uint32_t gs0 = g0 & ~1u;
+  uint4 i0 = padv, i1 = padv;
+  if (gs0 + q0 < g1) i0 = ld_ids_u4(ids16 + (gs0 >> 1) + 2 * lane);
+  if (gs0 + q0 + 2 < g1) i1 = ld_ids_u4(ids16 + (gs0 >> 1) + 2 * lane + 1);
+  for (uint32_t gs = gs0; gs < g1; gs += 128) {
+    uint4 n0 = padv, n1 = padv;
+    if (gs + 128 + q0 < g1) n0 = ld_ids_u4(ids16 + ((gs + 128) >> 1) + 2 * lane);
+    if (gs + 128 + q0 + 2 < g1) n1 = ld_ids_u4(ids16 + ((gs + 128) >> 1) + 2 * lane + 1);
+    if (gs + q0 < g0) i0.x = i0.y = pad2;  // only position 0 can lie before g0 (gs0 = g0 & ~1)
+    if (gs + q0 + 1 >= g1) i0.z = i0.w = pad2;
+    if (gs + q0 + 2 >= g1) i1.x = i1.y = pad2;
+    if (gs + q0 + 3 >= g1) i1.z = i1.w = pad2;
+    const uint32_t wi = gs >> 5, sh = gs & 31u;
+    const uint32_t w0 = __ldg(a.cb_bits + wi), w1 = __ldg(a.cb_bits + wi + 1), w2 = __ldg(a.cb_bits + wi + 2),
+                   w3 = __ldg(a.cb_bits + wi + 3), w4 = __ldg(a.cb_bits + wi + 4);
+    unsigned long long WL = ((unsigned long long)__funnelshift_r(w1, w2, sh) << 32) | __funnelshift_r(w0, w1, sh);
+    unsigned long long WH = ((unsigned long long)__funnelshift_r(w3, w4, sh) << 32) | __funnelshift_r(w2, w3, sh);
+    const uint32_t nvalid = min(128u, g1 - gs);
+    if (nvalid < 64) {
+      WL &= (1ull << nvalid) - 1ull;
+      WH = 0;
+    } else if (nvalid < 128) {
+      WH &= (1ull << (nvalid - 64)) - 1ull;
+    }
+    if (gs < g0) WL &= ~1ull;
+    const uint32_t last = nvalid - 1;
+    const bool last_step = gs + 128 >= g1;
+    const bool run_continues = last_step ? tail_cont : !((w4 >> sh) & 1u);
+    const float v0 = cb_group_sum(xs, i0.x, i0.y), v1 = cb_group_sum(xs, i0.z, i0.w);
+    const float v2 = cb_group_sum(xs, i1.x, i1.y), v3 = cb_group_sum(xs, i1.z, i1.w);
+    const unsigned long long Wm = lane < 16 ? WL : WH;
+    const uint32_t s4 = q0 & 63u;
+    const uint32_t F = (uint32_t)(Wm >> s4) & 15u;  // segment starts at the lane's four positions
+    const bool nxt = lane == 31 ? false : lane == 15 ? (WH & 1ull) != 0 : ((Wm >> (s4 + 4)) & 1ull) != 0;
+    // runs inside the lane (restarted at every start)
+    const float r0 = v0;
+    const float r1 = (F & 2u) ? v1 : r0 + v1;
+    const float r2 = (F & 4u) ? v2 : r1 + v2;
+    float incl = (F & 8u) ? v3 : r2 + v3;  // this lane's share of the run open at its end
+    const uint32_t below = __ballot_sync(0xFFFFFFFFu, F != 0) & le_mask;
+    const int seg_start = below ? 31 - __clz(below) : -1;
+    const int lo = seg_start < 0 ? 0 : seg_start;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const float t = __shfl_up_sync(0xFFFFFFFFu, incl, d);
+      if ((int)lane - d >= lo) incl += t;
+    }
+    const double incl_d = (double)incl + (seg_start < 0 ? carry : 0.0);
+    double x_in = __shfl_up_sync(0xFFFFFFFFu, incl_d, 1);
+    if (lane == 0) x_in = carry;
+    const uint32_t pre = (lane < 16 ? 0u : (uint32_t)__popcll(WL)) + (uint32_t)__popcll(Wm & ((1ull << s4) - 1ull));
+    const bool valid0 = gs + q0 >= g0 && q0 <= last;
+    cb_emit<SPECIAL>(a, c, valid0 && (q0 == last || (F & 2u)), q0, last, run_continues, last_step, tail_cont,
+                     in_head, pre + (F & 1u), slot0, (double)r0 + ((F & 1u) ? 0.0 : x_in));
+    cb_emit<SPECIAL>(a, c, q0 + 1 <= last && (q0 + 1 == last || (F & 4u)), q0 + 1, last, run_continues, last_step,
+                     tail_cont, in_head, pre + __popc(F & 3u), slot0, (double)r1 + ((F & 3u) ? 0.0 : x_in));
+    cb_emit<SPECIAL>(a, c, q0 + 2 <= last && (q0 + 2 == last || (F & 8u)), q0 + 2, last, run_continues, last_step,
+                     tail_cont, in_head, pre + __popc(F & 7u), slot0, (double)r2 + ((F & 7u) ? 0.0 : x_in));
+    cb_emit<SPECIAL>(a, c, q0 + 3 <= last && (q0 + 3 == last || nxt), q0 + 3, last, run_continues, last_step,
+                     tail_cont, in_head, pre + __popc(F), slot0, incl_d);
+    const double tl = __shfl_sync(0xFFFFFFFFu, incl_d, 31);
+    carry = (run_continues && !last_step) ? tl : 0.0;
+    if (SPECIAL && (WL | WH)) in_head = false;
+    slot0 += __popcll(WL) + __popcll(WH);
+    i0 = n0;
+    i1 = n1;
+  }
+}
 __device__ __forceinline__ void cb_chunk(const PrArgs& a, const float* xs, uint32_t c, uint32_t lane, uint32_t pad2) {
   const uint4 ch = a.chunks[c];
   if (ch.x >= ch.y) return;
-  if ((ch.w >> 24) & (CB_HEAD_CONT | CB_TAIL_CONT)) cb_chunk_impl<true>(a, xs, c, ch, lane, pad2);
-  else cb_chunk_impl<false>(a, xs, c, ch, lane, pad2);
+  const bool special = (ch.w >> 24) & (CB_HEAD_CONT | CB_TAIL_CONT);
+  if (ch.y - ch.x >= CB_WIDE_MIN) {
+    if (special) cb_chunk_wide<true>(a, xs, c, ch, lane, pad2);
+    else cb_chunk_wide<false>(a, xs, c, ch, lane, pad2);
+  } else {
+    if (special) cb_chunk_impl<true>(a, xs, c, ch, lane, pad2);
+    else cb_chunk_impl<false>(a, xs, c, ch, lane, pad2);
+  }
 }
 
 // ---- TMA bulk copy of a source block into shared memory (cp.async.bulk + mbarrier) -----------------
@@ -1643,8 +1834,8 @@ static gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan
     }
     // 6. fill: segments + SELL remainders of the rows below n_cb, whole rows above
     GB_TRY(p->cb_ids.alloc(std::max<uint64_t>(p->NG, 1), 64));
-    GB_TRY(p->cb_bits.alloc(p->NG / 32 + 4));
-    GB_CUDA(cudaMemsetAsync(p->cb_bits.p, 0, (p->NG / 32 + 4) * 4, s));
+    GB_TRY(p->cb_bits.alloc(p->NG / 32 + 8));  // a 128-group step reads 5 words from its first
+    GB_CUDA(cudaMemsetAsync(p->cb_bits.p, 0, (p->NG / 32 + 8) * 4, s));
     if (p->NG) {
       k_fill_u2<<<grid_for(p->NG + 64, 256), 256, 0, s>>>(p->cb_ids.p, p->NG + 64, make_uint2(B | (B << 16), B | (B << 16)));
       k_cb_bits<<<grid_for(p->S, 256), 256, 0, s>>>(goff.p, p->S, p->cb_bits.p);
@@ -1712,6 +1903,10 @@ static gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan
       k_cb_chunks<<<grid_for(p->n_chunks, 128), 128, 0, s>>>(goff.p, p->poff.p, p->nrows.p, gbeg.p, cfirst.p, cgrp.p,
                                                            p->KB, p->n_chunks, p->chunks.p, p->tail_slot.p,
                                                            p->fix_list.p, d_nfix);
+      // GB_PR_BANK_ORDER=0 (experiment): keep the ids of every group in CSR order
+      if (env_u32("GB_PR_BANK_ORDER", 1) != 0)
+        k_cb_bank_order<<<grid_for((uint64_t)p->n_chunks * 32, CB_BANK_THREADS), CB_BANK_THREADS, 0, s>>>(
+            p->chunks.p, p->n_chunks, B, p->cb_ids.p);
       GB_CUDA(cudaGetLastError());
       uint32_t h_fix[2] = {0, 0};
       GB_CUDA(cudaMemcpyAsync(h_fix, d_nfix, 8, cudaMemcpyDeviceToHost, s));

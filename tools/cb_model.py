@@ -58,11 +58,18 @@ def build_chunks(goff, poff, nrows, gbeg, C):
     return chunks, tail_slot, fix
 
 
+WIDE_MIN = 128   # CB_WIDE_MIN: chunks of at least this many groups take the 128-group step
+
+
 def run_chunk(c, chunks, vals, bits, poff, partial, side):
     """cb_chunk: vals[g] = f32 sum of group g's four gathers; bits[g] = group g starts a segment.
-    A step covers 64 groups; lane L owns the adjacent groups 2L and 2L+1 of the (even-aligned) window."""
+    A step covers 64 groups; lane L owns the adjacent groups 2L and 2L+1 of the (even-aligned) window.
+    Chunks of at least WIDE_MIN groups take the 128-group step of run_chunk_wide."""
     g0, g1, row_before, j, fl = chunks[c]
     if g0 >= g1:
+        return
+    if g1 - g0 >= WIDE_MIN:
+        run_chunk_wide(c, chunks, vals, bits, poff, partial, side)
         return
     head_cont, tail_cont = bool(fl & HEAD), bool(fl & TAIL)
     in_head = head_cont
@@ -117,6 +124,80 @@ def run_chunk(c, chunks, vals, bits, poff, partial, side):
                     continue
                 head_run = in_head and cum[q] == 0
                 if head_run:
+                    side[2 * c] = tot
+                elif q == last and last_step and tail_cont:
+                    side[2 * c + 1] = tot
+                else:
+                    partial[poff[j] + row_before + cum[q]] = np.float32(tot)
+        carry = inclD[31] if (run_continues and not last_step) else 0.0
+        if W.any():
+            in_head = False
+        row_before += int(W.sum())
+
+
+def seg_scan(T, F, carry):
+    """the segmented inclusive warp scan of cb_chunk_impl: T = each lane's share of the run open at its
+    end (f32), F = the lane holds a segment start.  Returns (inclD, XD): the run open at the end of each
+    lane and at the end of the lane before it, in f64 with the carried run added."""
+    lanes = np.arange(32)
+    seg_start = np.full(32, -1)
+    cur = -1
+    for l in range(32):
+        if F[l]:
+            cur = l
+        seg_start[l] = cur
+    lo = np.maximum(seg_start, 0)
+    incl = T.astype(np.float32).copy()
+    d = 1
+    while d < 32:
+        t = np.zeros(32, np.float32)
+        t[d:] = incl[:-d]
+        incl = np.where((lanes - d) >= lo, (incl + t).astype(np.float32), incl)
+        d <<= 1
+    inclD = incl.astype(np.float64) + np.where(seg_start < 0, carry, 0.0)
+    XD = np.empty(32)
+    XD[0] = carry
+    XD[1:] = inclD[:-1]
+    return inclD, XD
+
+
+def run_chunk_wide(c, chunks, vals, bits, poff, partial, side):
+    """cb_chunk_impl's 128-group step: lane L owns groups 4L..4L+3 of the window (two 128-bit loads),
+    adds the runs inside the lane in f32, and takes part in ONE segmented scan per 512 ids."""
+    g0, g1, row_before, j, fl = chunks[c]
+    head_cont, tail_cont = bool(fl & HEAD), bool(fl & TAIL)
+    in_head = head_cont
+    carry = 0.0
+    for gs in range(g0 & ~1, g1, 128):
+        pos = np.arange(128)
+        valid = (gs + pos >= g0) & (gs + pos < g1)
+        W = np.zeros(128, bool)
+        W[valid] = bits[gs + pos[valid]]
+        v = np.zeros(128, np.float32)
+        v[valid] = vals[gs + pos[valid]]
+        last = int(np.nonzero(valid)[0][-1])
+        last_step = gs + 128 >= g1
+        run_continues = tail_cont if last_step else (not bits[gs + 128])
+        F, V = W.reshape(32, 4), v.reshape(32, 4)
+        r = np.zeros((32, 4), np.float32)        # run sums inside the lane, restarted at each start
+        for i in range(4):
+            prev = r[:, i - 1] if i else np.zeros(32, np.float32)
+            r[:, i] = np.where(F[:, i], V[:, i], (prev + V[:, i]).astype(np.float32))
+        inclD, XD = seg_scan(r[:, 3], F.any(axis=1), carry)
+        cum = np.cumsum(W)
+        for l in range(32):
+            for i in range(4):
+                q = 4 * l + i
+                nxt = W[q + 1] if q + 1 < 128 else False
+                if not (valid[q] and (q == last or nxt)):
+                    continue
+                if q == last and run_continues and not last_step:
+                    continue
+                if i == 3:
+                    tot = inclD[l]
+                else:
+                    tot = float(r[l, i]) + (0.0 if F[l, :i + 1].any() else XD[l])
+                if in_head and cum[q] == 0:
                     side[2 * c] = tot
                 elif q == last and last_step and tail_cont:
                     side[2 * c + 1] = tot
