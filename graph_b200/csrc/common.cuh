@@ -115,6 +115,22 @@ struct DevBuf {
   size_t bytes() const { return n * sizeof(T); }
 };
 
+// CUB's two-phase call: call(nullptr, bytes) sizes the temporary storage, call(tmp.p, bytes) runs.  tmp is
+// the caller's, so its release (which waits for the stream) stays where the caller puts it; a buffer that
+// already holds enough is reused, a new one gets `headroom` times the size asked for.
+template <typename Call>
+gb_status cub_call(DevBuf<uint8_t>& tmp, Call&& call, size_t headroom = 1) {
+  size_t bytes = 0;
+  GB_CUDA(call(nullptr, bytes));
+  if (!tmp.p || tmp.n < bytes) {
+    DevBuf<uint8_t> fresh;
+    GB_TRY(fresh.alloc(bytes * headroom));
+    tmp = std::move(fresh);  // an old buffer is released once the stream is done with it
+  }
+  GB_CUDA(call(tmp.p, bytes));
+  return GB_OK;
+}
+
 // ---- device CSR ----------------------------------------------------------------------------
 // offsets[n+1] u32, targets[len] u32 (+8 entries of zeroed slack for 128-bit loads), optional
 // SoA weights[len] f32 (the host API exposes the reference's 8-byte AoS Target{u32,f32}).
@@ -126,7 +142,7 @@ struct DevCsr {
   uint64_t bytes() const { return off.bytes() + tgt.bytes() + w.bytes(); }
 };
 
-struct PrPlan;  // pagerank.cu
+struct PrPlan;  // pr_plan.cuh
 
 }  // namespace gb
 

@@ -82,11 +82,10 @@ static gb_status offsets_from_sorted(cudaStream_t s, RowFn row_of, uint64_t coun
                                      uint32_t* off) {
   GB_CUDA(cudaMemsetAsync(off, 0, ((size_t)n + 1) * 4, s));
   if (count) k_mark_row_ends<<<grid_for(count, 256), 256, 0, s>>>(row_of, count, off);
-  size_t tb = 0;
-  GB_CUDA(cub::DeviceScan::InclusiveScan(nullptr, tb, off, off, cub::Max(), (int64_t)n + 1, s));
   DevBuf<uint8_t> tmp;
-  GB_TRY(tmp.alloc(tb));
-  GB_CUDA(cub::DeviceScan::InclusiveScan(tmp.p, tb, off, off, cub::Max(), (int64_t)n + 1, s));
+  GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
+    return cub::DeviceScan::InclusiveScan(t, tb, off, off, cub::Max(), (int64_t)n + 1, s);
+  }));
   GB_CUDA(cudaStreamSynchronize(s));  // tmp is released on return
   return GB_OK;
 }
@@ -205,11 +204,10 @@ gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, c
     k_iota<<<grid_for(count, blk), blk, 0, s>>>(idx.p, count);
     cub::DoubleBuffer<uint32_t> kb(rows_copy.p, keys_alt.p);
     cub::DoubleBuffer<uint32_t> vb(idx.p, idx_alt.p);
-    size_t tmp_bytes = 0;
-    GB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, kb, vb, count, 0, (int)bits, s));
     DevBuf<uint8_t> tmp;
-    GB_TRY(tmp.alloc(tmp_bytes));
-    GB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, kb, vb, count, 0, (int)bits, s));
+    GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
+      return cub::DeviceRadixSort::SortPairs(t, tb, kb, vb, count, 0, (int)bits, s);
+    }));
     GB_TRY(csr->tgt.alloc(count, 8));
     GB_CUDA(cudaMemsetAsync(csr->tgt.p + count, 0, 8 * 4, s));
     k_gather<uint32_t><<<grid_for(count, blk), blk, 0, s>>>(d_cols, vb.Current(), count, csr->tgt.p);
@@ -231,21 +229,20 @@ gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, c
   cub::DoubleBuffer<uint64_t> kb(keys.p, keys_alt.p);
   DevBuf<uint32_t> idx, idx_alt;
   DevBuf<uint8_t> tmp;
-  size_t tmp_bytes = 0;
   const uint32_t* order = nullptr;
   if (d_w) {
     GB_TRY(idx.alloc(count));
     GB_TRY(idx_alt.alloc(count));
     k_iota<<<grid_for(count, blk), blk, 0, s>>>(idx.p, count);
     cub::DoubleBuffer<uint32_t> vb(idx.p, idx_alt.p);
-    GB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, kb, vb, count, 0, (int)(2 * bits), s));
-    GB_TRY(tmp.alloc(tmp_bytes));
-    GB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, kb, vb, count, 0, (int)(2 * bits), s));
+    GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
+      return cub::DeviceRadixSort::SortPairs(t, tb, kb, vb, count, 0, (int)(2 * bits), s);
+    }));
     order = vb.Current();
   } else {
-    GB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, kb, count, 0, (int)(2 * bits), s));
-    GB_TRY(tmp.alloc(tmp_bytes));
-    GB_CUDA(cub::DeviceRadixSort::SortKeys(tmp.p, tmp_bytes, kb, count, 0, (int)(2 * bits), s));
+    GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
+      return cub::DeviceRadixSort::SortKeys(t, tb, kb, count, 0, (int)(2 * bits), s);
+    }));
   }
   uint64_t* sorted = kb.Current();
   uint64_t* spare = kb.Alternate();
@@ -258,23 +255,17 @@ gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, c
     GB_TRY(flags.alloc(count));
     GB_TRY(d_num.alloc(1));
     k_dedup_flags<<<grid_for(count, blk), blk, 0, s>>>(sorted, count, bits, flags.p);
-    size_t sel_bytes = 0;
-    GB_CUDA(cub::DeviceSelect::Flagged(nullptr, sel_bytes, sorted, flags.p, spare, d_num.p,
-                                       (int64_t)count, s));
     DevBuf<uint8_t> sel_tmp;
-    GB_TRY(sel_tmp.alloc(sel_bytes));
-    GB_CUDA(cub::DeviceSelect::Flagged(sel_tmp.p, sel_bytes, sorted, flags.p, spare, d_num.p,
-                                       (int64_t)count, s));
+    GB_TRY(cub_call(sel_tmp, [&](void* t, size_t& tb) {
+      return cub::DeviceSelect::Flagged(t, tb, sorted, flags.p, spare, d_num.p, (int64_t)count, s);
+    }));
     if (order) {
       GB_TRY(order_c.alloc(count));
       // the uint32 selection has its own temporary-storage size: query it (never reuse the uint64 one)
-      size_t sel_bytes32 = 0;
-      GB_CUDA(cub::DeviceSelect::Flagged(nullptr, sel_bytes32, order, flags.p, order_c.p, d_num.p,
-                                         (int64_t)count, s));
       DevBuf<uint8_t> sel_tmp32;
-      GB_TRY(sel_tmp32.alloc(sel_bytes32));
-      GB_CUDA(cub::DeviceSelect::Flagged(sel_tmp32.p, sel_bytes32, order, flags.p, order_c.p, d_num.p,
-                                         (int64_t)count, s));
+      GB_TRY(cub_call(sel_tmp32, [&](void* t, size_t& tb) {
+        return cub::DeviceSelect::Flagged(t, tb, order, flags.p, order_c.p, d_num.p, (int64_t)count, s);
+      }));
       GB_CUDA(cudaStreamSynchronize(s));  // sel_tmp32 is released at the end of this scope
       order = order_c.p;
     }
@@ -774,11 +765,10 @@ gb_status gb_make_degree_ordered(gb_graph* g) {
   GB_TRY(dk_alt.alloc(n));
   k_degree_keys<<<grid_for(n, 256), 256, 0, s>>>(g->out.off.p, n, dk.p);
   cub::DoubleBuffer<uint64_t> db(dk.p, dk_alt.p);
-  size_t tmp_bytes = 0;
-  GB_CUDA(cub::DeviceRadixSort::SortKeysDescending(nullptr, tmp_bytes, db, (int)n, 0, 64, s));
   DevBuf<uint8_t> tmp;
-  GB_TRY(tmp.alloc(tmp_bytes));
-  GB_CUDA(cub::DeviceRadixSort::SortKeysDescending(tmp.p, tmp_bytes, db, (int)n, 0, 64, s));
+  GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
+    return cub::DeviceRadixSort::SortKeysDescending(t, tb, db, (int)n, 0, 64, s);
+  }));
   DevBuf<uint32_t> new_id, new_deg, rows;
   GB_TRY(new_id.alloc(n));
   GB_TRY(new_deg.alloc(n));
@@ -796,11 +786,10 @@ gb_status gb_make_degree_ordered(gb_graph* g) {
     GB_TRY(keys_alt.alloc(len));
     k_relabel_keys<<<grid_for(len, 256), 256, 0, s>>>(rows.p, g->out.tgt.p, new_id.p, len, bits, keys.p);
     cub::DoubleBuffer<uint64_t> kb(keys.p, keys_alt.p);
-    size_t sb = 0;
-    GB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, sb, kb, len, 0, (int)(2 * bits), s));
     DevBuf<uint8_t> stmp;
-    GB_TRY(stmp.alloc(sb));
-    GB_CUDA(cub::DeviceRadixSort::SortKeys(stmp.p, sb, kb, len, 0, (int)(2 * bits), s));
+    GB_TRY(cub_call(stmp, [&](void* t, size_t& tb) {
+      return cub::DeviceRadixSort::SortKeys(t, tb, kb, len, 0, (int)(2 * bits), s);
+    }));
     k_unpack_targets<<<grid_for(len, 256), 256, 0, s>>>(kb.Current(), len, bits, fresh.tgt.p);
     GB_TRY(offsets_from_sorted(s, RowOfKey{kb.Current(), bits}, len, n, fresh.off.p));
     GB_CUDA(cudaGetLastError());

@@ -479,10 +479,9 @@ static gb_status load_file(int device, const char* path, gb_file_format format, 
     if (tiles) {
       GB_TRY(grow(counts, tiles, 2 * tiles, 0, sp.work));
       k_load_count_lines<<<(unsigned)tiles, LOAD_BLOCK, 0, sp.work>>>(d, sg.len, counts.p);
-      size_t tb = 0;
-      GB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, counts.p, counts.p, (int)tiles, sp.work));
-      GB_TRY(grow(scan_tmp, tb, 2 * tb, 0, sp.work));
-      GB_CUDA(cub::DeviceScan::InclusiveSum(scan_tmp.p, tb, counts.p, counts.p, (int)tiles, sp.work));
+      GB_TRY(cub_call(scan_tmp, [&](void* t, size_t& tb) {
+        return cub::DeviceScan::InclusiveSum(t, tb, counts.p, counts.p, (int)tiles, sp.work);
+      }, 2));
       GB_CUDA(cudaMemcpyAsync(hsmall, counts.p + tiles - 1, 4, cudaMemcpyDeviceToHost, sp.work));
       GB_CUDA(cudaMemcpyAsync(hsmall + 1, &ctr.p->declined, 4, cudaMemcpyDeviceToHost, sp.work));
     }

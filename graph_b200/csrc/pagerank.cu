@@ -34,120 +34,12 @@
 //
 // Algorithmic bytes per sweep: 4m (targets) + 4(n+1) (offsets) + 5*4n (out_scores read+write,
 // scores read+write, out-degree read) = 4m + 24n + 4  (BASELINE.md §3).
-#include <cub/cub.cuh>
-
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
-#include <numeric>
 
-#include "common.cuh"
+#include "pr_plan.cuh"
 
 namespace gb {
-
-constexpr int PR_WARPS = 32;        // warps per CTA of the sweep kernels: one persistent CTA per SM
-constexpr int PR_THREADS = PR_WARPS * 32;
-constexpr int PR_SELL_THREADS = 512; // SELL kernel: two 16-warp CTAs per SM and no shared memory (L1 keeps it all)
-constexpr int PR_FIN_THREADS = 256;
-constexpr uint32_t PR_MAX_PROFILE_EVENTS = 256;  // sweeps bracketed by CUDA events when profiling is on
-constexpr uint32_t CB_G = 4;                 // block-local ids per group (one 64-bit load per lane)
-constexpr uint32_t CB_BLOCK_DEFAULT = 49152; // source-vector entries per block (192 KB of shared memory)
-constexpr uint32_t CB_BLOCK_MAX = 56 * 1024;
-constexpr double CB_TAU_DEFAULT = 1.5;       // a (row, block) pair gets a segment if it expects >= tau edges
-constexpr uint32_t CB_MAX_BLOCKS = 8192;     // hot blocks kept (the staircase rarely needs more than ~1000)
-constexpr uint32_t CB_TASK_CHUNKS = 32;      // chunks per task (one per warp)
-constexpr uint32_t CB_WIDE_MIN = 128;        // chunks of at least this many groups take k_pr_cb's 128-group step
-constexpr uint32_t SELL_FEW = 4;             // rows with segments in at most this many blocks are finished by k_pr_sell itself
-constexpr uint32_t FIN_CTA_BLOCKS = 64;      // finish: 32-row groups with segments in more blocks get a CTA each
-constexpr uint32_t CB_NONE = 0xFFFFFFFFu;
-constexpr uint32_t CB_MEGA_DEG = 32768;      // layout build: rows with more in-edges go through one stable radix sort
-constexpr uint32_t CB_MEGA_JBITS = 14;       // key = row << 14 | block rank (0x3FFF = not in a segment)
-constexpr uint32_t CB_ILP = 4;               // 32-edge batches in flight per warp in the layout build
-// chunk flags (bits 24.. of PrChunk.w)
-constexpr uint32_t CB_HEAD_CONT = 1u, CB_TAIL_CONT = 2u, CB_INTERIOR = 4u;
-
-// ---- the cyclic deal of 32-row slices over the ranks of the 1-D edge-cut ---------------------------
-struct PrDeal {
-  uint32_t P = 1, p = 0;
-};
-__host__ __device__ __forceinline__ uint32_t deal_global(uint32_t l, uint32_t P, uint32_t p) {
-  return (((l >> 5) * P + p) << 5) | (l & 31u);
-}
-// number of local rows whose global index is below R
-static inline uint32_t deal_count(uint32_t R, uint32_t P, uint32_t p) {
-  const uint32_t F = R >> 5, rem = R & 31u;
-  const uint32_t full = F > p ? (F - p + P - 1) / P : 0;
-  uint32_t c = full * 32;
-  if (rem && (F % P) == p) c += rem;
-  return c;
-}
-
-struct PrPlan {
-  uint32_t n = 0;
-  uint32_t n_active = 0;  // global rows with in-degree > 0 (renumbered to [0, n_active))
-  uint64_t m = 0;
-  PrDeal deal;
-  uint32_t n_loc = 0;     // local active rows
-  uint32_t n_cb = 0;      // local rows [0, n_cb) own at least one column-block segment
-  uint64_t loc_edges = 0; // in-edges of the local rows
-  uint64_t cb_edges = 0;  // of which served from column blocks
-  DevBuf<uint32_t> new_id;    // old id -> internal id
-  DevBuf<uint32_t> outdeg;    // out-degree by internal id [n]
-  // column blocks
-  uint32_t B = 0, KB = 0;       // block entries, hot blocks
-  uint64_t S = 0;               // staircase size = sum of nrows[j]
-  uint64_t NG = 0;              // groups in all block streams
-  uint32_t chunk_groups = 0, n_chunks = 0, n_tasks = 0, n_fix = 0;
-  uint32_t fix_max_row = 0;     // largest local row that owns a segment cut by a chunk boundary
-  uint32_t n_mega = 0;          // local rows [0, n_mega) went through the sort path of the layout build
-  uint32_t last_hot_block = CB_NONE;  // largest source block index among the hot blocks
-  DevBuf<uint32_t> blk;         // [KB] source block of hot rank j
-  DevBuf<uint32_t> nrows;       // [KB] local rows [0, nrows[j]) have a segment in block j (non-increasing)
-  DevBuf<uint32_t> poff;        // [KB+1] staircase offsets
-  DevBuf<uint2> cb_ids;         // [NG] groups of 4 block-local 16-bit ids (pad id = B)
-  DevBuf<uint32_t> cb_bits;     // [NG/32 + 8] bit g set <=> group g starts a segment
-  DevBuf<float> partial;        // [S] one partial sum per (block, row) pair
-  DevBuf<uint4> chunks;         // [n_chunks] (g_begin, g_end, row_before, j | flags << 24)
-  DevBuf<uint32_t> tail_slot;   // [n_chunks] staircase slot of the segment cut by the chunk end
-  DevBuf<double> side;          // [2 n_chunks] head / tail parts of segments cut by chunk boundaries
-  DevBuf<uint32_t> fix_list;    // [n_fix] chunks whose tail segment continues in later chunks
-  DevBuf<uint2> tasks;          // [n_tasks] (first chunk, chunk count | block rank << 8), fattest blocks first
-  DevBuf<uint32_t> task_ctr;    // [grid_cb] per-range task cursors (reset by the finish kernel)
-  DevBuf<float> rem;            // [n_cb] SELL remainder sums of the rows that also have segments
-  DevBuf<uint32_t> fin_kb;      // [ceil(n_cb / 32)] blocks of the first row of each 32-row group (finish kernel)
-  // SELL-32 (all local active rows; rows < n_cb hold only the edges outside their segments)
-  uint32_t num_slices = 0;
-  DevBuf<uint4> sell;         // slice-major, then 4-edge group, then lane
-  DevBuf<uint2> slice_meta;   // per slice: (first uint4 index, uint4 groups per lane)
-  // state (single-GPU path; the shard API brings its own vectors)
-  DevBuf<float> x[2];
-  DevBuf<float> scores;
-  unsigned grid_cb = 0, grid_sell = 0, grid_fin = 1;
-  uint32_t n_fin_warp = 0;   // rows [0, n_fin_warp) own segments in more than FIN_CTA_BLOCKS blocks
-  uint32_t fin_u = 4;        // finish: row groups per warp iteration (template argument of k_pr_finish)
-  uint32_t fin_hub_ctas = 0; // finish CTAs that take the hub groups (the others take rows [n_fin_warp, n_fin))
-  uint32_t n_fin = 0;        // rows [0, n_fin) are completed by k_pr_finish, [n_fin, n_cb) by k_pr_sell
-  uint32_t few_nrows[SELL_FEW] = {}, few_poff[SELL_FEW] = {};
-  // dual mode: k_pr_cb and k_pr_sell run at the same time on the same SMs (two streams, 512-thread CTAs)
-  bool dual = false;
-  cudaStream_t s2 = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  DevBuf<double> block_err;  // per CTA error partials (SELL CTAs, then finish CTAs)
-  DevBuf<double> err_hist;   // error of each sweep of the current batch
-  DevBuf<uint32_t> ctrl;     // [0] = done flag (sweep number at which tolerance was met), [1] = ticket
-  size_t smem_cb = 0;
-  std::vector<cudaEvent_t> prof_events;
-  // GB_PR_TRACE=1 (diagnostics): CUDA events between the kernels of every sweep; averages are printed
-  // to stderr when the layout is released
-  bool trace = false;
-  mutable std::vector<cudaEvent_t> trace_events;  // 5 per traced sweep
-  uint64_t bytes() const {
-    return new_id.bytes() + outdeg.bytes() + blk.bytes() + nrows.bytes() + poff.bytes() + cb_ids.bytes() +
-           cb_bits.bytes() + partial.bytes() + chunks.bytes() + tail_slot.bytes() + side.bytes() +
-           fix_list.bytes() + tasks.bytes() + rem.bytes() + fin_kb.bytes() + sell.bytes() + slice_meta.bytes() + x[0].bytes() +
-           x[1].bytes() + scores.bytes() + block_err.bytes() + err_hist.bytes();
-  }
-};
 
 void free_pr_plan(PrPlan* p) {
   if (!p) return;
@@ -166,9 +58,6 @@ void free_pr_plan(PrPlan* p) {
   }
   for (cudaEvent_t e : p->trace_events) cudaEventDestroy(e);
   for (cudaEvent_t e : p->prof_events) cudaEventDestroy(e);
-  if (p->ev_fork) cudaEventDestroy(p->ev_fork);
-  if (p->ev_join) cudaEventDestroy(p->ev_join);
-  if (p->s2) cudaStreamDestroy(p->s2);
   delete p;
 }
 uint64_t pr_plan_bytes(const PrPlan* p) { return p ? p->bytes() : 0; }
@@ -195,543 +84,6 @@ __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);
   return v;
-}
-__device__ __forceinline__ uint32_t warp_max(uint32_t v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(0xFFFFFFFFu, v, o));
-  return v;
-}
-
-// ---- plan construction kernels ---------------------------------------------------------------
-__global__ void k_perm_keys(const uint32_t* __restrict__ in_off, const uint32_t* __restrict__ out_off,
-                            uint32_t n, uint64_t* __restrict__ keys, uint32_t* __restrict__ ids) {
-  for (uint32_t v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += gridDim.x * blockDim.x) {
-    uint32_t indeg = in_off[v + 1] - in_off[v];
-    uint32_t outdeg = out_off[v + 1] - out_off[v];
-    // in-degree descending (hub rows first, rows of similar length become neighbours), then
-    // out-degree descending (hot sources first inside equal in-degrees).  R-MAT's expected in- and
-    // out-degree of a vertex coincide, so this is also a hot-first order of the SOURCES.
-    keys[v] = ((uint64_t)(uint32_t)(~indeg) << 32) | (uint32_t)(~outdeg);
-    ids[v] = v;
-  }
-}
-__global__ void k_perm_scatter(const uint32_t* __restrict__ sorted_ids, const uint32_t* __restrict__ out_off,
-                               const uint32_t* __restrict__ in_off, uint32_t n, uint32_t* __restrict__ new_id,
-                               uint32_t* __restrict__ outdeg, uint32_t* __restrict__ indeg) {
-  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r <= n; r += gridDim.x * blockDim.x) {
-    if (r == n) {
-      indeg[n] = 0;
-      continue;
-    }
-    uint32_t v = sorted_ids[r];
-    new_id[v] = r;
-    outdeg[r] = out_off[v + 1] - out_off[v];
-    indeg[r] = in_off[v + 1] - in_off[v];
-  }
-}
-__global__ void k_count_active(const uint32_t* __restrict__ indeg, uint32_t n, uint32_t* __restrict__ count) {
-  uint32_t act = 0;
-  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n; r += gridDim.x * blockDim.x) act += indeg[r] > 0;
-  for (int o = 16; o > 0; o >>= 1) act += __shfl_xor_sync(0xFFFFFFFFu, act, o);
-  if ((threadIdx.x & 31) == 0 && act) atomicAdd(count, act);
-}
-// out-edges leaving each source block (one CTA per block): the block's share of all gathers
-__global__ void k_blk_edges(const uint32_t* __restrict__ outdeg, uint32_t n, uint32_t B,
-                            unsigned long long* __restrict__ blk_edges) {
-  __shared__ unsigned long long part[8];
-  const uint32_t b = blockIdx.x;
-  const uint64_t lo = (uint64_t)b * B, hi = min((uint64_t)n, lo + B);
-  unsigned long long s = 0;
-  for (uint64_t i = lo + threadIdx.x; i < hi; i += blockDim.x) s += outdeg[i];
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, o);
-  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    unsigned long long t = 0;
-    for (uint32_t w = 0; w < blockDim.x / 32; ++w) t += part[w];
-    blk_edges[b] = t;
-  }
-}
-// rows_ge[b] = number of (global) rows with in-degree >= dmin[b] (indeg is non-increasing);
-// edges_ge[b] = the in-edges of those rows (deg_prefix = inclusive prefix sums of indeg)
-__global__ void k_rows_ge(const uint32_t* __restrict__ indeg, const unsigned long long* __restrict__ deg_prefix,
-                          uint32_t n_active, const uint32_t* __restrict__ dmin, uint32_t nblk,
-                          uint32_t* __restrict__ rows_ge, unsigned long long* __restrict__ edges_ge) {
-  for (uint32_t b = blockIdx.x * blockDim.x + threadIdx.x; b < nblk; b += gridDim.x * blockDim.x) {
-    const uint32_t d = dmin[b];
-    uint32_t lo = 0, hi = n_active;  // first index with indeg < d
-    while (lo < hi) {
-      const uint32_t mid = lo + (hi - lo) / 2;
-      if (indeg[mid] >= d) lo = mid + 1;
-      else hi = mid;
-    }
-    rows_ge[b] = lo;
-    edges_ge[b] = lo ? deg_prefix[lo - 1] : 0ull;
-  }
-}
-struct U32ToU64 {
-  __host__ __device__ unsigned long long operator()(uint32_t v) const { return v; }
-};
-
-// Classification of the in-edges of the rows that own segments (local rows [n_mega, n_cb)).  An edge
-// from source s (internal id) lands in block s / B; if that block is hot (rank j) and the row is inside
-// the block's row prefix it belongs to segment (j, row), else to the row's SELL remainder.  One warp walks
-// a row in CSR order and leaves one 8-byte RECORD per edge, so that the fill pass — which has to wait for
-// the scan over all segment sizes — is a plain scatter with no lookups left:
-//   segment edge:   x = block-local id | j << 16,   y = 1 << 31 | position inside the segment
-//   remainder edge: x = internal source id,         y = position inside the row's SELL lane
-// Positions follow the CSR order (the per-pair counter is advanced batch by batch, each batch waits for
-// the previous one's counter value): the layout is deterministic.
-constexpr uint32_t CB_REC_SEG = 0x80000000u;
-template <bool CHECK>
-__device__ __forceinline__ uint32_t cb_classify_row(uint32_t l, uint32_t b0, uint32_t d, uint32_t n,
-                                                    const uint32_t* __restrict__ in_tgt,
-                                                    const uint32_t* __restrict__ new_id,
-                                                    const uint32_t* __restrict__ hot_of_blk,
-                                                    const uint32_t* __restrict__ nrows,
-                                                    const uint32_t* __restrict__ poff,
-                                                    const uint32_t* __restrict__ blk, uint32_t B,
-                                                    uint32_t* __restrict__ cnt, uint2* __restrict__ rec, uint32_t lane) {
-  uint32_t rem = 0;
-  // CB_ILP batches of 32 edges per iteration: their dependent loads (target -> internal id -> block
-  // rank -> row prefix) are issued together, so a long row's single warp is not latency bound
-  for (uint32_t i = 0; i < d; i += 32 * CB_ILP) {
-    uint32_t j[CB_ILP], src[CB_ILP];
-    bool valid[CB_ILP];
-#pragma unroll
-    for (uint32_t u = 0; u < CB_ILP; ++u) {
-      const uint32_t k = i + 32 * u + lane;
-      valid[u] = k < d;
-      src[u] = 0;
-      if (valid[u]) {
-        uint32_t t = in_tgt[b0 + k];
-        if (CHECK && t >= n) t = 0;  // reported by the chunk's id check; keep the lookups in range meanwhile
-        src[u] = new_id[t];
-      }
-    }
-#pragma unroll
-    for (uint32_t u = 0; u < CB_ILP; ++u) j[u] = valid[u] ? hot_of_blk[src[u] / B] : CB_NONE;
-#pragma unroll
-    for (uint32_t u = 0; u < CB_ILP; ++u)
-      if (j[u] != CB_NONE && l >= nrows[j[u]]) j[u] = CB_NONE;
-#pragma unroll
-    for (uint32_t u = 0; u < CB_ILP; ++u) {
-      const bool cb = j[u] != CB_NONE;
-      const uint32_t peers = __match_any_sync(0xFFFFFFFFu, j[u]);
-      const uint32_t leader = (uint32_t)__ffs(peers) - 1u;
-      uint32_t base = 0, local = 0;
-      if (cb) {
-        local = src[u] - blk[j[u]] * B;
-        if (lane == leader) base = atomicAdd(cnt + poff[j[u]] + l, (uint32_t)__popc(peers));
-      }
-      base = __shfl_sync(0xFFFFFFFFu, base, leader);  // also orders this batch's counter update before the next
-      const uint32_t rb = __ballot_sync(0xFFFFFFFFu, valid[u] && !cb);
-      if (cb) {
-        rec[b0 + i + 32 * u + lane] = make_uint2(local | (j[u] << 16), CB_REC_SEG | (base + __popc(peers & ((1u << lane) - 1u))));
-      } else if (valid[u]) {
-        rec[b0 + i + 32 * u + lane] = make_uint2(src[u], rem + __popc(rb & ((1u << lane) - 1u)));
-      }
-      rem += __popc(rb);
-    }
-  }
-  return rem;
-}
-// rows in internal order (the whole in-CSR is resident): one warp per local row
-__global__ void k_cb_count(const uint32_t* __restrict__ in_off, const uint32_t* __restrict__ in_tgt,
-                           const uint32_t* __restrict__ old_of, const uint32_t* __restrict__ new_id,
-                           const uint32_t* __restrict__ hot_of_blk, const uint32_t* __restrict__ nrows,
-                           const uint32_t* __restrict__ poff, const uint32_t* __restrict__ blk, uint32_t B,
-                           uint32_t row0, uint32_t n_cb, PrDeal deal, uint32_t* __restrict__ cnt,
-                           uint2* __restrict__ rec, uint32_t* __restrict__ lens,
-                           unsigned long long* __restrict__ cb_edges) {
-  const uint32_t lane = threadIdx.x & 31;
-  const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
-  unsigned long long in_cb = 0;
-  for (uint32_t l = row0 + warp; l < n_cb; l += nwarps) {
-    const uint32_t old = old_of[deal_global(l, deal.P, deal.p)];
-    const uint32_t b0 = in_off[old], d = in_off[old + 1] - b0;
-    const uint32_t rem = cb_classify_row<false>(l, b0, d, 0u, in_tgt, new_id, hot_of_blk, nrows, poff, blk, B, cnt, rec, lane);
-    if (lane == 0) {
-      lens[l] = rem;
-      in_cb += d - rem;
-    }
-  }
-  if (lane == 0 && in_cb) atomicAdd(cb_edges, in_cb);
-}
-// rows [v0, v1) in ORIGINAL order (a chunk of the in-CSR that has just arrived over PCIe): a warp takes
-// 32 consecutive rows, keeps those that are local and own segments, and walks them one after the other
-__global__ void k_cb_count_rows(const uint32_t* __restrict__ in_off, const uint32_t* __restrict__ in_tgt,
-                                const uint32_t* __restrict__ new_id, const uint32_t* __restrict__ hot_of_blk,
-                                const uint32_t* __restrict__ nrows, const uint32_t* __restrict__ poff,
-                                const uint32_t* __restrict__ blk, uint32_t B, uint32_t v0, uint32_t v1, uint32_t n,
-                                uint32_t row0, uint32_t n_cb, PrDeal deal, uint32_t* __restrict__ cnt,
-                                uint2* __restrict__ rec, uint32_t* __restrict__ lens,
-                                unsigned long long* __restrict__ cb_edges) {
-  const uint32_t lane = threadIdx.x & 31;
-  const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
-  unsigned long long in_cb = 0;
-  for (uint64_t base = (uint64_t)v0 + 32ull * warp; base < v1; base += 32ull * nwarps) {
-    const uint64_t v = base + lane;
-    uint32_t l = CB_NONE, b0 = 0, d = 0;
-    if (v < v1) {
-      const uint32_t gid = new_id[v], slice = gid >> 5;
-      if (slice % deal.P == deal.p) {
-        const uint32_t loc = ((slice / deal.P) << 5) | (gid & 31u);
-        if (loc >= row0 && loc < n_cb) {
-          l = loc;
-          b0 = in_off[v];
-          d = in_off[v + 1] - b0;
-        }
-      }
-    }
-    uint32_t todo = __ballot_sync(0xFFFFFFFFu, l != CB_NONE);
-    while (todo) {
-      const int src_lane = __ffs(todo) - 1;
-      todo &= todo - 1;
-      const uint32_t rl = __shfl_sync(0xFFFFFFFFu, l, src_lane);
-      const uint32_t rb = __shfl_sync(0xFFFFFFFFu, b0, src_lane);
-      const uint32_t rd = __shfl_sync(0xFFFFFFFFu, d, src_lane);
-      const uint32_t rem = cb_classify_row<true>(rl, rb, rd, n, in_tgt, new_id, hot_of_blk, nrows, poff, blk, B, cnt, rec, lane);
-      if (lane == 0) {
-        lens[rl] = rem;
-        in_cb += rd - rem;
-      }
-    }
-  }
-  if (lane == 0 && in_cb) atomicAdd(cb_edges, in_cb);
-}
-// ---- the longest rows (a prefix of the local rows) go through ONE stable radix sort -----------------
-// A row's warp walks it 128 edges at a time, ~3 us per step: a million-edge hub would take tens of
-// milliseconds on its own.  Its edges are instead keyed (row << 14 | block rank), sorted stably — so
-// the edges of one (row, block) pair end up contiguous AND in CSR order — and counted / placed from the
-// sorted sequence, one thread per edge.
-__global__ void k_mega_deg(const uint32_t* __restrict__ indeg, uint32_t n_mega, PrDeal deal, uint32_t* __restrict__ out) {
-  for (uint32_t l = blockIdx.x * blockDim.x + threadIdx.x; l < n_mega; l += gridDim.x * blockDim.x)
-    out[l] = indeg[deal_global(l, deal.P, deal.p)];
-}
-__global__ void k_mega_keys(const uint32_t* __restrict__ in_off, const uint32_t* __restrict__ in_tgt,
-                            const uint32_t* __restrict__ old_of, const uint32_t* __restrict__ new_id,
-                            const uint32_t* __restrict__ hot_of_blk, const uint32_t* __restrict__ nrows, uint32_t B,
-                            const uint32_t* __restrict__ moff, uint32_t n_mega, uint32_t M, PrDeal deal,
-                            uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < M; i += gridDim.x * blockDim.x) {
-    uint32_t lo = 0, hi = n_mega;  // row with moff[row] <= i < moff[row + 1]
-    while (hi - lo > 1) {
-      const uint32_t mid = (lo + hi) / 2;
-      if (moff[mid] <= i) lo = mid;
-      else hi = mid;
-    }
-    const uint32_t l = lo;
-    const uint32_t old = old_of[deal_global(l, deal.P, deal.p)];
-    const uint32_t src = new_id[in_tgt[in_off[old] + (i - moff[l])]];
-    uint32_t j = hot_of_blk[src / B];
-    if (j != CB_NONE && l >= nrows[j]) j = CB_NONE;
-    keys[i] = (l << CB_MEGA_JBITS) | (j == CB_NONE ? (1u << CB_MEGA_JBITS) - 1u : j);
-    vals[i] = src;
-  }
-}
-__global__ void k_mega_starts(const uint32_t* __restrict__ keys, uint32_t M, uint32_t* __restrict__ start) {
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < M; i += gridDim.x * blockDim.x)
-    start[i] = (i == 0 || keys[i] != keys[i - 1]) ? i : 0u;  // max-scanned into "first index of my run"
-}
-__global__ void k_mega_counts(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ start, uint32_t M,
-                              const uint32_t* __restrict__ poff, uint32_t* __restrict__ cnt,
-                              uint32_t* __restrict__ lens, unsigned long long* __restrict__ cb_edges) {
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < M; i += gridDim.x * blockDim.x) {
-    if (i + 1 < M && keys[i + 1] == keys[i]) continue;  // not the last edge of its run
-    const uint32_t len = i + 1 - start[i];
-    const uint32_t l = keys[i] >> CB_MEGA_JBITS, j = keys[i] & ((1u << CB_MEGA_JBITS) - 1u);
-    if (j == (1u << CB_MEGA_JBITS) - 1u) {
-      lens[l] = len;
-    } else {
-      cnt[poff[j] + l] = len;
-      atomicAdd(cb_edges, (unsigned long long)len);
-    }
-  }
-}
-__global__ void k_mega_fill(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ vals,
-                            const uint32_t* __restrict__ start, uint32_t M, const uint32_t* __restrict__ poff,
-                            const uint32_t* __restrict__ blk, uint32_t B, const uint32_t* __restrict__ goff,
-                            uint16_t* __restrict__ ids, const uint2* __restrict__ slice_meta,
-                            uint32_t* __restrict__ sell) {
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < M; i += gridDim.x * blockDim.x) {
-    const uint32_t pos = i - start[i];
-    const uint32_t l = keys[i] >> CB_MEGA_JBITS, j = keys[i] & ((1u << CB_MEGA_JBITS) - 1u);
-    if (j == (1u << CB_MEGA_JBITS) - 1u) {
-      const uint2 meta = slice_meta[l >> 5];
-      sell[((uint64_t)meta.x + (uint64_t)(pos / 4) * 32 + (l & 31u)) * 4 + (pos % 4)] = vals[i];
-    } else {
-      ids[(uint64_t)goff[poff[j] + l] * CB_G + pos] = (uint16_t)(vals[i] - blk[j] * B);
-    }
-  }
-}
-__global__ void k_lens_tail(const uint32_t* __restrict__ indeg, uint32_t n_cb, uint32_t n_loc, PrDeal deal,
-                            uint32_t* __restrict__ lens) {
-  for (uint32_t l = n_cb + blockIdx.x * blockDim.x + threadIdx.x; l < n_loc; l += gridDim.x * blockDim.x)
-    lens[l] = indeg[deal_global(l, deal.P, deal.p)];
-}
-__global__ void k_loc_edges(const uint32_t* __restrict__ indeg, uint32_t n_loc, PrDeal deal,
-                            unsigned long long* __restrict__ total) {
-  unsigned long long s = 0;
-  for (uint32_t l = blockIdx.x * blockDim.x + threadIdx.x; l < n_loc; l += gridDim.x * blockDim.x)
-    s += indeg[deal_global(l, deal.P, deal.p)];
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, o);
-  if ((threadIdx.x & 31) == 0 && s) atomicAdd(total, s);
-}
-// edges of a pair -> groups of its segment (every pair of the staircase keeps at least one group, so
-// that the row of a group follows from counting segment starts)
-__global__ void k_cb_groups(uint32_t* __restrict__ cnt, uint64_t S) {
-  for (uint64_t e = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; e < S; e += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t c = cnt[e];
-    cnt[e] = c ? (c + CB_G - 1) / CB_G : 1u;
-  }
-}
-__global__ void k_fill_u2(uint2* __restrict__ a, uint64_t count, uint2 v) {
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count; i += (uint64_t)gridDim.x * blockDim.x)
-    a[i] = v;
-}
-__global__ void k_cb_bits(const uint32_t* __restrict__ goff, uint64_t S, uint32_t* __restrict__ bits) {
-  for (uint64_t e = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; e < S; e += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t g = goff[e];
-    atomicOr(bits + (g >> 5), 1u << (g & 31u));
-  }
-}
-// SELL slice widths: the longest lane of the slice, in 4-edge groups
-__global__ void k_sell_widths(const uint32_t* __restrict__ lens, uint32_t n_loc, uint32_t num_slices,
-                              uint32_t* __restrict__ units) {
-  const uint32_t lane = threadIdx.x & 31;
-  const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
-  for (uint32_t sidx = warp; sidx < num_slices; sidx += nwarps) {
-    const uint32_t l = 32 * sidx + lane;
-    const uint32_t w = warp_max(l < n_loc ? lens[l] : 0u);
-    if (lane == 0) units[sidx] = ((w + 3) / 4) * 32;  // uint4 entries of the slice
-  }
-}
-__global__ void k_sell_meta(const uint32_t* __restrict__ units, const uint32_t* __restrict__ bases,
-                            uint32_t num_slices, uint2* __restrict__ meta) {
-  for (uint32_t sidx = blockIdx.x * blockDim.x + threadIdx.x; sidx < num_slices; sidx += gridDim.x * blockDim.x)
-    meta[sidx] = make_uint2(bases[sidx], units[sidx] / 32);
-}
-// after the scan over the segment sizes: scatter the records left by the classification — block-local
-// ids into the segments, all other sources into the row's SELL lane
-__global__ void k_cb_fill(const uint32_t* __restrict__ in_off, const uint32_t* __restrict__ old_of,
-                          const uint2* __restrict__ rec, const uint32_t* __restrict__ poff, uint32_t row0,
-                          uint32_t n_cb, PrDeal deal, const uint32_t* __restrict__ goff, uint16_t* __restrict__ ids,
-                          const uint2* __restrict__ slice_meta, uint32_t* __restrict__ sell) {
-  const uint32_t lane = threadIdx.x & 31;
-  const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
-  for (uint32_t l = row0 + warp; l < n_cb; l += nwarps) {
-    const uint32_t old = old_of[deal_global(l, deal.P, deal.p)];
-    const uint32_t b0 = in_off[old], d = in_off[old + 1] - b0;
-    const uint2 meta = slice_meta[l >> 5];
-    for (uint32_t i = 0; i < d; i += 32 * CB_ILP) {
-      uint2 r[CB_ILP];
-      uint32_t g0[CB_ILP];
-#pragma unroll
-      for (uint32_t u = 0; u < CB_ILP; ++u) {
-        const uint32_t k = i + 32 * u + lane;
-        r[u] = k < d ? rec[b0 + k] : make_uint2(0u, 0xFFFFFFFFu);
-      }
-#pragma unroll
-      for (uint32_t u = 0; u < CB_ILP; ++u)
-        g0[u] = (r[u].y != 0xFFFFFFFFu && (r[u].y & CB_REC_SEG)) ? goff[poff[r[u].x >> 16] + l] : 0u;
-#pragma unroll
-      for (uint32_t u = 0; u < CB_ILP; ++u) {
-        if (r[u].y == 0xFFFFFFFFu) continue;
-        if (r[u].y & CB_REC_SEG) {
-          ids[(uint64_t)g0[u] * CB_G + (r[u].y & ~CB_REC_SEG)] = (uint16_t)(r[u].x & 0xFFFFu);
-        } else {
-          const uint32_t q = r[u].y;
-          sell[((uint64_t)meta.x + (uint64_t)(q / 4) * 32 + (l & 31u)) * 4 + (q % 4)] = r[u].x;
-        }
-      }
-    }
-  }
-}
-// rows without segments: the whole row goes to its SELL lane (one lane per row)
-__global__ void k_sell_fill_tail(const uint32_t* __restrict__ in_off, const uint32_t* __restrict__ in_tgt,
-                                 const uint32_t* __restrict__ old_of, const uint32_t* __restrict__ new_id,
-                                 uint32_t n_cb, uint32_t n_loc, PrDeal deal, uint32_t num_slices,
-                                 const uint2* __restrict__ meta, uint4* __restrict__ sell) {
-  const uint32_t lane = threadIdx.x & 31;
-  const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
-  for (uint32_t sidx = n_cb / 32 + warp; sidx < num_slices; sidx += nwarps) {
-    const uint2 m = meta[sidx];
-    const uint32_t l = 32 * sidx + lane;
-    if (l < n_cb) continue;  // filled by k_cb_fill (lanes of the boundary slice)
-    uint32_t b = 0, d = 0;
-    if (l < n_loc) {
-      const uint32_t old = old_of[deal_global(l, deal.P, deal.p)];
-      b = in_off[old];
-      d = in_off[old + 1] - b;
-    }
-    for (uint32_t q = 0; q * 4 < d; ++q) {
-      uint4 v = make_uint4(~0u, ~0u, ~0u, ~0u);
-      const uint32_t j = 4 * q;
-      if (j + 0 < d) v.x = new_id[in_tgt[b + j + 0]];
-      if (j + 1 < d) v.y = new_id[in_tgt[b + j + 1]];
-      if (j + 2 < d) v.z = new_id[in_tgt[b + j + 2]];
-      if (j + 3 < d) v.w = new_id[in_tgt[b + j + 3]];
-      sell[m.x + q * 32 + lane] = v;
-    }
-  }
-}
-__global__ void k_gather_u32(const uint32_t* __restrict__ src, const uint32_t* __restrict__ idx, uint32_t count,
-                             uint32_t* __restrict__ dst) {
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) dst[i] = src[idx[i]];
-}
-
-// Chunks: block j's stream [gbeg[j], gbeg[j+1]) is cut every C_j groups; a cut inside a segment moves to
-// the segment's end unless the segment is longer than C_j groups, in which case the cut stays and both
-// neighbours handle a PART of it (side buffer + fixup), so no warp ever owns more than 2 C_j groups.
-// C_j shrinks for thin blocks so that every block's stream is spread over all warps of a CTA (a lone
-// warp runs at its dependency latency, ~10x below the SM's throughput).
-struct CbCut {
-  uint32_t pos, row;
-  bool mid;
-};
-__device__ __forceinline__ CbCut cb_cut(const uint32_t* __restrict__ goff_j, uint32_t nr, uint32_t gend, uint32_t q,
-                                        uint32_t C) {
-  if (q >= gend) return CbCut{gend, nr, false};
-  uint32_t lo = 0, hi = nr;  // largest row with goff_j[row] <= q
-  while (hi - lo > 1) {
-    const uint32_t mid = lo + (hi - lo) / 2;
-    if (goff_j[mid] <= q) lo = mid;
-    else hi = mid;
-  }
-  const uint32_t s0 = goff_j[lo], s1 = (lo + 1 < nr) ? goff_j[lo + 1] : gend;
-  if (s0 == q) return CbCut{q, lo, false};
-  if (s1 - s0 > C) return CbCut{q, lo, true};
-  return CbCut{s1, lo + 1, false};
-}
-__global__ void k_cb_chunks(const uint32_t* __restrict__ goff, const uint32_t* __restrict__ poff,
-                            const uint32_t* __restrict__ nrows, const uint32_t* __restrict__ gbeg,
-                            const uint32_t* __restrict__ cfirst, const uint32_t* __restrict__ cgrp, uint32_t KB,
-                            uint32_t n_chunks, uint4* __restrict__ chunks, uint32_t* __restrict__ tail_slot,
-                            uint32_t* __restrict__ fix_list, uint32_t* __restrict__ n_fix /* [1] = largest cut row */) {
-  for (uint32_t c = blockIdx.x * blockDim.x + threadIdx.x; c < n_chunks; c += gridDim.x * blockDim.x) {
-    uint32_t lo = 0, hi = KB;  // block with cfirst[j] <= c < cfirst[j + 1]
-    while (hi - lo > 1) {
-      const uint32_t mid = lo + (hi - lo) / 2;
-      if (cfirst[mid] <= c) lo = mid;
-      else hi = mid;
-    }
-    const uint32_t j = lo, k = c - cfirst[j];
-    const uint32_t C = cgrp[j];  // groups per chunk in this block (thin blocks use small chunks)
-    const uint32_t* goff_j = goff + poff[j];
-    const uint32_t nr = nrows[j], g0 = gbeg[j], g1 = gbeg[j + 1];
-    const bool last = c + 1 == cfirst[j + 1];
-    const CbCut a = cb_cut(goff_j, nr, g1, g0 + k * C, C);
-    const CbCut b = last ? CbCut{g1, nr, false} : cb_cut(goff_j, nr, g1, g0 + (k + 1) * C, C);
-    uint32_t fl = 0;
-    if (a.mid) fl |= CB_HEAD_CONT;
-    if (b.mid) fl |= CB_TAIL_CONT;
-    const uint32_t last_row = b.mid ? b.row : b.row - 1;  // row of the chunk's last group
-    if (a.mid && last_row == a.row) fl |= CB_INTERIOR;
-    const uint32_t row_before = a.mid ? a.row : a.row - 1;
-    chunks[c] = make_uint4(a.pos, b.pos, row_before, j | (fl << 24));
-    tail_slot[c] = b.mid ? poff[j] + b.row : CB_NONE;
-    if (b.mid && !(fl & CB_INTERIOR)) {
-      fix_list[atomicAdd(n_fix, 1u)] = c;
-      atomicMax(n_fix + 1, b.row);
-    }
-  }
-}
-
-// Bank-aware order of the ids inside each group (tools/cb_bank_model.py restates it).  A step of k_pr_cb
-// reads a WINDOW of 32 G groups (G = 2, or 4 in chunks of at least CB_WIDE_MIN groups): lane L's groups
-// G L + i (i < G) feed its shared-memory reads 4i..4i+3, and each of those read instructions takes as many
-// wavefronts as its most crowded bank (id & 31) holds words.  The 4 ids of a group belong to one (row,
-// block) pair, so their order only changes the rounding of the group's sum.  One thread per SET i of a
-// window: lanes 0..31 in turn put the 4 ids of their group G L + i into the 4 read slots in the order (of
-// 24) that lands them on the least loaded banks so far; padding ids (all lanes read the same word, a
-// broadcast) are free.  A set keeps its old order unless the new one lowers the sum over its slots of the
-// largest bank count.  Windows are the kernel's steps: chunk c steps from g0 & ~1 by 32 G and reads groups
-// outside [g0, g1) as padding (they are ordered by their own chunk), so every group is ordered by exactly
-// one thread and the result does not depend on thread timing.
-constexpr int CB_BANK_THREADS = 128;
-__global__ void __launch_bounds__(CB_BANK_THREADS) k_cb_bank_order(const uint4* __restrict__ chunks, uint32_t n_chunks,
-                                                                   uint32_t B, uint2* __restrict__ ids) {
-  __shared__ uint8_t hist[4 * 32][CB_BANK_THREADS];  // [slot * 32 + bank][thread]: no two threads share a byte
-  uint8_t(*h)[CB_BANK_THREADS] = hist;
-  const uint32_t t = threadIdx.x, lane = t & 31;
-  const uint32_t warp = (blockIdx.x * blockDim.x + t) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
-  // the 24 orders, slot -> id index, two bits per slot; the identity first, so ties keep the old order
-  constexpr uint8_t perms[24] = {0xE4, 0xB4, 0xD8, 0x78, 0x9C, 0x6C, 0xE1, 0xB1, 0xC9, 0x39, 0x8D, 0x2D,
-                                 0xD2, 0x72, 0xC6, 0x36, 0x4E, 0x1E, 0x93, 0x63, 0x87, 0x27, 0x4B, 0x1B};
-  const auto clear = [&]() {
-    for (int i = 0; i < 4 * 32; ++i) h[i][t] = 0;
-  };
-  const auto bound = [&]() {  // sum over the slots of max(1, the largest bank count)
-    uint32_t tot = 0;
-    for (int s = 0; s < 4; ++s) {
-      uint32_t mx = 1;
-      for (int b = 0; b < 32; ++b) mx = max(mx, (uint32_t)h[s * 32 + b][t]);
-      tot += mx;
-    }
-    return tot;
-  };
-  uint2 out[32];
-  for (uint32_t c = warp; c < n_chunks; c += nwarps) {
-    const uint4 ch = chunks[c];
-    const uint32_t g0 = ch.x, g1 = ch.y;
-    if (g0 >= g1) continue;
-    const uint32_t G = g1 - g0 >= CB_WIDE_MIN ? 4u : 2u;  // groups per lane in the chunk's steps
-    const uint32_t set = lane % G;
-    for (uint32_t gw = (g0 & ~1u) + 32 * G * (lane / G); gw < g1; gw += 32 * 32) {
-      clear();
-      for (uint32_t L = 0; L < 32; ++L) {
-        const uint32_t g = gw + G * L + set;
-        if (g < g0 || g >= g1) continue;
-        const uint2 v = ids[g];
-        const uint32_t id[4] = {v.x & 0xFFFFu, v.x >> 16, v.y & 0xFFFFu, v.y >> 16};
-        for (int s = 0; s < 4; ++s)
-          if (id[s] != B) ++h[s * 32 + (id[s] & 31u)][t];
-      }
-      const uint32_t before = bound();
-      clear();
-      for (uint32_t L = 0; L < 32; ++L) {
-        const uint32_t g = gw + G * L + set;
-        if (g < g0 || g >= g1) continue;
-        const uint2 v = ids[g];
-        const uint32_t id[4] = {v.x & 0xFFFFu, v.x >> 16, v.y & 0xFFFFu, v.y >> 16};
-        uint32_t cost[4][4];  // [slot][id index]: load of the id's bank in that slot so far
-#pragma unroll
-        for (int s = 0; s < 4; ++s)
-#pragma unroll
-          for (int k = 0; k < 4; ++k) cost[s][k] = id[k] == B ? 0u : h[s * 32 + (id[k] & 31u)][t];
-        uint32_t best = 0, best_cost = 0xFFFFFFFFu;
-#pragma unroll
-        for (int p = 0; p < 24; ++p) {
-          uint32_t sum = 0;
-#pragma unroll
-          for (int s = 0; s < 4; ++s) sum += cost[s][(perms[p] >> (2 * s)) & 3u];
-          if (sum < best_cost) {
-            best_cost = sum;
-            best = perms[p];
-          }
-        }
-        uint32_t o[4];
-#pragma unroll
-        for (int s = 0; s < 4; ++s) {
-          const uint32_t k = (best >> (2 * s)) & 3u;
-          o[s] = k == 0 ? id[0] : k == 1 ? id[1] : k == 2 ? id[2] : id[3];
-          if (o[s] != B) ++h[s * 32 + (o[s] & 31u)][t];
-        }
-        out[L] = make_uint2(o[0] | (o[1] << 16), o[2] | (o[3] << 16));
-      }
-      if (bound() >= before) continue;
-      for (uint32_t L = 0; L < 32; ++L) {
-        const uint32_t g = gw + G * L + set;
-        if (g >= g0 && g < g1) ids[g] = out[L];
-      }
-    }
-  }
 }
 
 // ---- sweep kernels (JACOBI) ------------------------------------------------------------------
@@ -1058,8 +410,7 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
 // thin blocks are (a purely static split leaves thin blocks at single-warp latency, one global cursor reloads the
 // block for every task).  Claiming the next task one task ahead (to hide the atomic's
 // round trip) was measured and dropped: a claimed task cannot be stolen, which costs more at the tail.
-template <int NT>
-__device__ __forceinline__ void pr_cb_body(const PrArgs& a) {
+__global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
   extern __shared__ __align__(128) float smem[];
   float* xs = smem;  // B entries of x_cur + one zero slot (the pad id)
   __shared__ uint32_t s_task, s_next;
@@ -1110,7 +461,7 @@ __device__ __forceinline__ void pr_cb_body(const PrArgs& a) {
     }
     __syncthreads();  // also: every warp is done with the previous task's block
     const uint32_t t = s_task;
-    if (threadIdx.x == 0) s_next = NT / 32;  // every warp is past its last claim of the previous task
+    if (threadIdx.x == 0) s_next = PR_THREADS / 32;  // every warp is past its last claim of the previous task
     __syncthreads();
     if (t == CB_NONE) break;
     const uint2 task = a.tasks[t];  // (first chunk, chunk count | block rank << 8)
@@ -1130,7 +481,7 @@ __device__ __forceinline__ void pr_cb_body(const PrArgs& a) {
         mbar_wait(mbar, phase);
         phase ^= 1u;
       } else {
-        for (uint32_t i = threadIdx.x; i < cnt; i += NT) xs[i] = a.x_cur[x0 + i];
+        for (uint32_t i = threadIdx.x; i < cnt; i += PR_THREADS) xs[i] = a.x_cur[x0 + i];
       }
       cur_j = j;
       __syncthreads();
@@ -1141,14 +492,10 @@ __device__ __forceinline__ void pr_cb_body(const PrArgs& a) {
       cb_chunk(a, xs, task.x + k, lane, pad2);
       uint32_t nx = 0;
       if (lane == 0) nx = atomicAdd(&s_next, 1u);
-      k = (a.dbg & 2u) ? k + NT / 32 : __shfl_sync(0xFFFFFFFFu, nx, 0);
+      k = (a.dbg & 2u) ? k + PR_THREADS / 32 : __shfl_sync(0xFFFFFFFFu, nx, 0);
     }
   }
 }
-__global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) { pr_cb_body<PR_THREADS>(a); }
-// dual mode: 512 threads and at most 56 registers, so that a 512-thread k_pr_sell CTA (64 registers)
-// fits beside it on the SM
-__global__ void __maxnreg__(56) k_pr_cb_half(const PrArgs a) { pr_cb_body<PR_THREADS / 2>(a); }
 
 // Segments cut by chunk boundaries (segments longer than a chunk): one warp per segment adds its parts
 // in a fixed order — the head part of the first chunk, then lanes over the following chunks (a fixed
@@ -1179,8 +526,7 @@ __global__ void k_pr_fixup(const PrArgs a) {
 // lane-minor), gathers, and adds in row order.  The next slice's first targets and row metadata are
 // requested while the current slice is processed.  Rows below n_cb only hold the edges that are not in
 // a column-block segment: their sum goes to rem[] and the finish kernel completes them.
-// The kernel needs no shared memory: two 512-thread CTAs per SM when it runs alone, one beside a
-// k_pr_cb_half CTA in dual mode.
+// The kernel needs no shared memory: two 512-thread CTAs per SM.
 template <bool PEERS>
 __global__ void __launch_bounds__(PR_SELL_THREADS, 2) k_pr_sell(const PrArgs a) {
   constexpr int NT = PR_SELL_THREADS;
@@ -1291,20 +637,6 @@ __global__ void __launch_bounds__(PR_SELL_THREADS, 2) k_pr_sell(const PrArgs a) 
   }
 }
 
-// ---- finish: rows with segments = partials of their blocks (fixed order, f64) + SELL remainder -----
-// 32-row groups that own segments in more than FIN_CTA_BLOCKS blocks (the hubs: a prefix) get a CTA
-// each; all other rows one lane each (coalesced across the warp's 32 rows).  The last CTA to
-// finish reduces all CTA error partials in a fixed order and evaluates the stop rule of
-// page_rank.rs:107 on the device.
-__host__ __device__ __forceinline__ uint32_t fin_blocks_of(const uint32_t* __restrict__ nrows, uint32_t KB, uint32_t l) {
-  uint32_t lo = 0, hi = KB;  // first j with nrows[j] <= l  (nrows is non-increasing)
-  while (lo < hi) {
-    const uint32_t mid = (lo + hi) / 2;
-    if (nrows[mid] > l) lo = mid + 1;
-    else hi = mid;
-  }
-  return lo;
-}
 // FIN_U = 32-row groups per warp iteration of the rows that are not hub groups: 2 (and 16 blocks' partials
 // in flight) when every warp has a single iteration to do — the walk is a latency chain, fewer rounds win;
 // 4 (4 blocks in flight) when the grid is capped and the kernel is throughput bound (RMAT-26 on one GPU).
@@ -1527,471 +859,54 @@ __global__ void __launch_bounds__(32) k_pr_exact(const uint32_t* __restrict__ in
   }
 }
 
-// ---- plan ------------------------------------------------------------------------------------
-template <typename T>
-static gb_status scan_exclusive(cudaStream_t s, T* data, uint64_t count) {
-  GB_REQUIRE(count < (1ull << 31), "scan of %llu items is too long", (unsigned long long)count);
-  size_t tb = 0;
-  GB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, data, data, (int)count, s));
-  DevBuf<uint8_t> tmp;
-  GB_TRY(tmp.alloc(tb));
-  GB_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, data, data, (int)count, s));
-  GB_CUDA(cudaStreamSynchronize(s));
-  return GB_OK;
-}
-template <typename T>
-static gb_status upload(cudaStream_t s, DevBuf<T>* dst, const std::vector<T>& src, size_t pad = 0) {
-  GB_TRY(dst->alloc(std::max<size_t>(src.size(), 1), pad));
-  if (!src.empty()) GB_CUDA(cudaMemcpyAsync(dst->p, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice, s));
-  GB_CUDA(cudaStreamSynchronize(s));  // src may be a temporary
-  return GB_OK;
-}
-static uint32_t env_u32(const char* name, uint32_t dflt) {
-  const char* e = getenv(name);
-  return e && *e ? (uint32_t)strtoul(e, nullptr, 10) : dflt;
-}
-
-static gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan) {
-  cudaStream_t s = g->stream;
-  const uint32_t n = g->n;
-  const uint64_t m = g->in.len;
-  GB_REQUIRE(deal.P >= 1 && deal.p < deal.P, "bad shard %u of %u", deal.p, deal.P);
-  PrPlan* p = new (std::nothrow) PrPlan();
-  if (!p) return fail(GB_ERR_OOM, "host allocation failed");
-  p->n = n;
-  p->m = m;
-  p->deal = deal;
-  // every temporary below is used on s only: releasing one waits for s, not for the device (a copy
-  // stream may still be bringing in the targets, see TargetFeed)
-  DevBufStreamScope scope(s);
-  const TargetFeed* feed = g->feed;
-  gb_status st = [&]() -> gb_status {
-    int dev_sms = H100_SMS;
-    GB_CUDA(cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, g->device));
-    // knobs (experiments; defaults are the measured optima)
-    uint32_t B = env_u32("GB_PR_BLOCK", CB_BLOCK_DEFAULT);
-    B = std::min<uint32_t>(std::max<uint32_t>(B & ~1023u, 1024u), CB_BLOCK_MAX);
-    double tau = CB_TAU_DEFAULT;
-    if (const char* e = getenv("GB_PR_TAU")) tau = atof(e);
-    if (!(tau > 0.0)) tau = 1e30;  // tau <= 0 switches the column blocks off
-    p->B = B;
-    // 1. permutation: in-degree descending, then out-degree descending, then id
-    DevBuf<uint32_t> old_of;  // internal id -> original id (plan-time only)
-    DevBuf<uint32_t> indeg;   // in-degree by internal id (plan-time only)
-    {
-      DevBuf<uint64_t> keys, keys_alt;
-      DevBuf<uint32_t> ids, ids_alt;
-      GB_TRY(keys.alloc(n));
-      GB_TRY(keys_alt.alloc(n));
-      GB_TRY(ids.alloc(n));
-      GB_TRY(ids_alt.alloc(n));
-      k_perm_keys<<<grid_for(n, 256), 256, 0, s>>>(g->in.off.p, g->out.off.p, n, keys.p, ids.p);
-      cub::DoubleBuffer<uint64_t> kb(keys.p, keys_alt.p);
-      cub::DoubleBuffer<uint32_t> vb(ids.p, ids_alt.p);
-      size_t tb = 0;
-      GB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, kb, vb, (int)n, 0, 64, s));
-      DevBuf<uint8_t> tmp;
-      GB_TRY(tmp.alloc(tb));
-      GB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, kb, vb, (int)n, 0, 64, s));
-      GB_TRY(p->new_id.alloc(n));
-      GB_TRY(p->outdeg.alloc(n));
-      GB_TRY(indeg.alloc((size_t)n + 1));
-      k_perm_scatter<<<grid_for(n, 256), 256, 0, s>>>(vb.Current(), g->out.off.p, g->in.off.p, n, p->new_id.p,
-                                                     p->outdeg.p, indeg.p);
-      GB_TRY(old_of.alloc(n));
-      GB_CUDA(cudaMemcpyAsync(old_of.p, vb.Current(), (size_t)n * 4, cudaMemcpyDeviceToDevice, s));
-      GB_CUDA(cudaGetLastError());
-      GB_CUDA(cudaStreamSynchronize(s));
-    }
-    // 2. active rows (a prefix of the internal order) and this rank's share of them
-    DevBuf<unsigned long long> counters;  // [0] active rows, [1] local edges, [2] edges in segments, [3] fix count
-    GB_TRY(counters.alloc(4));
-    GB_CUDA(cudaMemsetAsync(counters.p, 0, 32, s));
-    k_count_active<<<grid_for(n, 256), 256, 0, s>>>(indeg.p, n, reinterpret_cast<uint32_t*>(counters.p));
-    {
-      unsigned long long h = 0;
-      GB_CUDA(cudaMemcpyAsync(&h, counters.p, 8, cudaMemcpyDeviceToHost, s));
-      GB_CUDA(cudaStreamSynchronize(s));
-      p->n_active = (uint32_t)h;
-    }
-    p->n_loc = deal_count(p->n_active, deal.P, deal.p);
-    if (p->n_loc) k_loc_edges<<<grid_for(p->n_loc, 256), 256, 0, s>>>(indeg.p, p->n_loc, deal, counters.p + 1);
-    // 3. hot blocks: block b carries the share e_b / m of all gathers; a row of in-degree d expects
-    //    d * e_b / m edges from it, and gets a segment when that is at least tau
-    const uint32_t nblk = (uint32_t)(((uint64_t)n + B - 1) / B);
-    uint32_t n_mega = 0;  // local rows [0, n_mega) are long enough for the sort path of the build
-    std::vector<uint32_t> h_hot(nblk, CB_NONE), h_blk, h_nrows, h_poff;
-    if (p->n_loc && m) {
-      DevBuf<unsigned long long> blk_edges, deg_prefix, edges_ge;
-      DevBuf<uint32_t> dmin, rows_ge;
-      GB_TRY(blk_edges.alloc(nblk));
-      GB_TRY(dmin.alloc(nblk + 1));  // + one probe: the rows long enough for the sort path of the build
-      GB_TRY(rows_ge.alloc(nblk + 1));
-      GB_TRY(edges_ge.alloc(nblk + 1));
-      GB_TRY(deg_prefix.alloc(std::max<uint32_t>(p->n_active, 1)));
-      {
-        cub::TransformInputIterator<unsigned long long, U32ToU64, const uint32_t*> it(indeg.p, U32ToU64());
-        size_t tb = 0;
-        GB_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, it, deg_prefix.p, (int)p->n_active, s));
-        DevBuf<uint8_t> tmp;
-        GB_TRY(tmp.alloc(tb));
-        GB_CUDA(cub::DeviceScan::InclusiveSum(tmp.p, tb, it, deg_prefix.p, (int)p->n_active, s));
-        GB_CUDA(cudaStreamSynchronize(s));
-      }
-      k_blk_edges<<<nblk, 256, 0, s>>>(p->outdeg.p, n, B, blk_edges.p);
-      std::vector<unsigned long long> h_edges(nblk);
-      GB_CUDA(cudaMemcpyAsync(h_edges.data(), blk_edges.p, (size_t)nblk * 8, cudaMemcpyDeviceToHost, s));
-      GB_CUDA(cudaStreamSynchronize(s));
-      std::vector<uint32_t> h_dmin(nblk + 1, 0xFFFFFFFFu);
-      h_dmin[nblk] = env_u32("GB_PR_MEGA", CB_MEGA_DEG) + 1;
-      for (uint32_t b = 0; b < nblk; ++b)
-        if (h_edges[b]) {
-          const double d = std::ceil(tau * (double)m / (double)h_edges[b]);
-          h_dmin[b] = d >= 4294967295.0 ? 0xFFFFFFFFu : std::max<uint32_t>(1u, (uint32_t)d);
-        }
-      GB_CUDA(cudaMemcpyAsync(dmin.p, h_dmin.data(), (size_t)(nblk + 1) * 4, cudaMemcpyHostToDevice, s));
-      k_rows_ge<<<grid_for(nblk + 1, 128), 128, 0, s>>>(indeg.p, deg_prefix.p, p->n_active, dmin.p, nblk + 1, rows_ge.p,
-                                                         edges_ge.p);
-      std::vector<uint32_t> h_rows(nblk + 1);
-      std::vector<unsigned long long> h_ege(nblk + 1);
-      GB_CUDA(cudaMemcpyAsync(h_rows.data(), rows_ge.p, (size_t)(nblk + 1) * 4, cudaMemcpyDeviceToHost, s));
-      GB_CUDA(cudaMemcpyAsync(h_ege.data(), edges_ge.p, (size_t)(nblk + 1) * 8, cudaMemcpyDeviceToHost, s));
-      GB_CUDA(cudaStreamSynchronize(s));
-      n_mega = deal_count(h_rows[nblk], deal.P, deal.p);
-      // GB_PR_MIN_BLOCK (experiment): drop blocks whose segments are expected to hold fewer ids than this
-      // (this shard's share of: in-edges of the qualifying rows x the block's share of all gathers).
-      // Default 0: a thin block costs one block load (~2 us on one SM), while its ids would otherwise
-      // lengthen the SELL lanes of the hub rows, which one lane walks serially.
-      double min_ids = 0.0;
-      if (const char* e = getenv("GB_PR_MIN_BLOCK")) min_ids = atof(e);
-      std::vector<uint32_t> order;
-      for (uint32_t b = 0; b < nblk; ++b) {
-        if (h_dmin[b] == 0xFFFFFFFFu || deal_count(h_rows[b], deal.P, deal.p) == 0) continue;
-        const double expect = (double)h_ege[b] * ((double)h_edges[b] / (double)m) / (double)deal.P;
-        if (expect >= min_ids) order.push_back(b);
-      }
-      std::sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) {
-        return h_rows[x] != h_rows[y] ? h_rows[x] > h_rows[y] : x < y;
-      });
-      if (order.size() > CB_MAX_BLOCKS) order.resize(CB_MAX_BLOCKS);
-      uint64_t S = 0;
-      for (uint32_t j = 0; j < order.size(); ++j) {
-        const uint32_t b = order[j];
-        h_hot[b] = j;
-        h_blk.push_back(b);
-        h_nrows.push_back(deal_count(h_rows[b], deal.P, deal.p));
-        h_poff.push_back((uint32_t)S);
-        S += h_nrows.back();
-        GB_REQUIRE(S < 0xFFFFFFF0ull, "column-block staircase too large (%llu pairs)", (unsigned long long)S);
-      }
-      h_poff.push_back((uint32_t)S);
-      p->S = S;
-    }
-    p->KB = (uint32_t)h_blk.size();
-    if (p->KB) p->last_hot_block = *std::max_element(h_blk.begin(), h_blk.end());
-    p->n_cb = p->KB ? h_nrows[0] : 0;
-    if (h_poff.empty()) h_poff.push_back(0);
-    DevBuf<uint32_t> hot_of_blk;
-    GB_TRY(upload(s, &hot_of_blk, h_hot));
-    GB_TRY(upload(s, &p->blk, h_blk));
-    GB_TRY(upload(s, &p->nrows, h_nrows));
-    GB_TRY(upload(s, &p->poff, h_poff));
-    // 4. segment sizes (pairs of the staircase) and SELL lane lengths
-    DevBuf<uint32_t> goff;  // [S + 1] edges per pair -> groups per pair -> first group of each pair
-    DevBuf<uint32_t> lens;  // [n_loc] SELL lane lengths
-    GB_TRY(goff.alloc(p->S + 1));
-    GB_CUDA(cudaMemsetAsync(goff.p, 0, (p->S + 1) * 4, s));
-    GB_TRY(lens.alloc(std::max<uint32_t>(p->n_loc, 1)));
-    // the longest rows: key, sort, count from the sorted sequence (kept for the fill pass below)
-    n_mega = std::min(n_mega, std::min(p->n_cb, (1u << (32 - CB_MEGA_JBITS)) - 1u));
-    if (p->KB >= (1u << CB_MEGA_JBITS) - 1u) n_mega = 0;
-    DevBuf<uint32_t> mega_keys, mega_vals, mega_start, mega_off;
-    uint32_t M = 0;
-    if (n_mega) {
-      DevBuf<uint32_t> mdeg;
-      GB_TRY(mdeg.alloc(n_mega));
-      k_mega_deg<<<grid_for(n_mega, 128), 128, 0, s>>>(indeg.p, n_mega, deal, mdeg.p);
-      std::vector<uint32_t> h_moff(n_mega + 1, 0);
-      GB_CUDA(cudaMemcpyAsync(h_moff.data() + 1, mdeg.p, (size_t)n_mega * 4, cudaMemcpyDeviceToHost, s));
-      GB_CUDA(cudaStreamSynchronize(s));
-      uint64_t acc = 0;
-      for (uint32_t r = 0; r < n_mega; ++r) {
-        acc += h_moff[r + 1];
-        if (acc >= 0xFFFFFFF0ull) {  // more mega edges than a 32-bit sort index holds: shorten the prefix
-          n_mega = r;
-          acc -= h_moff[r + 1];
-          break;
-        }
-        h_moff[r + 1] = (uint32_t)acc;
-      }
-      h_moff.resize(n_mega + 1);
-      M = n_mega ? h_moff[n_mega] : 0;
-      if (M) GB_TRY(upload(s, &mega_off, h_moff));
-      else n_mega = 0;
-    }
-    p->n_mega = n_mega;
-    // all other rows that own segments: one record per in-edge (consumed by the fill pass)
-    DevBuf<uint2> rec;
-    if (p->n_cb > n_mega) {
-      uint32_t dmax = 0;  // a record holds a 31-bit position
-      GB_CUDA(cudaMemcpyAsync(&dmax, indeg.p + deal_global(n_mega, deal.P, deal.p), 4, cudaMemcpyDeviceToHost, s));
-      GB_CUDA(cudaStreamSynchronize(s));
-      GB_REQUIRE(dmax < 0x7FFFFFFFu, "a row with %u in-edges outside the sort path of the layout build", dmax);
-      GB_TRY(rec.alloc(std::max<uint64_t>(m, 1)));
-    }
-    if (feed) {
-      // the targets arrive chunk by chunk: check and classify each chunk as soon as it is there
-      DevBuf<unsigned int> bad;
-      GB_TRY(bad.alloc(1));
-      GB_CUDA(cudaMemsetAsync(bad.p, 0, 4, s));
-      for (size_t k = 0; k + 1 < feed->row_begin.size(); ++k) {
-        const uint32_t v0 = feed->row_begin[k], v1 = feed->row_begin[k + 1];
-        const uint64_t e0 = feed->edge_begin[k], e1 = feed->edge_begin[k + 1];
-        GB_CUDA(cudaStreamWaitEvent(s, feed->ready[k], 0));
-        check_ids_async(s, g->in.tgt.p + e0, e1 - e0, n, bad.p);
-        if (p->n_cb > n_mega && v1 > v0)
-          k_cb_count_rows<<<grid_for((uint64_t)(v1 - v0), 256), 256, 0, s>>>(
-              g->in.off.p, g->in.tgt.p, p->new_id.p, hot_of_blk.p, p->nrows.p, p->poff.p, p->blk.p, B, v0, v1, n, n_mega,
-              p->n_cb, deal, goff.p, rec.p, lens.p, counters.p + 2);
-      }
-      unsigned int nbad = 0;
-      GB_CUDA(cudaGetLastError());
-      GB_CUDA(cudaMemcpyAsync(&nbad, bad.p, 4, cudaMemcpyDeviceToHost, s));
-      GB_CUDA(cudaStreamSynchronize(s));
-      GB_REQUIRE(nbad == 0, "in CSR holds %u targets >= node_count %u", nbad, n);
-    } else if (p->n_cb > n_mega) {
-      k_cb_count<<<grid_for((uint64_t)(p->n_cb - n_mega) * 32, 256), 256, 0, s>>>(
-          g->in.off.p, g->in.tgt.p, old_of.p, p->new_id.p, hot_of_blk.p, p->nrows.p, p->poff.p, p->blk.p, B, n_mega,
-          p->n_cb, deal, goff.p, rec.p, lens.p, counters.p + 2);
-    }
-    if (M) {
-      DevBuf<uint32_t> keys_in, vals_in;
-      GB_TRY(keys_in.alloc(M));
-      GB_TRY(vals_in.alloc(M));
-      GB_TRY(mega_keys.alloc(M));
-      GB_TRY(mega_vals.alloc(M));
-      GB_TRY(mega_start.alloc(M));
-      k_mega_keys<<<grid_for(M, 256), 256, 0, s>>>(g->in.off.p, g->in.tgt.p, old_of.p, p->new_id.p, hot_of_blk.p,
-                                                   p->nrows.p, B, mega_off.p, n_mega, M, deal, keys_in.p, vals_in.p);
-      uint32_t row_bits = 1;
-      while ((1u << row_bits) < n_mega) ++row_bits;
-      size_t tb = 0;
-      GB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, keys_in.p, mega_keys.p, vals_in.p, mega_vals.p, (int)M, 0,
-                                              (int)(CB_MEGA_JBITS + row_bits), s));
-      DevBuf<uint8_t> tmp;
-      GB_TRY(tmp.alloc(tb));
-      GB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, keys_in.p, mega_keys.p, vals_in.p, mega_vals.p, (int)M, 0,
-                                              (int)(CB_MEGA_JBITS + row_bits), s));
-      k_mega_starts<<<grid_for(M, 256), 256, 0, s>>>(mega_keys.p, M, mega_start.p);
-      size_t sb = 0;
-      GB_CUDA(cub::DeviceScan::InclusiveScan(nullptr, sb, mega_start.p, mega_start.p, cub::Max(), (int)M, s));
-      DevBuf<uint8_t> stmp;
-      GB_TRY(stmp.alloc(sb));
-      GB_CUDA(cub::DeviceScan::InclusiveScan(stmp.p, sb, mega_start.p, mega_start.p, cub::Max(), (int)M, s));
-      GB_CUDA(cudaMemsetAsync(lens.p, 0, (size_t)n_mega * 4, s));
-      k_mega_counts<<<grid_for(M, 256), 256, 0, s>>>(mega_keys.p, mega_start.p, M, p->poff.p, goff.p, lens.p,
-                                                     counters.p + 2);
-      GB_CUDA(cudaGetLastError());
-      GB_CUDA(cudaStreamSynchronize(s));  // keys_in / vals_in / tmp / stmp are released here
-    }
-    if (p->n_loc > p->n_cb)
-      k_lens_tail<<<grid_for(p->n_loc - p->n_cb, 256), 256, 0, s>>>(indeg.p, p->n_cb, p->n_loc, deal, lens.p);
-    if (p->S) {
-      k_cb_groups<<<grid_for(p->S, 256), 256, 0, s>>>(goff.p, p->S);
-      GB_TRY(scan_exclusive(s, goff.p, p->S + 1));
-      uint32_t ng = 0;
-      GB_CUDA(cudaMemcpyAsync(&ng, goff.p + p->S, 4, cudaMemcpyDeviceToHost, s));
-      GB_CUDA(cudaStreamSynchronize(s));
-      p->NG = ng;
-    }
-    {
-      unsigned long long h[3] = {0, 0, 0};
-      GB_CUDA(cudaMemcpyAsync(h, counters.p, 24, cudaMemcpyDeviceToHost, s));
-      GB_CUDA(cudaStreamSynchronize(s));
-      p->loc_edges = h[1];
-      p->cb_edges = h[2];
-    }
-    // 5. SELL-32 layout of all local rows
-    p->num_slices = (p->n_loc + 31) / 32;
-    if (p->num_slices) {
-      DevBuf<uint32_t> units, bases;
-      GB_TRY(units.alloc(p->num_slices));
-      GB_TRY(bases.alloc(p->num_slices));
-      k_sell_widths<<<grid_for((uint64_t)p->num_slices * 32, 256), 256, 0, s>>>(lens.p, p->n_loc, p->num_slices, units.p);
-      GB_CUDA(cudaMemcpyAsync(bases.p, units.p, (size_t)p->num_slices * 4, cudaMemcpyDeviceToDevice, s));
-      GB_TRY(scan_exclusive(s, bases.p, p->num_slices));
-      uint32_t last_base = 0, last_units = 0;
-      GB_CUDA(cudaMemcpyAsync(&last_base, bases.p + p->num_slices - 1, 4, cudaMemcpyDeviceToHost, s));
-      GB_CUDA(cudaMemcpyAsync(&last_units, units.p + p->num_slices - 1, 4, cudaMemcpyDeviceToHost, s));
-      GB_CUDA(cudaStreamSynchronize(s));
-      const size_t total_units = (size_t)last_base + last_units;
-      GB_TRY(p->slice_meta.alloc(p->num_slices));
-      GB_TRY(p->sell.alloc(total_units, 64));
-      GB_CUDA(cudaMemsetAsync(p->sell.p, 0xFF, (total_units + 64) * sizeof(uint4), s));  // ~0 = padding
-      k_sell_meta<<<grid_for(p->num_slices, 256), 256, 0, s>>>(units.p, bases.p, p->num_slices, p->slice_meta.p);
-      GB_CUDA(cudaGetLastError());
-      GB_CUDA(cudaStreamSynchronize(s));
-    }
-    // 6. fill: segments + SELL remainders of the rows below n_cb, whole rows above
-    GB_TRY(p->cb_ids.alloc(std::max<uint64_t>(p->NG, 1), 64));
-    GB_TRY(p->cb_bits.alloc(p->NG / 32 + 8));  // a 128-group step reads 5 words from its first
-    GB_CUDA(cudaMemsetAsync(p->cb_bits.p, 0, (p->NG / 32 + 8) * 4, s));
-    if (p->NG) {
-      k_fill_u2<<<grid_for(p->NG + 64, 256), 256, 0, s>>>(p->cb_ids.p, p->NG + 64, make_uint2(B | (B << 16), B | (B << 16)));
-      k_cb_bits<<<grid_for(p->S, 256), 256, 0, s>>>(goff.p, p->S, p->cb_bits.p);
-      if (M)
-        k_mega_fill<<<grid_for(M, 256), 256, 0, s>>>(mega_keys.p, mega_vals.p, mega_start.p, M, p->poff.p, p->blk.p, B,
-                                                     goff.p, reinterpret_cast<uint16_t*>(p->cb_ids.p), p->slice_meta.p,
-                                                     reinterpret_cast<uint32_t*>(p->sell.p));
-      if (p->n_cb > n_mega)
-        k_cb_fill<<<grid_for((uint64_t)(p->n_cb - n_mega) * 32, 256), 256, 0, s>>>(
-            g->in.off.p, old_of.p, rec.p, p->poff.p, n_mega, p->n_cb, deal, goff.p,
-            reinterpret_cast<uint16_t*>(p->cb_ids.p), p->slice_meta.p, reinterpret_cast<uint32_t*>(p->sell.p));
-      GB_CUDA(cudaGetLastError());
-      GB_CUDA(cudaStreamSynchronize(s));
-    }
-    if (p->n_loc > p->n_cb) {
-      k_sell_fill_tail<<<grid_for((uint64_t)(p->num_slices - p->n_cb / 32) * 32, 256), 256, 0, s>>>(
-          g->in.off.p, g->in.tgt.p, old_of.p, p->new_id.p, p->n_cb, p->n_loc, deal, p->num_slices, p->slice_meta.p,
-          p->sell.p);
-      GB_CUDA(cudaGetLastError());
-    }
-    // 7. chunks of the column-block kernel and every persistent CTA's share of them
-    p->grid_cb = 0;
-    p->trace = env_u32("GB_PR_TRACE", 0) != 0;
-    if (p->NG) {
-      // first group of every block's stream
-      DevBuf<uint32_t> gbeg;
-      GB_TRY(gbeg.alloc(p->KB + 1));
-      k_gather_u32<<<grid_for(p->KB + 1, 128), 128, 0, s>>>(goff.p, p->poff.p, p->KB + 1, gbeg.p);
-      std::vector<uint32_t> h_gbeg(p->KB + 1);
-      GB_CUDA(cudaMemcpyAsync(h_gbeg.data(), gbeg.p, (size_t)(p->KB + 1) * 4, cudaMemcpyDeviceToHost, s));
-      GB_CUDA(cudaStreamSynchronize(s));
-      // ~8 tasks per SM keep the dynamic schedule level; a task is 32 chunks (one per warp) of 512..2048
-      // groups (fewer, longer chunks = fewer segments cut by chunk boundaries); a thin block is cut into
-      // >= 64 chunks (down to one 64-group step each) so that all warps share it — a lone warp runs at
-      // its dependency latency, ~10x below the SM's throughput
-      uint32_t C = env_u32("GB_PR_CHUNK", 0);
-      const uint32_t T = std::min<uint32_t>(std::max<uint32_t>(env_u32("GB_PR_TASK_CHUNKS", CB_TASK_CHUNKS), 32u), 128u);
-      if (!C) C = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(p->NG / ((uint64_t)dev_sms * 8 * T), 16384 / T), 65536 / T);
-      C = std::max<uint32_t>(32u, (C + 31) / 32 * 32);
-      p->chunk_groups = C;
-      std::vector<uint32_t> h_cfirst(p->KB + 1, 0), h_cgrp(p->KB, C);
-      std::vector<uint2> h_tasks;
-      for (uint32_t j = 0; j < p->KB; ++j) {
-        const uint32_t G = h_gbeg[j + 1] - h_gbeg[j];
-        h_cgrp[j] = std::min<uint32_t>(C, std::max<uint32_t>(std::min<uint32_t>(64u, C), (G / 64 + 63) / 64 * 64));
-        const uint32_t nc = (G + h_cgrp[j] - 1) / h_cgrp[j];
-        h_cfirst[j + 1] = h_cfirst[j] + nc;
-        for (uint32_t c = 0; c < nc; c += T)
-          h_tasks.push_back(make_uint2(h_cfirst[j] + c, (std::min(nc, c + T) - c) | (j << 8)));
-      }
-      p->n_chunks = h_cfirst[p->KB];
-      p->n_tasks = (uint32_t)h_tasks.size();
-      p->grid_cb = (unsigned)std::min<uint64_t>(p->n_tasks, (uint64_t)dev_sms);  // one persistent CTA per SM
-      GB_TRY(upload(s, &p->tasks, h_tasks));
-      DevBuf<uint32_t> cfirst, cgrp;
-      GB_TRY(upload(s, &cfirst, h_cfirst));
-      GB_TRY(upload(s, &cgrp, h_cgrp));
-      GB_TRY(p->chunks.alloc(p->n_chunks, 1));
-      GB_TRY(p->tail_slot.alloc(p->n_chunks));
-      GB_TRY(p->fix_list.alloc(p->n_chunks));
-      GB_TRY(p->side.alloc((size_t)2 * p->n_chunks + 2));
-      GB_CUDA(cudaMemsetAsync(p->side.p, 0, ((size_t)2 * p->n_chunks + 2) * 8, s));
-      GB_CUDA(cudaMemsetAsync(p->chunks.p + p->n_chunks, 0, sizeof(uint4), s));  // sentinel: ends every fixup walk
-      uint32_t* d_nfix = reinterpret_cast<uint32_t*>(counters.p + 3);
-      k_cb_chunks<<<grid_for(p->n_chunks, 128), 128, 0, s>>>(goff.p, p->poff.p, p->nrows.p, gbeg.p, cfirst.p, cgrp.p,
-                                                           p->KB, p->n_chunks, p->chunks.p, p->tail_slot.p,
-                                                           p->fix_list.p, d_nfix);
-      // GB_PR_BANK_ORDER=0 (experiment): keep the ids of every group in CSR order
-      if (env_u32("GB_PR_BANK_ORDER", 1) != 0)
-        k_cb_bank_order<<<grid_for((uint64_t)p->n_chunks * 32, CB_BANK_THREADS), CB_BANK_THREADS, 0, s>>>(
-            p->chunks.p, p->n_chunks, B, p->cb_ids.p);
-      GB_CUDA(cudaGetLastError());
-      uint32_t h_fix[2] = {0, 0};
-      GB_CUDA(cudaMemcpyAsync(h_fix, d_nfix, 8, cudaMemcpyDeviceToHost, s));
-      GB_CUDA(cudaStreamSynchronize(s));
-      p->n_fix = h_fix[0];
-      p->fix_max_row = h_fix[1];
-    } else {
-      GB_TRY(p->chunks.alloc(1));
-      GB_TRY(p->tail_slot.alloc(1));
-      GB_TRY(p->fix_list.alloc(1));
-      GB_TRY(p->side.alloc(2));
-      GB_TRY(p->tasks.alloc(1));
-    }
-    GB_TRY(p->task_ctr.alloc(std::max<unsigned>(p->grid_cb, 1)));
-    GB_CUDA(cudaMemsetAsync(p->task_ctr.p, 0, (size_t)std::max<unsigned>(p->grid_cb, 1) * 4, s));
-    GB_TRY(p->partial.alloc(std::max<uint64_t>(p->S, 1)));
-    GB_CUDA(cudaMemsetAsync(p->partial.p, 0, std::max<uint64_t>(p->S, 1) * 4, s));
-    GB_TRY(p->rem.alloc(std::max<uint32_t>(p->n_cb, 1)));
-    {
-      std::vector<uint32_t> h_kb((p->n_cb + 31) / 32);
-      for (size_t w = 0; w < h_kb.size(); ++w) h_kb[w] = fin_blocks_of(h_nrows.data(), p->KB, (uint32_t)w * 32);
-      GB_TRY(upload(s, &p->fin_kb, h_kb));
-    }
-    // 8. launch shapes and error buffers
-    p->smem_cb = ((size_t)B + 4) * sizeof(float);
-    GB_CUDA(cudaFuncSetAttribute(k_pr_cb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cb));
-    GB_CUDA(cudaFuncSetAttribute(k_pr_cb_half, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cb));
-    // GB_PR_DUAL=1 (experiment): k_pr_cb_half and k_pr_sell at the same time on two streams.  Both kernels
-    // load the same LSU data pipe and k_pr_sell starves for L1 next to a large block: on an H100 at RMAT-26
-    // the overlap is slower than the sequential sweep (4.98 vs 4.56-4.77 ms); default off.
-    p->dual = p->grid_cb > 0 && p->num_slices > 0 && env_u32("GB_PR_DUAL", 0) != 0;
-    if (p->dual) {
-      GB_CUDA(cudaStreamCreateWithFlags(&p->s2, cudaStreamNonBlocking));
-      GB_CUDA(cudaEventCreateWithFlags(&p->ev_fork, cudaEventDisableTiming));
-      GB_CUDA(cudaEventCreateWithFlags(&p->ev_join, cudaEventDisableTiming));
-    }
-    const uint64_t want_sell = ((uint64_t)p->num_slices + PR_SELL_THREADS / 32 - 1) / (PR_SELL_THREADS / 32);
-    p->grid_sell = (unsigned)std::min<uint64_t>(want_sell, (uint64_t)dev_sms * 2);
-    // rows with segments in more than SELL_FEW blocks are a prefix (nrows[] is non-increasing): k_pr_finish
-    // completes them; all others are completed by their k_pr_sell lane (sequential mode: k_pr_cb is done by then)
-    p->n_fin = p->dual ? p->n_cb : (p->KB > SELL_FEW ? std::min<uint32_t>(p->n_cb, (h_nrows[SELL_FEW] + 31) / 32 * 32) : 0);
-    for (uint32_t j = 0; j < SELL_FEW && j < p->KB; ++j) {
-      p->few_nrows[j] = h_nrows[j];
-      p->few_poff[j] = h_poff[j];
-    }
-    p->n_fin_warp = p->KB > FIN_CTA_BLOCKS ? std::min<uint32_t>(p->n_fin, (h_nrows[FIN_CTA_BLOCKS] + 31) / 32 * 32) : 0;
-    const uint64_t fin_warps2 = (uint64_t)p->n_fin_warp / 32 * (PR_FIN_THREADS / 32) + (p->n_fin - p->n_fin_warp + 63) / 64;
-    const uint64_t fin_warps4 = (uint64_t)p->n_fin_warp / 32 * (PR_FIN_THREADS / 32) + (p->n_fin - p->n_fin_warp + 127) / 128;
-    p->fin_u = (fin_warps2 + PR_FIN_THREADS / 32 - 1) / (PR_FIN_THREADS / 32) <= (uint64_t)dev_sms * 8 ? 2 : 4;
-    // GB_PR_FIN_U (experiment / tests): 2 or 4 forces that instantiation of k_pr_finish; anything else = automatic
-    const uint32_t force_u = env_u32("GB_PR_FIN_U", 0);
-    if (force_u == 2 || force_u == 4) p->fin_u = force_u;
-    const uint64_t fin_tasks = p->fin_u == 2 ? fin_warps2 : fin_warps4;
-    const uint64_t want_fin = (fin_tasks + PR_FIN_THREADS / 32 - 1) / (PR_FIN_THREADS / 32);
-    p->grid_fin = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(want_fin, (uint64_t)dev_sms * 8));
-    // Role split of the finish CTAs: when every CTA has at most one pass of each kind to do (the grid is not
-    // capped) and the hub chain is long (hundreds of blocks per row), CTAs [0, hub groups) take one hub
-    // group each and the others the remaining rows — the two latency chains then run side by side instead
-    // of one after the other in every CTA.  It pays on a shard of a large graph; there is nothing to gain
-    // when the grid is capped (RMAT-26 on one GPU) or the hub chain is short (RMAT-22), where every CTA keeps
-    // doing both parts.
-    // GB_PR_FIN_SPLIT (experiment / tests): 1 forces the split, 2 never splits, 0 = automatic.  Forcing waives
-    // only the two conditions above that decide whether it pays; the structural ones stay (a hub group to
-    // take, rows left for the others, and at least one CTA beyond the hub CTAs: else no CTA would update
-    // the tail rows).
-    p->fin_hub_ctas = 0;
-    const uint32_t split = env_u32("GB_PR_FIN_SPLIT", 0);
-    const bool split_pays = want_fin <= (uint64_t)dev_sms * 8 && p->KB > 4 * FIN_CTA_BLOCKS;
-    if (p->n_fin_warp && p->n_fin > p->n_fin_warp && p->grid_fin > p->n_fin_warp / 32 &&
-        (split == 1 || (split == 0 && split_pays)))
-      p->fin_hub_ctas = p->n_fin_warp / 32;
-    const size_t nerr = (size_t)p->grid_sell + p->grid_fin;
-    GB_TRY(p->block_err.alloc(nerr));
-    GB_CUDA(cudaMemsetAsync(p->block_err.p, 0, nerr * sizeof(double), s));
-    GB_TRY(p->err_hist.alloc(64));
-    GB_TRY(p->ctrl.alloc(2));
-    GB_CUDA(cudaMemsetAsync(p->ctrl.p, 0, 8, s));
-    GB_CUDA(cudaStreamSynchronize(s));
-    return GB_OK;
-  }();
-  if (st != GB_OK) {
-    free_pr_plan(p);
-    return st;
+// ---- launch shapes: the last stage of the layout build --------------------------------------------
+gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, const std::vector<uint32_t>& h_poff,
+                           int dev_sms, cudaStream_t s) {
+  p->trace = env_u32("GB_PR_TRACE", 0) != 0;
+  p->smem_cb = ((size_t)p->B + 4) * sizeof(float);
+  GB_CUDA(cudaFuncSetAttribute(k_pr_cb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cb));
+  const uint64_t want_sell = ((uint64_t)p->num_slices + PR_SELL_THREADS / 32 - 1) / (PR_SELL_THREADS / 32);
+  p->grid_sell = (unsigned)std::min<uint64_t>(want_sell, (uint64_t)dev_sms * 2);
+  // rows with segments in more than SELL_FEW blocks are a prefix (nrows[] is non-increasing): k_pr_finish
+  // completes them; all others are completed by their k_pr_sell lane (k_pr_cb is done by then)
+  p->n_fin = p->KB > SELL_FEW ? std::min<uint32_t>(p->n_cb, (h_nrows[SELL_FEW] + 31) / 32 * 32) : 0;
+  for (uint32_t j = 0; j < SELL_FEW && j < p->KB; ++j) {
+    p->few_nrows[j] = h_nrows[j];
+    p->few_poff[j] = h_poff[j];
   }
-  *out_plan = p;
+  p->n_fin_warp = p->KB > FIN_CTA_BLOCKS ? std::min<uint32_t>(p->n_fin, (h_nrows[FIN_CTA_BLOCKS] + 31) / 32 * 32) : 0;
+  const uint64_t fin_warps2 = (uint64_t)p->n_fin_warp / 32 * (PR_FIN_THREADS / 32) + (p->n_fin - p->n_fin_warp + 63) / 64;
+  const uint64_t fin_warps4 = (uint64_t)p->n_fin_warp / 32 * (PR_FIN_THREADS / 32) + (p->n_fin - p->n_fin_warp + 127) / 128;
+  p->fin_u = (fin_warps2 + PR_FIN_THREADS / 32 - 1) / (PR_FIN_THREADS / 32) <= (uint64_t)dev_sms * 8 ? 2 : 4;
+  // GB_PR_FIN_U (experiment / tests): 2 or 4 forces that instantiation of k_pr_finish; anything else = automatic
+  const uint32_t force_u = env_u32("GB_PR_FIN_U", 0);
+  if (force_u == 2 || force_u == 4) p->fin_u = force_u;
+  const uint64_t fin_tasks = p->fin_u == 2 ? fin_warps2 : fin_warps4;
+  const uint64_t want_fin = (fin_tasks + PR_FIN_THREADS / 32 - 1) / (PR_FIN_THREADS / 32);
+  p->grid_fin = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(want_fin, (uint64_t)dev_sms * 8));
+  // Role split of the finish CTAs: when every CTA has at most one pass of each kind to do (the grid is not
+  // capped) and the hub chain is long (hundreds of blocks per row), CTAs [0, hub groups) take one hub
+  // group each and the others the remaining rows — the two latency chains then run side by side instead
+  // of one after the other in every CTA.  It pays on a shard of a large graph; there is nothing to gain
+  // when the grid is capped (RMAT-26 on one GPU) or the hub chain is short (RMAT-22), where every CTA keeps
+  // doing both parts.
+  // GB_PR_FIN_SPLIT (experiment / tests): 1 forces the split, 2 never splits, 0 = automatic.  Forcing waives
+  // only the two conditions above that decide whether it pays; the structural ones stay (a hub group to
+  // take, rows left for the others, and at least one CTA beyond the hub CTAs: else no CTA would update
+  // the tail rows).
+  p->fin_hub_ctas = 0;
+  const uint32_t split = env_u32("GB_PR_FIN_SPLIT", 0);
+  const bool split_pays = want_fin <= (uint64_t)dev_sms * 8 && p->KB > 4 * FIN_CTA_BLOCKS;
+  if (p->n_fin_warp && p->n_fin > p->n_fin_warp && p->grid_fin > p->n_fin_warp / 32 &&
+      (split == 1 || (split == 0 && split_pays)))
+    p->fin_hub_ctas = p->n_fin_warp / 32;
+  const size_t nerr = (size_t)p->grid_sell + p->grid_fin;
+  GB_TRY(p->block_err.alloc(nerr));
+  GB_CUDA(cudaMemsetAsync(p->block_err.p, 0, nerr * sizeof(double), s));
+  GB_TRY(p->err_hist.alloc(64));
+  GB_TRY(p->ctrl.alloc(2));
+  GB_CUDA(cudaMemsetAsync(p->ctrl.p, 0, 8, s));
+  GB_CUDA(cudaStreamSynchronize(s));
   return GB_OK;
 }
 
@@ -1999,8 +914,9 @@ static gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan
 // row is completed later, by k_pr_finish (rows below n_fin).  A row that its k_pr_sell lane completes itself
 // (few hot blocks: small graphs) needs the sum BEFORE that kernel: k_pr_fixup runs in between.
 static bool fix_in_sell(const PrPlan* p) {
-  return !p->dual && p->n_fix && p->grid_sell && p->fix_max_row < p->n_fin;
+  return p->n_fix && p->grid_sell && p->fix_max_row < p->n_fin;
 }
+static bool fixup_launched(const PrPlan* p) { return p->grid_cb && p->n_fix && !fix_in_sell(p); }
 static PrArgs make_args(const PrPlan* p, float base, float damping, double tolerance) {
   PrArgs a{};
   a.outdeg = p->outdeg.p;
@@ -2053,55 +969,64 @@ static PrArgs make_args(const PrPlan* p, float base, float damping, double toler
   return a;
 }
 
-// one sweep = column blocks (+ fixup of cut segments) and SELL rows — at the same time in dual mode —
-// then finish; *launches is advanced by the kernels launched
+// one sweep = column blocks (+ fixup of cut segments), SELL rows, then finish; *launches is advanced by
+// the kernels launched
 template <bool PEERS>
 static gb_status launch_sweep(const PrPlan* p, const PrArgs& a, cudaStream_t s, uint64_t* launches) {
-  const unsigned fix_grid = grid_for((uint64_t)p->n_fix * 32, 128, 296);
-  if (p->dual) {
-    GB_CUDA(cudaEventRecord(p->ev_fork, s));
-    GB_CUDA(cudaStreamWaitEvent(p->s2, p->ev_fork, 0));
-    k_pr_cb_half<<<p->grid_cb, PR_THREADS / 2, p->smem_cb, s>>>(a);
-    k_pr_sell<PEERS><<<p->grid_sell, PR_SELL_THREADS, 0, p->s2>>>(a);
-    if (p->n_fix) k_pr_fixup<<<fix_grid, 128, 0, s>>>(a);
-    GB_CUDA(cudaEventRecord(p->ev_join, p->s2));
-    GB_CUDA(cudaStreamWaitEvent(s, p->ev_join, 0));
-    *launches += 2 + (p->n_fix ? 1 : 0);
-  } else {
-    cudaEvent_t* ev = nullptr;
-    if (p->trace && p->trace_events.size() < 5 * 256) {
-      const size_t base = p->trace_events.size();
-      p->trace_events.resize(base + 5);
-      for (int k = 0; k < 5; ++k) GB_CUDA(cudaEventCreate(&p->trace_events[base + k]));
-      ev = &p->trace_events[base];
-      GB_CUDA(cudaEventRecord(ev[0], s));
-    }
-    if (p->grid_cb) {
-      k_pr_cb<<<p->grid_cb, PR_THREADS, p->smem_cb, s>>>(a);
-      if (ev) GB_CUDA(cudaEventRecord(ev[1], s));
-      if (p->n_fix && !a.fix_in_sell) k_pr_fixup<<<fix_grid, 128, 0, s>>>(a);
-      *launches += 1 + (p->n_fix && !a.fix_in_sell ? 1 : 0);
-    } else if (ev) {
-      GB_CUDA(cudaEventRecord(ev[1], s));
-    }
-    if (ev) GB_CUDA(cudaEventRecord(ev[2], s));
-    if (p->grid_sell) {
-      k_pr_sell<PEERS><<<p->grid_sell, PR_SELL_THREADS, 0, s>>>(a);
-      *launches += 1;
-    }
-    if (ev) GB_CUDA(cudaEventRecord(ev[3], s));
-    if (p->fin_u == 2) k_pr_finish<PEERS, 2><<<p->grid_fin, PR_FIN_THREADS, 0, s>>>(a);
-    else k_pr_finish<PEERS, 4><<<p->grid_fin, PR_FIN_THREADS, 0, s>>>(a);
-    if (ev) GB_CUDA(cudaEventRecord(ev[4], s));
-    *launches += 1;
-    GB_CUDA(cudaGetLastError());
-    return GB_OK;
+  cudaEvent_t* ev = nullptr;
+  if (p->trace && p->trace_events.size() < 5 * 256) {
+    const size_t base = p->trace_events.size();
+    p->trace_events.resize(base + 5);
+    for (int k = 0; k < 5; ++k) GB_CUDA(cudaEventCreate(&p->trace_events[base + k]));
+    ev = &p->trace_events[base];
+    GB_CUDA(cudaEventRecord(ev[0], s));
   }
+  if (p->grid_cb) {
+    k_pr_cb<<<p->grid_cb, PR_THREADS, p->smem_cb, s>>>(a);
+    *launches += 1;
+  }
+  if (ev) GB_CUDA(cudaEventRecord(ev[1], s));
+  if (fixup_launched(p)) {
+    k_pr_fixup<<<grid_for((uint64_t)p->n_fix * 32, 128, 296), 128, 0, s>>>(a);
+    *launches += 1;
+  }
+  if (ev) GB_CUDA(cudaEventRecord(ev[2], s));
+  if (p->grid_sell) {
+    k_pr_sell<PEERS><<<p->grid_sell, PR_SELL_THREADS, 0, s>>>(a);
+    *launches += 1;
+  }
+  if (ev) GB_CUDA(cudaEventRecord(ev[3], s));
   if (p->fin_u == 2) k_pr_finish<PEERS, 2><<<p->grid_fin, PR_FIN_THREADS, 0, s>>>(a);
   else k_pr_finish<PEERS, 4><<<p->grid_fin, PR_FIN_THREADS, 0, s>>>(a);
+  if (ev) GB_CUDA(cudaEventRecord(ev[4], s));
   *launches += 1;
   GB_CUDA(cudaGetLastError());
   return GB_OK;
+}
+
+struct PrStart {  // init and base of page_rank.rs:70-71
+  float init, base;
+  PrStart(uint32_t n, float damping) : init(1.0f / (float)n), base((1.0f - damping) / (float)n) {}
+};
+// x0 = init / outdeg, the constant part of x1, the scores (k_pr_init), and the stop flag and task cursors
+static gb_status pr_reset(const PrPlan* p, PrStart v, float* x0, float* x1, float* scores, cudaStream_t s) {
+  k_pr_init<<<grid_for(p->n, 256), 256, 0, s>>>(p->n, p->n_active, v.init, v.base, p->deal, p->outdeg.p, x0, x1,
+                                                scores);
+  GB_CUDA(cudaMemsetAsync(p->ctrl.p, 0, 8, s));
+  GB_CUDA(cudaMemsetAsync(p->task_ctr.p, 0, (size_t)std::max<unsigned>(p->grid_cb, 1) * 4, s));
+  return GB_OK;
+}
+// the closed-form error of the rows without in-edges, contributed to sweep 1 once, by rank 0
+static double first_sweep_err(const PrPlan* p, uint64_t sweep_no, PrStart v) {
+  return (sweep_no == 1 && p->deal.p == 0) ? (double)(p->n - p->n_active) * fabs((double)(v.base - v.init)) : 0.0;
+}
+// sources without in-edges change exactly once (init/deg -> base/deg): after sweep 1, patch the vector that
+// sweep has just finished reading
+static void pr_fill_inactive(const PrPlan* p, const PrArgs& a, float base, cudaStream_t s, uint64_t* launches) {
+  if (a.sweep_no != 1 || p->n_active >= p->n) return;
+  k_pr_fill_inactive<<<grid_for(p->n - p->n_active, 256), 256, 0, s>>>(p->n, p->n_active, base, p->outdeg.p,
+                                                                     const_cast<float*>(a.x_cur));
+  *launches += 1;
 }
 
 // ---- drivers ---------------------------------------------------------------------------------
@@ -2126,13 +1051,10 @@ static gb_status run_exact(const gb_graph* g, const gb_page_rank_config* cfg, fl
 
 static gb_status run_jacobi(const gb_graph* g, const gb_page_rank_config* cfg, float* d_scores,
                             uint64_t* ran, double* error) {
-  if (!g->pr_plan) GB_TRY(build_pr_plan(g, PrDeal{}, &g->pr_plan));
-  PrPlan* p = g->pr_plan;
+  PrPlan* p = g->pr_plan;  // built by page_rank_impl
   cudaStream_t s = g->stream;
   const uint32_t n = p->n;
-  const float nf = (float)n;
-  const float init = 1.0f / nf;                             // page_rank.rs:70
-  const float base = (1.0f - cfg->damping_factor) / nf;     // page_rank.rs:71
+  const PrStart v(n, cfg->damping_factor);
   const bool profile = profiling_on();
   if (!p->x[0].p) {
     GB_TRY(p->x[0].alloc(n));
@@ -2140,13 +1062,10 @@ static gb_status run_jacobi(const gb_graph* g, const gb_page_rank_config* cfg, f
     GB_TRY(p->scores.alloc(n));
   }
 
-  k_pr_init<<<grid_for(n, 256), 256, 0, s>>>(n, p->n_active, init, base, p->deal, p->outdeg.p, p->x[0].p, p->x[1].p,
-                                            p->scores.p);
-  GB_CUDA(cudaMemsetAsync(p->ctrl.p, 0, 8, s));
-  GB_CUDA(cudaMemsetAsync(p->task_ctr.p, 0, (size_t)std::max<unsigned>(p->grid_cb, 1) * 4, s));
+  GB_TRY(pr_reset(p, v, p->x[0].p, p->x[1].p, p->scores.p, s));
   g->timing.kernel_launches += 1;
 
-  PrArgs a = make_args(p, base, cfg->damping_factor, cfg->tolerance);
+  PrArgs a = make_args(p, v.base, cfg->damping_factor, cfg->tolerance);
   a.scores = p->scores.p;
 
   // max_iterations == 0 never satisfies `iteration == max_iterations` (page_rank.rs:107): the
@@ -2166,9 +1085,7 @@ static gb_status run_jacobi(const gb_graph* g, const gb_page_rank_config* cfg, f
       a.x_next = p->x[sweep_no & 1].p;
       a.sweep = b;
       a.sweep_no = (uint32_t)std::min<uint64_t>(sweep_no, 0xFFFFFFFFull);
-      a.extra_err = (sweep_no == 1)
-                        ? (double)(n - p->n_active) * fabs((double)(base - init))
-                        : 0.0;
+      a.extra_err = first_sweep_err(p, sweep_no, v);
       cudaEvent_t e0 = nullptr, e1 = nullptr;
       if (profile && ev_used + 2 <= 2 * PR_MAX_PROFILE_EVENTS) {
         while (p->prof_events.size() < ev_used + 2) {
@@ -2183,13 +1100,7 @@ static gb_status run_jacobi(const gb_graph* g, const gb_page_rank_config* cfg, f
       }
       GB_TRY(launch_sweep<false>(p, a, s, &g->timing.kernel_launches));
       if (e1) GB_CUDA(cudaEventRecord(e1, s));
-      if (sweep_no == 1 && p->n_active < n) {
-        // sources without in-edges change exactly once (init/deg -> base/deg): patch the buffer
-        // sweep 1 has just finished reading
-        k_pr_fill_inactive<<<grid_for(n - p->n_active, 256), 256, 0, s>>>(n, p->n_active, base, p->outdeg.p,
-                                                                         p->x[0].p);
-        g->timing.kernel_launches += 1;
-      }
+      pr_fill_inactive(p, a, v.base, s, &g->timing.kernel_launches);
     }
     GB_CUDA(cudaGetLastError());
     done += batch;
@@ -2223,6 +1134,45 @@ static gb_status run_jacobi(const gb_graph* g, const gb_page_rank_config* cfg, f
   return GB_OK;
 }
 
+static gb_status ensure_plan(const gb_graph* g) {
+  if (!g->pr_plan) GB_TRY(build_pr_plan(g, PrDeal{}, &g->pr_plan));
+  return GB_OK;
+}
+static void plan_stats(const PrPlan* p, gb_pr_shard_stats* stats) {
+  stats->rank = p->deal.p;
+  stats->world = p->deal.P;
+  stats->active_rows = p->n_active;
+  stats->local_rows = p->n_loc;
+  stats->local_edges = p->loc_edges;
+  stats->block_edges = p->cb_edges;
+  stats->block_entries = p->B;
+  stats->hot_blocks = p->KB;
+  stats->segments = p->S;
+  stats->groups = p->NG;
+  stats->chunks = p->n_chunks;
+  stats->tasks = p->n_tasks;
+  stats->cut_segments = p->n_fix;
+  stats->chunk_groups = p->chunk_groups;
+  stats->launches_per_sweep = 1 + (p->grid_cb ? 1 : 0) + (p->grid_sell ? 1 : 0) + (fixup_launched(p) ? 1 : 0);
+  stats->device_bytes = p->bytes();
+}
+static void plan_shape(const PrPlan* p, gb_pr_plan_shape* shape) {
+  shape->hot_blocks = p->KB;
+  shape->n_cb = p->n_cb;
+  shape->n_fin = p->n_fin;
+  shape->n_fin_warp = p->n_fin_warp;
+  shape->fin_u = p->fin_u;
+  shape->fin_hub_ctas = p->fin_hub_ctas;
+  shape->grid_cb = p->grid_cb;
+  shape->grid_sell = p->grid_sell;
+  shape->grid_fin = p->grid_fin;
+  shape->n_mega = p->n_mega;
+  shape->n_fix = p->n_fix;
+  shape->fix_in_sell = fix_in_sell(p) ? 1u : 0u;
+  shape->dual = 0;
+  shape->last_hot_block = p->last_hot_block;
+}
+
 static gb_status page_rank_impl(const gb_graph* g, const gb_page_rank_config* cfg, float* d_scores,
                                 float* h_scores, uint64_t* ran, double* error) {
   GB_REQUIRE(g && cfg && ran && error, "NULL argument");
@@ -2241,7 +1191,7 @@ static gb_status page_rank_impl(const gb_graph* g, const gb_page_rank_config* cf
     GB_TRY(tmp_scores.alloc(g->n));
     d_scores = tmp_scores.p;
   }
-  if (mode == GB_PR_JACOBI && !g->pr_plan) GB_TRY(build_pr_plan(g, PrDeal{}, &g->pr_plan));  // not timed
+  if (mode == GB_PR_JACOBI) GB_TRY(ensure_plan(g));  // not timed
   g->timing = gb_timing{};
   GB_CUDA(cudaEventRecord(g->ev_begin, s));
   if (mode == GB_PR_EXACT) GB_TRY(run_exact(g, cfg, d_scores, ran, error));
@@ -2305,15 +1255,8 @@ gb_status gb_pr_shard_init(const gb_pr_shard* shard, float damping, float* d_x0,
   const gb_graph* g = shard->graph;
   const gb::PrPlan* p = shard->plan;
   gb::DeviceGuard guard(g->device);
-  cudaStream_t s = (cudaStream_t)cuda_stream;
-  const float nf = (float)p->n;
-  const float init = 1.0f / nf;
-  const float base = (1.0f - damping) / nf;
   // every rank fills the whole initial vector itself (no exchange needed before sweep 1)
-  gb::k_pr_init<<<gb::grid_for(p->n, 256), 256, 0, s>>>(p->n, p->n_active, init, base, p->deal, p->outdeg.p, d_x0,
-                                                       d_x1, d_scores);
-  GB_CUDA(cudaMemsetAsync(p->ctrl.p, 0, 8, s));
-  GB_CUDA(cudaMemsetAsync(p->task_ctr.p, 0, (size_t)std::max<unsigned>(p->grid_cb, 1) * 4, s));
+  GB_TRY(gb::pr_reset(p, gb::PrStart(p->n, damping), d_x0, d_x1, d_scores, (cudaStream_t)cuda_stream));
   GB_CUDA(cudaGetLastError());
   return GB_OK;
 }
@@ -2329,10 +1272,8 @@ gb_status gb_pr_shard_step(const gb_pr_shard* shard, float damping, uint64_t swe
   const gb::PrPlan* p = shard->plan;
   gb::DeviceGuard guard(g->device);
   cudaStream_t s = (cudaStream_t)cuda_stream;
-  const float nf = (float)p->n;
-  const float init = 1.0f / nf;
-  const float base = (1.0f - damping) / nf;
-  gb::PrArgs a = gb::make_args(p, base, damping, -1.0 /* the caller owns the stop rule */);
+  const gb::PrStart v(p->n, damping);
+  gb::PrArgs a = gb::make_args(p, v.base, damping, -1.0 /* the caller owns the stop rule */);
   a.x_cur = d_x_cur;
   a.x_next = d_x_next;
   a.scores = d_scores;
@@ -2342,16 +1283,11 @@ gb_status gb_pr_shard_step(const gb_pr_shard* shard, float damping, uint64_t swe
   a.err_hist = d_error;
   a.sweep = 0;
   a.sweep_no = (uint32_t)std::min<uint64_t>(sweep_no, 0xFFFFFFFFull);
-  // the closed-form error of the rows without in-edges is contributed once, by rank 0
-  a.extra_err = (sweep_no == 1 && p->deal.p == 0)
-                    ? (double)(p->n - p->n_active) * fabs((double)(base - init))
-                    : 0.0;
+  a.extra_err = gb::first_sweep_err(p, sweep_no, v);
   uint64_t launches = 0;
   if (peer_count || d_mc_x_next) GB_TRY(gb::launch_sweep<true>(p, a, s, &launches));
   else GB_TRY(gb::launch_sweep<false>(p, a, s, &launches));
-  if (sweep_no == 1 && p->n_active < p->n)
-    gb::k_pr_fill_inactive<<<gb::grid_for(p->n - p->n_active, 256), 256, 0, s>>>(
-        p->n, p->n_active, base, p->outdeg.p, const_cast<float*>(d_x_cur));
+  gb::pr_fill_inactive(p, a, v.base, s, &launches);
   GB_CUDA(cudaGetLastError());
   return GB_OK;
 }
@@ -2396,24 +1332,7 @@ gb_status gb_pr_shard_finish(const gb_pr_shard* shard, const float* d_scores_int
 
 gb_status gb_pr_shard_info(const gb_pr_shard* shard, gb_pr_shard_stats* stats) {
   GB_REQUIRE(shard && stats, "NULL argument");
-  const gb::PrPlan* p = shard->plan;
-  stats->rank = p->deal.p;
-  stats->world = p->deal.P;
-  stats->active_rows = p->n_active;
-  stats->local_rows = p->n_loc;
-  stats->local_edges = p->loc_edges;
-  stats->block_edges = p->cb_edges;
-  stats->block_entries = p->B;
-  stats->hot_blocks = p->KB;
-  stats->segments = p->S;
-  stats->groups = p->NG;
-  stats->chunks = p->n_chunks;
-  stats->tasks = p->n_tasks;
-  stats->cut_segments = p->n_fix;
-  stats->chunk_groups = p->chunk_groups;
-  stats->launches_per_sweep = 1 + (p->grid_cb ? 1 : 0) + (p->grid_sell ? 1 : 0) +
-                              (p->grid_cb && p->n_fix && !gb::fix_in_sell(p) ? 1 : 0);
-  stats->device_bytes = p->bytes();
+  gb::plan_stats(shard->plan, stats);
   return GB_OK;
 }
 
@@ -2422,30 +1341,14 @@ gb_status gb_page_rank_plan_info(const gb_graph* g, gb_pr_shard_stats* stats) {
   if (g->kind != GB_KIND_DIRECTED) return gb::fail(GB_ERR_UNSUPPORTED, "page rank needs a directed graph");
   gb::DeviceGuard guard(g->device);
   std::lock_guard<std::mutex> lock(g->mu);
-  if (!g->pr_plan) GB_TRY(gb::build_pr_plan(g, gb::PrDeal{}, &g->pr_plan));
-  gb_pr_shard tmp;
-  tmp.graph = g;
-  tmp.plan = g->pr_plan;
-  return gb_pr_shard_info(&tmp, stats);
+  GB_TRY(gb::ensure_plan(g));
+  gb::plan_stats(g->pr_plan, stats);
+  return GB_OK;
 }
 
 gb_status gb_pr_shard_plan_shape(const gb_pr_shard* shard, gb_pr_plan_shape* shape) {
   GB_REQUIRE(shard && shape, "NULL argument");
-  const gb::PrPlan* p = shard->plan;
-  shape->hot_blocks = p->KB;
-  shape->n_cb = p->n_cb;
-  shape->n_fin = p->n_fin;
-  shape->n_fin_warp = p->n_fin_warp;
-  shape->fin_u = p->fin_u;
-  shape->fin_hub_ctas = p->fin_hub_ctas;
-  shape->grid_cb = p->grid_cb;
-  shape->grid_sell = p->grid_sell;
-  shape->grid_fin = p->grid_fin;
-  shape->n_mega = p->n_mega;
-  shape->n_fix = p->n_fix;
-  shape->fix_in_sell = gb::fix_in_sell(p) ? 1u : 0u;
-  shape->dual = p->dual ? 1u : 0u;
-  shape->last_hot_block = p->last_hot_block;
+  gb::plan_shape(shard->plan, shape);
   return GB_OK;
 }
 
@@ -2454,11 +1357,9 @@ gb_status gb_page_rank_plan_shape(const gb_graph* g, gb_pr_plan_shape* shape) {
   if (g->kind != GB_KIND_DIRECTED) return gb::fail(GB_ERR_UNSUPPORTED, "page rank needs a directed graph");
   gb::DeviceGuard guard(g->device);
   std::lock_guard<std::mutex> lock(g->mu);
-  if (!g->pr_plan) GB_TRY(gb::build_pr_plan(g, gb::PrDeal{}, &g->pr_plan));
-  gb_pr_shard tmp;
-  tmp.graph = g;
-  tmp.plan = g->pr_plan;
-  return gb_pr_shard_plan_shape(&tmp, shape);
+  GB_TRY(gb::ensure_plan(g));
+  gb::plan_shape(g->pr_plan, shape);
+  return GB_OK;
 }
 
 gb_status gb_page_rank_plan_reset(const gb_graph* g) {
@@ -2479,7 +1380,7 @@ gb_status gb_page_rank(const gb_graph* graph, const gb_page_rank_config* config,
 // One-shot PageRank of a host CSR.  The 4 bytes per edge of the targets dominate the upload, so they are
 // streamed: offsets first, then the targets in row-aligned chunks on a copy stream, while the graph's own
 // stream sorts the degrees, picks the hot blocks and classifies every chunk as it lands (TargetFeed in
-// build_pr_plan).  Only the fill pass, the sweeps and the copy of the ranks run after the last byte.
+// layout_classify, pr_layout.cu).  Only the fill pass, the sweeps and the copy of the ranks run after the last byte.
 // GB_PR_FEED_CHUNKS (default 16; 0 = upload everything, then build) and GB_PR_FEED_MIN_EDGES (default 2^22)
 // are experiment knobs.
 gb_status gb_page_rank_csr_u32(int device, uint32_t n, const uint32_t* in_off, const uint32_t* in_tgt,

@@ -354,7 +354,8 @@ typedef struct gb_pr_plan_shape {
   uint32_t n_mega;             /* local rows laid out through the sort path of the layout build */
   uint32_t n_fix;              /* chunks whose last segment continues in the next chunk */
   uint32_t fix_in_sell;        /* 1: those parts are added by k_pr_sell, 0: by k_pr_fixup */
-  uint32_t dual;               /* 1: k_pr_cb_half and k_pr_sell on two streams (GB_PR_DUAL) */
+  uint32_t dual;               /* always 0 (the sweep's kernels run one after the other on one stream);
+                                  kept so that the fields after it keep their offsets */
   uint32_t last_hot_block;     /* largest source block index among the hot blocks (0xFFFFFFFF: none) */
 } gb_pr_plan_shape;
 gb_status gb_page_rank_plan_shape(const gb_graph* graph, gb_pr_plan_shape* shape);

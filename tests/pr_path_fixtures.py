@@ -1,4 +1,4 @@
-"""Graphs that steer the JACOBI PageRank layout (graph_b200/csrc/pagerank.cu, build_pr_plan) onto its less
+"""Graphs that steer the JACOBI PageRank layout (graph_b200/csrc/pr_layout.cu, build_pr_plan) onto its less
 common paths, and the path each is meant to reach.  Shared by the CPU check against the layout model
 (test_pr_path_model.py) and the GPU tests (test_gpu_pr_paths.py), so that a retuned default that moves a
 graph off its path fails on the CPU already instead of silently thinning the GPU coverage."""
@@ -16,9 +16,9 @@ import layout_model as lm  # noqa: E402
 import oracle  # noqa: E402
 
 TAIL_R = (1, 2, 3, 5, 33)
-# every environment knob of the plan build and the sweep (graph_b200/csrc/pagerank.cu)
-KNOBS = ("GB_PR_BLOCK", "GB_PR_TAU", "GB_PR_MIN_BLOCK", "GB_PR_MEGA", "GB_PR_CHUNK", "GB_PR_TASK_CHUNKS",
-         "GB_PR_DUAL", "GB_PR_DEBUG", "GB_PR_FIN_U", "GB_PR_FIN_SPLIT", "GB_PR_FEED_CHUNKS", "GB_PR_FEED_MIN_EDGES")
+# every environment knob of the plan build and the sweep (graph_b200/csrc/pr_layout.cu, pagerank.cu)
+KNOBS = ("GB_PR_BLOCK", "GB_PR_TAU", "GB_PR_MEGA", "GB_PR_CHUNK", "GB_PR_TASK_CHUNKS", "GB_PR_DEBUG", "GB_PR_FIN_U",
+         "GB_PR_FIN_SPLIT", "GB_PR_FEED_CHUNKS", "GB_PR_FEED_MIN_EDGES")
 
 
 def tail_block(r):

@@ -1,5 +1,5 @@
 """CPU check of the bank-aware order of the ids inside each column-block group (tools/cb_bank_model.py,
-the restatement of k_cb_bank_order in graph_b200/csrc/pagerank.cu): the pass only permutes the ids of a
+the restatement of k_cb_bank_order in graph_b200/csrc/pr_layout.cu): the pass only permutes the ids of a
 group, follows the kernel's steps chunk by chunk, and never raises a window's modelled conflict count."""
 import sys
 from pathlib import Path

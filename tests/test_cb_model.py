@@ -1,5 +1,5 @@
 """CPU check of the column-block chunk logic (tools/cb_model.py): the lane-level numpy restatement of
-cb_cut / k_cb_chunks / cb_chunk_impl / cb_fix_segment in graph_b200/csrc/pagerank.cu must reproduce a direct
+cb_cut / k_cb_chunks (graph_b200/csrc/pr_layout.cu) and cb_chunk_impl / cb_fix_segment (pagerank.cu) must reproduce a direct
 per-segment sum for random segment lengths, including segments cut by chunk and step boundaries."""
 import sys
 from pathlib import Path

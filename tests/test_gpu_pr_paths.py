@@ -1,8 +1,8 @@
 """The JACOBI PageRank sweep on graphs built to reach its less common paths (tests/pr_path_fixtures.py):
 the partial last column block (scalar tail of the block load), a rectangular staircase, a mega row cut by
 chunk boundaries, a repeated source, fewer than 32 active rows, the hub-group CTAs of k_pr_finish, its
-FIN_U = 4 instantiation, its role split, a capped finish grid, and the GB_PR_DUAL / GB_PR_DEBUG /
-GB_PR_TASK_CHUNKS variants.  Every case asserts that the device plan took the path (against the layout
+FIN_U = 4 instantiation, its role split, a capped finish grid, and the GB_PR_DEBUG / GB_PR_TASK_CHUNKS
+variants.  Every case asserts that the device plan took the path (against the layout
 model), that the ranks match the f64-accumulating oracle, and that runs and arithmetic-preserving variants
 give the same bits."""
 import ctypes as C
@@ -155,17 +155,6 @@ def test_rmat18_task_chunks(gb, sms, monkeypatch):
     g = device_graph(gb, "rmat18")
     assert g.page_rank_plan_info()["chunk_groups"] != 512
     assert_matches_oracle(run(g), "rmat18", SWEEPS, 0.0)
-
-
-def test_rmat18_dual(gb, sms, monkeypatch):
-    """GB_PR_DUAL=1 moves rows from k_pr_sell to k_pr_finish: held to the oracle, not to the bits"""
-    set_knobs(monkeypatch, "rmat18", GB_PR_DUAL=1)
-    g = device_graph(gb, "rmat18")
-    _, shape, _ = assert_shape(g, "rmat18", sms, dual=True)
-    assert shape["dual"] == 1 and shape["n_fin"] == shape["n_cb"]
-    pr = run(g)
-    assert_matches_oracle(pr, "rmat18", SWEEPS, 0.0)
-    assert run(g).scores().tobytes() == pr.scores().tobytes()
 
 
 def test_capped_finish_grid(gb, sms, monkeypatch):

@@ -1,5 +1,5 @@
 """CPU check of the PageRank layout build's contract (tools/layout_model.py): the numpy restatement of
-cb_classify_row / k_cb_count[_rows] / k_cb_groups / k_cb_fill in graph_b200/csrc/pagerank.cu — one record per
+cb_classify_row / k_cb_count[_rows] / k_cb_groups / k_cb_fill in graph_b200/csrc/pr_layout.cu — one record per
 edge, positions in CSR order — must reproduce the layout stated directly, for every rank of a cyclic deal,
 and must not depend on the order in which rows are classified (streamed upload vs resident graph)."""
 import sys

@@ -1,5 +1,6 @@
 """CPU check that every fixture graph of test_gpu_pr_paths.py reaches the sweep path it was built for,
-by the layout model (tools/layout_model.py: steps 1-3 and 8 of build_pr_plan) on an H100's 132 SMs.
+by the layout model (tools/layout_model.py: the layout_order, layout_hot_blocks and plan_sweep_shape
+stages of build_pr_plan) on an H100's 132 SMs.
 If a retuned default moves a graph off its path, this fails here, without a GPU."""
 import pytest
 
@@ -23,8 +24,6 @@ def test_finish_knobs_on_rmat18():
     both = fx.lm.launch_shape(plan, fin_u=4, fin_split=1)
     assert both["fin_u"] == 4 and both["fin_hub_ctas"] == 6
     assert fx.lm.launch_shape(plan, fin_split=2)["fin_hub_ctas"] == 0
-    dual = fx.lm.launch_shape(plan, dual=True)
-    assert dual["dual"] and dual["n_fin"] == auto["n_cb"]
 
 
 def test_finish_knobs_on_the_capped_grid():

@@ -1,5 +1,5 @@
 """cb_bank_model.py — CPU count of the shared-memory bank conflicts of k_pr_cb's gathers, before and
-after the bank-aware order of the ids inside each group (pagerank.cu: k_cb_bank_order).
+after the bank-aware order of the ids inside each group (pr_layout.cu: k_cb_bank_order).
 
 A warp step of k_pr_cb covers a WINDOW of 32 G groups (G = 2, or 4 in chunks of at least CB_WIDE_MIN
 groups): lane L reads groups G L .. G L + G - 1 and then issues 4 shared-memory reads xs[id] per group, one
@@ -60,7 +60,7 @@ def build_streams(in_off, in_tgt, out_deg, B=lm.CB_BLOCK_DEFAULT, tau=lm.CB_TAU_
 
 
 def chunk_table(plan, goff, sms=lm.H100_SMS, T=CB_TASK_CHUNKS):
-    """Step 7 of build_pr_plan: per-block chunk sizes, then k_cb_chunks (cb_model.cb_cut)."""
+    """The layout_chunks stage of build_pr_plan: per-block chunk sizes, then k_cb_chunks (cb_model.cb_cut)."""
     NG = int(goff[-1])
     gbeg = goff[plan["poff"]]
     C = min(max(NG // (sms * 8 * T), 16384 // T), 65536 // T)

@@ -1,5 +1,5 @@
-"""cb_model.py — lane-level numpy model of the column-block kernel's chunk logic (pagerank.cu:
-cb_cut / k_cb_chunks / cb_chunk_impl / cb_fix_segment).
+"""cb_model.py — lane-level numpy model of the column-block kernel's chunk logic (pr_layout.cu:
+cb_cut / k_cb_chunks; pagerank.cu: cb_chunk_impl / cb_fix_segment).
 
 There is no GPU in the build container, so the trickiest index logic (chunk cuts inside long
 segments, start-bit row counting, the carried run, side buffers and their fixed-order fixup) is

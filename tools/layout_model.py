@@ -1,5 +1,5 @@
 """layout_model.py — numpy restatement of the PageRank layout build's edge classification and fill
-(pagerank.cu: cb_classify_row / k_cb_count[_rows] -> k_cb_groups + scan -> k_cb_fill, and the cyclic deal).
+(pr_layout.cu: cb_classify_row / k_cb_count[_rows] -> k_cb_groups + scan -> k_cb_fill, and the cyclic deal).
 
 There is no GPU in the build container; this model pins down the CONTRACT of the two passes so that it
 can be checked on the CPU: one 8-byte record per edge, positions in CSR order, every (row, block) pair of
@@ -54,7 +54,8 @@ def clamp_block(B):
 
 
 def make_plan(in_off, in_tgt, out_deg, B, tau, P=1, p=0, mega=CB_MEGA_DEG):
-    """Renumbering + staircase, like steps 1-3 of build_pr_plan (host side, no edge data needed).
+    """Renumbering + staircase, like the layout_order and layout_hot_blocks stages of build_pr_plan
+    (pr_layout.cu; host side, no edge data needed).
     B is used as given (see clamp_block); `mega` is GB_PR_MEGA, the in-degree above which a row takes the
     sort path of the layout build."""
     n = len(in_off) - 1
@@ -100,17 +101,15 @@ def make_plan(in_off, in_tgt, out_deg, B, tau, P=1, p=0, mega=CB_MEGA_DEG):
                 B=B, P=P, p=p)
 
 
-def launch_shape(plan, sms=H100_SMS, fin_u=0, fin_split=0, dual=False):
-    """Step 8 of build_pr_plan: the SELL grid (one warp per 32-row slice, no launch for a shard without
-    rows) and which rows k_pr_finish completes and how (fin_u, grid, role split).
-    fin_u / fin_split are GB_PR_FIN_U / GB_PR_FIN_SPLIT; dual is GB_PR_DUAL=1 (taken when there are hot
-    blocks and active rows)."""
+def launch_shape(plan, sms=H100_SMS, fin_u=0, fin_split=0):
+    """plan_sweep_shape (pagerank.cu), the last stage of build_pr_plan: the SELL grid (one warp per 32-row
+    slice, no launch for a shard without rows) and which rows k_pr_finish completes and how (fin_u, grid,
+    role split).  fin_u / fin_split are GB_PR_FIN_U / GB_PR_FIN_SPLIT."""
     KB, n_cb, nr = plan["KB"], plan["n_cb"], plan["nrows"]
-    dual = bool(dual) and KB > 0 and plan["n_loc"] > 0
     ceil32 = lambda x: (int(x) + 31) // 32 * 32
     num_slices = (plan["n_loc"] + 31) // 32
     grid_sell = min((num_slices + PR_SELL_WARPS - 1) // PR_SELL_WARPS, sms * 2)
-    n_fin = n_cb if dual else (min(n_cb, ceil32(nr[SELL_FEW])) if KB > SELL_FEW else 0)
+    n_fin = min(n_cb, ceil32(nr[SELL_FEW])) if KB > SELL_FEW else 0
     n_fin_warp = min(n_fin, ceil32(nr[FIN_CTA_BLOCKS])) if KB > FIN_CTA_BLOCKS else 0
     warps2 = n_fin_warp // 32 * PR_FIN_WARPS + (n_fin - n_fin_warp + 63) // 64
     warps4 = n_fin_warp // 32 * PR_FIN_WARPS + (n_fin - n_fin_warp + 127) // 128
@@ -125,7 +124,7 @@ def launch_shape(plan, sms=H100_SMS, fin_u=0, fin_split=0, dual=False):
     return dict(hot_blocks=KB, n_cb=n_cb, n_fin=n_fin, n_fin_warp=n_fin_warp, fin_u=u, grid_sell=grid_sell,
                 grid_fin=grid_fin,
                 fin_hub_ctas=n_fin_warp // 32 if split else 0, grid_capped=want_fin > sms * 8,
-                n_mega=plan["n_mega"], dual=int(dual), last_hot_block=plan["last_hot_block"])
+                n_mega=plan["n_mega"], dual=0, last_hot_block=plan["last_hot_block"])  # gb_pr_plan_shape.dual is 0
 
 
 def layout_counts(plan, in_off, in_tgt):
@@ -168,7 +167,8 @@ def classify_row(plan, l, tgt_row, cnt, rec_out):
 
 
 def build(plan, in_off, in_tgt, row_order):
-    """Classification in the given order of ORIGINAL row ids, then the scans and the fill."""
+    """The layout_classify stage of build_pr_plan (pr_layout.cu) in the given order of ORIGINAL row ids,
+    then the group scan and the layout_fill stage."""
     cnt = np.zeros(plan["S"] + 1, np.int64)
     lens = np.zeros(max(plan["n_loc"], 1), np.int64)
     rec = [None] * int(in_off[-1])
