@@ -144,6 +144,11 @@ struct DevCsr {
 
 struct PrPlan;  // pr_plan.cuh
 
+// Whether every row of the undirected CSR is in ascending order (an inversion across a row boundary does not
+// count).  Sorted and Deduplicated builds and make_degree_ordered write sorted rows; an Unsorted build or a
+// caller's CSR is Unknown until gb_triangle_count looks once and caches the answer.
+enum class RowOrder : uint8_t { Unknown, Sorted, Unsorted };
+
 }  // namespace gb
 
 // the opaque handle of the C ABI
@@ -164,6 +169,7 @@ struct gb_graph {
   uint32_t n = 0;
   gb::DevCsr out;  // directed: csr_out; undirected: the single csr
   gb::DevCsr in;   // directed only: csr_inc
+  mutable gb::RowOrder row_order = gb::RowOrder::Unknown;  // of `out`; set by the builds, cached by tc.cu
   cudaStream_t stream = nullptr;
   cudaEvent_t ev_begin = nullptr, ev_end = nullptr;
   mutable std::mutex mu;            // algorithms on one handle serialise on its stream

@@ -389,6 +389,8 @@ static gb_status build_graph_csrs(gb_graph* g, const uint32_t* d_src, const uint
     }
     GB_TRY(build_csr_device(s, g->n, rows.p, cols.p, nullptr, 2 * m, layout, &g->out));
   }
+  // an Unsorted build keeps the edge-list order inside each row, which may or may not be ascending
+  g->row_order = (layout == GB_LAYOUT_UNSORTED) ? RowOrder::Unknown : RowOrder::Sorted;
   return GB_OK;
 }
 
@@ -799,6 +801,7 @@ gb_status gb_make_degree_ordered(gb_graph* g) {
     GB_CUDA(cudaStreamSynchronize(s));
   }
   g->out = std::move(fresh);  // SwapCsr::swap_csr, csr.rs:120-122
+  g->row_order = RowOrder::Sorted;  // the (row, target) keys were sorted above
   return GB_OK;
 }
 

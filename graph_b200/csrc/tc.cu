@@ -1,13 +1,25 @@
-// tc.cu — global triangle count on the sorted undirected device CSR.
+// tc.cu — global triangle count on the undirected device CSR.
 //
 // Replaces crates/algos/src/triangle_count.rs:22-86 (`global_triangle_count`).  The reference walks
 //   for u: for v in N(u), stop at v > u: for w in N(v), stop at w > v: advance a put-back cursor over
 //   N(u) while *cursor < w; count if *cursor == w
-// which evaluates  T = sum_u sum_{v-occurrence in N(u), v<=u} sum_{w-occurrence in N(v), w<=v} [w in set(N(u))]
+// in list order, whatever the order of the rows.  On sorted rows that evaluates
+//   T = sum_u sum_{v-occurrence in N(u), v<=u} sum_{w-occurrence in N(v), w<=v} [w in set(N(u))]
 // (duplicate v and w occurrences multiply, duplicate x in N(u) do not; self loops take part) —
-// SURVEY.md A.5.  The kernel evaluates the same sum edge-parallel: one CSR entry (u, v) with v <= u
-// per work item; every w-occurrence of N(v) with w <= v is looked up in N(u) by binary search.
-// Short N(v) prefixes are handled by one lane, long ones by the whole warp.
+// SURVEY.md A.5.  On unsorted rows the stops and the cursor give a different number, and the reference
+// returns that number; Layout::Unsorted is the default layout, so it is the common case, not an error.
+//
+// The row order picks one of two paths.  Sorted and Deduplicated builds and make_degree_ordered write
+// sorted rows (gb_graph::row_order); for any other CSR the first call runs k_tc_rows_unsorted once, which
+// looks for a descent inside a row (one across a row boundary does not count), and caches the answer.
+//   sorted rows   — k_tc, one launch: the sum above, edge-parallel.  One CSR entry (u, v) with v <= u per
+//                   work item; both lists are cut to values <= v by binary search, and the cheaper one is
+//                   walked while the other is searched.  Walks of at most TC_SHORT entries stay in one
+//                   lane, longer ones go to the whole warp in steps of 32.
+//   unsorted rows — k_tc_cut + k_tc_list, the reference loop restated: cut[u] is the first index of row
+//                   u whose target is > u, and one thread per entry i < cut[u] walks N(v)[.. cut[v]) in
+//                   list order with the put-back cursor over N(u).  A path for correctness: its work is
+//                   O(deg u + deg v) per entry in one thread, and no benchmark runs it.
 //
 // Compulsory bytes per run: 8m + 4(n+1) (the undirected CSR once); the kernel is bound by the
 // dependent lookups (latency / L2), not by HBM.
@@ -114,6 +126,73 @@ __global__ void __launch_bounds__(256) k_tc(const uint32_t* __restrict__ off, co
   if (lane == 0 && count) atomicAdd(total, count);
 }
 
+// *found = 1 when some row holds tgt[i-1] > tgt[i]; a descent at an entry that begins a row does not count
+__global__ void __launch_bounds__(256) k_tc_rows_unsorted(const uint32_t* __restrict__ off,
+                                                          const uint32_t* __restrict__ tgt, uint32_t n, uint64_t len,
+                                                          unsigned long long* found) {
+  for (uint64_t i = 1 + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < len;
+       i += (uint64_t)gridDim.x * blockDim.x) {
+    if (__ldg(tgt + i - 1) <= __ldg(tgt + i)) continue;
+    // a row begins at entry i iff some off[u] == i; p == n means i lies inside row n-1 (off[n] = len > i)
+    const uint32_t p = tc_lower_bound(off, 0, n, (uint32_t)i);
+    if (p == n || __ldg(off + p) != i) *found = 1ull;
+  }
+}
+
+// cut[u] = the first index of row u whose target is > u, else off[u + 1]: where the reference stops its
+// walk of N(u) (triangle_count.rs:49-51) and, for u in the role of v, its walk of N(v) (:56-58).
+// One warp per row.
+__global__ void __launch_bounds__(256) k_tc_cut(const uint32_t* __restrict__ off, const uint32_t* __restrict__ tgt,
+                                                uint32_t n, uint32_t* __restrict__ cut) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+  for (uint64_t u = warp; u < n; u += nwarps) {
+    const uint64_t b = __ldg(off + u), e = __ldg(off + u + 1);
+    uint64_t c = e;
+    for (uint64_t j0 = b; j0 < e; j0 += 32) {
+      const uint64_t j = j0 + lane;
+      const unsigned hit = __ballot_sync(0xFFFFFFFFu, j < e && __ldg(tgt + j) > u);
+      if (hit) {
+        c = j0 + __ffs(hit) - 1;
+        break;
+      }
+    }
+    if (lane == 0) cut[u] = (uint32_t)c;
+  }
+}
+
+// One thread per entry i of row u with i < cut[u] (so v = tgt[i] <= u): the reference's loop for that
+// v-occurrence, in list order — a fresh cursor over all of N(u), advanced while *cursor < w, stops once
+// it runs out (oracle.c tc_vertex).
+__global__ void __launch_bounds__(256) k_tc_list(const uint32_t* __restrict__ off, const uint32_t* __restrict__ tgt,
+                                                 const uint32_t* __restrict__ cut, uint32_t n, uint64_t len,
+                                                 unsigned long long* total) {
+  unsigned long long count = 0;
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < len;
+       i += (uint64_t)gridDim.x * blockDim.x) {
+    // row of entry i: last u with off[u] <= i
+    uint32_t lo = 0, hi = n;
+    while (hi - lo > 1) {
+      const uint32_t mid = lo + ((hi - lo) >> 1);
+      if (__ldg(off + mid) <= i) lo = mid; else hi = mid;
+    }
+    const uint32_t u = lo;
+    if (i >= __ldg(cut + u)) continue;
+    const uint32_t v = __ldg(tgt + i);
+    uint32_t it = __ldg(off + u);
+    const uint32_t ue = __ldg(off + u + 1), ve = __ldg(cut + v);
+    for (uint32_t j = __ldg(off + v); j < ve; ++j) {
+      const uint32_t w = __ldg(tgt + j);
+      while (it < ue && __ldg(tgt + it) < w) ++it;
+      if (it == ue) break;  // later w find nothing either
+      count += __ldg(tgt + it) == w ? 1u : 0u;
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) count += __shfl_xor_sync(0xFFFFFFFFu, count, o);
+  if ((threadIdx.x & 31) == 0 && count) atomicAdd(total, count);
+}
+
 }  // namespace gb
 
 extern "C" gb_status gb_triangle_count(const gb_graph* g, uint64_t* triangles) {
@@ -124,14 +203,31 @@ extern "C" gb_status gb_triangle_count(const gb_graph* g, uint64_t* triangles) {
   DeviceGuard guard(g->device);
   std::lock_guard<std::mutex> lock(g->mu);
   cudaStream_t s = g->stream;
-  DevBuf<unsigned long long> total;
-  GB_TRY(total.alloc(1));
+  const DevCsr& c = g->out;
+  DevBuf<unsigned long long> total;  // [0] the count, [1] the row-order flag
+  DevBuf<uint32_t> cut;
+  GB_TRY(total.alloc(2));
   g->timing = gb_timing{};
   GB_CUDA(cudaEventRecord(g->ev_begin, s));
-  GB_CUDA(cudaMemsetAsync(total.p, 0, 8, s));
-  if (g->out.len) {
-    k_tc<<<grid_for(g->out.len, 256, H100_SMS * 32u), 256, 0, s>>>(g->out.off.p, g->out.tgt.p, g->n, g->out.len, total.p);
+  GB_CUDA(cudaMemsetAsync(total.p, 0, 16, s));
+  const unsigned grid = grid_for(c.len, 256, H100_SMS * 32u);
+  if (c.len && g->row_order == RowOrder::Unknown) {  // once per CSR
+    k_tc_rows_unsorted<<<grid, 256, 0, s>>>(c.off.p, c.tgt.p, g->n, c.len, total.p + 1);
     g->timing.kernel_launches += 1;
+    GB_CUDA(cudaGetLastError());
+    unsigned long long found = 0;
+    GB_CUDA(cudaMemcpyAsync(&found, total.p + 1, 8, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaStreamSynchronize(s));
+    g->row_order = found ? RowOrder::Unsorted : RowOrder::Sorted;
+  }
+  if (c.len && g->row_order == RowOrder::Sorted) {
+    k_tc<<<grid, 256, 0, s>>>(c.off.p, c.tgt.p, g->n, c.len, total.p);
+    g->timing.kernel_launches += 1;
+  } else if (c.len) {
+    GB_TRY(cut.alloc(g->n));
+    k_tc_cut<<<grid_for((uint64_t)g->n * 32, 256, H100_SMS * 32u), 256, 0, s>>>(c.off.p, c.tgt.p, g->n, cut.p);
+    k_tc_list<<<grid, 256, 0, s>>>(c.off.p, c.tgt.p, cut.p, g->n, c.len, total.p);
+    g->timing.kernel_launches += 2;
   }
   GB_CUDA(cudaGetLastError());
   GB_CUDA(cudaEventRecord(g->ev_end, s));

@@ -298,7 +298,9 @@ gb_status gb_wcc_sample_label(const gb_graph* graph, const gb_wcc_config* config
 gb_status gb_sssp(const gb_graph* graph, const gb_sssp_config* config, float* distances);
 gb_status gb_sssp_device(const gb_graph* graph, const gb_sssp_config* config, float* d_distances);
 
-/* global_triangle_count(&graph) -> u64                      triangle_count.rs:22-86 */
+/* global_triangle_count(&graph) -> u64                      triangle_count.rs:22-86
+ * Any row order, as the reference counts it.  The first call on a graph whose rows are not known to be
+ * sorted (an Unsorted build, gb_graph_from_csr_u32) checks them once and caches the answer. */
 gb_status gb_triangle_count(const gb_graph* graph, uint64_t* triangles);
 
 /* ---- PageRank layout statistics / multi-GPU shard (1-D edge-cut by destination) -----------------

@@ -401,7 +401,8 @@ def test_triangle_count_goldens(gb, goldens, scale8_edges):
     assert ud.global_triangle_count().triangles == sd["scale8_triangles_deduplicated"]
 
 
-@pytest.mark.parametrize("scale,layout", [(10, "Sorted"), (13, "Sorted"), (13, "Deduplicated"), (15, "Sorted")])
+@pytest.mark.parametrize("scale,layout", [(10, "Sorted"), (13, "Sorted"), (13, "Deduplicated"), (13, "Unsorted"),
+                                          (15, "Sorted")])
 def test_triangle_count_bit_exact(gb, scale, layout):
     src, dst = oracle.rmat_edges(scale, seed=42)
     n = 1 << scale

@@ -123,18 +123,20 @@ def clique(k, base=0):
 
 
 def list_pairs(lengths=(15, 16, 17, 33)):
-    """for every (Lu, Lv): an edge u-v where u and v have Lu and Lv neighbours, half of them shared"""
+    """for every (Lu, Lv): an edge u-v (v < u) whose item in k_tc cuts N(u) and N(v) to Lu and Lv entries: u
+    has Lu neighbours (v among them), v has Lv besides u, about half of them shared.  The neighbours have ids
+    below both endpoints, so every one counts toward the `<= v` prefixes."""
     src, dst, nxt = [], [], 0
     for lu in lengths:
         for lv in lengths:
-            u, v = nxt, nxt + 1
-            shared = min(lu, lv) // 2
-            common = list(range(nxt + 2, nxt + 2 + shared))
-            k = (common[-1] + 1) if common else nxt + 2
+            shared = min(lu - 1, lv) // 2
+            common = list(range(nxt, nxt + shared))
+            k = nxt + shared
             only_u = list(range(k, k + lu - 1 - shared))
             k += len(only_u)
-            only_v = list(range(k, k + lv - 1 - shared))
+            only_v = list(range(k, k + lv - shared))
             k += len(only_v)
+            v, u = k, k + 1
             for x in common + only_u:
                 src.append(u)
                 dst.append(x)
@@ -146,7 +148,7 @@ def list_pairs(lengths=(15, 16, 17, 33)):
             for i in range(0, len(common) - 1, 2):     # a few edges among the shared neighbours too
                 src.append(common[i])
                 dst.append(common[i + 1])
-            nxt = k
+            nxt = u + 1
     return np.array(src, np.uint32), np.array(dst, np.uint32), nxt
 
 
