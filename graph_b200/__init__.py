@@ -101,6 +101,7 @@ class Layout:
 class FileFormat:
     Graph500 = _Enum("FileFormat", "Graph500", 0)
     EdgeList = _Enum("FileFormat", "EdgeList", 1)
+    Binary = _Enum("FileFormat", "Binary", 2)  # SerializeGraphOp's file (input/binary.rs); see serialize()
 
 
 def _layout_value(layout) -> int:
@@ -197,10 +198,8 @@ class SsspResult:
 # and are the reference the device loader is tested against.
 def _load_args(path, file_format, layout):
     """(path bytes, format value, layout value) for gb_*_load_u32; raises what opening the file raises."""
-    if file_format is FileFormat.Graph500:
-        fmt = 0
-    elif file_format is FileFormat.EdgeList:
-        fmt = 1
+    if file_format in (FileFormat.Graph500, FileFormat.EdgeList, FileFormat.Binary):
+        fmt = file_format.value
     else:
         raise TypeError(f"unknown file format {file_format!r}")
     path = os.fspath(path)
@@ -242,6 +241,24 @@ def _read_edge_list(path, with_values=False):
     w = np.empty(m.value, np.float32) if with_values else None
     check(lib.gb_edge_list_parse(text, len(text), _ptr(src), _ptr(dst), _ptr(w), C.byref(m)))
     return (src, dst, w) if with_values else (src, dst)
+
+
+def _decode_binary(data: bytes, directed: bool, with_values: bool = False):
+    """The host decoder of binary graph files (gb_binary_decode): (out_offsets, out_targets, out_values,
+    in_offsets, in_targets) for a directed file, (offsets, targets) for an undirected one.  out_values is None
+    unless with_values; in-CSR values are never returned."""
+    raw = np.frombuffer(data, np.uint8)
+    kind = _capi.KIND_DIRECTED if directed else _capi.KIND_UNDIRECTED
+    n, m, hv = C.c_uint32(0), C.c_uint64(0), C.c_int(0)
+    args = (_ptr(raw) if raw.size else None, raw.size, kind, C.byref(n), C.byref(m), C.byref(hv))
+    check(lib.gb_binary_decode(*args, None, None, None, None, None))
+    if with_values and not hv.value:
+        raise ValueError("the binary graph file holds no edge values")
+    csrs = [(np.empty(n.value + 1, np.uint32), np.empty(m.value, np.uint32)) for _ in range(2 if directed else 1)]
+    w = np.empty(m.value, np.float32) if with_values else None
+    inc = csrs[1] if directed else (None, None)
+    check(lib.gb_binary_decode(*args, _ptr(csrs[0][0]), _ptr(csrs[0][1]), _ptr(w), _ptr(inc[0]), _ptr(inc[1])))
+    return (*csrs[0], w, *csrs[1]) if directed else csrs[0]
 
 
 def _check_host_csr(off: np.ndarray, tgt: np.ndarray, what: str) -> None:
@@ -388,6 +405,13 @@ class _Handle:
         check(lib.gb_graph_load_info(self._g, C.byref(info)))
         return info.as_dict()
 
+    def serialize(self, path) -> None:
+        """SerializeGraphOp::serialize (graph_ops.rs:232-238): writes the graph as the binary file that
+        `load(path, file_format=FileFormat.Binary)` here and DeserializeGraphOp in the reference read (NI = u32;
+        a weighted digraph writes Target<u32, f32> records for both CSRs).  The file is written next to `path`
+        under a temporary name and renamed over it."""
+        check(lib.gb_graph_serialize(self._g, os.fsencode(os.fspath(path))))
+
     def __repr__(self):
         return (f"{type(self).__name__} {{ node_count: {self.node_count()}, edge_count: {self.edge_count()}, "
                 f"load_took: {_took(self.load_micros)} }}")
@@ -426,9 +450,12 @@ class DiGraph(_Handle):
         return _construct(DiGraph, lib.gb_digraph_load_u32, _device, *_load_args(path, file_format, layout), 0)
 
     @staticmethod
-    def load_weighted(path, layout=None) -> "DiGraph":
-        """Weighted text edge list `<src> <dst> <f32>` (DirectedCsrGraph<u32, (), f32>, for sssp)."""
-        return _construct(DiGraph, lib.gb_digraph_load_u32, _device, *_load_args(path, FileFormat.EdgeList, layout), 1)
+    def load_weighted(path, layout=None, file_format=FileFormat.EdgeList) -> "DiGraph":
+        """Weighted text edge list `<src> <dst> <f32>`, or a binary file with Target<NI, f32> records
+        (DirectedCsrGraph<u32, (), f32>, for sssp)."""
+        if file_format is FileFormat.Graph500:
+            raise ValueError("Graph500 files carry no edge values")
+        return _construct(DiGraph, lib.gb_digraph_load_u32, _device, *_load_args(path, file_format, layout), 1)
 
     @staticmethod
     def from_torch(src, dst, weights=None, node_count: int = 0, layout=None) -> "DiGraph":

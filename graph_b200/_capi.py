@@ -96,6 +96,9 @@ SIGNATURES = {
     "gb_graph500_decode": (C.c_int, [_P, C.c_uint64, _P, _P, C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]),
     "gb_graph500_encode": (C.c_int, [_P, _P, C.c_uint64, _P]),
     "gb_edge_list_parse": (C.c_int, [C.c_char_p, C.c_uint64, _P, _P, _P, C.POINTER(C.c_uint64)]),
+    "gb_binary_decode": (C.c_int, [_P, C.c_uint64, C.c_int, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64),
+                                   C.POINTER(C.c_int), _P, _P, _P, _P, _P]),
+    "gb_graph_serialize": (C.c_int, [_P, C.c_char_p]),
     "gb_digraph_load_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
     "gb_graph_load_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.c_int, C.POINTER(_P)]),
     "gb_graph_load_info": (C.c_int, [_P, C.POINTER(LoadInfo)]),

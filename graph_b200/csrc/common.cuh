@@ -227,6 +227,11 @@ gb_status graph_from_device_arrays(int device, gb_graph_kind kind, const uint32_
                                    const float* d_w, uint64_t m, uint32_t n, gb_layout layout, cudaStream_t caller,
                                    gb_graph** out);
 
+// Values for a weighted digraph's in-CSR (graph.cu): the k-th occurrence of s in in-row t gets the value of the
+// k-th occurrence of t in out-row s.  Fails when the in-CSR is not the transpose of the out-CSR.  Runs on the
+// graph's stream; the caller holds g->mu.
+gb_status in_csr_values(const gb_graph* g, DevBuf<float>* in_w);
+
 constexpr unsigned H100_SMS = 132;  // streaming multiprocessors of an H100 SXM: sizes the grid-stride grids
 
 inline unsigned grid_for(uint64_t items, unsigned block, unsigned max_blocks = H100_SMS * 16u) {

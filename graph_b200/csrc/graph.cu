@@ -499,6 +499,56 @@ gb_status graph_from_device_arrays(int device, gb_graph_kind kind, const uint32_
   return GB_OK;
 }
 
+__global__ void k_count_diff(const uint32_t* __restrict__ a, const uint32_t* __restrict__ b, uint64_t count,
+                             unsigned int* __restrict__ bad) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
+       i += (uint64_t)gridDim.x * blockDim.x)
+    if (a[i] != b[i]) atomicAdd(bad, 1u);
+}
+
+__global__ void k_scatter_values(const float* __restrict__ w, const uint32_t* __restrict__ pos, uint64_t count,
+                                 float* __restrict__ out) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
+       i += (uint64_t)gridDim.x * blockDim.x)
+    out[pos[i]] = w[i];
+}
+
+// Both CSRs are re-sorted by (t, s) with the stable build: the out-CSR's entries, transposed, carry their
+// values, and equal keys stay in out-row order; the in-CSR's entries carry their position, and equal keys stay
+// in in-row order.  Equal key sequences pair the k-th occurrences, and the values are scattered by position.
+gb_status in_csr_values(const gb_graph* g, DevBuf<float>* in_w) {
+  cudaStream_t s = g->stream;
+  const uint32_t n = g->n;
+  const uint64_t m = g->out.len;
+  GB_REQUIRE(g->in.len == m && g->in.tgt.p && g->out.w.p, "the graph has no weighted out-CSR and in-CSR pair");
+  GB_TRY(in_w->alloc(m, 8));
+  if (m == 0) return GB_OK;
+  DevBuf<uint32_t> rows, pos;
+  GB_TRY(rows.alloc(m));
+  GB_TRY(pos.alloc(m));
+  const unsigned grid_rows = grid_for((uint64_t)n * 32, 256);
+  k_expand_rows<<<grid_rows, 256, 0, s>>>(g->out.off.p, n, rows.p);
+  DevCsr tr;  // rows t, targets s, out values
+  GB_TRY(build_csr_device(s, n, g->out.tgt.p, rows.p, g->out.w.p, m, GB_LAYOUT_SORTED, &tr));
+  k_expand_rows<<<grid_rows, 256, 0, s>>>(g->in.off.p, n, rows.p);
+  k_iota<<<grid_for(m, 256), 256, 0, s>>>(pos.p, m);
+  DevCsr in;  // rows t, targets s, in-CSR positions (the build moves the 32-bit "values" without reading them)
+  GB_TRY(build_csr_device(s, n, rows.p, g->in.tgt.p, reinterpret_cast<const float*>(pos.p), m, GB_LAYOUT_SORTED,
+                          &in));
+  DevBuf<unsigned int> bad;
+  GB_TRY(bad.alloc(1));
+  GB_CUDA(cudaMemsetAsync(bad.p, 0, 4, s));
+  k_count_diff<<<grid_for((uint64_t)n + 1, 256), 256, 0, s>>>(tr.off.p, in.off.p, (uint64_t)n + 1, bad.p);
+  k_count_diff<<<grid_for(m, 256), 256, 0, s>>>(tr.tgt.p, in.tgt.p, m, bad.p);
+  k_scatter_values<<<grid_for(m, 256), 256, 0, s>>>(tr.w.p, reinterpret_cast<const uint32_t*>(in.w.p), m, in_w->p);
+  GB_CUDA(cudaGetLastError());
+  unsigned int h = 0;
+  GB_CUDA(cudaMemcpyAsync(&h, bad.p, 4, cudaMemcpyDeviceToHost, s));
+  GB_CUDA(cudaStreamSynchronize(s));
+  GB_REQUIRE(h == 0, "the in-CSR is not the transpose of the out-CSR: no in-CSR values can be written");
+  return GB_OK;
+}
+
 template <typename T>
 __global__ void k_ids_to_u32(const T* __restrict__ in, uint64_t count, uint32_t* __restrict__ out,
                              unsigned int* __restrict__ bad) {

@@ -28,6 +28,7 @@
 
 #include <cub/cub.cuh>
 
+#include "binary_format.h"
 #include "common.cuh"
 #include "edgelist_line.h"
 #include "edgelist_scan.h"
@@ -150,6 +151,39 @@ __global__ void k_load_patch(const uint32_t* __restrict__ edge, const float* __r
     w[edge[i]] = val[i];
 }
 
+// 32 bits at an unaligned byte position of a device buffer whose base is 4-byte aligned (may read 4 bytes past)
+__device__ __forceinline__ uint32_t load_u32_at(const uint8_t* base, uint64_t pos) {
+  const uint32_t* w = reinterpret_cast<const uint32_t*>(base + (pos & ~3ull));
+  const uint32_t shift = (uint32_t)(pos & 3) * 8;
+  return shift ? __funnelshift_r(w[0], w[1], shift) : w[0];
+}
+
+// Binary files: elements [first, first + count) of a section staged in buf, whose byte 0 is file byte buf_off.
+// Element e starts at file byte sec + e * stride with an id of id_bytes (u64 ids are narrowed; a high word
+// that is not 0 sets *wide), followed by an f32 value that goes to w[e] when w is not NULL.
+__global__ void k_bin_split(const uint8_t* __restrict__ buf, uint64_t buf_off, uint64_t sec, uint32_t stride,
+                            uint32_t id_bytes, uint64_t first, uint64_t count, uint32_t* __restrict__ ids,
+                            float* __restrict__ w, unsigned int* __restrict__ wide) {
+  bool big = false;
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
+       i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t e = first + i;
+    const uint64_t pos = sec + e * stride - buf_off;
+    ids[e] = load_u32_at(buf, pos);
+    if (id_bytes == 8) big |= load_u32_at(buf, pos + 4) != 0;
+    if (w) w[e] = __uint_as_float(load_u32_at(buf, pos + id_bytes));
+  }
+  if (__any_sync(0xFFFFFFFFu, big) && (threadIdx.x & 31) == 0) atomicOr(wide, 1u);
+}
+
+// Target<u32, f32> records (8 bytes, #[repr(C)]) from the SoA arrays, for the writer
+__global__ void k_bin_interleave(const uint32_t* __restrict__ tgt, const float* __restrict__ w, uint64_t count,
+                                 uint2* __restrict__ out) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
+       i += (uint64_t)gridDim.x * blockDim.x)
+    out[i] = make_uint2(tgt[i], __float_as_uint(w[i]));
+}
+
 // ---- host side ---------------------------------------------------------------------------------------
 static uint64_t env_chunk_bytes() {
   const char* s = std::getenv("GB_LOAD_CHUNK_BYTES");
@@ -218,7 +252,15 @@ struct ChunkReader {
   uint64_t chunk_bytes(uint64_t k) const { return std::min(chunk, read_end - k * chunk); }
   char* data(unsigned r) { return host[r].p + LOAD_CARRY_RESERVE; }
 
+  // the reader threads over the ring
   gb_status start() {
+    GB_TRY(acquire());
+    for (unsigned r = 0; r < ring; ++r) threads.emplace_back([this, r] { run(r); });
+    return GB_OK;
+  }
+
+  // the pinned buffers and their events alone (the binary writer fills them from the device)
+  gb_status acquire() {
     host.resize(ring);
     copied.assign(ring, nullptr);
     filled.assign(ring, 0);
@@ -254,7 +296,6 @@ struct ChunkReader {
       if (!cached) GB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&host[r].p), bytes, cudaHostAllocDefault));
       GB_CUDA(cudaEventCreateWithFlags(&copied[r], cudaEventDisableTiming));
     }
-    for (unsigned r = 0; r < ring; ++r) threads.emplace_back([this, r] { run(r); });
     return GB_OK;
   }
 
@@ -553,6 +594,205 @@ static gb_status load_file(int device, const char* path, gb_file_format format, 
   return GB_OK;
 }
 
+// pinned buffer size for streaming `bytes`: GB_LOAD_CHUNK_BYTES, else a quarter of the file within
+// [LOAD_MIN_CHUNK, LOAD_DEFAULT_CHUNK] so that a small file keeps every buffer busy
+static uint64_t ring_chunk(uint64_t bytes) {
+  uint64_t chunk = env_chunk_bytes();
+  if (chunk == 0) {
+    const uint64_t quarter = (bytes / LOAD_RING + 4095) & ~(uint64_t)4095;
+    chunk = std::min(LOAD_DEFAULT_CHUNK, std::max(LOAD_MIN_CHUNK, quarter));
+  }
+  return std::max<uint64_t>(chunk, 16);  // >= the largest record: an element spans at most two chunks
+}
+
+// The CSR arrays a binary file's section fills.  Elements of `stride` bytes start at file byte `pos`; a u32
+// section without values (stride 4) is DMA'd straight into `ids`, the others are staged and split by
+// k_bin_split.
+struct BinSection {
+  uint64_t pos = 0, count = 0;
+  uint32_t stride = 0;
+  uint32_t* ids = nullptr;
+  float* w = nullptr;
+  bool direct() const { return stride == 4; }
+  uint64_t end() const { return pos + count * stride; }
+};
+
+// the checks of gb_binary_decode on the device arrays: offsets[0] == 0, monotone, offsets[n] == entries, targets
+// below n; `wide` is the flag of the narrowing kernel
+static gb_status check_loaded_csrs(gb_graph* g, const BinLayout& l, DevCsr* const* csr, unsigned int* d_wide,
+                                   cudaStream_t s) {
+  DevBuf<unsigned int> bad;  // per CSR: [2c] targets >= n, [2c + 1] decreasing rows
+  DevBuf<uint32_t> ends;     // per CSR: offsets[0], offsets[n]
+  GB_TRY(bad.alloc(4));
+  GB_TRY(ends.alloc(4));
+  GB_CUDA(cudaMemsetAsync(bad.p, 0, 16, s));
+  for (unsigned c = 0; c < l.ncsr; ++c) {
+    check_ids_async(s, csr[c]->tgt.p, l.entries, l.n, bad.p + 2 * c);
+    check_monotone_async(s, csr[c]->off.p, l.n, bad.p + 2 * c + 1);
+    GB_CUDA(cudaMemcpyAsync(ends.p + 2 * c, csr[c]->off.p, 4, cudaMemcpyDeviceToDevice, s));
+    GB_CUDA(cudaMemcpyAsync(ends.p + 2 * c + 1, csr[c]->off.p + l.n, 4, cudaMemcpyDeviceToDevice, s));
+  }
+  GB_CUDA(cudaGetLastError());
+  unsigned int h[5] = {0, 0, 0, 0, 0};
+  uint32_t e[4] = {0, 0, 0, 0};
+  GB_CUDA(cudaMemcpyAsync(h, bad.p, 16, cudaMemcpyDeviceToHost, s));
+  GB_CUDA(cudaMemcpyAsync(h + 4, d_wide, 4, cudaMemcpyDeviceToHost, s));
+  GB_CUDA(cudaMemcpyAsync(e, ends.p, 16, cudaMemcpyDeviceToHost, s));
+  GB_CUDA(cudaStreamSynchronize(s));
+  GB_REQUIRE(h[4] == 0, "binary graph file: an id or offset does not fit 32 bits");
+  for (unsigned c = 0; c < l.ncsr; ++c) {
+    const char* what = bin_csr_name(l, c);
+    GB_REQUIRE(e[2 * c] == 0, "%s offsets[0] must be 0", what);
+    GB_REQUIRE(h[2 * c + 1] == 0, "%s offsets are not monotone (%u rows)", what, h[2 * c + 1]);
+    GB_REQUIRE(e[2 * c + 1] == l.entries, "%s offsets end at %u, not at its %llu entries", what, e[2 * c + 1],
+               (unsigned long long)l.entries);
+    GB_REQUIRE(h[2 * c] == 0, "%s CSR holds %u targets >= node_count %u", what, h[2 * c], g->n);
+  }
+  return GB_OK;
+}
+
+// Binary graph files on the device: the host preads the headers (bin_parse gives the section table), then the
+// ring streams the file and every chunk is cut against the table.  Direct sections go from the pinned buffer
+// to their CSR array at their byte offset; when a chunk meets a staged section, the chunk goes to a device
+// buffer with the bytes of the element it cuts in front (at most 15, carried from the chunk before), and
+// k_bin_split decodes the elements that end inside the chunk.
+static gb_status load_binary_streamed(int device, gb_graph_kind kind, const char* path, bool want_value,
+                                      gb_graph** graph, gb_load_info* info) {
+  FileHandle f;
+  f.fd = ::open(path, O_RDONLY | O_CLOEXEC);
+  if (f.fd < 0) return fail(GB_ERR_INVALID, "cannot open %s: %s", path, std::strerror(errno));
+  struct stat st {};
+  if (::fstat(f.fd, &st) != 0 || !S_ISREG(st.st_mode)) return fail(GB_ERR_INVALID, "%s is not a regular file", path);
+  const uint64_t size = (uint64_t)st.st_size;
+  info->file_bytes = size;
+  BinLayout l;
+  GB_TRY(bin_parse([&](uint64_t pos, void* dst, uint64_t n) { return pread_all(f.fd, static_cast<char*>(dst), n, pos); },
+                   size, kind, &l));
+  GB_REQUIRE(!want_value || l.values, "the binary graph file holds no edge values");
+  GraphPtr g;
+  GB_TRY(new_graph(device, kind, l.n, &g));
+
+  StreamPair sp;
+  GB_CUDA(cudaStreamCreateWithFlags(&sp.copy, cudaStreamNonBlocking));
+  GB_CUDA(cudaStreamCreateWithFlags(&sp.work, cudaStreamNonBlocking));
+  DevBufStreamScope scope(sp.work);
+  DevCsr* csr[2] = {&g->out, &g->in};
+  std::vector<BinSection> secs;
+  for (unsigned c = 0; c < l.ncsr; ++c) {
+    DevCsr& d = *csr[c];
+    d.len = l.entries;
+    GB_TRY(d.off.alloc((size_t)l.n + 1));
+    GB_TRY(d.tgt.alloc(l.entries, 8));
+    GB_CUDA(cudaMemsetAsync(d.tgt.p + l.entries, 0, 8 * 4, sp.work));
+    if (c == 0 && want_value) GB_TRY(d.w.alloc(l.entries, 8));  // only a digraph's out-CSR keeps values
+    BinSection o, t;
+    o.pos = l.csr[c].off_pos, o.count = (uint64_t)l.n + 1, o.stride = l.id_bytes, o.ids = d.off.p;
+    t.pos = l.csr[c].rec_pos, t.count = l.entries, t.stride = l.rec_bytes, t.ids = d.tgt.p, t.w = d.w.p;
+    secs.push_back(o);
+    if (t.count) secs.push_back(t);
+  }
+
+  ChunkReader rd;
+  rd.fd = f.fd;
+  rd.device = device;
+  rd.read_end = size;
+  rd.chunk = ring_chunk(size);
+  rd.nchunks = (size + rd.chunk - 1) / rd.chunk;
+  rd.ring = (unsigned)std::min<uint64_t>(LOAD_RING, rd.nchunks);
+  info->chunks = rd.nchunks;
+  GB_TRY(rd.start());
+  const unsigned R = rd.ring;
+  std::vector<DevBuf<uint8_t>> dbuf(R);
+  std::vector<cudaEvent_t> parsed(R, nullptr);
+  struct Events {
+    std::vector<cudaEvent_t>* v;
+    ~Events() {
+      for (cudaEvent_t e : *v)
+        if (e) cudaEventDestroy(e);
+    }
+  } parsed_guard{&parsed};
+  for (unsigned r = 0; r < R; ++r) GB_CUDA(cudaEventCreateWithFlags(&parsed[r], cudaEventDisableTiming));
+  DevBuf<unsigned int> wide;
+  GB_TRY(wide.alloc(1));
+  GB_CUDA(cudaMemsetAsync(wide.p, 0, 4, sp.work));
+  struct Drain {
+    StreamPair* sp;
+    ~Drain() { cudaStreamSynchronize(sp->copy); }
+  } drain{&sp};
+
+  std::vector<uint64_t> staged_off(R, 0);  // file byte of dbuf[r][0], or ~0: the chunk was not staged
+  std::string carry;                       // bytes of the staged element that the next chunk completes
+  uint64_t h2d = 0;
+  auto prepare = [&](uint64_t k) -> gb_status {
+    const unsigned r = (unsigned)(k % R);
+    GB_TRY(rd.wait_filled(k));
+    char* data = rd.data(r);
+    const uint64_t a = k * rd.chunk, len = rd.chunk_bytes(k), b = a + len;
+    bool stage = false;
+    for (const BinSection& s : secs) stage |= !s.direct() && s.pos < b && s.end() > a;
+    const uint64_t cl = stage ? carry.size() : 0;
+    staged_off[r] = stage ? a - cl : ~0ull;
+    if (stage) {
+      if (dbuf[r].n < cl + len + 16) {
+        GB_CUDA(cudaEventSynchronize(parsed[r]));
+        DevBuf<uint8_t> nb;
+        GB_TRY(nb.alloc(std::max<uint64_t>(cl + len, rd.chunk + 16) + 16));
+        dbuf[r] = std::move(nb);
+      }
+      GB_CUDA(cudaStreamWaitEvent(sp.copy, parsed[r], 0));  // the kernels that read this device buffer are done
+      std::memcpy(data - cl, carry.data(), cl);
+      GB_CUDA(cudaMemcpyAsync(dbuf[r].p, data - cl, cl + len, cudaMemcpyHostToDevice, sp.copy));
+      h2d += cl + len;
+    }
+    for (const BinSection& s : secs) {
+      if (!s.direct()) continue;
+      const uint64_t x = std::max(a, s.pos), y = std::min(b, s.end());
+      if (x >= y) continue;
+      GB_CUDA(cudaMemcpyAsync(reinterpret_cast<char*>(s.ids) + (x - s.pos), data + (x - a), y - x,
+                              cudaMemcpyHostToDevice, sp.copy));
+      h2d += y - x;
+    }
+    carry.clear();
+    for (const BinSection& s : secs)
+      if (!s.direct() && s.pos < b && s.end() > b) {
+        const uint64_t cut = (b - s.pos) % s.stride;  // bytes of the element that begins before b
+        carry.assign(data + (len - cut), cut);
+      }
+    GB_CUDA(cudaEventRecord(rd.copied[r], sp.copy));
+    rd.release(k);
+    GB_CUDA(cudaStreamWaitEvent(sp.work, rd.copied[r], 0));
+    return GB_OK;
+  };
+  auto split = [&](uint64_t k) -> gb_status {
+    const unsigned r = (unsigned)(k % R);
+    if (staged_off[r] == ~0ull) return GB_OK;
+    const uint64_t a = k * rd.chunk, b = a + rd.chunk_bytes(k);
+    for (const BinSection& s : secs) {
+      if (s.direct() || s.pos >= b || s.end() <= a) continue;
+      const uint64_t first = a > s.pos ? (a - s.pos) / s.stride : 0;  // the first element that ends after a
+      const uint64_t last = std::min(s.count, (b - s.pos) / s.stride);  // elements that end by b
+      if (last <= first) continue;
+      k_bin_split<<<grid_for(last - first, 256), 256, 0, sp.work>>>(dbuf[r].p, staged_off[r], s.pos, s.stride,
+                                                                      l.id_bytes, first, last - first, s.ids, s.w,
+                                                                      wide.p);
+      GB_CUDA(cudaGetLastError());
+    }
+    GB_CUDA(cudaEventRecord(parsed[r], sp.work));
+    return GB_OK;
+  };
+  GB_TRY(prepare(0));
+  for (uint64_t k = 0; k < rd.nchunks; ++k) {
+    if (k + 1 < rd.nchunks) GB_TRY(prepare(k + 1));  // the next chunk crosses the bus meanwhile
+    GB_TRY(split(k));
+  }
+  GB_CUDA(cudaStreamSynchronize(sp.copy));
+  GB_TRY(check_loaded_csrs(g.get(), l, csr, wide.p, sp.work));
+  info->edges = kind == GB_KIND_DIRECTED ? l.entries : l.entries / 2;
+  info->h2d_bytes = h2d;
+  *graph = g.release();
+  return GB_OK;
+}
+
 // Below these sizes the fixed costs of the pipeline (threads, streams, pinned ring) exceed what it saves, and
 // the host readers are faster (H100 80GB HBM3, 400 W; tools/bench_load.py).  GB_LOAD_CHUNK_BYTES, when
 // set, selects the device path whatever the size.
@@ -596,19 +836,169 @@ static gb_status load_on_host(int device, gb_graph_kind kind, const char* path, 
   return GB_OK;
 }
 
+// a small binary file: gb_binary_decode, then the upload of gb_[di]graph_from_csr_u32
+static gb_status load_binary_on_host(int device, gb_graph_kind kind, const char* path, bool want_value,
+                                     gb_graph** graph, gb_load_info* info) {
+  FileHandle f;
+  f.fd = ::open(path, O_RDONLY | O_CLOEXEC);
+  if (f.fd < 0) return fail(GB_ERR_INVALID, "cannot open %s: %s", path, std::strerror(errno));
+  struct stat st {};
+  if (::fstat(f.fd, &st) != 0 || !S_ISREG(st.st_mode)) return fail(GB_ERR_INVALID, "%s is not a regular file", path);
+  const uint64_t len = (uint64_t)st.st_size;
+  std::vector<char> bytes(len);
+  if (len && !pread_all(f.fd, bytes.data(), len, 0)) return fail(GB_ERR_INVALID, "reading %s failed", path);
+  uint32_t n = 0;
+  uint64_t m = 0;
+  int has_values = 0;
+  GB_TRY(gb_binary_decode(bytes.data(), len, kind, &n, &m, &has_values, nullptr, nullptr, nullptr, nullptr, nullptr));
+  GB_REQUIRE(!want_value || has_values, "the binary graph file holds no edge values");
+  const unsigned ncsr = kind == GB_KIND_DIRECTED ? 2 : 1;
+  std::vector<uint32_t> off[2], tgt[2];
+  std::vector<float> w(want_value ? m : 0);
+  for (unsigned c = 0; c < ncsr; ++c) off[c].resize((size_t)n + 1), tgt[c].resize(m);
+  GB_TRY(gb_binary_decode(bytes.data(), len, kind, &n, &m, &has_values, off[0].data(), tgt[0].data(),
+                          want_value ? w.data() : nullptr, off[1].data(), tgt[1].data()));
+  GraphPtr g;
+  GB_TRY(new_graph(device, kind, n, &g));
+  GB_TRY(upload_host_csr(g->stream, n, off[0].data(), tgt[0].data(), want_value ? w.data() : nullptr, &g->out,
+                         kind == GB_KIND_DIRECTED ? "csr_out" : "csr"));
+  if (kind == GB_KIND_DIRECTED)
+    GB_TRY(upload_host_csr(g->stream, n, off[1].data(), tgt[1].data(), nullptr, &g->in, "csr_inc"));
+  *graph = g.release();
+  info->file_bytes = len;
+  info->edges = kind == GB_KIND_DIRECTED ? m : m / 2;
+  info->h2d_bytes = ncsr * (((uint64_t)n + 1) * 4 + m * 4) + (want_value ? m * 4 : 0);
+  return GB_OK;
+}
+
+static bool pwrite_all(int fd, const char* src, uint64_t bytes, uint64_t off) {
+  while (bytes) {
+    const ssize_t r = ::pwrite(fd, src, bytes, (off_t)off);
+    if (r < 0 && errno == EINTR) continue;
+    if (r <= 0) return false;
+    src += r;
+    off += (uint64_t)r;
+    bytes -= (uint64_t)r;
+  }
+  return true;
+}
+
+// the file being written; removed unless it was renamed over the destination
+struct TempFile {
+  std::string path;
+  int fd = -1;
+  bool renamed = false;
+  ~TempFile() {
+    if (fd >= 0) ::close(fd);
+    if (!renamed && !path.empty()) ::unlink(path.c_str());
+  }
+};
+
+// SerializeGraphOp::serialize: the file is a sequence of pieces (headers from host memory, arrays from device
+// memory; Target<u32, f32> records are interleaved on the device first) that the pinned ring carries to the
+// file: chunk k + 1 is copied from the device on a copy stream while chunk k is written with pwrite.
+static gb_status serialize_graph(const gb_graph* g, const char* path) {
+  GB_REQUIRE(g && path, "NULL argument");
+  GB_REQUIRE(g->out.tgt.p != nullptr, "this handle holds no out targets (page-rank-only twin) and cannot be serialized");
+  DeviceGuard guard(g->device);
+  std::lock_guard<std::mutex> lock(g->mu);
+  const bool values = g->kind == GB_KIND_DIRECTED && g->out.w.p != nullptr;
+  const BinLayout l = bin_layout_u32(g->kind, g->n, g->out.len, values);
+  const DevCsr* csr[2] = {&g->out, &g->in};
+  DevBuf<float> in_w;
+  if (values) GB_TRY(in_csr_values(g, &in_w));
+  struct Piece {
+    uint64_t pos, len;
+    const void* src;
+    bool device;
+  };
+  std::vector<Piece> pieces;
+  std::string headers[2];
+  DevBuf<uint2> records[2];
+  for (unsigned c = 0; c < l.ncsr; ++c) {
+    headers[c] = bin_header_bytes(l, c);
+    pieces.push_back({c == 0 ? 0 : l.csr[c].header, headers[c].size(), headers[c].data(), false});
+    pieces.push_back({l.csr[c].off_pos, ((uint64_t)l.n + 1) * 4, csr[c]->off.p, true});
+    if (!l.entries) continue;
+    if (values) {
+      GB_TRY(records[c].alloc(l.entries));
+      k_bin_interleave<<<grid_for(l.entries, 256), 256, 0, g->stream>>>(csr[c]->tgt.p, c == 0 ? g->out.w.p : in_w.p,
+                                                                         l.entries, records[c].p);
+      GB_CUDA(cudaGetLastError());
+      pieces.push_back({l.csr[c].rec_pos, l.entries * 8, records[c].p, true});
+    } else {
+      pieces.push_back({l.csr[c].rec_pos, l.entries * 4, csr[c]->tgt.p, true});
+    }
+  }
+  GB_CUDA(cudaStreamSynchronize(g->stream));
+
+  TempFile tmp;
+  tmp.path = std::string(path) + ".XXXXXX";
+  tmp.fd = ::mkstemp(&tmp.path[0]);
+  if (tmp.fd < 0) {
+    tmp.path.clear();
+    return fail(GB_ERR_INVALID, "cannot create a temporary file next to %s: %s", path, std::strerror(errno));
+  }
+  ::fchmod(tmp.fd, 0644);
+  const uint64_t total = l.file_bytes;
+  ChunkReader ring;  // its pinned buffers and events only: no reader threads
+  ring.device = g->device;
+  ring.chunk = ring_chunk(total);
+  ring.read_end = total;
+  ring.nchunks = (total + ring.chunk - 1) / ring.chunk;
+  ring.ring = (unsigned)std::min<uint64_t>(LOAD_RING, ring.nchunks);  // >= 2 whenever there is a next chunk
+  GB_TRY(ring.acquire());
+  StreamPair sp;
+  GB_CUDA(cudaStreamCreateWithFlags(&sp.copy, cudaStreamNonBlocking));
+  auto fill = [&](uint64_t k) -> gb_status {
+    const unsigned r = (unsigned)(k % ring.ring);
+    char* data = ring.data(r);
+    const uint64_t a = k * ring.chunk, b = a + ring.chunk_bytes(k);
+    for (const Piece& p : pieces) {
+      const uint64_t x = std::max(a, p.pos), y = std::min(b, p.pos + p.len);
+      if (x >= y) continue;
+      const char* src = static_cast<const char*>(p.src) + (x - p.pos);
+      if (p.device) GB_CUDA(cudaMemcpyAsync(data + (x - a), src, y - x, cudaMemcpyDeviceToHost, sp.copy));
+      else std::memcpy(data + (x - a), src, y - x);
+    }
+    GB_CUDA(cudaEventRecord(ring.copied[r], sp.copy));
+    return GB_OK;
+  };
+  GB_TRY(fill(0));
+  for (uint64_t k = 0; k < ring.nchunks; ++k) {
+    if (k + 1 < ring.nchunks) GB_TRY(fill(k + 1));  // its buffer was written out R - 1 chunks ago
+    const unsigned r = (unsigned)(k % ring.ring);
+    GB_CUDA(cudaEventSynchronize(ring.copied[r]));
+    if (!pwrite_all(tmp.fd, ring.data(r), ring.chunk_bytes(k), k * ring.chunk))
+      return fail(GB_ERR_INVALID, "writing %s failed: %s", tmp.path.c_str(), std::strerror(errno));
+  }
+  const int fd = tmp.fd;
+  tmp.fd = -1;
+  if (::close(fd) != 0) return fail(GB_ERR_INVALID, "writing %s failed: %s", tmp.path.c_str(), std::strerror(errno));
+  if (::rename(tmp.path.c_str(), path) != 0)
+    return fail(GB_ERR_INVALID, "cannot rename %s to %s: %s", tmp.path.c_str(), path, std::strerror(errno));
+  tmp.renamed = true;
+  return GB_OK;
+}
+
 static gb_status load_graph(int device, gb_graph_kind kind, const char* path, gb_file_format format,
                             gb_layout layout, int with_values, gb_graph** graph) {
   GB_REQUIRE(graph != nullptr, "graph out-pointer is NULL");
   GB_REQUIRE(path != nullptr, "path is NULL");
-  GB_REQUIRE(format == GB_FORMAT_GRAPH500 || format == GB_FORMAT_EDGE_LIST, "unknown file format %d", (int)format);
-  GB_REQUIRE(!with_values || format == GB_FORMAT_EDGE_LIST, "only edge lists carry edge values");
+  GB_REQUIRE(format == GB_FORMAT_GRAPH500 || format == GB_FORMAT_EDGE_LIST || format == GB_FORMAT_BINARY,
+             "unknown file format %d", (int)format);
+  GB_REQUIRE(!with_values || format != GB_FORMAT_GRAPH500, "only edge lists and binary files carry edge values");
   GB_TRY(check_layout(layout));
   GB_TRY(require_device(device));
   DeviceGuard guard(device);
   struct stat st {};
   if (::stat(path, &st) != 0) return fail(GB_ERR_INVALID, "cannot open %s: %s", path, std::strerror(errno));
   gb_load_info info{};
-  if (env_chunk_bytes() == 0 && (uint64_t)st.st_size < LOAD_DEVICE_MIN_BYTES) {
+  const bool on_host = env_chunk_bytes() == 0 && (uint64_t)st.st_size < LOAD_DEVICE_MIN_BYTES;
+  if (format == GB_FORMAT_BINARY) {
+    if (on_host) GB_TRY(load_binary_on_host(device, kind, path, with_values != 0, graph, &info));
+    else GB_TRY(load_binary_streamed(device, kind, path, with_values != 0, graph, &info));
+  } else if (on_host) {
     GB_TRY(load_on_host(device, kind, path, format, layout, with_values != 0, graph, &info));
   } else {
     LoadedEdges e;
@@ -633,6 +1023,8 @@ gb_status gb_graph_load_u32(int device, const char* path, gb_file_format format,
                             gb_graph** graph) {
   return gb::load_graph(device, GB_KIND_UNDIRECTED, path, format, layout, 0, graph);
 }
+
+gb_status gb_graph_serialize(const gb_graph* graph, const char* path) { return gb::serialize_graph(graph, path); }
 
 gb_status gb_graph_load_info(const gb_graph* g, gb_load_info* info) {
   GB_REQUIRE(g && info, "NULL argument");

@@ -174,6 +174,16 @@ gb_status gb_graph500_encode(const uint32_t* src, const uint32_t* dst, uint64_t 
  * NULL.  Edges come out in file order. */
 gb_status gb_edge_list_parse(const char* text, uint64_t len, uint32_t* src, uint32_t* dst,
                              float* values, uint64_t* edge_count);
+/* Binary graph file of SerializeGraphOp (graph_ops.rs:232-238; csr.rs:252-341, :606-656, :817-851; the
+ * layout is restated in graph_b200/csrc/binary_format.h): NI "u32", "u64" or "usize", records with or
+ * without f32 values (told apart by the file size).  Call with out_offsets == NULL to check the headers and
+ * obtain *node_count, *entries (targets per CSR; undirected: 2m) and *has_values; then again with arrays of
+ * node_count + 1 offsets and `entries` targets (in_* only for a directed file).  out_values may be NULL (the
+ * values are dropped) and must be NULL for a file without values; in-CSR values are never returned.  u64
+ * ids are narrowed; ids or offsets >= 2^32, malformed offsets and targets >= node_count are errors. */
+gb_status gb_binary_decode(const void* bytes, uint64_t len, gb_graph_kind kind, uint32_t* node_count,
+                           uint64_t* entries, int* has_values, uint32_t* out_offsets, uint32_t* out_targets,
+                           float* out_values, uint32_t* in_offsets, uint32_t* in_targets);
 
 /* ---- loading files on the device ----------------------------------------------------------------
  * The file is streamed through a ring of pinned buffers (pread on several threads, copy stream, parse
@@ -185,14 +195,28 @@ gb_status gb_edge_list_parse(const char* text, uint64_t len, uint32_t* src, uint
  * GB_LOAD_CHUNK_BYTES (environment, read per call) sets the buffer size and selects the device path at
  * any file size, for tests. */
 typedef enum gb_file_format {
-  GB_FORMAT_GRAPH500 = 0, /* packed 12-byte records; node_count = edges / 16 */
-  GB_FORMAT_EDGE_LIST = 1 /* text "<src> <dst>[ <f32>]"; node_count = max id + 1 */
+  GB_FORMAT_GRAPH500 = 0,  /* packed 12-byte records; node_count = edges / 16 */
+  GB_FORMAT_EDGE_LIST = 1, /* text "<src> <dst>[ <f32>]"; node_count = max id + 1 */
+  GB_FORMAT_BINARY = 2     /* SerializeGraphOp's file (see gb_binary_decode): the CSRs as stored */
 } gb_file_format;
-/* with_values: read the third column of an edge list as f32 edge values (Graph500 has none) */
+/* with_values: read the third column of an edge list as f32 edge values (Graph500 has none).
+ * A binary file's rows are kept byte for byte: `layout` is checked and otherwise ignored, as the reference
+ * ignores it (csr.rs:650), and the row order is left unknown, as after gb_graph_from_csr_u32.  with_values
+ * = 1 needs a file with values; with 0 they are dropped, and so are the in-CSR values (the device keeps
+ * none) and an undirected file's values.  The streamed path DMAs u32 sections without values straight into
+ * the CSR arrays and narrows / splits the others on the device. */
 gb_status gb_digraph_load_u32(int device, const char* path, gb_file_format format, gb_layout layout,
                               int with_values, gb_graph** graph);
 gb_status gb_graph_load_u32(int device, const char* path, gb_file_format format, gb_layout layout,
                             gb_graph** graph);
+/* SerializeGraphOp::serialize (graph_ops.rs:232-238): writes the graph as a binary file with NI = "u32";
+ * a weighted digraph writes Target<u32,f32> records for both CSRs, the in-CSR value of the k-th occurrence
+ * of s in in-row t being that of the k-th occurrence of t in out-row s (for every graph built here the
+ * value of the same edge; the in-CSR must be the transpose of the out-CSR).  So save(load(f)) is byte-equal
+ * to f for files written here, and for a foreign weighted file up to the order of the values among parallel
+ * (s, t) edges.  The file is written to a temporary file in the same directory, which is renamed over
+ * `path` on success and removed on failure.  GB_ERR_INVALID for a gb_digraph_for_page_rank_u32 twin. */
+gb_status gb_graph_serialize(const gb_graph* graph, const char* path);
 /* Statistics of the load that created the graph (all zero for graphs made otherwise). */
 typedef struct gb_load_info {
   uint64_t file_bytes;     /* size of the file */

@@ -41,7 +41,8 @@ namespace prelude {
 enum class CsrLayout { Unsorted = GB_LAYOUT_UNSORTED, Sorted = GB_LAYOUT_SORTED, Deduplicated = GB_LAYOUT_DEDUPLICATED };
 
 // input formats of `GraphBuilder::file_format(..).path(..)` (builder.rs:283-361; input/graph500.rs, input/edgelist.rs)
-enum class FileFormat { Graph500, EdgeList };
+// Binary: the file of SerializeGraphOp (input/binary.rs), loaded as stored by gb_[di]graph_load_u32
+enum class FileFormat { Graph500, EdgeList, Binary };
 
 // crates/algos/src/page_rank.rs:14-56
 struct PageRankConfig {
@@ -100,6 +101,8 @@ class CsrGraphBase {
   std::uint32_t node_count() const { return info().node_count; }  // Graph::node_count, lib.rs:315-321
   std::uint64_t edge_count() const { return info().edge_count; }
   gb_graph* handle() const { return g_; }
+  // SerializeGraphOp::serialize, graph_ops.rs:232-238 (NI = u32)
+  void serialize(const std::string& path) const { detail::check(gb_graph_serialize(g_, path.c_str())); }
 
  protected:
   struct HostCsr {
@@ -189,9 +192,14 @@ class GraphBuilder {
   GraphBuilder& path(const std::string& p) {
     std::ifstream in(p, std::ios::binary);
     if (!in) throw Error(GB_ERR_INVALID, "cannot open " + p);  // Error::IoError, lib.rs:276-281
+    src_.clear(); dst_.clear(); w_.clear();
+    binary_path_.clear();
+    if (format_ == FileFormat::Binary) {  // the CSRs are read as stored at build time (csr.rs:636-656)
+      binary_path_ = p;
+      return *this;
+    }
     std::vector<char> bytes((std::istreambuf_iterator<char>(in)), std::istreambuf_iterator<char>());
     std::uint64_t m = 0;
-    w_.clear();
     if (format_ == FileFormat::Graph500) {
       src_.resize(bytes.size() / 12);
       dst_.resize(bytes.size() / 12);
@@ -217,12 +225,21 @@ class GraphBuilder {
   const std::vector<float>& pending_values() const { return w_; }
   DirectedCsrGraph build_directed() const {
     gb_graph* g = nullptr;
+    if (!binary_path_.empty()) {
+      detail::check(gb_digraph_load_u32(device_, binary_path_.c_str(), GB_FORMAT_BINARY, static_cast<gb_layout>(layout_),
+                                        with_values_ ? 1 : 0, &g));
+      return DirectedCsrGraph(g);
+    }
     detail::check(gb_digraph_from_edges_u32(device_, src_.data(), dst_.data(), w_.empty() ? nullptr : w_.data(), src_.size(), n_,
                                             static_cast<gb_layout>(layout_), &g));
     return DirectedCsrGraph(g);
   }
   UndirectedCsrGraph build_undirected() const {
     gb_graph* g = nullptr;
+    if (!binary_path_.empty()) {
+      detail::check(gb_graph_load_u32(device_, binary_path_.c_str(), GB_FORMAT_BINARY, static_cast<gb_layout>(layout_), &g));
+      return UndirectedCsrGraph(g);
+    }
     detail::check(gb_graph_from_edges_u32(device_, src_.data(), dst_.data(), src_.size(), n_, static_cast<gb_layout>(layout_), &g));
     return UndirectedCsrGraph(g);
   }
@@ -233,6 +250,7 @@ class GraphBuilder {
   bool with_values_ = false;
   int device_ = 0;
   std::uint32_t n_ = 0;
+  std::string binary_path_;  // set by path(..) for FileFormat::Binary
   std::vector<std::uint32_t> src_, dst_;
   std::vector<float> w_;
 };
