@@ -1,11 +1,18 @@
-// load.cu — Graph500 and text edge-list files read straight into device edge arrays.
+// load.cu — graph files streamed between the file and device memory: Graph500 and text edge lists parsed into
+// device edge arrays, and binary CSR files read into and written from the device CSR arrays.
 //
-// The host readers (io.cu) decode the whole file in pageable memory, and the edges then cross PCIe.  Here
-// the file is streamed through a ring of pinned buffers: one thread per buffer preads the chunks that map
-// to it, the chunk goes to the device on a copy stream, and kernels on a second stream decode it into the
-// edge arrays.  A buffer is refilled only after its copy has completed, and a device buffer only after the
-// kernel that read it has.  The graph is then built from the device arrays (graph_from_device_arrays), so
-// it is the one the host readers followed by gb_[di]graph_from_edges_u32 give.
+// load_graph opens the file once.  Below LOAD_DEVICE_MIN_BYTES the host decoders of io.cu read it whole in
+// pageable memory and their result is uploaded.  Larger files go through a ring of pinned buffers
+// (PinnedRing): chunk k of the file travels through buffer k % ring.  On a load, one reader thread per buffer
+// preads the chunks that map to it (ChunkReader), a copy stream moves each chunk to the device slot's staging
+// buffer (DeviceStaging), and kernels on a work stream decode it.  On a save the copy stream fills the buffers
+// from device memory and the host writes them out.  Ordering rules:
+//   - a pinned buffer is refilled only after the copy out of it has completed (its `copied` event);
+//   - a device staging buffer is overwritten or reallocated only after the kernels that read it have completed
+//     (its `parsed` event);
+//   - on every exit, errors included, the copy stream is drained before any buffer it writes into is freed;
+//   - the ring's buffers go back to PinnedRingCache for the next load or save and are not freed; one that finds
+//     the cache in use allocates its own ring and frees it.
 //
 //   Graph500: records never straddle a chunk (chunks are a multiple of 48 bytes = 4 records), m = len / 12 is
 //   known up front, and k_load_graph500 decodes 4 records per thread with three 128-bit loads.
@@ -14,7 +21,15 @@
 //   the '\n' of each 4 KB tile, a CUB scan turns the counts into tile bases, and k_load_parse_text finds the
 //   line starts of a tile from 128-bit loads (a block scan ranks them) and parses one line per start
 //   (edgelist_scan.h).  m is unknown until the end, so the edge arrays grow; values the device parser
-//   declines are listed (file offset, edge index) and re-parsed on the host with gb::parse_line.
+//   declines are listed (file offset, edge index) and re-parsed on the host with gb::parse_line.  Both build
+//   the graph from the device arrays (graph_from_device_arrays), so it is the one the host readers followed by
+//   gb_[di]graph_from_edges_u32 give.
+//   Binary: the host preads the headers (bin_parse gives the section table) and every chunk is cut against the
+//   table.  u32 sections without values go from the pinned buffer straight into their CSR array; a chunk that
+//   meets another section is staged with the bytes of the element it cuts carried in front, and k_bin_split
+//   narrows the ids and splits the records.
+//   Writer: the file is pieces of host and device memory; chunk k + 1 is copied from the device into the ring
+//   while chunk k is written with pwrite to a temporary file, which is then renamed over the destination.
 #include <fcntl.h>
 #include <sys/stat.h>
 #include <unistd.h>
@@ -204,10 +219,29 @@ static bool pread_all(int fd, char* dst, uint64_t bytes, uint64_t off) {
   return true;
 }
 
-struct FileHandle {
+// a file open for reading, its size, and the path its errors name
+struct InputFile {
+  const char* path = nullptr;
   int fd = -1;
-  ~FileHandle() {
+  uint64_t bytes = 0;
+  ~InputFile() {
     if (fd >= 0) ::close(fd);
+  }
+  gb_status open(const char* p) {
+    path = p;
+    fd = ::open(p, O_RDONLY | O_CLOEXEC);
+    if (fd < 0) return fail(GB_ERR_INVALID, "cannot open %s: %s", p, std::strerror(errno));
+    struct stat st {};
+    if (::fstat(fd, &st) != 0 || !S_ISREG(st.st_mode)) return fail(GB_ERR_INVALID, "%s is not a regular file", p);
+    bytes = (uint64_t)st.st_size;
+    return GB_OK;
+  }
+  // the whole file in host memory (not zero-filled first), for the host decoders
+  gb_status read_all(std::unique_ptr<char[]>* out) const {
+    out->reset(new (std::nothrow) char[bytes ? bytes : 1]);
+    if (!*out) return fail(GB_ERR_OOM, "host allocation of %llu bytes failed", (unsigned long long)bytes);
+    if (bytes && !pread_all(fd, out->get(), bytes, 0)) return fail(GB_ERR_INVALID, "reading %s failed", path);
+    return GB_OK;
   }
 };
 
@@ -219,8 +253,7 @@ struct PinnedBuf {
 };
 
 // Pinning host memory costs about as much as reading it from the page cache, so the ring is kept for the
-// next load (at most LOAD_RING buffers of one default chunk each).  A load that finds it in use allocates
-// its own ring and frees it.
+// next load (at most LOAD_RING buffers of one default chunk each).
 struct PinnedRingCache {
   std::mutex mu;
   bool busy = false;
@@ -232,39 +265,38 @@ static PinnedRingCache& pinned_ring_cache() {
   return *c;
 }
 
-// The ring of pinned buffers and the reader threads that fill it.  Thread r reads chunks r, r + R, ... into
-// buffer r, each after the consumer has released the buffer for it and the copy out of it has completed.
-struct ChunkReader {
-  int fd = -1, device = 0;
+// The pinned buffers a file streams through, LOAD_CARRY_RESERVE bytes then one chunk each, and per buffer the
+// event recorded behind the last copy out of it (into it, for the writer).  Chunk k is bytes
+// [k * chunk, min((k + 1) * chunk, read_end)) of the file and goes through buffer k % ring.
+struct PinnedRing {
   uint64_t chunk = 0, read_end = 0, nchunks = 0;
   unsigned ring = 0;
-  std::vector<PinnedBuf> host;          // [ring]: LOAD_CARRY_RESERVE bytes, then the chunk
-  bool cached = false;                  // host[] belongs to the pinned ring cache
-  std::vector<cudaEvent_t> copied;      // [ring]: recorded behind the last copy out of the buffer
-  std::vector<uint64_t> filled;         // [ring]: chunk index + 1 the buffer holds (0: none yet)
-  std::vector<uint64_t> released_for;   // [ring]: the buffer may be filled with this chunk
-  std::vector<std::thread> threads;
-  std::mutex mu;
-  std::condition_variable cv;
-  bool stop = false, failed = false;
-  std::string error;
+  std::vector<PinnedBuf> host;      // [ring]
+  bool cached = false;              // host[] belongs to the pinned ring cache
+  std::vector<cudaEvent_t> copied;  // [ring]
 
+  // the geometry for streaming `bytes`: chunks of GB_LOAD_CHUNK_BYTES, else of a quarter of the file within
+  // [LOAD_MIN_CHUNK, LOAD_DEFAULT_CHUNK] so that a small file keeps every buffer busy; then rounded down to
+  // whole `unit`s (the Graph500 loader's 4-record groups)
+  void plan(uint64_t bytes, uint64_t unit = 1) {
+    chunk = env_chunk_bytes();
+    if (chunk == 0) {
+      const uint64_t quarter = (bytes / LOAD_RING + 4095) & ~(uint64_t)4095;
+      chunk = std::min(LOAD_DEFAULT_CHUNK, std::max(LOAD_MIN_CHUNK, quarter));
+    }
+    chunk = std::max<uint64_t>(chunk, 16);  // >= the largest binary element: it spans at most two chunks
+    chunk = std::max(unit, chunk / unit * unit);
+    read_end = bytes;
+    nchunks = (bytes + chunk - 1) / chunk;
+    ring = (unsigned)std::min<uint64_t>(LOAD_RING, std::max<uint64_t>(nchunks, 1));
+  }
   uint64_t chunk_bytes(uint64_t k) const { return std::min(chunk, read_end - k * chunk); }
   char* data(unsigned r) { return host[r].p + LOAD_CARRY_RESERVE; }
 
-  // the reader threads over the ring
-  gb_status start() {
-    GB_TRY(acquire());
-    for (unsigned r = 0; r < ring; ++r) threads.emplace_back([this, r] { run(r); });
-    return GB_OK;
-  }
-
-  // the pinned buffers and their events alone (the binary writer fills them from the device)
+  // the buffers (the cached ones when the cache is free and they are large enough) and their events
   gb_status acquire() {
     host.resize(ring);
     copied.assign(ring, nullptr);
-    filled.assign(ring, 0);
-    released_for.resize(ring);
     const uint64_t bytes = LOAD_CARRY_RESERVE + chunk;
     PinnedRingCache& pc = pinned_ring_cache();
     {
@@ -292,10 +324,51 @@ struct ChunkReader {
       }
     }
     for (unsigned r = 0; r < ring; ++r) {
-      released_for[r] = r;
       if (!cached) GB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&host[r].p), bytes, cudaHostAllocDefault));
       GB_CUDA(cudaEventCreateWithFlags(&copied[r], cudaEventDisableTiming));
     }
+    return GB_OK;
+  }
+
+  ~PinnedRing() {
+    for (cudaEvent_t e : copied) {
+      if (e) cudaEventSynchronize(e), cudaEventDestroy(e);  // no copy may still use a buffer
+    }
+    if (cached) {
+      for (auto& h : host) h.p = nullptr;  // back to the cache, not freed
+      PinnedRingCache& pc = pinned_ring_cache();
+      std::lock_guard<std::mutex> lock(pc.mu);
+      pc.busy = false;
+    }
+  }
+};
+
+struct StreamPair {
+  cudaStream_t copy = nullptr, work = nullptr;
+  ~StreamPair() {
+    if (copy) cudaStreamSynchronize(copy), cudaStreamDestroy(copy);
+    if (work) cudaStreamSynchronize(work), cudaStreamDestroy(work);
+  }
+};
+
+// The reader threads over a ring: thread r preads chunks r, r + R, ... into buffer r, each after the consumer
+// has released the buffer for it and the copy out of it has completed.
+struct ChunkReader : PinnedRing {
+  int fd = -1, device = 0;
+  std::vector<uint64_t> filled;        // [ring]: chunk index + 1 the buffer holds (0: none yet)
+  std::vector<uint64_t> released_for;  // [ring]: the buffer may be filled with this chunk
+  std::vector<std::thread> threads;
+  std::mutex mu;
+  std::condition_variable cv;
+  bool stop = false, failed = false;
+  std::string error;
+
+  ChunkReader(int fd, int device) : fd(fd), device(device) {}
+  gb_status start() {
+    GB_TRY(acquire());
+    filled.assign(ring, 0);
+    for (unsigned r = 0; r < ring; ++r) released_for.push_back(r);
+    for (unsigned r = 0; r < ring; ++r) threads.emplace_back([this, r] { run(r); });
     return GB_OK;
   }
 
@@ -329,36 +402,75 @@ struct ChunkReader {
     return GB_OK;
   }
 
-  void release(uint64_t k) {
-    std::lock_guard<std::mutex> lock(mu);
-    released_for[k % ring] = k + ring;
+  // every copy out of chunk k's buffer is issued on sp.copy: the buffer is refilled once they complete, and
+  // sp.work waits for them
+  gb_status release(uint64_t k, const StreamPair& sp) {
+    const unsigned r = (unsigned)(k % ring);
+    GB_CUDA(cudaEventRecord(copied[r], sp.copy));
+    {
+      std::lock_guard<std::mutex> lock(mu);
+      released_for[r] = k + ring;
+    }
     cv.notify_all();
+    GB_CUDA(cudaStreamWaitEvent(sp.work, copied[r], 0));
+    return GB_OK;
   }
 
-  ~ChunkReader() {
+  ~ChunkReader() {  // then ~PinnedRing waits for the copies out of the buffers
     {
       std::lock_guard<std::mutex> lock(mu);
       stop = true;
     }
     cv.notify_all();
     for (auto& t : threads) t.join();
-    for (cudaEvent_t e : copied) {
-      if (e) cudaEventSynchronize(e), cudaEventDestroy(e);  // no copy may still read a buffer
-    }
-    if (cached) {
-      for (auto& h : host) h.p = nullptr;  // back to the cache, not freed
-      PinnedRingCache& pc = pinned_ring_cache();
-      std::lock_guard<std::mutex> lock(pc.mu);
-      pc.busy = false;
-    }
   }
 };
 
-struct StreamPair {
-  cudaStream_t copy = nullptr, work = nullptr;
-  ~StreamPair() {
-    if (copy) cudaStreamSynchronize(copy), cudaStreamDestroy(copy);
-    if (work) cudaStreamSynchronize(work), cudaStreamDestroy(work);
+// The device side of a streamed load: per ring slot a staging buffer and the event recorded behind the kernels
+// that read it.  Chunks reach the device on sp.copy and are decoded on sp.work.  Declare it inside the
+// DevBufStreamScope of sp.work.
+struct DeviceStaging {
+  ChunkReader& rd;
+  StreamPair& sp;
+  std::vector<DevBuf<uint8_t>> dbuf;  // [ring]: LOAD_TILE bytes of slack, as the text kernels read whole tiles
+  std::vector<cudaEvent_t> parsed;    // [ring]
+  uint64_t h2d = 0;                   // bytes copied to the device
+
+  DeviceStaging(ChunkReader& r, StreamPair& s) : rd(r), sp(s), dbuf(r.ring), parsed(r.ring, nullptr) {}
+  gb_status create_events() {
+    for (cudaEvent_t& e : parsed) GB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    return GB_OK;
+  }
+  ~DeviceStaging() {
+    cudaStreamSynchronize(sp.copy);  // nothing may still be copying into dbuf when it is freed
+    for (cudaEvent_t e : parsed)
+      if (e) cudaEventDestroy(e);
+  }
+
+  // Copies cl carried bytes and then the first `body` bytes of chunk k (cl + body > 0) to the slot's staging
+  // buffer, once the kernels that read it are done.  A carry that fits the LOAD_CARRY_RESERVE gap in front of
+  // the pinned chunk goes with it in one copy; a longer one (a text line longer than the reserve) goes from
+  // pageable memory.
+  gb_status stage(uint64_t k, const char* carry, uint64_t cl, uint64_t body) {
+    const unsigned r = (unsigned)(k % rd.ring);
+    char* data = rd.data(r);
+    const uint64_t len = cl + body;
+    if (dbuf[r].n < len + LOAD_TILE) {
+      GB_CUDA(cudaEventSynchronize(parsed[r]));
+      DevBuf<uint8_t> nb;
+      GB_TRY(nb.alloc(std::max<uint64_t>(len, rd.chunk + LOAD_CARRY_RESERVE) + LOAD_TILE));
+      dbuf[r] = std::move(nb);
+    }
+    GB_CUDA(cudaStreamWaitEvent(sp.copy, parsed[r], 0));
+    if (cl <= LOAD_CARRY_RESERVE) {
+      std::memcpy(data - cl, carry, cl);
+      GB_CUDA(cudaMemcpyAsync(dbuf[r].p, data - cl, len, cudaMemcpyHostToDevice, sp.copy));
+    } else {
+      GB_CUDA(cudaMemcpyAsync(dbuf[r].p, carry, cl, cudaMemcpyHostToDevice, sp.copy));
+      if (body) GB_CUDA(cudaMemcpyAsync(dbuf[r].p + cl, data, body, cudaMemcpyHostToDevice, sp.copy));
+    }
+    h2d += len;
+    return GB_OK;
   }
 };
 
@@ -380,32 +492,12 @@ struct LoadedEdges {
   uint32_t n = 0;  // 0: max id + 1
 };
 
-static gb_status load_file(int device, const char* path, gb_file_format format, bool want_value,
+static gb_status load_file(int device, const InputFile& f, gb_file_format format, bool want_value,
                            LoadedEdges* out, gb_load_info* info) {
-  FileHandle f;
-  f.fd = ::open(path, O_RDONLY | O_CLOEXEC);
-  if (f.fd < 0) return fail(GB_ERR_INVALID, "cannot open %s: %s", path, std::strerror(errno));
-  struct stat st {};
-  if (::fstat(f.fd, &st) != 0 || !S_ISREG(st.st_mode)) return fail(GB_ERR_INVALID, "%s is not a regular file", path);
-  const uint64_t file_bytes = (uint64_t)st.st_size;
   const bool g500 = format == GB_FORMAT_GRAPH500;
-  info->file_bytes = file_bytes;
-
-  ChunkReader rd;
-  rd.fd = f.fd;
-  rd.device = device;
-  const uint64_t m500 = file_bytes / 12;
-  rd.read_end = g500 ? 12 * m500 : file_bytes;  // a Graph500 tail shorter than a record is ignored
-  uint64_t chunk = env_chunk_bytes();
-  if (chunk == 0) {
-    const uint64_t quarter = (rd.read_end / LOAD_RING + 4095) & ~(uint64_t)4095;  // small files: all buffers busy
-    chunk = std::min(LOAD_DEFAULT_CHUNK, std::max(LOAD_MIN_CHUNK, quarter));
-  }
-  if (g500) chunk = std::max<uint64_t>(48, chunk / 48 * 48);  // whole 4-record groups
-  chunk = std::max<uint64_t>(chunk, 16);
-  rd.chunk = chunk;
-  rd.nchunks = (rd.read_end + chunk - 1) / chunk;
-  rd.ring = (unsigned)std::min<uint64_t>(LOAD_RING, std::max<uint64_t>(rd.nchunks, 1));
+  ChunkReader rd(f.fd, device);
+  const uint64_t m500 = f.bytes / 12;
+  rd.plan(g500 ? 12 * m500 : f.bytes, g500 ? 48 : 1);  // Graph500: whole 4-record groups, a partial tail ignored
   info->chunks = rd.nchunks;
   if (rd.nchunks == 0) return GB_OK;  // empty: gb_*_from_device_edges reports it
 
@@ -414,18 +506,10 @@ static gb_status load_file(int device, const char* path, gb_file_format format, 
   GB_CUDA(cudaStreamCreateWithFlags(&sp.work, cudaStreamNonBlocking));
   GB_TRY(rd.start());
   DevBufStreamScope scope(sp.work);
+  DeviceStaging st(rd, sp);
+  GB_TRY(st.create_events());
 
   const unsigned R = rd.ring;
-  std::vector<DevBuf<uint8_t>> dbuf(R);
-  std::vector<cudaEvent_t> parsed(R, nullptr);
-  struct Events {
-    std::vector<cudaEvent_t>* v;
-    ~Events() {
-      for (cudaEvent_t e : *v)
-        if (e) cudaEventDestroy(e);
-    }
-  } parsed_guard{&parsed};
-  for (unsigned r = 0; r < R; ++r) GB_CUDA(cudaEventCreateWithFlags(&parsed[r], cudaEventDisableTiming));
   DevBuf<LoadCounters> ctr;
   GB_TRY(ctr.alloc(1));
   GB_CUDA(cudaMemsetAsync(ctr.p, 0, sizeof(LoadCounters), sp.work));
@@ -437,12 +521,7 @@ static gb_status load_file(int device, const char* path, gb_file_format format, 
   DevBuf<uint8_t> scan_tmp;
   DevBuf<uint64_t> dec_off;
   DevBuf<uint32_t> dec_edge;
-  // on every exit, nothing may still be copying into the buffers above when they are released
-  struct Drain {
-    StreamPair* sp;
-    ~Drain() { cudaStreamSynchronize(sp->copy); }
-  } drain{&sp};
-  uint64_t h2d = 0, m = 0;
+  uint64_t m = 0;
   if (g500) {
     GB_TRY(out->src.alloc(m500));
     GB_TRY(out->dst.alloc(m500));
@@ -460,7 +539,7 @@ static gb_status load_file(int device, const char* path, gb_file_format format, 
   auto prepare = [&](uint64_t k) -> gb_status {
     const unsigned r = (unsigned)(k % R);
     GB_TRY(rd.wait_filled(k));
-    char* data = rd.data(r);
+    const char* data = rd.data(r);
     const uint64_t n = rd.chunk_bytes(k);
     const bool last = k + 1 == rd.nchunks;
     uint64_t body = n;  // bytes of this chunk that go to the device now
@@ -476,26 +555,8 @@ static gb_status load_file(int device, const char* path, gb_file_format format, 
     sg.len = cl + body;
     sg.file_off = k * rd.chunk - cl;
     sg.ends_with_newline = sg.len == 0 || (body ? data[body - 1] == '\n' : carry.back() == '\n');
-    if (sg.len) {
-      if (dbuf[r].n < sg.len + LOAD_TILE) {
-        GB_CUDA(cudaEventSynchronize(parsed[r]));
-        DevBuf<uint8_t> nb;
-        GB_TRY(nb.alloc(std::max<uint64_t>(sg.len, rd.chunk + LOAD_CARRY_RESERVE) + LOAD_TILE));
-        dbuf[r] = std::move(nb);
-      }
-      GB_CUDA(cudaStreamWaitEvent(sp.copy, parsed[r], 0));  // the kernel that read this device buffer is done
-      if (cl <= LOAD_CARRY_RESERVE) {
-        std::memcpy(data - cl, carry.data(), cl);
-        GB_CUDA(cudaMemcpyAsync(dbuf[r].p, data - cl, sg.len, cudaMemcpyHostToDevice, sp.copy));
-      } else {  // a line longer than the reserve: its head goes from pageable memory
-        GB_CUDA(cudaMemcpyAsync(dbuf[r].p, carry.data(), cl, cudaMemcpyHostToDevice, sp.copy));
-        if (body) GB_CUDA(cudaMemcpyAsync(dbuf[r].p + cl, data, body, cudaMemcpyHostToDevice, sp.copy));
-      }
-      h2d += sg.len;
-      GB_CUDA(cudaEventRecord(rd.copied[r], sp.copy));
-    }
-    rd.release(k);
-    if (sg.len) GB_CUDA(cudaStreamWaitEvent(sp.work, rd.copied[r], 0));
+    if (sg.len) GB_TRY(st.stage(k, carry.data(), cl, body));
+    GB_TRY(rd.release(k, sp));
     if (!g500) carry.swap(next_carry);
     return GB_OK;
   };
@@ -504,7 +565,7 @@ static gb_status load_file(int device, const char* path, gb_file_format format, 
   for (uint64_t k = 0; k < rd.nchunks; ++k) {
     const unsigned r = (unsigned)(k % R);
     const Staged sg = staged[r];
-    const uint4* d = reinterpret_cast<const uint4*>(dbuf[r].p);
+    const uint4* d = reinterpret_cast<const uint4*>(st.dbuf[r].p);
     if (g500) {
       if (k + 1 < rd.nchunks) GB_TRY(prepare(k + 1));
       const uint64_t nrec = sg.len / 12;
@@ -513,7 +574,7 @@ static gb_status load_file(int device, const char* path, gb_file_format format, 
                                                                              out->dst.p, ctr.p);
         GB_CUDA(cudaGetLastError());
       }
-      GB_CUDA(cudaEventRecord(parsed[r], sp.work));
+      GB_CUDA(cudaEventRecord(st.parsed[r], sp.work));
       continue;
     }
     const uint64_t tiles = (sg.len + LOAD_TILE - 1) / LOAD_TILE;
@@ -548,7 +609,7 @@ static gb_status load_file(int device, const char* path, gb_file_format format, 
       GB_CUDA(cudaGetLastError());
       m += lines;
     }
-    GB_CUDA(cudaEventRecord(parsed[r], sp.work));
+    GB_CUDA(cudaEventRecord(st.parsed[r], sp.work));
   }
   LoadCounters hc{};
   GB_CUDA(cudaMemcpyAsync(&hc, ctr.p, sizeof hc, cudaMemcpyDeviceToHost, sp.work));
@@ -568,10 +629,10 @@ static gb_status load_file(int device, const char* path, gb_file_format format, 
     for (uint64_t i = 0; i < hc.declined; ++i) {
       uint64_t want = 256;
       for (;;) {
-        const uint64_t n = std::min(want, file_bytes - off[i]);
+        const uint64_t n = std::min(want, f.bytes - off[i]);
         line.resize(n);
-        if (!pread_all(f.fd, &line[0], n, off[i])) return fail(GB_ERR_INVALID, "reading %s failed", path);
-        if (n == file_bytes - off[i] || std::memchr(line.data(), '\n', n)) break;
+        if (!pread_all(f.fd, &line[0], n, off[i])) return fail(GB_ERR_INVALID, "reading %s failed", f.path);
+        if (n == f.bytes - off[i] || std::memchr(line.data(), '\n', n)) break;
         want *= 2;
       }
       uint64_t s, t;
@@ -583,26 +644,15 @@ static gb_status load_file(int device, const char* path, gb_file_format format, 
     k_load_patch<<<grid_for(hc.declined, 256), 256, 0, sp.work>>>(dec_edge.p, dval.p, hc.declined, out->w.p);
     GB_CUDA(cudaGetLastError());
     GB_CUDA(cudaStreamSynchronize(sp.work));
-    h2d += hc.declined * 4ull;
+    st.h2d += hc.declined * 4ull;
   }
   out->m = m;
   out->n = g500 ? (uint32_t)std::min<uint64_t>(m500 / 16, 0xFFFFFFFFull) : 0;  // graph500.rs:74
   info->edges = m;
   info->fallback_lines = hc.declined;
-  info->h2d_bytes = h2d;
+  info->h2d_bytes = st.h2d;
   GB_CUDA(cudaStreamSynchronize(sp.copy));
   return GB_OK;
-}
-
-// pinned buffer size for streaming `bytes`: GB_LOAD_CHUNK_BYTES, else a quarter of the file within
-// [LOAD_MIN_CHUNK, LOAD_DEFAULT_CHUNK] so that a small file keeps every buffer busy
-static uint64_t ring_chunk(uint64_t bytes) {
-  uint64_t chunk = env_chunk_bytes();
-  if (chunk == 0) {
-    const uint64_t quarter = (bytes / LOAD_RING + 4095) & ~(uint64_t)4095;
-    chunk = std::min(LOAD_DEFAULT_CHUNK, std::max(LOAD_MIN_CHUNK, quarter));
-  }
-  return std::max<uint64_t>(chunk, 16);  // >= the largest record: an element spans at most two chunks
 }
 
 // The CSR arrays a binary file's section fills.  Elements of `stride` bytes start at file byte `pos`; a u32
@@ -651,23 +701,13 @@ static gb_status check_loaded_csrs(gb_graph* g, const BinLayout& l, DevCsr* cons
   return GB_OK;
 }
 
-// Binary graph files on the device: the host preads the headers (bin_parse gives the section table), then the
-// ring streams the file and every chunk is cut against the table.  Direct sections go from the pinned buffer
-// to their CSR array at their byte offset; when a chunk meets a staged section, the chunk goes to a device
-// buffer with the bytes of the element it cuts in front (at most 15, carried from the chunk before), and
-// k_bin_split decodes the elements that end inside the chunk.
-static gb_status load_binary_streamed(int device, gb_graph_kind kind, const char* path, bool want_value,
+// Binary graph files streamed into the CSR arrays.  A staged chunk carries at most 15 bytes of a cut element
+// in front, and k_bin_split decodes the elements that end inside the chunk.
+static gb_status load_binary_streamed(int device, gb_graph_kind kind, const InputFile& f, bool want_value,
                                       gb_graph** graph, gb_load_info* info) {
-  FileHandle f;
-  f.fd = ::open(path, O_RDONLY | O_CLOEXEC);
-  if (f.fd < 0) return fail(GB_ERR_INVALID, "cannot open %s: %s", path, std::strerror(errno));
-  struct stat st {};
-  if (::fstat(f.fd, &st) != 0 || !S_ISREG(st.st_mode)) return fail(GB_ERR_INVALID, "%s is not a regular file", path);
-  const uint64_t size = (uint64_t)st.st_size;
-  info->file_bytes = size;
   BinLayout l;
   GB_TRY(bin_parse([&](uint64_t pos, void* dst, uint64_t n) { return pread_all(f.fd, static_cast<char*>(dst), n, pos); },
-                   size, kind, &l));
+                   f.bytes, kind, &l));
   GB_REQUIRE(!want_value || l.values, "the binary graph file holds no edge values");
   GraphPtr g;
   GB_TRY(new_graph(device, kind, l.n, &g));
@@ -692,65 +732,36 @@ static gb_status load_binary_streamed(int device, gb_graph_kind kind, const char
     if (t.count) secs.push_back(t);
   }
 
-  ChunkReader rd;
-  rd.fd = f.fd;
-  rd.device = device;
-  rd.read_end = size;
-  rd.chunk = ring_chunk(size);
-  rd.nchunks = (size + rd.chunk - 1) / rd.chunk;
-  rd.ring = (unsigned)std::min<uint64_t>(LOAD_RING, rd.nchunks);
+  ChunkReader rd(f.fd, device);
+  rd.plan(f.bytes);
   info->chunks = rd.nchunks;
   GB_TRY(rd.start());
+  DeviceStaging st(rd, sp);
+  GB_TRY(st.create_events());
   const unsigned R = rd.ring;
-  std::vector<DevBuf<uint8_t>> dbuf(R);
-  std::vector<cudaEvent_t> parsed(R, nullptr);
-  struct Events {
-    std::vector<cudaEvent_t>* v;
-    ~Events() {
-      for (cudaEvent_t e : *v)
-        if (e) cudaEventDestroy(e);
-    }
-  } parsed_guard{&parsed};
-  for (unsigned r = 0; r < R; ++r) GB_CUDA(cudaEventCreateWithFlags(&parsed[r], cudaEventDisableTiming));
   DevBuf<unsigned int> wide;
   GB_TRY(wide.alloc(1));
   GB_CUDA(cudaMemsetAsync(wide.p, 0, 4, sp.work));
-  struct Drain {
-    StreamPair* sp;
-    ~Drain() { cudaStreamSynchronize(sp->copy); }
-  } drain{&sp};
 
-  std::vector<uint64_t> staged_off(R, 0);  // file byte of dbuf[r][0], or ~0: the chunk was not staged
+  std::vector<uint64_t> staged_off(R, 0);  // file byte of st.dbuf[r][0], or ~0: the chunk was not staged
   std::string carry;                       // bytes of the staged element that the next chunk completes
-  uint64_t h2d = 0;
   auto prepare = [&](uint64_t k) -> gb_status {
     const unsigned r = (unsigned)(k % R);
     GB_TRY(rd.wait_filled(k));
-    char* data = rd.data(r);
+    const char* data = rd.data(r);
     const uint64_t a = k * rd.chunk, len = rd.chunk_bytes(k), b = a + len;
     bool stage = false;
     for (const BinSection& s : secs) stage |= !s.direct() && s.pos < b && s.end() > a;
     const uint64_t cl = stage ? carry.size() : 0;
     staged_off[r] = stage ? a - cl : ~0ull;
-    if (stage) {
-      if (dbuf[r].n < cl + len + 16) {
-        GB_CUDA(cudaEventSynchronize(parsed[r]));
-        DevBuf<uint8_t> nb;
-        GB_TRY(nb.alloc(std::max<uint64_t>(cl + len, rd.chunk + 16) + 16));
-        dbuf[r] = std::move(nb);
-      }
-      GB_CUDA(cudaStreamWaitEvent(sp.copy, parsed[r], 0));  // the kernels that read this device buffer are done
-      std::memcpy(data - cl, carry.data(), cl);
-      GB_CUDA(cudaMemcpyAsync(dbuf[r].p, data - cl, cl + len, cudaMemcpyHostToDevice, sp.copy));
-      h2d += cl + len;
-    }
+    if (stage) GB_TRY(st.stage(k, carry.data(), cl, len));
     for (const BinSection& s : secs) {
       if (!s.direct()) continue;
       const uint64_t x = std::max(a, s.pos), y = std::min(b, s.end());
       if (x >= y) continue;
       GB_CUDA(cudaMemcpyAsync(reinterpret_cast<char*>(s.ids) + (x - s.pos), data + (x - a), y - x,
                               cudaMemcpyHostToDevice, sp.copy));
-      h2d += y - x;
+      st.h2d += y - x;
     }
     carry.clear();
     for (const BinSection& s : secs)
@@ -758,10 +769,7 @@ static gb_status load_binary_streamed(int device, gb_graph_kind kind, const char
         const uint64_t cut = (b - s.pos) % s.stride;  // bytes of the element that begins before b
         carry.assign(data + (len - cut), cut);
       }
-    GB_CUDA(cudaEventRecord(rd.copied[r], sp.copy));
-    rd.release(k);
-    GB_CUDA(cudaStreamWaitEvent(sp.work, rd.copied[r], 0));
-    return GB_OK;
+    return rd.release(k, sp);
   };
   auto split = [&](uint64_t k) -> gb_status {
     const unsigned r = (unsigned)(k % R);
@@ -772,12 +780,12 @@ static gb_status load_binary_streamed(int device, gb_graph_kind kind, const char
       const uint64_t first = a > s.pos ? (a - s.pos) / s.stride : 0;  // the first element that ends after a
       const uint64_t last = std::min(s.count, (b - s.pos) / s.stride);  // elements that end by b
       if (last <= first) continue;
-      k_bin_split<<<grid_for(last - first, 256), 256, 0, sp.work>>>(dbuf[r].p, staged_off[r], s.pos, s.stride,
+      k_bin_split<<<grid_for(last - first, 256), 256, 0, sp.work>>>(st.dbuf[r].p, staged_off[r], s.pos, s.stride,
                                                                       l.id_bytes, first, last - first, s.ids, s.w,
                                                                       wide.p);
       GB_CUDA(cudaGetLastError());
     }
-    GB_CUDA(cudaEventRecord(parsed[r], sp.work));
+    GB_CUDA(cudaEventRecord(st.parsed[r], sp.work));
     return GB_OK;
   };
   GB_TRY(prepare(0));
@@ -788,7 +796,7 @@ static gb_status load_binary_streamed(int device, gb_graph_kind kind, const char
   GB_CUDA(cudaStreamSynchronize(sp.copy));
   GB_TRY(check_loaded_csrs(g.get(), l, csr, wide.p, sp.work));
   info->edges = kind == GB_KIND_DIRECTED ? l.entries : l.entries / 2;
-  info->h2d_bytes = h2d;
+  info->h2d_bytes = st.h2d;
   *graph = g.release();
   return GB_OK;
 }
@@ -799,17 +807,11 @@ static gb_status load_binary_streamed(int device, gb_graph_kind kind, const char
 constexpr uint64_t LOAD_DEVICE_MIN_BYTES = 64ull << 20;
 
 // the host readers of io.cu and the upload of gb_[di]graph_from_edges_u32
-static gb_status load_on_host(int device, gb_graph_kind kind, const char* path, gb_file_format format,
+static gb_status load_on_host(int device, gb_graph_kind kind, const InputFile& f, gb_file_format format,
                               gb_layout layout, bool want_value, gb_graph** graph, gb_load_info* info) {
-  FileHandle f;
-  f.fd = ::open(path, O_RDONLY | O_CLOEXEC);
-  if (f.fd < 0) return fail(GB_ERR_INVALID, "cannot open %s: %s", path, std::strerror(errno));
-  struct stat st {};
-  if (::fstat(f.fd, &st) != 0 || !S_ISREG(st.st_mode)) return fail(GB_ERR_INVALID, "%s is not a regular file", path);
-  const uint64_t len = (uint64_t)st.st_size;
-  std::unique_ptr<char[]> bytes(new (std::nothrow) char[len ? len : 1]);  // not zero-filled
-  if (!bytes) return fail(GB_ERR_OOM, "host allocation of %llu bytes failed", (unsigned long long)len);
-  if (len && !pread_all(f.fd, bytes.get(), len, 0)) return fail(GB_ERR_INVALID, "reading %s failed", path);
+  std::unique_ptr<char[]> bytes;
+  GB_TRY(f.read_all(&bytes));
+  const uint64_t len = f.bytes;
   std::vector<uint32_t> src, dst;
   std::vector<float> w;
   uint64_t m = 0;
@@ -830,33 +832,27 @@ static gb_status load_on_host(int device, gb_graph_kind kind, const char* path, 
                                      graph));
   else
     GB_TRY(gb_graph_from_edges_u32(device, src.data(), dst.data(), m, n, layout, graph));
-  info->file_bytes = len;
   info->edges = m;
   info->h2d_bytes = m * (want_value ? 12 : 8);
   return GB_OK;
 }
 
 // a small binary file: gb_binary_decode, then the upload of gb_[di]graph_from_csr_u32
-static gb_status load_binary_on_host(int device, gb_graph_kind kind, const char* path, bool want_value,
+static gb_status load_binary_on_host(int device, gb_graph_kind kind, const InputFile& f, bool want_value,
                                      gb_graph** graph, gb_load_info* info) {
-  FileHandle f;
-  f.fd = ::open(path, O_RDONLY | O_CLOEXEC);
-  if (f.fd < 0) return fail(GB_ERR_INVALID, "cannot open %s: %s", path, std::strerror(errno));
-  struct stat st {};
-  if (::fstat(f.fd, &st) != 0 || !S_ISREG(st.st_mode)) return fail(GB_ERR_INVALID, "%s is not a regular file", path);
-  const uint64_t len = (uint64_t)st.st_size;
-  std::vector<char> bytes(len);
-  if (len && !pread_all(f.fd, bytes.data(), len, 0)) return fail(GB_ERR_INVALID, "reading %s failed", path);
+  std::unique_ptr<char[]> bytes;
+  GB_TRY(f.read_all(&bytes));
+  const uint64_t len = f.bytes;
   uint32_t n = 0;
   uint64_t m = 0;
   int has_values = 0;
-  GB_TRY(gb_binary_decode(bytes.data(), len, kind, &n, &m, &has_values, nullptr, nullptr, nullptr, nullptr, nullptr));
+  GB_TRY(gb_binary_decode(bytes.get(), len, kind, &n, &m, &has_values, nullptr, nullptr, nullptr, nullptr, nullptr));
   GB_REQUIRE(!want_value || has_values, "the binary graph file holds no edge values");
   const unsigned ncsr = kind == GB_KIND_DIRECTED ? 2 : 1;
   std::vector<uint32_t> off[2], tgt[2];
   std::vector<float> w(want_value ? m : 0);
   for (unsigned c = 0; c < ncsr; ++c) off[c].resize((size_t)n + 1), tgt[c].resize(m);
-  GB_TRY(gb_binary_decode(bytes.data(), len, kind, &n, &m, &has_values, off[0].data(), tgt[0].data(),
+  GB_TRY(gb_binary_decode(bytes.get(), len, kind, &n, &m, &has_values, off[0].data(), tgt[0].data(),
                           want_value ? w.data() : nullptr, off[1].data(), tgt[1].data()));
   GraphPtr g;
   GB_TRY(new_graph(device, kind, n, &g));
@@ -865,7 +861,6 @@ static gb_status load_binary_on_host(int device, gb_graph_kind kind, const char*
   if (kind == GB_KIND_DIRECTED)
     GB_TRY(upload_host_csr(g->stream, n, off[1].data(), tgt[1].data(), nullptr, &g->in, "csr_inc"));
   *graph = g.release();
-  info->file_bytes = len;
   info->edges = kind == GB_KIND_DIRECTED ? m : m / 2;
   info->h2d_bytes = ncsr * (((uint64_t)n + 1) * 4 + m * 4) + (want_value ? m * 4 : 0);
   return GB_OK;
@@ -894,9 +889,8 @@ struct TempFile {
   }
 };
 
-// SerializeGraphOp::serialize: the file is a sequence of pieces (headers from host memory, arrays from device
-// memory; Target<u32, f32> records are interleaved on the device first) that the pinned ring carries to the
-// file: chunk k + 1 is copied from the device on a copy stream while chunk k is written with pwrite.
+// SerializeGraphOp::serialize (headers from host memory, arrays from device memory; Target<u32, f32> records are
+// interleaved on the device first)
 static gb_status serialize_graph(const gb_graph* g, const char* path) {
   GB_REQUIRE(g && path, "NULL argument");
   GB_REQUIRE(g->out.tgt.p != nullptr, "this handle holds no out targets (page-rank-only twin) and cannot be serialized");
@@ -940,13 +934,8 @@ static gb_status serialize_graph(const gb_graph* g, const char* path) {
     return fail(GB_ERR_INVALID, "cannot create a temporary file next to %s: %s", path, std::strerror(errno));
   }
   ::fchmod(tmp.fd, 0644);
-  const uint64_t total = l.file_bytes;
-  ChunkReader ring;  // its pinned buffers and events only: no reader threads
-  ring.device = g->device;
-  ring.chunk = ring_chunk(total);
-  ring.read_end = total;
-  ring.nchunks = (total + ring.chunk - 1) / ring.chunk;
-  ring.ring = (unsigned)std::min<uint64_t>(LOAD_RING, ring.nchunks);  // >= 2 whenever there is a next chunk
+  PinnedRing ring;
+  ring.plan(l.file_bytes);  // ring >= 2 whenever there is a next chunk
   GB_TRY(ring.acquire());
   StreamPair sp;
   GB_CUDA(cudaStreamCreateWithFlags(&sp.copy, cudaStreamNonBlocking));
@@ -991,18 +980,19 @@ static gb_status load_graph(int device, gb_graph_kind kind, const char* path, gb
   GB_TRY(check_layout(layout));
   GB_TRY(require_device(device));
   DeviceGuard guard(device);
-  struct stat st {};
-  if (::stat(path, &st) != 0) return fail(GB_ERR_INVALID, "cannot open %s: %s", path, std::strerror(errno));
+  InputFile f;
+  GB_TRY(f.open(path));
   gb_load_info info{};
-  const bool on_host = env_chunk_bytes() == 0 && (uint64_t)st.st_size < LOAD_DEVICE_MIN_BYTES;
+  info.file_bytes = f.bytes;
+  const bool on_host = env_chunk_bytes() == 0 && f.bytes < LOAD_DEVICE_MIN_BYTES;
   if (format == GB_FORMAT_BINARY) {
-    if (on_host) GB_TRY(load_binary_on_host(device, kind, path, with_values != 0, graph, &info));
-    else GB_TRY(load_binary_streamed(device, kind, path, with_values != 0, graph, &info));
+    if (on_host) GB_TRY(load_binary_on_host(device, kind, f, with_values != 0, graph, &info));
+    else GB_TRY(load_binary_streamed(device, kind, f, with_values != 0, graph, &info));
   } else if (on_host) {
-    GB_TRY(load_on_host(device, kind, path, format, layout, with_values != 0, graph, &info));
+    GB_TRY(load_on_host(device, kind, f, format, layout, with_values != 0, graph, &info));
   } else {
     LoadedEdges e;
-    GB_TRY(load_file(device, path, format, with_values != 0, &e, &info));
+    GB_TRY(load_file(device, f, format, with_values != 0, &e, &info));
     GB_TRY(graph_from_device_arrays(device, kind, e.src.p, e.dst.p, with_values ? e.w.p : nullptr, e.m, e.n, layout,
                                     nullptr, graph));
   }
