@@ -103,7 +103,6 @@ struct PrArgs {
   uint32_t n_fin;       // rows [0, n_fin) are completed by k_pr_finish (rem[] + partials); rows [n_fin, n_cb) own
                         // segments in at most SELL_FEW blocks and are completed by their k_pr_sell lane
   uint32_t few_kb, few_nrows[SELL_FEW], few_poff[SELL_FEW];  // the first blocks' row prefixes / partial offsets
-  uint32_t dbg;         // GB_PR_DEBUG bits (diagnostics): 1 = SELL slices CTA-major, 2 = static chunk->warp map, 4 = no TMA
   uint32_t fix_in_sell; // k_pr_sell adds the parts of cut segments first (sequential mode: no k_pr_fixup launch)
   const uint32_t* fin_kb;  // [ceil(n_cb / 32)] blocks in which the first row of each 32-row group owns a segment
   // column blocks
@@ -180,13 +179,14 @@ __device__ __forceinline__ double pr_update(uint32_t gr, float sum, float old, u
 }
 
 // ---- column blocks ------------------------------------------------------------------------------------
-// One warp, one chunk: groups [g0, g1) of block j's stream.  Chunks shorter than CB_WIDE_MIN groups (thin
-// blocks) take this 64-group step, longer ones the 128-group step of cb_chunk_wide below.  Lane L owns
-// the ADJACENT groups 2L and 2L+1 of the even-aligned window (one 128-bit load).  Inside a lane the two
-// group sums are combined when they belong to the same row; across lanes the value of the run that is
-// open at the end of each lane goes through a segmented inclusive scan (5 shuffles per 256 ids); a run
-// that spans steps is carried in f64.  The row of a group follows from counting segment-start bits.
-// A lane ends at most two runs per step: the one its first group closes and the one open at its end.
+// One warp, one chunk: groups [g0, g1) of block j's stream, in steps of 32 G groups from the even-aligned
+// g0 & ~1 (G = cb_step_groups: 4, or 2 in the short chunks of thin blocks so that their lanes do not idle).
+// Lane L owns the ADJACENT positions G L .. G L + G - 1 of the step (G / 2 128-bit loads) and adds the
+// runs inside the lane in f32; across lanes the value of the run that is open at the end of each lane goes
+// through ONE segmented inclusive scan (5 shuffles, one ballot and one read of the start bits per step); a
+// run that spans steps is carried in f64.  The row of a group follows from counting segment-start bits.
+// A lane ends at most G runs per step: one at each position followed by a segment start, and the one open
+// at its end.
 // SPECIAL = the chunk starts or ends inside a segment (rare: segments longer than a chunk); the common
 // instantiation carries none of the side-buffer logic.
 template <bool SPECIAL>
@@ -204,9 +204,27 @@ __device__ __forceinline__ void cb_emit(const PrArgs& a, uint32_t c, bool is_end
     a.partial[slot0 + cum] = (float)tot;
   }
 }
-template <bool SPECIAL>
-__device__ __forceinline__ void cb_chunk_impl(const PrArgs& a, const float* xs, uint32_t c, const uint4 ch,
-                                              uint32_t lane, uint32_t pad2) {
+// A lane's k-th load of a step.  With one load per lane (G = 2) the ids are streamed past L1, so that
+// the gathered vector stays there; with two (G = 4) the second load reads the other half of the sectors
+// of the first one, so they are kept in L1.
+template <uint32_t G>
+__device__ __forceinline__ uint4 cb_ld_ids(const uint4* p) {
+  if constexpr (G == 2) {
+    return ld_stream_u4(reinterpret_cast<const uint32_t*>(p));
+  } else {
+    uint4 r;
+    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
+    return r;
+  }
+}
+__device__ __forceinline__ float cb_group_sum(const float* xs, uint32_t lo, uint32_t hi) {
+  return xs[lo & 0xFFFFu] + xs[lo >> 16] + (xs[hi & 0xFFFFu] + xs[hi >> 16]);
+}
+template <uint32_t G, bool SPECIAL>
+__device__ __forceinline__ void cb_walk(const PrArgs& a, const float* xs, uint32_t c, const uint4 ch, uint32_t lane,
+                                        uint32_t pad2) {
+  constexpr uint32_t NL = G / 2;    // 128-bit loads and 64-bit start-bit words per lane and step
+  constexpr uint32_t STEP = 32 * G;  // groups per step
   const uint32_t g0 = ch.x, g1 = ch.y;
   const uint32_t j = ch.w & 0xFFFFFFu, fl = ch.w >> 24;
   const bool head_cont = SPECIAL && (fl & CB_HEAD_CONT), tail_cont = SPECIAL && (fl & CB_TAIL_CONT);
@@ -214,34 +232,64 @@ __device__ __forceinline__ void cb_chunk_impl(const PrArgs& a, const float* xs, 
   bool in_head = head_cont;
   double carry = 0.0;
   const uint32_t le_mask = 0xFFFFFFFFu >> (31u - lane);
-  const uint32_t ia = 2 * lane, ib = ia + 1;
-  const uint4* ids16 = reinterpret_cast<const uint4*>(a.cb_ids);  // pairs of groups
+  const uint32_t q0 = G * lane;  // the lane's first position in the step
+  const uint4* ids16 = reinterpret_cast<const uint4*>(a.cb_ids) + NL * lane;  // pairs of groups
   const uint4 padv = make_uint4(pad2, pad2, pad2, pad2);
-  const uint32_t gs0 = g0 & ~1u;
-  uint4 ids = padv;
-  if (gs0 + ia < g1) ids = ld_stream_u4(reinterpret_cast<const uint32_t*>(ids16 + (gs0 >> 1) + lane));
-  for (uint32_t gs = gs0; gs < g1; gs += 64) {
-    uint4 nids = padv;
-    if (gs + 64 + ia < g1) nids = ld_stream_u4(reinterpret_cast<const uint32_t*>(ids16 + ((gs + 64) >> 1) + lane));
-    // groups outside [g0, g1) belong to the neighbouring chunks
-    if (gs + ia < g0) ids.x = ids.y = pad2;
-    if (gs + ib >= g1) ids.z = ids.w = pad2;
+  const auto load = [&](uint4(&d)[NL], uint32_t gs) {  // the lane's pairs of the step at gs that start below g1
+#pragma unroll
+    for (uint32_t k = 0; k < NL; ++k) d[k] = gs + q0 + 2 * k < g1 ? cb_ld_ids<G>(ids16 + (gs >> 1) + k) : padv;
+  };
+  uint4 ids[NL], nids[NL];
+  load(ids, g0 & ~1u);
+  for (uint32_t gs = g0 & ~1u; gs < g1; gs += STEP) {
+    load(nids, gs + STEP);
+    // groups outside [g0, g1) belong to the neighbouring chunks: only position 0 can lie before g0, and the
+    // loads above already left out the pairs that start past g1
+    if (gs + q0 < g0) ids[0].x = ids[0].y = pad2;
+#pragma unroll
+    for (uint32_t k = 0; k < NL; ++k)
+      if (gs + q0 + 2 * k + 1 >= g1) ids[k].z = ids[k].w = pad2;
     const uint32_t wi = gs >> 5, sh = gs & 31u;
-    const uint32_t w0 = __ldg(a.cb_bits + wi), w1 = __ldg(a.cb_bits + wi + 1), w2 = __ldg(a.cb_bits + wi + 2);
-    unsigned long long W = ((unsigned long long)__funnelshift_r(w1, w2, sh) << 32) | __funnelshift_r(w0, w1, sh);
-    const uint32_t nvalid = min(64u, g1 - gs);
-    if (nvalid < 64) W &= (1ull << nvalid) - 1ull;
-    if (gs < g0) W &= ~1ull;
+    uint32_t w[G + 1];
+#pragma unroll
+    for (uint32_t k = 0; k <= G; ++k) w[k] = __ldg(a.cb_bits + wi + k);
+    const uint32_t nvalid = min(STEP, g1 - gs);
+    unsigned long long W[NL];  // segment starts at the step's positions 64 k .. 64 k + 63, inside [g0, g1)
+#pragma unroll
+    for (uint32_t k = 0; k < NL; ++k) {
+      W[k] = ((unsigned long long)__funnelshift_r(w[2 * k + 1], w[2 * k + 2], sh) << 32) |
+             __funnelshift_r(w[2 * k], w[2 * k + 1], sh);
+      if (nvalid < 64 * k + 64) W[k] = k == 0 || nvalid > 64 * k ? W[k] & ((1ull << (nvalid - 64 * k)) - 1ull) : 0ull;
+    }
+    if (gs < g0) W[0] &= ~1ull;
     const uint32_t last = nvalid - 1;
-    const bool last_step = gs + 64 >= g1;
+    const bool last_step = gs + STEP >= g1;
     // does the run of the last valid group go on after this step (inside the chunk / past its end)?
-    const bool run_continues = last_step ? tail_cont : !((w2 >> sh) & 1u);
-    const float va = xs[ids.x & 0xFFFFu] + xs[ids.x >> 16] + (xs[ids.y & 0xFFFFu] + xs[ids.y >> 16]);
-    const float vb = xs[ids.z & 0xFFFFu] + xs[ids.z >> 16] + (xs[ids.w & 0xFFFFu] + xs[ids.w >> 16]);
-    const uint32_t pair = (uint32_t)(W >> ia) & 3u;
-    const bool fa = pair & 1u, fb = pair & 2u;
-    float incl = fb ? vb : va + vb;  // this lane's share of the run open at its end
-    const uint32_t below = __ballot_sync(0xFFFFFFFFu, pair != 0) & le_mask;
+    const bool run_continues = last_step ? tail_cont : !((w[G] >> sh) & 1u);
+    // the word of the lane's positions, the word of the position after them, and the starts before them
+    const uint32_t s = q0 & 63u, e = q0 + G;
+    unsigned long long Wm = W[0], We = W[0];
+    uint32_t pre = 0;
+#pragma unroll
+    for (uint32_t k = 1; k < NL; ++k) {
+      if (q0 >= 64 * k) {
+        pre += __popcll(W[k - 1]);
+        Wm = W[k];
+      }
+      if (e >= 64 * k) We = W[k];
+    }
+    pre += __popcll(Wm & ((1ull << s) - 1ull));
+    const uint32_t F = (uint32_t)(Wm >> s) & ((1u << G) - 1u);  // segment starts at the lane's G positions
+    const bool nxt = lane < 31 && ((We >> (e & 63u)) & 1ull);   // and at the position after them
+    float v[G], r[G];  // group sums; runs inside the lane (restarted at every start)
+#pragma unroll
+    for (uint32_t i = 0; i < G; ++i) v[i] = i & 1 ? cb_group_sum(xs, ids[i / 2].z, ids[i / 2].w)
+                                                  : cb_group_sum(xs, ids[i / 2].x, ids[i / 2].y);
+    r[0] = v[0];
+#pragma unroll
+    for (uint32_t i = 1; i < G; ++i) r[i] = (F >> i) & 1u ? v[i] : r[i - 1] + v[i];
+    float incl = r[G - 1];  // this lane's share of the run open at its end
+    const uint32_t below = __ballot_sync(0xFFFFFFFFu, F != 0) & le_mask;
     const int seg_start = below ? 31 - __clz(below) : -1;
     const int lo = seg_start < 0 ? 0 : seg_start;
 #pragma unroll
@@ -252,123 +300,36 @@ __device__ __forceinline__ void cb_chunk_impl(const PrArgs& a, const float* xs, 
     const double incl_d = (double)incl + (seg_start < 0 ? carry : 0.0);
     double x_in = __shfl_up_sync(0xFFFFFFFFu, incl_d, 1);  // the run open at the end of the previous lane
     if (lane == 0) x_in = carry;
-    const uint32_t cum_a = __popcll(W & ((2ull << ia) - 1ull));  // segment starts at positions <= ia
-    const uint32_t cum_b = cum_a + (fb ? 1u : 0u);
-    const bool valid_a = gs + ia >= g0 && ia <= last, valid_b = ib <= last;
-    const bool nxt = ib < 63 ? ((W >> (ib + 1)) & 1ull) != 0 : false;
-    cb_emit<SPECIAL>(a, c, valid_a && (ia == last || fb), ia, last, run_continues, last_step, tail_cont, in_head,
-                     cum_a, slot0, (fa ? 0.0 : x_in) + (double)va);
-    cb_emit<SPECIAL>(a, c, valid_b && (ib == last || nxt), ib, last, run_continues, last_step, tail_cont, in_head,
-                     cum_b, slot0, incl_d);
-    const double tl = __shfl_sync(0xFFFFFFFFu, incl_d, 31);
-    carry = (run_continues && !last_step) ? tl : 0.0;
-    if (SPECIAL && W) in_head = false;
-    slot0 += __popcll(W);
-    ids = nids;
-  }
-}
-// The 128-group step (512 ids) of chunks with at least CB_WIDE_MIN groups: lane L owns groups 4L..4L+3
-// (two 128-bit loads), adds the runs inside the lane in f32 and ends up to four of them, and the warp
-// runs ONE segmented scan, one ballot and one read of the start bits per 512 ids instead of two.
-__device__ __forceinline__ uint4 ld_ids_u4(const uint4* p) {
-  uint4 r;  // the lane's second load reads the other half of the sectors of its first one: keep them in L1
-  asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
-  return r;
-}
-__device__ __forceinline__ float cb_group_sum(const float* xs, uint32_t lo, uint32_t hi) {
-  return xs[lo & 0xFFFFu] + xs[lo >> 16] + (xs[hi & 0xFFFFu] + xs[hi >> 16]);
-}
-template <bool SPECIAL>
-__device__ __forceinline__ void cb_chunk_wide(const PrArgs& a, const float* xs, uint32_t c, const uint4 ch,
-                                              uint32_t lane, uint32_t pad2) {
-  const uint32_t g0 = ch.x, g1 = ch.y;
-  const uint32_t j = ch.w & 0xFFFFFFu, fl = ch.w >> 24;
-  const bool head_cont = SPECIAL && (fl & CB_HEAD_CONT), tail_cont = SPECIAL && (fl & CB_TAIL_CONT);
-  uint32_t slot0 = a.poff[j] + ch.z;
-  bool in_head = head_cont;
-  double carry = 0.0;
-  const uint32_t le_mask = 0xFFFFFFFFu >> (31u - lane);
-  const uint32_t q0 = 4 * lane;  // the lane's first position in the step
-  const uint4* ids16 = reinterpret_cast<const uint4*>(a.cb_ids);
-  const uint4 padv = make_uint4(pad2, pad2, pad2, pad2);
-  const uint32_t gs0 = g0 & ~1u;
-  uint4 i0 = padv, i1 = padv;
-  if (gs0 + q0 < g1) i0 = ld_ids_u4(ids16 + (gs0 >> 1) + 2 * lane);
-  if (gs0 + q0 + 2 < g1) i1 = ld_ids_u4(ids16 + (gs0 >> 1) + 2 * lane + 1);
-  for (uint32_t gs = gs0; gs < g1; gs += 128) {
-    uint4 n0 = padv, n1 = padv;
-    if (gs + 128 + q0 < g1) n0 = ld_ids_u4(ids16 + ((gs + 128) >> 1) + 2 * lane);
-    if (gs + 128 + q0 + 2 < g1) n1 = ld_ids_u4(ids16 + ((gs + 128) >> 1) + 2 * lane + 1);
-    if (gs + q0 < g0) i0.x = i0.y = pad2;  // only position 0 can lie before g0 (gs0 = g0 & ~1)
-    if (gs + q0 + 1 >= g1) i0.z = i0.w = pad2;
-    if (gs + q0 + 2 >= g1) i1.x = i1.y = pad2;
-    if (gs + q0 + 3 >= g1) i1.z = i1.w = pad2;
-    const uint32_t wi = gs >> 5, sh = gs & 31u;
-    const uint32_t w0 = __ldg(a.cb_bits + wi), w1 = __ldg(a.cb_bits + wi + 1), w2 = __ldg(a.cb_bits + wi + 2),
-                   w3 = __ldg(a.cb_bits + wi + 3), w4 = __ldg(a.cb_bits + wi + 4);
-    unsigned long long WL = ((unsigned long long)__funnelshift_r(w1, w2, sh) << 32) | __funnelshift_r(w0, w1, sh);
-    unsigned long long WH = ((unsigned long long)__funnelshift_r(w3, w4, sh) << 32) | __funnelshift_r(w2, w3, sh);
-    const uint32_t nvalid = min(128u, g1 - gs);
-    if (nvalid < 64) {
-      WL &= (1ull << nvalid) - 1ull;
-      WH = 0;
-    } else if (nvalid < 128) {
-      WH &= (1ull << (nvalid - 64)) - 1ull;
-    }
-    if (gs < g0) WL &= ~1ull;
-    const uint32_t last = nvalid - 1;
-    const bool last_step = gs + 128 >= g1;
-    const bool run_continues = last_step ? tail_cont : !((w4 >> sh) & 1u);
-    const float v0 = cb_group_sum(xs, i0.x, i0.y), v1 = cb_group_sum(xs, i0.z, i0.w);
-    const float v2 = cb_group_sum(xs, i1.x, i1.y), v3 = cb_group_sum(xs, i1.z, i1.w);
-    const unsigned long long Wm = lane < 16 ? WL : WH;
-    const uint32_t s4 = q0 & 63u;
-    const uint32_t F = (uint32_t)(Wm >> s4) & 15u;  // segment starts at the lane's four positions
-    const bool nxt = lane == 31 ? false : lane == 15 ? (WH & 1ull) != 0 : ((Wm >> (s4 + 4)) & 1ull) != 0;
-    // runs inside the lane (restarted at every start)
-    const float r0 = v0;
-    const float r1 = (F & 2u) ? v1 : r0 + v1;
-    const float r2 = (F & 4u) ? v2 : r1 + v2;
-    float incl = (F & 8u) ? v3 : r2 + v3;  // this lane's share of the run open at its end
-    const uint32_t below = __ballot_sync(0xFFFFFFFFu, F != 0) & le_mask;
-    const int seg_start = below ? 31 - __clz(below) : -1;
-    const int lo = seg_start < 0 ? 0 : seg_start;
 #pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const float t = __shfl_up_sync(0xFFFFFFFFu, incl, d);
-      if ((int)lane - d >= lo) incl += t;
+    for (uint32_t i = 0; i < G; ++i) {
+      const uint32_t q = q0 + i, Fi = F & ((2u << i) - 1u);  // segment starts at the lane's positions <= q
+      const bool valid = q <= last && (i > 0 || gs + q0 >= g0);
+      const bool ends = i + 1 < G ? ((F >> (i + 1)) & 1u) != 0 : nxt;
+      cb_emit<SPECIAL>(a, c, valid && (q == last || ends), q, last, run_continues, last_step, tail_cont, in_head,
+                       pre + __popc(Fi), slot0, i + 1 < G ? (double)r[i] + (Fi ? 0.0 : x_in) : incl_d);
     }
-    const double incl_d = (double)incl + (seg_start < 0 ? carry : 0.0);
-    double x_in = __shfl_up_sync(0xFFFFFFFFu, incl_d, 1);
-    if (lane == 0) x_in = carry;
-    const uint32_t pre = (lane < 16 ? 0u : (uint32_t)__popcll(WL)) + (uint32_t)__popcll(Wm & ((1ull << s4) - 1ull));
-    const bool valid0 = gs + q0 >= g0 && q0 <= last;
-    cb_emit<SPECIAL>(a, c, valid0 && (q0 == last || (F & 2u)), q0, last, run_continues, last_step, tail_cont,
-                     in_head, pre + (F & 1u), slot0, (double)r0 + ((F & 1u) ? 0.0 : x_in));
-    cb_emit<SPECIAL>(a, c, q0 + 1 <= last && (q0 + 1 == last || (F & 4u)), q0 + 1, last, run_continues, last_step,
-                     tail_cont, in_head, pre + __popc(F & 3u), slot0, (double)r1 + ((F & 3u) ? 0.0 : x_in));
-    cb_emit<SPECIAL>(a, c, q0 + 2 <= last && (q0 + 2 == last || (F & 8u)), q0 + 2, last, run_continues, last_step,
-                     tail_cont, in_head, pre + __popc(F & 7u), slot0, (double)r2 + ((F & 7u) ? 0.0 : x_in));
-    cb_emit<SPECIAL>(a, c, q0 + 3 <= last && (q0 + 3 == last || nxt), q0 + 3, last, run_continues, last_step,
-                     tail_cont, in_head, pre + __popc(F), slot0, incl_d);
     const double tl = __shfl_sync(0xFFFFFFFFu, incl_d, 31);
     carry = (run_continues && !last_step) ? tl : 0.0;
-    if (SPECIAL && (WL | WH)) in_head = false;
-    slot0 += __popcll(WL) + __popcll(WH);
-    i0 = n0;
-    i1 = n1;
+    unsigned long long any = 0;
+#pragma unroll
+    for (uint32_t k = 0; k < NL; ++k) {
+      any |= W[k];
+      slot0 += __popcll(W[k]);
+      ids[k] = nids[k];
+    }
+    if (SPECIAL && any) in_head = false;
   }
 }
 __device__ __forceinline__ void cb_chunk(const PrArgs& a, const float* xs, uint32_t c, uint32_t lane, uint32_t pad2) {
   const uint4 ch = a.chunks[c];
   if (ch.x >= ch.y) return;
   const bool special = (ch.w >> 24) & (CB_HEAD_CONT | CB_TAIL_CONT);
-  if (ch.y - ch.x >= CB_WIDE_MIN) {
-    if (special) cb_chunk_wide<true>(a, xs, c, ch, lane, pad2);
-    else cb_chunk_wide<false>(a, xs, c, ch, lane, pad2);
+  if (cb_step_groups(ch.x, ch.y) == 4) {
+    if (special) cb_walk<4, true>(a, xs, c, ch, lane, pad2);
+    else cb_walk<4, false>(a, xs, c, ch, lane, pad2);
   } else {
-    if (special) cb_chunk_impl<true>(a, xs, c, ch, lane, pad2);
-    else cb_chunk_impl<false>(a, xs, c, ch, lane, pad2);
+    if (special) cb_walk<2, true>(a, xs, c, ch, lane, pad2);
+    else cb_walk<2, false>(a, xs, c, ch, lane, pad2);
   }
 }
 
@@ -422,7 +383,7 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
   const uint32_t R = gridDim.x;  // ranges = CTAs
   const uint32_t mbar = (uint32_t)__cvta_generic_to_shared(&s_mbar);
   const uint32_t xs_smem = (uint32_t)__cvta_generic_to_shared(xs);
-  const bool bulk_ok = (reinterpret_cast<uintptr_t>(a.x_cur) & 15u) == 0 && !(a.dbg & 4u);  // cp.async.bulk moves 16-byte units
+  const bool bulk_ok = (reinterpret_cast<uintptr_t>(a.x_cur) & 15u) == 0;  // cp.async.bulk moves 16-byte units
   uint32_t phase = 0;
   if (threadIdx.x == 0) mbar_init(mbar, 1);
   if (threadIdx.x < 4) xs[B + threadIdx.x] = 0.0f;  // the pad id's zero slot: never overwritten
@@ -492,7 +453,7 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
       cb_chunk(a, xs, task.x + k, lane, pad2);
       uint32_t nx = 0;
       if (lane == 0) nx = atomicAdd(&s_next, 1u);
-      k = (a.dbg & 2u) ? k + PR_THREADS / 32 : __shfl_sync(0xFFFFFFFFu, nx, 0);
+      k = __shfl_sync(0xFFFFFFFFu, nx, 0);
     }
   }
 }
@@ -546,7 +507,7 @@ __global__ void __launch_bounds__(PR_SELL_THREADS, 2) k_pr_sell(const PrArgs a) 
   const uint32_t P = a.deal.P, pp = a.deal.p;
   // slices are dealt CTA-minor: the widest slices (the first ones) land on different SMs, not on the 16
   // warps of CTA 0 (an eighth-shard ran with its busiest SM 31 % above the average otherwise)
-  uint32_t sidx = (a.dbg & 1u) ? blockIdx.x * NW + warp : warp * gridDim.x + blockIdx.x;
+  uint32_t sidx = warp * gridDim.x + blockIdx.x;
   // pipeline state: metadata of this and the next slice, first two target groups + row data of this one
   uint2 meta = make_uint2(0, 0), nmeta = meta;
   uint4 ta = pad, tb = pad;
@@ -933,7 +894,6 @@ static PrArgs make_args(const PrPlan* p, float base, float damping, double toler
     a.few_poff[j] = p->few_poff[j];
   }
   a.fix_in_sell = fix_in_sell(p) ? 1u : 0u;
-  a.dbg = env_u32("GB_PR_DEBUG", 0);
   a.B = p->B;
   a.KB = p->KB;
   a.blk = p->blk.p;

@@ -459,7 +459,7 @@ __global__ void k_cb_chunks(const uint32_t* __restrict__ goff, const uint32_t* _
 }
 
 // Bank-aware order of the ids inside each group (tools/cb_bank_model.py restates it).  A step of k_pr_cb
-// reads a WINDOW of 32 G groups (G = 2, or 4 in chunks of at least CB_WIDE_MIN groups): lane L's groups
+// reads a WINDOW of 32 G groups (G = cb_step_groups, the kernel's choice for the chunk): lane L's groups
 // G L + i (i < G) feed its shared-memory reads 4i..4i+3, and each of those read instructions takes as many
 // wavefronts as its most crowded bank (id & 31) holds words.  The 4 ids of a group belong to one (row,
 // block) pair, so their order only changes the rounding of the group's sum.  One thread per SET i of a
@@ -496,7 +496,7 @@ __global__ void __launch_bounds__(CB_BANK_THREADS) k_cb_bank_order(const uint4* 
     const uint4 ch = chunks[c];
     const uint32_t g0 = ch.x, g1 = ch.y;
     if (g0 >= g1) continue;
-    const uint32_t G = g1 - g0 >= CB_WIDE_MIN ? 4u : 2u;  // groups per lane in the chunk's steps
+    const uint32_t G = cb_step_groups(g0, g1);
     const uint32_t set = lane % G;
     for (uint32_t gw = (g0 & ~1u) + 32 * G * (lane / G); gw < g1; gw += 32 * 32) {
       clear();

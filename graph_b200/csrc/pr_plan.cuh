@@ -21,6 +21,10 @@ constexpr double CB_TAU_DEFAULT = 1.5;       // a (row, block) pair gets a segme
 constexpr uint32_t CB_MAX_BLOCKS = 8192;     // hot blocks kept (the staircase rarely needs more than ~1000)
 constexpr uint32_t CB_TASK_CHUNKS = 32;      // chunks per task (one per warp)
 constexpr uint32_t CB_WIDE_MIN = 128;        // chunks of at least this many groups take k_pr_cb's 128-group step
+// groups per lane in k_pr_cb's steps over chunk [g0, g1); k_cb_bank_order orders the ids for those steps
+__host__ __device__ __forceinline__ uint32_t cb_step_groups(uint32_t g0, uint32_t g1) {
+  return g1 - g0 >= CB_WIDE_MIN ? 4u : 2u;
+}
 constexpr uint32_t SELL_FEW = 4;             // rows with segments in at most this many blocks are finished by k_pr_sell itself
 constexpr uint32_t FIN_CTA_BLOCKS = 64;      // finish: 32-row groups with segments in more blocks get a CTA each
 constexpr uint32_t CB_NONE = 0xFFFFFFFFu;

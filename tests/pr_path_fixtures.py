@@ -11,13 +11,14 @@ import numpy as np
 
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT / "tools"))
+import cb_bank_model as bm  # noqa: E402
 import layout_model as lm  # noqa: E402
 
 import oracle  # noqa: E402
 
 TAIL_R = (1, 2, 3, 5, 33)
 # every environment knob of the plan build and the sweep (graph_b200/csrc/pr_layout.cu, pagerank.cu)
-KNOBS = ("GB_PR_BLOCK", "GB_PR_TAU", "GB_PR_MEGA", "GB_PR_CHUNK", "GB_PR_TASK_CHUNKS", "GB_PR_DEBUG", "GB_PR_FIN_U",
+KNOBS = ("GB_PR_BLOCK", "GB_PR_TAU", "GB_PR_MEGA", "GB_PR_CHUNK", "GB_PR_TASK_CHUNKS", "GB_PR_FIN_U",
          "GB_PR_FIN_SPLIT", "GB_PR_FEED_CHUNKS", "GB_PR_FEED_MIN_EDGES")
 
 
@@ -133,6 +134,14 @@ def model(name, P=1, p=0, sms=lm.H100_SMS, **knobs):
     plan = lm.make_plan(inc[0].astype(np.int64), inc[1], np.diff(out[0].astype(np.int64)), B, lm.CB_TAU_DEFAULT,
                         P=P, p=p)
     return plan, lm.launch_shape(plan, sms=sms, **knobs), lm.layout_counts(plan, inc[0], inc[1])
+
+
+def chunks(name, sms=lm.H100_SMS):
+    """k_pr_cb's chunks of a fixture at its knobs, by the layout model: (g0, g1, a segment is cut at either end)"""
+    _, _, n, out, inc = graph(name)
+    B = lm.clamp_block(FIXTURES[name][1] or lm.CB_BLOCK_DEFAULT)
+    plan, goff, _ = bm.build_streams(inc[0].astype(np.int64), inc[1], np.diff(out[0].astype(np.int64)), B=B)
+    return bm.chunk_table(plan, goff, sms=sms)
 
 
 def check_path(name, plan, shape):

@@ -1,8 +1,8 @@
 """The JACOBI PageRank sweep on graphs built to reach its less common paths (tests/pr_path_fixtures.py):
 the partial last column block (scalar tail of the block load), a rectangular staircase, a mega row cut by
 chunk boundaries, a repeated source, fewer than 32 active rows, the hub-group CTAs of k_pr_finish, its
-FIN_U = 4 instantiation, its role split, a capped finish grid, and the GB_PR_DEBUG / GB_PR_TASK_CHUNKS
-variants.  Every case asserts that the device plan took the path (against the layout
+FIN_U = 4 instantiation, its role split, a capped finish grid, the GB_PR_TASK_CHUNKS variant, and x vectors
+that are not 16-byte aligned.  Every case asserts that the device plan took the path (against the layout
 model), that the ranks match the f64-accumulating oracle, and that runs and arithmetic-preserving variants
 give the same bits."""
 import ctypes as C
@@ -80,6 +80,7 @@ def test_fixture_path_ranks_and_determinism(gb, sms, monkeypatch, name):
     set_knobs(monkeypatch, name)
     g = device_graph(gb, name)
     plan, shape, info = assert_shape(g, name, sms)
+    assert info["chunks"] == len(fx.chunks(name, sms))                # the chunk table of the model
     if sms == fx.lm.H100_SMS:
         fx.check_path(name, plan, shape)
     pr = run(g)
@@ -95,16 +96,26 @@ def test_fixture_path_ranks_and_determinism(gb, sms, monkeypatch, name):
 
 @pytest.mark.parametrize("r", fx.TAIL_R)
 def test_tail_block_loads_and_streamed_upload(gb, monkeypatch, r):
+    import torch
     from graph_b200 import _capi
     from graph_b200._capi import check, lib
+    from graph_b200.multigpu import CudaShardBackend
     name = f"tail_r{r}"
     set_knobs(monkeypatch, name)
     g = device_graph(gb, name)
     want = run(g)
-    monkeypatch.setenv("GB_PR_DEBUG", "4")                            # element-wise block loads, no TMA
-    assert_same_bits(run(g), want, "GB_PR_DEBUG=4")
-    monkeypatch.delenv("GB_PR_DEBUG")
     _, _, n, out, inc = fx.graph(name)
+    # a one-rank shard whose x vectors start one float past a 16-byte boundary: no TMA, element-wise block loads
+    b = CudaShardBackend(g, 0, 1)
+    x = [torch.zeros(n + 4, dtype=torch.float32, device=b.device)[1:n + 1] for _ in range(2)]
+    assert all(v.data_ptr() % 16 == 4 for v in x)
+    scores = torch.empty(n, dtype=torch.float32, device=b.device)
+    err = torch.zeros(1, dtype=torch.float64, device=b.device)
+    b.init(0.85, x[0], x[1], scores)
+    for sweep in range(1, SWEEPS + 1):
+        b.step(0.85, sweep, x[(sweep - 1) & 1], x[sweep & 1], None, scores, err)
+    assert b.finish(scores).cpu().numpy().tobytes() == want.scores().tobytes()
+    assert abs(err.item() - want.error) <= 1e-12 * abs(want.error)
     P = lambda a: a.ctypes.data_as(C.c_void_p)
     monkeypatch.setenv("GB_PR_FEED_MIN_EDGES", "0")
     for chunks in (1, 7):
@@ -117,17 +128,13 @@ def test_tail_block_loads_and_streamed_upload(gb, monkeypatch, r):
         assert it.value == SWEEPS and scores.tobytes() == want.scores().tobytes() and err.value == want.error, chunks
 
 
-# GB_PR_FIN_U 2 vs 4 and the role split keep every row's f64 sum in the same block order; the GB_PR_DEBUG
-# bits change who does the work, not the arithmetic: all bit-equal to the automatic plan
+# GB_PR_FIN_U 2 vs 4 and the role split keep every row's f64 sum in the same block order: all bit-equal to
+# the automatic plan
 BIT_EQUAL = [
     ({"GB_PR_FIN_U": 4}, {"fin_u": 4}),
     ({"GB_PR_FIN_SPLIT": 1}, {"fin_split": 1}),
     ({"GB_PR_FIN_U": 4, "GB_PR_FIN_SPLIT": 1}, {"fin_u": 4, "fin_split": 1}),
     ({"GB_PR_FIN_SPLIT": 2}, {"fin_split": 2}),
-    ({"GB_PR_DEBUG": 1}, {}),
-    ({"GB_PR_DEBUG": 2}, {}),
-    ({"GB_PR_DEBUG": 4}, {}),
-    ({"GB_PR_DEBUG": 7}, {}),
 ]
 
 

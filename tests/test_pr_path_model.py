@@ -14,6 +14,15 @@ def test_fixture_reaches_its_path(name):
     assert counts["segments"] == plan["S"] and counts["block_edges"] > 0
 
 
+def test_fixtures_reach_every_walker_instantiation():
+    """k_pr_cb walks a chunk with G = 2 or 4 groups per lane (cb_step_groups), with or without the side-buffer
+    logic of a segment cut at a chunk end: the fixtures reach all four instantiations"""
+    kinds = set()
+    for name in fx.FIXTURES:
+        kinds |= {(fx.bm.cb_model.step_groups(g0, g1), cut) for g0, g1, cut in fx.chunks(name) if g0 < g1}
+    assert kinds == {(2, False), (2, True), (4, False), (4, True)}
+
+
 def test_finish_knobs_on_rmat18():
     plan, auto, _ = fx.model("rmat18")
     assert (auto["hot_blocks"], auto["n_cb"], auto["n_fin"], auto["n_fin_warp"]) == (148, 69628, 12640, 192)

@@ -1,9 +1,9 @@
 """cb_bank_model.py — CPU count of the shared-memory bank conflicts of k_pr_cb's gathers, before and
 after the bank-aware order of the ids inside each group (pr_layout.cu: k_cb_bank_order).
 
-A warp step of k_pr_cb covers a WINDOW of 32 G groups (G = 2, or 4 in chunks of at least CB_WIDE_MIN
-groups): lane L reads groups G L .. G L + G - 1 and then issues 4 shared-memory reads xs[id] per group, one
-per SLOT.  The reads of group G L + i of all lanes form the SET i of the window.  One read instruction
+A warp step of k_pr_cb covers a WINDOW of 32 G groups (G = cb_step_groups: 4 in chunks of at least
+CB_WIDE_MIN groups, else 2): lane L reads groups G L .. G L + G - 1 and then issues 4 shared-memory reads
+xs[id] per group, one per SLOT.  The reads of group G L + i of all lanes form the SET i of the window.  One read instruction
 takes as many wavefronts as the most crowded bank holds distinct words (bank = id & 31); all lanes that
 read the padding id B hit the same word, which is a broadcast.  The 4 ids of a group belong to one
 (row, block) pair, so their order is free: k_cb_bank_order lets lane 0, 1, ... in turn put the 4 ids of
@@ -60,7 +60,8 @@ def build_streams(in_off, in_tgt, out_deg, B=lm.CB_BLOCK_DEFAULT, tau=lm.CB_TAU_
 
 
 def chunk_table(plan, goff, sms=lm.H100_SMS, T=CB_TASK_CHUNKS):
-    """The layout_chunks stage of build_pr_plan: per-block chunk sizes, then k_cb_chunks (cb_model.cb_cut)."""
+    """The layout_chunks stage of build_pr_plan: per-block chunk sizes, then k_cb_chunks (cb_model.cb_cut).
+    Returns (g0, g1, a segment is cut at either end) per chunk."""
     NG = int(goff[-1])
     gbeg = goff[plan["poff"]]
     C = min(max(NG // (sms * 8 * T), 16384 // T), 65536 // T)
@@ -75,21 +76,16 @@ def chunk_table(plan, goff, sms=lm.H100_SMS, T=CB_TASK_CHUNKS):
         for k in range(nc):
             a = cb_model.cb_cut(goff_j, nr, g1, g0 + k * Cj, Cj)
             b = (g1, nr, False) if k + 1 == nc else cb_model.cb_cut(goff_j, nr, g1, g0 + (k + 1) * Cj, Cj)
-            chunks.append((int(a[0]), int(b[0])))
+            chunks.append((int(a[0]), int(b[0]), bool(a[2] or b[2])))
     return chunks
-
-
-def step_groups(g0, g1):
-    """groups per lane in the steps of chunk [g0, g1): 4 from CB_WIDE_MIN groups on, else 2"""
-    return 4 if g1 - g0 >= cb_model.WIDE_MIN else 2
 
 
 def windows(chunks):
     """(first group of the step, lowest and highest+1 group the step may read, groups per lane) for every
     kernel step"""
     out = []
-    for g0, g1 in chunks:
-        G = step_groups(g0, g1)
+    for g0, g1, *_ in chunks:
+        G = cb_model.step_groups(g0, g1)
         for gs in range(g0 & ~1, g1, 32 * G):
             out.append((gs, g0, g1, G))
     return np.array(out, np.int64).reshape(-1, 4)

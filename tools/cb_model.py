@@ -1,5 +1,5 @@
 """cb_model.py — lane-level numpy model of the column-block kernel's chunk logic (pr_layout.cu:
-cb_cut / k_cb_chunks; pagerank.cu: cb_chunk_impl / cb_fix_segment).
+cb_cut / k_cb_chunks; pagerank.cu: cb_walk / cb_fix_segment).
 
 There is no GPU in the build container, so the trickiest index logic (chunk cuts inside long
 segments, start-bit row counting, the carried run, side buffers and their fixed-order fixup) is
@@ -58,87 +58,18 @@ def build_chunks(goff, poff, nrows, gbeg, C):
     return chunks, tail_slot, fix
 
 
-WIDE_MIN = 128   # CB_WIDE_MIN: chunks of at least this many groups take the 128-group step
+WIDE_MIN = 128   # CB_WIDE_MIN
 
 
-def run_chunk(c, chunks, vals, bits, poff, partial, side):
-    """cb_chunk: vals[g] = f32 sum of group g's four gathers; bits[g] = group g starts a segment.
-    A step covers 64 groups; lane L owns the adjacent groups 2L and 2L+1 of the (even-aligned) window.
-    Chunks of at least WIDE_MIN groups take the 128-group step of run_chunk_wide."""
-    g0, g1, row_before, j, fl = chunks[c]
-    if g0 >= g1:
-        return
-    if g1 - g0 >= WIDE_MIN:
-        run_chunk_wide(c, chunks, vals, bits, poff, partial, side)
-        return
-    head_cont, tail_cont = bool(fl & HEAD), bool(fl & TAIL)
-    in_head = head_cont
-    carry = 0.0
-    lanes = np.arange(32)
-    gs0 = g0 & ~1
-    for gs in range(gs0, g1, 64):
-        pos = np.arange(64)
-        valid = (gs + pos >= g0) & (gs + pos < g1)
-        W = np.zeros(64, bool)
-        W[valid] = bits[gs + pos[valid]]
-        v = np.zeros(64, np.float32)
-        v[valid] = vals[gs + pos[valid]]
-        last = int(np.nonzero(valid)[0][-1])
-        last_step = gs + 64 >= g1
-        run_continues = tail_cont if last_step else (not bits[gs + 64])
-        fa, fb = W[0::2], W[1::2]
-        va, vb = v[0::2], v[1::2]
-        T = np.where(fb, vb, (va + vb).astype(np.float32)).astype(np.float32)
-        F = fa | fb
-        seg_start = np.full(32, -1)
-        cur = -1
-        for l in range(32):
-            if F[l]:
-                cur = l
-            seg_start[l] = cur
-        lo = np.maximum(seg_start, 0)
-        incl = T.copy()
-        d = 1
-        while d < 32:
-            t = np.zeros(32, np.float32)
-            t[d:] = incl[:-d]
-            add = (lanes - d) >= lo
-            incl = np.where(add, (incl + t).astype(np.float32), incl)
-            d <<= 1
-        inclD = incl.astype(np.float64) + np.where(seg_start < 0, carry, 0.0)
-        XD = np.empty(32)
-        XD[0] = carry
-        XD[1:] = inclD[:-1]
-        cum = np.cumsum(W)                 # starts at positions <= q
-        for l in range(32):
-            ia, ib = 2 * l, 2 * l + 1
-            tot_a = (0.0 if fa[l] else XD[l]) + float(va[l])
-            tot_b = inclD[l]
-            end_a = valid[ia] and (ia == last or fb[l])
-            nxt = W[ib + 1] if ib + 1 < 64 else False
-            end_b = valid[ib] and (ib == last or nxt)
-            for (q, is_end, tot) in ((ia, end_a, tot_a), (ib, end_b, tot_b)):
-                if not is_end:
-                    continue
-                if q == last and run_continues and not last_step:
-                    continue
-                head_run = in_head and cum[q] == 0
-                if head_run:
-                    side[2 * c] = tot
-                elif q == last and last_step and tail_cont:
-                    side[2 * c + 1] = tot
-                else:
-                    partial[poff[j] + row_before + cum[q]] = np.float32(tot)
-        carry = inclD[31] if (run_continues and not last_step) else 0.0
-        if W.any():
-            in_head = False
-        row_before += int(W.sum())
+def step_groups(g0, g1):
+    """cb_step_groups: groups per lane in the steps of chunk [g0, g1), 4 from WIDE_MIN groups on, else 2"""
+    return 4 if g1 - g0 >= WIDE_MIN else 2
 
 
 def seg_scan(T, F, carry):
-    """the segmented inclusive warp scan of cb_chunk_impl: T = each lane's share of the run open at its
-    end (f32), F = the lane holds a segment start.  Returns (inclD, XD): the run open at the end of each
-    lane and at the end of the lane before it, in f64 with the carried run added."""
+    """the segmented inclusive warp scan of cb_walk: T = each lane's share of the run open at its end
+    (f32), F = the lane holds a segment start.  Returns (inclD, XD): the run open at the end of each lane
+    and at the end of the lane before it, in f64 with the carried run added."""
     lanes = np.arange(32)
     seg_start = np.full(32, -1)
     cur = -1
@@ -161,39 +92,45 @@ def seg_scan(T, F, carry):
     return inclD, XD
 
 
-def run_chunk_wide(c, chunks, vals, bits, poff, partial, side):
-    """cb_chunk_impl's 128-group step: lane L owns groups 4L..4L+3 of the window (two 128-bit loads),
-    adds the runs inside the lane in f32, and takes part in ONE segmented scan per 512 ids."""
+def run_chunk(c, chunks, vals, bits, poff, partial, side):
+    """cb_walk: vals[g] = f32 sum of group g's four gathers; bits[g] = group g starts a segment.
+    A step covers 32 G groups (G = step_groups) from g0 & ~1; lane L owns groups G L .. G L + G - 1 of the
+    window, adds the runs inside the lane in f32, and takes part in ONE segmented scan per step.
+    Returns G (None for an empty chunk)."""
     g0, g1, row_before, j, fl = chunks[c]
+    if g0 >= g1:
+        return None
+    G = step_groups(g0, g1)
+    S = 32 * G
     head_cont, tail_cont = bool(fl & HEAD), bool(fl & TAIL)
     in_head = head_cont
     carry = 0.0
-    for gs in range(g0 & ~1, g1, 128):
-        pos = np.arange(128)
+    for gs in range(g0 & ~1, g1, S):
+        pos = np.arange(S)
         valid = (gs + pos >= g0) & (gs + pos < g1)
-        W = np.zeros(128, bool)
+        W = np.zeros(S, bool)
         W[valid] = bits[gs + pos[valid]]
-        v = np.zeros(128, np.float32)
+        v = np.zeros(S, np.float32)
         v[valid] = vals[gs + pos[valid]]
         last = int(np.nonzero(valid)[0][-1])
-        last_step = gs + 128 >= g1
-        run_continues = tail_cont if last_step else (not bits[gs + 128])
-        F, V = W.reshape(32, 4), v.reshape(32, 4)
-        r = np.zeros((32, 4), np.float32)        # run sums inside the lane, restarted at each start
-        for i in range(4):
+        last_step = gs + S >= g1
+        run_continues = tail_cont if last_step else (not bits[gs + S])
+        F, V = W.reshape(32, G), v.reshape(32, G)
+        r = np.zeros((32, G), np.float32)        # run sums inside the lane, restarted at each start
+        for i in range(G):
             prev = r[:, i - 1] if i else np.zeros(32, np.float32)
             r[:, i] = np.where(F[:, i], V[:, i], (prev + V[:, i]).astype(np.float32))
-        inclD, XD = seg_scan(r[:, 3], F.any(axis=1), carry)
-        cum = np.cumsum(W)
+        inclD, XD = seg_scan(r[:, G - 1], F.any(axis=1), carry)
+        cum = np.cumsum(W)                 # starts at positions <= q
         for l in range(32):
-            for i in range(4):
-                q = 4 * l + i
-                nxt = W[q + 1] if q + 1 < 128 else False
+            for i in range(G):
+                q = G * l + i
+                nxt = W[q + 1] if q + 1 < S else False
                 if not (valid[q] and (q == last or nxt)):
                     continue
                 if q == last and run_continues and not last_step:
                     continue
-                if i == 3:
+                if i == G - 1:
                     tot = inclD[l]
                 else:
                     tot = float(r[l, i]) + (0.0 if F[l, :i + 1].any() else XD[l])
@@ -207,6 +144,7 @@ def run_chunk_wide(c, chunks, vals, bits, poff, partial, side):
         if W.any():
             in_head = False
         row_before += int(W.sum())
+    return G
 
 
 def fixup(fix, chunks, tail_slot, side, partial):
@@ -223,8 +161,9 @@ def fixup(fix, chunks, tail_slot, side, partial):
         partial[tail_slot[c0]] = np.float32(t)
 
 
-def simulate(nrows, groups_per_pair, C, rng):
-    """nrows[j] non-increasing; groups_per_pair: list of arrays (>= 1 group each)."""
+def simulate(nrows, groups_per_pair, C, rng, kinds=None):
+    """nrows[j] non-increasing; groups_per_pair: list of arrays (>= 1 group each).  kinds: a set that
+    receives (G, a segment is cut at either end) of every chunk that ran."""
     poff = np.concatenate([[0], np.cumsum(nrows)]).astype(np.int64)
     gpp = np.concatenate(groups_per_pair).astype(np.int64)
     goff = np.concatenate([[0], np.cumsum(gpp)]).astype(np.int64)
@@ -238,7 +177,9 @@ def simulate(nrows, groups_per_pair, C, rng):
     partial = np.full(int(poff[-1]), np.nan, np.float32)
     side = np.zeros(2 * len(chunks) + 2)
     for c in range(len(chunks)):
-        run_chunk(c, chunks, vals, bits, poff, partial, side)
+        G = run_chunk(c, chunks, vals, bits, poff, partial, side)
+        if G and kinds is not None:
+            kinds.add((G, bool(chunks[c][4] & (HEAD | TAIL))))
     fixup(fix, chunks, tail_slot, side, partial)
     want = np.array([vals[goff[e]:goff[e + 1]].astype(np.float64).sum() for e in range(len(gpp))])
     # coverage: every chunk boundary is consistent and every group belongs to exactly one chunk
