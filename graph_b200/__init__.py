@@ -21,7 +21,7 @@ from ._capi import GraphB200Error, check, lib
 
 __all__ = ["DiGraph", "Graph", "Layout", "FileFormat", "PageRankResult", "WccResult",
            "TriangleCountResult", "SsspResult", "PageRankConfig", "WccConfig", "DeltaSteppingConfig",
-           "GraphB200Error", "device_count", "set_device", "write_graph500"]
+           "GraphB200Error", "device_count", "set_device", "write_graph500", "wcc_csr"]
 
 _device = 0
 
@@ -695,3 +695,25 @@ class Graph(_Handle):
             check(lib.gb_triangle_count(self._g, C.byref(tri)))
         _, micros = _timed(go)
         return TriangleCountResult(int(tri.value), micros)
+
+
+def wcc_csr(offsets, targets, *, chunk_size: int = WccConfig.DEFAULT_CHUNK_SIZE,
+            neighbor_rounds: int = WccConfig.DEFAULT_NEIGHBOR_ROUNDS,
+            sampling_size: int = WccConfig.DEFAULT_SAMPLING_SIZE) -> WccResult:
+    """wcc_baseline (wcc.rs:103-123) of a host out-CSR without a resident twin: the offsets are uploaded, the
+    targets streamed through a ring of device buffers and linked as they land.  Same labels as
+    DiGraph.wcc() on the twin (the minimum node id of each component); the config is checked and otherwise
+    ignored.  Arrays are used as given: pass pinned contiguous uint32 arrays to overlap the links with the copy."""
+    off, tgt = np.asarray(offsets), np.asarray(targets)
+    for a in (off, tgt):
+        if a.dtype != np.uint32 or not a.flags.c_contiguous:
+            raise TypeError("wcc_csr needs contiguous uint32 arrays")
+    _check_host_csr(off, tgt, "out")
+    cfg = _capi.WccConfig(int(chunk_size), int(neighbor_rounds), int(sampling_size))
+    comp = np.empty(len(off) - 1, np.uint32)
+
+    def go():
+        check(lib.gb_wcc_csr_u32(_device, len(off) - 1, _ptr(off), _ptr(tgt) if len(tgt) else None, C.byref(cfg),
+                                 _ptr(comp)))
+    _, micros = _timed(go)
+    return WccResult(comp, micros)

@@ -122,6 +122,7 @@ SIGNATURES = {
     "gb_digraph_for_page_rank_u32": (C.c_int, [C.c_int, C.c_uint32, _P, _P, _P, C.POINTER(_P)]),
     "gb_wcc": (C.c_int, [_P, C.POINTER(WccConfig), _P]),
     "gb_wcc_device": (C.c_int, [_P, C.POINTER(WccConfig), _P]),
+    "gb_wcc_csr_u32": (C.c_int, [C.c_int, C.c_uint32, _P, _P, C.POINTER(WccConfig), _P]),
     "gb_wcc_shard_phase": (C.c_int, [_P, C.POINTER(WccConfig), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                      C.c_int, _P, _P, _P]),
     "gb_wcc_sample_label": (C.c_int, [_P, C.POINTER(WccConfig), _P, C.POINTER(C.c_uint32), C.POINTER(C.c_int), _P]),

@@ -9,6 +9,7 @@
 // Algorithmic bytes per run: 8m + 16n + 8 (both CSRs once, parent read + write); the sampling
 // phase lets most vertices skip their edge lists, so effective GB/s can exceed the HBM peak.
 #include <algorithm>
+#include <cstdlib>
 #include <vector>
 
 #include "common.cuh"
@@ -152,6 +153,106 @@ __global__ void k_cc_merge(uint32_t* parent, const uint32_t* __restrict__ other,
   }
 }
 
+// ---- one-shot WCC of a host out-CSR (gb_wcc_csr_u32): wcc_baseline, wcc.rs:103-123 ----------------------
+constexpr uint32_t LINK_TILE = 128;  // edges per warp step of k_cc_link_edges: one uint4 of targets per lane
+
+// the row r in [lo, hi) with off[r] <= e < off[r + 1], given off[lo] <= e < off[hi]
+__device__ __forceinline__ uint32_t row_search(const uint32_t* __restrict__ off, uint32_t lo, uint32_t hi, uint32_t e) {
+  while (hi - lo > 1) {
+    const uint32_t mid = lo + ((hi - lo) >> 1);
+    if (off[mid] <= e) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// the same search by a whole warp: 31 probes per step cut [lo, hi) 32-fold, so a row among 2^24 is found
+// in five dependent loads
+__device__ __forceinline__ uint32_t warp_row_search(const uint32_t* __restrict__ off, uint32_t lo, uint32_t hi,
+                                                    uint32_t e, uint32_t lane) {
+  while (hi - lo > 1) {
+    const uint32_t p = lo + (uint32_t)(((uint64_t)(hi - lo) * (lane + 1)) >> 5);  // lane 31 would probe hi
+    const unsigned le = __ballot_sync(0xFFFFFFFFu, lane < 31 && off[p] <= e);   // a prefix of the lanes
+    const int c = __popc(le);
+    const uint32_t below = __shfl_sync(0xFFFFFFFFu, p, c > 0 ? c - 1 : 0);
+    const uint32_t above = __shfl_sync(0xFFFFFFFFu, p, c < 31 ? c : 0);
+    if (c > 0) lo = below;
+    if (c < 31) hi = above;
+  }
+  return lo;
+}
+
+// the root of x; every non-root on the way is pointed at its grandparent (path halving).  The writes race
+// only with writes of other ancestors, and a CAS only ever changes a root, so parent[y] <= y and every tree
+// stay as they were
+__device__ __forceinline__ uint32_t find_halving(uint32_t* parent, uint32_t x) {
+  uint32_t p = ld_parent(parent, x);
+  while (true) {
+    const uint32_t gp = ld_parent(parent, p);
+    if (gp == p) return p;
+    parent[x] = gp;
+    x = gp;
+    p = ld_parent(parent, x);
+  }
+}
+
+// Afforest::union's rule (hook the higher root under the lower with a CAS) on roots found with path halving.
+// af_link walks parent chains without shortening them; edges linked all at once in id order (a path) build
+// chains as long as the chunk, which only path halving keeps cheap to walk and to compress
+__device__ __forceinline__ void link_halving(uint32_t* parent, uint32_t u, uint32_t v) {
+  uint32_t a = find_halving(parent, u), b = find_halving(parent, v);
+  while (a != b) {
+    const uint32_t high = a > b ? a : b;
+    const uint32_t low = a + b - high;
+    const uint32_t prev = atomicCAS(parent + high, high, low);
+    if (prev == high) return;
+    a = find_halving(parent, prev);  // high was hooked meanwhile
+    b = find_halving(parent, low);
+  }
+}
+
+// Links every edge of one chunk: tgt holds the targets of the edges [e0, e0 + len) of the CSR whose device
+// offsets are off (e0 a multiple of 4, 8 entries of slack behind len).  Edge-parallel: warp step t takes
+// the 128 edges from e0 + 128t, finds the row of the first one with a warp search over all offsets and an
+// upper bound for the last one with 32 galloping probes, and each lane then places its 4 edges by binary
+// search inside that window.  A hub row split over chunks and warps, or a run of empty rows, costs a
+// search of logarithmic depth, never a walk.  Targets >= n are counted in *bad and not linked.
+__global__ void __launch_bounds__(256) k_cc_link_edges(const uint32_t* __restrict__ off,
+                                                       const uint32_t* __restrict__ tgt, uint32_t e0, uint32_t len,
+                                                       uint32_t n, uint32_t* parent, unsigned int* bad) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
+  const uint32_t tiles = (len + LINK_TILE - 1) / LINK_TILE;
+  unsigned int nbad = 0;
+  for (uint32_t t = warp; t < tiles; t += nwarps) {
+    const uint32_t b = t * LINK_TILE;  // chunk-local
+    const uint32_t g0 = e0 + b, glast = g0 + min(LINK_TILE, len - b) - 1;
+    const uint32_t r0 = warp_row_search(off, 0, n, g0, lane);
+    // hi: the first of r0 + 1, r0 + 2, r0 + 4, ... whose row starts after the tile (off[n] = m > glast)
+    const uint64_t step = (uint64_t)r0 + (1ull << lane);
+    const uint32_t probe = step < n ? (uint32_t)step : n;
+    const unsigned past = __ballot_sync(0xFFFFFFFFu, off[probe] > glast);
+    const uint32_t hi = past ? __shfl_sync(0xFFFFFFFFu, probe, __ffs(past) - 1) : n;
+    const uint32_t l0 = b + 4 * lane;
+    if (l0 < len) {
+      const uint4 v4 = *reinterpret_cast<const uint4*>(tgt + l0);
+      const uint32_t v[4] = {v4.x, v4.y, v4.z, v4.w};
+      uint32_t r = row_search(off, r0, hi, e0 + l0);
+#pragma unroll
+      for (uint32_t j = 0; j < 4; ++j) {
+        if (l0 + j >= len) break;
+        const uint32_t e = e0 + l0 + j;
+        if (j && off[r + 1] <= e) r = row_search(off, r + 1, hi, e);
+        if (v[j] < n) link_halving(parent, r, v[j]);
+        else ++nbad;
+      }
+    }
+  }
+  nbad = __reduce_add_sync(0xFFFFFFFFu, nbad);
+  if (lane == 0 && nbad) atomicAdd(bad, nbad);
+}
+
 static gb_status wcc_impl(const gb_graph* g, const gb_wcc_config* cfg, uint32_t* d_comp, uint32_t* h_comp) {
   GB_REQUIRE(g && cfg, "NULL argument");
   if (g->kind != GB_KIND_DIRECTED)
@@ -197,6 +298,112 @@ static gb_status wcc_impl(const gb_graph* g, const gb_wcc_config* cfg, uint32_t*
   return GB_OK;
 }
 
+// The targets of gb_wcc_csr_u32 cross the bus in chunks of C edges through a ring of WCC_FEED_RING device
+// buffers; chunk k is the edges [kC, min((k + 1)C, m)), whatever rows it cuts.
+constexpr uint32_t WCC_FEED_RING = 3;
+constexpr uint64_t WCC_FEED_EDGES = 1u << 22;  // C: 16 MiB per buffer (DESIGN.md §5)
+
+static uint64_t env_u64(const char* name, uint64_t dflt) {
+  const char* s = std::getenv(name);
+  return s && *s ? std::strtoull(s, nullptr, 10) : dflt;
+}
+
+// the streams and events of one call; the streams are drained before they go
+struct WccFeed {
+  cudaStream_t copy = nullptr, link = nullptr;
+  cudaEvent_t offsets_in = nullptr;
+  cudaEvent_t landed[WCC_FEED_RING] = {}, freed[WCC_FEED_RING] = {};
+  gb_status create() {
+    GB_CUDA(cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking));
+    GB_CUDA(cudaStreamCreateWithFlags(&link, cudaStreamNonBlocking));
+    GB_CUDA(cudaEventCreateWithFlags(&offsets_in, cudaEventDisableTiming));
+    for (uint32_t i = 0; i < WCC_FEED_RING; ++i) {
+      GB_CUDA(cudaEventCreateWithFlags(&landed[i], cudaEventDisableTiming));
+      GB_CUDA(cudaEventCreateWithFlags(&freed[i], cudaEventDisableTiming));
+    }
+    return GB_OK;
+  }
+  ~WccFeed() {
+    if (copy) cudaStreamSynchronize(copy);
+    if (link) cudaStreamSynchronize(link);
+    for (uint32_t i = 0; i < WCC_FEED_RING; ++i) {
+      if (landed[i]) cudaEventDestroy(landed[i]);
+      if (freed[i]) cudaEventDestroy(freed[i]);
+    }
+    if (offsets_in) cudaEventDestroy(offsets_in);
+    if (copy) cudaStreamDestroy(copy);
+    if (link) cudaStreamDestroy(link);
+  }
+};
+
+// Union of every out-edge (wcc_baseline), linked chunk by chunk as the targets land: union-find does not
+// depend on the order of the links, and hooking the higher root under the lower keeps parent[x] <= x, so
+// after the final compress every label is the minimum node id of its component, as gb_wcc gives.  The
+// finds halve the paths they walk, so no compress is needed between chunks (DESIGN.md §5).
+static gb_status wcc_csr(int device, uint32_t n, const uint32_t* off, const uint32_t* tgt, uint32_t* comp) {
+  GB_TRY(require_device(device));
+  GB_REQUIRE(off[0] == 0, "offsets[0] must be 0");
+  const uint64_t m = off[n];
+  GB_REQUIRE(m == 0 || tgt != nullptr, "targets is NULL");
+  DeviceGuard guard(device);
+  // C: a multiple of 4 edges (chunk starts stay 16-byte aligned for the uint4 loads), no more than m needs
+  uint64_t C = std::min<uint64_t>(std::max<uint64_t>(env_u64("GB_WCC_FEED_EDGES", WCC_FEED_EDGES), 4), 1u << 28);
+  C = std::min<uint64_t>(C, (m + 3)) & ~3ull;
+  if (C == 0) C = 4;
+  const uint64_t K = (m + C - 1) / C;
+  const uint32_t R = (uint32_t)std::min<uint64_t>(WCC_FEED_RING, K);
+  WccFeed feed;  // outlives the buffers below, whose release waits for the device
+  GB_TRY(feed.create());
+  DevBuf<uint32_t> d_off, parent, ring[WCC_FEED_RING];
+  DevBuf<unsigned int> bad;  // [0] rows whose offsets decrease, [1] targets >= n
+  GB_TRY(d_off.alloc((size_t)n + 1));
+  GB_TRY(parent.alloc(n));
+  GB_TRY(bad.alloc(2));
+  for (uint32_t r = 0; r < R; ++r) {
+    GB_TRY(ring[r].alloc(C, 8));
+    GB_CUDA(cudaMemsetAsync(ring[r].p + C, 0, 8 * 4, feed.copy));
+  }
+  GB_CUDA(cudaMemcpyAsync(d_off.p, off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, feed.copy));
+  GB_CUDA(cudaEventRecord(feed.offsets_in, feed.copy));
+  // copy k waits until link k - R has read its buffer.  cudaStreamWaitEvent takes the event's latest record
+  // at the time of the call, so copy k and link k are enqueued in that order, chunk after chunk
+  auto enqueue_copy = [&](uint64_t k) -> gb_status {
+    const uint64_t e0 = k * C, len = std::min<uint64_t>(C, m - e0);
+    if (k >= R) GB_CUDA(cudaStreamWaitEvent(feed.copy, feed.freed[k % R], 0));
+    GB_CUDA(cudaMemcpyAsync(ring[k % R].p, tgt + e0, len * 4, cudaMemcpyHostToDevice, feed.copy));
+    GB_CUDA(cudaEventRecord(feed.landed[k % R], feed.copy));
+    return GB_OK;
+  };
+  for (uint32_t k = 0; k < R; ++k) GB_TRY(enqueue_copy(k));  // the bus stays busy during the check below
+  // offsets: monotone, checked before anything indexes with them
+  GB_CUDA(cudaStreamWaitEvent(feed.link, feed.offsets_in, 0));
+  GB_CUDA(cudaMemsetAsync(bad.p, 0, 8, feed.link));
+  check_monotone_async(feed.link, d_off.p, n, bad.p);
+  unsigned int nbad[2] = {0, 0};
+  GB_CUDA(cudaMemcpyAsync(nbad, bad.p, 4, cudaMemcpyDeviceToHost, feed.link));
+  GB_CUDA(cudaStreamSynchronize(feed.link));
+  GB_REQUIRE(nbad[0] == 0, "offsets are not monotone (%u rows)", nbad[0]);
+  const unsigned blk = 256;
+  const unsigned grid = grid_for(n, blk);
+  k_cc_init<<<grid, blk, 0, feed.link>>>(parent.p, n);
+  for (uint64_t k = 0; k < K; ++k) {
+    if (k >= R) GB_TRY(enqueue_copy(k));
+    const uint64_t e0 = k * C, len = std::min<uint64_t>(C, m - e0);
+    GB_CUDA(cudaStreamWaitEvent(feed.link, feed.landed[k % R], 0));
+    k_cc_link_edges<<<grid_for(len, LINK_TILE * (blk / 32)), blk, 0, feed.link>>>(
+        d_off.p, ring[k % R].p, (uint32_t)e0, (uint32_t)len, n, parent.p, bad.p + 1);
+    GB_CUDA(cudaEventRecord(feed.freed[k % R], feed.link));
+  }
+  k_cc_compress<<<grid, blk, 0, feed.link>>>(parent.p, n);
+  GB_CUDA(cudaGetLastError());
+  GB_CUDA(cudaMemcpyAsync(nbad + 1, bad.p + 1, 4, cudaMemcpyDeviceToHost, feed.link));
+  GB_CUDA(cudaStreamSynchronize(feed.link));
+  GB_REQUIRE(nbad[1] == 0, "CSR holds %u targets >= node_count %u", nbad[1], n);
+  GB_CUDA(cudaMemcpyAsync(comp, parent.p, (size_t)n * 4, cudaMemcpyDeviceToHost, feed.link));
+  GB_CUDA(cudaStreamSynchronize(feed.link));
+  return GB_OK;
+}
+
 }  // namespace gb
 
 extern "C" {
@@ -207,6 +414,14 @@ gb_status gb_wcc(const gb_graph* graph, const gb_wcc_config* config, uint32_t* c
 gb_status gb_wcc_device(const gb_graph* graph, const gb_wcc_config* config, uint32_t* d_components) {
   GB_REQUIRE(d_components != nullptr, "d_components is NULL");
   return gb::wcc_impl(graph, config, d_components, nullptr);
+}
+gb_status gb_wcc_csr_u32(int device, uint32_t node_count, const uint32_t* offsets, const uint32_t* targets,
+                         const gb_wcc_config* config, uint32_t* components) {
+  GB_REQUIRE(components != nullptr, "components is NULL");
+  GB_REQUIRE(config != nullptr, "config is NULL");  // chunk_size / neighbor_rounds / sampling_size: labels unchanged
+  GB_REQUIRE(node_count > 0, "node_count must be > 0");
+  GB_REQUIRE(offsets != nullptr, "offsets is NULL");
+  return gb::wcc_csr(device, node_count, offsets, targets, components);
 }
 
 // ---- multi-GPU WCC: the phases of wcc() (wcc.rs:158-183) over one rank's vertex range ----------------

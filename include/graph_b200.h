@@ -292,6 +292,19 @@ gb_status gb_digraph_for_page_rank_u32(int device, uint32_t node_count, const ui
 gb_status gb_wcc(const gb_graph* graph, const gb_wcc_config* config, uint32_t* components);
 gb_status gb_wcc_device(const gb_graph* graph, const gb_wcc_config* config, uint32_t* d_components);
 
+/* wcc_baseline(&graph, config) (wcc.rs:103-123) -- and, since the labels are the same, wcc_afforest(...).to_vec() --
+ * from a HOST CSR, with no resident twin.  Reads what wcc_baseline reads: node_count and the out-CSR (any CSR
+ * whose rows list the graph's edges gives the same labels; weak connectivity does not depend on the direction).
+ * The offsets go first; the targets are streamed in fixed-size edge chunks through a ring of device buffers and
+ * every chunk is linked (Afforest::union, afforest.rs:22-39) while the next one is on the bus.  Pass page-locked
+ * arrays to get the overlap; from pageable memory the copies are synchronous and the result is the same.
+ * components: node_count entries, caller-owned; not written when the call fails.  config is checked and otherwise
+ * ignored (the reference's chunk_size / neighbor_rounds / sampling_size change the work, never the labels).
+ * targets may be NULL when offsets[node_count] == 0.  GB_WCC_FEED_EDGES (environment, read per call) sets the
+ * chunk size in edges (rounded down to a multiple of 4; default 2^22). */
+gb_status gb_wcc_csr_u32(int device, uint32_t node_count, const uint32_t* offsets, const uint32_t* targets,
+                         const gb_wcc_config* config, uint32_t* components);
+
 /* Multi-GPU WCC (1-D cut by vertex range, one process per GPU; the caller owns the exchange of the
  * parent arrays, e.g. an NCCL all-gather).  The phases of wcc() (wcc.rs:158-183) restricted to the rank's
  * vertices [vertex_begin, vertex_end) over a FULL parent[n] on every rank:

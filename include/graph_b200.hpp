@@ -278,6 +278,16 @@ inline Components wcc_afforest(const DirectedCsrGraph& g, WccConfig c = {}) {
   detail::check(gb_wcc(g.handle(), &cfg, out.ids.data()));
   return out;
 }
+// wcc_baseline(&graph, config) of a host out-CSR (offsets: node_count + 1 entries, targets: offsets[node_count]),
+// streamed to the device without a resident twin (gb_wcc_csr_u32); the same labels as wcc_afforest
+inline Components wcc_baseline_csr(std::uint32_t node_count, const std::uint32_t* offsets,
+                                   const std::uint32_t* targets, WccConfig c = {}, int device = 0) {
+  gb_wcc_config cfg{c.chunk_size, c.neighbor_rounds, c.sampling_size};
+  Components out;
+  out.ids.resize(node_count);
+  detail::check(gb_wcc_csr_u32(device, node_count, offsets, targets, &cfg, out.ids.data()));
+  return out;
+}
 
 // delta_stepping(&graph, config) -> Vec<AtomicF32>             sssp.rs:38
 inline std::vector<float> delta_stepping(const DirectedCsrGraph& g, DeltaSteppingConfig c) {
