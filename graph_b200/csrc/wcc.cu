@@ -73,7 +73,40 @@ __global__ void k_cc_sample_labels(const uint32_t* __restrict__ parent, uint32_t
   }
 }
 
-// link_remaining, wcc.rs:274-301: one warp per vertex outside the sampled giant component
+// the root of x; every non-root on the way is pointed at its grandparent (path halving).  The writes race
+// only with writes of other ancestors, and a CAS only ever changes a root, so parent[y] <= y and every tree
+// stay as they were
+__device__ __forceinline__ uint32_t find_halving(uint32_t* parent, uint32_t x) {
+  uint32_t p = ld_parent(parent, x);
+  while (true) {
+    const uint32_t gp = ld_parent(parent, p);
+    if (gp == p) return p;
+    parent[x] = gp;
+    x = gp;
+    p = ld_parent(parent, x);
+  }
+}
+
+// Afforest::union's rule (hook the higher root under the lower with a CAS) on roots found with path halving.
+// af_link walks parent chains without shortening them; edges linked all at once in id order (a path) build
+// chains as long as the chunk, which only path halving keeps cheap to walk and to compress.  k_cc_link_remaining
+// links with it too: its lanes hook the vertices of an unsampled path into a chain as deep as the path while
+// the warp of a hub on that path walks the chain once per entry of its lists
+__device__ __forceinline__ void link_halving(uint32_t* parent, uint32_t u, uint32_t v) {
+  uint32_t a = find_halving(parent, u), b = find_halving(parent, v);
+  while (a != b) {
+    const uint32_t high = a > b ? a : b;
+    const uint32_t low = a + b - high;
+    const uint32_t prev = atomicCAS(parent + high, high, low);
+    if (prev == high) return;
+    a = find_halving(parent, prev);  // high was hooked meanwhile
+    b = find_halving(parent, low);
+  }
+}
+
+// link_remaining, wcc.rs:274-301: one warp per vertex outside the sampled giant component.  A vertex is
+// skipped only while parent[v] == skip, so it is already joined to the giant; once skip is hooked under a
+// lower root a halving find may point a giant vertex past it, and that vertex then links its lists again
 __global__ void k_cc_link_remaining(const uint32_t* __restrict__ out_off, const uint32_t* __restrict__ out_tgt,
                                     const uint32_t* __restrict__ in_off, const uint32_t* __restrict__ in_tgt,
                                     uint32_t vb, uint32_t n, uint32_t rounds, uint32_t skip, int use_skip,
@@ -101,8 +134,8 @@ __global__ void k_cc_link_remaining(const uint32_t* __restrict__ out_off, const 
     const uint32_t work = (oe - ob) + (ie - ib);
     const bool small = live && work <= 8;
     if (small) {
-      for (uint32_t i = ob; i < oe; ++i) af_link(parent, mine, out_tgt[i]);
-      for (uint32_t i = ib; i < ie; ++i) af_link(parent, mine, in_tgt[i]);
+      for (uint32_t i = ob; i < oe; ++i) link_halving(parent, mine, out_tgt[i]);
+      for (uint32_t i = ib; i < ie; ++i) link_halving(parent, mine, in_tgt[i]);
     }
     unsigned mask = __ballot_sync(0xFFFFFFFFu, live && !small);
     while (mask) {
@@ -111,8 +144,8 @@ __global__ void k_cc_link_remaining(const uint32_t* __restrict__ out_off, const 
       const uint32_t u = base + owner;
       const uint32_t b0 = __shfl_sync(0xFFFFFFFFu, ob, owner), e0 = __shfl_sync(0xFFFFFFFFu, oe, owner);
       const uint32_t b1 = __shfl_sync(0xFFFFFFFFu, ib, owner), e1 = __shfl_sync(0xFFFFFFFFu, ie, owner);
-      for (uint32_t i = b0 + lane; i < e0; i += 32) af_link(parent, u, out_tgt[i]);
-      for (uint32_t i = b1 + lane; i < e1; i += 32) af_link(parent, u, in_tgt[i]);
+      for (uint32_t i = b0 + lane; i < e0; i += 32) link_halving(parent, u, out_tgt[i]);
+      for (uint32_t i = b1 + lane; i < e1; i += 32) link_halving(parent, u, in_tgt[i]);
     }
   }
 }
@@ -180,35 +213,6 @@ __device__ __forceinline__ uint32_t warp_row_search(const uint32_t* __restrict__
     if (c < 31) hi = above;
   }
   return lo;
-}
-
-// the root of x; every non-root on the way is pointed at its grandparent (path halving).  The writes race
-// only with writes of other ancestors, and a CAS only ever changes a root, so parent[y] <= y and every tree
-// stay as they were
-__device__ __forceinline__ uint32_t find_halving(uint32_t* parent, uint32_t x) {
-  uint32_t p = ld_parent(parent, x);
-  while (true) {
-    const uint32_t gp = ld_parent(parent, p);
-    if (gp == p) return p;
-    parent[x] = gp;
-    x = gp;
-    p = ld_parent(parent, x);
-  }
-}
-
-// Afforest::union's rule (hook the higher root under the lower with a CAS) on roots found with path halving.
-// af_link walks parent chains without shortening them; edges linked all at once in id order (a path) build
-// chains as long as the chunk, which only path halving keeps cheap to walk and to compress
-__device__ __forceinline__ void link_halving(uint32_t* parent, uint32_t u, uint32_t v) {
-  uint32_t a = find_halving(parent, u), b = find_halving(parent, v);
-  while (a != b) {
-    const uint32_t high = a > b ? a : b;
-    const uint32_t low = a + b - high;
-    const uint32_t prev = atomicCAS(parent + high, high, low);
-    if (prev == high) return;
-    a = find_halving(parent, prev);  // high was hooked meanwhile
-    b = find_halving(parent, low);
-  }
 }
 
 // Links every edge of one chunk: tgt holds the targets of the edges [e0, e0 + len) of the CSR whose device

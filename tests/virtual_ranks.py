@@ -72,11 +72,14 @@ class VirtualRanks:
         return self.ranks[0].finish(full).cpu().numpy()
 
 
-def wcc_virtual_ranks(g, world: int, **cfg):
+def wcc_virtual_ranks(g, world: int, ranges=None, forests=None, **cfg):
     """The phases of ShardedWcc.run on `world` virtual ranks: every rank runs them on its vertex range over
-    its own full parent array, and the all-gather is a list of snapshots.  Returns (parents, labels)."""
+    its own full parent array, and the all-gather is a list of snapshots.  `ranges`: the ranks' vertex
+    ranges (default vertex_ranges, 32-aligned).  `forests`: a list that receives, per rank, host copies of
+    the parent array after the rank's own SAMPLE + COMPRESS and after the first merge.  Returns (parents,
+    labels)."""
     b = CudaWccBackend(g, **cfg)
-    ranges = vertex_ranges(g.node_count(), world)
+    ranges = vertex_ranges(g.node_count(), world) if ranges is None else ranges
     parents = [b.new_parent() for _ in range(world)]
 
     def merge_all():
@@ -87,11 +90,17 @@ def wcc_virtual_ranks(g, world: int, **cfg):
                     b.phase(_capi.WCC_MERGE, p, other=snap[q])
             b.phase(_capi.WCC_COMPRESS, p)
 
+    def host():
+        return [p.cpu().numpy().view(np.uint32) for p in parents]
+
     for r, p in enumerate(parents):
         b.phase(_capi.WCC_INIT, p)
         b.phase(_capi.WCC_SAMPLE, p, *ranges[r])
         b.phase(_capi.WCC_COMPRESS, p)
+    own = host() if forests is not None else None
     merge_all()
+    if forests is not None:
+        forests.extend(zip(own, host()))
     labels = [b.sample_label(p) for p in parents]
     for r, p in enumerate(parents):
         b.phase(_capi.WCC_LINK_REMAINING, p, *ranges[r], labels[r][0], labels[r][1])
