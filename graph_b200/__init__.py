@@ -78,6 +78,17 @@ class Comm:
         _, micros = _timed(go)
         return PageRankResult(scores, int(it.value), float(err.value), micros)
 
+    def wcc_csr(self, offsets, targets, *, chunk_size: int | None = None, neighbor_rounds: int | None = None,
+                sampling_size: int | None = None, out=None):
+        """graph_b200.wcc_csr over the communicator's devices (gb_wcc_csr_multi_u32): each device streams and
+        links about 1/ndev of the edges over its own bus, the forests merge over NVLink, and the labels are
+        the same.  Same checks and `out` as wcc_csr; a config value left at None is WccConfig's default."""
+        d = WccConfig()
+        return _wcc_csr_call(lib.gb_wcc_csr_multi_u32, self._c, offsets, targets,
+                             d.chunk_size if chunk_size is None else chunk_size,
+                             d.neighbor_rounds if neighbor_rounds is None else neighbor_rounds,
+                             d.sampling_size if sampling_size is None else sampling_size, out)
+
 
 # ---- enums (crates/mate/src/graphs/mod.rs Layout / FileFormat; csr.rs:35-45) --------------------
 class _Enum:
@@ -697,23 +708,37 @@ class Graph(_Handle):
         return TriangleCountResult(int(tri.value), micros)
 
 
-def wcc_csr(offsets, targets, *, chunk_size: int = WccConfig.DEFAULT_CHUNK_SIZE,
-            neighbor_rounds: int = WccConfig.DEFAULT_NEIGHBOR_ROUNDS,
-            sampling_size: int = WccConfig.DEFAULT_SAMPLING_SIZE) -> WccResult:
-    """wcc_baseline (wcc.rs:103-123) of a host out-CSR without a resident twin: the offsets are uploaded, the
-    targets streamed through a ring of device buffers and linked as they land.  Same labels as
-    DiGraph.wcc() on the twin (the minimum node id of each component); the config is checked and otherwise
-    ignored.  Arrays are used as given: pass pinned contiguous uint32 arrays to overlap the links with the copy."""
+def _wcc_csr_call(fn, first, offsets, targets, chunk_size, neighbor_rounds, sampling_size, out) -> WccResult:
+    """fn(first, node_count, offsets, targets, &config, components): gb_wcc_csr_u32 or gb_wcc_csr_multi_u32."""
     off, tgt = np.asarray(offsets), np.asarray(targets)
     for a in (off, tgt):
         if a.dtype != np.uint32 or not a.flags.c_contiguous:
             raise TypeError("wcc_csr needs contiguous uint32 arrays")
     _check_host_csr(off, tgt, "out")
     cfg = _capi.WccConfig(int(chunk_size), int(neighbor_rounds), int(sampling_size))
-    comp = np.empty(len(off) - 1, np.uint32)
+    if out is None:
+        comp = np.empty(len(off) - 1, np.uint32)
+    else:
+        comp = out
+        if not isinstance(comp, np.ndarray) or comp.dtype != np.uint32 or not comp.flags.c_contiguous:
+            raise TypeError("out must be a contiguous uint32 numpy array")
+        if comp.shape != (len(off) - 1,) or not comp.flags.writeable:
+            raise ValueError(f"out must be a writeable array of node_count = {len(off) - 1} entries")
 
     def go():
-        check(lib.gb_wcc_csr_u32(_device, len(off) - 1, _ptr(off), _ptr(tgt) if len(tgt) else None, C.byref(cfg),
-                                 _ptr(comp)))
+        check(fn(first, len(off) - 1, _ptr(off), _ptr(tgt) if len(tgt) else None, C.byref(cfg), _ptr(comp)))
     _, micros = _timed(go)
-    return WccResult(comp, micros)
+    return WccResult(comp if out is None else comp.view(), micros)  # a view: `out` itself stays writeable
+
+
+def wcc_csr(offsets, targets, *, chunk_size: int = WccConfig.DEFAULT_CHUNK_SIZE,
+            neighbor_rounds: int = WccConfig.DEFAULT_NEIGHBOR_ROUNDS,
+            sampling_size: int = WccConfig.DEFAULT_SAMPLING_SIZE, out=None) -> WccResult:
+    """wcc_baseline (wcc.rs:103-123) of a host out-CSR without a resident twin: the offsets are uploaded, the
+    targets streamed through a ring of device buffers and linked as they land.  Same labels as
+    DiGraph.wcc() on the twin (the minimum node id of each component); the config is checked and otherwise
+    ignored.  Arrays are used as given: pass pinned contiguous uint32 arrays to overlap the links with the copy.
+    `out`, a contiguous uint32 array of node_count entries (e.g. a pinned torch buffer viewed as numpy), receives
+    the labels instead of a new array; it is left untouched when the call fails."""
+    return _wcc_csr_call(lib.gb_wcc_csr_u32, _device, offsets, targets, chunk_size, neighbor_rounds,
+                         sampling_size, out)

@@ -232,6 +232,9 @@ gb_status graph_from_device_arrays(int device, gb_graph_kind kind, const uint32_
 // graph's stream; the caller holds g->mu.
 gb_status in_csr_values(const gb_graph* g, DevBuf<float>* in_w);
 
+// the devices of a communicator, in its order (multi.cu); peer access among them is enabled
+const std::vector<int>& comm_devices(const gb_comm* c);
+
 constexpr unsigned H100_SMS = 132;  // streaming multiprocessors of an H100 SXM: sizes the grid-stride grids
 
 inline unsigned grid_for(uint64_t items, unsigned block, unsigned max_blocks = H100_SMS * 16u) {

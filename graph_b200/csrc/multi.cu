@@ -244,6 +244,8 @@ static gb_status comm_prepare(gb_comm* c, uint32_t n) {
   return GB_OK;
 }
 
+const std::vector<int>& comm_devices(const gb_comm* c) { return c->devs; }
+
 }  // namespace gb
 
 extern "C" {

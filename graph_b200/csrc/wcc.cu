@@ -10,9 +10,11 @@
 // phase lets most vertices skip their edge lists, so effective GB/s can exceed the HBM peak.
 #include <algorithm>
 #include <cstdlib>
+#include <memory>
 #include <vector>
 
 #include "common.cuh"
+#include "wcc_split.h"
 
 namespace gb {
 
@@ -215,15 +217,17 @@ __device__ __forceinline__ uint32_t warp_row_search(const uint32_t* __restrict__
   return lo;
 }
 
-// Links every edge of one chunk: tgt holds the targets of the edges [e0, e0 + len) of the CSR whose device
-// offsets are off (e0 a multiple of 4, 8 entries of slack behind len).  Edge-parallel: warp step t takes
-// the 128 edges from e0 + 128t, finds the row of the first one with a warp search over all offsets and an
-// upper bound for the last one with 32 galloping probes, and each lane then places its 4 edges by binary
-// search inside that window.  A hub row split over chunks and warps, or a run of empty rows, costs a
-// search of logarithmic depth, never a walk.  Targets >= n are counted in *bad and not linked.
-__global__ void __launch_bounds__(256) k_cc_link_edges(const uint32_t* __restrict__ off,
-                                                       const uint32_t* __restrict__ tgt, uint32_t e0, uint32_t len,
-                                                       uint32_t n, uint32_t* parent, unsigned int* bad) {
+// Links every edge of one chunk: tgt holds the targets of the edges [e0, e0 + len) of the CSR (e0 a multiple
+// of 4, 8 entries of slack behind len), and off the device offsets of its rows [row_base, row_base + rows]
+// (the whole CSR: row_base 0, rows n), with off[0] <= e0 and e0 + len <= off[rows].  Edge-parallel: warp
+// step t takes the 128 edges from e0 + 128t, finds the row of the first one with a warp search over all
+// those offsets and an upper bound for the last one with 32 galloping probes, and each lane then places its
+// 4 edges by binary search inside that window.  A hub row split over chunks and warps, or a run of empty
+// rows, costs a search of logarithmic depth, never a walk.  Targets >= n are counted in *bad and not linked.
+__global__ void __launch_bounds__(256) k_cc_link_edges(const uint32_t* __restrict__ off, uint32_t rows,
+                                                       uint32_t row_base, const uint32_t* __restrict__ tgt,
+                                                       uint32_t e0, uint32_t len, uint32_t n, uint32_t* parent,
+                                                       unsigned int* bad) {
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
@@ -232,12 +236,12 @@ __global__ void __launch_bounds__(256) k_cc_link_edges(const uint32_t* __restric
   for (uint32_t t = warp; t < tiles; t += nwarps) {
     const uint32_t b = t * LINK_TILE;  // chunk-local
     const uint32_t g0 = e0 + b, glast = g0 + min(LINK_TILE, len - b) - 1;
-    const uint32_t r0 = warp_row_search(off, 0, n, g0, lane);
-    // hi: the first of r0 + 1, r0 + 2, r0 + 4, ... whose row starts after the tile (off[n] = m > glast)
+    const uint32_t r0 = warp_row_search(off, 0, rows, g0, lane);
+    // hi: the first of r0 + 1, r0 + 2, r0 + 4, ... whose row starts after the tile (off[rows] > glast)
     const uint64_t step = (uint64_t)r0 + (1ull << lane);
-    const uint32_t probe = step < n ? (uint32_t)step : n;
+    const uint32_t probe = step < rows ? (uint32_t)step : rows;
     const unsigned past = __ballot_sync(0xFFFFFFFFu, off[probe] > glast);
-    const uint32_t hi = past ? __shfl_sync(0xFFFFFFFFu, probe, __ffs(past) - 1) : n;
+    const uint32_t hi = past ? __shfl_sync(0xFFFFFFFFu, probe, __ffs(past) - 1) : rows;
     const uint32_t l0 = b + 4 * lane;
     if (l0 < len) {
       const uint4 v4 = *reinterpret_cast<const uint4*>(tgt + l0);
@@ -248,13 +252,23 @@ __global__ void __launch_bounds__(256) k_cc_link_edges(const uint32_t* __restric
         if (l0 + j >= len) break;
         const uint32_t e = e0 + l0 + j;
         if (j && off[r + 1] <= e) r = row_search(off, r + 1, hi, e);
-        if (v[j] < n) link_halving(parent, r, v[j]);
+        if (v[j] < n) link_halving(parent, row_base + r, v[j]);
         else ++nbad;
       }
     }
   }
   nbad = __reduce_add_sync(0xFFFFFFFFu, nbad);
   if (lane == 0 && nbad) atomicAdd(bad, nbad);
+}
+
+// union of another part's forest into this one (gb_wcc_csr_multi_u32): other is that part's compressed
+// parent[], a peer device's memory or this device's, read once and coalesced.  The links halve paths as the
+// edge links do, for the same reason: a forest can hold chains as long as the graph's paths
+__global__ void k_cc_merge_halving(uint32_t* parent, const uint32_t* __restrict__ other, uint32_t n) {
+  for (uint32_t v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += gridDim.x * blockDim.x) {
+    const uint32_t o = other[v];
+    if (o != v) link_halving(parent, v, o);
+  }
 }
 
 static gb_status wcc_impl(const gb_graph* g, const gb_wcc_config* cfg, uint32_t* d_comp, uint32_t* h_comp) {
@@ -306,17 +320,19 @@ static gb_status wcc_impl(const gb_graph* g, const gb_wcc_config* cfg, uint32_t*
 // buffers; chunk k is the edges [kC, min((k + 1)C, m)), whatever rows it cuts.
 constexpr uint32_t WCC_FEED_RING = 3;
 constexpr uint64_t WCC_FEED_EDGES = 1u << 22;  // C: 16 MiB per buffer (DESIGN.md §5)
+constexpr uint32_t WCC_MULTI_MAX_PARTS = 64;   // GB_WCC_MULTI_PARTS is clamped to [1, 64] parts per device
 
 static uint64_t env_u64(const char* name, uint64_t dflt) {
   const char* s = std::getenv(name);
   return s && *s ? std::strtoull(s, nullptr, 10) : dflt;
 }
 
-// the streams and events of one call; the streams are drained before they go
+// the streams and events of one part; the streams are drained before they go
 struct WccFeed {
   cudaStream_t copy = nullptr, link = nullptr;
   cudaEvent_t offsets_in = nullptr;
   cudaEvent_t landed[WCC_FEED_RING] = {}, freed[WCC_FEED_RING] = {};
+  cudaEvent_t forest = nullptr;  // recorded behind the part's finished forest, for the part that merges it
   gb_status create() {
     GB_CUDA(cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking));
     GB_CUDA(cudaStreamCreateWithFlags(&link, cudaStreamNonBlocking));
@@ -325,86 +341,196 @@ struct WccFeed {
       GB_CUDA(cudaEventCreateWithFlags(&landed[i], cudaEventDisableTiming));
       GB_CUDA(cudaEventCreateWithFlags(&freed[i], cudaEventDisableTiming));
     }
+    GB_CUDA(cudaEventCreateWithFlags(&forest, cudaEventDisableTiming));
     return GB_OK;
   }
-  ~WccFeed() {
+  void drain() const {
     if (copy) cudaStreamSynchronize(copy);
     if (link) cudaStreamSynchronize(link);
+  }
+  ~WccFeed() {
+    drain();
     for (uint32_t i = 0; i < WCC_FEED_RING; ++i) {
       if (landed[i]) cudaEventDestroy(landed[i]);
       if (freed[i]) cudaEventDestroy(freed[i]);
     }
     if (offsets_in) cudaEventDestroy(offsets_in);
+    if (forest) cudaEventDestroy(forest);
     if (copy) cudaStreamDestroy(copy);
     if (link) cudaStreamDestroy(link);
   }
 };
 
+// One part of a one-shot WCC (wcc_split.h): the edges [e_begin, e_end) stream through the part's ring in
+// chunks of C edges (chunk k is [e_begin + kC, min(e_begin + (k + 1)C, e_end)), whatever rows it cuts) and
+// are linked into the part's own parent[n] on device dev.
+//
+// When there are several parts, another part may read this parent[] from another device.  cudaMalloc memory
+// is mapped into the peers by cudaDeviceEnablePeerAccess (gb_comm_init); blocks of the stream-ordered pool
+// that DevBuf draws from are not (a pool is reachable from its own device only unless cudaMemPoolSetAccess
+// says otherwise).  So the forest of one part among several is cudaMalloc'd, on one device as on many, and a
+// lone part (gb_wcc_csr_u32) keeps the pool's cached block.
+struct WccPart {
+  int dev = -1;
+  WccPartRange range{};
+  uint64_t C = 4, K = 0;  // chunk size in edges, chunks
+  uint32_t R = 0;         // ring buffers in use
+  unsigned int nbad[2] = {0, 0};
+  uint32_t* parent = nullptr;  // pooled.p or shared
+  uint32_t* shared = nullptr;  // cudaMalloc'd parent[] of one part among several
+  WccFeed feed;  // outlives the buffers below, whose release waits for the device
+  DevBuf<uint32_t> off, pooled, ring[WCC_FEED_RING];
+  DevBuf<unsigned int> bad;  // [0] rows whose offsets decrease, [1] targets >= n
+  gb_status alloc_parent(uint32_t n, bool peers_read) {
+    if (!peers_read) {
+      GB_TRY(pooled.alloc(n));
+      parent = pooled.p;
+      return GB_OK;
+    }
+    GB_CUDA(cudaMalloc(reinterpret_cast<void**>(&shared), (size_t)n * sizeof(uint32_t)));
+    parent = shared;
+    return GB_OK;
+  }
+  ~WccPart() {
+    if (dev >= 0) cudaSetDevice(dev);  // the members are released on the part's device
+    if (shared) cudaFree(shared);
+  }
+};
+
+// Every part's streams drain before any part's buffers go: a merge reads its partner's parent[].
+struct WccParts {
+  std::vector<std::unique_ptr<WccPart>> v;
+  ~WccParts() {
+    for (auto& q : v) q->feed.drain();
+  }
+};
+
+// copy k of a part waits until its link k - R has read the buffer.  cudaStreamWaitEvent takes the event's
+// latest record at the time of the call, so copy k and link k are enqueued in that order, chunk after chunk
+static gb_status wcc_enqueue_copy(WccPart& q, const uint32_t* tgt, uint64_t k) {
+  const uint64_t e0 = q.range.e_begin + k * q.C, len = std::min<uint64_t>(q.C, q.range.e_end - e0);
+  if (k >= q.R) GB_CUDA(cudaStreamWaitEvent(q.feed.copy, q.feed.freed[k % q.R], 0));
+  GB_CUDA(cudaMemcpyAsync(q.ring[k % q.R].p, tgt + e0, len * 4, cudaMemcpyHostToDevice, q.feed.copy));
+  GB_CUDA(cudaEventRecord(q.feed.landed[k % q.R], q.feed.copy));
+  return GB_OK;
+}
+
 // Union of every out-edge (wcc_baseline), linked chunk by chunk as the targets land: union-find does not
 // depend on the order of the links, and hooking the higher root under the lower keeps parent[x] <= x, so
 // after the final compress every label is the minimum node id of its component, as gb_wcc gives.  The
 // finds halve the paths they walk, so no compress is needed between chunks (DESIGN.md §5).
-static gb_status wcc_csr(int device, uint32_t n, const uint32_t* off, const uint32_t* tgt, uint32_t* comp) {
-  GB_TRY(require_device(device));
+// The edges are cut into devs.size() * per_dev parts (wcc_split.h), part p on devs[p / per_dev], each with
+// its own streams, ring and forest.  One part is gb_wcc_csr_u32.  With more, the forests merge in
+// ceil(log2 P) tree rounds: in round s = 1, 2, 4, ... part p (p mod 2s == 0) links the forest of part p + s
+// into its own through a peer pointer and compresses, and part 0 ends with the union of all edges.
+static gb_status wcc_csr_parts(const std::vector<int>& devs, uint32_t per_dev, uint32_t n, const uint32_t* off,
+                               const uint32_t* tgt, uint32_t* comp) {
   GB_REQUIRE(off[0] == 0, "offsets[0] must be 0");
   const uint64_t m = off[n];
   GB_REQUIRE(m == 0 || tgt != nullptr, "targets is NULL");
-  DeviceGuard guard(device);
-  // C: a multiple of 4 edges (chunk starts stay 16-byte aligned for the uint4 loads), no more than m needs
-  uint64_t C = std::min<uint64_t>(std::max<uint64_t>(env_u64("GB_WCC_FEED_EDGES", WCC_FEED_EDGES), 4), 1u << 28);
-  C = std::min<uint64_t>(C, (m + 3)) & ~3ull;
-  if (C == 0) C = 4;
-  const uint64_t K = (m + C - 1) / C;
-  const uint32_t R = (uint32_t)std::min<uint64_t>(WCC_FEED_RING, K);
-  WccFeed feed;  // outlives the buffers below, whose release waits for the device
-  GB_TRY(feed.create());
-  DevBuf<uint32_t> d_off, parent, ring[WCC_FEED_RING];
-  DevBuf<unsigned int> bad;  // [0] rows whose offsets decrease, [1] targets >= n
-  GB_TRY(d_off.alloc((size_t)n + 1));
-  GB_TRY(parent.alloc(n));
-  GB_TRY(bad.alloc(2));
-  for (uint32_t r = 0; r < R; ++r) {
-    GB_TRY(ring[r].alloc(C, 8));
-    GB_CUDA(cudaMemsetAsync(ring[r].p + C, 0, 8 * 4, feed.copy));
+  const uint32_t P = (uint32_t)devs.size() * per_dev;
+  const std::vector<WccPartRange> split = wcc_split(off, n, P);
+  DeviceGuard guard(devs[0]);
+  // C: a multiple of 4 edges (chunk starts stay 16-byte aligned for the uint4 loads), no more than a part needs
+  const uint64_t C = std::min<uint64_t>(std::max<uint64_t>(env_u64("GB_WCC_FEED_EDGES", WCC_FEED_EDGES), 4), 1u << 28);
+  WccParts parts;
+  // every part's offsets and first copies are enqueued before the host waits for any check: all buses stay busy
+  for (uint32_t p = 0; p < P; ++p) {
+    parts.v.emplace_back(new (std::nothrow) WccPart());
+    GB_REQUIRE(parts.v.back() != nullptr, "host allocation failed");
+    WccPart& q = *parts.v.back();
+    q.dev = devs[p / per_dev];
+    q.range = split[p];
+    GB_CUDA(cudaSetDevice(q.dev));
+    const uint64_t len = q.range.e_end - q.range.e_begin;
+    q.C = std::min<uint64_t>(C, (len + 3)) & ~3ull;
+    if (q.C == 0) q.C = 4;
+    q.K = (len + q.C - 1) / q.C;
+    q.R = (uint32_t)std::min<uint64_t>(WCC_FEED_RING, q.K);
+    GB_TRY(q.feed.create());
+    const uint32_t rows = q.range.r_end - q.range.r_begin;
+    GB_TRY(q.off.alloc((size_t)rows + 1));
+    GB_TRY(q.alloc_parent(n, P > 1));
+    GB_TRY(q.bad.alloc(2));
+    for (uint32_t r = 0; r < q.R; ++r) {
+      GB_TRY(q.ring[r].alloc(q.C, 8));
+      GB_CUDA(cudaMemsetAsync(q.ring[r].p + q.C, 0, 8 * 4, q.feed.copy));
+    }
+    GB_CUDA(cudaMemcpyAsync(q.off.p, off + q.range.r_begin, ((size_t)rows + 1) * 4, cudaMemcpyHostToDevice,
+                            q.feed.copy));
+    GB_CUDA(cudaEventRecord(q.feed.offsets_in, q.feed.copy));
+    for (uint32_t k = 0; k < q.R; ++k) GB_TRY(wcc_enqueue_copy(q, tgt, k));
   }
-  GB_CUDA(cudaMemcpyAsync(d_off.p, off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, feed.copy));
-  GB_CUDA(cudaEventRecord(feed.offsets_in, feed.copy));
-  // copy k waits until link k - R has read its buffer.  cudaStreamWaitEvent takes the event's latest record
-  // at the time of the call, so copy k and link k are enqueued in that order, chunk after chunk
-  auto enqueue_copy = [&](uint64_t k) -> gb_status {
-    const uint64_t e0 = k * C, len = std::min<uint64_t>(C, m - e0);
-    if (k >= R) GB_CUDA(cudaStreamWaitEvent(feed.copy, feed.freed[k % R], 0));
-    GB_CUDA(cudaMemcpyAsync(ring[k % R].p, tgt + e0, len * 4, cudaMemcpyHostToDevice, feed.copy));
-    GB_CUDA(cudaEventRecord(feed.landed[k % R], feed.copy));
-    return GB_OK;
-  };
-  for (uint32_t k = 0; k < R; ++k) GB_TRY(enqueue_copy(k));  // the bus stays busy during the check below
-  // offsets: monotone, checked before anything indexes with them
-  GB_CUDA(cudaStreamWaitEvent(feed.link, feed.offsets_in, 0));
-  GB_CUDA(cudaMemsetAsync(bad.p, 0, 8, feed.link));
-  check_monotone_async(feed.link, d_off.p, n, bad.p);
-  unsigned int nbad[2] = {0, 0};
-  GB_CUDA(cudaMemcpyAsync(nbad, bad.p, 4, cudaMemcpyDeviceToHost, feed.link));
-  GB_CUDA(cudaStreamSynchronize(feed.link));
-  GB_REQUIRE(nbad[0] == 0, "offsets are not monotone (%u rows)", nbad[0]);
+  // offsets: monotone, checked before anything indexes with them.  The slices tile [0, n], so the rows each
+  // part checks cover every row once, whatever the host array holds
+  for (auto& qp : parts.v) {
+    WccPart& q = *qp;
+    GB_CUDA(cudaSetDevice(q.dev));
+    GB_CUDA(cudaStreamWaitEvent(q.feed.link, q.feed.offsets_in, 0));
+    GB_CUDA(cudaMemsetAsync(q.bad.p, 0, 8, q.feed.link));
+    check_monotone_async(q.feed.link, q.off.p + (q.range.check_begin - q.range.r_begin),
+                         q.range.r_end - q.range.check_begin, q.bad.p);
+    GB_CUDA(cudaMemcpyAsync(q.nbad, q.bad.p, 4, cudaMemcpyDeviceToHost, q.feed.link));
+  }
+  unsigned int nbad = 0;
+  for (auto& q : parts.v) {
+    GB_CUDA(cudaStreamSynchronize(q->feed.link));
+    nbad += q->nbad[0];
+  }
+  GB_REQUIRE(nbad == 0, "offsets are not monotone (%u rows)", nbad);
   const unsigned blk = 256;
   const unsigned grid = grid_for(n, blk);
-  k_cc_init<<<grid, blk, 0, feed.link>>>(parent.p, n);
-  for (uint64_t k = 0; k < K; ++k) {
-    if (k >= R) GB_TRY(enqueue_copy(k));
-    const uint64_t e0 = k * C, len = std::min<uint64_t>(C, m - e0);
-    GB_CUDA(cudaStreamWaitEvent(feed.link, feed.landed[k % R], 0));
-    k_cc_link_edges<<<grid_for(len, LINK_TILE * (blk / 32)), blk, 0, feed.link>>>(
-        d_off.p, ring[k % R].p, (uint32_t)e0, (uint32_t)len, n, parent.p, bad.p + 1);
-    GB_CUDA(cudaEventRecord(feed.freed[k % R], feed.link));
+  uint64_t chunks = 0;
+  for (auto& q : parts.v) {
+    GB_CUDA(cudaSetDevice(q->dev));
+    k_cc_init<<<grid, blk, 0, q->feed.link>>>(q->parent, n);
+    chunks = std::max(chunks, q->K);
   }
-  k_cc_compress<<<grid, blk, 0, feed.link>>>(parent.p, n);
+  for (uint64_t k = 0; k < chunks; ++k) {
+    for (auto& qp : parts.v) {
+      WccPart& q = *qp;
+      if (k >= q.K) continue;
+      GB_CUDA(cudaSetDevice(q.dev));
+      if (k >= q.R) GB_TRY(wcc_enqueue_copy(q, tgt, k));
+      const uint64_t e0 = q.range.e_begin + k * q.C, len = std::min<uint64_t>(q.C, q.range.e_end - e0);
+      GB_CUDA(cudaStreamWaitEvent(q.feed.link, q.feed.landed[k % q.R], 0));
+      k_cc_link_edges<<<grid_for(len, LINK_TILE * (blk / 32)), blk, 0, q.feed.link>>>(
+          q.off.p, q.range.r_end - q.range.r_begin, q.range.r_begin, q.ring[k % q.R].p, (uint32_t)e0,
+          (uint32_t)len, n, q.parent, q.bad.p + 1);
+      GB_CUDA(cudaEventRecord(q.feed.freed[k % q.R], q.feed.link));
+    }
+  }
+  for (auto& q : parts.v) {
+    GB_CUDA(cudaSetDevice(q->dev));
+    k_cc_compress<<<grid, blk, 0, q->feed.link>>>(q->parent, n);
+  }
+  // a partner p + s never merges again after round s, so its forest is final when its event is recorded
+  for (uint32_t s = 1; s < P; s *= 2) {
+    for (uint32_t p = 0; p + s < P; p += 2 * s) {
+      WccPart &a = *parts.v[p], &b = *parts.v[p + s];
+      GB_CUDA(cudaSetDevice(b.dev));
+      GB_CUDA(cudaEventRecord(b.feed.forest, b.feed.link));
+      GB_CUDA(cudaSetDevice(a.dev));
+      GB_CUDA(cudaStreamWaitEvent(a.feed.link, b.feed.forest, 0));
+      k_cc_merge_halving<<<grid, blk, 0, a.feed.link>>>(a.parent, b.parent, n);
+      k_cc_compress<<<grid, blk, 0, a.feed.link>>>(a.parent, n);
+    }
+  }
   GB_CUDA(cudaGetLastError());
-  GB_CUDA(cudaMemcpyAsync(nbad + 1, bad.p + 1, 4, cudaMemcpyDeviceToHost, feed.link));
-  GB_CUDA(cudaStreamSynchronize(feed.link));
-  GB_REQUIRE(nbad[1] == 0, "CSR holds %u targets >= node_count %u", nbad[1], n);
-  GB_CUDA(cudaMemcpyAsync(comp, parent.p, (size_t)n * 4, cudaMemcpyDeviceToHost, feed.link));
-  GB_CUDA(cudaStreamSynchronize(feed.link));
+  for (auto& q : parts.v) {
+    GB_CUDA(cudaSetDevice(q->dev));
+    GB_CUDA(cudaMemcpyAsync(q->nbad + 1, q->bad.p + 1, 4, cudaMemcpyDeviceToHost, q->feed.link));
+  }
+  nbad = 0;
+  for (auto& q : parts.v) {
+    GB_CUDA(cudaStreamSynchronize(q->feed.link));
+    nbad += q->nbad[1];
+  }
+  GB_REQUIRE(nbad == 0, "CSR holds %u targets >= node_count %u", nbad, n);
+  WccPart& root = *parts.v[0];
+  GB_CUDA(cudaSetDevice(root.dev));
+  GB_CUDA(cudaMemcpyAsync(comp, root.parent, (size_t)n * 4, cudaMemcpyDeviceToHost, root.feed.link));
+  GB_CUDA(cudaStreamSynchronize(root.feed.link));
   return GB_OK;
 }
 
@@ -425,7 +551,19 @@ gb_status gb_wcc_csr_u32(int device, uint32_t node_count, const uint32_t* offset
   GB_REQUIRE(config != nullptr, "config is NULL");  // chunk_size / neighbor_rounds / sampling_size: labels unchanged
   GB_REQUIRE(node_count > 0, "node_count must be > 0");
   GB_REQUIRE(offsets != nullptr, "offsets is NULL");
-  return gb::wcc_csr(device, node_count, offsets, targets, components);
+  GB_TRY(gb::require_device(device));
+  return gb::wcc_csr_parts({device}, 1, node_count, offsets, targets, components);
+}
+gb_status gb_wcc_csr_multi_u32(gb_comm* comm, uint32_t node_count, const uint32_t* offsets,
+                               const uint32_t* targets, const gb_wcc_config* config, uint32_t* components) {
+  GB_REQUIRE(comm != nullptr, "comm is NULL");
+  GB_REQUIRE(components != nullptr, "components is NULL");
+  GB_REQUIRE(config != nullptr, "config is NULL");  // chunk_size / neighbor_rounds / sampling_size: labels unchanged
+  GB_REQUIRE(node_count > 0, "node_count must be > 0");
+  GB_REQUIRE(offsets != nullptr, "offsets is NULL");
+  const uint64_t per_dev = gb::env_u64("GB_WCC_MULTI_PARTS", 1);
+  const uint32_t v = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(per_dev, 1), gb::WCC_MULTI_MAX_PARTS);
+  return gb::wcc_csr_parts(gb::comm_devices(comm), v, node_count, offsets, targets, components);
 }
 
 // ---- multi-GPU WCC: the phases of wcc() (wcc.rs:158-183) over one rank's vertex range ----------------

@@ -443,6 +443,19 @@ gb_status gb_comm_info(const gb_comm* comm, int* ndev, int* multicast);
 gb_status gb_comm_free(gb_comm* comm);
 gb_status gb_page_rank_multi(gb_comm* comm, const gb_graph* const* graphs, const gb_page_rank_config* config,
                              float* scores, uint64_t* ran_iterations, double* error);
+/* wcc_baseline(&graph, config) (wcc.rs:103-123) of a HOST out-CSR over the devices of a communicator: the
+ * contract, checks, messages and labels of gb_wcc_csr_u32 (the minimum node id of each component; components
+ * is not written when the call fails; config is checked and otherwise ignored; targets may be NULL when
+ * offsets[node_count] == 0).  The edges are cut into P = ndev x V parts of about m / P edges (cuts at
+ * multiples of 4 edges, not at rows); part p runs on devices[p / V], uploads only the offsets of the rows its
+ * edges touch, streams its targets over that device's own PCIe link through its own ring of buffers and links
+ * them into its own forest.  The P forests then merge in ceil(log2 P) rounds over NVLink (peer reads of the
+ * partner's forest), and device 0 copies the labels to the host.  The comm's PageRank buffers are neither used
+ * nor changed.  V = 1 unless GB_WCC_MULTI_PARTS (environment, read per call; clamped to 1..64) says otherwise:
+ * V > 1 runs several parts per device, which tests every multi-part path on one GPU.  GB_WCC_FEED_EDGES sets
+ * the chunk size as for gb_wcc_csr_u32.  Pass page-locked arrays (and components) to get the overlap. */
+gb_status gb_wcc_csr_multi_u32(gb_comm* comm, uint32_t node_count, const uint32_t* offsets,
+                               const uint32_t* targets, const gb_wcc_config* config, uint32_t* components);
 
 #ifdef __cplusplus
 }
