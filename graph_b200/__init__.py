@@ -78,6 +78,36 @@ class Comm:
         _, micros = _timed(go)
         return PageRankResult(scores, int(it.value), float(err.value), micros)
 
+    def page_rank_csr(self, in_offsets, in_targets, out_offsets, *, max_iterations: int = 20,
+                      tolerance: float = 1e-4, damping_factor: float = 0.85) -> "PageRankResult":
+        """page_rank of a host CSR over the communicator's devices, with no resident twin
+        (gb_page_rank_csr_multi_u32): each device uploads about 1/ndev of the arrays over its own bus, every rank
+        gathers its rows from the parts and builds its shard, and the sweeps are those of page_rank (JACOBI).
+        Same arrays and checks as DiGraph.for_page_rank; pass pinned arrays to overlap the upload."""
+        io, it_, oo = _page_rank_csr_arrays(in_offsets, in_targets, out_offsets, "page_rank_csr")
+        cfg = _capi.PageRankConfig(int(max_iterations), float(tolerance), float(damping_factor), _capi.PR_JACOBI)
+        scores = np.empty(len(io) - 1, np.float32)
+        it, err = C.c_uint64(0), C.c_double(0.0)
+
+        def go():
+            check(lib.gb_page_rank_csr_multi_u32(self._c, len(io) - 1, _ptr(io), _ptr(it_) if len(it_) else None,
+                                                 _ptr(oo), C.byref(cfg), _ptr(scores), C.byref(it), C.byref(err)))
+        _, micros = _timed(go)
+        return PageRankResult(scores, int(it.value), float(err.value), micros)
+
+    def pr_shards_csr(self, in_offsets, in_targets, out_offsets, *, ranks_per_device: int = 1):
+        """The shards of page_rank_csr (gb_pr_shards_csr_u32) as multigpu.CudaShardBackend objects, rank r on
+        devices[r // ranks_per_device], for a caller that drives the sweeps itself."""
+        from .multigpu import CudaShardBackend
+        io, it_, oo = _page_rank_csr_arrays(in_offsets, in_targets, out_offsets, "pr_shards_csr")
+        world = len(self.devices) * int(ranks_per_device)
+        arr = (C.c_void_p * max(world, 1))()
+        check(lib.gb_pr_shards_csr_u32(self._c, int(ranks_per_device), len(io) - 1, _ptr(io),
+                                       _ptr(it_) if len(it_) else None, _ptr(oo), arr))
+        return [CudaShardBackend.from_handle(arr[r], r, world, len(io) - 1,
+                                             f"cuda:{self.devices[r // int(ranks_per_device)]}")
+                for r in range(world)]
+
     def wcc_csr(self, offsets, targets, *, chunk_size: int | None = None, neighbor_rounds: int | None = None,
                 sampling_size: int | None = None, out=None):
         """graph_b200.wcc_csr over the communicator's devices (gb_wcc_csr_multi_u32): each device streams and
@@ -510,13 +540,7 @@ class DiGraph(_Handle):
     def for_page_rank(in_offsets, in_targets, out_offsets) -> "DiGraph":
         """Device twin holding only what page_rank reads: the in-CSR and the out-degrees (as out offsets).
         Arrays are used as given (pass pinned uint32 arrays to upload at PCIe speed)."""
-        io, it, oo = (np.asarray(a) for a in (in_offsets, in_targets, out_offsets))
-        for a in (io, it, oo):
-            if a.dtype != np.uint32 or not a.flags.c_contiguous:
-                raise TypeError("for_page_rank needs contiguous uint32 arrays")
-        _check_host_csr(io, it, "in")
-        if len(oo) != len(io):
-            raise ValueError("in and out offsets must have the same length (node_count + 1)")
+        io, it, oo = _page_rank_csr_arrays(in_offsets, in_targets, out_offsets, "for_page_rank")
         return _construct(DiGraph, lib.gb_digraph_for_page_rank_u32, _device, len(io) - 1, _ptr(io), _ptr(it),
                           _ptr(oo))
 
@@ -706,6 +730,18 @@ class Graph(_Handle):
             check(lib.gb_triangle_count(self._g, C.byref(tri)))
         _, micros = _timed(go)
         return TriangleCountResult(int(tri.value), micros)
+
+
+def _page_rank_csr_arrays(in_offsets, in_targets, out_offsets, what: str):
+    """The host arrays of a page-rank CSR as given: contiguous uint32, consistent lengths."""
+    io, it, oo = (np.asarray(a) for a in (in_offsets, in_targets, out_offsets))
+    for a in (io, it, oo):
+        if a.dtype != np.uint32 or not a.flags.c_contiguous:
+            raise TypeError(f"{what} needs contiguous uint32 arrays")
+    _check_host_csr(io, it, "in")
+    if len(oo) != len(io):
+        raise ValueError("in and out offsets must have the same length (node_count + 1)")
+    return io, it, oo
 
 
 def _wcc_csr_call(fn, first, offsets, targets, chunk_size, neighbor_rounds, sampling_size, out) -> WccResult:

@@ -147,6 +147,9 @@ SIGNATURES = {
     "gb_page_rank_multi": (C.c_int, [_P, _P, C.POINTER(PageRankConfig), _P, C.POINTER(C.c_uint64),
                                      C.POINTER(C.c_double)]),
     "gb_wcc_csr_multi_u32": (C.c_int, [_P, C.c_uint32, _P, _P, C.POINTER(WccConfig), _P]),
+    "gb_page_rank_csr_multi_u32": (C.c_int, [_P, C.c_uint32, _P, _P, _P, C.POINTER(PageRankConfig), _P,
+                                             C.POINTER(C.c_uint64), C.POINTER(C.c_double)]),
+    "gb_pr_shards_csr_u32": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P, _P, _P, C.POINTER(_P)]),
 }
 
 

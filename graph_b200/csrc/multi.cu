@@ -15,7 +15,10 @@
 #include <cstring>
 #include <vector>
 
-#include "common.cuh"
+#include <cub/cub.cuh>
+
+#include "pr_plan.cuh"
+#include "pr_split.h"
 
 struct gb_comm {
   std::vector<int> devs;
@@ -244,6 +247,390 @@ static gb_status comm_prepare(gb_comm* c, uint32_t n) {
   return GB_OK;
 }
 
+// The shards of one call, freed together
+struct ShardSet {
+  std::vector<gb_pr_shard*> v;
+  explicit ShardSet(uint32_t count) : v(count, nullptr) {}
+  void clear() {
+    for (gb_pr_shard* sh : v)
+      if (sh) gb_pr_shard_free(sh);
+    v.clear();
+  }
+  ~ShardSet() { clear(); }
+};
+
+// The sweeps of the sharded JACOBI schedule over the communicator, one shard per device (shards[i] on
+// devs[i]), and the assembly of the ranks on device 0.  scores, *ran and *error are written only on success.
+static gb_status comm_sweeps(gb_comm* c, uint32_t n, const std::vector<gb_pr_shard*>& shards,
+                             const gb_page_rank_config* cfg, float* scores, uint64_t* ran, double* error) {
+  const uint32_t P = (uint32_t)c->devs.size();
+  GB_TRY(comm_prepare(c, n));
+  const uint32_t n_pad = c->n_pad;
+  for (uint32_t i = 0; i < P; ++i)
+    GB_TRY(gb_pr_shard_init(shards[i], cfg->damping_factor, c->x[i], c->x[i] + n_pad, c->scores[i], c->streams[i]));
+  // every device has finished its init before anybody's sweep-2 stores could land in its x0
+  for (uint32_t i = 0; i < P; ++i) {
+    GB_CUDA(cudaSetDevice(c->devs[i]));
+    GB_CUDA(cudaStreamSynchronize(c->streams[i]));
+  }
+  const uint64_t limit = cfg->max_iterations ? cfg->max_iterations : 100000ull;
+  const bool can_stop = cfg->tolerance > 0.0;
+  uint64_t sweep = 0;
+  double total = 0.0;
+  std::vector<float*> peers(8, nullptr);
+  std::vector<void*> blocks(8, nullptr);
+  for (;;) {
+    ++sweep;
+    const uint32_t cur = (uint32_t)((sweep - 1) & 1), nxt = (uint32_t)(sweep & 1);
+    for (uint32_t i = 0; i < P; ++i) {
+      uint32_t np = 0;
+      for (uint32_t q = 0; q < P; ++q)
+        if (q != i) peers[np++] = c->x[q] + (size_t)nxt * n_pad;
+      float* mc = c->multicast ? reinterpret_cast<float*>(c->mc_va[i]) + (size_t)nxt * n_pad : nullptr;
+      GB_TRY(gb_pr_shard_step(shards[i], cfg->damping_factor, sweep, c->x[i] + (size_t)cur * n_pad,
+                              c->x[i] + (size_t)nxt * n_pad, peers.data(), P - 1, P > 1 ? mc : nullptr, c->scores[i],
+                              c->err[i], c->streams[i]));
+    }
+    for (uint32_t i = 0; i < P; ++i) {
+      for (uint32_t q = 0; q < P; ++q) blocks[q] = c->ctl[q];
+      GB_TRY(gb_pr_shard_sync(shards[i], c->sync_seq + sweep, c->err[i], c->ctl[i], blocks.data(), c->total_err[i],
+                              (uint32_t)(sweep % 64), c->streams[i]));
+    }
+    const bool last = sweep == limit;
+    if (can_stop || last) {
+      GB_CUDA(cudaSetDevice(c->devs[0]));
+      GB_CUDA(cudaMemcpyAsync(&total, c->total_err[0] + (sweep % 64), sizeof(double), cudaMemcpyDeviceToHost,
+                              c->streams[0]));
+      GB_CUDA(cudaStreamSynchronize(c->streams[0]));
+      if ((can_stop && total < cfg->tolerance) || last) break;
+    }
+  }
+  c->sync_seq += sweep;
+  *ran = sweep;
+  *error = total;
+  // every device holds its own rows' scores (zero elsewhere): sum them on device 0, then original ids
+  for (uint32_t i = 0; i < P; ++i) {
+    GB_CUDA(cudaSetDevice(c->devs[i]));
+    GB_CUDA(cudaStreamSynchronize(c->streams[i]));
+  }
+  GB_CUDA(cudaSetDevice(c->devs[0]));
+  float* tmp = c->x[0];  // the out_scores vectors are free again: staging for the peers' score vectors
+  for (uint32_t q = 1; q < P; ++q) {
+    GB_CUDA(cudaMemcpyPeerAsync(tmp, c->devs[0], c->scores[q], c->devs[q], (size_t)n * sizeof(float), c->streams[0]));
+    k_add_f32<<<grid_for(n, 256), 256, 0, c->streams[0]>>>(c->scores[0], tmp, n);
+  }
+  GB_TRY(gb_pr_shard_finish(shards[0], c->scores[0], tmp, c->streams[0]));
+  GB_CUDA(cudaMemcpyAsync(scores, tmp, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, c->streams[0]));
+  GB_CUDA(cudaStreamSynchronize(c->streams[0]));
+  return GB_OK;
+}
+
+// ---- shards from a host in-CSR (gb_pr_shards_csr_u32) ----------------------------------------------------
+// Rank r's in-degree of every original row, 0 for the rows another rank owns (the deal of 32-row slices of the
+// internal order over U ranks); entry n is 0, so that an exclusive scan gives the local offsets
+__global__ void k_pr_owned_deg(const uint32_t* __restrict__ in_off, const uint32_t* __restrict__ new_id, uint32_t n,
+                               uint32_t U, uint32_t r, uint32_t* __restrict__ deg) {
+  for (uint32_t v = blockIdx.x * blockDim.x + threadIdx.x; v <= n; v += gridDim.x * blockDim.x)
+    deg[v] = v < n && (new_id[v] >> 5) % U == r ? in_off[v + 1] - in_off[v] : 0u;
+}
+
+constexpr uint32_t GATHER_ILP = 8;  // 32-entry loads in flight per warp while it copies one row
+// One landed chunk of one part, rows [v0, v1) of the original order: a warp takes 32 consecutive rows, ballots
+// those rank r owns and copies each with the whole warp, 32 entries per step, from the part's targets (a peer
+// pointer when the part lives on another device; part_tgt[0] is edge part_e0) to loc_tgt + loc_off[v].  Every
+// copied target is checked against n; a warp adds its count of bad ones to *bad once.
+__global__ void __launch_bounds__(256) k_pr_gather_rows(const uint32_t* __restrict__ in_off,
+                                                        const uint32_t* __restrict__ part_tgt, uint64_t part_e0,
+                                                        uint32_t v0, uint32_t v1, const uint32_t* __restrict__ new_id,
+                                                        uint32_t U, uint32_t r, const uint32_t* __restrict__ loc_off,
+                                                        uint32_t* __restrict__ loc_tgt, uint32_t n,
+                                                        unsigned int* __restrict__ bad) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
+  uint32_t nbad = 0;
+  for (uint64_t base = (uint64_t)v0 + 32ull * warp; base < v1; base += 32ull * nwarps) {
+    const uint64_t v = base + lane;
+    uint32_t b0 = 0, d = 0, dst = 0;
+    if (v < v1 && (new_id[v] >> 5) % U == r) {
+      b0 = in_off[v];
+      d = in_off[v + 1] - b0;
+      dst = loc_off[v];
+    }
+    uint32_t todo = __ballot_sync(0xFFFFFFFFu, d != 0);
+    while (todo) {
+      const int src_lane = __ffs(todo) - 1;
+      todo &= todo - 1;
+      const uint32_t rb = __shfl_sync(0xFFFFFFFFu, b0, src_lane);
+      const uint32_t rd = __shfl_sync(0xFFFFFFFFu, d, src_lane);
+      const uint32_t rdst = __shfl_sync(0xFFFFFFFFu, dst, src_lane);
+      const uint32_t* __restrict__ from = part_tgt + (rb - part_e0);
+      uint32_t* __restrict__ to = loc_tgt + rdst;
+      for (uint64_t i = lane; i < rd; i += 32 * GATHER_ILP) {
+        uint32_t t[GATHER_ILP];
+#pragma unroll
+        for (uint32_t u = 0; u < GATHER_ILP; ++u) t[u] = i + 32 * u < rd ? from[i + 32 * u] : 0u;
+#pragma unroll
+        for (uint32_t u = 0; u < GATHER_ILP; ++u)
+          if (i + 32 * u < rd) {
+            nbad += t[u] >= n;
+            to[i + 32 * u] = t[u];
+          }
+      }
+    }
+  }
+  nbad = __reduce_add_sync(0xFFFFFFFFu, nbad);
+  if (lane == 0 && nbad) atomicAdd(bad, nbad);
+}
+
+// Device memory that another device may read or copy from.  cudaDeviceEnablePeerAccess (gb_comm_init) maps
+// cudaMalloc memory into the peers, not blocks of the stream-ordered pool DevBuf draws from (DESIGN.md §4.2),
+// so with several parts it is cudaMalloc'd; a lone part keeps the pool's cached blocks.
+struct PeerBuf {
+  uint32_t* p = nullptr;
+  uint32_t* shared = nullptr;
+  DevBuf<uint32_t> pooled;
+  gb_status alloc(size_t count, bool peers) {
+    if (!peers) {
+      GB_TRY(pooled.alloc(count));
+      p = pooled.p;
+      return GB_OK;
+    }
+    GB_CUDA(cudaMalloc(reinterpret_cast<void**>(&shared), std::max<size_t>(count, 1) * sizeof(uint32_t)));
+    p = shared;
+    return GB_OK;
+  }
+  void release() {  // on the buffer's device, nothing may still use it
+    if (shared) cudaFree(shared);
+    shared = p = nullptr;
+    pooled.release();
+  }
+  ~PeerBuf() { release(); }
+};
+
+constexpr uint64_t PR_PART_CHUNK_EDGES = 1u << 23;  // 32 MiB of targets per chunk (GB_PR_PART_CHUNK_EDGES)
+
+// One part of the host in-CSR (pr_split.h) on device dev: its offsets and targets, uploaded on its own copy stream
+struct PrCsrPart {
+  int dev = -1;
+  PrPart range;
+  cudaStream_t copy = nullptr;
+  cudaEvent_t offsets_in = nullptr;
+  std::vector<cudaEvent_t> landed;  // [K] recorded behind each chunk of targets
+  PeerBuf in_off, out_off, tgt;     // rows + 1, rows + 1 and e_end - e_begin entries
+  ~PrCsrPart() {
+    if (dev < 0) return;
+    cudaSetDevice(dev);
+    if (copy) cudaStreamSynchronize(copy);
+    tgt.release();
+    out_off.release();
+    in_off.release();
+    for (cudaEvent_t ev : landed) cudaEventDestroy(ev);
+    if (offsets_in) cudaEventDestroy(offsets_in);
+    if (copy) cudaStreamDestroy(copy);
+  }
+};
+
+// One rank r on device dev: the full offsets gathered from the parts, the order stage of its layout, and the
+// compact local in-CSR of the rows it owns (loc_off by original id, loc_tgt in CSR order)
+struct PrCsrRank {
+  int dev = -1;
+  cudaStream_t s = nullptr;
+  PeerBuf in_off, out_off;     // [n + 1] each
+  LayoutBuild* build = nullptr;
+  DevBuf<uint32_t> loc_off, loc_tgt;
+  uint64_t entries = 0;        // loc_off[n]
+  DevBuf<unsigned int> bad;    // [0] in rows whose offsets decrease, [1] out rows, [2] targets >= n
+  unsigned int h_bad[3] = {0, 0, 0};
+  ~PrCsrRank() {
+    if (dev < 0) return;
+    cudaSetDevice(dev);
+    if (s) cudaStreamSynchronize(s);
+    layout_free(build);
+    loc_tgt.release();
+    loc_off.release();
+    bad.release();
+    out_off.release();
+    in_off.release();
+    if (s) cudaStreamDestroy(s);
+  }
+};
+
+// Every rank's stream drains before any part goes: the gathers read the parts
+struct PrCsrRun {
+  std::vector<std::unique_ptr<PrCsrPart>> parts;
+  std::vector<std::unique_ptr<PrCsrRank>> ranks;
+  ~PrCsrRun() {
+    ranks.clear();
+    parts.clear();
+  }
+};
+
+// The shards of ranks 0 .. U-1 (U = devs.size() * V, rank r on devs[r / V]) of a host in-CSR.  Part u of the
+// split (pr_split.h) is uploaded by the device of rank u; every rank then gathers the rows it owns from all
+// parts into a local in-CSR and builds its layout from it.  shards (U entries) are the caller's to free.
+static gb_status pr_csr_shards(const std::vector<int>& devs, uint32_t V, uint32_t n, const uint32_t* in_off,
+                               const uint32_t* in_tgt, const uint32_t* out_off, std::vector<gb_pr_shard*>& shards) {
+  GB_REQUIRE(n > 0, "node_count must be > 0");
+  GB_REQUIRE(in_off && out_off, "offset arrays are NULL");
+  GB_REQUIRE(in_off[n] == out_off[n], "in and out offsets disagree on the edge count");
+  GB_REQUIRE(in_off[0] == 0, "in offsets[0] must be 0");
+  const uint64_t m = in_off[n];
+  GB_REQUIRE(m == 0 || in_tgt != nullptr, "in targets is NULL");
+  GB_REQUIRE(out_off[0] == 0, "out offsets[0] must be 0");
+  GB_REQUIRE(n < 0x7FFFFFFFu, "node_count %u: the local offsets are scanned in one pass of < 2^31 items", n);
+  const uint32_t U = (uint32_t)devs.size() * V;
+  const bool peers = U > 1;
+  const uint64_t chunk_edges = std::max<uint64_t>(env_u32("GB_PR_PART_CHUNK_EDGES", (uint32_t)PR_PART_CHUNK_EDGES), 1);
+  const std::vector<PrPart> split = pr_split(in_off, n, U, chunk_edges);
+  PrCsrRun run;
+  // 1. every part's offsets, then its targets chunk by chunk, round robin over the parts: the copies go out
+  // before the host waits for any check, so every bus is busy from the start
+  size_t max_chunks = 0;
+  for (uint32_t u = 0; u < U; ++u) {
+    run.parts.emplace_back(new (std::nothrow) PrCsrPart());
+    GB_REQUIRE(run.parts.back() != nullptr, "host allocation failed");
+    PrCsrPart& q = *run.parts.back();
+    q.dev = devs[u / V];
+    q.range = split[u];
+    GB_CUDA(cudaSetDevice(q.dev));
+    GB_CUDA(cudaStreamCreateWithFlags(&q.copy, cudaStreamNonBlocking));
+    GB_CUDA(cudaEventCreateWithFlags(&q.offsets_in, cudaEventDisableTiming));
+    const size_t rows = q.range.r_end - q.range.r_begin;
+    GB_TRY(q.in_off.alloc(rows + 1, peers));
+    GB_TRY(q.out_off.alloc(rows + 1, peers));
+    GB_TRY(q.tgt.alloc(q.range.e_end - q.range.e_begin, peers));
+    GB_CUDA(cudaMemcpyAsync(q.in_off.p, in_off + q.range.r_begin, (rows + 1) * 4, cudaMemcpyHostToDevice, q.copy));
+    GB_CUDA(cudaMemcpyAsync(q.out_off.p, out_off + q.range.r_begin, (rows + 1) * 4, cudaMemcpyHostToDevice, q.copy));
+    GB_CUDA(cudaEventRecord(q.offsets_in, q.copy));
+    max_chunks = std::max(max_chunks, q.range.chunk_row.size() - 1);
+  }
+  for (size_t k = 0; k < max_chunks; ++k)
+    for (auto& qp : run.parts) {
+      PrCsrPart& q = *qp;
+      if (k + 1 >= q.range.chunk_edge.size()) continue;
+      GB_CUDA(cudaSetDevice(q.dev));
+      const uint64_t e0 = q.range.chunk_edge[k], e1 = q.range.chunk_edge[k + 1];
+      if (e1 > e0)
+        GB_CUDA(cudaMemcpyAsync(q.tgt.p + (e0 - q.range.e_begin), in_tgt + e0, (e1 - e0) * 4, cudaMemcpyHostToDevice,
+                                q.copy));
+      cudaEvent_t ev = nullptr;
+      GB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+      q.landed.push_back(ev);
+      GB_CUDA(cudaEventRecord(ev, q.copy));
+    }
+  // 2. rank u checks part u's rows (the slices tile [0, n]: every row once, whatever the host arrays hold), and
+  // every rank assembles the full offsets from the parts
+  for (uint32_t r = 0; r < U; ++r) {
+    run.ranks.emplace_back(new (std::nothrow) PrCsrRank());
+    GB_REQUIRE(run.ranks.back() != nullptr, "host allocation failed");
+    PrCsrRank& k = *run.ranks.back();
+    k.dev = devs[r / V];
+    GB_CUDA(cudaSetDevice(k.dev));
+    GB_CUDA(cudaStreamCreateWithFlags(&k.s, cudaStreamNonBlocking));
+    GB_TRY(k.bad.alloc(3));
+    GB_CUDA(cudaMemsetAsync(k.bad.p, 0, 12, k.s));
+    const PrCsrPart& own = *run.parts[r];
+    const uint32_t rows = own.range.r_end - own.range.r_begin;
+    GB_CUDA(cudaStreamWaitEvent(k.s, own.offsets_in, 0));
+    check_monotone_async(k.s, own.in_off.p, rows, k.bad.p);
+    check_monotone_async(k.s, own.out_off.p, rows, k.bad.p + 1);
+    GB_CUDA(cudaMemcpyAsync(k.h_bad, k.bad.p, 8, cudaMemcpyDeviceToHost, k.s));
+    GB_TRY(k.in_off.alloc((size_t)n + 1, peers));
+    GB_TRY(k.out_off.alloc((size_t)n + 1, peers));
+    for (uint32_t u = 0; u < U; ++u) {
+      const PrCsrPart& q = *run.parts[u];
+      const size_t count = (size_t)(q.range.r_end - q.range.r_begin) + (u + 1 == U ? 1 : 0);
+      if (!count) continue;
+      GB_CUDA(cudaStreamWaitEvent(k.s, q.offsets_in, 0));
+      GB_CUDA(cudaMemcpyPeerAsync(k.in_off.p + q.range.r_begin, k.dev, q.in_off.p, q.dev, count * 4, k.s));
+      GB_CUDA(cudaMemcpyPeerAsync(k.out_off.p + q.range.r_begin, k.dev, q.out_off.p, q.dev, count * 4, k.s));
+    }
+  }
+  unsigned int nbad[2] = {0, 0};
+  for (auto& k : run.ranks) {
+    GB_CUDA(cudaSetDevice(k->dev));
+    GB_CUDA(cudaStreamSynchronize(k->s));
+    nbad[0] += k->h_bad[0];
+    nbad[1] += k->h_bad[1];
+  }
+  GB_REQUIRE(nbad[0] == 0, "in offsets are not monotone (%u rows)", nbad[0]);
+  GB_REQUIRE(nbad[1] == 0, "out offsets are not monotone (%u rows)", nbad[1]);
+  // 3. order stage, the local offsets, and the gathers of every chunk as it lands
+  for (uint32_t r = 0; r < U; ++r) {
+    PrCsrRank& k = *run.ranks[r];
+    GB_CUDA(cudaSetDevice(k.dev));
+    PrSource src;
+    src.device = k.dev;
+    src.stream = k.s;
+    src.n = n;
+    src.m = m;
+    src.in_off = k.in_off.p;
+    src.out_off = k.out_off.p;
+    PrDeal deal;
+    deal.P = U;
+    deal.p = r;
+    GB_TRY(layout_begin(src, deal, &k.build));
+    const uint32_t* new_id = layout_new_id(k.build);
+    {
+      DevBufStreamScope scope(k.s);  // the copy streams may still be busy: release waits for this stream only
+      GB_TRY(k.loc_off.alloc((size_t)n + 1));
+      k_pr_owned_deg<<<grid_for((uint64_t)n + 1, 256), 256, 0, k.s>>>(k.in_off.p, new_id, n, U, r, k.loc_off.p);
+      DevBuf<uint8_t> tmp;
+      GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
+        return cub::DeviceScan::ExclusiveSum(t, tb, k.loc_off.p, k.loc_off.p, (int)(n + 1), k.s);
+      }));
+      uint32_t total = 0;
+      GB_CUDA(cudaMemcpyAsync(&total, k.loc_off.p + n, 4, cudaMemcpyDeviceToHost, k.s));
+      GB_CUDA(cudaStreamSynchronize(k.s));
+      k.entries = total;
+      GB_TRY(k.loc_tgt.alloc(std::max<uint64_t>(k.entries, 1)));
+    }
+    for (size_t c = 0; c < max_chunks; ++c)
+      for (auto& qp : run.parts) {
+        const PrCsrPart& q = *qp;
+        if (c >= q.landed.size()) continue;
+        const uint32_t v0 = q.range.chunk_row[c], v1 = q.range.chunk_row[c + 1];
+        if (v1 == v0) continue;
+        GB_CUDA(cudaStreamWaitEvent(k.s, q.landed[c], 0));
+        k_pr_gather_rows<<<grid_for((uint64_t)(v1 - v0), 256), 256, 0, k.s>>>(
+            k.in_off.p, q.tgt.p, q.range.e_begin, v0, v1, new_id, U, r, k.loc_off.p, k.loc_tgt.p, n, k.bad.p + 2);
+      }
+    GB_CUDA(cudaGetLastError());
+    GB_CUDA(cudaMemcpyAsync(k.h_bad + 2, k.bad.p + 2, 4, cudaMemcpyDeviceToHost, k.s));
+  }
+  unsigned int nbad_tgt = 0;
+  for (auto& k : run.ranks) {
+    GB_CUDA(cudaSetDevice(k->dev));
+    GB_CUDA(cudaStreamSynchronize(k->s));
+    nbad_tgt += k->h_bad[2];
+  }
+  GB_REQUIRE(nbad_tgt == 0, "in CSR holds %u targets >= node_count %u", nbad_tgt, n);
+  // 4. every rank has gathered: the parts and the full offsets go (the order stage has read the degrees), and
+  // each rank builds its layout from its local CSR, which goes too
+  run.parts.clear();
+  for (auto& k : run.ranks) {
+    GB_CUDA(cudaSetDevice(k->dev));
+    k->in_off.release();
+    k->out_off.release();
+  }
+  for (uint32_t r = 0; r < U; ++r) {
+    PrCsrRank& k = *run.ranks[r];
+    GB_CUDA(cudaSetDevice(k.dev));
+    PrPlan* plan = nullptr;
+    LayoutBuild* b = k.build;
+    k.build = nullptr;
+    GB_TRY(layout_end(b, k.loc_off.p, k.loc_tgt.p, k.entries, &plan));
+    {
+      DevBufStreamScope scope(k.s);
+      k.loc_tgt.release();
+      k.loc_off.release();
+    }
+    GB_TRY(shard_from_plan(k.dev, plan, &shards[r]));
+  }
+  return GB_OK;
+}
+
 const std::vector<int>& comm_devices(const gb_comm* c) { return c->devs; }
 
 }  // namespace gb
@@ -337,71 +724,51 @@ gb_status gb_page_rank_multi(gb_comm* c, const gb_graph* const* graphs, const gb
   const uint32_t n = info0.node_count;
   int prev = 0;
   cudaGetDevice(&prev);
-  std::vector<gb_pr_shard*> shards(P, nullptr);
+  gb::ShardSet shards(P);
   gb_status st = [&]() -> gb_status {
-    GB_TRY(gb::comm_prepare(c, n));
-    for (uint32_t i = 0; i < P; ++i) GB_TRY(gb_pr_shard_create(graphs[i], i, P, &shards[i]));
-    const uint32_t n_pad = c->n_pad;
-    for (uint32_t i = 0; i < P; ++i)
-      GB_TRY(gb_pr_shard_init(shards[i], cfg->damping_factor, c->x[i], c->x[i] + n_pad, c->scores[i], c->streams[i]));
-    // every device has finished its init before anybody's sweep-2 stores could land in its x0
-    for (uint32_t i = 0; i < P; ++i) {
-      GB_CUDA(cudaSetDevice(c->devs[i]));
-      GB_CUDA(cudaStreamSynchronize(c->streams[i]));
-    }
-    const uint64_t limit = cfg->max_iterations ? cfg->max_iterations : 100000ull;
-    const bool can_stop = cfg->tolerance > 0.0;
-    uint64_t sweep = 0;
-    double total = 0.0;
-    std::vector<float*> peers(8, nullptr);
-    std::vector<void*> blocks(8, nullptr);
-    for (;;) {
-      ++sweep;
-      const uint32_t cur = (uint32_t)((sweep - 1) & 1), nxt = (uint32_t)(sweep & 1);
-      for (uint32_t i = 0; i < P; ++i) {
-        uint32_t np = 0;
-        for (uint32_t q = 0; q < P; ++q)
-          if (q != i) peers[np++] = c->x[q] + (size_t)nxt * n_pad;
-        float* mc = c->multicast ? reinterpret_cast<float*>(c->mc_va[i]) + (size_t)nxt * n_pad : nullptr;
-        GB_TRY(gb_pr_shard_step(shards[i], cfg->damping_factor, sweep, c->x[i] + (size_t)cur * n_pad,
-                                c->x[i] + (size_t)nxt * n_pad, peers.data(), P - 1, P > 1 ? mc : nullptr, c->scores[i],
-                                c->err[i], c->streams[i]));
-      }
-      for (uint32_t i = 0; i < P; ++i) {
-        for (uint32_t q = 0; q < P; ++q) blocks[q] = c->ctl[q];
-        GB_TRY(gb_pr_shard_sync(shards[i], c->sync_seq + sweep, c->err[i], c->ctl[i], blocks.data(), c->total_err[i],
-                                (uint32_t)(sweep % 64), c->streams[i]));
-      }
-      const bool last = sweep == limit;
-      if (can_stop || last) {
-        GB_CUDA(cudaSetDevice(c->devs[0]));
-        GB_CUDA(cudaMemcpyAsync(&total, c->total_err[0] + (sweep % 64), sizeof(double), cudaMemcpyDeviceToHost,
-                                c->streams[0]));
-        GB_CUDA(cudaStreamSynchronize(c->streams[0]));
-        if ((can_stop && total < cfg->tolerance) || last) break;
-      }
-    }
-    c->sync_seq += sweep;
-    *ran_iterations = sweep;
-    *error = total;
-    // every device holds its own rows' scores (zero elsewhere): sum them on device 0, then original ids
-    for (uint32_t i = 0; i < P; ++i) {
-      GB_CUDA(cudaSetDevice(c->devs[i]));
-      GB_CUDA(cudaStreamSynchronize(c->streams[i]));
-    }
-    GB_CUDA(cudaSetDevice(c->devs[0]));
-    float* tmp = c->x[0];  // the out_scores vectors are free again: staging for the peers' score vectors
-    for (uint32_t q = 1; q < P; ++q) {
-      GB_CUDA(cudaMemcpyPeerAsync(tmp, c->devs[0], c->scores[q], c->devs[q], (size_t)n * sizeof(float), c->streams[0]));
-      gb::k_add_f32<<<gb::grid_for(n, 256), 256, 0, c->streams[0]>>>(c->scores[0], tmp, n);
-    }
-    GB_TRY(gb_pr_shard_finish(shards[0], c->scores[0], tmp, c->streams[0]));
-    GB_CUDA(cudaMemcpyAsync(scores, tmp, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, c->streams[0]));
-    GB_CUDA(cudaStreamSynchronize(c->streams[0]));
-    return GB_OK;
+    for (uint32_t i = 0; i < P; ++i) GB_TRY(gb_pr_shard_create(graphs[i], i, P, &shards.v[i]));
+    return gb::comm_sweeps(c, n, shards.v, cfg, scores, ran_iterations, error);
   }();
-  for (uint32_t i = 0; i < P; ++i)
-    if (shards[i]) gb_pr_shard_free(shards[i]);
+  shards.clear();
+  cudaSetDevice(prev);
+  return st;
+}
+
+gb_status gb_pr_shards_csr_u32(gb_comm* c, uint32_t ranks_per_device, uint32_t n, const uint32_t* in_off,
+                               const uint32_t* in_tgt, const uint32_t* out_off, gb_pr_shard** shards) {
+  GB_REQUIRE(c != nullptr, "comm is NULL");
+  GB_REQUIRE(shards != nullptr, "shards is NULL");
+  GB_REQUIRE(ranks_per_device >= 1, "ranks_per_device must be >= 1");
+  const uint64_t U = (uint64_t)c->devs.size() * ranks_per_device;
+  GB_REQUIRE(U <= 8, "%zu devices x %u ranks per device: at most 8 ranks", c->devs.size(), ranks_per_device);
+  int prev = 0;
+  cudaGetDevice(&prev);
+  gb::ShardSet set((uint32_t)U);
+  gb_status st = gb::pr_csr_shards(c->devs, ranks_per_device, n, in_off, in_tgt, out_off, set.v);
+  cudaSetDevice(prev);
+  if (st != GB_OK) return st;
+  for (uint32_t r = 0; r < U; ++r) shards[r] = set.v[r];
+  set.v.clear();
+  return GB_OK;
+}
+
+gb_status gb_page_rank_csr_multi_u32(gb_comm* c, uint32_t n, const uint32_t* in_off, const uint32_t* in_tgt,
+                                     const uint32_t* out_off, const gb_page_rank_config* cfg, float* scores,
+                                     uint64_t* ran_iterations, double* error) {
+  GB_REQUIRE(c != nullptr, "comm is NULL");
+  GB_REQUIRE(scores != nullptr, "scores is NULL");
+  GB_REQUIRE(cfg && ran_iterations && error, "NULL argument");
+  GB_REQUIRE(!(cfg->max_iterations == 0 && !(cfg->tolerance > 0.0)),
+             "max_iterations == 0 with tolerance <= 0 never terminates (page_rank.rs:107)");
+  const uint32_t P = (uint32_t)c->devs.size();
+  int prev = 0;
+  cudaGetDevice(&prev);
+  gb::ShardSet shards(P);
+  gb_status st = [&]() -> gb_status {
+    GB_TRY(gb::pr_csr_shards(c->devs, 1, n, in_off, in_tgt, out_off, shards.v));
+    return gb::comm_sweeps(c, n, shards.v, cfg, scores, ran_iterations, error);
+  }();
+  shards.clear();
   cudaSetDevice(prev);
   return st;
 }

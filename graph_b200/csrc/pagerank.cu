@@ -1169,12 +1169,27 @@ static gb_status page_rank_impl(const gb_graph* g, const gb_page_rank_config* cf
 
 // ---- multi-GPU shard (1-D edge-cut by destination, 32-row slices dealt round-robin) ----------------
 struct gb_pr_shard {
-  const gb_graph* graph = nullptr;
-  int device = 0;                     // the graph's device: gb_pr_shard_free must not read a freed graph
+  const gb_graph* graph = nullptr;    // NULL for the shards of gb_pr_shards_csr_u32, which hold no graph
+  int device = 0;                     // the plan's device: gb_pr_shard_free must not read a freed graph
   gb::PrPlan* plan = nullptr;
   gb::DevBuf<void*> sync_table;       // device copy of the ranks' control-block pointers (gb_pr_shard_sync)
   void* sync_table_host[8] = {nullptr};
 };
+
+namespace gb {
+gb_status shard_from_plan(int device, PrPlan* plan, gb_pr_shard** out) {
+  gb_pr_shard* sh = new (std::nothrow) gb_pr_shard();
+  if (!sh) {
+    DeviceGuard guard(device);
+    free_pr_plan(plan);
+    return fail(GB_ERR_OOM, "host allocation failed");
+  }
+  sh->device = device;
+  sh->plan = plan;
+  *out = sh;
+  return GB_OK;
+}
+}  // namespace gb
 
 extern "C" {
 
@@ -1212,9 +1227,8 @@ gb_status gb_pr_shard_free(gb_pr_shard* shard) {
 gb_status gb_pr_shard_init(const gb_pr_shard* shard, float damping, float* d_x0, float* d_x1,
                            float* d_scores, void* cuda_stream) {
   GB_REQUIRE(shard && d_x0 && d_x1 && d_scores, "NULL argument");
-  const gb_graph* g = shard->graph;
   const gb::PrPlan* p = shard->plan;
-  gb::DeviceGuard guard(g->device);
+  gb::DeviceGuard guard(shard->device);
   // every rank fills the whole initial vector itself (no exchange needed before sweep 1)
   GB_TRY(gb::pr_reset(p, gb::PrStart(p->n, damping), d_x0, d_x1, d_scores, (cudaStream_t)cuda_stream));
   GB_CUDA(cudaGetLastError());
@@ -1228,9 +1242,8 @@ gb_status gb_pr_shard_step(const gb_pr_shard* shard, float damping, uint64_t swe
   GB_REQUIRE(peer_count <= 7, "at most 7 peers");
   GB_REQUIRE(peer_count == 0 || d_peer_x_next || d_mc_x_next, "peer pointer array is NULL");
   GB_REQUIRE(sweep_no >= 1, "sweep_no is 1-based");
-  const gb_graph* g = shard->graph;
   const gb::PrPlan* p = shard->plan;
-  gb::DeviceGuard guard(g->device);
+  gb::DeviceGuard guard(shard->device);
   cudaStream_t s = (cudaStream_t)cuda_stream;
   const gb::PrStart v(p->n, damping);
   gb::PrArgs a = gb::make_args(p, v.base, damping, -1.0 /* the caller owns the stop rule */);
@@ -1260,7 +1273,7 @@ gb_status gb_pr_shard_sync(const gb_pr_shard* shard, uint64_t sweep_no, const do
   GB_REQUIRE(p->deal.P <= 8, "at most 8 ranks");
   GB_REQUIRE(p->deal.P == 1 || d_peer_blocks, "peer block array is NULL");
   GB_REQUIRE(sweep_no >= 1 && sweep_no < 0x7FFFFFFFull, "bad sweep number");
-  gb::DeviceGuard guard(shard->graph->device);
+  gb::DeviceGuard guard(shard->device);
   cudaStream_t s = (cudaStream_t)cuda_stream;
   // the peer pointer table lives in the shard (device copy, refreshed when the pointers change)
   gb_pr_shard* sh = const_cast<gb_pr_shard*>(shard);
@@ -1281,9 +1294,8 @@ gb_status gb_pr_shard_sync(const gb_pr_shard* shard, uint64_t sweep_no, const do
 gb_status gb_pr_shard_finish(const gb_pr_shard* shard, const float* d_scores_internal, float* d_scores_out,
                              void* cuda_stream) {
   GB_REQUIRE(shard && d_scores_internal && d_scores_out, "NULL argument");
-  const gb_graph* g = shard->graph;
   const gb::PrPlan* p = shard->plan;
-  gb::DeviceGuard guard(g->device);
+  gb::DeviceGuard guard(shard->device);
   gb::k_unpermute<<<gb::grid_for(p->n, 256), 256, 0, (cudaStream_t)cuda_stream>>>(d_scores_internal, p->new_id.p,
                                                                                  p->n, d_scores_out);
   GB_CUDA(cudaGetLastError());

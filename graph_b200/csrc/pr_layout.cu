@@ -151,7 +151,7 @@ __device__ __forceinline__ uint32_t cb_classify_row(uint32_t l, uint32_t b0, uin
   }
   return rem;
 }
-// rows in internal order (the whole in-CSR is resident): one warp per local row
+// rows in internal order (the row source is resident): one warp per local row
 __global__ void k_cb_count(const uint32_t* __restrict__ in_off, const uint32_t* __restrict__ in_tgt,
                            const uint32_t* __restrict__ old_of, const uint32_t* __restrict__ new_id,
                            const uint32_t* __restrict__ hot_of_blk, const uint32_t* __restrict__ nrows,
@@ -550,6 +550,8 @@ __global__ void __launch_bounds__(CB_BANK_THREADS) k_cb_bank_order(const uint4* 
 }
 
 // ---- layout build ----------------------------------------------------------------------------------
+// The degrees (order, hot blocks, staircase) come from the PrSource's full offsets; the rows' edges from the
+// row source (row_off, row_tgt) given to layout_end, which for a resident twin is its in-CSR.
 template <typename T>
 static gb_status scan_exclusive(cudaStream_t s, T* data, uint64_t count) {
   GB_REQUIRE(count < (1ull << 31), "scan of %llu items is too long", (unsigned long long)count);
@@ -570,15 +572,19 @@ static gb_status upload(cudaStream_t s, DevBuf<T>* dst, const std::vector<T>& sr
 // buffer waits for the stream (the streamed upload overlaps with those waits), and rec alone holds 8 bytes
 // per in-edge, so a longer lifetime raises the build's peak memory.
 struct LayoutBuild {
-  const gb_graph* g;
-  PrPlan* p;
+  PrSource src;
+  PrPlan* p = nullptr;
   PrDeal deal;
-  cudaStream_t s;
-  uint32_t n;
-  uint64_t m;
-  uint32_t B;
-  double tau;
-  int dev_sms;
+  cudaStream_t s = nullptr;
+  uint32_t n = 0;
+  uint64_t m = 0;
+  uint32_t B = 0;
+  double tau = CB_TAU_DEFAULT;
+  int dev_sms = (int)H100_SMS;
+  // the row source (layout_end): row v's in-edges are row_tgt[row_off[v] .. row_off[v + 1]), row_entries in all
+  const uint32_t* row_off = nullptr;
+  const uint32_t* row_tgt = nullptr;
+  uint64_t row_entries = 0;
   uint32_t n_mega = 0;  // local rows [0, n_mega) take the sort path of the build
   uint32_t M = 0;       // their in-edges
   std::vector<uint32_t> h_nrows, h_poff;  // the staircase on the host
@@ -609,7 +615,7 @@ gb_status LayoutBuild::layout_order() {
     GB_TRY(keys_alt.alloc(n));
     GB_TRY(ids.alloc(n));
     GB_TRY(ids_alt.alloc(n));
-    k_perm_keys<<<grid_for(n, 256), 256, 0, s>>>(g->in.off.p, g->out.off.p, n, keys.p, ids.p);
+    k_perm_keys<<<grid_for(n, 256), 256, 0, s>>>(src.in_off, src.out_off, n, keys.p, ids.p);
     cub::DoubleBuffer<uint64_t> kb(keys.p, keys_alt.p);
     cub::DoubleBuffer<uint32_t> vb(ids.p, ids_alt.p);
     DevBuf<uint8_t> tmp;
@@ -617,7 +623,7 @@ gb_status LayoutBuild::layout_order() {
     GB_TRY(p->new_id.alloc(n));
     GB_TRY(p->outdeg.alloc(n));
     GB_TRY(indeg.alloc((size_t)n + 1));
-    k_perm_scatter<<<grid_for(n, 256), 256, 0, s>>>(vb.Current(), g->out.off.p, g->in.off.p, n, p->new_id.p,
+    k_perm_scatter<<<grid_for(n, 256), 256, 0, s>>>(vb.Current(), src.out_off, src.in_off, n, p->new_id.p,
                                                    p->outdeg.p, indeg.p);
     GB_TRY(old_of.alloc(n));
     GB_CUDA(cudaMemcpyAsync(old_of.p, vb.Current(), (size_t)n * 4, cudaMemcpyDeviceToDevice, s));
@@ -750,9 +756,9 @@ gb_status LayoutBuild::layout_classify() {
     GB_CUDA(cudaMemcpyAsync(&dmax, indeg.p + deal_global(n_mega, deal.P, deal.p), 4, cudaMemcpyDeviceToHost, s));
     GB_CUDA(cudaStreamSynchronize(s));
     GB_REQUIRE(dmax < 0x7FFFFFFFu, "a row with %u in-edges outside the sort path of the layout build", dmax);
-    GB_TRY(rec.alloc(std::max<uint64_t>(m, 1)));
+    GB_TRY(rec.alloc(std::max<uint64_t>(row_entries, 1)));
   }
-  if (const TargetFeed* feed = g->feed) {
+  if (const TargetFeed* feed = src.feed) {
     // the targets arrive chunk by chunk: check and classify each chunk as soon as it is there
     DevBuf<unsigned int> bad;
     GB_TRY(bad.alloc(1));
@@ -761,10 +767,10 @@ gb_status LayoutBuild::layout_classify() {
       const uint32_t v0 = feed->row_begin[k], v1 = feed->row_begin[k + 1];
       const uint64_t e0 = feed->edge_begin[k], e1 = feed->edge_begin[k + 1];
       GB_CUDA(cudaStreamWaitEvent(s, feed->ready[k], 0));
-      check_ids_async(s, g->in.tgt.p + e0, e1 - e0, n, bad.p);
+      check_ids_async(s, row_tgt + e0, e1 - e0, n, bad.p);
       if (p->n_cb > n_mega && v1 > v0)
         k_cb_count_rows<<<grid_for((uint64_t)(v1 - v0), 256), 256, 0, s>>>(
-            g->in.off.p, g->in.tgt.p, p->new_id.p, hot_of_blk.p, p->nrows.p, p->poff.p, p->blk.p, B, v0, v1, n,
+            row_off, row_tgt, p->new_id.p, hot_of_blk.p, p->nrows.p, p->poff.p, p->blk.p, B, v0, v1, n,
             n_mega, p->n_cb, deal, goff.p, rec.p, lens.p, counters.p + 2);
     }
     unsigned int nbad = 0;
@@ -774,7 +780,7 @@ gb_status LayoutBuild::layout_classify() {
     GB_REQUIRE(nbad == 0, "in CSR holds %u targets >= node_count %u", nbad, n);
   } else if (p->n_cb > n_mega) {
     k_cb_count<<<grid_for((uint64_t)(p->n_cb - n_mega) * 32, 256), 256, 0, s>>>(
-        g->in.off.p, g->in.tgt.p, old_of.p, p->new_id.p, hot_of_blk.p, p->nrows.p, p->poff.p, p->blk.p, B,
+        row_off, row_tgt, old_of.p, p->new_id.p, hot_of_blk.p, p->nrows.p, p->poff.p, p->blk.p, B,
         n_mega, p->n_cb, deal, goff.p, rec.p, lens.p, counters.p + 2);
   }
   if (M) {
@@ -784,7 +790,7 @@ gb_status LayoutBuild::layout_classify() {
     GB_TRY(mega_keys.alloc(M));
     GB_TRY(mega_vals.alloc(M));
     GB_TRY(mega_start.alloc(M));
-    k_mega_keys<<<grid_for(M, 256), 256, 0, s>>>(g->in.off.p, g->in.tgt.p, old_of.p, p->new_id.p,
+    k_mega_keys<<<grid_for(M, 256), 256, 0, s>>>(row_off, row_tgt, old_of.p, p->new_id.p,
                                                  hot_of_blk.p, p->nrows.p, B, mega_off.p, n_mega, M, deal,
                                                  keys_in.p, vals_in.p);
     uint32_t row_bits = 1;
@@ -862,14 +868,14 @@ gb_status LayoutBuild::layout_fill() {
                                                        p->poff.p, p->blk.p, B, goff.p, ids, p->slice_meta.p, sell);
     if (p->n_cb > n_mega)
       k_cb_fill<<<grid_for((uint64_t)(p->n_cb - n_mega) * 32, 256), 256, 0, s>>>(
-          g->in.off.p, old_of.p, rec.p, p->poff.p, n_mega, p->n_cb, deal, goff.p, ids, p->slice_meta.p,
+          row_off, old_of.p, rec.p, p->poff.p, n_mega, p->n_cb, deal, goff.p, ids, p->slice_meta.p,
           sell);
     GB_CUDA(cudaGetLastError());
     GB_CUDA(cudaStreamSynchronize(s));
   }
   if (p->n_loc > p->n_cb) {
     k_sell_fill_tail<<<grid_for((uint64_t)(p->num_slices - p->n_cb / 32) * 32, 256), 256, 0, s>>>(
-        g->in.off.p, g->in.tgt.p, old_of.p, p->new_id.p, p->n_cb, p->n_loc, deal, p->num_slices,
+        row_off, row_tgt, old_of.p, p->new_id.p, p->n_cb, p->n_loc, deal, p->num_slices,
         p->slice_meta.p, p->sell.p);
     GB_CUDA(cudaGetLastError());
   }
@@ -950,38 +956,96 @@ gb_status LayoutBuild::layout_chunks() {
   return GB_OK;
 }
 
-gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan) {
+// The order stage runs first, on its own: a caller that builds its rows from the internal order (the local
+// CSR of gb_pr_shards_csr_u32) reads layout_new_id before it hands the rows to layout_end.
+gb_status layout_begin(const PrSource& src, PrDeal deal, LayoutBuild** out) {
   GB_REQUIRE(deal.P >= 1 && deal.p < deal.P, "bad shard %u of %u", deal.p, deal.P);
-  PrPlan* p = new (std::nothrow) PrPlan();
-  if (!p) return fail(GB_ERR_OOM, "host allocation failed");
-  p->n = g->n;
-  p->m = g->in.len;
-  p->deal = deal;
-  // every temporary of the build is used on g->stream only: releasing one waits for that stream, not for
+  DeviceGuard guard(src.device);
+  LayoutBuild* b = new (std::nothrow) LayoutBuild();
+  if (!b) return fail(GB_ERR_OOM, "host allocation failed");
+  b->p = new (std::nothrow) PrPlan();
+  if (!b->p) {
+    delete b;
+    return fail(GB_ERR_OOM, "host allocation failed");
+  }
+  b->src = src;
+  b->deal = deal;
+  b->s = src.stream;
+  b->n = src.n;
+  b->m = src.m;
+  b->p->n = src.n;
+  b->p->m = src.m;
+  b->p->deal = deal;
+  // every temporary of the build is used on src.stream only: releasing one waits for that stream, not for
   // the device (a copy stream may still be bringing in the targets, see TargetFeed)
-  DevBufStreamScope scope(g->stream);
+  DevBufStreamScope scope(src.stream);
   gb_status st = [&]() -> gb_status {
-    LayoutBuild ctx{g, p, deal, g->stream, g->n, g->in.len, 0, CB_TAU_DEFAULT, (int)H100_SMS};
-    GB_CUDA(cudaDeviceGetAttribute(&ctx.dev_sms, cudaDevAttrMultiProcessorCount, g->device));
+    GB_CUDA(cudaDeviceGetAttribute(&b->dev_sms, cudaDevAttrMultiProcessorCount, src.device));
     // knobs (experiments; defaults are the measured optima)
     const uint32_t B = env_u32("GB_PR_BLOCK", CB_BLOCK_DEFAULT);
-    ctx.B = p->B = std::min<uint32_t>(std::max<uint32_t>(B & ~1023u, 1024u), CB_BLOCK_MAX);
-    if (const char* e = getenv("GB_PR_TAU")) ctx.tau = atof(e);
-    if (!(ctx.tau > 0.0)) ctx.tau = 1e30;  // tau <= 0 switches the column blocks off
-    GB_TRY(ctx.layout_order());
-    GB_TRY(ctx.layout_hot_blocks());
-    GB_TRY(ctx.layout_classify());
-    GB_TRY(ctx.layout_sell());
-    GB_TRY(ctx.layout_fill());
-    GB_TRY(ctx.layout_chunks());
-    return plan_sweep_shape(p, ctx.h_nrows, ctx.h_poff, ctx.dev_sms, ctx.s);
+    b->B = b->p->B = std::min<uint32_t>(std::max<uint32_t>(B & ~1023u, 1024u), CB_BLOCK_MAX);
+    if (const char* e = getenv("GB_PR_TAU")) b->tau = atof(e);
+    if (!(b->tau > 0.0)) b->tau = 1e30;  // tau <= 0 switches the column blocks off
+    return b->layout_order();
   }();
   if (st != GB_OK) {
-    free_pr_plan(p);
+    layout_free(b);
     return st;
   }
-  *out_plan = p;
+  *out = b;
   return GB_OK;
+}
+
+const uint32_t* layout_new_id(const LayoutBuild* b) { return b->p->new_id.p; }
+
+gb_status layout_end(LayoutBuild* b, const uint32_t* row_off, const uint32_t* row_tgt, uint64_t row_entries,
+                     PrPlan** out_plan) {
+  DeviceGuard guard(b->src.device);
+  b->row_off = row_off;
+  b->row_tgt = row_tgt;
+  b->row_entries = row_entries;
+  gb_status st = [&]() -> gb_status {
+    DevBufStreamScope scope(b->s);
+    GB_TRY(b->layout_hot_blocks());
+    GB_TRY(b->layout_classify());
+    GB_TRY(b->layout_sell());
+    GB_TRY(b->layout_fill());
+    GB_TRY(b->layout_chunks());
+    return plan_sweep_shape(b->p, b->h_nrows, b->h_poff, b->dev_sms, b->s);
+  }();
+  if (st == GB_OK) {
+    *out_plan = b->p;
+    b->p = nullptr;
+  }
+  layout_free(b);
+  return st;
+}
+
+void layout_free(LayoutBuild* b) {
+  if (!b) return;
+  DeviceGuard guard(b->src.device);
+  DevBufStreamScope scope(b->s);
+  free_pr_plan(b->p);
+  delete b;
+}
+
+gb_status build_pr_plan(const PrSource& src, PrDeal deal, const uint32_t* row_off, const uint32_t* row_tgt,
+                        uint64_t row_entries, PrPlan** out_plan) {
+  LayoutBuild* b = nullptr;
+  GB_TRY(layout_begin(src, deal, &b));
+  return layout_end(b, row_off, row_tgt, row_entries, out_plan);
+}
+
+gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan) {
+  PrSource src;
+  src.device = g->device;
+  src.stream = g->stream;
+  src.n = g->n;
+  src.m = g->in.len;
+  src.in_off = g->in.off.p;
+  src.out_off = g->out.off.p;
+  src.feed = g->feed;
+  return build_pr_plan(src, deal, g->in.off.p, g->in.tgt.p, g->in.len, out_plan);
 }
 
 }  // namespace gb

@@ -129,8 +129,37 @@ static inline uint32_t env_u32(const char* name, uint32_t dflt) {
   return e && *e ? (uint32_t)strtoul(e, nullptr, 10) : dflt;
 }
 
-// the layout of rank deal.p's rows of g (pr_layout.cu); its last stage is plan_sweep_shape
+// Where a layout build (pr_layout.cu) finds the degrees: the internal order, the active rows and the hot
+// blocks come from the full in- and out-offsets (n + 1 each, device memory of `device`), and the build runs
+// on `stream`.  m is the graph's edge count (the hot-block threshold tau m / e_b).  The rows themselves come
+// from a separate row source (layout_end), which need not be the in-CSR: it only has to hold the rows of the
+// rank being built, in CSR order.
+struct PrSource {
+  int device = 0;
+  cudaStream_t stream = nullptr;
+  uint32_t n = 0;
+  uint64_t m = 0;
+  const uint32_t* in_off = nullptr;
+  const uint32_t* out_off = nullptr;
+  const TargetFeed* feed = nullptr;  // targets still landing (gb_page_rank_csr_u32; the rows are the in-CSR)
+};
+struct LayoutBuild;
+// The order stage of rank deal.p's layout; afterwards layout_new_id(*out) (old id -> internal id, n entries on
+// src.device) is valid.
+gb_status layout_begin(const PrSource& src, PrDeal deal, LayoutBuild** out);
+const uint32_t* layout_new_id(const LayoutBuild* b);
+// The other stages, ending with plan_sweep_shape.  Row v's in-edges are row_tgt[row_off[v] .. row_off[v + 1])
+// (row_off indexed by original id, row_entries entries in all); only the rows of rank deal.p are read.  Frees
+// b whatever it returns.
+gb_status layout_end(LayoutBuild* b, const uint32_t* row_off, const uint32_t* row_tgt, uint64_t row_entries,
+                     PrPlan** out_plan);
+void layout_free(LayoutBuild* b);
+gb_status build_pr_plan(const PrSource& src, PrDeal deal, const uint32_t* row_off, const uint32_t* row_tgt,
+                        uint64_t row_entries, PrPlan** out_plan);
+// the layout of rank deal.p's rows of g: its in-CSR is both the degree and the row source
 gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan);
+// a shard of the sweep API that owns `plan` and no graph (gb_pr_shards_csr_u32; pagerank.cu)
+gb_status shard_from_plan(int device, PrPlan* plan, gb_pr_shard** out);
 // launch shapes of the sweep kernels, their error buffers and k_pr_cb's shared-memory size (pagerank.cu).
 // h_nrows / h_poff: the staircase (nrows[], poff[]) as the layout build holds it on the host.
 gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, const std::vector<uint32_t>& h_poff,

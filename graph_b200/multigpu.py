@@ -50,6 +50,20 @@ class CudaShardBackend:
         self.stats = self.info()
         self.n_active = self.stats["active_rows"]
 
+    @classmethod
+    def from_handle(cls, handle, rank: int, world: int, n: int, device):
+        """A backend around a shard built elsewhere (gb_pr_shards_csr_u32), which it now owns and frees; the
+        shard holds no graph."""
+        self = cls.__new__(cls)
+        self.graph = None
+        self.rank, self.world, self.n = rank, world, n
+        self.device = torch.device(device)
+        self._shard = handle if isinstance(handle, C.c_void_p) else C.c_void_p(handle)
+        self.launches = 0
+        self.stats = self.info()
+        self.n_active = self.stats["active_rows"]
+        return self
+
     def info(self) -> dict:
         st = _capi.PrShardStats()
         check(lib.gb_pr_shard_info(self._shard, C.byref(st)))

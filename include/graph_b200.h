@@ -443,6 +443,27 @@ gb_status gb_comm_info(const gb_comm* comm, int* ndev, int* multicast);
 gb_status gb_comm_free(gb_comm* comm);
 gb_status gb_page_rank_multi(gb_comm* comm, const gb_graph* const* graphs, const gb_page_rank_config* config,
                              float* scores, uint64_t* ran_iterations, double* error);
+/* page_rank (page_rank.rs:58-111) of a HOST CSR over the devices of a communicator, with no resident twin:
+ * the contract, checks, messages and config handling of gb_page_rank_csr_u32 + gb_page_rank_multi (the
+ * sharded JACOBI schedule, one rank per device; scores not written when the call fails).  Each device uploads
+ * one row-aligned part of the arrays (about 1/ndev of the edges, and 1/ndev of each offset array) over its
+ * own link; the offsets are all-gathered over NVLink, and every rank gathers the targets of the rows it
+ * owns from the parts (peer reads) into a compact local in-CSR, builds its shard layout from it and frees
+ * it.  The ranks are bit-equal to gb_page_rank_multi on the same communicator with a full twin per device.
+ * GB_PR_PART_CHUNK_EDGES (environment, read per call; default 2^23) sets the size of the target chunks that
+ * the gathers wait for one by one.  Pass page-locked arrays to get the overlap. */
+gb_status gb_page_rank_csr_multi_u32(gb_comm* comm, uint32_t node_count, const uint32_t* in_offsets,
+                                     const uint32_t* in_targets, const uint32_t* out_offsets,
+                                     const gb_page_rank_config* config, float* scores,
+                                     uint64_t* ran_iterations, double* error);
+/* The shards of that call, for a caller that drives the sweeps itself (gb_pr_shard_init / step / sync /
+ * finish).  ranks_per_device = V puts ranks i*V .. i*V+V-1 (of ndev*V <= 8) on devices[i]; shards[r] is rank r.
+ * Each shard is identical (plan shape, statistics, device bytes, sweep results) to
+ * gb_pr_shard_create(twin, r, ndev*V) on a full twin.  V > 1 runs every multi-part path on one GPU.  The shards
+ * hold no graph; free each with gb_pr_shard_free. */
+gb_status gb_pr_shards_csr_u32(gb_comm* comm, uint32_t ranks_per_device, uint32_t node_count,
+                               const uint32_t* in_offsets, const uint32_t* in_targets,
+                               const uint32_t* out_offsets, gb_pr_shard** shards);
 /* wcc_baseline(&graph, config) (wcc.rs:103-123) of a HOST out-CSR over the devices of a communicator: the
  * contract, checks, messages and labels of gb_wcc_csr_u32 (the minimum node id of each component; components
  * is not written when the call fails; config is checked and otherwise ignored; targets may be NULL when

@@ -264,6 +264,20 @@ inline std::tuple<std::vector<float>, std::size_t, double> page_rank(const Direc
   detail::check(gb_page_rank(g.handle(), &cfg, scores.data(), &it, &err));
   return {std::move(scores), static_cast<std::size_t>(it), err};
 }
+// page_rank of a host CSR (in offsets / targets, out offsets: node_count + 1, in_offsets[node_count] and
+// node_count + 1 entries) over the devices of a communicator, with no resident twin (gb_page_rank_csr_multi_u32):
+// each device uploads about 1/ndev of the arrays; the sharded JACOBI schedule of gb_page_rank_multi
+inline std::tuple<std::vector<float>, std::size_t, double> page_rank_csr_multi(
+    gb_comm* comm, std::uint32_t node_count, const std::uint32_t* in_offsets, const std::uint32_t* in_targets,
+    const std::uint32_t* out_offsets, PageRankConfig c) {
+  gb_page_rank_config cfg{c.max_iterations, c.tolerance, c.damping_factor, GB_PR_JACOBI};
+  std::vector<float> scores(node_count);
+  std::uint64_t it = 0;
+  double err = 0.0;
+  detail::check(gb_page_rank_csr_multi_u32(comm, node_count, in_offsets, in_targets, out_offsets, &cfg,
+                                           scores.data(), &it, &err));
+  return {std::move(scores), static_cast<std::size_t>(it), err};
+}
 
 // wcc_afforest(&graph, config) -> impl Components; `to_vec()` / `component(n)`   wcc.rs:95-99,127
 struct Components {
