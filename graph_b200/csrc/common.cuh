@@ -5,6 +5,7 @@
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <memory>
 #include <mutex>
@@ -115,6 +116,39 @@ struct DevBuf {
   size_t bytes() const { return n * sizeof(T); }
 };
 
+// Device memory that another device may read or copy from.  cudaDeviceEnablePeerAccess (gb_comm_init) maps
+// cudaMalloc memory into the peers, not blocks of the stream-ordered pool DevBuf draws from (a pool is
+// reachable from its own device only unless cudaMemPoolSetAccess says otherwise), so a buffer that peers read
+// is cudaMalloc'd, on one device as on many; one that no peer reads keeps the pool's cached blocks.
+struct PeerBuf {
+  uint32_t* p = nullptr;
+  uint32_t* shared = nullptr;
+  DevBuf<uint32_t> pooled;
+  gb_status alloc(size_t count, bool peers, size_t pad = 0) {
+    if (!peers) {
+      GB_TRY(pooled.alloc(count, pad));
+      p = pooled.p;
+      return GB_OK;
+    }
+    const size_t words = count + pad ? count + pad : 1;
+    GB_CUDA(cudaMalloc(reinterpret_cast<void**>(&shared), words * sizeof(uint32_t)));
+    p = shared;
+    return GB_OK;
+  }
+  void release() {  // on the buffer's device, nothing may still use it
+    if (shared) cudaFree(shared);
+    shared = p = nullptr;
+    pooled.release();
+  }
+  ~PeerBuf() { release(); }
+};
+
+// an unsigned decimal knob from the environment (experiments); dflt when it is unset or empty
+inline uint64_t env_u64(const char* name, uint64_t dflt) {
+  const char* e = getenv(name);
+  return e && *e ? strtoull(e, nullptr, 10) : dflt;
+}
+
 // CUB's two-phase call: call(nullptr, bytes) sizes the temporary storage, call(tmp.p, bytes) runs.  tmp is
 // the caller's, so its release (which waits for the stream) stays where the caller puts it; a buffer that
 // already holds enough is reused, a new one gets `headroom` times the size asked for.
@@ -152,17 +186,6 @@ enum class RowOrder : uint8_t { Unknown, Sorted, Unsorted };
 }  // namespace gb
 
 // the opaque handle of the C ABI
-namespace gb {
-// Host targets of the in-CSR that are still on their way to the device (gb_page_rank_csr_u32): the copy
-// stream brings them in row-aligned chunks, and the layout build classifies chunk k while chunk k+1 is
-// on the bus.  row_begin[k] .. row_begin[k+1] are the ORIGINAL row ids of chunk k.
-struct TargetFeed {
-  std::vector<uint32_t> row_begin;   // [chunks + 1]
-  std::vector<uint64_t> edge_begin;  // [chunks + 1] = in_off[row_begin[k]]
-  std::vector<cudaEvent_t> ready;    // [chunks] recorded on the copy stream behind each chunk
-};
-}  // namespace gb
-
 struct gb_graph {
   int device = 0;
   gb_graph_kind kind = GB_KIND_DIRECTED;
@@ -174,7 +197,6 @@ struct gb_graph {
   cudaEvent_t ev_begin = nullptr, ev_end = nullptr;
   mutable std::mutex mu;            // algorithms on one handle serialise on its stream
   mutable gb::PrPlan* pr_plan = nullptr;  // lazily built PageRank layout (pagerank.cu)
-  mutable const gb::TargetFeed* feed = nullptr;  // set only while gb_page_rank_csr_u32 streams the targets in
   mutable gb_timing timing{};
   gb_load_info load{};  // filled by gb_[di]graph_load_u32 (load.cu)
 };

@@ -383,61 +383,17 @@ __global__ void __launch_bounds__(256) k_pr_gather_rows(const uint32_t* __restri
   if (lane == 0 && nbad) atomicAdd(bad, nbad);
 }
 
-// Device memory that another device may read or copy from.  cudaDeviceEnablePeerAccess (gb_comm_init) maps
-// cudaMalloc memory into the peers, not blocks of the stream-ordered pool DevBuf draws from (DESIGN.md §4.2),
-// so with several parts it is cudaMalloc'd; a lone part keeps the pool's cached blocks.
-struct PeerBuf {
-  uint32_t* p = nullptr;
-  uint32_t* shared = nullptr;
-  DevBuf<uint32_t> pooled;
-  gb_status alloc(size_t count, bool peers) {
-    if (!peers) {
-      GB_TRY(pooled.alloc(count));
-      p = pooled.p;
-      return GB_OK;
-    }
-    GB_CUDA(cudaMalloc(reinterpret_cast<void**>(&shared), std::max<size_t>(count, 1) * sizeof(uint32_t)));
-    p = shared;
-    return GB_OK;
-  }
-  void release() {  // on the buffer's device, nothing may still use it
-    if (shared) cudaFree(shared);
-    shared = p = nullptr;
-    pooled.release();
-  }
-  ~PeerBuf() { release(); }
-};
-
 constexpr uint64_t PR_PART_CHUNK_EDGES = 1u << 23;  // 32 MiB of targets per chunk (GB_PR_PART_CHUNK_EDGES)
 
-// One part of the host in-CSR (pr_split.h) on device dev: its offsets and targets, uploaded on its own copy stream
-struct PrCsrPart {
-  int dev = -1;
-  PrPart range;
-  cudaStream_t copy = nullptr;
-  cudaEvent_t offsets_in = nullptr;
-  std::vector<cudaEvent_t> landed;  // [K] recorded behind each chunk of targets
-  PeerBuf in_off, out_off, tgt;     // rows + 1, rows + 1 and e_end - e_begin entries
-  ~PrCsrPart() {
-    if (dev < 0) return;
-    cudaSetDevice(dev);
-    if (copy) cudaStreamSynchronize(copy);
-    tgt.release();
-    out_off.release();
-    in_off.release();
-    for (cudaEvent_t ev : landed) cudaEventDestroy(ev);
-    if (offsets_in) cudaEventDestroy(offsets_in);
-    if (copy) cudaStreamDestroy(copy);
-  }
-};
-
 // One rank r on device dev: the full offsets gathered from the parts, the order stage of its layout, and the
-// compact local in-CSR of the rows it owns (loc_off by original id, loc_tgt in CSR order)
+// compact local in-CSR of the rows it owns (loc_off by original id, loc_tgt in CSR order).  A lone rank needs
+// neither the gathered offsets nor the local CSR: its part is all of them.
 struct PrCsrRank {
   int dev = -1;
   cudaStream_t s = nullptr;
   PeerBuf in_off, out_off;     // [n + 1] each
   LayoutBuild* build = nullptr;
+  PrPlan* plan = nullptr;      // the finished layout, until the caller takes it
   DevBuf<uint32_t> loc_off, loc_tgt;
   uint64_t entries = 0;        // loc_off[n]
   DevBuf<unsigned int> bad;    // [0] in rows whose offsets decrease, [1] out rows, [2] targets >= n
@@ -447,6 +403,7 @@ struct PrCsrRank {
     cudaSetDevice(dev);
     if (s) cudaStreamSynchronize(s);
     layout_free(build);
+    free_pr_plan(plan);
     loc_tgt.release();
     loc_off.release();
     bad.release();
@@ -456,7 +413,7 @@ struct PrCsrRank {
   }
 };
 
-// Every rank's stream drains before any part goes: the gathers read the parts
+// Every rank's stream drains before any part goes: the gathers and a lone rank's layout read the parts
 struct PrCsrRun {
   std::vector<std::unique_ptr<PrCsrPart>> parts;
   std::vector<std::unique_ptr<PrCsrRank>> ranks;
@@ -466,26 +423,28 @@ struct PrCsrRun {
   }
 };
 
-// The shards of ranks 0 .. U-1 (U = devs.size() * V, rank r on devs[r / V]) of a host in-CSR.  Part u of the
-// split (pr_split.h) is uploaded by the device of rank u; every rank then gathers the rows it owns from all
-// parts into a local in-CSR and builds its layout from it.  shards (U entries) are the caller's to free.
-static gb_status pr_csr_shards(const std::vector<int>& devs, uint32_t V, uint32_t n, const uint32_t* in_off,
-                               const uint32_t* in_tgt, const uint32_t* out_off, std::vector<gb_pr_shard*>& shards) {
+gb_status check_pr_host_csr(uint32_t n, const uint32_t* in_off, const uint32_t* in_tgt, const uint32_t* out_off) {
   GB_REQUIRE(n > 0, "node_count must be > 0");
   GB_REQUIRE(in_off && out_off, "offset arrays are NULL");
   GB_REQUIRE(in_off[n] == out_off[n], "in and out offsets disagree on the edge count");
   GB_REQUIRE(in_off[0] == 0, "in offsets[0] must be 0");
-  const uint64_t m = in_off[n];
-  GB_REQUIRE(m == 0 || in_tgt != nullptr, "in targets is NULL");
+  GB_REQUIRE(in_off[n] == 0 || in_tgt != nullptr, "in targets is NULL");
   GB_REQUIRE(out_off[0] == 0, "out offsets[0] must be 0");
-  GB_REQUIRE(n < 0x7FFFFFFFu, "node_count %u: the local offsets are scanned in one pass of < 2^31 items", n);
+  return GB_OK;
+}
+
+gb_status pr_csr_plans(const std::vector<int>& devs, uint32_t V, uint32_t n, const uint32_t* in_off,
+                       const uint32_t* in_tgt, const uint32_t* out_off, uint64_t chunk_edges,
+                       std::vector<PrPlan*>* plans) {
+  const uint64_t m = in_off[n];
   const uint32_t U = (uint32_t)devs.size() * V;
   const bool peers = U > 1;
-  const uint64_t chunk_edges = std::max<uint64_t>(env_u32("GB_PR_PART_CHUNK_EDGES", (uint32_t)PR_PART_CHUNK_EDGES), 1);
   const std::vector<PrPart> split = pr_split(in_off, n, U, chunk_edges);
+  DeviceGuard guard(devs[0]);
   PrCsrRun run;
   // 1. every part's offsets, then its targets chunk by chunk, round robin over the parts: the copies go out
-  // before the host waits for any check, so every bus is busy from the start
+  // before the host waits for any check, so every bus is busy from the start.  The targets keep 8 zeroed
+  // entries of slack, as a resident in-CSR does (DevCsr).
   size_t max_chunks = 0;
   for (uint32_t u = 0; u < U; ++u) {
     run.parts.emplace_back(new (std::nothrow) PrCsrPart());
@@ -496,13 +455,14 @@ static gb_status pr_csr_shards(const std::vector<int>& devs, uint32_t V, uint32_
     GB_CUDA(cudaSetDevice(q.dev));
     GB_CUDA(cudaStreamCreateWithFlags(&q.copy, cudaStreamNonBlocking));
     GB_CUDA(cudaEventCreateWithFlags(&q.offsets_in, cudaEventDisableTiming));
-    const size_t rows = q.range.r_end - q.range.r_begin;
+    const size_t rows = q.range.r_end - q.range.r_begin, len = q.range.e_end - q.range.e_begin;
     GB_TRY(q.in_off.alloc(rows + 1, peers));
     GB_TRY(q.out_off.alloc(rows + 1, peers));
-    GB_TRY(q.tgt.alloc(q.range.e_end - q.range.e_begin, peers));
+    GB_TRY(q.tgt.alloc(len, peers, 8));
     GB_CUDA(cudaMemcpyAsync(q.in_off.p, in_off + q.range.r_begin, (rows + 1) * 4, cudaMemcpyHostToDevice, q.copy));
     GB_CUDA(cudaMemcpyAsync(q.out_off.p, out_off + q.range.r_begin, (rows + 1) * 4, cudaMemcpyHostToDevice, q.copy));
     GB_CUDA(cudaEventRecord(q.offsets_in, q.copy));
+    GB_CUDA(cudaMemsetAsync(q.tgt.p + len, 0, 8 * 4, q.copy));
     max_chunks = std::max(max_chunks, q.range.chunk_row.size() - 1);
   }
   for (size_t k = 0; k < max_chunks; ++k)
@@ -520,7 +480,7 @@ static gb_status pr_csr_shards(const std::vector<int>& devs, uint32_t V, uint32_
       GB_CUDA(cudaEventRecord(ev, q.copy));
     }
   // 2. rank u checks part u's rows (the slices tile [0, n]: every row once, whatever the host arrays hold), and
-  // every rank assembles the full offsets from the parts
+  // with several ranks every rank assembles the full offsets from the parts
   for (uint32_t r = 0; r < U; ++r) {
     run.ranks.emplace_back(new (std::nothrow) PrCsrRank());
     GB_REQUIRE(run.ranks.back() != nullptr, "host allocation failed");
@@ -536,6 +496,7 @@ static gb_status pr_csr_shards(const std::vector<int>& devs, uint32_t V, uint32_
     check_monotone_async(k.s, own.in_off.p, rows, k.bad.p);
     check_monotone_async(k.s, own.out_off.p, rows, k.bad.p + 1);
     GB_CUDA(cudaMemcpyAsync(k.h_bad, k.bad.p, 8, cudaMemcpyDeviceToHost, k.s));
+    if (!peers) continue;
     GB_TRY(k.in_off.alloc((size_t)n + 1, peers));
     GB_TRY(k.out_off.alloc((size_t)n + 1, peers));
     for (uint32_t u = 0; u < U; ++u) {
@@ -556,7 +517,8 @@ static gb_status pr_csr_shards(const std::vector<int>& devs, uint32_t V, uint32_
   }
   GB_REQUIRE(nbad[0] == 0, "in offsets are not monotone (%u rows)", nbad[0]);
   GB_REQUIRE(nbad[1] == 0, "out offsets are not monotone (%u rows)", nbad[1]);
-  // 3. order stage, the local offsets, and the gathers of every chunk as it lands
+  // 3. order stage.  A lone rank owns every row: its part is its in-CSR, whose chunks the layout build checks
+  // and classifies as they land.  Otherwise the local offsets, and the gathers of every chunk as it lands.
   for (uint32_t r = 0; r < U; ++r) {
     PrCsrRank& k = *run.ranks[r];
     GB_CUDA(cudaSetDevice(k.dev));
@@ -565,12 +527,19 @@ static gb_status pr_csr_shards(const std::vector<int>& devs, uint32_t V, uint32_
     src.stream = k.s;
     src.n = n;
     src.m = m;
-    src.in_off = k.in_off.p;
-    src.out_off = k.out_off.p;
+    src.in_off = peers ? k.in_off.p : run.parts[0]->in_off.p;
+    src.out_off = peers ? k.out_off.p : run.parts[0]->out_off.p;
+    src.feed = peers ? nullptr : run.parts[0].get();
     PrDeal deal;
     deal.P = U;
     deal.p = r;
     GB_TRY(layout_begin(src, deal, &k.build));
+    if (!peers) {
+      LayoutBuild* b = k.build;
+      k.build = nullptr;
+      GB_TRY(layout_end(b, src.in_off, run.parts[0]->tgt.p, m, &k.plan));
+      continue;
+    }
     const uint32_t* new_id = layout_new_id(k.build);
     {
       DevBufStreamScope scope(k.s);  // the copy streams may still be busy: release waits for this stream only
@@ -599,36 +568,59 @@ static gb_status pr_csr_shards(const std::vector<int>& devs, uint32_t V, uint32_
     GB_CUDA(cudaGetLastError());
     GB_CUDA(cudaMemcpyAsync(k.h_bad + 2, k.bad.p + 2, 4, cudaMemcpyDeviceToHost, k.s));
   }
-  unsigned int nbad_tgt = 0;
-  for (auto& k : run.ranks) {
-    GB_CUDA(cudaSetDevice(k->dev));
-    GB_CUDA(cudaStreamSynchronize(k->s));
-    nbad_tgt += k->h_bad[2];
-  }
-  GB_REQUIRE(nbad_tgt == 0, "in CSR holds %u targets >= node_count %u", nbad_tgt, n);
-  // 4. every rank has gathered: the parts and the full offsets go (the order stage has read the degrees), and
-  // each rank builds its layout from its local CSR, which goes too
-  run.parts.clear();
-  for (auto& k : run.ranks) {
-    GB_CUDA(cudaSetDevice(k->dev));
-    k->in_off.release();
-    k->out_off.release();
-  }
-  for (uint32_t r = 0; r < U; ++r) {
-    PrCsrRank& k = *run.ranks[r];
-    GB_CUDA(cudaSetDevice(k.dev));
-    PrPlan* plan = nullptr;
-    LayoutBuild* b = k.build;
-    k.build = nullptr;
-    GB_TRY(layout_end(b, k.loc_off.p, k.loc_tgt.p, k.entries, &plan));
-    {
-      DevBufStreamScope scope(k.s);
-      k.loc_tgt.release();
-      k.loc_off.release();
+  if (peers) {
+    unsigned int nbad_tgt = 0;
+    for (auto& k : run.ranks) {
+      GB_CUDA(cudaSetDevice(k->dev));
+      GB_CUDA(cudaStreamSynchronize(k->s));
+      nbad_tgt += k->h_bad[2];
     }
-    GB_TRY(shard_from_plan(k.dev, plan, &shards[r]));
+    GB_REQUIRE(nbad_tgt == 0, "in CSR holds %u targets >= node_count %u", nbad_tgt, n);
+    // 4. every rank has gathered: the parts and the full offsets go (the order stage has read the degrees), and
+    // each rank builds its layout from its local CSR, which goes too
+    run.parts.clear();
+    for (auto& k : run.ranks) {
+      GB_CUDA(cudaSetDevice(k->dev));
+      k->in_off.release();
+      k->out_off.release();
+    }
+    for (auto& k : run.ranks) {
+      GB_CUDA(cudaSetDevice(k->dev));
+      LayoutBuild* b = k->build;
+      k->build = nullptr;
+      GB_TRY(layout_end(b, k->loc_off.p, k->loc_tgt.p, k->entries, &k->plan));
+      DevBufStreamScope scope(k->s);
+      k->loc_tgt.release();
+      k->loc_off.release();
+    }
+  }
+  plans->clear();
+  for (auto& k : run.ranks) {
+    plans->push_back(k->plan);
+    k->plan = nullptr;
   }
   return GB_OK;
+}
+
+// The shards of ranks 0 .. U-1 (U = devs.size() * V, rank r on devs[r / V]) of a host in-CSR: shards (U entries)
+// are the caller's to free.
+static gb_status pr_csr_shards(const std::vector<int>& devs, uint32_t V, uint32_t n, const uint32_t* in_off,
+                               const uint32_t* in_tgt, const uint32_t* out_off, std::vector<gb_pr_shard*>& shards) {
+  GB_TRY(check_pr_host_csr(n, in_off, in_tgt, out_off));
+  GB_REQUIRE(n < 0x7FFFFFFFu, "node_count %u: the local offsets are scanned in one pass of < 2^31 items", n);
+  const uint64_t chunk_edges = std::max<uint64_t>((uint32_t)env_u64("GB_PR_PART_CHUNK_EDGES", PR_PART_CHUNK_EDGES), 1);
+  std::vector<PrPlan*> plans;
+  GB_TRY(pr_csr_plans(devs, V, n, in_off, in_tgt, out_off, chunk_edges, &plans));
+  gb_status st = GB_OK;
+  for (size_t r = 0; r < plans.size(); ++r) {  // shard_from_plan takes its plan, whatever it returns
+    if (st == GB_OK) {
+      st = shard_from_plan(devs[r / V], plans[r], &shards[r]);
+    } else {
+      DeviceGuard guard(devs[r / V]);
+      free_pr_plan(plans[r]);
+    }
+  }
+  return st;
 }
 
 const std::vector<int>& comm_devices(const gb_comm* c) { return c->devs; }
@@ -741,12 +733,8 @@ gb_status gb_pr_shards_csr_u32(gb_comm* c, uint32_t ranks_per_device, uint32_t n
   GB_REQUIRE(ranks_per_device >= 1, "ranks_per_device must be >= 1");
   const uint64_t U = (uint64_t)c->devs.size() * ranks_per_device;
   GB_REQUIRE(U <= 8, "%zu devices x %u ranks per device: at most 8 ranks", c->devs.size(), ranks_per_device);
-  int prev = 0;
-  cudaGetDevice(&prev);
   gb::ShardSet set((uint32_t)U);
-  gb_status st = gb::pr_csr_shards(c->devs, ranks_per_device, n, in_off, in_tgt, out_off, set.v);
-  cudaSetDevice(prev);
-  if (st != GB_OK) return st;
+  GB_TRY(gb::pr_csr_shards(c->devs, ranks_per_device, n, in_off, in_tgt, out_off, set.v));
   for (uint32_t r = 0; r < U; ++r) shards[r] = set.v[r];
   set.v.clear();
   return GB_OK;

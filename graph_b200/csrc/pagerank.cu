@@ -823,7 +823,7 @@ __global__ void __launch_bounds__(32) k_pr_exact(const uint32_t* __restrict__ in
 // ---- launch shapes: the last stage of the layout build --------------------------------------------
 gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, const std::vector<uint32_t>& h_poff,
                            int dev_sms, cudaStream_t s) {
-  p->trace = env_u32("GB_PR_TRACE", 0) != 0;
+  p->trace = (uint32_t)env_u64("GB_PR_TRACE", 0) != 0;
   p->smem_cb = ((size_t)p->B + 4) * sizeof(float);
   GB_CUDA(cudaFuncSetAttribute(k_pr_cb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cb));
   const uint64_t want_sell = ((uint64_t)p->num_slices + PR_SELL_THREADS / 32 - 1) / (PR_SELL_THREADS / 32);
@@ -840,7 +840,7 @@ gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, cons
   const uint64_t fin_warps4 = (uint64_t)p->n_fin_warp / 32 * (PR_FIN_THREADS / 32) + (p->n_fin - p->n_fin_warp + 127) / 128;
   p->fin_u = (fin_warps2 + PR_FIN_THREADS / 32 - 1) / (PR_FIN_THREADS / 32) <= (uint64_t)dev_sms * 8 ? 2 : 4;
   // GB_PR_FIN_U (experiment / tests): 2 or 4 forces that instantiation of k_pr_finish; anything else = automatic
-  const uint32_t force_u = env_u32("GB_PR_FIN_U", 0);
+  const uint32_t force_u = (uint32_t)env_u64("GB_PR_FIN_U", 0);
   if (force_u == 2 || force_u == 4) p->fin_u = force_u;
   const uint64_t fin_tasks = p->fin_u == 2 ? fin_warps2 : fin_warps4;
   const uint64_t want_fin = (fin_tasks + PR_FIN_THREADS / 32 - 1) / (PR_FIN_THREADS / 32);
@@ -856,7 +856,7 @@ gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, cons
   // take, rows left for the others, and at least one CTA beyond the hub CTAs: else no CTA would update
   // the tail rows).
   p->fin_hub_ctas = 0;
-  const uint32_t split = env_u32("GB_PR_FIN_SPLIT", 0);
+  const uint32_t split = (uint32_t)env_u64("GB_PR_FIN_SPLIT", 0);
   const bool split_pays = want_fin <= (uint64_t)dev_sms * 8 && p->KB > 4 * FIN_CTA_BLOCKS;
   if (p->n_fin_warp && p->n_fin > p->n_fin_warp && p->grid_fin > p->n_fin_warp / 32 &&
       (split == 1 || (split == 0 && split_pays)))
@@ -1165,6 +1165,15 @@ static gb_status page_rank_impl(const gb_graph* g, const gb_page_rank_config* cf
   return GB_OK;
 }
 
+// A resident digraph of a host CSR that passed check_pr_host_csr: the in-CSR, and the out-offsets for the
+// out-degrees
+static gb_status page_rank_digraph(int device, uint32_t n, const uint32_t* in_off, const uint32_t* in_tgt,
+                                   const uint32_t* out_off, GraphPtr* g) {
+  GB_TRY(new_graph(device, GB_KIND_DIRECTED, n, g));
+  GB_TRY(upload_host_csr((*g)->stream, n, in_off, in_tgt, nullptr, &(*g)->in, "in"));
+  return upload_host_csr((*g)->stream, n, out_off, nullptr, nullptr, &(*g)->out, "out", true);
+}
+
 }  // namespace gb
 
 // ---- multi-GPU shard (1-D edge-cut by destination, 32-row slices dealt round-robin) ----------------
@@ -1350,111 +1359,42 @@ gb_status gb_page_rank(const gb_graph* graph, const gb_page_rank_config* config,
 }
 
 // One-shot PageRank of a host CSR.  The 4 bytes per edge of the targets dominate the upload, so they are
-// streamed: offsets first, then the targets in row-aligned chunks on a copy stream, while the graph's own
-// stream sorts the degrees, picks the hot blocks and classifies every chunk as it lands (TargetFeed in
-// layout_classify, pr_layout.cu).  Only the fill pass, the sweeps and the copy of the ranks run after the last byte.
-// GB_PR_FEED_CHUNKS (default 16; 0 = upload everything, then build) and GB_PR_FEED_MIN_EDGES (default 2^22)
-// are experiment knobs.
+// streamed, as the one-rank case of the communicator's upload (pr_csr_plans, multi.cu): offsets first, then the
+// targets in row-aligned chunks on a copy stream, while the rank's stream sorts the degrees, picks the hot
+// blocks and classifies every chunk as it lands (layout_classify, pr_layout.cu).  Only the fill pass, the
+// sweeps and the copy of the ranks run after the last byte.  EXACT mode and small graphs upload everything
+// first.  GB_PR_FEED_CHUNKS (default 16 chunks of ceil(m / 16) edges; 0 = upload everything, then build) and
+// GB_PR_FEED_MIN_EDGES (default 2^22) are experiment knobs.
 gb_status gb_page_rank_csr_u32(int device, uint32_t n, const uint32_t* in_off, const uint32_t* in_tgt,
                                const uint32_t* out_off, const gb_page_rank_config* config, float* scores,
                                uint64_t* ran_iterations, double* error) {
   GB_REQUIRE(scores != nullptr, "scores is NULL");
-  GB_REQUIRE(n > 0, "node_count must be > 0");
-  GB_REQUIRE(in_off && out_off, "offset arrays are NULL");
-  GB_REQUIRE(in_off[n] == out_off[n], "in and out offsets disagree on the edge count");
+  GB_TRY(gb::check_pr_host_csr(n, in_off, in_tgt, out_off));
   const uint64_t m = in_off[n];
-  uint32_t chunks = gb::env_u32("GB_PR_FEED_CHUNKS", 16);
-  if (m < gb::env_u32("GB_PR_FEED_MIN_EDGES", 1u << 22)) chunks = 0;
+  uint32_t chunks = (uint32_t)gb::env_u64("GB_PR_FEED_CHUNKS", 16);
+  if (m < (uint32_t)gb::env_u64("GB_PR_FEED_MIN_EDGES", 1u << 22)) chunks = 0;
   // the single-warp EXACT mode (small graphs) reads the CSR directly: nothing to overlap
   if (!config || config->mode == GB_PR_EXACT || (config->mode == GB_PR_AUTO && n <= 16384)) chunks = 0;
   gb::GraphPtr g;
-  GB_TRY(gb::new_graph(device, GB_KIND_DIRECTED, n, &g));
   if (chunks == 0) {
-    GB_TRY(gb::upload_host_csr(g->stream, n, in_off, in_tgt, nullptr, &g->in, "in"));
-    GB_TRY(gb::upload_host_csr(g->stream, n, out_off, nullptr, nullptr, &g->out, "out", true));
+    GB_TRY(gb::page_rank_digraph(device, n, in_off, in_tgt, out_off, &g));
     return gb::page_rank_impl(g.get(), config, nullptr, scores, ran_iterations, error);
   }
-  gb::TargetFeed feed;
-  cudaStream_t copy = nullptr;
-  cudaEvent_t offsets_in = nullptr;
-  gb_status st = [&]() -> gb_status {
-    GB_REQUIRE(in_off[0] == 0 && out_off[0] == 0, "offsets[0] must be 0");
-    GB_REQUIRE(in_tgt != nullptr, "in targets is NULL");
-    GB_CUDA(cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking));
-    GB_CUDA(cudaEventCreateWithFlags(&offsets_in, cudaEventDisableTiming));
-    g->in.len = m;
-    g->out.len = m;
-    GB_TRY(g->in.off.alloc((size_t)n + 1));
-    GB_TRY(g->out.off.alloc((size_t)n + 1));
-    GB_TRY(g->in.tgt.alloc(m, 8));
-    GB_CUDA(cudaMemcpyAsync(g->in.off.p, in_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, copy));
-    GB_CUDA(cudaMemcpyAsync(g->out.off.p, out_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, copy));
-    GB_CUDA(cudaEventRecord(offsets_in, copy));
-    GB_CUDA(cudaMemsetAsync(g->in.tgt.p + m, 0, 8 * 4, copy));
-    // chunk boundaries: rows, at about equal edge counts (a monotone in_off is checked on the device below;
-    // a malformed one only makes uneven chunks here, the bounds stay inside [0, m])
-    feed.row_begin.push_back(0);
-    feed.edge_begin.push_back(0);
-    for (uint32_t k = 1; k <= chunks; ++k) {
-      uint32_t v = n;
-      if (k < chunks) {
-        const uint64_t want = m / chunks * k;
-        v = (uint32_t)(std::upper_bound(in_off, in_off + n + 1, (uint32_t)want) - in_off);
-        v = std::min(std::max(v, feed.row_begin.back()), n);
-      }
-      uint64_t e = std::min<uint64_t>(in_off[v], m);
-      e = std::max(e, feed.edge_begin.back());
-      if (k == chunks) e = m;
-      feed.row_begin.push_back(v);
-      feed.edge_begin.push_back(e);
-    }
-    for (uint32_t k = 0; k < chunks; ++k) {
-      const uint64_t e0 = feed.edge_begin[k], e1 = feed.edge_begin[k + 1];
-      if (e1 > e0)
-        GB_CUDA(cudaMemcpyAsync(g->in.tgt.p + e0, in_tgt + e0, (e1 - e0) * 4, cudaMemcpyHostToDevice, copy));
-      cudaEvent_t ev = nullptr;
-      GB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-      feed.ready.push_back(ev);
-      GB_CUDA(cudaEventRecord(ev, copy));
-    }
-    // offsets: monotone, checked before anything indexes with them
-    GB_CUDA(cudaStreamWaitEvent(g->stream, offsets_in, 0));
-    gb::DevBuf<unsigned int> bad;
-    GB_TRY(bad.alloc(2));
-    GB_CUDA(cudaMemsetAsync(bad.p, 0, 8, g->stream));
-    gb::check_monotone_async(g->stream, g->in.off.p, n, bad.p);
-    gb::check_monotone_async(g->stream, g->out.off.p, n, bad.p + 1);
-    unsigned int nbad[2] = {0, 0};
-    GB_CUDA(cudaMemcpyAsync(nbad, bad.p, 8, cudaMemcpyDeviceToHost, g->stream));
-    GB_CUDA(cudaStreamSynchronize(g->stream));
-    {
-      gb::DevBufStreamScope scope(g->stream);  // do not wait for the copy stream here
-      bad.release();
-    }
-    GB_REQUIRE(nbad[0] == 0, "in offsets are not monotone (%u rows)", nbad[0]);
-    GB_REQUIRE(nbad[1] == 0, "out offsets are not monotone (%u rows)", nbad[1]);
-    g->feed = &feed;
-    return gb::page_rank_impl(g.get(), config, nullptr, scores, ran_iterations, error);
-  }();
-  g->feed = nullptr;
-  if (copy) cudaStreamSynchronize(copy);  // an early error must not free buffers under a running copy
-  g.reset();
-  for (cudaEvent_t ev : feed.ready) cudaEventDestroy(ev);
-  if (offsets_in) cudaEventDestroy(offsets_in);
-  if (copy) cudaStreamDestroy(copy);
-  return st;
+  // the graph brings the stream, the timing events and the lock; the sweeps read only the plan
+  GB_TRY(gb::new_graph(device, GB_KIND_DIRECTED, n, &g));
+  std::vector<gb::PrPlan*> plans;
+  GB_TRY(gb::pr_csr_plans({device}, 1, n, in_off, in_tgt, out_off, std::max<uint64_t>((m + chunks - 1) / chunks, 1),
+                          &plans));
+  g->pr_plan = plans[0];
+  return gb::page_rank_impl(g.get(), config, nullptr, scores, ran_iterations, error);
 }
 
 gb_status gb_digraph_for_page_rank_u32(int device, uint32_t n, const uint32_t* in_off, const uint32_t* in_tgt,
                                        const uint32_t* out_off, gb_graph** graph) {
   GB_REQUIRE(graph != nullptr, "graph is NULL");
-  GB_REQUIRE(n > 0, "node_count must be > 0");
-  GB_REQUIRE(in_off && out_off, "offset arrays are NULL");
-  GB_REQUIRE(in_off[n] == out_off[n], "in and out offsets disagree on the edge count");
+  GB_TRY(gb::check_pr_host_csr(n, in_off, in_tgt, out_off));
   gb::GraphPtr g;
-  GB_TRY(gb::new_graph(device, GB_KIND_DIRECTED, n, &g));
-  GB_TRY(gb::upload_host_csr(g->stream, n, in_off, in_tgt, nullptr, &g->in, "in"));
-  GB_TRY(gb::upload_host_csr(g->stream, n, out_off, nullptr, nullptr, &g->out, "out", true));
+  GB_TRY(gb::page_rank_digraph(device, n, in_off, in_tgt, out_off, &g));
   *graph = g.release();
   return GB_OK;
 }

@@ -669,7 +669,7 @@ gb_status LayoutBuild::layout_hot_blocks() {
     GB_CUDA(cudaMemcpyAsync(h_edges.data(), blk_edges.p, (size_t)nblk * 8, cudaMemcpyDeviceToHost, s));
     GB_CUDA(cudaStreamSynchronize(s));
     std::vector<uint32_t> h_dmin(nblk + 1, 0xFFFFFFFFu);
-    h_dmin[nblk] = env_u32("GB_PR_MEGA", CB_MEGA_DEG) + 1;
+    h_dmin[nblk] = (uint32_t)env_u64("GB_PR_MEGA", CB_MEGA_DEG) + 1;
     for (uint32_t b = 0; b < nblk; ++b)
       if (h_edges[b]) {
         const double d = std::ceil(tau * (double)m / (double)h_edges[b]);
@@ -720,8 +720,8 @@ gb_status LayoutBuild::layout_hot_blocks() {
 
 // Segment sizes (pairs of the staircase) and SELL lane lengths: the longest rows are keyed and sorted once
 // (the sorted edges are kept for layout_fill), every other row that owns segments is classified into one
-// record per in-edge; the targets are classified chunk by chunk as they arrive when a TargetFeed streams
-// them in.  Ends with goff = the first group of every pair.
+// record per in-edge; the targets are classified chunk by chunk as they arrive when they stream in from a
+// part (PrSource::feed).  Ends with goff = the first group of every pair.
 gb_status LayoutBuild::layout_classify() {
   GB_TRY(goff.alloc(p->S + 1));
   GB_CUDA(cudaMemsetAsync(goff.p, 0, (p->S + 1) * 4, s));
@@ -758,15 +758,15 @@ gb_status LayoutBuild::layout_classify() {
     GB_REQUIRE(dmax < 0x7FFFFFFFu, "a row with %u in-edges outside the sort path of the layout build", dmax);
     GB_TRY(rec.alloc(std::max<uint64_t>(row_entries, 1)));
   }
-  if (const TargetFeed* feed = src.feed) {
+  if (const PrCsrPart* feed = src.feed) {
     // the targets arrive chunk by chunk: check and classify each chunk as soon as it is there
     DevBuf<unsigned int> bad;
     GB_TRY(bad.alloc(1));
     GB_CUDA(cudaMemsetAsync(bad.p, 0, 4, s));
-    for (size_t k = 0; k + 1 < feed->row_begin.size(); ++k) {
-      const uint32_t v0 = feed->row_begin[k], v1 = feed->row_begin[k + 1];
-      const uint64_t e0 = feed->edge_begin[k], e1 = feed->edge_begin[k + 1];
-      GB_CUDA(cudaStreamWaitEvent(s, feed->ready[k], 0));
+    for (size_t k = 0; k < feed->landed.size(); ++k) {
+      const uint32_t v0 = feed->range.chunk_row[k], v1 = feed->range.chunk_row[k + 1];
+      const uint64_t e0 = feed->range.chunk_edge[k], e1 = feed->range.chunk_edge[k + 1];
+      GB_CUDA(cudaStreamWaitEvent(s, feed->landed[k], 0));
       check_ids_async(s, row_tgt + e0, e1 - e0, n, bad.p);
       if (p->n_cb > n_mega && v1 > v0)
         k_cb_count_rows<<<grid_for((uint64_t)(v1 - v0), 256), 256, 0, s>>>(
@@ -898,8 +898,8 @@ gb_status LayoutBuild::layout_chunks() {
     // groups (fewer, longer chunks = fewer segments cut by chunk boundaries); a thin block is cut into
     // >= 64 chunks (down to one 64-group step each) so that all warps share it — a lone warp runs at
     // its dependency latency, ~10x below the SM's throughput
-    uint32_t C = env_u32("GB_PR_CHUNK", 0);
-    const uint32_t T = std::min<uint32_t>(std::max<uint32_t>(env_u32("GB_PR_TASK_CHUNKS", CB_TASK_CHUNKS), 32u), 128u);
+    uint32_t C = (uint32_t)env_u64("GB_PR_CHUNK", 0);
+    const uint32_t T = std::min<uint32_t>(std::max<uint32_t>((uint32_t)env_u64("GB_PR_TASK_CHUNKS", CB_TASK_CHUNKS), 32u), 128u);
     if (!C) C = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(p->NG / ((uint64_t)dev_sms * 8 * T), 16384 / T), 65536 / T);
     C = std::max<uint32_t>(32u, (C + 31) / 32 * 32);
     p->chunk_groups = C;
@@ -977,12 +977,12 @@ gb_status layout_begin(const PrSource& src, PrDeal deal, LayoutBuild** out) {
   b->p->m = src.m;
   b->p->deal = deal;
   // every temporary of the build is used on src.stream only: releasing one waits for that stream, not for
-  // the device (a copy stream may still be bringing in the targets, see TargetFeed)
+  // the device (a copy stream may still be bringing in the targets, see PrSource::feed)
   DevBufStreamScope scope(src.stream);
   gb_status st = [&]() -> gb_status {
     GB_CUDA(cudaDeviceGetAttribute(&b->dev_sms, cudaDevAttrMultiProcessorCount, src.device));
     // knobs (experiments; defaults are the measured optima)
-    const uint32_t B = env_u32("GB_PR_BLOCK", CB_BLOCK_DEFAULT);
+    const uint32_t B = (uint32_t)env_u64("GB_PR_BLOCK", CB_BLOCK_DEFAULT);
     b->B = b->p->B = std::min<uint32_t>(std::max<uint32_t>(B & ~1023u, 1024u), CB_BLOCK_MAX);
     if (const char* e = getenv("GB_PR_TAU")) b->tau = atof(e);
     if (!(b->tau > 0.0)) b->tau = 1e30;  // tau <= 0 switches the column blocks off
@@ -1044,7 +1044,6 @@ gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan) {
   src.m = g->in.len;
   src.in_off = g->in.off.p;
   src.out_off = g->out.off.p;
-  src.feed = g->feed;
   return build_pr_plan(src, deal, g->in.off.p, g->in.tgt.p, g->in.len, out_plan);
 }
 

@@ -6,6 +6,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "pr_split.h"
 
 namespace gb {
 
@@ -124,10 +125,27 @@ __host__ __device__ __forceinline__ uint32_t fin_blocks_of(const uint32_t* __res
   return lo;
 }
 
-static inline uint32_t env_u32(const char* name, uint32_t dflt) {
-  const char* e = getenv(name);
-  return e && *e ? (uint32_t)strtoul(e, nullptr, 10) : dflt;
-}
+// One part of a host in-CSR (pr_split.h) on device dev: its offsets and targets, uploaded on its own copy
+// stream, the targets in row-aligned chunks with an event recorded behind each
+struct PrCsrPart {
+  int dev = -1;
+  PrPart range;
+  cudaStream_t copy = nullptr;
+  cudaEvent_t offsets_in = nullptr;
+  std::vector<cudaEvent_t> landed;  // [K] recorded behind each chunk of targets
+  PeerBuf in_off, out_off, tgt;     // rows + 1, rows + 1 and e_end - e_begin (+ 8 zeroed) entries
+  ~PrCsrPart() {
+    if (dev < 0) return;
+    cudaSetDevice(dev);
+    if (copy) cudaStreamSynchronize(copy);
+    tgt.release();
+    out_off.release();
+    in_off.release();
+    for (cudaEvent_t ev : landed) cudaEventDestroy(ev);
+    if (offsets_in) cudaEventDestroy(offsets_in);
+    if (copy) cudaStreamDestroy(copy);
+  }
+};
 
 // Where a layout build (pr_layout.cu) finds the degrees: the internal order, the active rows and the hot
 // blocks come from the full in- and out-offsets (n + 1 each, device memory of `device`), and the build runs
@@ -141,7 +159,9 @@ struct PrSource {
   uint64_t m = 0;
   const uint32_t* in_off = nullptr;
   const uint32_t* out_off = nullptr;
-  const TargetFeed* feed = nullptr;  // targets still landing (gb_page_rank_csr_u32; the rows are the in-CSR)
+  // a part covering [0, n] whose targets are still landing: the row source is its in-CSR, and the build checks
+  // and classifies each chunk as soon as its landed event fires
+  const PrCsrPart* feed = nullptr;
 };
 struct LayoutBuild;
 // The order stage of rank deal.p's layout; afterwards layout_new_id(*out) (old id -> internal id, n entries on
@@ -160,6 +180,18 @@ gb_status build_pr_plan(const PrSource& src, PrDeal deal, const uint32_t* row_of
 gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan);
 // a shard of the sweep API that owns `plan` and no graph (gb_pr_shards_csr_u32; pagerank.cu)
 gb_status shard_from_plan(int device, PrPlan* plan, gb_pr_shard** out);
+
+// The O(1) host checks of a host PageRank CSR (n + 1 in- and out-offsets, the in-targets), in the order and
+// with the messages of every entry point that takes one (multi.cu)
+gb_status check_pr_host_csr(uint32_t n, const uint32_t* in_off, const uint32_t* in_tgt, const uint32_t* out_off);
+// The layouts of ranks 0 .. U-1 (U = devs.size() * V, rank r on devs[r / V]) of a host CSR that passed
+// check_pr_host_csr (multi.cu).  Part u of the split (pr_split.h, targets in chunks of about chunk_edges >= 1
+// edges) is uploaded by the device of rank u; the offsets are checked on the device.  A lone rank builds its
+// layout from its part as the chunks land; with several, every rank gathers the rows it owns from all parts into
+// a local in-CSR first.  On success plans holds U plans, the caller's to free; on failure nothing is left.
+gb_status pr_csr_plans(const std::vector<int>& devs, uint32_t V, uint32_t n, const uint32_t* in_off,
+                       const uint32_t* in_tgt, const uint32_t* out_off, uint64_t chunk_edges,
+                       std::vector<PrPlan*>* plans);
 // launch shapes of the sweep kernels, their error buffers and k_pr_cb's shared-memory size (pagerank.cu).
 // h_nrows / h_poff: the staircase (nrows[], poff[]) as the layout build holds it on the host.
 gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, const std::vector<uint32_t>& h_poff,

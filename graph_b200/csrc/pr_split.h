@@ -1,5 +1,5 @@
-// pr_split.h — how gb_page_rank_csr_multi_u32 / gb_pr_shards_csr_u32 cut a host in-CSR into parts, kept free of
-// CUDA so that it can be tested on the CPU.
+// pr_split.h — how gb_page_rank_csr_multi_u32 / gb_pr_shards_csr_u32 cut a host in-CSR into parts (and
+// gb_page_rank_csr_u32 into the chunks of its one part), kept free of CUDA so that it can be tested on the CPU.
 //
 // Part u of U takes the rows [R_u, R_{u+1}), R_0 = 0, R_U = n, where R_u is the first row whose offset reaches
 // floor(m u / U): cuts fall at rows, so a part holds at most about m / U edges plus one row, and a hub longer

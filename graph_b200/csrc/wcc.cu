@@ -322,11 +322,6 @@ constexpr uint32_t WCC_FEED_RING = 3;
 constexpr uint64_t WCC_FEED_EDGES = 1u << 22;  // C: 16 MiB per buffer (DESIGN.md §5)
 constexpr uint32_t WCC_MULTI_MAX_PARTS = 64;   // GB_WCC_MULTI_PARTS is clamped to [1, 64] parts per device
 
-static uint64_t env_u64(const char* name, uint64_t dflt) {
-  const char* s = std::getenv(name);
-  return s && *s ? std::strtoull(s, nullptr, 10) : dflt;
-}
-
 // the streams and events of one part; the streams are drained before they go
 struct WccFeed {
   cudaStream_t copy = nullptr, link = nullptr;
@@ -363,37 +358,20 @@ struct WccFeed {
 
 // One part of a one-shot WCC (wcc_split.h): the edges [e_begin, e_end) stream through the part's ring in
 // chunks of C edges (chunk k is [e_begin + kC, min(e_begin + (k + 1)C, e_end)), whatever rows it cuts) and
-// are linked into the part's own parent[n] on device dev.
-//
-// When there are several parts, another part may read this parent[] from another device.  cudaMalloc memory
-// is mapped into the peers by cudaDeviceEnablePeerAccess (gb_comm_init); blocks of the stream-ordered pool
-// that DevBuf draws from are not (a pool is reachable from its own device only unless cudaMemPoolSetAccess
-// says otherwise).  So the forest of one part among several is cudaMalloc'd, on one device as on many, and a
-// lone part (gb_wcc_csr_u32) keeps the pool's cached block.
+// are linked into the part's own forest parent[n] on device dev, which the other parts read when there are
+// several.
 struct WccPart {
   int dev = -1;
   WccPartRange range{};
   uint64_t C = 4, K = 0;  // chunk size in edges, chunks
   uint32_t R = 0;         // ring buffers in use
   unsigned int nbad[2] = {0, 0};
-  uint32_t* parent = nullptr;  // pooled.p or shared
-  uint32_t* shared = nullptr;  // cudaMalloc'd parent[] of one part among several
   WccFeed feed;  // outlives the buffers below, whose release waits for the device
-  DevBuf<uint32_t> off, pooled, ring[WCC_FEED_RING];
+  PeerBuf forest;  // parent[n]
+  DevBuf<uint32_t> off, ring[WCC_FEED_RING];
   DevBuf<unsigned int> bad;  // [0] rows whose offsets decrease, [1] targets >= n
-  gb_status alloc_parent(uint32_t n, bool peers_read) {
-    if (!peers_read) {
-      GB_TRY(pooled.alloc(n));
-      parent = pooled.p;
-      return GB_OK;
-    }
-    GB_CUDA(cudaMalloc(reinterpret_cast<void**>(&shared), (size_t)n * sizeof(uint32_t)));
-    parent = shared;
-    return GB_OK;
-  }
   ~WccPart() {
     if (dev >= 0) cudaSetDevice(dev);  // the members are released on the part's device
-    if (shared) cudaFree(shared);
   }
 };
 
@@ -450,7 +428,7 @@ static gb_status wcc_csr_parts(const std::vector<int>& devs, uint32_t per_dev, u
     GB_TRY(q.feed.create());
     const uint32_t rows = q.range.r_end - q.range.r_begin;
     GB_TRY(q.off.alloc((size_t)rows + 1));
-    GB_TRY(q.alloc_parent(n, P > 1));
+    GB_TRY(q.forest.alloc(n, P > 1));
     GB_TRY(q.bad.alloc(2));
     for (uint32_t r = 0; r < q.R; ++r) {
       GB_TRY(q.ring[r].alloc(q.C, 8));
@@ -483,7 +461,7 @@ static gb_status wcc_csr_parts(const std::vector<int>& devs, uint32_t per_dev, u
   uint64_t chunks = 0;
   for (auto& q : parts.v) {
     GB_CUDA(cudaSetDevice(q->dev));
-    k_cc_init<<<grid, blk, 0, q->feed.link>>>(q->parent, n);
+    k_cc_init<<<grid, blk, 0, q->feed.link>>>(q->forest.p, n);
     chunks = std::max(chunks, q->K);
   }
   for (uint64_t k = 0; k < chunks; ++k) {
@@ -496,13 +474,13 @@ static gb_status wcc_csr_parts(const std::vector<int>& devs, uint32_t per_dev, u
       GB_CUDA(cudaStreamWaitEvent(q.feed.link, q.feed.landed[k % q.R], 0));
       k_cc_link_edges<<<grid_for(len, LINK_TILE * (blk / 32)), blk, 0, q.feed.link>>>(
           q.off.p, q.range.r_end - q.range.r_begin, q.range.r_begin, q.ring[k % q.R].p, (uint32_t)e0,
-          (uint32_t)len, n, q.parent, q.bad.p + 1);
+          (uint32_t)len, n, q.forest.p, q.bad.p + 1);
       GB_CUDA(cudaEventRecord(q.feed.freed[k % q.R], q.feed.link));
     }
   }
   for (auto& q : parts.v) {
     GB_CUDA(cudaSetDevice(q->dev));
-    k_cc_compress<<<grid, blk, 0, q->feed.link>>>(q->parent, n);
+    k_cc_compress<<<grid, blk, 0, q->feed.link>>>(q->forest.p, n);
   }
   // a partner p + s never merges again after round s, so its forest is final when its event is recorded
   for (uint32_t s = 1; s < P; s *= 2) {
@@ -512,8 +490,8 @@ static gb_status wcc_csr_parts(const std::vector<int>& devs, uint32_t per_dev, u
       GB_CUDA(cudaEventRecord(b.feed.forest, b.feed.link));
       GB_CUDA(cudaSetDevice(a.dev));
       GB_CUDA(cudaStreamWaitEvent(a.feed.link, b.feed.forest, 0));
-      k_cc_merge_halving<<<grid, blk, 0, a.feed.link>>>(a.parent, b.parent, n);
-      k_cc_compress<<<grid, blk, 0, a.feed.link>>>(a.parent, n);
+      k_cc_merge_halving<<<grid, blk, 0, a.feed.link>>>(a.forest.p, b.forest.p, n);
+      k_cc_compress<<<grid, blk, 0, a.feed.link>>>(a.forest.p, n);
     }
   }
   GB_CUDA(cudaGetLastError());
@@ -529,7 +507,7 @@ static gb_status wcc_csr_parts(const std::vector<int>& devs, uint32_t per_dev, u
   GB_REQUIRE(nbad == 0, "CSR holds %u targets >= node_count %u", nbad, n);
   WccPart& root = *parts.v[0];
   GB_CUDA(cudaSetDevice(root.dev));
-  GB_CUDA(cudaMemcpyAsync(comp, root.parent, (size_t)n * 4, cudaMemcpyDeviceToHost, root.feed.link));
+  GB_CUDA(cudaMemcpyAsync(comp, root.forest.p, (size_t)n * 4, cudaMemcpyDeviceToHost, root.feed.link));
   GB_CUDA(cudaStreamSynchronize(root.feed.link));
   return GB_OK;
 }

@@ -3,7 +3,9 @@
 // exactly one part; each part's chunks tile its rows and its edges; every bound stays inside [0, m] and inside
 // its part, on malformed offsets too; and on monotone offsets the parts cut at rows, their edge ranges are the
 // rows' edges and tile [0, m], each part holds at most ceil(m / U) edges plus one row, and the cuts are the
-// first rows whose offsets reach floor(m u / U).
+// first rows whose offsets reach floor(m u / U).  The one-part split of gb_page_rank_csr_u32, cut into
+// ceil(m / c) edges per chunk, yields at most min(c, 4096) chunks.
+#include <algorithm>
 #include <cstdint>
 #include <cstdio>
 #include <random>
@@ -90,9 +92,23 @@ static std::vector<uint32_t> from_degrees(const std::vector<uint32_t>& deg) {
   return off;
 }
 
+// gb_page_rank_csr_u32's split: one part in chunks of ceil(m / c) edges (at least 1) for c chunks asked, which
+// must come out as at most min(c, 4096) chunks that tile [0, n] and [0, m]
+static void one_device(const char* name, const std::vector<uint32_t>& off) {
+  const uint32_t n = (uint32_t)off.size() - 1, parts = 1;
+  const uint64_t m = off[n];
+  for (uint64_t c : {1ull, 3ull, 7ull, 16ull, 5000ull}) {
+    const uint64_t chunk = std::max<uint64_t>((m + c - 1) / c, 1);
+    check(name, off, parts, chunk);
+    const size_t K = gb::pr_split(off.data(), n, parts, chunk)[0].chunk_row.size() - 1;
+    EXPECT(K <= std::min<uint64_t>(c, 4096), "%zu chunks for %llu asked", K, (unsigned long long)c);
+  }
+}
+
 static void all_parts(const char* name, const std::vector<uint32_t>& off) {
   for (uint64_t chunk : {1ull, 3ull, 64ull, 1ull << 23})
     for (uint32_t parts = 1; parts <= 8; ++parts) check(name, off, parts, chunk);
+  one_device(name, off);
 }
 
 int main() {

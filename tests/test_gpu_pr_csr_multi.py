@@ -233,6 +233,17 @@ def part_rows(off, parts):
 
 
 def test_errors_match_single_device_call(gb, comm):
+    check_errors_match_single_device_call(comm)
+
+
+def test_errors_match_streamed_single_device_call(gb, comm, monkeypatch):
+    """rmat16 is below GB_PR_FEED_MIN_EDGES: lowered to 0, gb_page_rank_csr_u32 streams its targets in as it does
+    from 2^22 edges up, and must reject every malformed input as the communicator calls do"""
+    monkeypatch.setenv("GB_PR_FEED_MIN_EDGES", "0")
+    check_errors_match_single_device_call(comm)
+
+
+def check_errors_match_single_device_call(comm):
     n, out, inc = rmat16()
     io, it, oo = inc[0], inc[1], out[0]
     U = 4
