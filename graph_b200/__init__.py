@@ -21,7 +21,8 @@ from ._capi import GraphB200Error, check, lib
 
 __all__ = ["DiGraph", "Graph", "Layout", "FileFormat", "PageRankResult", "WccResult",
            "TriangleCountResult", "SsspResult", "PageRankConfig", "WccConfig", "DeltaSteppingConfig",
-           "GraphB200Error", "device_count", "set_device", "write_graph500", "wcc_csr"]
+           "GraphB200Error", "device_count", "set_device", "write_graph500", "wcc_csr",
+           "triangle_count_csr"]
 
 _device = 0
 
@@ -214,8 +215,9 @@ class WccResult:
 
 
 class TriangleCountResult:
-    def __init__(self, triangles, micros):
+    def __init__(self, triangles, micros, info=None):
         self.triangles, self.micros = triangles, micros
+        self.info = info  # triangle_count_csr: the call's gb_tc_csr_info as a dict
 
     def __repr__(self):
         return f"TriangleCountResult {{ triangles: {self.triangles}, took: {_took(self.micros)} }}"
@@ -744,13 +746,19 @@ def _page_rank_csr_arrays(in_offsets, in_targets, out_offsets, what: str):
     return io, it, oo
 
 
-def _wcc_csr_call(fn, first, offsets, targets, chunk_size, neighbor_rounds, sampling_size, out) -> WccResult:
-    """fn(first, node_count, offsets, targets, &config, components): gb_wcc_csr_u32 or gb_wcc_csr_multi_u32."""
+def _host_csr_arrays(offsets, targets, what: str, kind: str):
+    """The host arrays of a one-shot call as given: contiguous uint32 (pinned arrays stay pinned)."""
     off, tgt = np.asarray(offsets), np.asarray(targets)
     for a in (off, tgt):
         if a.dtype != np.uint32 or not a.flags.c_contiguous:
-            raise TypeError("wcc_csr needs contiguous uint32 arrays")
-    _check_host_csr(off, tgt, "out")
+            raise TypeError(f"{what} needs contiguous uint32 arrays")
+    _check_host_csr(off, tgt, kind)
+    return off, tgt
+
+
+def _wcc_csr_call(fn, first, offsets, targets, chunk_size, neighbor_rounds, sampling_size, out) -> WccResult:
+    """fn(first, node_count, offsets, targets, &config, components): gb_wcc_csr_u32 or gb_wcc_csr_multi_u32."""
+    off, tgt = _host_csr_arrays(offsets, targets, "wcc_csr", "out")
     cfg = _capi.WccConfig(int(chunk_size), int(neighbor_rounds), int(sampling_size))
     if out is None:
         comp = np.empty(len(off) - 1, np.uint32)
@@ -778,3 +786,22 @@ def wcc_csr(offsets, targets, *, chunk_size: int = WccConfig.DEFAULT_CHUNK_SIZE,
     the labels instead of a new array; it is left untouched when the call fails."""
     return _wcc_csr_call(lib.gb_wcc_csr_u32, _device, offsets, targets, chunk_size, neighbor_rounds,
                          sampling_size, out)
+
+
+def triangle_count_csr(offsets, targets) -> TriangleCountResult:
+    """global_triangle_count (triangle_count.rs:22-86) of a host undirected CSR without a resident twin: the
+    number Graph.from_csr(offsets, targets).global_triangle_count() gives, rows in any order.  The offsets are
+    uploaded first, the targets in row-aligned chunks, and each chunk is checked and counted as soon as its rows
+    are on the device while the next ones are on the bus; the CSR is freed before the call returns.  Arrays are
+    used as given: pass pinned contiguous uint32 arrays to overlap the counts with the copy.  `info` on the
+    result holds the call's chunk count, h2d bytes, chunks per kernel path and device times."""
+    off, tgt = _host_csr_arrays(offsets, targets, "triangle_count_csr", "undirected")
+    tri = C.c_uint64(0)
+
+    def go():
+        check(lib.gb_triangle_count_csr_u32(_device, len(off) - 1, _ptr(off), _ptr(tgt) if len(tgt) else None,
+                                            C.byref(tri)))
+    _, micros = _timed(go)
+    info = _capi.TcCsrInfo()
+    check(lib.gb_triangle_count_csr_info(C.byref(info)))
+    return TriangleCountResult(int(tri.value), micros, info.as_dict())

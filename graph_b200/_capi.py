@@ -72,6 +72,16 @@ class LoadInfo(C.Structure):
         return {k: int(getattr(self, k)) for k, _ in self._fields_}
 
 
+class TcCsrInfo(C.Structure):
+    _fields_ = [("chunks", C.c_uint64), ("chunk_entries", C.c_uint64), ("h2d_bytes", C.c_uint64),
+                ("sorted_chunks", C.c_uint64), ("list_chunks", C.c_uint64), ("first_list_chunk", C.c_uint64),
+                ("kernel_launches", C.c_uint64), ("pinned", C.c_uint32), ("reserved", C.c_uint32),
+                ("upload_ms", C.c_double), ("total_ms", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_ if k != "reserved"}
+
+
 class GraphB200Error(RuntimeError):
     """CUDA / allocation failure inside libgraph_b200."""
 
@@ -129,6 +139,8 @@ SIGNATURES = {
     "gb_sssp": (C.c_int, [_P, C.POINTER(SsspConfig), _P]),
     "gb_sssp_device": (C.c_int, [_P, C.POINTER(SsspConfig), _P]),
     "gb_triangle_count": (C.c_int, [_P, C.POINTER(C.c_uint64)]),
+    "gb_triangle_count_csr_u32": (C.c_int, [C.c_int, C.c_uint32, _P, _P, C.POINTER(C.c_uint64)]),
+    "gb_triangle_count_csr_info": (C.c_int, [C.POINTER(TcCsrInfo)]),
     "gb_in_degree_partition": (C.c_int, [_P, C.c_uint32, _P]),
     "gb_page_rank_plan_info": (C.c_int, [_P, C.POINTER(PrShardStats)]),
     "gb_page_rank_plan_shape": (C.c_int, [_P, C.POINTER(PrPlanShape)]),

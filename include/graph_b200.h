@@ -340,6 +340,39 @@ gb_status gb_sssp_device(const gb_graph* graph, const gb_sssp_config* config, fl
  * sorted (an Unsorted build, gb_graph_from_csr_u32) checks them once and caches the answer. */
 gb_status gb_triangle_count(const gb_graph* graph, uint64_t* triangles);
 
+/* global_triangle_count (triangle_count.rs:22-86) of a HOST undirected CSR, with no twin kept: the number
+ * gb_graph_from_csr_u32 + gb_triangle_count give for the same arrays, with the same checks and messages
+ * (on unsorted rows, the reference's list-order number).  Layout rule: offsets has node_count + 1 entries
+ * from 0, targets offsets[node_count] (may be NULL when that is 0); the rows are taken as they are, in any
+ * order.  Each term of the sum is one entry (u, v <= u) and reads rows u and v only, so the call is causal
+ * in row order: the offsets go first, the targets follow in row-aligned chunks of about equal entry counts
+ * (a row longer than a chunk gets one of its own), and every chunk is checked (targets < node_count, row
+ * order) and counted as soon as its rows have landed, while the next chunks are on the bus.  Chunks count
+ * with the sorted-row kernel while every row so far is sorted, and with the list-order kernels from the
+ * first chunk with an unsorted row on.  Residency: the terms read earlier rows at random, so unlike
+ * gb_wcc_csr_u32's ring the whole CSR (4(n+1) + 4m bytes) is on the device by the end of the call; it is
+ * freed before the call returns.  Pass page-locked targets to get the overlap: all chunks then go out at
+ * once on a copy stream; from pageable memory the copies are synchronous, one chunk ahead of the count,
+ * and the result is the same.  GB_TC_FEED_ENTRIES (environment, read per call) sets the entries per chunk
+ * (default ceil(m / 16), at least 2^20; never fewer than m / 4096). */
+gb_status gb_triangle_count_csr_u32(int device, uint32_t node_count, const uint32_t* offsets,
+                                    const uint32_t* targets, uint64_t* triangles);
+/* Statistics of the calling thread's last gb_triangle_count_csr_u32 (all zero after a failed call). */
+typedef struct gb_tc_csr_info {
+  uint64_t chunks;           /* row-aligned chunks the targets were uploaded and counted in */
+  uint64_t chunk_entries;    /* the entry budget of a chunk */
+  uint64_t h2d_bytes;        /* bytes copied host -> device: 4(n+1) + 4m */
+  uint64_t sorted_chunks;    /* chunks counted by the sorted-row kernel (k_tc) */
+  uint64_t list_chunks;      /* chunks counted by the list-order kernels (k_tc_cut + k_tc_list) */
+  uint64_t first_list_chunk; /* the first of those; == chunks when every row is sorted */
+  uint64_t kernel_launches;  /* checks and counts */
+  uint32_t pinned;           /* 1: the targets were page-locked */
+  uint32_t reserved;
+  double upload_ms;          /* CUDA-event time from the first copy to the last target landing */
+  double total_ms;           /* CUDA-event time from the first copy to the end of the last count */
+} gb_tc_csr_info;
+gb_status gb_triangle_count_csr_info(gb_tc_csr_info* info);
+
 /* ---- PageRank layout statistics / multi-GPU shard (1-D edge-cut by destination) -----------------
  * The JACOBI path renumbers vertices internally (in-degree descending, then out-degree descending)
  * and column-blocks the sweep (graph_b200/csrc/pagerank.cu).  For N GPUs (one process per GPU;

@@ -302,6 +302,15 @@ inline Components wcc_baseline_csr(std::uint32_t node_count, const std::uint32_t
   detail::check(gb_wcc_csr_u32(device, node_count, offsets, targets, &cfg, out.ids.data()));
   return out;
 }
+// global_triangle_count of a host undirected CSR (same layout), streamed to the device in row-aligned chunks and
+// counted as they land, without a resident twin (gb_triangle_count_csr_u32); the number global_triangle_count
+// gives on UndirectedCsrGraph::from_csr of the same arrays
+inline std::uint64_t global_triangle_count_csr(std::uint32_t node_count, const std::uint32_t* offsets,
+                                               const std::uint32_t* targets, int device = 0) {
+  std::uint64_t t = 0;
+  detail::check(gb_triangle_count_csr_u32(device, node_count, offsets, targets, &t));
+  return t;
+}
 
 // delta_stepping(&graph, config) -> Vec<AtomicF32>             sssp.rs:38
 inline std::vector<float> delta_stepping(const DirectedCsrGraph& g, DeltaSteppingConfig c) {
