@@ -143,6 +143,50 @@ struct PeerBuf {
   ~PeerBuf() { release(); }
 };
 
+// ---- one device's feed of a slice of a host CSR (graph.cu; csr_split.h cuts the slices) -------------------
+// The offsets [r_begin, r_end] of a host CSR, and with them the same rows of a second offsets array when the
+// caller has one, go to device dev on the feed's own copy stream, with offsets_in recorded behind them.  The
+// targets [e_begin, e_end) follow chunk by chunk, each with an event behind it, either resident (each chunk at
+// its place in tgt, one landed event per chunk) or through a ring of R slots (chunk k in slot k mod R, one
+// landed and one freed event per slot).  A ring consumer records freed[k mod R] behind its last read of chunk k,
+// and must enqueue that record before send(k + R) is called: cudaStreamWaitEvent takes the event's latest
+// record at the time of the call, so every wait then refers to a record already enqueued, and a pageable copy,
+// which returns only once its stream has drained, blocks the host only until work already enqueued has run.
+// The consumers' streams are the caller's, and must drain before the feed goes.
+struct CsrFeed {
+  int dev = -1;
+  uint32_t r_begin = 0, r_end = 0;
+  uint64_t e_begin = 0;
+  cudaStream_t copy = nullptr;
+  cudaEvent_t offsets_in = nullptr;
+  PeerBuf off, off2;                      // [r_end - r_begin + 1] each; off2 only with a second offsets array
+  PeerBuf tgt;                            // resident: [e_end - e_begin] + 8 zeroed
+  std::vector<DevBuf<uint32_t>> ring;     // ring: R slots of `slot` entries + 8 zeroed
+  std::vector<cudaEvent_t> landed, freed; // resident: landed[K]; ring: landed[R], freed[R]
+
+  // makes dev current, creates the stream and offsets_in and allocates the offsets (peers: PeerBuf)
+  gb_status open(int device, uint32_t rb, uint32_t re, bool peers, bool two_offsets = false);
+  gb_status resident(uint64_t eb, uint64_t ee, uint32_t chunks, bool peers);
+  gb_status open_ring(uint32_t slots, uint64_t slot);
+  // copies off[r_begin .. r_end] (and off2's) and records offsets_in
+  gb_status send_offsets(const uint32_t* host_off, const uint32_t* host_off2 = nullptr);
+  // chunk k = the targets [e0, e0 + len) of host_tgt; an empty chunk only records its event
+  gb_status send(uint64_t k, const uint32_t* host_tgt, uint64_t e0, uint64_t len);
+  // on s, behind offsets_in: bad[0] += the rows v in [r0, r1) with off[v] > off[v + 1], bad[1] the same of off2
+  gb_status check_monotone(cudaStream_t s, uint32_t r0, uint32_t r1, unsigned int* bad) const;
+  // whether host memory is page-locked: such a copy does not wait for its stream to drain
+  static bool pinned(const void* host);
+  ~CsrFeed();
+};
+
+// The O(1) host checks of a host CSR, in this order: offsets NULL, offsets[0] == 0, then targets NULL when it
+// has entries (not with offsets_only).  Messages begin with `what` ("in", "out", "undirected"; "" for none).
+gb_status require_host_csr(uint32_t n, const uint32_t* off, const uint32_t* tgt, const char* what,
+                           bool offsets_only = false);
+// The verdicts of the device checks on their summed counts: GB_OK when it is 0, else the failure
+gb_status require_monotone(const char* what, uint64_t bad_rows);
+gb_status require_ids(const char* what, uint64_t bad_targets, uint32_t n);
+
 // an unsigned decimal knob from the environment (experiments); dflt when it is unset or empty
 inline uint64_t env_u64(const char* name, uint64_t dflt) {
   const char* e = getenv(name);
@@ -235,9 +279,9 @@ gb_status check_layout(gb_layout layout);
 gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, const uint32_t* d_cols,
                            const float* d_w, uint64_t count, gb_layout layout, DevCsr* csr);
 gb_status new_graph(int device, gb_graph_kind kind, uint32_t n, GraphPtr* out);
-// Uploads a host CSR on stream s and checks it: offsets[0] == 0 on the host, the offsets monotone and the
-// targets below n on the device.  offsets_only uploads the offsets alone (degrees); otherwise tgt must
-// be non-NULL when the CSR has entries, and w may be NULL.  Returns with s synchronised.
+// Uploads a host CSR on stream s and checks it: require_host_csr on the host, the offsets monotone and the
+// targets below n on the device.  offsets_only uploads the offsets alone (degrees); w may be NULL.  Returns
+// with s synchronised.
 gb_status upload_host_csr(cudaStream_t s, uint32_t n, const uint32_t* off, const uint32_t* tgt, const float* w,
                           DevCsr* csr, const char* what, bool offsets_only = false);
 // enqueue on s: *bad += the number of ids in a[0, count) that are >= n

@@ -336,14 +336,113 @@ void check_monotone_async(cudaStream_t s, const uint32_t* off, uint32_t n, unsig
   k_check_monotone<<<grid_for(n, 256), 256, 0, s>>>(off, n, bad);
 }
 
+// `what` and the space after it, or nothing
+#define GB_WHAT(what) (what), (*(what) ? " " : "")
+
+gb_status require_host_csr(uint32_t n, const uint32_t* off, const uint32_t* tgt, const char* what,
+                           bool offsets_only) {
+  GB_REQUIRE(off != nullptr, "%s%soffsets is NULL", GB_WHAT(what));
+  GB_REQUIRE(off[0] == 0, "%s%soffsets[0] must be 0", GB_WHAT(what));
+  GB_REQUIRE(offsets_only || off[n] == 0 || tgt != nullptr, "%s%stargets is NULL", GB_WHAT(what));
+  return GB_OK;
+}
+
+gb_status require_monotone(const char* what, uint64_t bad_rows) {
+  if (!bad_rows) return GB_OK;
+  return fail(GB_ERR_INVALID, "%s%soffsets are not monotone (%llu rows)", GB_WHAT(what), (unsigned long long)bad_rows);
+}
+
+gb_status require_ids(const char* what, uint64_t bad_targets, uint32_t n) {
+  if (!bad_targets) return GB_OK;
+  return fail(GB_ERR_INVALID, "%s%sCSR holds %llu targets >= node_count %u", GB_WHAT(what),
+              (unsigned long long)bad_targets, n);
+}
+
+gb_status CsrFeed::open(int device, uint32_t rb, uint32_t re, bool peers, bool two_offsets) {
+  dev = device;
+  r_begin = rb;
+  r_end = re;
+  GB_CUDA(cudaSetDevice(dev));
+  GB_CUDA(cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking));
+  GB_CUDA(cudaEventCreateWithFlags(&offsets_in, cudaEventDisableTiming));
+  GB_TRY(off.alloc((size_t)(re - rb) + 1, peers));
+  if (two_offsets) GB_TRY(off2.alloc((size_t)(re - rb) + 1, peers));
+  return GB_OK;
+}
+
+gb_status CsrFeed::resident(uint64_t eb, uint64_t ee, uint32_t chunks, bool peers) {
+  e_begin = eb;
+  GB_TRY(tgt.alloc(ee - eb, peers, 8));
+  GB_CUDA(cudaMemsetAsync(tgt.p + (ee - eb), 0, 8 * 4, copy));
+  landed.assign(chunks, nullptr);
+  for (cudaEvent_t& ev : landed) GB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  return GB_OK;
+}
+
+gb_status CsrFeed::open_ring(uint32_t slots, uint64_t slot) {
+  ring.resize(slots);
+  landed.assign(slots, nullptr);
+  freed.assign(slots, nullptr);
+  for (uint32_t i = 0; i < slots; ++i) {
+    GB_TRY(ring[i].alloc(slot, 8));
+    GB_CUDA(cudaMemsetAsync(ring[i].p + slot, 0, 8 * 4, copy));
+    GB_CUDA(cudaEventCreateWithFlags(&landed[i], cudaEventDisableTiming));
+    GB_CUDA(cudaEventCreateWithFlags(&freed[i], cudaEventDisableTiming));
+  }
+  return GB_OK;
+}
+
+gb_status CsrFeed::send_offsets(const uint32_t* host_off, const uint32_t* host_off2) {
+  const size_t bytes = ((size_t)(r_end - r_begin) + 1) * 4;
+  GB_CUDA(cudaMemcpyAsync(off.p, host_off + r_begin, bytes, cudaMemcpyHostToDevice, copy));
+  if (host_off2) GB_CUDA(cudaMemcpyAsync(off2.p, host_off2 + r_begin, bytes, cudaMemcpyHostToDevice, copy));
+  GB_CUDA(cudaEventRecord(offsets_in, copy));
+  return GB_OK;
+}
+
+gb_status CsrFeed::send(uint64_t k, const uint32_t* host_tgt, uint64_t e0, uint64_t len) {
+  uint32_t* dst = ring.empty() ? tgt.p + (e0 - e_begin) : ring[k % ring.size()].p;
+  if (!ring.empty() && k >= ring.size()) GB_CUDA(cudaStreamWaitEvent(copy, freed[k % ring.size()], 0));
+  if (len) GB_CUDA(cudaMemcpyAsync(dst, host_tgt + e0, len * 4, cudaMemcpyHostToDevice, copy));
+  GB_CUDA(cudaEventRecord(landed[k % landed.size()], copy));
+  return GB_OK;
+}
+
+gb_status CsrFeed::check_monotone(cudaStream_t s, uint32_t r0, uint32_t r1, unsigned int* bad) const {
+  GB_CUDA(cudaStreamWaitEvent(s, offsets_in, 0));
+  check_monotone_async(s, off.p + (r0 - r_begin), r1 - r0, bad);
+  if (off2.p) check_monotone_async(s, off2.p + (r0 - r_begin), r1 - r0, bad + 1);
+  return GB_OK;
+}
+
+bool CsrFeed::pinned(const void* host) {
+  cudaPointerAttributes a{};
+  if (cudaPointerGetAttributes(&a, host) == cudaSuccess) return a.type == cudaMemoryTypeHost;
+  cudaGetLastError();
+  return false;
+}
+
+CsrFeed::~CsrFeed() {
+  if (dev < 0) return;
+  cudaSetDevice(dev);
+  if (copy) cudaStreamSynchronize(copy);
+  ring.clear();
+  tgt.release();
+  off2.release();
+  off.release();
+  for (const std::vector<cudaEvent_t>* events : {&landed, &freed})
+    for (cudaEvent_t ev : *events)
+      if (ev) cudaEventDestroy(ev);
+  if (offsets_in) cudaEventDestroy(offsets_in);
+  if (copy) cudaStreamDestroy(copy);
+}
+
 // Only O(1) checks read the host arrays; the O(n + m) ones run on the device after the upload, so that a
 // billion-edge twin is not validated by one CPU thread.
 gb_status upload_host_csr(cudaStream_t s, uint32_t n, const uint32_t* off, const uint32_t* tgt, const float* w,
                           DevCsr* csr, const char* what, bool offsets_only) {
-  GB_REQUIRE(off != nullptr, "%s offsets is NULL", what);
-  GB_REQUIRE(off[0] == 0, "%s offsets[0] must be 0", what);
+  GB_TRY(require_host_csr(n, off, tgt, what, offsets_only));
   const uint64_t len = off[n];
-  GB_REQUIRE(offsets_only || len == 0 || tgt != nullptr, "%s targets is NULL", what);
   DevBuf<unsigned int> bad;  // [0] targets >= n, [1] rows whose offsets decrease
   GB_TRY(bad.alloc(2));
   GB_CUDA(cudaMemsetAsync(bad.p, 0, 8, s));
@@ -364,9 +463,8 @@ gb_status upload_host_csr(cudaStream_t s, uint32_t n, const uint32_t* off, const
   unsigned int nbad[2] = {0, 0};
   GB_CUDA(cudaMemcpyAsync(nbad, bad.p, 8, cudaMemcpyDeviceToHost, s));
   GB_CUDA(cudaStreamSynchronize(s));
-  GB_REQUIRE(nbad[1] == 0, "%s offsets are not monotone (%u rows)", what, nbad[1]);
-  GB_REQUIRE(nbad[0] == 0, "%s CSR holds %u targets >= node_count %u", what, nbad[0], n);
-  return GB_OK;
+  GB_TRY(require_monotone(what, nbad[1]));
+  return require_ids(what, nbad[0], n);
 }
 
 // builds a directed or undirected graph's CSRs from DEVICE edge arrays

@@ -194,9 +194,9 @@ gb_status gb_binary_decode(const void* bytes, uint64_t len, gb_graph_kind kind, 
     for (unsigned t = 0; t < T; ++t) big += big_t[t], wide |= wide_t[t] != 0;
     GB_REQUIRE(!wide, "binary graph file: %s holds an id or offset that does not fit 32 bits", what);
     GB_REQUIRE(off[0] == 0, "%s offsets[0] must be 0", what);
-    GB_REQUIRE(decreasing == 0, "%s offsets are not monotone (%llu rows)", what, (unsigned long long)decreasing);
+    GB_TRY(gb::require_monotone(what, decreasing));
     GB_REQUIRE(off[n] == m, "%s offsets end at %u, not at its %llu entries", what, off[n], (unsigned long long)m);
-    GB_REQUIRE(big == 0, "%s CSR holds %llu targets >= node_count %u", what, (unsigned long long)big, l.n);
+    GB_TRY(gb::require_ids(what, big, l.n));
   }
   return GB_OK;
 }

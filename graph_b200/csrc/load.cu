@@ -693,10 +693,10 @@ static gb_status check_loaded_csrs(gb_graph* g, const BinLayout& l, DevCsr* cons
   for (unsigned c = 0; c < l.ncsr; ++c) {
     const char* what = bin_csr_name(l, c);
     GB_REQUIRE(e[2 * c] == 0, "%s offsets[0] must be 0", what);
-    GB_REQUIRE(h[2 * c + 1] == 0, "%s offsets are not monotone (%u rows)", what, h[2 * c + 1]);
+    GB_TRY(require_monotone(what, h[2 * c + 1]));
     GB_REQUIRE(e[2 * c + 1] == l.entries, "%s offsets end at %u, not at its %llu entries", what, e[2 * c + 1],
                (unsigned long long)l.entries);
-    GB_REQUIRE(h[2 * c] == 0, "%s CSR holds %u targets >= node_count %u", what, h[2 * c], g->n);
+    GB_TRY(require_ids(what, h[2 * c], g->n));
   }
   return GB_OK;
 }

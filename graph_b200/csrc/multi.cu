@@ -18,7 +18,6 @@
 #include <cub/cub.cuh>
 
 #include "pr_plan.cuh"
-#include "pr_split.h"
 
 struct gb_comm {
   std::vector<int> devs;
@@ -413,24 +412,12 @@ struct PrCsrRank {
   }
 };
 
-// Every rank's stream drains before any part goes: the gathers and a lone rank's layout read the parts
-struct PrCsrRun {
-  std::vector<std::unique_ptr<PrCsrPart>> parts;
-  std::vector<std::unique_ptr<PrCsrRank>> ranks;
-  ~PrCsrRun() {
-    ranks.clear();
-    parts.clear();
-  }
-};
-
 gb_status check_pr_host_csr(uint32_t n, const uint32_t* in_off, const uint32_t* in_tgt, const uint32_t* out_off) {
   GB_REQUIRE(n > 0, "node_count must be > 0");
   GB_REQUIRE(in_off && out_off, "offset arrays are NULL");
   GB_REQUIRE(in_off[n] == out_off[n], "in and out offsets disagree on the edge count");
-  GB_REQUIRE(in_off[0] == 0, "in offsets[0] must be 0");
-  GB_REQUIRE(in_off[n] == 0 || in_tgt != nullptr, "in targets is NULL");
-  GB_REQUIRE(out_off[0] == 0, "out offsets[0] must be 0");
-  return GB_OK;
+  GB_TRY(require_host_csr(n, in_off, in_tgt, "in"));
+  return require_host_csr(n, out_off, nullptr, "out", true);
 }
 
 gb_status pr_csr_plans(const std::vector<int>& devs, uint32_t V, uint32_t n, const uint32_t* in_off,
@@ -441,95 +428,77 @@ gb_status pr_csr_plans(const std::vector<int>& devs, uint32_t V, uint32_t n, con
   const bool peers = U > 1;
   const std::vector<PrPart> split = pr_split(in_off, n, U, chunk_edges);
   DeviceGuard guard(devs[0]);
-  PrCsrRun run;
-  // 1. every part's offsets, then its targets chunk by chunk, round robin over the parts: the copies go out
-  // before the host waits for any check, so every bus is busy from the start.  The targets keep 8 zeroed
-  // entries of slack, as a resident in-CSR does (DevCsr).
-  size_t max_chunks = 0;
+  // declared after the parts, the ranks go first on any return, and each drains its stream as it goes: the
+  // gathers and a lone rank's layout read the parts
+  std::vector<std::unique_ptr<CsrFeed>> parts;
+  std::vector<std::unique_ptr<PrCsrRank>> ranks;
+  // 1. every part's in and out offsets, then its targets chunk by chunk, round robin over the parts: the copies go
+  // out before the host waits for any check, so every bus is busy from the start
+  uint32_t max_chunks = 0;
   for (uint32_t u = 0; u < U; ++u) {
-    run.parts.emplace_back(new (std::nothrow) PrCsrPart());
-    GB_REQUIRE(run.parts.back() != nullptr, "host allocation failed");
-    PrCsrPart& q = *run.parts.back();
-    q.dev = devs[u / V];
-    q.range = split[u];
-    GB_CUDA(cudaSetDevice(q.dev));
-    GB_CUDA(cudaStreamCreateWithFlags(&q.copy, cudaStreamNonBlocking));
-    GB_CUDA(cudaEventCreateWithFlags(&q.offsets_in, cudaEventDisableTiming));
-    const size_t rows = q.range.r_end - q.range.r_begin, len = q.range.e_end - q.range.e_begin;
-    GB_TRY(q.in_off.alloc(rows + 1, peers));
-    GB_TRY(q.out_off.alloc(rows + 1, peers));
-    GB_TRY(q.tgt.alloc(len, peers, 8));
-    GB_CUDA(cudaMemcpyAsync(q.in_off.p, in_off + q.range.r_begin, (rows + 1) * 4, cudaMemcpyHostToDevice, q.copy));
-    GB_CUDA(cudaMemcpyAsync(q.out_off.p, out_off + q.range.r_begin, (rows + 1) * 4, cudaMemcpyHostToDevice, q.copy));
-    GB_CUDA(cudaEventRecord(q.offsets_in, q.copy));
-    GB_CUDA(cudaMemsetAsync(q.tgt.p + len, 0, 8 * 4, q.copy));
-    max_chunks = std::max(max_chunks, q.range.chunk_row.size() - 1);
+    parts.emplace_back(new (std::nothrow) CsrFeed());
+    GB_REQUIRE(parts.back() != nullptr, "host allocation failed");
+    CsrFeed& q = *parts.back();
+    GB_TRY(q.open(devs[u / V], split[u].r_begin, split[u].r_end, peers, true));
+    GB_TRY(q.resident(split[u].e_begin, split[u].e_end, split[u].chunks.count(), peers));
+    GB_TRY(q.send_offsets(in_off, out_off));
+    max_chunks = std::max(max_chunks, split[u].chunks.count());
   }
-  for (size_t k = 0; k < max_chunks; ++k)
-    for (auto& qp : run.parts) {
-      PrCsrPart& q = *qp;
-      if (k + 1 >= q.range.chunk_edge.size()) continue;
-      GB_CUDA(cudaSetDevice(q.dev));
-      const uint64_t e0 = q.range.chunk_edge[k], e1 = q.range.chunk_edge[k + 1];
-      if (e1 > e0)
-        GB_CUDA(cudaMemcpyAsync(q.tgt.p + (e0 - q.range.e_begin), in_tgt + e0, (e1 - e0) * 4, cudaMemcpyHostToDevice,
-                                q.copy));
-      cudaEvent_t ev = nullptr;
-      GB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-      q.landed.push_back(ev);
-      GB_CUDA(cudaEventRecord(ev, q.copy));
+  for (uint32_t k = 0; k < max_chunks; ++k)
+    for (uint32_t u = 0; u < U; ++u) {
+      const CsrChunks& ch = split[u].chunks;
+      if (k >= ch.count()) continue;
+      GB_CUDA(cudaSetDevice(parts[u]->dev));
+      GB_TRY(parts[u]->send(k, in_tgt, ch.edge[k], ch.edge[k + 1] - ch.edge[k]));
     }
   // 2. rank u checks part u's rows (the slices tile [0, n]: every row once, whatever the host arrays hold), and
   // with several ranks every rank assembles the full offsets from the parts
   for (uint32_t r = 0; r < U; ++r) {
-    run.ranks.emplace_back(new (std::nothrow) PrCsrRank());
-    GB_REQUIRE(run.ranks.back() != nullptr, "host allocation failed");
-    PrCsrRank& k = *run.ranks.back();
+    ranks.emplace_back(new (std::nothrow) PrCsrRank());
+    GB_REQUIRE(ranks.back() != nullptr, "host allocation failed");
+    PrCsrRank& k = *ranks.back();
     k.dev = devs[r / V];
     GB_CUDA(cudaSetDevice(k.dev));
     GB_CUDA(cudaStreamCreateWithFlags(&k.s, cudaStreamNonBlocking));
     GB_TRY(k.bad.alloc(3));
     GB_CUDA(cudaMemsetAsync(k.bad.p, 0, 12, k.s));
-    const PrCsrPart& own = *run.parts[r];
-    const uint32_t rows = own.range.r_end - own.range.r_begin;
-    GB_CUDA(cudaStreamWaitEvent(k.s, own.offsets_in, 0));
-    check_monotone_async(k.s, own.in_off.p, rows, k.bad.p);
-    check_monotone_async(k.s, own.out_off.p, rows, k.bad.p + 1);
+    GB_TRY(parts[r]->check_monotone(k.s, split[r].r_begin, split[r].r_end, k.bad.p));
     GB_CUDA(cudaMemcpyAsync(k.h_bad, k.bad.p, 8, cudaMemcpyDeviceToHost, k.s));
     if (!peers) continue;
     GB_TRY(k.in_off.alloc((size_t)n + 1, peers));
     GB_TRY(k.out_off.alloc((size_t)n + 1, peers));
     for (uint32_t u = 0; u < U; ++u) {
-      const PrCsrPart& q = *run.parts[u];
-      const size_t count = (size_t)(q.range.r_end - q.range.r_begin) + (u + 1 == U ? 1 : 0);
+      const CsrFeed& q = *parts[u];
+      const size_t count = (size_t)(q.r_end - q.r_begin) + (u + 1 == U ? 1 : 0);
       if (!count) continue;
       GB_CUDA(cudaStreamWaitEvent(k.s, q.offsets_in, 0));
-      GB_CUDA(cudaMemcpyPeerAsync(k.in_off.p + q.range.r_begin, k.dev, q.in_off.p, q.dev, count * 4, k.s));
-      GB_CUDA(cudaMemcpyPeerAsync(k.out_off.p + q.range.r_begin, k.dev, q.out_off.p, q.dev, count * 4, k.s));
+      GB_CUDA(cudaMemcpyPeerAsync(k.in_off.p + q.r_begin, k.dev, q.off.p, q.dev, count * 4, k.s));
+      GB_CUDA(cudaMemcpyPeerAsync(k.out_off.p + q.r_begin, k.dev, q.off2.p, q.dev, count * 4, k.s));
     }
   }
   unsigned int nbad[2] = {0, 0};
-  for (auto& k : run.ranks) {
+  for (auto& k : ranks) {
     GB_CUDA(cudaSetDevice(k->dev));
     GB_CUDA(cudaStreamSynchronize(k->s));
     nbad[0] += k->h_bad[0];
     nbad[1] += k->h_bad[1];
   }
-  GB_REQUIRE(nbad[0] == 0, "in offsets are not monotone (%u rows)", nbad[0]);
-  GB_REQUIRE(nbad[1] == 0, "out offsets are not monotone (%u rows)", nbad[1]);
+  GB_TRY(require_monotone("in", nbad[0]));
+  GB_TRY(require_monotone("out", nbad[1]));
   // 3. order stage.  A lone rank owns every row: its part is its in-CSR, whose chunks the layout build checks
   // and classifies as they land.  Otherwise the local offsets, and the gathers of every chunk as it lands.
   for (uint32_t r = 0; r < U; ++r) {
-    PrCsrRank& k = *run.ranks[r];
+    PrCsrRank& k = *ranks[r];
     GB_CUDA(cudaSetDevice(k.dev));
     PrSource src;
     src.device = k.dev;
     src.stream = k.s;
     src.n = n;
     src.m = m;
-    src.in_off = peers ? k.in_off.p : run.parts[0]->in_off.p;
-    src.out_off = peers ? k.out_off.p : run.parts[0]->out_off.p;
-    src.feed = peers ? nullptr : run.parts[0].get();
+    src.in_off = peers ? k.in_off.p : parts[0]->off.p;
+    src.out_off = peers ? k.out_off.p : parts[0]->off2.p;
+    src.feed = peers ? nullptr : parts[0].get();
+    src.chunks = peers ? nullptr : &split[0].chunks;
     PrDeal deal;
     deal.P = U;
     deal.p = r;
@@ -537,7 +506,7 @@ gb_status pr_csr_plans(const std::vector<int>& devs, uint32_t V, uint32_t n, con
     if (!peers) {
       LayoutBuild* b = k.build;
       k.build = nullptr;
-      GB_TRY(layout_end(b, src.in_off, run.parts[0]->tgt.p, m, &k.plan));
+      GB_TRY(layout_end(b, src.in_off, parts[0]->tgt.p, m, &k.plan));
       continue;
     }
     const uint32_t* new_id = layout_new_id(k.build);
@@ -555,36 +524,37 @@ gb_status pr_csr_plans(const std::vector<int>& devs, uint32_t V, uint32_t n, con
       k.entries = total;
       GB_TRY(k.loc_tgt.alloc(std::max<uint64_t>(k.entries, 1)));
     }
-    for (size_t c = 0; c < max_chunks; ++c)
-      for (auto& qp : run.parts) {
-        const PrCsrPart& q = *qp;
-        if (c >= q.landed.size()) continue;
-        const uint32_t v0 = q.range.chunk_row[c], v1 = q.range.chunk_row[c + 1];
+    for (uint32_t c = 0; c < max_chunks; ++c)
+      for (uint32_t u = 0; u < U; ++u) {
+        const CsrChunks& ch = split[u].chunks;
+        if (c >= ch.count()) continue;
+        const uint32_t v0 = ch.row[c], v1 = ch.row[c + 1];
         if (v1 == v0) continue;
-        GB_CUDA(cudaStreamWaitEvent(k.s, q.landed[c], 0));
+        GB_CUDA(cudaStreamWaitEvent(k.s, parts[u]->landed[c], 0));
         k_pr_gather_rows<<<grid_for((uint64_t)(v1 - v0), 256), 256, 0, k.s>>>(
-            k.in_off.p, q.tgt.p, q.range.e_begin, v0, v1, new_id, U, r, k.loc_off.p, k.loc_tgt.p, n, k.bad.p + 2);
+            k.in_off.p, parts[u]->tgt.p, split[u].e_begin, v0, v1, new_id, U, r, k.loc_off.p, k.loc_tgt.p, n,
+            k.bad.p + 2);
       }
     GB_CUDA(cudaGetLastError());
     GB_CUDA(cudaMemcpyAsync(k.h_bad + 2, k.bad.p + 2, 4, cudaMemcpyDeviceToHost, k.s));
   }
   if (peers) {
     unsigned int nbad_tgt = 0;
-    for (auto& k : run.ranks) {
+    for (auto& k : ranks) {
       GB_CUDA(cudaSetDevice(k->dev));
       GB_CUDA(cudaStreamSynchronize(k->s));
       nbad_tgt += k->h_bad[2];
     }
-    GB_REQUIRE(nbad_tgt == 0, "in CSR holds %u targets >= node_count %u", nbad_tgt, n);
+    GB_TRY(require_ids("in", nbad_tgt, n));
     // 4. every rank has gathered: the parts and the full offsets go (the order stage has read the degrees), and
     // each rank builds its layout from its local CSR, which goes too
-    run.parts.clear();
-    for (auto& k : run.ranks) {
+    parts.clear();
+    for (auto& k : ranks) {
       GB_CUDA(cudaSetDevice(k->dev));
       k->in_off.release();
       k->out_off.release();
     }
-    for (auto& k : run.ranks) {
+    for (auto& k : ranks) {
       GB_CUDA(cudaSetDevice(k->dev));
       LayoutBuild* b = k->build;
       k->build = nullptr;
@@ -595,7 +565,7 @@ gb_status pr_csr_plans(const std::vector<int>& devs, uint32_t V, uint32_t n, con
     }
   }
   plans->clear();
-  for (auto& k : run.ranks) {
+  for (auto& k : ranks) {
     plans->push_back(k->plan);
     k->plan = nullptr;
   }

@@ -758,14 +758,14 @@ gb_status LayoutBuild::layout_classify() {
     GB_REQUIRE(dmax < 0x7FFFFFFFu, "a row with %u in-edges outside the sort path of the layout build", dmax);
     GB_TRY(rec.alloc(std::max<uint64_t>(row_entries, 1)));
   }
-  if (const PrCsrPart* feed = src.feed) {
+  if (const CsrFeed* feed = src.feed) {
     // the targets arrive chunk by chunk: check and classify each chunk as soon as it is there
     DevBuf<unsigned int> bad;
     GB_TRY(bad.alloc(1));
     GB_CUDA(cudaMemsetAsync(bad.p, 0, 4, s));
-    for (size_t k = 0; k < feed->landed.size(); ++k) {
-      const uint32_t v0 = feed->range.chunk_row[k], v1 = feed->range.chunk_row[k + 1];
-      const uint64_t e0 = feed->range.chunk_edge[k], e1 = feed->range.chunk_edge[k + 1];
+    for (uint32_t k = 0; k < src.chunks->count(); ++k) {
+      const uint32_t v0 = src.chunks->row[k], v1 = src.chunks->row[k + 1];
+      const uint64_t e0 = src.chunks->edge[k], e1 = src.chunks->edge[k + 1];
       GB_CUDA(cudaStreamWaitEvent(s, feed->landed[k], 0));
       check_ids_async(s, row_tgt + e0, e1 - e0, n, bad.p);
       if (p->n_cb > n_mega && v1 > v0)
@@ -777,7 +777,7 @@ gb_status LayoutBuild::layout_classify() {
     GB_CUDA(cudaGetLastError());
     GB_CUDA(cudaMemcpyAsync(&nbad, bad.p, 4, cudaMemcpyDeviceToHost, s));
     GB_CUDA(cudaStreamSynchronize(s));
-    GB_REQUIRE(nbad == 0, "in CSR holds %u targets >= node_count %u", nbad, n);
+    GB_TRY(require_ids("in", nbad, n));
   } else if (p->n_cb > n_mega) {
     k_cb_count<<<grid_for((uint64_t)(p->n_cb - n_mega) * 32, 256), 256, 0, s>>>(
         row_off, row_tgt, old_of.p, p->new_id.p, hot_of_blk.p, p->nrows.p, p->poff.p, p->blk.p, B,

@@ -6,7 +6,7 @@
 #include <vector>
 
 #include "common.cuh"
-#include "pr_split.h"
+#include "csr_split.h"
 
 namespace gb {
 
@@ -125,28 +125,6 @@ __host__ __device__ __forceinline__ uint32_t fin_blocks_of(const uint32_t* __res
   return lo;
 }
 
-// One part of a host in-CSR (pr_split.h) on device dev: its offsets and targets, uploaded on its own copy
-// stream, the targets in row-aligned chunks with an event recorded behind each
-struct PrCsrPart {
-  int dev = -1;
-  PrPart range;
-  cudaStream_t copy = nullptr;
-  cudaEvent_t offsets_in = nullptr;
-  std::vector<cudaEvent_t> landed;  // [K] recorded behind each chunk of targets
-  PeerBuf in_off, out_off, tgt;     // rows + 1, rows + 1 and e_end - e_begin (+ 8 zeroed) entries
-  ~PrCsrPart() {
-    if (dev < 0) return;
-    cudaSetDevice(dev);
-    if (copy) cudaStreamSynchronize(copy);
-    tgt.release();
-    out_off.release();
-    in_off.release();
-    for (cudaEvent_t ev : landed) cudaEventDestroy(ev);
-    if (offsets_in) cudaEventDestroy(offsets_in);
-    if (copy) cudaStreamDestroy(copy);
-  }
-};
-
 // Where a layout build (pr_layout.cu) finds the degrees: the internal order, the active rows and the hot
 // blocks come from the full in- and out-offsets (n + 1 each, device memory of `device`), and the build runs
 // on `stream`.  m is the graph's edge count (the hot-block threshold tau m / e_b).  The rows themselves come
@@ -159,9 +137,10 @@ struct PrSource {
   uint64_t m = 0;
   const uint32_t* in_off = nullptr;
   const uint32_t* out_off = nullptr;
-  // a part covering [0, n] whose targets are still landing: the row source is its in-CSR, and the build checks
-  // and classifies each chunk as soon as its landed event fires
-  const PrCsrPart* feed = nullptr;
+  // a feed of the whole in-CSR whose targets are still landing, in the chunks `chunks`: the row source is its
+  // in-CSR, and the build checks and classifies each chunk as soon as its landed event fires
+  const CsrFeed* feed = nullptr;
+  const CsrChunks* chunks = nullptr;
 };
 struct LayoutBuild;
 // The order stage of rank deal.p's layout; afterwards layout_new_id(*out) (old id -> internal id, n entries on
@@ -185,7 +164,7 @@ gb_status shard_from_plan(int device, PrPlan* plan, gb_pr_shard** out);
 // with the messages of every entry point that takes one (multi.cu)
 gb_status check_pr_host_csr(uint32_t n, const uint32_t* in_off, const uint32_t* in_tgt, const uint32_t* out_off);
 // The layouts of ranks 0 .. U-1 (U = devs.size() * V, rank r on devs[r / V]) of a host CSR that passed
-// check_pr_host_csr (multi.cu).  Part u of the split (pr_split.h, targets in chunks of about chunk_edges >= 1
+// check_pr_host_csr (multi.cu).  Part u of the split (pr_split, targets in chunks of about chunk_edges >= 1
 // edges) is uploaded by the device of rank u; the offsets are checked on the device.  A lone rank builds its
 // layout from its part as the chunks land; with several, every rank gathers the rows it owns from all parts into
 // a local in-CSR first.  On success plans holds U plans, the caller's to free; on failure nothing is left.

@@ -27,7 +27,7 @@
 // One-shot count of a host CSR (gb_triangle_count_csr_u32).  Each term of the sum is one entry (u, v <= u)
 // and reads N(u) and N(v) only, on both paths, so the entries of the rows [r0, r1) can be counted once the
 // rows 0 .. r1 - 1 are on the device: the stream is causal in row order.  The offsets go first; the targets
-// follow in row-aligned chunks (tc_split.h) straight into their final place in one targets[m] array, because
+// follow in row-aligned chunks (tc_split, csr_split.h) straight into their final place in one targets[m] array, because
 // the terms read earlier rows at random: unlike the WCC ring, the whole CSR ends up resident.  Once chunk k
 // has landed, a check stream runs k_tc_rows_unsorted and the id check over its rows only, and the host counts
 // its entries with k_tc while every chunk so far had sorted rows, and with k_tc_cut + k_tc_list from the first
@@ -38,7 +38,7 @@
 #include <vector>
 
 #include "common.cuh"
-#include "tc_split.h"
+#include "csr_split.h"
 
 namespace gb {
 
@@ -218,7 +218,7 @@ __global__ void __launch_bounds__(256) k_tc_list(const uint32_t* __restrict__ of
 
 // ---- one-shot count of a host CSR (gb_triangle_count_csr_u32) ----------------------------------------------
 // C, the entries per chunk: GB_TC_FEED_ENTRIES when set, else ceil(m / 16) but at least 2^20; never below
-// ceil(m / 4096), so that a call makes at most 2 * 4096 + 1 chunks (tc_split.h)
+// ceil(m / 4096), so that a call makes at most 2 * 4096 + 1 chunks (tc_split)
 constexpr uint64_t TC_FEED_CHUNKS = 16;
 constexpr uint64_t TC_FEED_MIN_ENTRIES = 1u << 20;
 constexpr uint64_t TC_FEED_MAX_CHUNKS = 4096;
@@ -228,24 +228,24 @@ constexpr uint32_t TC_COUNT_LANES = 4;
 
 thread_local gb_tc_csr_info tc_csr_last{};  // behind gb_triangle_count_csr_info
 
-// Everything one call holds.  The destructor drains the streams before anything they use goes: the pinned
-// flags, the events, and (after it, as members) the device buffers.
+// Everything one call holds besides its feed.  The destructor drains the consumer streams before anything
+// they read goes: the pinned flags, the events, the device buffers (members) and the feed (the first member).
 struct TcCall {
-  DevBuf<uint32_t> off, tgt, cut;
+  CsrFeed feed;  // the offsets [0, n] and the resident targets, one landed event per chunk
+  DevBuf<uint32_t> cut;
   DevBuf<unsigned int> bad;                 // [0] rows whose offsets decrease, [1 + k] targets >= n in chunk k
   DevBuf<unsigned long long> found, total;  // found[k]: chunk k has a descent inside a row
   unsigned long long* h_found = nullptr;    // page-locked: found[K], then the total
   unsigned int* h_bad = nullptr;            // page-locked: bad[1 + K]
   void* host = nullptr;
-  cudaStream_t copy = nullptr, check = nullptr, count = nullptr;  // count: the list-order path, and the join
-  cudaStream_t lanes[TC_COUNT_LANES] = {};                        // the k_tc launches
+  cudaStream_t check = nullptr, count = nullptr;  // count: the list-order path, and the join
+  cudaStream_t lanes[TC_COUNT_LANES] = {};        // the k_tc launches
   cudaEvent_t lane_done[TC_COUNT_LANES] = {};
   cudaEvent_t begin = nullptr, uploaded = nullptr, end = nullptr;  // timed
-  cudaEvent_t offsets_in = nullptr, offsets_checked = nullptr;
-  std::vector<cudaEvent_t> landed, checked;  // [K]
+  cudaEvent_t offsets_checked = nullptr;
+  std::vector<cudaEvent_t> checked;  // [K]
 
   gb_status create(uint32_t K) {
-    GB_CUDA(cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking));
     GB_CUDA(cudaStreamCreateWithFlags(&check, cudaStreamNonBlocking));
     GB_CUDA(cudaStreamCreateWithFlags(&count, cudaStreamNonBlocking));
     for (uint32_t i = 0; i < TC_COUNT_LANES; ++i) {
@@ -253,32 +253,26 @@ struct TcCall {
       GB_CUDA(cudaEventCreateWithFlags(&lane_done[i], cudaEventDisableTiming));
     }
     for (cudaEvent_t* e : {&begin, &uploaded, &end}) GB_CUDA(cudaEventCreate(e));
-    for (cudaEvent_t* e : {&offsets_in, &offsets_checked}) GB_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
-    landed.assign(K, nullptr);
+    GB_CUDA(cudaEventCreateWithFlags(&offsets_checked, cudaEventDisableTiming));
     checked.assign(K, nullptr);
-    for (uint32_t k = 0; k < K; ++k) {
-      GB_CUDA(cudaEventCreateWithFlags(&landed[k], cudaEventDisableTiming));
-      GB_CUDA(cudaEventCreateWithFlags(&checked[k], cudaEventDisableTiming));
-    }
+    for (uint32_t k = 0; k < K; ++k) GB_CUDA(cudaEventCreateWithFlags(&checked[k], cudaEventDisableTiming));
     GB_CUDA(cudaHostAlloc(&host, ((size_t)K + 1) * 12, cudaHostAllocDefault));
     h_found = static_cast<unsigned long long*>(host);
     h_bad = reinterpret_cast<unsigned int*>(h_found + K + 1);
     return GB_OK;
   }
   ~TcCall() {
-    for (cudaStream_t s : {copy, check, count})
+    for (cudaStream_t s : {check, count})
       if (s) cudaStreamSynchronize(s);
     for (uint32_t i = 0; i < TC_COUNT_LANES; ++i) {
       if (lanes[i]) cudaStreamSynchronize(lanes[i]), cudaStreamDestroy(lanes[i]);
       if (lane_done[i]) cudaEventDestroy(lane_done[i]);
     }
-    for (cudaEvent_t e : landed)
-      if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : checked)
       if (e) cudaEventDestroy(e);
-    for (cudaEvent_t e : {begin, uploaded, end, offsets_in, offsets_checked})
+    for (cudaEvent_t e : {begin, uploaded, end, offsets_checked})
       if (e) cudaEventDestroy(e);
-    for (cudaStream_t s : {copy, check, count})
+    for (cudaStream_t s : {check, count})
       if (s) cudaStreamDestroy(s);
     if (host) cudaFreeHost(host);
   }
@@ -290,29 +284,22 @@ static gb_status tc_csr(int device, uint32_t n, const uint32_t* off, const uint3
   GB_REQUIRE(triangles != nullptr, "triangles is NULL");
   GB_REQUIRE(n > 0, "node_count must be > 0");
   GB_TRY(require_device(device));
-  GB_REQUIRE(off != nullptr, "undirected offsets is NULL");
-  GB_REQUIRE(off[0] == 0, "undirected offsets[0] must be 0");
+  GB_TRY(require_host_csr(n, off, tgt, "undirected"));
   const uint64_t m = off[n];
-  GB_REQUIRE(m == 0 || tgt != nullptr, "undirected targets is NULL");
   DeviceGuard guard(device);
   GB_CUDA(cudaSetDevice(device));
   uint64_t C = env_u64("GB_TC_FEED_ENTRIES", 0);
   if (C == 0) C = std::max<uint64_t>((m + TC_FEED_CHUNKS - 1) / TC_FEED_CHUNKS, TC_FEED_MIN_ENTRIES);
   C = std::max<uint64_t>(C, (m + TC_FEED_MAX_CHUNKS - 1) / TC_FEED_MAX_CHUNKS);
-  const TcChunks ch = tc_split(off, n, C);
+  const CsrChunks ch = tc_split(off, n, C);
   const uint32_t K = ch.count();
   // page-locked targets go out all at once; a pageable copy returns only once it is done, so from pageable
   // memory one chunk is kept on the bus ahead of the one being counted
-  bool pinned = false;
-  if (m) {
-    cudaPointerAttributes a{};
-    if (cudaPointerGetAttributes(&a, tgt) == cudaSuccess) pinned = a.type == cudaMemoryTypeHost;
-    else cudaGetLastError();
-  }
+  const bool pinned = m && CsrFeed::pinned(tgt);
   TcCall t;
   GB_TRY(t.create(K));
-  GB_TRY(t.off.alloc((size_t)n + 1));
-  GB_TRY(t.tgt.alloc(m));
+  GB_TRY(t.feed.open(device, 0, n, false));
+  GB_TRY(t.feed.resident(0, m, K, false));
   GB_TRY(t.bad.alloc((size_t)K + 1));
   GB_TRY(t.found.alloc(K));
   GB_TRY(t.total.alloc(1));
@@ -325,32 +312,30 @@ static gb_status tc_csr(int device, uint32_t n, const uint32_t* off, const uint3
   GB_CUDA(cudaMemsetAsync(t.bad.p, 0, ((size_t)K + 1) * 4, t.check));
   GB_CUDA(cudaMemsetAsync(t.found.p, 0, (size_t)K * 8, t.check));
   GB_CUDA(cudaMemsetAsync(t.total.p, 0, 8, t.count));
-  GB_CUDA(cudaEventRecord(t.begin, t.copy));
-  GB_CUDA(cudaMemcpyAsync(t.off.p, off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, t.copy));
-  GB_CUDA(cudaEventRecord(t.offsets_in, t.copy));
-  GB_CUDA(cudaStreamWaitEvent(t.check, t.offsets_in, 0));
-  check_monotone_async(t.check, t.off.p, n, t.bad.p);
+  GB_CUDA(cudaEventRecord(t.begin, t.feed.copy));
+  GB_TRY(t.feed.send_offsets(off));
+  GB_TRY(t.feed.check_monotone(t.check, 0, n, t.bad.p));
   GB_CUDA(cudaMemcpyAsync(t.h_bad, t.bad.p, 4, cudaMemcpyDeviceToHost, t.check));
   GB_CUDA(cudaEventRecord(t.offsets_checked, t.check));
   info.kernel_launches += 1;
+  const uint32_t *d_off = t.feed.off.p, *d_tgt = t.feed.tgt.p;
   // chunk k: its copy, then its checks behind its landing.  The check kernels read the rows and entries of
   // the chunk only, and the bounds stay inside the arrays whatever the offsets hold
   uint32_t issued = 0;
   auto issue = [&]() -> gb_status {
     const uint32_t k = issued++;
-    const uint64_t e0 = ch.entry[k], e1 = ch.entry[k + 1];
+    const uint64_t e0 = ch.edge[k], e1 = ch.edge[k + 1];
     const uint32_t r0 = ch.row[k], r1 = ch.row[k + 1];
-    if (e1 > e0) GB_CUDA(cudaMemcpyAsync(t.tgt.p + e0, tgt + e0, (e1 - e0) * 4, cudaMemcpyHostToDevice, t.copy));
-    GB_CUDA(cudaEventRecord(t.landed[k], t.copy));
-    if (k + 1 == K) GB_CUDA(cudaEventRecord(t.uploaded, t.copy));
-    GB_CUDA(cudaStreamWaitEvent(t.check, t.landed[k], 0));
+    GB_TRY(t.feed.send(k, tgt, e0, e1 - e0));
+    if (k + 1 == K) GB_CUDA(cudaEventRecord(t.uploaded, t.feed.copy));
+    GB_CUDA(cudaStreamWaitEvent(t.check, t.feed.landed[k], 0));
     if (e1 - e0 >= 2) {
-      k_tc_rows_unsorted<<<grid_for(e1 - e0, 256, H100_SMS * 32u), 256, 0, t.check>>>(t.off.p, t.tgt.p, r0, r1, e0,
+      k_tc_rows_unsorted<<<grid_for(e1 - e0, 256, H100_SMS * 32u), 256, 0, t.check>>>(d_off, d_tgt, r0, r1, e0,
                                                                                       e1, t.found.p + k);
       info.kernel_launches += 1;
     }
     if (e1 > e0) {
-      check_ids_async(t.check, t.tgt.p + e0, e1 - e0, n, t.bad.p + 1 + k);
+      check_ids_async(t.check, d_tgt + e0, e1 - e0, n, t.bad.p + 1 + k);
       info.kernel_launches += 1;
     }
     GB_CUDA(cudaGetLastError());
@@ -363,7 +348,7 @@ static gb_status tc_csr(int device, uint32_t n, const uint32_t* off, const uint3
   while (issued < ahead) GB_TRY(issue());
   // the offsets are monotone before anything indexes with them
   GB_CUDA(cudaEventSynchronize(t.offsets_checked));
-  GB_REQUIRE(t.h_bad[0] == 0, "undirected offsets are not monotone (%u rows)", t.h_bad[0]);
+  GB_TRY(require_monotone("undirected", t.h_bad[0]));
   bool list = false;  // from the first chunk with an unsorted row on, every chunk takes k_tc_cut + k_tc_list
   for (uint32_t k = 0; k < K; ++k) {
     if (issued < K) GB_TRY(issue());  // the next chunk is on the bus while this one is checked and counted
@@ -373,9 +358,9 @@ static gb_status tc_csr(int device, uint32_t n, const uint32_t* off, const uint3
       GB_CUDA(cudaStreamSynchronize(t.check));
       unsigned int nbad = 0;
       for (uint32_t j = 0; j < K; ++j) nbad += t.h_bad[1 + j];
-      return fail(GB_ERR_INVALID, "undirected CSR holds %u targets >= node_count %u", nbad, n);
+      return require_ids("undirected", nbad, n);
     }
-    const uint64_t e0 = ch.entry[k], e1 = ch.entry[k + 1];
+    const uint64_t e0 = ch.edge[k], e1 = ch.edge[k + 1];
     const uint32_t r0 = ch.row[k], r1 = ch.row[k + 1];
     if (e1 == e0) continue;
     const unsigned grid = grid_for(e1 - e0, 256, H100_SMS * 32u);
@@ -383,7 +368,7 @@ static gb_status tc_csr(int device, uint32_t n, const uint32_t* off, const uint3
     if (!list) {  // k_tc reads only landed rows: the chunks count side by side
       cudaStream_t lane = t.lanes[info.sorted_chunks % TC_COUNT_LANES];
       GB_CUDA(cudaStreamWaitEvent(lane, t.checked[k], 0));
-      k_tc<<<grid, 256, 0, lane>>>(t.off.p, t.tgt.p, r0, r1, e0, e1, t.total.p);
+      k_tc<<<grid, 256, 0, lane>>>(d_off, d_tgt, r0, r1, e0, e1, t.total.p);
       info.sorted_chunks += 1;
       info.kernel_launches += 1;
     } else {  // k_tc_list reads cut[v] for every v <= u: the cuts and counts go in row order on one stream
@@ -393,9 +378,9 @@ static gb_status tc_csr(int device, uint32_t n, const uint32_t* off, const uint3
         info.first_list_chunk = k;
         GB_TRY(t.cut.alloc(n));
       }
-      k_tc_cut<<<grid_for((uint64_t)(r1 - c0) * 32, 256, H100_SMS * 32u), 256, 0, t.count>>>(t.off.p, t.tgt.p, c0,
-                                                                                             r1, t.cut.p);
-      k_tc_list<<<grid, 256, 0, t.count>>>(t.off.p, t.tgt.p, t.cut.p, r0, r1, e0, e1, t.total.p);
+      k_tc_cut<<<grid_for((uint64_t)(r1 - c0) * 32, 256, H100_SMS * 32u), 256, 0, t.count>>>(d_off, d_tgt, c0, r1,
+                                                                                             t.cut.p);
+      k_tc_list<<<grid, 256, 0, t.count>>>(d_off, d_tgt, t.cut.p, r0, r1, e0, e1, t.total.p);
       info.list_chunks += 1;
       info.kernel_launches += 2;
     }

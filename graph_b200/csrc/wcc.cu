@@ -14,7 +14,7 @@
 #include <vector>
 
 #include "common.cuh"
-#include "wcc_split.h"
+#include "csr_split.h"
 
 namespace gb {
 
@@ -322,90 +322,48 @@ constexpr uint32_t WCC_FEED_RING = 3;
 constexpr uint64_t WCC_FEED_EDGES = 1u << 22;  // C: 16 MiB per buffer (DESIGN.md §5)
 constexpr uint32_t WCC_MULTI_MAX_PARTS = 64;   // GB_WCC_MULTI_PARTS is clamped to [1, 64] parts per device
 
-// the streams and events of one part; the streams are drained before they go
-struct WccFeed {
-  cudaStream_t copy = nullptr, link = nullptr;
-  cudaEvent_t offsets_in = nullptr;
-  cudaEvent_t landed[WCC_FEED_RING] = {}, freed[WCC_FEED_RING] = {};
-  cudaEvent_t forest = nullptr;  // recorded behind the part's finished forest, for the part that merges it
-  gb_status create() {
-    GB_CUDA(cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking));
-    GB_CUDA(cudaStreamCreateWithFlags(&link, cudaStreamNonBlocking));
-    GB_CUDA(cudaEventCreateWithFlags(&offsets_in, cudaEventDisableTiming));
-    for (uint32_t i = 0; i < WCC_FEED_RING; ++i) {
-      GB_CUDA(cudaEventCreateWithFlags(&landed[i], cudaEventDisableTiming));
-      GB_CUDA(cudaEventCreateWithFlags(&freed[i], cudaEventDisableTiming));
-    }
-    GB_CUDA(cudaEventCreateWithFlags(&forest, cudaEventDisableTiming));
-    return GB_OK;
-  }
-  void drain() const {
-    if (copy) cudaStreamSynchronize(copy);
-    if (link) cudaStreamSynchronize(link);
-  }
-  ~WccFeed() {
-    drain();
-    for (uint32_t i = 0; i < WCC_FEED_RING; ++i) {
-      if (landed[i]) cudaEventDestroy(landed[i]);
-      if (freed[i]) cudaEventDestroy(freed[i]);
-    }
-    if (offsets_in) cudaEventDestroy(offsets_in);
-    if (forest) cudaEventDestroy(forest);
-    if (copy) cudaStreamDestroy(copy);
+// One part of a one-shot WCC (csr_split.h): the edges [e_begin, e_end) stream through the ring of the part's
+// feed in chunks of C edges (chunk k is [e_begin + kC, min(e_begin + (k + 1)C, e_end)), whatever rows it cuts)
+// and are linked on the part's link stream into its own forest parent[n], which the other parts read when
+// there are several.
+struct WccPart {
+  WccPartRange range{};
+  uint64_t C = 4, K = 0;  // chunk size in edges, chunks
+  unsigned int nbad[2] = {0, 0};
+  CsrFeed feed;  // the offsets and the ring; destroyed last
+  cudaStream_t link = nullptr;
+  cudaEvent_t forest_done = nullptr;  // recorded behind the part's finished forest, for the part that merges it
+  PeerBuf forest;  // parent[n]
+  DevBuf<unsigned int> bad;  // [0] rows whose offsets decrease, [1] targets >= n
+  uint64_t e0(uint64_t k) const { return range.e_begin + k * C; }
+  uint64_t len(uint64_t k) const { return std::min<uint64_t>(C, range.e_end - e0(k)); }
+  ~WccPart() {
+    if (feed.dev >= 0) cudaSetDevice(feed.dev);  // the members are released on the part's device
+    if (forest_done) cudaEventDestroy(forest_done);
     if (link) cudaStreamDestroy(link);
   }
 };
 
-// One part of a one-shot WCC (wcc_split.h): the edges [e_begin, e_end) stream through the part's ring in
-// chunks of C edges (chunk k is [e_begin + kC, min(e_begin + (k + 1)C, e_end)), whatever rows it cuts) and
-// are linked into the part's own forest parent[n] on device dev, which the other parts read when there are
-// several.
-struct WccPart {
-  int dev = -1;
-  WccPartRange range{};
-  uint64_t C = 4, K = 0;  // chunk size in edges, chunks
-  uint32_t R = 0;         // ring buffers in use
-  unsigned int nbad[2] = {0, 0};
-  WccFeed feed;  // outlives the buffers below, whose release waits for the device
-  PeerBuf forest;  // parent[n]
-  DevBuf<uint32_t> off, ring[WCC_FEED_RING];
-  DevBuf<unsigned int> bad;  // [0] rows whose offsets decrease, [1] targets >= n
-  ~WccPart() {
-    if (dev >= 0) cudaSetDevice(dev);  // the members are released on the part's device
-  }
-};
-
-// Every part's streams drain before any part's buffers go: a merge reads its partner's parent[].
+// Every part's link stream drains before any part goes: a merge reads its partner's parent[].
 struct WccParts {
   std::vector<std::unique_ptr<WccPart>> v;
   ~WccParts() {
-    for (auto& q : v) q->feed.drain();
+    for (auto& q : v)
+      if (q->link) cudaStreamSynchronize(q->link);
   }
 };
-
-// copy k of a part waits until its link k - R has read the buffer.  cudaStreamWaitEvent takes the event's
-// latest record at the time of the call, so copy k and link k are enqueued in that order, chunk after chunk
-static gb_status wcc_enqueue_copy(WccPart& q, const uint32_t* tgt, uint64_t k) {
-  const uint64_t e0 = q.range.e_begin + k * q.C, len = std::min<uint64_t>(q.C, q.range.e_end - e0);
-  if (k >= q.R) GB_CUDA(cudaStreamWaitEvent(q.feed.copy, q.feed.freed[k % q.R], 0));
-  GB_CUDA(cudaMemcpyAsync(q.ring[k % q.R].p, tgt + e0, len * 4, cudaMemcpyHostToDevice, q.feed.copy));
-  GB_CUDA(cudaEventRecord(q.feed.landed[k % q.R], q.feed.copy));
-  return GB_OK;
-}
 
 // Union of every out-edge (wcc_baseline), linked chunk by chunk as the targets land: union-find does not
 // depend on the order of the links, and hooking the higher root under the lower keeps parent[x] <= x, so
 // after the final compress every label is the minimum node id of its component, as gb_wcc gives.  The
 // finds halve the paths they walk, so no compress is needed between chunks (DESIGN.md §5).
-// The edges are cut into devs.size() * per_dev parts (wcc_split.h), part p on devs[p / per_dev], each with
+// The edges are cut into devs.size() * per_dev parts (wcc_split), part p on devs[p / per_dev], each with
 // its own streams, ring and forest.  One part is gb_wcc_csr_u32.  With more, the forests merge in
 // ceil(log2 P) tree rounds: in round s = 1, 2, 4, ... part p (p mod 2s == 0) links the forest of part p + s
 // into its own through a peer pointer and compresses, and part 0 ends with the union of all edges.
 static gb_status wcc_csr_parts(const std::vector<int>& devs, uint32_t per_dev, uint32_t n, const uint32_t* off,
                                const uint32_t* tgt, uint32_t* comp) {
-  GB_REQUIRE(off[0] == 0, "offsets[0] must be 0");
-  const uint64_t m = off[n];
-  GB_REQUIRE(m == 0 || tgt != nullptr, "targets is NULL");
+  GB_TRY(require_host_csr(n, off, tgt, ""));
   const uint32_t P = (uint32_t)devs.size() * per_dev;
   const std::vector<WccPartRange> split = wcc_split(off, n, P);
   DeviceGuard guard(devs[0]);
@@ -417,98 +375,89 @@ static gb_status wcc_csr_parts(const std::vector<int>& devs, uint32_t per_dev, u
     parts.v.emplace_back(new (std::nothrow) WccPart());
     GB_REQUIRE(parts.v.back() != nullptr, "host allocation failed");
     WccPart& q = *parts.v.back();
-    q.dev = devs[p / per_dev];
     q.range = split[p];
-    GB_CUDA(cudaSetDevice(q.dev));
     const uint64_t len = q.range.e_end - q.range.e_begin;
     q.C = std::min<uint64_t>(C, (len + 3)) & ~3ull;
     if (q.C == 0) q.C = 4;
     q.K = (len + q.C - 1) / q.C;
-    q.R = (uint32_t)std::min<uint64_t>(WCC_FEED_RING, q.K);
-    GB_TRY(q.feed.create());
-    const uint32_t rows = q.range.r_end - q.range.r_begin;
-    GB_TRY(q.off.alloc((size_t)rows + 1));
+    GB_TRY(q.feed.open(devs[p / per_dev], q.range.r_begin, q.range.r_end, false));
+    GB_CUDA(cudaStreamCreateWithFlags(&q.link, cudaStreamNonBlocking));
+    GB_CUDA(cudaEventCreateWithFlags(&q.forest_done, cudaEventDisableTiming));
     GB_TRY(q.forest.alloc(n, P > 1));
     GB_TRY(q.bad.alloc(2));
-    for (uint32_t r = 0; r < q.R; ++r) {
-      GB_TRY(q.ring[r].alloc(q.C, 8));
-      GB_CUDA(cudaMemsetAsync(q.ring[r].p + q.C, 0, 8 * 4, q.feed.copy));
-    }
-    GB_CUDA(cudaMemcpyAsync(q.off.p, off + q.range.r_begin, ((size_t)rows + 1) * 4, cudaMemcpyHostToDevice,
-                            q.feed.copy));
-    GB_CUDA(cudaEventRecord(q.feed.offsets_in, q.feed.copy));
-    for (uint32_t k = 0; k < q.R; ++k) GB_TRY(wcc_enqueue_copy(q, tgt, k));
+    const uint32_t R = (uint32_t)std::min<uint64_t>(WCC_FEED_RING, q.K);
+    GB_TRY(q.feed.open_ring(R, q.C));
+    GB_TRY(q.feed.send_offsets(off));
+    for (uint32_t k = 0; k < R; ++k) GB_TRY(q.feed.send(k, tgt, q.e0(k), q.len(k)));
   }
   // offsets: monotone, checked before anything indexes with them.  The slices tile [0, n], so the rows each
   // part checks cover every row once, whatever the host array holds
   for (auto& qp : parts.v) {
     WccPart& q = *qp;
-    GB_CUDA(cudaSetDevice(q.dev));
-    GB_CUDA(cudaStreamWaitEvent(q.feed.link, q.feed.offsets_in, 0));
-    GB_CUDA(cudaMemsetAsync(q.bad.p, 0, 8, q.feed.link));
-    check_monotone_async(q.feed.link, q.off.p + (q.range.check_begin - q.range.r_begin),
-                         q.range.r_end - q.range.check_begin, q.bad.p);
-    GB_CUDA(cudaMemcpyAsync(q.nbad, q.bad.p, 4, cudaMemcpyDeviceToHost, q.feed.link));
+    GB_CUDA(cudaSetDevice(q.feed.dev));
+    GB_CUDA(cudaMemsetAsync(q.bad.p, 0, 8, q.link));
+    GB_TRY(q.feed.check_monotone(q.link, q.range.check_begin, q.range.r_end, q.bad.p));
+    GB_CUDA(cudaMemcpyAsync(q.nbad, q.bad.p, 4, cudaMemcpyDeviceToHost, q.link));
   }
   unsigned int nbad = 0;
   for (auto& q : parts.v) {
-    GB_CUDA(cudaStreamSynchronize(q->feed.link));
+    GB_CUDA(cudaStreamSynchronize(q->link));
     nbad += q->nbad[0];
   }
-  GB_REQUIRE(nbad == 0, "offsets are not monotone (%u rows)", nbad);
+  GB_TRY(require_monotone("", nbad));
   const unsigned blk = 256;
   const unsigned grid = grid_for(n, blk);
   uint64_t chunks = 0;
   for (auto& q : parts.v) {
-    GB_CUDA(cudaSetDevice(q->dev));
-    k_cc_init<<<grid, blk, 0, q->feed.link>>>(q->forest.p, n);
+    GB_CUDA(cudaSetDevice(q->feed.dev));
+    k_cc_init<<<grid, blk, 0, q->link>>>(q->forest.p, n);
     chunks = std::max(chunks, q->K);
   }
   for (uint64_t k = 0; k < chunks; ++k) {
     for (auto& qp : parts.v) {
       WccPart& q = *qp;
       if (k >= q.K) continue;
-      GB_CUDA(cudaSetDevice(q.dev));
-      if (k >= q.R) GB_TRY(wcc_enqueue_copy(q, tgt, k));
-      const uint64_t e0 = q.range.e_begin + k * q.C, len = std::min<uint64_t>(q.C, q.range.e_end - e0);
-      GB_CUDA(cudaStreamWaitEvent(q.feed.link, q.feed.landed[k % q.R], 0));
-      k_cc_link_edges<<<grid_for(len, LINK_TILE * (blk / 32)), blk, 0, q.feed.link>>>(
-          q.off.p, q.range.r_end - q.range.r_begin, q.range.r_begin, q.ring[k % q.R].p, (uint32_t)e0,
-          (uint32_t)len, n, q.forest.p, q.bad.p + 1);
-      GB_CUDA(cudaEventRecord(q.feed.freed[k % q.R], q.feed.link));
+      GB_CUDA(cudaSetDevice(q.feed.dev));
+      const uint64_t R = q.feed.ring.size();
+      if (k >= R) GB_TRY(q.feed.send(k, tgt, q.e0(k), q.len(k)));
+      GB_CUDA(cudaStreamWaitEvent(q.link, q.feed.landed[k % R], 0));
+      k_cc_link_edges<<<grid_for(q.len(k), LINK_TILE * (blk / 32)), blk, 0, q.link>>>(
+          q.feed.off.p, q.range.r_end - q.range.r_begin, q.range.r_begin, q.feed.ring[k % R].p, (uint32_t)q.e0(k),
+          (uint32_t)q.len(k), n, q.forest.p, q.bad.p + 1);
+      GB_CUDA(cudaEventRecord(q.feed.freed[k % R], q.link));
     }
   }
   for (auto& q : parts.v) {
-    GB_CUDA(cudaSetDevice(q->dev));
-    k_cc_compress<<<grid, blk, 0, q->feed.link>>>(q->forest.p, n);
+    GB_CUDA(cudaSetDevice(q->feed.dev));
+    k_cc_compress<<<grid, blk, 0, q->link>>>(q->forest.p, n);
   }
   // a partner p + s never merges again after round s, so its forest is final when its event is recorded
   for (uint32_t s = 1; s < P; s *= 2) {
     for (uint32_t p = 0; p + s < P; p += 2 * s) {
       WccPart &a = *parts.v[p], &b = *parts.v[p + s];
-      GB_CUDA(cudaSetDevice(b.dev));
-      GB_CUDA(cudaEventRecord(b.feed.forest, b.feed.link));
-      GB_CUDA(cudaSetDevice(a.dev));
-      GB_CUDA(cudaStreamWaitEvent(a.feed.link, b.feed.forest, 0));
-      k_cc_merge_halving<<<grid, blk, 0, a.feed.link>>>(a.forest.p, b.forest.p, n);
-      k_cc_compress<<<grid, blk, 0, a.feed.link>>>(a.forest.p, n);
+      GB_CUDA(cudaSetDevice(b.feed.dev));
+      GB_CUDA(cudaEventRecord(b.forest_done, b.link));
+      GB_CUDA(cudaSetDevice(a.feed.dev));
+      GB_CUDA(cudaStreamWaitEvent(a.link, b.forest_done, 0));
+      k_cc_merge_halving<<<grid, blk, 0, a.link>>>(a.forest.p, b.forest.p, n);
+      k_cc_compress<<<grid, blk, 0, a.link>>>(a.forest.p, n);
     }
   }
   GB_CUDA(cudaGetLastError());
   for (auto& q : parts.v) {
-    GB_CUDA(cudaSetDevice(q->dev));
-    GB_CUDA(cudaMemcpyAsync(q->nbad + 1, q->bad.p + 1, 4, cudaMemcpyDeviceToHost, q->feed.link));
+    GB_CUDA(cudaSetDevice(q->feed.dev));
+    GB_CUDA(cudaMemcpyAsync(q->nbad + 1, q->bad.p + 1, 4, cudaMemcpyDeviceToHost, q->link));
   }
   nbad = 0;
   for (auto& q : parts.v) {
-    GB_CUDA(cudaStreamSynchronize(q->feed.link));
+    GB_CUDA(cudaStreamSynchronize(q->link));
     nbad += q->nbad[1];
   }
-  GB_REQUIRE(nbad == 0, "CSR holds %u targets >= node_count %u", nbad, n);
+  GB_TRY(require_ids("", nbad, n));
   WccPart& root = *parts.v[0];
-  GB_CUDA(cudaSetDevice(root.dev));
-  GB_CUDA(cudaMemcpyAsync(comp, root.forest.p, (size_t)n * 4, cudaMemcpyDeviceToHost, root.feed.link));
-  GB_CUDA(cudaStreamSynchronize(root.feed.link));
+  GB_CUDA(cudaSetDevice(root.feed.dev));
+  GB_CUDA(cudaMemcpyAsync(comp, root.forest.p, (size_t)n * 4, cudaMemcpyDeviceToHost, root.link));
+  GB_CUDA(cudaStreamSynchronize(root.link));
   return GB_OK;
 }
 

@@ -1,4 +1,4 @@
-// CPU check of the part split of gb_page_rank_csr_multi_u32 / gb_pr_shards_csr_u32 (graph_b200/csrc/pr_split.h).
+// CPU check of the part split of gb_page_rank_csr_multi_u32 / gb_pr_shards_csr_u32 (graph_b200/csrc/csr_split.h).
 // For every case and part count U = 1..8: the row slices tile [0, n] in order, so every row is checked by
 // exactly one part; each part's chunks tile its rows and its edges; every bound stays inside [0, m] and inside
 // its part, on malformed offsets too; and on monotone offsets the parts cut at rows, their edge ranges are the
@@ -11,7 +11,7 @@
 #include <random>
 #include <vector>
 
-#include "pr_split.h"
+#include "csr_split.h"
 
 static int failures = 0;
 static long checked = 0;
@@ -50,20 +50,20 @@ static void check(const char* name, const std::vector<uint32_t>& off, uint32_t p
     EXPECT(q.e_begin == (u ? s[u - 1].e_end : 0), "part %u starts at edge %llu", u, (unsigned long long)q.e_begin);
     for (uint32_t v = q.r_begin; v < q.r_end && v < n; ++v) ++checks[v];
     // chunks: rows and edges tile the part's, in order, inside it
-    const size_t K = q.chunk_row.size() - 1;
-    EXPECT(K >= 1 && q.chunk_edge.size() == K + 1, "part %u has %zu chunks", u, K);
-    if (K < 1 || q.chunk_edge.size() != K + 1) continue;
-    EXPECT(q.chunk_row[0] == q.r_begin && q.chunk_row[K] == q.r_end, "part %u chunk rows [%u, %u]", u,
-           q.chunk_row[0], q.chunk_row[K]);
-    EXPECT(q.chunk_edge[0] == q.e_begin && q.chunk_edge[K] == q.e_end, "part %u chunk edges", u);
+    const size_t K = q.chunks.row.size() - 1;
+    EXPECT(K >= 1 && q.chunks.edge.size() == K + 1, "part %u has %zu chunks", u, K);
+    if (K < 1 || q.chunks.edge.size() != K + 1) continue;
+    EXPECT(q.chunks.row[0] == q.r_begin && q.chunks.row[K] == q.r_end, "part %u chunk rows [%u, %u]", u,
+           q.chunks.row[0], q.chunks.row[K]);
+    EXPECT(q.chunks.edge[0] == q.e_begin && q.chunks.edge[K] == q.e_end, "part %u chunk edges", u);
     for (size_t k = 0; k < K; ++k) {
-      EXPECT(q.chunk_row[k] <= q.chunk_row[k + 1], "part %u chunk %zu rows [%u, %u)", u, k, q.chunk_row[k],
-             q.chunk_row[k + 1]);
-      EXPECT(q.chunk_edge[k] <= q.chunk_edge[k + 1], "part %u chunk %zu edges", u, k);
+      EXPECT(q.chunks.row[k] <= q.chunks.row[k + 1], "part %u chunk %zu rows [%u, %u)", u, k, q.chunks.row[k],
+             q.chunks.row[k + 1]);
+      EXPECT(q.chunks.edge[k] <= q.chunks.edge[k + 1], "part %u chunk %zu edges", u, k);
       if (mono)  // a chunk's edges are its rows' edges
-        EXPECT(q.chunk_edge[k] == off[q.chunk_row[k]] && q.chunk_edge[k + 1] == off[q.chunk_row[k + 1]],
-               "part %u chunk %zu edges [%llu, %llu) of rows [%u, %u)", u, k, (unsigned long long)q.chunk_edge[k],
-               (unsigned long long)q.chunk_edge[k + 1], q.chunk_row[k], q.chunk_row[k + 1]);
+        EXPECT(q.chunks.edge[k] == off[q.chunks.row[k]] && q.chunks.edge[k + 1] == off[q.chunks.row[k + 1]],
+               "part %u chunk %zu edges [%llu, %llu) of rows [%u, %u)", u, k, (unsigned long long)q.chunks.edge[k],
+               (unsigned long long)q.chunks.edge[k + 1], q.chunks.row[k], q.chunks.row[k + 1]);
     }
     if (!mono) continue;
     EXPECT(q.e_begin == off[q.r_begin] && q.e_end == off[q.r_end], "part %u edges [%llu, %llu) of rows [%u, %u)", u,
@@ -100,7 +100,7 @@ static void one_device(const char* name, const std::vector<uint32_t>& off) {
   for (uint64_t c : {1ull, 3ull, 7ull, 16ull, 5000ull}) {
     const uint64_t chunk = std::max<uint64_t>((m + c - 1) / c, 1);
     check(name, off, parts, chunk);
-    const size_t K = gb::pr_split(off.data(), n, parts, chunk)[0].chunk_row.size() - 1;
+    const size_t K = gb::pr_split(off.data(), n, parts, chunk)[0].chunks.row.size() - 1;
     EXPECT(K <= std::min<uint64_t>(c, 4096), "%zu chunks for %llu asked", K, (unsigned long long)c);
   }
 }

@@ -1,6 +1,6 @@
-// CPU check of the chunk cut of gb_triangle_count_csr_u32 (graph_b200/csrc/tc_split.h).  For every case and
+// CPU check of the chunk cut of gb_triangle_count_csr_u32 (graph_b200/csrc/csr_split.h).  For every case and
 // chunk size C: the chunks cover the rows [0, n) exactly once, in order, each with at least one row; every
-// boundary is row-aligned (entry[k] == off[row[k]]) and the entries end at m; a chunk holds at most C entries
+// boundary is row-aligned (edge[k] == off[row[k]]) and the entries end at m; a chunk holds at most C entries
 // unless it has a single non-empty row (a hub longer than C), and every such hub stands alone; only an edgeless
 // CSR has an empty chunk; no chunk could have taken the next row (the cut is greedy), so there are at most
 // 2 ceil(m / C) + 1 chunks; and on offsets that are not monotone the cut still ends, with entry bounds
@@ -10,7 +10,7 @@
 #include <random>
 #include <vector>
 
-#include "tc_split.h"
+#include "csr_split.h"
 
 static int failures = 0;
 static long checked = 0;
@@ -33,24 +33,24 @@ static bool monotone(const std::vector<uint32_t>& off) {
 static void check(const char* name, const std::vector<uint32_t>& off, uint64_t chunk_entries) {
   const uint32_t n = (uint32_t)off.size() - 1;
   const uint64_t m = off[n];
-  const gb::TcChunks c = gb::tc_split(off.data(), n, chunk_entries);
+  const gb::CsrChunks c = gb::tc_split(off.data(), n, chunk_entries);
   ++checked;
   const uint32_t K = c.count();
-  EXPECT(c.row.size() == c.entry.size() && K >= 1, "%zu row bounds, %zu entry bounds", c.row.size(), c.entry.size());
-  if (c.row.size() != c.entry.size() || K < 1) return;
+  EXPECT(c.row.size() == c.edge.size() && K >= 1, "%zu row bounds, %zu entry bounds", c.row.size(), c.edge.size());
+  if (c.row.size() != c.edge.size() || K < 1) return;
   EXPECT(c.row[0] == 0 && c.row[K] == n, "rows [%u, %u), n = %u", c.row[0], c.row[K], n);
-  EXPECT(c.entry[0] == 0 && c.entry[K] == m, "entries [%llu, %llu), m = %llu", (unsigned long long)c.entry[0],
-         (unsigned long long)c.entry[K], (unsigned long long)m);
+  EXPECT(c.edge[0] == 0 && c.edge[K] == m, "entries [%llu, %llu), m = %llu", (unsigned long long)c.edge[0],
+         (unsigned long long)c.edge[K], (unsigned long long)m);
   std::vector<int> covered(n, 0);
   for (uint32_t k = 0; k < K; ++k) {
     EXPECT(c.row[k] < c.row[k + 1], "chunk %u rows [%u, %u)", k, c.row[k], c.row[k + 1]);
-    EXPECT(c.entry[k] <= c.entry[k + 1] && c.entry[k + 1] <= m, "chunk %u entries [%llu, %llu)", k,
-           (unsigned long long)c.entry[k], (unsigned long long)c.entry[k + 1]);
+    EXPECT(c.edge[k] <= c.edge[k + 1] && c.edge[k + 1] <= m, "chunk %u entries [%llu, %llu)", k,
+           (unsigned long long)c.edge[k], (unsigned long long)c.edge[k + 1]);
     for (uint32_t v = c.row[k]; v < c.row[k + 1] && v < n; ++v) ++covered[v];
     if (!monotone(off)) continue;
-    EXPECT(c.entry[k] == off[c.row[k]], "chunk %u starts at entry %llu, row %u at %u", k,
-           (unsigned long long)c.entry[k], c.row[k], off[c.row[k]]);
-    const uint64_t len = c.entry[k + 1] - c.entry[k];
+    EXPECT(c.edge[k] == off[c.row[k]], "chunk %u starts at entry %llu, row %u at %u", k,
+           (unsigned long long)c.edge[k], c.row[k], off[c.row[k]]);
+    const uint64_t len = c.edge[k + 1] - c.edge[k];
     uint32_t live = 0;  // rows with entries
     for (uint32_t v = c.row[k]; v < c.row[k + 1]; ++v) live += off[v + 1] > off[v];
     const bool single = live == 1;
@@ -124,11 +124,11 @@ int main() {
   {  // the hub stands alone, with the rows before and after it in chunks of their own
     std::vector<uint32_t> deg = {1, 2, 3, 50, 1, 1};
     const std::vector<uint32_t> off = from_degrees(deg);
-    const gb::TcChunks c = gb::tc_split(off.data(), 6, 10);
+    const gb::CsrChunks c = gb::tc_split(off.data(), 6, 10);
     const char* name = "hub alone";
     const uint64_t chunk_entries = 10;
     EXPECT(c.row == (std::vector<uint32_t>{0, 3, 4, 6}), "rows %zu bounds", c.row.size());
-    EXPECT(c.entry == (std::vector<uint64_t>{0, 6, 56, 58}), "entries %zu bounds", c.entry.size());
+    EXPECT(c.edge == (std::vector<uint64_t>{0, 6, 56, 58}), "entries %zu bounds", c.edge.size());
     ++checked;
   }
   std::printf("tc_split: %ld cases, %d failures\n", checked, failures);

@@ -1,4 +1,4 @@
-// CPU check of the part split of gb_wcc_csr_multi_u32 (graph_b200/csrc/wcc_split.h).  For every case and part
+// CPU check of the part split of gb_wcc_csr_multi_u32 (graph_b200/csrc/csr_split.h).  For every case and part
 // count: the edge ranges partition [0, m) in order with cuts at multiples of 4; the row slices tile [0, n]
 // (the first starts at 0, the last ends at n, each starts no later than the previous one ended and ends no
 // earlier) and their checked rows cover [0, n) exactly once; and on monotone offsets every edge of a part lies
@@ -8,7 +8,7 @@
 #include <random>
 #include <vector>
 
-#include "wcc_split.h"
+#include "csr_split.h"
 
 static int failures = 0;
 static long checked = 0;

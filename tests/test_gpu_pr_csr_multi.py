@@ -226,7 +226,7 @@ def shards_call(comm, v, inc_off, inc_tgt, out_off, n):
 
 
 def part_rows(off, parts):
-    """R_0 .. R_U of pr_split.h on monotone offsets"""
+    """R_0 .. R_U of pr_split (csr_split.h) on monotone offsets"""
     m, n = int(off[-1]), len(off) - 1
     cuts = [0] + [int(np.searchsorted(off, m * u // parts, side="left")) for u in range(1, parts)] + [n]
     return [min(max(c, p), n) for c, p in zip(cuts, [0] + cuts[:-1])]

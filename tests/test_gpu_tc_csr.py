@@ -21,8 +21,8 @@ def gb():
 
 
 def chunk_rows(off, c):
-    """tc_split.h restated: greedy row-aligned chunks of at most c entries; a longer row stands alone with the
-    empty rows next to it"""
+    """tc_split (csr_split.h) restated: greedy row-aligned chunks of at most c entries; a longer row stands alone
+    with the empty rows next to it"""
     off = [int(x) for x in off]
     n, rows, r = len(off) - 1, [0], 0
     while r < n:

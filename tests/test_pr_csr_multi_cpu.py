@@ -1,6 +1,6 @@
 """CPU-side checks of the multi-GPU one-shot PageRank (gb_page_rank_csr_multi_u32 / gb_pr_shards_csr_u32 /
-graph_b200.Comm.page_rank_csr): the part split (graph_b200/csrc/pr_split.h) compiled with g++ and checked on
-random, tiny, hub-heavy, all-empty and non-monotone offsets for 1..8 parts, the C symbols with their ctypes
+graph_b200.Comm.page_rank_csr): the part split (pr_split, graph_b200/csrc/csr_split.h) compiled with g++ and
+checked on random, tiny, hub-heavy, all-empty and non-monotone offsets for 1..8 parts, the C symbols with their ctypes
 declarations and header lines, and the Python argument checks, which raise before any device is touched."""
 import ctypes
 import subprocess

@@ -1,5 +1,5 @@
 """CPU-side checks of graph_b200.triangle_count_csr (one-shot triangle count of a host undirected CSR): the
-chunk cut (graph_b200/csrc/tc_split.h) compiled with g++ and checked on random, tiny, edgeless, hub-heavy and
+chunk cut (tc_split, graph_b200/csrc/csr_split.h) compiled with g++ and checked on random, tiny, edgeless, hub-heavy and
 non-monotone offsets; a restatement of the call's sorted-prefix rule, which counts chunk by chunk in row order
 and switches from k_tc's term to the list-order term at the first chunk with an unsorted row, against
 oracle.triangle_count on the tc_fixtures.py graphs; the C symbols with their ctypes declarations and header

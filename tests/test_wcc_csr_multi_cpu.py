@@ -1,6 +1,6 @@
 """CPU-side checks of the multi-GPU one-shot WCC (gb_wcc_csr_multi_u32 / graph_b200.Comm.wcc_csr): the part
-split (graph_b200/csrc/wcc_split.h) compiled with g++ and checked on random, tiny, hub, sparse and non-monotone
-offsets, and the C symbol with its ctypes declaration."""
+split (wcc_split, graph_b200/csrc/csr_split.h) compiled with g++ and checked on random, tiny, hub, sparse and
+non-monotone offsets, and the C symbol with its ctypes declaration."""
 import ctypes
 import subprocess
 from pathlib import Path

@@ -9,7 +9,7 @@ these calls (20 JACOBI sweeps, tolerance 0) are run in one process, alternated, 
   comm[0..P-1] csr / twin   the same over devices 0..P-1 for P = 2, 4, 8 where the box has them (the twin path
                       uploads a full twin to every device).
 Wall times (time.perf_counter around each call, every device synchronised) are reported as best / median.  Also
-per device: the H2D bytes each path moves, computed from the split (graph_b200/csrc/pr_split.h), and the peak
+per device: the H2D bytes each path moves, computed from the split (pr_split, graph_b200/csrc/csr_split.h), and the peak
 device bytes of one call: the high-water mark of the device's default memory pool (cudaMemPoolAttrUsedMemHigh,
 which holds every buffer of the one-device paths) plus, with several parts, the cudaMalloc'd part and offset
 buffers computed from the split.  The communicator's score vectors, the same for both comm paths, are not
@@ -87,7 +87,7 @@ class Pools:
 
 
 def split_rows(off, parts):
-    """R_0 .. R_U of pr_split.h (monotone offsets)"""
+    """R_0 .. R_U of pr_split (csr_split.h; monotone offsets)"""
     m, n = int(off[-1]), len(off) - 1
     cuts = [0] + [int(np.searchsorted(off, m * u // parts, side="left")) for u in range(1, parts)] + [n]
     for i in range(1, len(cuts)):
