@@ -31,6 +31,8 @@
 // round-robin to the P ranks, so every rank holds the same mix of hub and tail rows; a rank builds the
 // layout of its own rows only and stores each finished out_score into every peer's next vector
 // (multimem.st through the NVSwitch when a multicast mapping is given, else one store per peer).
+// The shard API at the end of this file is one rank's side of that; multi.cu drives the ranks of one process,
+// and pr_csr.cu builds layouts and shards straight from a host CSR.
 //
 // Algorithmic bytes per sweep: 4m (targets) + 4(n+1) (offsets) + 5*4n (out_scores read+write,
 // scores read+write, out-degree read) = 4m + 24n + 4  (BASELINE.md §3).
@@ -990,6 +992,15 @@ static void pr_fill_inactive(const PrPlan* p, const PrArgs& a, float base, cudaS
 }
 
 // ---- drivers ---------------------------------------------------------------------------------
+gb_status require_pr_config(const gb_page_rank_config* cfg) {
+  GB_REQUIRE(!(cfg->max_iterations == 0 && !(cfg->tolerance > 0.0)),
+             "max_iterations == 0 with tolerance <= 0 never terminates (page_rank.rs:107)");
+  return GB_OK;
+}
+uint64_t pr_sweep_limit(const gb_page_rank_config* cfg) {
+  return cfg->max_iterations ? cfg->max_iterations : 100000ull;
+}
+
 static gb_status run_exact(const gb_graph* g, const gb_page_rank_config* cfg, float* d_scores,
                            uint64_t* ran, double* error) {
   cudaStream_t s = g->stream;
@@ -1028,9 +1039,7 @@ static gb_status run_jacobi(const gb_graph* g, const gb_page_rank_config* cfg, f
   PrArgs a = make_args(p, v.base, cfg->damping_factor, cfg->tolerance);
   a.scores = p->scores.p;
 
-  // max_iterations == 0 never satisfies `iteration == max_iterations` (page_rank.rs:107): the
-  // reference then runs until the tolerance is met; we bound that at 100000 sweeps.
-  const uint64_t limit = cfg->max_iterations ? cfg->max_iterations : 100000ull;
+  const uint64_t limit = pr_sweep_limit(cfg);
   const bool can_stop_early = cfg->tolerance > 0.0;
   const uint32_t batch_cap = 64;
   uint64_t done = 0;      // sweeps launched so far
@@ -1133,14 +1142,13 @@ static void plan_shape(const PrPlan* p, gb_pr_plan_shape* shape) {
   shape->last_hot_block = p->last_hot_block;
 }
 
-static gb_status page_rank_impl(const gb_graph* g, const gb_page_rank_config* cfg, float* d_scores,
-                                float* h_scores, uint64_t* ran, double* error) {
+gb_status page_rank_impl(const gb_graph* g, const gb_page_rank_config* cfg, float* d_scores, float* h_scores,
+                         uint64_t* ran, double* error) {
   GB_REQUIRE(g && cfg && ran && error, "NULL argument");
   if (g->kind != GB_KIND_DIRECTED)
     return fail(GB_ERR_UNSUPPORTED, "page_rank needs a directed graph (page_rank.rs:61)");
   GB_REQUIRE(cfg->mode <= GB_PR_JACOBI, "bad page rank mode %u", cfg->mode);
-  GB_REQUIRE(!(cfg->max_iterations == 0 && !(cfg->tolerance > 0.0)),
-             "max_iterations == 0 with tolerance <= 0 never terminates (page_rank.rs:107)");
+  GB_TRY(require_pr_config(cfg));
   DeviceGuard guard(g->device);
   std::lock_guard<std::mutex> lock(g->mu);
   cudaStream_t s = g->stream;
@@ -1165,21 +1173,11 @@ static gb_status page_rank_impl(const gb_graph* g, const gb_page_rank_config* cf
   return GB_OK;
 }
 
-// A resident digraph of a host CSR that passed check_pr_host_csr: the in-CSR, and the out-offsets for the
-// out-degrees
-static gb_status page_rank_digraph(int device, uint32_t n, const uint32_t* in_off, const uint32_t* in_tgt,
-                                   const uint32_t* out_off, GraphPtr* g) {
-  GB_TRY(new_graph(device, GB_KIND_DIRECTED, n, g));
-  GB_TRY(upload_host_csr((*g)->stream, n, in_off, in_tgt, nullptr, &(*g)->in, "in"));
-  return upload_host_csr((*g)->stream, n, out_off, nullptr, nullptr, &(*g)->out, "out", true);
-}
-
 }  // namespace gb
 
 // ---- multi-GPU shard (1-D edge-cut by destination, 32-row slices dealt round-robin) ----------------
 struct gb_pr_shard {
-  const gb_graph* graph = nullptr;    // NULL for the shards of gb_pr_shards_csr_u32, which hold no graph
-  int device = 0;                     // the plan's device: gb_pr_shard_free must not read a freed graph
+  int device = 0;                     // the plan's device: a shard holds no graph, which may be freed before it
   gb::PrPlan* plan = nullptr;
   gb::DevBuf<void*> sync_table;       // device copy of the ranks' control-block pointers (gb_pr_shard_sync)
   void* sync_table_host[8] = {nullptr};
@@ -1210,12 +1208,8 @@ gb_status gb_pr_shard_create(const gb_graph* g, uint32_t rank, uint32_t world, g
   std::lock_guard<std::mutex> lock(g->mu);
   gb_pr_shard* sh = new (std::nothrow) gb_pr_shard();
   if (!sh) return gb::fail(GB_ERR_OOM, "host allocation failed");
-  sh->graph = g;
   sh->device = g->device;
-  gb::PrDeal deal;
-  deal.P = world;
-  deal.p = rank;
-  gb_status st = gb::build_pr_plan(g, deal, &sh->plan);
+  gb_status st = gb::build_pr_plan(g, gb::PrDeal(world, rank), &sh->plan);
   if (st != GB_OK) {
     delete sh;
     return st;
@@ -1356,47 +1350,6 @@ gb_status gb_page_rank(const gb_graph* graph, const gb_page_rank_config* config,
                        uint64_t* ran_iterations, double* error) {
   GB_REQUIRE(scores != nullptr, "scores is NULL");
   return gb::page_rank_impl(graph, config, nullptr, scores, ran_iterations, error);
-}
-
-// One-shot PageRank of a host CSR.  The 4 bytes per edge of the targets dominate the upload, so they are
-// streamed, as the one-rank case of the communicator's upload (pr_csr_plans, multi.cu): offsets first, then the
-// targets in row-aligned chunks on a copy stream, while the rank's stream sorts the degrees, picks the hot
-// blocks and classifies every chunk as it lands (layout_classify, pr_layout.cu).  Only the fill pass, the
-// sweeps and the copy of the ranks run after the last byte.  EXACT mode and small graphs upload everything
-// first.  GB_PR_FEED_CHUNKS (default 16 chunks of ceil(m / 16) edges; 0 = upload everything, then build) and
-// GB_PR_FEED_MIN_EDGES (default 2^22) are experiment knobs.
-gb_status gb_page_rank_csr_u32(int device, uint32_t n, const uint32_t* in_off, const uint32_t* in_tgt,
-                               const uint32_t* out_off, const gb_page_rank_config* config, float* scores,
-                               uint64_t* ran_iterations, double* error) {
-  GB_REQUIRE(scores != nullptr, "scores is NULL");
-  GB_TRY(gb::check_pr_host_csr(n, in_off, in_tgt, out_off));
-  const uint64_t m = in_off[n];
-  uint32_t chunks = (uint32_t)gb::env_u64("GB_PR_FEED_CHUNKS", 16);
-  if (m < (uint32_t)gb::env_u64("GB_PR_FEED_MIN_EDGES", 1u << 22)) chunks = 0;
-  // the single-warp EXACT mode (small graphs) reads the CSR directly: nothing to overlap
-  if (!config || config->mode == GB_PR_EXACT || (config->mode == GB_PR_AUTO && n <= 16384)) chunks = 0;
-  gb::GraphPtr g;
-  if (chunks == 0) {
-    GB_TRY(gb::page_rank_digraph(device, n, in_off, in_tgt, out_off, &g));
-    return gb::page_rank_impl(g.get(), config, nullptr, scores, ran_iterations, error);
-  }
-  // the graph brings the stream, the timing events and the lock; the sweeps read only the plan
-  GB_TRY(gb::new_graph(device, GB_KIND_DIRECTED, n, &g));
-  std::vector<gb::PrPlan*> plans;
-  GB_TRY(gb::pr_csr_plans({device}, 1, n, in_off, in_tgt, out_off, std::max<uint64_t>((m + chunks - 1) / chunks, 1),
-                          &plans));
-  g->pr_plan = plans[0];
-  return gb::page_rank_impl(g.get(), config, nullptr, scores, ran_iterations, error);
-}
-
-gb_status gb_digraph_for_page_rank_u32(int device, uint32_t n, const uint32_t* in_off, const uint32_t* in_tgt,
-                                       const uint32_t* out_off, gb_graph** graph) {
-  GB_REQUIRE(graph != nullptr, "graph is NULL");
-  GB_TRY(gb::check_pr_host_csr(n, in_off, in_tgt, out_off));
-  gb::GraphPtr g;
-  GB_TRY(gb::page_rank_digraph(device, n, in_off, in_tgt, out_off, &g));
-  *graph = g.release();
-  return GB_OK;
 }
 
 gb_status gb_page_rank_device(const gb_graph* graph, const gb_page_rank_config* config, float* d_scores,

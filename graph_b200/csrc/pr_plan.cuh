@@ -1,6 +1,6 @@
-// pr_plan.cuh — the JACOBI PageRank layout (PrPlan) and what its build (pr_layout.cu) and its sweep
-// (pagerank.cu) both need: the layout constants, the cyclic deal of rows over ranks, and the launch-shape
-// stage that ends the build.
+// pr_plan.cuh — the JACOBI PageRank layout (PrPlan) and what its build (pr_layout.cu), its sweep (pagerank.cu),
+// the host-CSR part pipeline (pr_csr.cu) and the communicator (multi.cu) share: the layout constants, the cyclic
+// deal of rows over ranks, the launch-shape stage that ends the build, and the rules every PageRank call keeps.
 #pragma once
 #include <cstdlib>
 #include <vector>
@@ -37,7 +37,9 @@ constexpr uint32_t CB_HEAD_CONT = 1u, CB_TAIL_CONT = 2u, CB_INTERIOR = 4u;
 
 // ---- the cyclic deal of 32-row slices over the ranks of the 1-D edge-cut ---------------------------
 struct PrDeal {
-  uint32_t P = 1, p = 0;
+  uint32_t P = 1, p = 0;  // rank p of P
+  PrDeal() = default;
+  PrDeal(uint32_t world, uint32_t rank) : P(world), p(rank) {}
 };
 __host__ __device__ __forceinline__ uint32_t deal_global(uint32_t l, uint32_t P, uint32_t p) {
   return (((l >> 5) * P + p) << 5) | (l & 31u);
@@ -166,20 +168,49 @@ gb_status build_pr_plan(const PrSource& src, PrDeal deal, const uint32_t* row_of
                         uint64_t row_entries, PrPlan** out_plan);
 // the layout of rank deal.p's rows of g: its in-CSR is both the degree and the row source
 gb_status build_pr_plan(const gb_graph* g, PrDeal deal, PrPlan** out_plan);
-// a shard of the sweep API that owns `plan` and no graph (gb_pr_shards_csr_u32; pagerank.cu)
-gb_status shard_from_plan(int device, PrPlan* plan, gb_pr_shard** out);
 
+// ---- the rules every PageRank call keeps (pagerank.cu) -----------------------------------------------------
+// GB_ERR_INVALID for a config that cannot stop: max_iterations == 0 (no sweep limit) with tolerance <= 0
+gb_status require_pr_config(const gb_page_rank_config* cfg);
+// max_iterations == 0 never satisfies `iteration == max_iterations` (page_rank.rs:107): the
+// reference then runs until the tolerance is met; we bound that at 100000 sweeps.
+uint64_t pr_sweep_limit(const gb_page_rank_config* cfg);
+// gb_page_rank / gb_page_rank_device: the ranks of g into d_scores (device) or h_scores (host), whichever is
+// given.  A g->pr_plan the caller has put there is used as it is; otherwise JACOBI builds it from g's in-CSR.
+gb_status page_rank_impl(const gb_graph* g, const gb_page_rank_config* cfg, float* d_scores, float* h_scores,
+                         uint64_t* ran, double* error);
+
+// a shard of the sweep API that owns `plan` (pagerank.cu); takes the plan, whatever it returns
+gb_status shard_from_plan(int device, PrPlan* plan, gb_pr_shard** out);
+// The shards of one call, freed together
+struct ShardSet {
+  std::vector<gb_pr_shard*> v;
+  explicit ShardSet(uint32_t count) : v(count, nullptr) {}
+  void clear() {
+    for (gb_pr_shard* sh : v)
+      if (sh) gb_pr_shard_free(sh);
+    v.clear();
+  }
+  ~ShardSet() { clear(); }
+};
+
+// ---- PageRank from a host CSR (pr_csr.cu) ------------------------------------------------------------------
 // The O(1) host checks of a host PageRank CSR (n + 1 in- and out-offsets, the in-targets), in the order and
-// with the messages of every entry point that takes one (multi.cu)
+// with the messages of every entry point that takes one
 gb_status check_pr_host_csr(uint32_t n, const uint32_t* in_off, const uint32_t* in_tgt, const uint32_t* out_off);
 // The layouts of ranks 0 .. U-1 (U = devs.size() * V, rank r on devs[r / V]) of a host CSR that passed
-// check_pr_host_csr (multi.cu).  Part u of the split (pr_split, targets in chunks of about chunk_edges >= 1
+// check_pr_host_csr.  Part u of the split (pr_split, targets in chunks of about chunk_edges >= 1
 // edges) is uploaded by the device of rank u; the offsets are checked on the device.  A lone rank builds its
 // layout from its part as the chunks land; with several, every rank gathers the rows it owns from all parts into
 // a local in-CSR first.  On success plans holds U plans, the caller's to free; on failure nothing is left.
 gb_status pr_csr_plans(const std::vector<int>& devs, uint32_t V, uint32_t n, const uint32_t* in_off,
                        const uint32_t* in_tgt, const uint32_t* out_off, uint64_t chunk_edges,
                        std::vector<PrPlan*>* plans);
+// check_pr_host_csr, then the plans of pr_csr_plans (chunks of GB_PR_PART_CHUNK_EDGES edges) as the shards of
+// ranks 0 .. U-1 of the sweep API: shards (U entries) are the caller's to free.
+gb_status pr_csr_shards(const std::vector<int>& devs, uint32_t V, uint32_t n, const uint32_t* in_off,
+                        const uint32_t* in_tgt, const uint32_t* out_off, std::vector<gb_pr_shard*>& shards);
+
 // launch shapes of the sweep kernels, their error buffers and k_pr_cb's shared-memory size (pagerank.cu).
 // h_nrows / h_poff: the staircase (nrows[], poff[]) as the layout build holds it on the host.
 gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, const std::vector<uint32_t>& h_poff,

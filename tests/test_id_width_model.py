@@ -112,8 +112,8 @@ def test_fixtures_touch_both_sides_of_half():
 
 
 # ---- loop counters -----------------------------------------------------------------------------------
-# The files whose kernels a graph with ids past 2^31 reaches.  pagerank.cu, pr_layout.cu and multi.cu are reached
-# by PageRank alone, which refuses node counts of 2^31 - 1 and more (require_pr_node_count, pr_layout.cu).
+# The files whose kernels a graph with ids past 2^31 reaches.  pagerank.cu, pr_layout.cu, pr_csr.cu and multi.cu are
+# reached by PageRank alone, which refuses node counts of 2^31 - 1 and more (require_pr_node_count, pr_layout.cu).
 SCANNED = ["graph.cu", "wcc.cu", "sssp.cu", "tc.cu", "load.cu"]
 # a loop strides over the grid when its step is the grid size or the grid's warp or thread count
 GRID_STEP = re.compile(r"gridDim|\bnwarps\b|\bnthreads\b|\bnw\b")
