@@ -22,7 +22,7 @@ from ._capi import GraphB200Error, check, lib
 __all__ = ["DiGraph", "Graph", "Layout", "FileFormat", "PageRankResult", "WccResult",
            "TriangleCountResult", "SsspResult", "PageRankConfig", "WccConfig", "DeltaSteppingConfig",
            "GraphB200Error", "device_count", "set_device", "write_graph500", "wcc_csr",
-           "triangle_count_csr"]
+           "triangle_count_csr", "sssp_csr"]
 
 _device = 0
 
@@ -224,9 +224,10 @@ class TriangleCountResult:
 
 
 class SsspResult:
-    def __init__(self, distances, micros):
+    def __init__(self, distances, micros, info=None):
         distances.flags.writeable = False
         self._distances, self.micros = distances, micros
+        self.info = info  # sssp_csr: the call's gb_sssp_csr_stats as a dict
 
     def distances(self) -> np.ndarray:
         return self._distances
@@ -805,3 +806,34 @@ def triangle_count_csr(offsets, targets) -> TriangleCountResult:
     info = _capi.TcCsrInfo()
     check(lib.gb_triangle_count_csr_info(C.byref(info)))
     return TriangleCountResult(int(tri.value), micros, info.as_dict())
+
+
+def sssp_csr(offsets, targets, weights, *, start_node: int, delta: float) -> SsspResult:
+    """delta_stepping (sssp.rs:38-102) of a host weighted out-CSR without a resident twin and without its
+    transpose: the distances DiGraph.from_csr(...).delta_stepping() gives for the same arrays, bit for bit.  The
+    offsets are uploaded first; the targets and their f32 weights follow in row-aligned chunks, from the start's
+    chunk on, and the bucket loop runs while they land: a queued vertex whose row is not on the device yet is
+    parked and relaxed once it is.  The CSR is freed before the call returns.  Arrays are used as given: pass
+    pinned contiguous arrays (uint32 offsets and targets, float32 weights) to overlap the passes with the copy.
+    `weights` may be None only when there are no edges.  `info` on the result holds the call's chunk count, h2d
+    bytes, parked vertices, pass counts and device times."""
+    off, tgt = _host_csr_arrays(offsets, targets, "sssp_csr", "out")
+    w = None
+    if weights is not None:
+        w = np.asarray(weights)
+        if w.dtype != np.float32 or not w.flags.c_contiguous:
+            raise TypeError("sssp_csr needs contiguous float32 weights")
+        if w.ndim != 1 or len(w) < int(off[-1]):
+            raise ValueError(f"weights hold {len(w)} entries but the offsets end at {int(off[-1])}")
+    if start_node < 0:
+        raise ValueError("start_node must be non-negative")
+    cfg = _capi.SsspConfig(int(start_node), float(delta))
+    dist = np.empty(len(off) - 1, np.float32)
+
+    def go():
+        check(lib.gb_sssp_csr_u32(_device, len(off) - 1, _ptr(off), _ptr(tgt) if len(tgt) else None,
+                                  _ptr(w) if w is not None and len(w) else None, C.byref(cfg), _ptr(dist)))
+    _, micros = _timed(go)
+    info = _capi.SsspCsrInfo()
+    check(lib.gb_sssp_csr_info(C.byref(info)))
+    return SsspResult(dist, micros, info.as_dict())

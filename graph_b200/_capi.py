@@ -82,6 +82,17 @@ class TcCsrInfo(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_ if k != "reserved"}
 
 
+class SsspCsrInfo(C.Structure):
+    _fields_ = [("chunks", C.c_uint64), ("chunk_entries", C.c_uint64), ("h2d_bytes", C.c_uint64),
+                ("parked", C.c_uint64), ("unpark_rounds", C.c_uint64), ("passes", C.c_uint64),
+                ("passes_before_last_landed", C.c_uint64), ("kernel_launches", C.c_uint64),
+                ("pinned", C.c_uint32), ("start_chunk", C.c_uint32), ("upload_ms", C.c_double),
+                ("total_ms", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class GraphB200Error(RuntimeError):
     """CUDA / allocation failure inside libgraph_b200."""
 
@@ -138,6 +149,8 @@ SIGNATURES = {
     "gb_wcc_sample_label": (C.c_int, [_P, C.POINTER(WccConfig), _P, C.POINTER(C.c_uint32), C.POINTER(C.c_int), _P]),
     "gb_sssp": (C.c_int, [_P, C.POINTER(SsspConfig), _P]),
     "gb_sssp_device": (C.c_int, [_P, C.POINTER(SsspConfig), _P]),
+    "gb_sssp_csr_u32": (C.c_int, [C.c_int, C.c_uint32, _P, _P, _P, C.POINTER(SsspConfig), _P]),
+    "gb_sssp_csr_info": (C.c_int, [C.POINTER(SsspCsrInfo)]),
     "gb_triangle_count": (C.c_int, [_P, C.POINTER(C.c_uint64)]),
     "gb_triangle_count_csr_u32": (C.c_int, [C.c_int, C.c_uint32, _P, _P, C.POINTER(C.c_uint64)]),
     "gb_triangle_count_csr_info": (C.c_int, [C.POINTER(TcCsrInfo)]),

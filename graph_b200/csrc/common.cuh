@@ -152,6 +152,8 @@ struct PeerBuf {
 // and must enqueue that record before send(k + R) is called: cudaStreamWaitEvent takes the event's latest
 // record at the time of the call, so every wait then refers to a record already enqueued, and a pageable copy,
 // which returns only once its stream has drained, blocks the host only until work already enqueued has run.
+// A resident feed may carry one f32 value per target (val, asked for with `values`): chunk k's values are
+// copied right after its targets, with the same bounds, before landed[k].
 // The consumers' streams are the caller's, and must drain before the feed goes.
 struct CsrFeed {
   int dev = -1;
@@ -161,17 +163,19 @@ struct CsrFeed {
   cudaEvent_t offsets_in = nullptr;
   PeerBuf off, off2;                      // [r_end - r_begin + 1] each; off2 only with a second offsets array
   PeerBuf tgt;                            // resident: [e_end - e_begin] + 8 zeroed
+  DevBuf<float> val;                      // resident with values: [e_end - e_begin]
   std::vector<DevBuf<uint32_t>> ring;     // ring: R slots of `slot` entries + 8 zeroed
   std::vector<cudaEvent_t> landed, freed; // resident: landed[K]; ring: landed[R], freed[R]
 
   // makes dev current, creates the stream and offsets_in and allocates the offsets (peers: PeerBuf)
   gb_status open(int device, uint32_t rb, uint32_t re, bool peers, bool two_offsets = false);
-  gb_status resident(uint64_t eb, uint64_t ee, uint32_t chunks, bool peers);
+  gb_status resident(uint64_t eb, uint64_t ee, uint32_t chunks, bool peers, bool values = false);
   gb_status open_ring(uint32_t slots, uint64_t slot);
   // copies off[r_begin .. r_end] (and off2's) and records offsets_in
   gb_status send_offsets(const uint32_t* host_off, const uint32_t* host_off2 = nullptr);
-  // chunk k = the targets [e0, e0 + len) of host_tgt; an empty chunk only records its event
-  gb_status send(uint64_t k, const uint32_t* host_tgt, uint64_t e0, uint64_t len);
+  // chunk k = the targets [e0, e0 + len) of host_tgt (and the same values of host_val, for a feed with values);
+  // an empty chunk only records its event
+  gb_status send(uint64_t k, const uint32_t* host_tgt, uint64_t e0, uint64_t len, const float* host_val = nullptr);
   // on s, behind offsets_in: bad[0] += the rows v in [r0, r1) with off[v] > off[v + 1], bad[1] the same of off2
   gb_status check_monotone(cudaStream_t s, uint32_t r0, uint32_t r1, unsigned int* bad) const;
   // whether host memory is page-locked: such a copy does not wait for its stream to drain

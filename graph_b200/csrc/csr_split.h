@@ -158,4 +158,18 @@ inline CsrChunks tc_split(const uint32_t* off, uint32_t n, uint64_t chunk_entrie
   return c;
 }
 
+// ---- SSSP (gb_sssp_csr_u32): the chunks of tc_split, sent from the start's chunk on ------------------------------
+// The send order of the chunks c (row[0] == 0, strictly increasing rows, row[K] == n > start): the chunk that
+// holds row `start` first, then the chunks after it, wrapping round to chunk 0.  The first j chunks of this order
+// hold one cyclic interval of rows, [row[ks], row[ks + j]) read modulo n, so "is u's row on the device" is a
+// distance from row[ks] compared with the number of rows sent.
+inline std::vector<uint32_t> sssp_send_order(const CsrChunks& c, uint32_t start) {
+  const uint32_t K = c.count();
+  // the last chunk whose first row is <= start
+  const uint32_t ks = (uint32_t)(std::upper_bound(c.row.begin(), c.row.end() - 1, start) - c.row.begin()) - 1;
+  std::vector<uint32_t> order(K);
+  for (uint32_t j = 0; j < K; ++j) order[j] = ks + j < K ? ks + j : ks + j - K;
+  return order;
+}
+
 }  // namespace gb

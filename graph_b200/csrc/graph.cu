@@ -372,10 +372,11 @@ gb_status CsrFeed::open(int device, uint32_t rb, uint32_t re, bool peers, bool t
   return GB_OK;
 }
 
-gb_status CsrFeed::resident(uint64_t eb, uint64_t ee, uint32_t chunks, bool peers) {
+gb_status CsrFeed::resident(uint64_t eb, uint64_t ee, uint32_t chunks, bool peers, bool values) {
   e_begin = eb;
   GB_TRY(tgt.alloc(ee - eb, peers, 8));
   GB_CUDA(cudaMemsetAsync(tgt.p + (ee - eb), 0, 8 * 4, copy));
+  if (values) GB_TRY(val.alloc(ee - eb));
   landed.assign(chunks, nullptr);
   for (cudaEvent_t& ev : landed) GB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
   return GB_OK;
@@ -402,10 +403,12 @@ gb_status CsrFeed::send_offsets(const uint32_t* host_off, const uint32_t* host_o
   return GB_OK;
 }
 
-gb_status CsrFeed::send(uint64_t k, const uint32_t* host_tgt, uint64_t e0, uint64_t len) {
+gb_status CsrFeed::send(uint64_t k, const uint32_t* host_tgt, uint64_t e0, uint64_t len, const float* host_val) {
   uint32_t* dst = ring.empty() ? tgt.p + (e0 - e_begin) : ring[k % ring.size()].p;
   if (!ring.empty() && k >= ring.size()) GB_CUDA(cudaStreamWaitEvent(copy, freed[k % ring.size()], 0));
   if (len) GB_CUDA(cudaMemcpyAsync(dst, host_tgt + e0, len * 4, cudaMemcpyHostToDevice, copy));
+  if (len && val.p)
+    GB_CUDA(cudaMemcpyAsync(val.p + (e0 - e_begin), host_val + e0, len * 4, cudaMemcpyHostToDevice, copy));
   GB_CUDA(cudaEventRecord(landed[k % landed.size()], copy));
   return GB_OK;
 }
@@ -429,6 +432,7 @@ CsrFeed::~CsrFeed() {
   cudaSetDevice(dev);
   if (copy) cudaStreamSynchronize(copy);
   ring.clear();
+  val.release();
   tgt.release();
   off2.release();
   off.release();

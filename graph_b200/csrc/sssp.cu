@@ -9,10 +9,26 @@
 // unique, so results are bit-exact with the reference for every schedule and every delta.
 //
 // Algorithmic bytes per run: 8m + 4(n+1) + 8n (weighted out-CSR once, distances read + write).
+//
+// One-shot SSSP of a host out-CSR (gb_sssp_csr_u32).  The offsets go first and are checked; the targets and
+// their f32 values follow in the row-aligned chunks of tc_split (csr_split.h), sent from the chunk that holds the
+// start on and wrapping round (sssp_send_order), into one resident CSR.  A chunk is available once its id check
+// has passed, and the available rows are then one cyclic interval from the start's chunk (SsspRows).  The bucket
+// loop is the twin's, with one change in k_sssp_relax<true>: a queue entry whose row is not available yet is
+// not relaxed but PARKED, once per vertex, in a parked list; between passes the host raises the available bound
+// and k_sssp_unpark moves the parked vertices whose rows are now present into the near queue.  When only parked
+// vertices are left the host blocks on the next chunk.
+// Parking breaks what the stale filter (`du < lower`) relies on: that a vertex below the current bucket was
+// relaxed with its final distance while its bucket drained.  A parked vertex relaxed late can improve a vertex
+// of a drained bucket to a distance below `lower`, and that vertex must be relaxed again.  So from the first park
+// on the relax passes take lower = 0 and drop nothing: every strict improvement is then relaxed once its row is
+// present, and the loop still ends at the unique fixed point above (SURVEY.md A.4), bit-equal to the twin.
 #include <algorithm>
 #include <cfloat>
+#include <vector>
 
 #include "common.cuh"
+#include "csr_split.h"
 #include "sssp_bucket.h"
 
 namespace gb {
@@ -58,6 +74,19 @@ struct SsspStamps {
   uint32_t* in_pile;
   uint32_t pass;
 };
+
+// The rows a relax pass may read: `span` rows from row `first` on, modulo n (the chunks sent and checked so
+// far, gb_sssp_csr_u32).  parked[u] is 1 while u has an entry in the parked list, so that the list holds a
+// vertex once, as in_pile does for the far pile; counts[4] is the list's length.  The twin's instantiation
+// of k_sssp_relax does not read it.
+struct SsspRows {
+  uint32_t first, span, n;
+  uint32_t* parked;
+  __device__ __forceinline__ bool present(uint32_t u) const {
+    return (u >= first ? u - first : u + (n - first)) < span;
+  }
+};
+
 __device__ __forceinline__ void sssp_relax_edge(const uint32_t* __restrict__ tgt, const float* __restrict__ w,
                                                 uint32_t* dist, uint32_t i, float du, float upper,
                                                 uint32_t* __restrict__ near_out, uint32_t* __restrict__ far,
@@ -81,10 +110,13 @@ __device__ __forceinline__ void sssp_relax_edge(const uint32_t* __restrict__ tgt
   }
 }
 
+// kPark: an entry whose row is not in `rows` is appended to park_list (once per vertex) instead of relaxed
+template <bool kPark>
 __global__ void k_sssp_relax(const uint32_t* __restrict__ off, const uint32_t* __restrict__ tgt,
                              const float* __restrict__ w, uint32_t* dist, const uint32_t* __restrict__ queue,
                              uint32_t count, float lower, float upper, uint32_t* __restrict__ near_out,
-                             uint32_t* __restrict__ far, uint32_t* counts, uint32_t cap, const SsspStamps st) {
+                             uint32_t* __restrict__ far, uint32_t* counts, uint32_t cap, const SsspStamps st,
+                             const SsspRows rows, uint32_t* __restrict__ park_list) {
   const uint32_t lane = threadIdx.x & 31;
   const uint64_t nthreads = (uint64_t)gridDim.x * blockDim.x;
   for (uint64_t qb = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) & ~31ull; qb < count; qb += nthreads) {
@@ -96,6 +128,13 @@ __global__ void k_sssp_relax(const uint32_t* __restrict__ off, const uint32_t* _
       const uint32_t u = queue[q];
       du = __uint_as_float(*((volatile uint32_t*)(dist + u)));
       live = !(du < lower);  // stale entry: settled in an earlier bucket (sssp.rs:126)
+      if (kPark && live && !rows.present(u)) {
+        if (atomicExch(rows.parked + u, 1u) == 0u) {
+          const uint32_t pos = sssp_reserve(counts + 4);
+          if (pos < cap) park_list[pos] = u;
+        }
+        live = false;
+      }
       if (live) {
         b = off[u];
         e = off[u + 1];
@@ -113,6 +152,27 @@ __global__ void k_sssp_relax(const uint32_t* __restrict__ off, const uint32_t* _
       const float odu = __shfl_sync(0xFFFFFFFFu, du, owner);
       for (uint32_t i = ob + lane; i < oe; i += 32)
         sssp_relax_edge(tgt, w, dist, i, odu, upper, near_out, far, counts, cap, st);
+    }
+  }
+}
+
+// The parked vertices whose rows are now in `rows` leave the list (clearing their flag) for the near queue,
+// appended after its counts[0] entries and stamped with the pass that filled it, so that a vertex already
+// queued there is not queued twice; the rest are carried to parked_out (counts[5]).
+__global__ void k_sssp_unpark(const uint32_t* __restrict__ parked, uint32_t count, const SsspRows rows,
+                              uint32_t* __restrict__ near_out, uint32_t* __restrict__ parked_out, uint32_t* counts,
+                              uint32_t cap, const SsspStamps st) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t u = parked[i];
+    if (rows.present(u)) {
+      rows.parked[u] = 0u;
+      if (atomicMax(st.near_stamp + u, st.pass) < st.pass) {
+        const uint32_t pos = sssp_reserve(counts + 0);
+        if (pos < cap) near_out[pos] = u;
+      }
+    } else {
+      const uint32_t pos = sssp_reserve(counts + 5);
+      if (pos < cap) parked_out[pos] = u;
     }
   }
 }
@@ -151,6 +211,249 @@ __global__ void k_sssp_min_far(const uint32_t* __restrict__ dist, const uint32_t
   if ((threadIdx.x & 31) == 0 && best != 0xFFFFFFFFu) atomicMin(min_bits, best);
 }
 
+// ---- the one-shot call's chunks (gb_sssp_csr_u32) ---------------------------------------------------------------
+// C, the entries per chunk: GB_SSSP_FEED_ENTRIES when set, else ceil(m / 16) but at least 2^20; never below
+// ceil(m / 4096) (the triangle count's rule)
+constexpr uint64_t SSSP_FEED_CHUNKS = 16;
+constexpr uint64_t SSSP_FEED_MIN_ENTRIES = 1u << 20;
+constexpr uint64_t SSSP_FEED_MAX_CHUNKS = 4096;
+
+thread_local gb_sssp_csr_stats sssp_csr_last{};  // behind gb_sssp_csr_info
+
+// Everything one call holds besides its work buffers.  Chunks go out in send order; `avail` of them (a prefix of
+// that order) have passed their checks and may be read by the compute stream, which waits on the last one's
+// `checked` event.  The destructor drains the streams before anything they use goes: the page-locked tally, the
+// events, the buffers and the feed (the first member).
+struct SsspCsrCall {
+  CsrFeed feed;  // the offsets [0, n], the resident targets and values, one landed event per chunk
+  DevBuf<unsigned int> bad;      // [0] rows whose offsets decrease, [1 + k] targets >= n in chunk k
+  unsigned int* h_bad = nullptr;  // page-locked: bad[1 + K]
+  cudaStream_t check = nullptr, compute = nullptr;
+  cudaEvent_t begin = nullptr, uploaded = nullptr, end = nullptr;  // timed
+  cudaEvent_t offsets_checked = nullptr;
+  std::vector<cudaEvent_t> checked;  // [j]: behind the checks of the j-th chunk of the send order
+  CsrChunks ch;
+  std::vector<uint32_t> order;
+  const uint32_t* tgt = nullptr;
+  const float* w = nullptr;
+  uint32_t n = 0, K = 0, issued = 0, avail = 0;
+  uint64_t step = 0;  // GB_SSSP_FEED_STEP: the j-th chunk goes out after j * step passes, and is waited for
+  bool pinned = false;
+  gb_sssp_csr_stats info{};
+
+  gb_status create() {
+    GB_CUDA(cudaStreamCreateWithFlags(&check, cudaStreamNonBlocking));
+    GB_CUDA(cudaStreamCreateWithFlags(&compute, cudaStreamNonBlocking));
+    for (cudaEvent_t* e : {&begin, &uploaded, &end}) GB_CUDA(cudaEventCreate(e));
+    GB_CUDA(cudaEventCreateWithFlags(&offsets_checked, cudaEventDisableTiming));
+    checked.assign(K, nullptr);
+    for (uint32_t j = 0; j < K; ++j) GB_CUDA(cudaEventCreateWithFlags(&checked[j], cudaEventDisableTiming));
+    GB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h_bad), ((size_t)K + 1) * 4, cudaHostAllocDefault));
+    return GB_OK;
+  }
+  ~SsspCsrCall() {
+    for (cudaStream_t s : {check, compute})
+      if (s) cudaStreamSynchronize(s);
+    for (cudaEvent_t e : checked)
+      if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : {begin, uploaded, end, offsets_checked})
+      if (e) cudaEventDestroy(e);
+    for (cudaStream_t s : {check, compute})
+      if (s) cudaStreamDestroy(s);
+    if (h_bad) cudaFreeHost(h_bad);
+  }
+
+  // the next chunk of the send order: its copy, then its id check behind its landing
+  gb_status issue() {
+    const uint32_t j = issued++, k = order[j];
+    const uint64_t e0 = ch.edge[k], e1 = ch.edge[k + 1];
+    GB_TRY(feed.send(k, tgt, e0, e1 - e0, w));
+    if (issued == K) GB_CUDA(cudaEventRecord(uploaded, feed.copy));
+    GB_CUDA(cudaStreamWaitEvent(check, feed.landed[k], 0));
+    if (e1 > e0) {
+      check_ids_async(check, feed.tgt.p + e0, e1 - e0, n, bad.p + 1 + k);
+      info.kernel_launches += 1;
+    }
+    GB_CUDA(cudaGetLastError());
+    GB_CUDA(cudaMemcpyAsync(h_bad + 1 + k, bad.p + 1 + k, 4, cudaMemcpyDeviceToHost, check));
+    GB_CUDA(cudaEventRecord(checked[j], check));
+    return GB_OK;
+  }
+  // once a relax pass is launched: from pageable memory the copies are synchronous, one chunk per pass
+  gb_status after_launch() {
+    info.passes += 1;
+    if (avail < K) info.passes_before_last_landed += 1;
+    if (!pinned && !step && issued < K) GB_TRY(issue());
+    return GB_OK;
+  }
+  // every chunk checked: the verdict of gb_digraph_from_csr_u32 on the targets
+  gb_status check_all() {
+    while (issued < K) GB_TRY(issue());
+    GB_CUDA(cudaStreamSynchronize(check));
+    uint64_t nbad = 0;
+    for (uint32_t k = 0; k < K; ++k) nbad += h_bad[1 + k];
+    return require_ids("out", nbad, n);
+  }
+  // Raises avail over the chunks whose checks have passed, without waiting, unless the step rule sends and
+  // waits for chunks or `block` asks for one more chunk at least.  A chunk that failed stops the call.
+  gb_status poll(bool block, bool* raised) {
+    const uint32_t was = avail;
+    if (step)
+      while (issued < K && issued * step <= info.passes) GB_TRY(issue());
+    if (block && avail == issued) {
+      if (issued == K) return fail(GB_ERR_CUDA, "sssp: parked vertices with every chunk available");
+      GB_TRY(issue());
+    }
+    while (avail < issued) {
+      if (step || (block && avail == was)) {
+        GB_CUDA(cudaEventSynchronize(checked[avail]));
+      } else {
+        const cudaError_t e = cudaEventQuery(checked[avail]);
+        if (e == cudaErrorNotReady) break;
+        GB_CUDA(e);
+      }
+      if (h_bad[1 + order[avail]]) return check_all();
+      ++avail;
+    }
+    *raised = avail > was;
+    if (*raised) GB_CUDA(cudaStreamWaitEvent(compute, checked[avail - 1], 0));
+    return GB_OK;
+  }
+  SsspRows rows(uint32_t* parked) const {
+    const uint32_t first = ch.row[order[0]];
+    uint32_t span = avail ? n : 0u;
+    if (avail && avail < K) {
+      const uint32_t stop = ch.row[order[avail]];  // the first row not yet available
+      span = stop > first ? stop - first : stop + (n - first);
+    }
+    return SsspRows{first, span, n, parked};
+  }
+};
+
+// ---- the bucket loop ----------------------------------------------------------------------------------------
+// The device buffers of one run; the parked list and flags only with a feed
+struct SsspWork {
+  DevBuf<uint32_t> qa, qb, fa, fb, counts, minb, near_stamp, in_pile;
+  DevBuf<uint32_t> pa, pb, parked;
+};
+
+// Delta-stepping from `start` over the out-CSR (off, tgt, w) on stream s, into dist.  Without a feed every row is
+// present (gb_sssp); with one (gb_sssp_csr_u32) the rows are those of feed->rows() and the loop parks, unparks
+// and waits for chunks as the header of this file says.
+static gb_status sssp_loop(cudaStream_t s, uint32_t n, const uint32_t* off, const uint32_t* tgt, const float* w,
+                           uint32_t* dist, uint32_t start, float delta, SsspWork& wk, SsspCsrCall* feed,
+                           uint64_t* launches) {
+  const unsigned blk = 256;
+  const uint32_t cap = n;
+  SsspStamps st{wk.near_stamp.p, wk.in_pile.p, 0u};
+  uint32_t* counts = wk.counts.p;
+  k_sssp_init<<<grid_for(n, blk), blk, 0, s>>>(dist, n, start);
+  GB_CUDA(cudaMemcpyAsync(wk.qa.p, &start, 4, cudaMemcpyHostToDevice, s));
+  *launches += 1;
+  uint32_t* near_in = wk.qa.p;
+  uint32_t* near_out = wk.qb.p;
+  uint32_t* far = wk.fa.p;
+  uint32_t* far_out = wk.fb.p;
+  uint32_t near_count = 1, far_count = 0, parked_count = 0;
+  float lower = 0.0f, upper = delta;  // the current bucket (sssp_bucket.h)
+  uint32_t h_counts[6];
+  SsspRows rows = feed ? feed->rows(wk.parked.p) : SsspRows{0u, n, n, nullptr};
+  bool any_parked = false;  // from the first park on, no pass drops an entry by `du < lower`
+  // the parked vertices whose rows are present now go to the near queue, after its near_count entries
+  auto unpark = [&]() -> gb_status {
+    rows = feed->rows(wk.parked.p);
+    const uint32_t set[6] = {near_count, far_count, 0u, 0u, parked_count, 0u};
+    GB_CUDA(cudaMemcpyAsync(counts, set, 24, cudaMemcpyHostToDevice, s));
+    k_sssp_unpark<<<grid_for(parked_count, blk), blk, 0, s>>>(wk.pa.p, parked_count, rows, near_in, wk.pb.p, counts,
+                                                              cap, st);
+    *launches += 1;
+    GB_CUDA(cudaMemcpyAsync(h_counts, counts, 24, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaStreamSynchronize(s));
+    if (h_counts[0] > cap || h_counts[5] > cap) return fail(GB_ERR_OOM, "sssp work queue overflow");
+    near_count = h_counts[0];
+    parked_count = h_counts[5];
+    std::swap(wk.pa.p, wk.pb.p);
+    feed->info.unpark_rounds += 1;
+    return GB_OK;
+  };
+  for (;;) {
+    // drain the near queue of this bucket
+    while (near_count > 0) {
+      st.pass += 1;
+      if (!feed) {
+        const uint32_t zero2[2] = {0u, far_count};
+        GB_CUDA(cudaMemcpyAsync(counts, zero2, 8, cudaMemcpyHostToDevice, s));
+        k_sssp_relax<false><<<grid_for((uint64_t)near_count, blk), blk, 0, s>>>(
+            off, tgt, w, dist, near_in, near_count, lower, upper, near_out, far, counts, cap, st, rows, nullptr);
+      } else {
+        const uint32_t zero5[5] = {0u, far_count, 0u, 0u, parked_count};
+        GB_CUDA(cudaMemcpyAsync(counts, zero5, 20, cudaMemcpyHostToDevice, s));
+        k_sssp_relax<true><<<grid_for((uint64_t)near_count, blk), blk, 0, s>>>(
+            off, tgt, w, dist, near_in, near_count, any_parked ? 0.0f : lower, upper, near_out, far, counts, cap, st,
+            rows, wk.pa.p);
+        GB_TRY(feed->after_launch());
+      }
+      *launches += 1;
+      GB_CUDA(cudaMemcpyAsync(h_counts, counts, feed ? 20 : 8, cudaMemcpyDeviceToHost, s));
+      GB_CUDA(cudaStreamSynchronize(s));
+      if (h_counts[0] > cap || h_counts[1] > cap) return fail(GB_ERR_OOM, "sssp work queue overflow");
+      near_count = h_counts[0];
+      far_count = h_counts[1];
+      std::swap(near_in, near_out);
+      if (feed) {
+        if (h_counts[4] > cap) return fail(GB_ERR_OOM, "sssp work queue overflow");
+        feed->info.parked += h_counts[4] - parked_count;
+        parked_count = h_counts[4];
+        any_parked = any_parked || parked_count > 0;
+        bool raised = false;
+        GB_TRY(feed->poll(false, &raised));
+        if (raised) rows = feed->rows(wk.parked.p);
+        if (raised && parked_count > 0) GB_TRY(unpark());
+      }
+    }
+    if (far_count > 0) {
+      // next non-empty bucket: the smallest live distance in the far pile decides (min_non_empty_bin,
+      // sssp.rs:159-168)
+      const uint32_t inf = 0xFFFFFFFFu;
+      GB_CUDA(cudaMemcpyAsync(wk.minb.p, &inf, 4, cudaMemcpyHostToDevice, s));
+      k_sssp_min_far<<<grid_for(far_count, blk), blk, 0, s>>>(dist, far, far_count, upper, wk.minb.p);
+      uint32_t h_min = inf;
+      GB_CUDA(cudaMemcpyAsync(&h_min, wk.minb.p, 4, cudaMemcpyDeviceToHost, s));
+      GB_CUDA(cudaStreamSynchronize(s));
+      *launches += 1;
+      if (h_min != inf) {
+        float dmin;
+        memcpy(&dmin, &h_min, 4);
+        const SsspBucket next = sssp_next_bucket(dmin, delta, upper);
+        lower = next.lower;
+        upper = next.upper;
+        const uint32_t zero3[3] = {0u, 0u, 0u};
+        GB_CUDA(cudaMemcpyAsync(counts, zero3, 12, cudaMemcpyHostToDevice, s));
+        // anything below lower in the pile was settled (its distance was final when its bucket drained)
+        k_sssp_split_far<<<grid_for(far_count, blk), blk, 0, s>>>(dist, far, far_count, 0.0f, upper, near_in,
+                                                                 far_out, counts, cap, st.in_pile);
+        *launches += 1;
+        GB_CUDA(cudaMemcpyAsync(h_counts, counts, 12, cudaMemcpyDeviceToHost, s));
+        GB_CUDA(cudaStreamSynchronize(s));
+        near_count = h_counts[0];
+        far_count = h_counts[2];
+        std::swap(far, far_out);
+        continue;
+      }
+      // everything left in the pile is stale: each of its vertices was improved below the pile's bucket since,
+      // and was queued near then
+      far_count = 0;
+    }
+    if (!feed || parked_count == 0) break;
+    // only parked vertices are left: wait for the next chunk
+    bool raised = false;
+    GB_TRY(feed->poll(true, &raised));
+    GB_TRY(unpark());
+  }
+  GB_CUDA(cudaGetLastError());
+  return GB_OK;
+}
+
 static gb_status sssp_impl(const gb_graph* g, const gb_sssp_config* cfg, float* d_dist, float* h_dist) {
   GB_REQUIRE(g && cfg, "NULL argument");
   if (g->kind != GB_KIND_DIRECTED) return fail(GB_ERR_UNSUPPORTED, "sssp needs a directed graph");
@@ -163,7 +466,6 @@ static gb_status sssp_impl(const gb_graph* g, const gb_sssp_config* cfg, float* 
   std::lock_guard<std::mutex> lock(g->mu);
   cudaStream_t s = g->stream;
   const uint32_t n = g->n;
-  const uint64_t m = g->out.len;
   DevBuf<float> tmp;
   if (!d_dist) {
     GB_TRY(tmp.alloc(n));
@@ -171,89 +473,117 @@ static gb_status sssp_impl(const gb_graph* g, const gb_sssp_config* cfg, float* 
   }
   uint32_t* dist = reinterpret_cast<uint32_t*>(d_dist);
   // a vertex is appended at most once per pass to the near queue (near stamps), and the far pile holds it
-  // at most once (in_pile): n bounds every queue for every delta (the overflow check below is an
+  // at most once (in_pile): n bounds every queue for every delta (the overflow check in the loop is an
   // internal-error guard only)
-  (void)m;
   const uint32_t cap = n;
-  DevBuf<uint32_t> qa, qb, fa, fb, counts, minb, near_stamp, in_pile;
-  GB_TRY(near_stamp.alloc(n));
-  GB_TRY(in_pile.alloc(n));
-  GB_CUDA(cudaMemsetAsync(near_stamp.p, 0, (size_t)n * 4, s));
-  GB_CUDA(cudaMemsetAsync(in_pile.p, 0, (size_t)n * 4, s));
-  SsspStamps st{near_stamp.p, in_pile.p, 0u};
-  GB_TRY(qa.alloc(cap));
-  GB_TRY(qb.alloc(cap));
-  GB_TRY(fa.alloc(cap));
-  GB_TRY(fb.alloc(cap));
-  GB_TRY(counts.alloc(4));
-  GB_TRY(minb.alloc(1));
+  SsspWork wk;
+  GB_TRY(wk.near_stamp.alloc(n));
+  GB_TRY(wk.in_pile.alloc(n));
+  GB_CUDA(cudaMemsetAsync(wk.near_stamp.p, 0, (size_t)n * 4, s));
+  GB_CUDA(cudaMemsetAsync(wk.in_pile.p, 0, (size_t)n * 4, s));
+  GB_TRY(wk.qa.alloc(cap));
+  GB_TRY(wk.qb.alloc(cap));
+  GB_TRY(wk.fa.alloc(cap));
+  GB_TRY(wk.fb.alloc(cap));
+  GB_TRY(wk.counts.alloc(4));
+  GB_TRY(wk.minb.alloc(1));
   g->timing = gb_timing{};
   GB_CUDA(cudaEventRecord(g->ev_begin, s));
-  const unsigned blk = 256;
-  k_sssp_init<<<grid_for(n, blk), blk, 0, s>>>(dist, n, (uint32_t)cfg->start_node);
-  const uint32_t start = (uint32_t)cfg->start_node;
-  GB_CUDA(cudaMemcpyAsync(qa.p, &start, 4, cudaMemcpyHostToDevice, s));
-  g->timing.kernel_launches += 1;
-  uint32_t* near_in = qa.p;
-  uint32_t* near_out = qb.p;
-  uint32_t* far = fa.p;
-  uint32_t* far_out = fb.p;
-  uint32_t near_count = 1, far_count = 0;
-  const float delta = cfg->delta;
-  float lower = 0.0f, upper = delta;  // the current bucket (sssp_bucket.h)
-  uint32_t h_counts[4];
-  for (;;) {
-    // drain the near queue of this bucket
-    while (near_count > 0) {
-      const uint32_t zero2[2] = {0u, far_count};
-      GB_CUDA(cudaMemcpyAsync(counts.p, zero2, 8, cudaMemcpyHostToDevice, s));
-      st.pass += 1;
-      k_sssp_relax<<<grid_for((uint64_t)near_count, blk), blk, 0, s>>>(
-          g->out.off.p, g->out.tgt.p, g->out.w.p, dist, near_in, near_count, lower, upper, near_out, far,
-          counts.p, cap, st);
-      g->timing.kernel_launches += 1;
-      GB_CUDA(cudaMemcpyAsync(h_counts, counts.p, 8, cudaMemcpyDeviceToHost, s));
-      GB_CUDA(cudaStreamSynchronize(s));
-      if (h_counts[0] > cap || h_counts[1] > cap) return fail(GB_ERR_OOM, "sssp work queue overflow");
-      near_count = h_counts[0];
-      far_count = h_counts[1];
-      std::swap(near_in, near_out);
-    }
-    if (far_count == 0) break;
-    // next non-empty bucket: the smallest live distance in the far pile decides (min_non_empty_bin,
-    // sssp.rs:159-168)
-    const uint32_t inf = 0xFFFFFFFFu;
-    GB_CUDA(cudaMemcpyAsync(minb.p, &inf, 4, cudaMemcpyHostToDevice, s));
-    k_sssp_min_far<<<grid_for(far_count, blk), blk, 0, s>>>(dist, far, far_count, upper, minb.p);
-    uint32_t h_min = inf;
-    GB_CUDA(cudaMemcpyAsync(&h_min, minb.p, 4, cudaMemcpyDeviceToHost, s));
-    GB_CUDA(cudaStreamSynchronize(s));
-    g->timing.kernel_launches += 1;
-    if (h_min == inf) break;  // everything left in the pile is stale
-    float dmin;
-    memcpy(&dmin, &h_min, 4);
-    const SsspBucket next = sssp_next_bucket(dmin, delta, upper);
-    lower = next.lower;
-    upper = next.upper;
-    const uint32_t zero3[3] = {0u, 0u, 0u};
-    GB_CUDA(cudaMemcpyAsync(counts.p, zero3, 12, cudaMemcpyHostToDevice, s));
-    // anything below lower in the pile was settled (its distance was final when its bucket drained)
-    k_sssp_split_far<<<grid_for(far_count, blk), blk, 0, s>>>(dist, far, far_count, 0.0f, upper, near_in, far_out,
-                                                             counts.p, cap, st.in_pile);
-    g->timing.kernel_launches += 1;
-    GB_CUDA(cudaMemcpyAsync(h_counts, counts.p, 12, cudaMemcpyDeviceToHost, s));
-    GB_CUDA(cudaStreamSynchronize(s));
-    near_count = h_counts[0];
-    far_count = h_counts[2];
-    std::swap(far, far_out);
-  }
-  GB_CUDA(cudaGetLastError());
+  GB_TRY(sssp_loop(s, n, g->out.off.p, g->out.tgt.p, g->out.w.p, dist, (uint32_t)cfg->start_node, cfg->delta, wk,
+                   nullptr, &g->timing.kernel_launches));
   GB_CUDA(cudaEventRecord(g->ev_end, s));
   if (h_dist) GB_CUDA(cudaMemcpyAsync(h_dist, d_dist, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
   GB_CUDA(cudaStreamSynchronize(s));
   float ms = 0.0f;
   GB_CUDA(cudaEventElapsedTime(&ms, g->ev_begin, g->ev_end));
   g->timing.total_ms = ms;
+  return GB_OK;
+}
+
+// ---- one-shot SSSP of a host out-CSR (gb_sssp_csr_u32) ----------------------------------------------------------
+// The checks and messages are those of gb_digraph_from_csr_u32 + gb_sssp for the same out-CSR, in the order of
+// the header: the O(1) host checks, the values, the config, then the device checks of the offsets and targets.
+static gb_status sssp_csr(int device, uint32_t n, const uint32_t* off, const uint32_t* tgt, const float* w,
+                          const gb_sssp_config* cfg, float* distances) {
+  sssp_csr_last = gb_sssp_csr_stats{};
+  GB_REQUIRE(distances != nullptr, "distances is NULL");
+  GB_REQUIRE(cfg != nullptr, "config is NULL");
+  GB_REQUIRE(n > 0, "node_count must be > 0");
+  GB_TRY(require_device(device));
+  GB_TRY(require_host_csr(n, off, tgt, "out"));
+  const uint64_t m = off[n];
+  if (m > 0 && !w)
+    return fail(GB_ERR_UNSUPPORTED, "sssp needs f32 edge values (DirectedNeighborsWithValues<NI, f32>, sssp.rs:41)");
+  GB_REQUIRE(cfg->start_node < n, "start_node %llu out of range (n = %u)", (unsigned long long)cfg->start_node, n);
+  GB_REQUIRE(cfg->delta > 0.0f && cfg->delta < FLT_MAX, "delta must be a positive finite f32");
+  DeviceGuard guard(device);
+  GB_CUDA(cudaSetDevice(device));
+  const uint32_t start = (uint32_t)cfg->start_node;
+  uint64_t C = env_u64("GB_SSSP_FEED_ENTRIES", 0);
+  if (C == 0) C = std::max<uint64_t>((m + SSSP_FEED_CHUNKS - 1) / SSSP_FEED_CHUNKS, SSSP_FEED_MIN_ENTRIES);
+  C = std::max<uint64_t>(C, (m + SSSP_FEED_MAX_CHUNKS - 1) / SSSP_FEED_MAX_CHUNKS);
+  SsspCsrCall t;
+  t.ch = tc_split(off, n, C);
+  t.order = sssp_send_order(t.ch, start);
+  t.K = t.ch.count();
+  t.n = n;
+  t.tgt = tgt;
+  t.w = w;
+  t.step = env_u64("GB_SSSP_FEED_STEP", 0);
+  // page-locked arrays go out all at once (unless the step rule holds them back); from pageable memory a copy
+  // returns once it is done, so one chunk goes out while each pass runs
+  t.pinned = m && CsrFeed::pinned(tgt) && CsrFeed::pinned(w);
+  gb_sssp_csr_stats& info = t.info;
+  info.chunks = t.K;
+  info.chunk_entries = C;
+  info.pinned = t.pinned ? 1 : 0;
+  info.start_chunk = t.order[0];
+  info.h2d_bytes = 4 * ((uint64_t)n + 1) + 8 * m;
+  GB_TRY(t.create());
+  GB_TRY(t.feed.open(device, 0, n, false));
+  GB_TRY(t.feed.resident(0, m, t.K, false, true));
+  GB_TRY(t.bad.alloc((size_t)t.K + 1));
+  SsspWork wk;
+  DevBuf<float> dist;
+  GB_TRY(dist.alloc(n));
+  for (DevBuf<uint32_t>* b : {&wk.qa, &wk.qb, &wk.fa, &wk.fb, &wk.pa, &wk.pb}) GB_TRY(b->alloc(n));
+  for (DevBuf<uint32_t>* b : {&wk.near_stamp, &wk.in_pile, &wk.parked}) {
+    GB_TRY(b->alloc(n));
+    GB_CUDA(cudaMemsetAsync(b->p, 0, (size_t)n * 4, t.compute));
+  }
+  GB_TRY(wk.counts.alloc(6));
+  GB_TRY(wk.minb.alloc(1));
+  GB_CUDA(cudaMemsetAsync(t.bad.p, 0, ((size_t)t.K + 1) * 4, t.check));
+  GB_CUDA(cudaEventRecord(t.begin, t.feed.copy));
+  GB_TRY(t.feed.send_offsets(off));
+  GB_TRY(t.feed.check_monotone(t.check, 0, n, t.bad.p));
+  GB_CUDA(cudaMemcpyAsync(t.h_bad, t.bad.p, 4, cudaMemcpyDeviceToHost, t.check));
+  GB_CUDA(cudaEventRecord(t.offsets_checked, t.check));
+  info.kernel_launches += 1;
+  const uint32_t ahead = t.pinned && !t.step ? t.K : 1;
+  while (t.issued < ahead) GB_TRY(t.issue());
+  // the offsets are monotone before anything indexes with them
+  GB_CUDA(cudaEventSynchronize(t.offsets_checked));
+  GB_TRY(require_monotone("out", t.h_bad[0]));
+  GB_CUDA(cudaStreamWaitEvent(t.compute, t.offsets_checked, 0));
+  bool raised = false;
+  GB_TRY(t.poll(true, &raised));  // the start's chunk
+  uint64_t launches = 0;
+  GB_TRY(sssp_loop(t.compute, n, t.feed.off.p, t.feed.tgt.p, t.feed.val.p, reinterpret_cast<uint32_t*>(dist.p),
+                   start, cfg->delta, wk, &t, &launches));
+  // the distances are final; a chunk the loop never read still fails the call as the twin's upload would
+  GB_TRY(t.check_all());
+  info.kernel_launches += launches;
+  GB_CUDA(cudaStreamWaitEvent(t.compute, t.uploaded, 0));  // so that `end` follows the whole upload
+  GB_CUDA(cudaEventRecord(t.end, t.compute));
+  GB_CUDA(cudaMemcpyAsync(distances, dist.p, (size_t)n * 4, cudaMemcpyDeviceToHost, t.compute));
+  GB_CUDA(cudaStreamSynchronize(t.compute));
+  float up = 0.0f, all = 0.0f;
+  GB_CUDA(cudaEventElapsedTime(&up, t.begin, t.uploaded));
+  GB_CUDA(cudaEventElapsedTime(&all, t.begin, t.end));
+  info.upload_ms = up;
+  info.total_ms = all;
+  sssp_csr_last = info;
   return GB_OK;
 }
 
@@ -267,5 +597,14 @@ gb_status gb_sssp(const gb_graph* graph, const gb_sssp_config* config, float* di
 gb_status gb_sssp_device(const gb_graph* graph, const gb_sssp_config* config, float* d_distances) {
   GB_REQUIRE(d_distances != nullptr, "d_distances is NULL");
   return gb::sssp_impl(graph, config, d_distances, nullptr);
+}
+gb_status gb_sssp_csr_u32(int device, uint32_t node_count, const uint32_t* offsets, const uint32_t* targets,
+                          const float* weights, const gb_sssp_config* config, float* distances) {
+  return gb::sssp_csr(device, node_count, offsets, targets, weights, config, distances);
+}
+gb_status gb_sssp_csr_info(gb_sssp_csr_stats* info) {
+  GB_REQUIRE(info != nullptr, "info is NULL");
+  *info = gb::sssp_csr_last;
+  return GB_OK;
 }
 }

@@ -341,6 +341,44 @@ gb_status gb_wcc_sample_label(const gb_graph* graph, const gb_wcc_config* config
 gb_status gb_sssp(const gb_graph* graph, const gb_sssp_config* config, float* distances);
 gb_status gb_sssp_device(const gb_graph* graph, const gb_sssp_config* config, float* d_distances);
 
+/* delta_stepping (sssp.rs:38-102) of a HOST weighted out-CSR, with no twin kept and no in-CSR needed: the
+ * distances gb_digraph_from_csr_u32 (with any in-CSR that is the transpose) + gb_sssp give for the same arrays,
+ * bit for bit, for every start, delta, chunk size and landing order; unreached vertices get FLT_MAX.  Layout:
+ * offsets has node_count + 1 entries from 0; targets and weights (f32, not checked, as on the twin) hold
+ * offsets[node_count] entries each, and may be NULL when that is 0.  Checks, in order: distances and config
+ * NULL, node_count, the device, offsets NULL, offsets[0], targets NULL; weights NULL while there are edges
+ * (GB_ERR_UNSUPPORTED, gb_sssp's message); start_node and delta (gb_sssp's messages); then on the device the
+ * offsets monotone and every target < node_count (gb_digraph_from_csr_u32's messages).  distances is not
+ * written when the call fails.
+ * The offsets go first; the targets and weights follow in row-aligned chunks (as gb_triangle_count_csr_u32 cuts
+ * them), from the chunk that holds start_node on, wrapping round to chunk 0.  A chunk may be read once its
+ * targets are checked, and the bucket loop runs meanwhile: a queued vertex whose row has not landed is parked
+ * and relaxed once it has.  Residency: the whole out-CSR (4(n+1) + 8m bytes) and about 11n words of work
+ * arrays are on the device by the end of the call; everything is freed before it returns.  Page-locked
+ * targets and weights go out all at once on a copy stream; from pageable memory the copies are synchronous, one
+ * chunk per relax pass, and the result is the same.  GB_SSSP_FEED_ENTRIES (environment, read per call) sets the
+ * entries per chunk (default ceil(m / 16), at least 2^20; never fewer than m / 4096).  GB_SSSP_FEED_STEP=p
+ * (environment, for tests) sends the j-th chunk of the order only after j * p relax passes and waits for it. */
+gb_status gb_sssp_csr_u32(int device, uint32_t node_count, const uint32_t* offsets, const uint32_t* targets,
+                          const float* weights, const gb_sssp_config* config, float* distances);
+/* Statistics of the calling thread's last gb_sssp_csr_u32 (all zero after a failed call).  The struct is
+ * not called gb_sssp_csr_info: C gives a typedef and a function one name space. */
+typedef struct gb_sssp_csr_stats {
+  uint64_t chunks;                    /* row-aligned chunks the targets and weights were uploaded in */
+  uint64_t chunk_entries;             /* the entry budget of a chunk */
+  uint64_t h2d_bytes;                 /* bytes copied host -> device: 4(n+1) + 8m */
+  uint64_t parked;                    /* distinct vertices deferred because their row had not landed */
+  uint64_t unpark_rounds;             /* launches that moved parked vertices back to the near queue */
+  uint64_t passes;                    /* relax passes */
+  uint64_t passes_before_last_landed; /* relax passes launched before every chunk was available */
+  uint64_t kernel_launches;           /* checks, relax passes, bucket advances and unparks */
+  uint32_t pinned;                    /* 1: the targets and weights were page-locked */
+  uint32_t start_chunk;               /* the chunk that holds start_node, sent first */
+  double upload_ms;                   /* CUDA-event time from the first copy to the last chunk landing */
+  double total_ms;                    /* CUDA-event time from the first copy to the final distances */
+} gb_sssp_csr_stats;
+gb_status gb_sssp_csr_info(gb_sssp_csr_stats* info);
+
 /* global_triangle_count(&graph) -> u64                      triangle_count.rs:22-86
  * Any row order, as the reference counts it.  The first call on a graph whose rows are not known to be
  * sorted (an Unsorted build, gb_graph_from_csr_u32) checks them once and caches the answer. */

@@ -319,6 +319,18 @@ inline std::vector<float> delta_stepping(const DirectedCsrGraph& g, DeltaSteppin
   detail::check(gb_sssp(g.handle(), &cfg, dist.data()));
   return dist;
 }
+// delta_stepping of a host weighted out-CSR (offsets[node_count + 1], targets and f32 weights[offsets[node_count]]),
+// streamed to the device in row-aligned chunks from the start's chunk on and relaxed as they land, without a
+// resident twin or an in-CSR (gb_sssp_csr_u32); the distances delta_stepping gives on DirectedCsrGraph::from_csr
+// of the same arrays
+inline std::vector<float> delta_stepping_csr(std::uint32_t node_count, const std::uint32_t* offsets,
+                                             const std::uint32_t* targets, const float* weights,
+                                             DeltaSteppingConfig c, int device = 0) {
+  gb_sssp_config cfg{c.start_node, c.delta};
+  std::vector<float> dist(node_count);
+  detail::check(gb_sssp_csr_u32(device, node_count, offsets, targets, weights, &cfg, dist.data()));
+  return dist;
+}
 
 // global_triangle_count(&graph) -> u64                         triangle_count.rs:22
 inline std::uint64_t global_triangle_count(const UndirectedCsrGraph& g) {
