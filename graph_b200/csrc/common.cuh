@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <new>
@@ -14,6 +15,7 @@
 #include <vector>
 
 #include "../../include/graph_b200.h"
+#include "csr_split.h"
 
 namespace gb {
 
@@ -154,7 +156,8 @@ struct PeerBuf {
 // which returns only once its stream has drained, blocks the host only until work already enqueued has run.
 // A resident feed may carry one f32 value per target (val, asked for with `values`): chunk k's values are
 // copied right after its targets, with the same bounds, before landed[k].
-// The consumers' streams are the caller's, and must drain before the feed goes.
+// The consumers' streams are the caller's, and must drain before the feed goes.  The id checks are the
+// caller's too: WCC and PageRank make their own, and CheckedFeed (below) makes them for a resident feed.
 struct CsrFeed {
   int dev = -1;
   uint32_t r_begin = 0, r_end = 0;
@@ -181,6 +184,65 @@ struct CsrFeed {
   // whether host memory is page-locked: such a copy does not wait for its stream to drain
   static bool pinned(const void* host);
   ~CsrFeed();
+};
+
+// ---- a checked, resident upload of a whole host CSR to one device (graph.cu) ---------------------------------
+// The triangle count and SSSP of a host CSR (gb_triangle_count_csr_u32, gb_sssp_csr_u32) read chunks of it while
+// the rest is on the bus.  open() cuts the targets (and values) into tc_split chunks of tc_chunk_entries(m, knob)
+// entries, sends the offsets [0, n] into a resident CsrFeed and queues their monotone check on the check stream.
+// issue() sends the next chunk of the send order (sssp_send_order from row `first`; first = 0 sends the chunks in
+// row order), and on the check stream behind its landed event counts its targets >= n into h_bad[1 + k], runs
+// per_chunk(k) when the caller set one, and records checked[j] (j: the chunk's place in the send order) behind
+// it all.  A consumer reads chunk order[j] only once checked[j] has passed and h_bad[1 + order[j]] is 0.
+// Page-locked targets (and values) go out all at once; a pageable copy returns only once it is done, so from
+// pageable memory the caller issues each chunk when it is ready for it.
+// The destructor drains the check stream before the events, the page-locked tally and the feed go.  The
+// consumer streams are the caller's, and must drain before it goes: a call keeps it as its first member.
+struct CheckedFeed {
+  CsrFeed feed;
+  CsrChunks ch;
+  std::vector<uint32_t> order;  // the send order: order[j] is the j-th chunk sent
+  std::function<gb_status(uint32_t k)> per_chunk;  // more of chunk k's checks, enqueued on `check`
+  cudaStream_t check = nullptr;
+  DevBuf<unsigned int> bad;       // [0] rows whose offsets decrease, [1 + k] targets >= n in chunk k
+  unsigned int* h_bad = nullptr;  // page-locked: bad[1 + K]
+  cudaEvent_t begin = nullptr, uploaded = nullptr, end = nullptr;  // timed; `end` is recorded by finish()
+  cudaEvent_t offsets_checked = nullptr;
+  std::vector<cudaEvent_t> checked;  // [j]: behind the checks of the j-th chunk sent
+  const uint32_t* tgt = nullptr;
+  const float* val = nullptr;
+  const char* what = "";  // begins the failure messages ("undirected", "out")
+  uint32_t n = 0, K = 0, issued = 0;
+  uint64_t chunk_entries = 0, launches = 0;  // launches: the check kernels enqueued
+  bool pinned = false;
+
+  // a host CSR of `nodes` rows (require_host_csr has passed) and its values (NULL: none)
+  gb_status open(int device, uint32_t nodes, const uint32_t* off, const uint32_t* host_tgt, const float* host_val,
+                 uint64_t knob, uint32_t first, const char* name);
+  gb_status issue();
+  // waits for the monotone check of the offsets: GB_OK, or require_monotone's failure
+  gb_status require_offsets();
+  // issues every chunk left and waits for their checks: GB_OK, or require_ids's failure on the summed tally
+  gb_status check_all();
+  // on the consumer stream s: waits for the last chunk to land (so that `end` follows the whole upload), records
+  // end, copies `bytes` of the result from dev to host and synchronises s
+  gb_status finish(cudaStream_t s, void* host, const void* dev, size_t bytes);
+  // the fields gb_tc_csr_info and gb_sssp_csr_stats share, once finish() has returned
+  template <typename Info>
+  gb_status report(Info* info) const {
+    info->chunks = K;
+    info->chunk_entries = chunk_entries;
+    info->pinned = pinned ? 1 : 0;
+    info->h2d_bytes = 4 * ((uint64_t)n + 1) + (val ? 8 : 4) * ch.edge[K];  // edge[K] == m
+    info->kernel_launches += launches;
+    float up = 0.0f, all = 0.0f;
+    GB_CUDA(cudaEventElapsedTime(&up, begin, uploaded));
+    GB_CUDA(cudaEventElapsedTime(&all, begin, end));
+    info->upload_ms = up;
+    info->total_ms = all;
+    return GB_OK;
+  }
+  ~CheckedFeed();
 };
 
 // The O(1) host checks of a host CSR, in this order: offsets NULL, offsets[0] == 0, then targets NULL when it

@@ -121,7 +121,7 @@ inline std::vector<PrPart> pr_split(const uint32_t* in_off, uint32_t n, uint32_t
   return out;
 }
 
-// ---- triangle count (gb_triangle_count_csr_u32): greedy chunks ------------------------------------------------
+// ---- triangle count (gb_triangle_count_csr_u32) and SSSP (gb_sssp_csr_u32): greedy chunks ----------------------
 // Chunk k holds the rows [row[k], row[k + 1]) and the entries [edge[k], edge[k + 1]) = [off[row[k]],
 // off[row[k + 1]]), row[0] = 0, row[K] = n: cuts fall at rows.  Each chunk takes as many whole rows as fit in C
 // entries, empty rows included, so every chunk holds at most C entries unless its one non-empty row is longer
@@ -156,6 +156,14 @@ inline CsrChunks tc_split(const uint32_t* off, uint32_t n, uint64_t chunk_entrie
     e = eb;
   }
   return c;
+}
+
+// C, the entries per chunk of tc_split for the triangle count and SSSP (CheckedFeed, common.cuh): `knob`
+// (GB_TC_FEED_ENTRIES, GB_SSSP_FEED_ENTRIES; 0 when unset) when set, else ceil(m / 16) but at least 2^20; never
+// below ceil(m / 4096), so that a call makes at most 2 * 4096 + 1 chunks
+inline uint64_t tc_chunk_entries(uint64_t m, uint64_t knob) {
+  const uint64_t c = knob ? knob : std::max<uint64_t>((m + 15) / 16, 1u << 20);
+  return std::max<uint64_t>(c, (m + 4095) / 4096);
 }
 
 // ---- SSSP (gb_sssp_csr_u32): the chunks of tc_split, sent from the start's chunk on ------------------------------

@@ -443,6 +443,89 @@ CsrFeed::~CsrFeed() {
   if (copy) cudaStreamDestroy(copy);
 }
 
+gb_status CheckedFeed::open(int device, uint32_t nodes, const uint32_t* off, const uint32_t* host_tgt,
+                            const float* host_val, uint64_t knob, uint32_t first, const char* name) {
+  const uint64_t m = off[nodes];
+  n = nodes;
+  tgt = host_tgt;
+  val = host_val;
+  what = name;
+  chunk_entries = tc_chunk_entries(m, knob);
+  ch = tc_split(off, n, chunk_entries);
+  order = sssp_send_order(ch, first);
+  K = ch.count();
+  pinned = m && CsrFeed::pinned(tgt) && (!val || CsrFeed::pinned(val));
+  GB_TRY(feed.open(device, 0, n, false));
+  GB_TRY(feed.resident(0, m, K, false, val != nullptr));
+  GB_CUDA(cudaStreamCreateWithFlags(&check, cudaStreamNonBlocking));
+  for (cudaEvent_t* e : {&begin, &uploaded, &end}) GB_CUDA(cudaEventCreate(e));
+  GB_CUDA(cudaEventCreateWithFlags(&offsets_checked, cudaEventDisableTiming));
+  checked.assign(K, nullptr);
+  for (cudaEvent_t& e : checked) GB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  GB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h_bad), ((size_t)K + 1) * 4, cudaHostAllocDefault));
+  GB_TRY(bad.alloc((size_t)K + 1));
+  GB_CUDA(cudaMemsetAsync(bad.p, 0, ((size_t)K + 1) * 4, check));
+  GB_CUDA(cudaEventRecord(begin, feed.copy));
+  GB_TRY(feed.send_offsets(off));
+  GB_TRY(feed.check_monotone(check, 0, n, bad.p));
+  GB_CUDA(cudaMemcpyAsync(h_bad, bad.p, 4, cudaMemcpyDeviceToHost, check));
+  GB_CUDA(cudaEventRecord(offsets_checked, check));
+  launches += 1;
+  return GB_OK;
+}
+
+// The check kernels read the rows and entries of the chunk only, and the bounds stay inside the arrays whatever
+// the offsets hold
+gb_status CheckedFeed::issue() {
+  const uint32_t j = issued++, k = order[j];
+  const uint64_t e0 = ch.edge[k], e1 = ch.edge[k + 1];
+  GB_TRY(feed.send(k, tgt, e0, e1 - e0, val));
+  if (issued == K) GB_CUDA(cudaEventRecord(uploaded, feed.copy));
+  GB_CUDA(cudaStreamWaitEvent(check, feed.landed[k], 0));
+  if (e1 > e0) {
+    check_ids_async(check, feed.tgt.p + e0, e1 - e0, n, bad.p + 1 + k);
+    launches += 1;
+  }
+  if (per_chunk) GB_TRY(per_chunk(k));
+  GB_CUDA(cudaGetLastError());
+  GB_CUDA(cudaMemcpyAsync(h_bad + 1 + k, bad.p + 1 + k, 4, cudaMemcpyDeviceToHost, check));
+  GB_CUDA(cudaEventRecord(checked[j], check));
+  return GB_OK;
+}
+
+gb_status CheckedFeed::require_offsets() {
+  GB_CUDA(cudaEventSynchronize(offsets_checked));
+  return require_monotone(what, h_bad[0]);
+}
+
+// the verdict gb_graph_from_csr_u32 / gb_digraph_from_csr_u32 give on the targets: a failed chunk's count
+// alone would not match it
+gb_status CheckedFeed::check_all() {
+  while (issued < K) GB_TRY(issue());
+  GB_CUDA(cudaStreamSynchronize(check));
+  uint64_t nbad = 0;
+  for (uint32_t k = 0; k < K; ++k) nbad += h_bad[1 + k];
+  return require_ids(what, nbad, n);
+}
+
+gb_status CheckedFeed::finish(cudaStream_t s, void* host, const void* dev, size_t bytes) {
+  GB_CUDA(cudaStreamWaitEvent(s, uploaded, 0));
+  GB_CUDA(cudaEventRecord(end, s));
+  GB_CUDA(cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, s));
+  GB_CUDA(cudaStreamSynchronize(s));
+  return GB_OK;
+}
+
+CheckedFeed::~CheckedFeed() {
+  if (check) cudaStreamSynchronize(check);
+  for (cudaEvent_t e : checked)
+    if (e) cudaEventDestroy(e);
+  for (cudaEvent_t e : {begin, uploaded, end, offsets_checked})
+    if (e) cudaEventDestroy(e);
+  if (check) cudaStreamDestroy(check);
+  if (h_bad) cudaFreeHost(h_bad);
+}
+
 // Only O(1) checks read the host arrays; the O(n + m) ones run on the device after the upload, so that a
 // billion-edge twin is not validated by one CPU thread.
 gb_status upload_host_csr(cudaStream_t s, uint32_t n, const uint32_t* off, const uint32_t* tgt, const float* w,

@@ -10,10 +10,10 @@
 //
 // Algorithmic bytes per run: 8m + 4(n+1) + 8n (weighted out-CSR once, distances read + write).
 //
-// One-shot SSSP of a host out-CSR (gb_sssp_csr_u32).  The offsets go first and are checked; the targets and
-// their f32 values follow in the row-aligned chunks of tc_split (csr_split.h), sent from the chunk that holds the
-// start on and wrapping round (sssp_send_order), into one resident CSR.  A chunk is available once its id check
-// has passed, and the available rows are then one cyclic interval from the start's chunk (SsspRows).  The bucket
+// One-shot SSSP of a host out-CSR (gb_sssp_csr_u32).  A CheckedFeed (common.cuh) sends the offsets first and
+// checks them; the targets and their f32 values follow in its chunks, sent from the chunk that holds the start on
+// and wrapping round (sssp_send_order), into one resident CSR.  A chunk is available once its id check has
+// passed, and the available rows are then one cyclic interval from the start's chunk (SsspRows).  The bucket
 // loop is the twin's, with one change in k_sssp_relax<true>: a queue entry whose row is not available yet is
 // not relaxed but PARKED, once per vertex, in a parked list; between passes the host raises the available bound
 // and k_sssp_unpark moves the parked vertices whose rows are now present into the near queue.  When only parked
@@ -25,10 +25,8 @@
 // present, and the loop still ends at the unique fixed point above (SURVEY.md A.4), bit-equal to the twin.
 #include <algorithm>
 #include <cfloat>
-#include <vector>
 
 #include "common.cuh"
-#include "csr_split.h"
 #include "sssp_bucket.h"
 
 namespace gb {
@@ -212,118 +210,58 @@ __global__ void k_sssp_min_far(const uint32_t* __restrict__ dist, const uint32_t
 }
 
 // ---- the one-shot call's chunks (gb_sssp_csr_u32) ---------------------------------------------------------------
-// C, the entries per chunk: GB_SSSP_FEED_ENTRIES when set, else ceil(m / 16) but at least 2^20; never below
-// ceil(m / 4096) (the triangle count's rule)
-constexpr uint64_t SSSP_FEED_CHUNKS = 16;
-constexpr uint64_t SSSP_FEED_MIN_ENTRIES = 1u << 20;
-constexpr uint64_t SSSP_FEED_MAX_CHUNKS = 4096;
-
 thread_local gb_sssp_csr_stats sssp_csr_last{};  // behind gb_sssp_csr_info
 
-// Everything one call holds besides its work buffers.  Chunks go out in send order; `avail` of them (a prefix of
-// that order) have passed their checks and may be read by the compute stream, which waits on the last one's
-// `checked` event.  The destructor drains the streams before anything they use goes: the page-locked tally, the
-// events, the buffers and the feed (the first member).
+// Everything one call holds besides its work buffers.  Chunks go out in the feed's send order; `avail` of them (a
+// prefix of that order) have passed their checks and may be read by the compute stream, which waits on the last
+// one's `checked` event.  The destructor drains the compute stream before the feed (the first member) goes.
 struct SsspCsrCall {
-  CsrFeed feed;  // the offsets [0, n], the resident targets and values, one landed event per chunk
-  DevBuf<unsigned int> bad;      // [0] rows whose offsets decrease, [1 + k] targets >= n in chunk k
-  unsigned int* h_bad = nullptr;  // page-locked: bad[1 + K]
-  cudaStream_t check = nullptr, compute = nullptr;
-  cudaEvent_t begin = nullptr, uploaded = nullptr, end = nullptr;  // timed
-  cudaEvent_t offsets_checked = nullptr;
-  std::vector<cudaEvent_t> checked;  // [j]: behind the checks of the j-th chunk of the send order
-  CsrChunks ch;
-  std::vector<uint32_t> order;
-  const uint32_t* tgt = nullptr;
-  const float* w = nullptr;
-  uint32_t n = 0, K = 0, issued = 0, avail = 0;
+  CheckedFeed feed;  // the offsets [0, n], the resident targets and values, sent from the start's chunk on
+  cudaStream_t compute = nullptr;
+  uint32_t avail = 0;
   uint64_t step = 0;  // GB_SSSP_FEED_STEP: the j-th chunk goes out after j * step passes, and is waited for
-  bool pinned = false;
   gb_sssp_csr_stats info{};
 
-  gb_status create() {
-    GB_CUDA(cudaStreamCreateWithFlags(&check, cudaStreamNonBlocking));
-    GB_CUDA(cudaStreamCreateWithFlags(&compute, cudaStreamNonBlocking));
-    for (cudaEvent_t* e : {&begin, &uploaded, &end}) GB_CUDA(cudaEventCreate(e));
-    GB_CUDA(cudaEventCreateWithFlags(&offsets_checked, cudaEventDisableTiming));
-    checked.assign(K, nullptr);
-    for (uint32_t j = 0; j < K; ++j) GB_CUDA(cudaEventCreateWithFlags(&checked[j], cudaEventDisableTiming));
-    GB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h_bad), ((size_t)K + 1) * 4, cudaHostAllocDefault));
-    return GB_OK;
-  }
   ~SsspCsrCall() {
-    for (cudaStream_t s : {check, compute})
-      if (s) cudaStreamSynchronize(s);
-    for (cudaEvent_t e : checked)
-      if (e) cudaEventDestroy(e);
-    for (cudaEvent_t e : {begin, uploaded, end, offsets_checked})
-      if (e) cudaEventDestroy(e);
-    for (cudaStream_t s : {check, compute})
-      if (s) cudaStreamDestroy(s);
-    if (h_bad) cudaFreeHost(h_bad);
-  }
-
-  // the next chunk of the send order: its copy, then its id check behind its landing
-  gb_status issue() {
-    const uint32_t j = issued++, k = order[j];
-    const uint64_t e0 = ch.edge[k], e1 = ch.edge[k + 1];
-    GB_TRY(feed.send(k, tgt, e0, e1 - e0, w));
-    if (issued == K) GB_CUDA(cudaEventRecord(uploaded, feed.copy));
-    GB_CUDA(cudaStreamWaitEvent(check, feed.landed[k], 0));
-    if (e1 > e0) {
-      check_ids_async(check, feed.tgt.p + e0, e1 - e0, n, bad.p + 1 + k);
-      info.kernel_launches += 1;
-    }
-    GB_CUDA(cudaGetLastError());
-    GB_CUDA(cudaMemcpyAsync(h_bad + 1 + k, bad.p + 1 + k, 4, cudaMemcpyDeviceToHost, check));
-    GB_CUDA(cudaEventRecord(checked[j], check));
-    return GB_OK;
+    if (compute) cudaStreamSynchronize(compute), cudaStreamDestroy(compute);
   }
   // once a relax pass is launched: from pageable memory the copies are synchronous, one chunk per pass
   gb_status after_launch() {
     info.passes += 1;
-    if (avail < K) info.passes_before_last_landed += 1;
-    if (!pinned && !step && issued < K) GB_TRY(issue());
+    if (avail < feed.K) info.passes_before_last_landed += 1;
+    if (!feed.pinned && !step && feed.issued < feed.K) GB_TRY(feed.issue());
     return GB_OK;
-  }
-  // every chunk checked: the verdict of gb_digraph_from_csr_u32 on the targets
-  gb_status check_all() {
-    while (issued < K) GB_TRY(issue());
-    GB_CUDA(cudaStreamSynchronize(check));
-    uint64_t nbad = 0;
-    for (uint32_t k = 0; k < K; ++k) nbad += h_bad[1 + k];
-    return require_ids("out", nbad, n);
   }
   // Raises avail over the chunks whose checks have passed, without waiting, unless the step rule sends and
   // waits for chunks or `block` asks for one more chunk at least.  A chunk that failed stops the call.
   gb_status poll(bool block, bool* raised) {
-    const uint32_t was = avail;
+    const uint32_t was = avail, K = feed.K;
     if (step)
-      while (issued < K && issued * step <= info.passes) GB_TRY(issue());
-    if (block && avail == issued) {
-      if (issued == K) return fail(GB_ERR_CUDA, "sssp: parked vertices with every chunk available");
-      GB_TRY(issue());
+      while (feed.issued < K && feed.issued * step <= info.passes) GB_TRY(feed.issue());
+    if (block && avail == feed.issued) {
+      if (feed.issued == K) return fail(GB_ERR_CUDA, "sssp: parked vertices with every chunk available");
+      GB_TRY(feed.issue());
     }
-    while (avail < issued) {
+    while (avail < feed.issued) {
       if (step || (block && avail == was)) {
-        GB_CUDA(cudaEventSynchronize(checked[avail]));
+        GB_CUDA(cudaEventSynchronize(feed.checked[avail]));
       } else {
-        const cudaError_t e = cudaEventQuery(checked[avail]);
+        const cudaError_t e = cudaEventQuery(feed.checked[avail]);
         if (e == cudaErrorNotReady) break;
         GB_CUDA(e);
       }
-      if (h_bad[1 + order[avail]]) return check_all();
+      if (feed.h_bad[1 + feed.order[avail]]) return feed.check_all();
       ++avail;
     }
     *raised = avail > was;
-    if (*raised) GB_CUDA(cudaStreamWaitEvent(compute, checked[avail - 1], 0));
+    if (*raised) GB_CUDA(cudaStreamWaitEvent(compute, feed.checked[avail - 1], 0));
     return GB_OK;
   }
   SsspRows rows(uint32_t* parked) const {
-    const uint32_t first = ch.row[order[0]];
+    const uint32_t n = feed.n, first = feed.ch.row[feed.order[0]];
     uint32_t span = avail ? n : 0u;
-    if (avail && avail < K) {
-      const uint32_t stop = ch.row[order[avail]];  // the first row not yet available
+    if (avail && avail < feed.K) {
+      const uint32_t stop = feed.ch.row[feed.order[avail]];  // the first row not yet available
       span = stop > first ? stop - first : stop + (n - first);
     }
     return SsspRows{first, span, n, parked};
@@ -519,30 +457,10 @@ static gb_status sssp_csr(int device, uint32_t n, const uint32_t* off, const uin
   DeviceGuard guard(device);
   GB_CUDA(cudaSetDevice(device));
   const uint32_t start = (uint32_t)cfg->start_node;
-  uint64_t C = env_u64("GB_SSSP_FEED_ENTRIES", 0);
-  if (C == 0) C = std::max<uint64_t>((m + SSSP_FEED_CHUNKS - 1) / SSSP_FEED_CHUNKS, SSSP_FEED_MIN_ENTRIES);
-  C = std::max<uint64_t>(C, (m + SSSP_FEED_MAX_CHUNKS - 1) / SSSP_FEED_MAX_CHUNKS);
   SsspCsrCall t;
-  t.ch = tc_split(off, n, C);
-  t.order = sssp_send_order(t.ch, start);
-  t.K = t.ch.count();
-  t.n = n;
-  t.tgt = tgt;
-  t.w = w;
+  CheckedFeed& f = t.feed;
   t.step = env_u64("GB_SSSP_FEED_STEP", 0);
-  // page-locked arrays go out all at once (unless the step rule holds them back); from pageable memory a copy
-  // returns once it is done, so one chunk goes out while each pass runs
-  t.pinned = m && CsrFeed::pinned(tgt) && CsrFeed::pinned(w);
-  gb_sssp_csr_stats& info = t.info;
-  info.chunks = t.K;
-  info.chunk_entries = C;
-  info.pinned = t.pinned ? 1 : 0;
-  info.start_chunk = t.order[0];
-  info.h2d_bytes = 4 * ((uint64_t)n + 1) + 8 * m;
-  GB_TRY(t.create());
-  GB_TRY(t.feed.open(device, 0, n, false));
-  GB_TRY(t.feed.resident(0, m, t.K, false, true));
-  GB_TRY(t.bad.alloc((size_t)t.K + 1));
+  GB_CUDA(cudaStreamCreateWithFlags(&t.compute, cudaStreamNonBlocking));
   SsspWork wk;
   DevBuf<float> dist;
   GB_TRY(dist.alloc(n));
@@ -553,36 +471,26 @@ static gb_status sssp_csr(int device, uint32_t n, const uint32_t* off, const uin
   }
   GB_TRY(wk.counts.alloc(6));
   GB_TRY(wk.minb.alloc(1));
-  GB_CUDA(cudaMemsetAsync(t.bad.p, 0, ((size_t)t.K + 1) * 4, t.check));
-  GB_CUDA(cudaEventRecord(t.begin, t.feed.copy));
-  GB_TRY(t.feed.send_offsets(off));
-  GB_TRY(t.feed.check_monotone(t.check, 0, n, t.bad.p));
-  GB_CUDA(cudaMemcpyAsync(t.h_bad, t.bad.p, 4, cudaMemcpyDeviceToHost, t.check));
-  GB_CUDA(cudaEventRecord(t.offsets_checked, t.check));
-  info.kernel_launches += 1;
-  const uint32_t ahead = t.pinned && !t.step ? t.K : 1;
-  while (t.issued < ahead) GB_TRY(t.issue());
+  GB_TRY(f.open(device, n, off, tgt, w, env_u64("GB_SSSP_FEED_ENTRIES", 0), start, "out"));
+  gb_sssp_csr_stats& info = t.info;
+  info.start_chunk = f.order[0];
+  // from pageable memory one chunk goes out while each pass runs (after_launch); the step rule holds page-locked
+  // chunks back as well
+  const uint32_t ahead = f.pinned && !t.step ? f.K : 1;
+  while (f.issued < ahead) GB_TRY(f.issue());
   // the offsets are monotone before anything indexes with them
-  GB_CUDA(cudaEventSynchronize(t.offsets_checked));
-  GB_TRY(require_monotone("out", t.h_bad[0]));
-  GB_CUDA(cudaStreamWaitEvent(t.compute, t.offsets_checked, 0));
+  GB_TRY(f.require_offsets());
+  GB_CUDA(cudaStreamWaitEvent(t.compute, f.offsets_checked, 0));
   bool raised = false;
   GB_TRY(t.poll(true, &raised));  // the start's chunk
   uint64_t launches = 0;
-  GB_TRY(sssp_loop(t.compute, n, t.feed.off.p, t.feed.tgt.p, t.feed.val.p, reinterpret_cast<uint32_t*>(dist.p),
+  GB_TRY(sssp_loop(t.compute, n, f.feed.off.p, f.feed.tgt.p, f.feed.val.p, reinterpret_cast<uint32_t*>(dist.p),
                    start, cfg->delta, wk, &t, &launches));
   // the distances are final; a chunk the loop never read still fails the call as the twin's upload would
-  GB_TRY(t.check_all());
+  GB_TRY(f.check_all());
   info.kernel_launches += launches;
-  GB_CUDA(cudaStreamWaitEvent(t.compute, t.uploaded, 0));  // so that `end` follows the whole upload
-  GB_CUDA(cudaEventRecord(t.end, t.compute));
-  GB_CUDA(cudaMemcpyAsync(distances, dist.p, (size_t)n * 4, cudaMemcpyDeviceToHost, t.compute));
-  GB_CUDA(cudaStreamSynchronize(t.compute));
-  float up = 0.0f, all = 0.0f;
-  GB_CUDA(cudaEventElapsedTime(&up, t.begin, t.uploaded));
-  GB_CUDA(cudaEventElapsedTime(&all, t.begin, t.end));
-  info.upload_ms = up;
-  info.total_ms = all;
+  GB_TRY(f.finish(t.compute, distances, dist.p, (size_t)n * 4));
+  GB_TRY(f.report(&info));
   sssp_csr_last = info;
   return GB_OK;
 }

@@ -4,7 +4,8 @@
 // unless it has a single non-empty row (a hub longer than C), and every such hub stands alone; only an edgeless
 // CSR has an empty chunk; no chunk could have taken the next row (the cut is greedy), so there are at most
 // 2 ceil(m / C) + 1 chunks; and on offsets that are not monotone the cut still ends, with entry bounds
-// non-decreasing inside [0, m].
+// non-decreasing inside [0, m].  Then the chunk size the triangle count and SSSP take (tc_chunk_entries): the
+// default, a knob, a knob below ceil(m / 4096), and m = 0.
 #include <cstdint>
 #include <cstdio>
 #include <random>
@@ -130,6 +131,31 @@ int main() {
     EXPECT(c.row == (std::vector<uint32_t>{0, 3, 4, 6}), "rows %zu bounds", c.row.size());
     EXPECT(c.edge == (std::vector<uint64_t>{0, 6, 56, 58}), "entries %zu bounds", c.edge.size());
     ++checked;
+  }
+  {  // the chunk size: the knob when set, else ceil(m / 16) but at least 2^20; never below ceil(m / 4096)
+    const char* name = "tc_chunk_entries";
+    const uint64_t chunk_entries = 0;
+    const uint64_t M = 1ull << 20;
+    struct Rule { uint64_t m, knob, want; };
+    const Rule rules[] = {
+        {0, 0, M},                                     // m = 0: the floor
+        {0, 5, 5},                                     // m = 0, knob set
+        {1000, 0, M},                                  // small m: the floor
+        {16 * M, 0, M},                                // ceil(m / 16) == 2^20
+        {16 * M + 1, 0, M + 1},                        // ceil(m / 16) above the floor
+        {0xFFFFFFFFull, 0, 0x10000000ull},             // the largest m: ceil(m / 16)
+        {1000, 7, 7},                                  // the knob, below the default
+        {1000, 3 * M, 3 * M},                          // the knob, above the default
+        {4096 * 100, 50, 100},                         // the knob below ceil(m / 4096)
+        {4096 * 100 + 1, 100, 101},                    // ... by a rounding
+        {4096 * 100, 100, 100},                        // the knob at ceil(m / 4096)
+    };
+    for (const Rule& r : rules) {
+      const uint64_t got = gb::tc_chunk_entries(r.m, r.knob);
+      EXPECT(got == r.want, "m = %llu, knob = %llu: %llu, want %llu", (unsigned long long)r.m,
+             (unsigned long long)r.knob, (unsigned long long)got, (unsigned long long)r.want);
+      ++checked;
+    }
   }
   std::printf("tc_split: %ld cases, %d failures\n", checked, failures);
   if (failures) return 1;
