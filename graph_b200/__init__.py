@@ -38,7 +38,8 @@ def set_device(index: int) -> None:
 
 
 class Comm:
-    """Single-process multi-GPU communicator (gb_comm_*): one host thread, N devices, no torch / NCCL.
+    """Single-process multi-GPU communicator (gb_comm_*): the calling thread drives all N devices, no torch /
+    NCCL.  Threads may share one; its PageRank calls run one at a time.
 
         comm = Comm([0, 1])
         graphs = [DiGraph.rmat(22) under set_device(d) for d in comm.devices]   # the same graph on each

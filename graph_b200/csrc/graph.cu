@@ -12,6 +12,8 @@
 // turns Deduplicated into a flagged compaction.
 #include <cub/cub.cuh>
 
+#include <atomic>
+
 #include "common.cuh"
 #include "rmat.cuh"
 
@@ -32,8 +34,9 @@ gb_status fail(gb_status st, const char* fmt, ...) {
   return st;
 }
 
-static bool g_profiling = false;
-bool profiling_on() { return g_profiling; }
+// written by gb_set_profiling, read by every PageRank call, possibly on other threads
+static std::atomic<bool> g_profiling{false};
+bool profiling_on() { return g_profiling.load(std::memory_order_relaxed); }
 
 static inline uint32_t bits_for(uint32_t n) {
   uint32_t b = 1;
@@ -791,7 +794,7 @@ int gb_device_count(void) {
   }
   return c;
 }
-void gb_set_profiling(int on) { gb::g_profiling = on != 0; }
+void gb_set_profiling(int on) { gb::g_profiling.store(on != 0, std::memory_order_relaxed); }
 
 gb_status gb_digraph_from_csr_u32(int device, uint32_t n, const uint32_t* out_off,
                                   const uint32_t* out_tgt, const float* out_w, const uint32_t* in_off,
@@ -908,8 +911,12 @@ gb_status gb_graph_free(gb_graph* g) {
   return GB_OK;
 }
 
+// The accessors below that read what a call on the handle may change (the PageRank plan, the CSRs that
+// gb_make_degree_ordered replaces, the timing an algorithm fills in) take the handle's lock, and so wait for
+// a running call.  No caller holds g->mu when it calls them.
 gb_status gb_graph_get_info(const gb_graph* g, gb_graph_info* info) {
   GB_REQUIRE(g && info, "NULL argument");
+  std::lock_guard<std::mutex> lock(g->mu);
   info->kind = (uint32_t)g->kind;
   info->node_count = g->n;
   info->target_count = g->out.len;
@@ -933,6 +940,7 @@ gb_status gb_graph_csr_len(const gb_graph* g, gb_csr_which which, uint64_t* len)
   GB_REQUIRE(g && len, "NULL argument");
   const DevCsr* c = pick_csr(g, which);
   if (!c) return fail(GB_ERR_UNSUPPORTED, "graph kind %d has no CSR %d", (int)g->kind, (int)which);
+  std::lock_guard<std::mutex> lock(g->mu);
   *len = c->len;
   return GB_OK;
 }
@@ -961,6 +969,7 @@ void* gb_graph_stream(const gb_graph* g) { return g ? (void*)g->stream : nullptr
 
 gb_status gb_graph_last_timing(const gb_graph* g, gb_timing* t) {
   GB_REQUIRE(g && t, "NULL argument");
+  std::lock_guard<std::mutex> lock(g->mu);
   *t = g->timing;
   return GB_OK;
 }

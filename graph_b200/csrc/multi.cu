@@ -23,6 +23,9 @@
 struct gb_comm {
   std::vector<int> devs;
   std::vector<cudaStream_t> streams;
+  // held by a PageRank call from its shard fill through the copy of the scores: the buffers below, which
+  // comm_prepare frees and reallocates for another n, and sync_seq are one call's at a time
+  mutable std::mutex mu;
   uint32_t n = 0, n_pad = 0;                  // vectors are sized lazily for the first graph
   std::vector<float*> x;                      // per device: 2 * n_pad floats
   std::vector<void*> ctl;                     // per device: control block of gb_pr_shard_sync
@@ -317,11 +320,13 @@ static gb_status comm_sweeps(gb_comm* c, uint32_t n, const std::vector<gb_pr_sha
 }
 
 // One PageRank call over the communicator: fill(shards) makes the P shards (shards[i] on devs[i]), comm_sweeps
-// runs them, and the shards go before the caller's device is current again, whatever either returned.
+// runs them, and the shards go before the caller's device is current again, whatever either returned.  Calls
+// on one communicator run one after the other, on its lock.
 template <class Fill>
 static gb_status comm_page_rank(gb_comm* c, uint32_t n, const gb_page_rank_config* cfg, float* scores, uint64_t* ran,
                                 double* error, Fill fill) {
   DeviceGuard guard(c->devs[0]);  // fill and comm_sweeps move from device to device
+  std::lock_guard<std::mutex> lock(c->mu);
   ShardSet shards((uint32_t)c->devs.size());
   GB_TRY(fill(shards.v));
   return comm_sweeps(c, n, shards.v, cfg, scores, ran, error);
@@ -391,6 +396,7 @@ gb_status gb_comm_free(gb_comm* c) {
 
 gb_status gb_comm_info(const gb_comm* c, int* ndev, int* multicast) {
   GB_REQUIRE(c, "NULL argument");
+  std::lock_guard<std::mutex> lock(c->mu);  // comm_prepare sets multicast
   if (ndev) *ndev = (int)c->devs.size();
   if (multicast) *multicast = c->multicast ? 1 : 0;
   return GB_OK;

@@ -16,8 +16,17 @@
  *     `d_` (device pointer on the graph's device).
  *   - all calls return gb_status; on failure gb_last_error() holds a
  *     thread-local message.  Nothing unwinds or aborts across the ABI.
- *   - a gb_graph is immutable after creation except gb_make_degree_ordered
- *     (exclusive access, like `&mut self` in graph_ops.rs:173).
+ *   - a gb_graph is immutable after creation except gb_make_degree_ordered,
+ *     which relabels it in place (graph_ops.rs:173).
+ *   - threads: calls on distinct handles may run concurrently.  Calls on one
+ *     handle serialise on its lock, gb_make_degree_ordered included; other
+ *     calls see the graph either before or after the relabelling.  The one
+ *     exception is gb_graph_free, which needs exclusive access.  So
+ *     gb_graph_get_info, gb_graph_csr_len and gb_graph_last_timing wait for
+ *     a call running on the same handle.  A communicator serialises its
+ *     PageRank calls (gb_page_rank_multi, gb_page_rank_csr_multi_u32).  The
+ *     statistics of the one-shot calls (gb_sssp_csr_info,
+ *     gb_triangle_count_csr_info) are thread-local, like gb_last_error().
  *   - there is NO CPU fallback: if no CUDA device is usable every graph
  *     constructor fails with GB_ERR_CUDA.
  */
@@ -512,8 +521,11 @@ gb_status gb_pr_shard_free(gb_pr_shard* shard);
  * takes the SAME graph resident on every device of the communicator (graphs[i] on devices[i]; a
  * gb_digraph_for_page_rank_u32 twin is enough), builds every device's shard, runs the sweeps with the fused
  * exchange (one multimem.st per value when the driver offers multicast objects, else one peer store per
- * device) and the device-side barrier, and returns page_rank's triple (page_rank.rs:58-111).  One host
- * thread drives all devices; inside the sweep loop the host never waits unless tolerance > 0. */
+ * device) and the device-side barrier, and returns page_rank's triple (page_rank.rs:58-111).  The calling
+ * thread drives all devices; inside the sweep loop the host never waits unless tolerance > 0.  The
+ * communicator's sweep buffers serve one PageRank call at a time: concurrent gb_page_rank_multi and
+ * gb_page_rank_csr_multi_u32 calls on one communicator wait for each other (gb_comm_info too).
+ * gb_wcc_csr_multi_u32 and gb_pr_shards_csr_u32 read only its device list and do not wait. */
 typedef struct gb_comm gb_comm;
 gb_status gb_comm_init(int ndev, const int* devices, gb_comm** comm);
 gb_status gb_comm_info(const gb_comm* comm, int* ndev, int* multicast);
