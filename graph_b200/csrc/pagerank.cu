@@ -55,7 +55,8 @@ void free_pr_plan(PrPlan* p) {
         cudaEventElapsedTime(&ms, p->trace_events[5 * i + k], p->trace_events[5 * i + k + 1]);
         acc[k] += ms;
       }
-    fprintf(stderr, "[gb trace] shard %u/%u, %zu sweeps: k_pr_cb %.4f  k_pr_fixup %.4f  k_pr_sell %.4f  k_pr_finish %.4f ms\n",
+    fprintf(stderr, p->vb ? "[gb trace] shard %u/%u, %zu sweeps: k_pr_cb %.4f  pass A %.4f  pass B %.4f  k_pr_finish %.4f ms\n"
+                          : "[gb trace] shard %u/%u, %zu sweeps: k_pr_cb %.4f  k_pr_fixup %.4f  k_pr_sell %.4f  k_pr_finish %.4f ms\n",
             p->deal.p, p->deal.P, sweeps, acc[0] / sweeps, acc[1] / sweeps, acc[2] / sweeps, acc[3] / sweeps);
   }
   for (cudaEvent_t e : p->trace_events) cudaEventDestroy(e);
@@ -125,6 +126,13 @@ struct PrArgs {
   uint32_t n_tasks, n_task_ranges;
   uint32_t* task_ctr;
   float* rem;
+  // pass A of the virtual blocks (k_pr_cb<CB_BIN>)
+  float* vals;
+  const uint16_t* bin_ids;
+  const uint32_t* bin_bits;
+  const uint32_t* bin_grun;
+  const uint2* bin_runs;
+  const uint2* bin_chunks;
   // SELL rows
   const uint4* sell;
   const uint2* slice_meta;
@@ -335,6 +343,41 @@ __device__ __forceinline__ void cb_chunk(const PrArgs& a, const float* xs, uint3
   }
 }
 
+// Pass A of the virtual blocks, one warp per chunk of 32-position groups of one source block: lane i of group g
+// stores the value of the pair at position 32 g + i to its slot of V.  A run's slots are consecutive, so the
+// stores of a group are coalesced; the run of a position is the group's first run plus the run starts after it.
+__device__ __forceinline__ void bin_chunk(const PrArgs& a, const float* xs, uint32_t c, uint32_t lane) {
+  const uint2 ch = a.bin_chunks[c];
+  const uint32_t after = (2u << lane) - 2u;  // positions 1 .. lane of the group
+#pragma unroll 4
+  for (uint32_t g = ch.x; g < ch.y; ++g) {
+    const uint32_t i = 32 * g + lane;
+    const uint32_t id = __ldg(a.bin_ids + i);
+    if (id == BIN_PAD) continue;
+    const uint2 run = __ldg(a.bin_runs + __ldg(a.bin_grun + g) + __popc(__ldg(a.bin_bits + g) & after));
+    a.vals[run.y + (i - run.x)] = xs[id];
+  }
+}
+
+// Segments cut by chunk boundaries (segments longer than a chunk): one warp per segment adds its parts
+// in a fixed order — the head part of the first chunk, then lanes over the following chunks (a fixed
+// xor tree per batch of 32).  Tiny; runs after k_pr_cb (as k_pr_fixup, or as the prologue of k_pr_sell or of
+// pass A).
+__device__ __forceinline__ void cb_fix_segment(const PrArgs& a, uint32_t c0, uint32_t lane) {
+  double t = a.side[2 * (size_t)c0 + 1];
+  for (uint32_t k0 = c0 + 1;; k0 += 32) {
+    const uint32_t k = k0 + lane;
+    // the walk ends at the first chunk that is not entirely inside the segment (sentinel chunk after the last)
+    const uint32_t fl = a.chunks[min(k, a.n_chunks)].w >> 24;
+    const bool inside = k < a.n_chunks && (fl & CB_INTERIOR) && (fl & CB_TAIL_CONT);
+    const uint32_t stop = __ballot_sync(0xFFFFFFFFu, !inside);
+    const uint32_t upto = stop ? (uint32_t)__ffs(stop) - 1 : 31u;  // last lane that contributes
+    t += warp_sum(lane <= upto ? a.side[2 * (size_t)k] : 0.0);
+    if (stop) break;
+  }
+  if (lane == 0) a.partial[a.tail_slot[c0]] = (float)t;
+}
+
 // ---- TMA bulk copy of a source block into shared memory (cp.async.bulk + mbarrier) -----------------
 // One thread asks the copy engine for the block's 192 KB and every thread waits on the mbarrier's phase:
 // no load/store instruction of the CTA is spent on the transfer and it runs at the SM's L2 bandwidth
@@ -373,6 +416,11 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
 // thin blocks are (a purely static split leaves thin blocks at single-warp latency, one global cursor reloads the
 // block for every task).  Claiming the next task one task ahead (to hide the atomic's
 // round trip) was measured and dropped: a claimed task cannot be stolen, which costs more at the tail.
+// KIND: CB_MAIN = the column blocks of x_cur; CB_BIN = pass A of the virtual blocks (the same loads of x_cur,
+// bin_chunk per chunk; its first warps also add the cut segments of CB_MAIN); CB_VIRT = pass B (block j is
+// V[blk[j] .. blk[j + 1]), the column-block walker as in CB_MAIN).
+constexpr uint32_t CB_MAIN = 0, CB_VIRT = 1, CB_BIN = 2;
+template <uint32_t KIND>
 __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
   extern __shared__ __align__(128) float smem[];
   float* xs = smem;  // B entries of x_cur + one zero slot (the pad id)
@@ -380,6 +428,9 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
   __shared__ __align__(8) unsigned long long s_mbar;
   if (a.ctrl[0] != 0) return;  // tolerance already met by an earlier sweep of this batch
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (KIND == CB_BIN)  // k_pr_cb<CB_MAIN> has finished: no k_pr_fixup launch on this path
+    for (uint32_t i = blockIdx.x * PR_WARPS + warp; i < a.n_fix; i += gridDim.x * PR_WARPS)
+      cb_fix_segment(a, a.fix_list[i], lane);
   const uint32_t B = a.B;
   const uint32_t pad2 = B | (B << 16);
   const uint32_t R = gridDim.x;  // ranges = CTAs
@@ -430,8 +481,8 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
     const uint2 task = a.tasks[t];  // (first chunk, chunk count | block rank << 8)
     const uint32_t j = task.y >> 8;
     if (j != cur_j) {
-      const uint64_t x0 = (uint64_t)a.blk[j] * B;
-      const uint32_t cnt = (uint32_t)min((uint64_t)B, (uint64_t)a.n - x0);
+      const uint64_t x0 = KIND == CB_VIRT ? (uint64_t)a.blk[j] : (uint64_t)a.blk[j] * B;
+      const uint32_t cnt = KIND == CB_VIRT ? a.blk[j + 1] - a.blk[j] : (uint32_t)min((uint64_t)B, (uint64_t)a.n - x0);
       if (bulk_ok) {
         const uint32_t bulk = cnt & ~3u;
         if (threadIdx.x == 0) {
@@ -452,7 +503,8 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
     // a warp starts with chunk `warp` of the task and claims further ones from the CTA's counter
     const uint32_t nchunks = task.y & 0xFFu;
     for (uint32_t k = warp; k < nchunks;) {
-      cb_chunk(a, xs, task.x + k, lane, pad2);
+      if (KIND == CB_BIN) bin_chunk(a, xs, task.x + k, lane);
+      else cb_chunk(a, xs, task.x + k, lane, pad2);
       uint32_t nx = 0;
       if (lane == 0) nx = atomicAdd(&s_next, 1u);
       k = __shfl_sync(0xFFFFFFFFu, nx, 0);
@@ -460,23 +512,6 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
   }
 }
 
-// Segments cut by chunk boundaries (segments longer than a chunk): one warp per segment adds its parts
-// in a fixed order — the head part of the first chunk, then lanes over the following chunks (a fixed
-// xor tree per batch of 32).  Tiny; runs after k_pr_cb (as k_pr_fixup, or as the prologue of k_pr_sell).
-__device__ __forceinline__ void cb_fix_segment(const PrArgs& a, uint32_t c0, uint32_t lane) {
-  double t = a.side[2 * (size_t)c0 + 1];
-  for (uint32_t k0 = c0 + 1;; k0 += 32) {
-    const uint32_t k = k0 + lane;
-    // the walk ends at the first chunk that is not entirely inside the segment (sentinel chunk after the last)
-    const uint32_t fl = a.chunks[min(k, a.n_chunks)].w >> 24;
-    const bool inside = k < a.n_chunks && (fl & CB_INTERIOR) && (fl & CB_TAIL_CONT);
-    const uint32_t stop = __ballot_sync(0xFFFFFFFFu, !inside);
-    const uint32_t upto = stop ? (uint32_t)__ffs(stop) - 1 : 31u;  // last lane that contributes
-    t += warp_sum(lane <= upto ? a.side[2 * (size_t)k] : 0.0);
-    if (stop) break;
-  }
-  if (lane == 0) a.partial[a.tail_slot[c0]] = (float)t;
-}
 __global__ void k_pr_fixup(const PrArgs a) {
   if (a.ctrl[0] != 0) return;
   const uint32_t lane = threadIdx.x & 31;
@@ -827,12 +862,16 @@ gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, cons
                            int dev_sms, cudaStream_t s) {
   p->trace = (uint32_t)env_u64("GB_PR_TRACE", 0) != 0;
   p->smem_cb = ((size_t)p->B + 4) * sizeof(float);
-  GB_CUDA(cudaFuncSetAttribute(k_pr_cb, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cb));
+  GB_CUDA(cudaFuncSetAttribute(k_pr_cb<CB_MAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cb));
+  GB_CUDA(cudaFuncSetAttribute(k_pr_cb<CB_VIRT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cb));
+  GB_CUDA(cudaFuncSetAttribute(k_pr_cb<CB_BIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cb));
   const uint64_t want_sell = ((uint64_t)p->num_slices + PR_SELL_THREADS / 32 - 1) / (PR_SELL_THREADS / 32);
   p->grid_sell = (unsigned)std::min<uint64_t>(want_sell, (uint64_t)dev_sms * 2);
   // rows with segments in more than SELL_FEW blocks are a prefix (nrows[] is non-increasing): k_pr_finish
-  // completes them; all others are completed by their k_pr_sell lane (k_pr_cb is done by then)
+  // completes them; all others are completed by their k_pr_sell lane (k_pr_cb is done by then).  With virtual
+  // blocks k_pr_finish completes every local row.
   p->n_fin = p->KB > SELL_FEW ? std::min<uint32_t>(p->n_cb, (h_nrows[SELL_FEW] + 31) / 32 * 32) : 0;
+  if (p->vb) p->n_fin = p->n_loc;
   for (uint32_t j = 0; j < SELL_FEW && j < p->KB; ++j) {
     p->few_nrows[j] = h_nrows[j];
     p->few_poff[j] = h_poff[j];
@@ -879,7 +918,7 @@ gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, cons
 static bool fix_in_sell(const PrPlan* p) {
   return p->n_fix && p->grid_sell && p->fix_max_row < p->n_fin;
 }
-static bool fixup_launched(const PrPlan* p) { return p->grid_cb && p->n_fix && !fix_in_sell(p); }
+static bool fixup_launched(const PrPlan* p) { return p->grid_cb && p->n_fix && !fix_in_sell(p) && !p->vb; }
 static PrArgs make_args(const PrPlan* p, float base, float damping, double tolerance) {
   PrArgs a{};
   a.outdeg = p->outdeg.p;
@@ -913,8 +952,8 @@ static PrArgs make_args(const PrPlan* p, float base, float damping, double toler
   a.tasks = p->tasks.p;
   a.n_tasks = p->n_tasks;
   a.task_ctr = p->task_ctr.p;
-  a.n_task_ranges = p->grid_cb;
-  a.rem = p->rem.p;
+  a.n_task_ranges = p->task_ranges();
+  a.rem = p->vb ? p->v.partial.p : p->rem.p;
   a.fin_kb = p->fin_kb.p;
   a.sell = p->sell.p;
   a.slice_meta = p->slice_meta.p;
@@ -930,6 +969,41 @@ static PrArgs make_args(const PrPlan* p, float base, float damping, double toler
   a.mc_next = nullptr;
   return a;
 }
+// pass A of the virtual blocks: a's source blocks and cut segments, the pass's own tasks and chunks
+static PrArgs bin_args(const PrPlan* p, const PrArgs& a) {
+  PrArgs b = a;
+  b.blk = p->v.bin_blk.p;
+  b.tasks = p->v.bin_tasks.p;
+  b.n_tasks = p->v.bin_n_tasks;
+  b.task_ctr = p->task_ctr.p + p->grid_cb;
+  b.vals = p->v.val.p;
+  b.bin_ids = p->v.bin_ids.p;
+  b.bin_bits = p->v.bin_bits.p;
+  b.bin_grun = p->v.bin_grun.p;
+  b.bin_runs = p->v.bin_runs.p;
+  b.bin_chunks = p->v.bin_chunks.p;
+  return b;
+}
+// pass B: the column-block stream of the virtual blocks, over V; partial = the rows' cold sums
+static PrArgs virt_args(const PrPlan* p, const PrArgs& a) {
+  PrArgs b = a;
+  b.x_cur = p->v.val.p;
+  b.blk = p->v.vbase.p;
+  b.poff = p->v.row0.p;
+  b.cb_ids = p->v.ids.p;
+  b.cb_bits = p->v.bits.p;
+  b.partial = p->v.partial.p;
+  b.chunks = p->v.cut.chunks.p;
+  b.n_chunks = p->v.cut.n_chunks;
+  b.tail_slot = p->v.cut.tail_slot.p;
+  b.side = p->v.cut.side.p;
+  b.fix_list = p->v.cut.fix_list.p;
+  b.n_fix = p->v.cut.n_fix;
+  b.tasks = p->v.cut.tasks.p;
+  b.n_tasks = p->v.cut.n_tasks;
+  b.task_ctr = p->task_ctr.p + p->grid_cb + p->grid_bin;
+  return b;
+}
 
 // one sweep = column blocks (+ fixup of cut segments), SELL rows, then finish; *launches is advanced by
 // the kernels launched
@@ -944,7 +1018,7 @@ static gb_status launch_sweep(const PrPlan* p, const PrArgs& a, cudaStream_t s, 
     GB_CUDA(cudaEventRecord(ev[0], s));
   }
   if (p->grid_cb) {
-    k_pr_cb<<<p->grid_cb, PR_THREADS, p->smem_cb, s>>>(a);
+    k_pr_cb<CB_MAIN><<<p->grid_cb, PR_THREADS, p->smem_cb, s>>>(a);
     *launches += 1;
   }
   if (ev) GB_CUDA(cudaEventRecord(ev[1], s));
@@ -952,9 +1026,17 @@ static gb_status launch_sweep(const PrPlan* p, const PrArgs& a, cudaStream_t s, 
     k_pr_fixup<<<grid_for((uint64_t)p->n_fix * 32, 128, 296), 128, 0, s>>>(a);
     *launches += 1;
   }
+  if (p->vb) {
+    k_pr_cb<CB_BIN><<<p->grid_bin, PR_THREADS, p->smem_cb, s>>>(bin_args(p, a));
+    *launches += 1;
+  }
   if (ev) GB_CUDA(cudaEventRecord(ev[2], s));
   if (p->grid_sell) {
     k_pr_sell<PEERS><<<p->grid_sell, PR_SELL_THREADS, 0, s>>>(a);
+    *launches += 1;
+  }
+  if (p->vb) {
+    k_pr_cb<CB_VIRT><<<p->grid_vb, PR_THREADS, p->smem_cb, s>>>(virt_args(p, a));
     *launches += 1;
   }
   if (ev) GB_CUDA(cudaEventRecord(ev[3], s));
@@ -975,7 +1057,7 @@ static gb_status pr_reset(const PrPlan* p, PrStart v, float* x0, float* x1, floa
   k_pr_init<<<grid_for(p->n, 256), 256, 0, s>>>(p->n, p->n_active, v.init, v.base, p->deal, p->outdeg.p, x0, x1,
                                                 scores);
   GB_CUDA(cudaMemsetAsync(p->ctrl.p, 0, 8, s));
-  GB_CUDA(cudaMemsetAsync(p->task_ctr.p, 0, (size_t)std::max<unsigned>(p->grid_cb, 1) * 4, s));
+  GB_CUDA(cudaMemsetAsync(p->task_ctr.p, 0, (size_t)std::max<unsigned>(p->task_ranges(), 1) * 4, s));
   return GB_OK;
 }
 // the closed-form error of the rows without in-edges, contributed to sweep 1 once, by rank 0
@@ -1122,8 +1204,12 @@ static void plan_stats(const PrPlan* p, gb_pr_shard_stats* stats) {
   stats->tasks = p->n_tasks;
   stats->cut_segments = p->n_fix;
   stats->chunk_groups = p->chunk_groups;
-  stats->launches_per_sweep = 1 + (p->grid_cb ? 1 : 0) + (p->grid_sell ? 1 : 0) + (fixup_launched(p) ? 1 : 0);
+  stats->launches_per_sweep = 1 + (p->grid_cb ? 1 : 0) + (p->grid_sell ? 1 : 0) + (fixup_launched(p) ? 1 : 0) +
+                              (p->vb ? 2 : 0);
   stats->device_bytes = p->bytes();
+  stats->vblock_parts = p->vb ? p->v.parts : 0;
+  stats->vblock_pairs = p->vb ? p->v.pairs : 0;
+  stats->vblock_edges = p->vb ? p->v.edges : 0;
 }
 static void plan_shape(const PrPlan* p, gb_pr_plan_shape* shape) {
   shape->hot_blocks = p->KB;

@@ -396,6 +396,99 @@ __global__ void k_sell_fill_tail(const uint32_t* __restrict__ in_off, const uint
     }
   }
 }
+// ---- virtual blocks (PrVBlocks): built from the SELL lanes, which hold every cold edge of a row in CSR order -----
+__host__ __device__ __forceinline__ uint32_t vb_part_of(const uint32_t* __restrict__ row0, uint32_t parts, uint32_t l) {
+  uint32_t lo = 0, hi = parts;  // last partition with row0[k] <= l
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) / 2;
+    if (row0[mid] <= l) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+// one thread per local row: key (partition << 32 | source) and row of each cold edge, edges numbered by row
+__global__ void k_vb_edges(const uint32_t* __restrict__ lens, const uint32_t* __restrict__ coff,
+                           const uint32_t* __restrict__ row0, uint32_t parts, uint32_t n_loc,
+                           const uint2* __restrict__ slice_meta, const uint32_t* __restrict__ sell,
+                           uint64_t* __restrict__ keys, uint32_t* __restrict__ idx, uint32_t* __restrict__ erow) {
+  for (uint32_t l = blockIdx.x * blockDim.x + threadIdx.x; l < n_loc; l += gridDim.x * blockDim.x) {
+    const uint32_t d = lens[l], o = coff[l];
+    const uint64_t k = vb_part_of(row0, parts, l);
+    const uint2 meta = slice_meta[l >> 5];
+    for (uint32_t q = 0; q < d; ++q) {
+      keys[o + q] = k << 32 | sell[((uint64_t)meta.x + (uint64_t)(q / 4) * 32 + (l & 31u)) * 4 + (q % 4)];
+      idx[o + q] = o + q;
+      erow[o + q] = l;
+    }
+  }
+}
+__global__ void k_vb_starts(const uint64_t* __restrict__ keys, uint32_t E, uint32_t* __restrict__ flag) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < E; i += gridDim.x * blockDim.x)
+    flag[i] = (i == 0 || keys[i] != keys[i - 1]) ? 1u : 0u;
+}
+// first[k] = first index of sorted keys with key >> shift >= k, then that entry's rank (inclusive rank - 1,
+// or the total past the end): the first pair of partition k, or of source block k
+__global__ void k_vb_bounds(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ rank, uint32_t E,
+                            uint32_t shift, uint32_t count, uint32_t total, uint32_t* __restrict__ first) {
+  for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k <= count; k += gridDim.x * blockDim.x) {
+    uint32_t lo = 0, hi = E;
+    while (lo < hi) {
+      const uint32_t mid = lo + (hi - lo) / 2;
+      if ((keys[mid] >> shift) < k) lo = mid + 1;
+      else hi = mid;
+    }
+    first[k] = lo < E ? (rank ? rank[lo] - 1 : lo) : total;
+  }
+}
+// every cold edge (sorted by pair): its V-local slot id into its row's segment of pass B; the first edge of every
+// pair also leaves the pair's pass A key (source block << 43 | partition << 16 | block-local source) and V slot
+constexpr uint32_t VB_BLK_SHIFT = 43;
+__global__ void k_vb_place(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ idx,
+                           const uint32_t* __restrict__ rank, uint32_t E, const uint32_t* __restrict__ erow,
+                           const uint32_t* __restrict__ coff, const uint32_t* __restrict__ goffv,
+                           const uint32_t* __restrict__ pfirst, const uint32_t* __restrict__ vbase, uint32_t B,
+                           uint16_t* __restrict__ ids, uint64_t* __restrict__ akey, uint32_t* __restrict__ aslot) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < E; i += gridDim.x * blockDim.x) {
+    const uint64_t key = keys[i];
+    const uint32_t k = (uint32_t)(key >> 32), src = (uint32_t)key;
+    const uint32_t pair = rank[i] - 1, slot = pair - pfirst[k];
+    const uint32_t e = idx[i], l = erow[e];
+    ids[(uint64_t)goffv[l] * CB_G + (e - coff[l])] = (uint16_t)slot;
+    if (i == 0 || keys[i - 1] != key) {
+      akey[pair] = (uint64_t)(src / B) << VB_BLK_SHIFT | (uint64_t)k << 16 | (src % B);
+      aslot[pair] = vbase[k] + slot;
+    }
+  }
+}
+// pass A positions: pair i of source block b goes to bpos[b] + (i - bfirst[b]); runs start where (block,
+// partition) changes
+__global__ void k_bin_place(const uint64_t* __restrict__ akey, const uint32_t* __restrict__ aslot, uint32_t NP,
+                            const uint32_t* __restrict__ bfirst, const uint32_t* __restrict__ bpos,
+                            const uint32_t* __restrict__ brank, const uint32_t* __restrict__ run_rank,
+                            uint16_t* __restrict__ ids, uint32_t* __restrict__ bits, uint32_t* __restrict__ grun,
+                            uint2* __restrict__ runs) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < NP; i += gridDim.x * blockDim.x) {
+    const uint64_t key = akey[i];
+    const uint32_t b = (uint32_t)(key >> VB_BLK_SHIFT);
+    const uint32_t pos = bpos[brank[b]] + (i - bfirst[b]);
+    const uint32_t r = run_rank[i] - 1;
+    ids[pos] = (uint16_t)(key & 0xFFFFu);
+    if (i == 0 || (akey[i - 1] >> 16) != (key >> 16)) {
+      atomicOr(bits + pos / 32, 1u << (pos % 32));
+      runs[r] = make_uint2(pos, aslot[i]);
+    }
+    if (pos % 32 == 0) grun[pos / 32] = r;
+  }
+}
+__global__ void k_run_starts(const uint64_t* __restrict__ akey, uint32_t NP, uint32_t* __restrict__ flag) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < NP; i += gridDim.x * blockDim.x)
+    flag[i] = (i == 0 || (akey[i - 1] >> 16) != (akey[i] >> 16)) ? 1u : 0u;
+}
+__global__ void k_vb_groups(const uint32_t* __restrict__ lens, uint32_t n_loc, uint32_t* __restrict__ g) {
+  for (uint32_t l = blockIdx.x * blockDim.x + threadIdx.x; l < n_loc; l += gridDim.x * blockDim.x)
+    g[l] = lens[l] ? (lens[l] + CB_G - 1) / CB_G : 1u;  // a row without cold edges keeps one padding group
+}
+
 __global__ void k_gather_u32(const uint32_t* __restrict__ src, const uint32_t* __restrict__ idx, uint32_t count,
                              uint32_t* __restrict__ dst) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) dst[i] = src[idx[i]];
@@ -602,6 +695,7 @@ struct LayoutBuild {
   gb_status layout_classify();
   gb_status layout_sell();
   gb_status layout_fill();
+  gb_status layout_vblocks();
   gb_status layout_chunks();
 };
 
@@ -882,62 +976,286 @@ gb_status LayoutBuild::layout_fill() {
   return GB_OK;
 }
 
-// Chunks of the column-block kernel, the bank order of the ids inside them, and every persistent CTA's
-// share of them (tasks); then the sweep's per-pair and per-row buffers.
+static gb_status cb_chunk_table(cudaStream_t s, int dev_sms, uint32_t B, const uint32_t* goff, const uint32_t* poff,
+                                const uint32_t* nrows, uint32_t KB, uint64_t NG, const std::vector<uint32_t>& min_cgrp,
+                                uint2* ids, CbChunks* out);
+constexpr uint64_t VB_L2_FACTOR = 2;  // the virtual blocks run when the source vector exceeds this many L2s
+static uint32_t bits_for(uint64_t count) {  // bits of the largest index below count
+  uint32_t b = 1;
+  while ((1ull << b) < count) ++b;
+  return b;
+}
+template <typename K, typename V>
+static gb_status sort_pairs(cudaStream_t s, cub::DoubleBuffer<K>& k, cub::DoubleBuffer<V>& v, uint32_t count,
+                            uint32_t end_bit) {
+  DevBuf<uint8_t> tmp;
+  GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
+    return cub::DeviceRadixSort::SortPairs(t, tb, k, v, (int)count, 0, (int)end_bit, s);
+  }));
+  GB_CUDA(cudaStreamSynchronize(s));
+  return GB_OK;
+}
+static gb_status scan_inclusive(cudaStream_t s, uint32_t* data, uint32_t count) {
+  DevBuf<uint8_t> tmp;
+  GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) { return cub::DeviceScan::InclusiveSum(t, tb, data, data, (int)count, s); }));
+  GB_CUDA(cudaStreamSynchronize(s));
+  return GB_OK;
+}
+
+// Virtual blocks (PrVBlocks) in place of the SELL slices, when the source vector is well past L2: there a SELL
+// gather of a cold edge is mostly a 32-byte sector from HBM for a 4-byte value, while the two passes stream ids
+// and values and gather from shared memory only.  Just past L2 most gathers still hit (H100, 50 MB L2: RMAT-24,
+// 64 MiB, ran 1.5 % slower with them; RMAT-26, 256 MiB, 28 % faster), hence VB_L2_FACTOR.  GB_PR_VBLOCKS (tests, experiments): 1 builds them whatever the
+// size, 2 never, 0 = automatic.  A row with more than B cold edges would need more than one virtual block: such a
+// graph keeps the SELL path.
+gb_status LayoutBuild::layout_vblocks() {
+  const uint32_t force = (uint32_t)env_u64("GB_PR_VBLOCKS", 0);
+  int l2 = 0;
+  GB_CUDA(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, src.device));
+  if (!p->n_loc || force == 2 || (force != 1 && 4ull * n <= VB_L2_FACTOR * (uint64_t)l2)) return GB_OK;
+  const uint32_t n_loc = p->n_loc;
+  std::vector<uint32_t> h_lens(n_loc);
+  GB_CUDA(cudaMemcpyAsync(h_lens.data(), lens.p, (size_t)n_loc * 4, cudaMemcpyDeviceToHost, s));
+  GB_CUDA(cudaStreamSynchronize(s));
+  // partitions: greedy, at most B cold edges each (so at most B distinct sources)
+  std::vector<uint32_t> h_row0{0}, h_mseg;  // first rows; longest segment of each partition, in groups
+  uint64_t E = 0, acc = 0;
+  uint32_t mseg = 0;
+  for (uint32_t l = 0; l < n_loc; ++l) {
+    const uint32_t d = h_lens[l];
+    if (d > B) return GB_OK;
+    if (acc + d > B && l > h_row0.back()) {
+      h_row0.push_back(l);
+      h_mseg.push_back(mseg);
+      acc = 0;
+      mseg = 0;
+    }
+    acc += d;
+    E += d;
+    mseg = std::max(mseg, d ? (d + CB_G - 1) / CB_G : 1u);
+  }
+  h_mseg.push_back(mseg);
+  h_row0.push_back(n_loc);
+  if (E == 0 || E >= 0x7FFFFFFFull) return GB_OK;
+  PrVBlocks& v = p->v;
+  const uint32_t parts = (uint32_t)h_mseg.size();
+  std::vector<uint32_t> h_rows(parts), h_min(parts);
+  for (uint32_t k = 0; k < parts; ++k) {
+    h_rows[k] = h_row0[k + 1] - h_row0[k];
+    h_min[k] = (h_mseg[k] + 31) / 32 * 32;  // no segment is cut by a chunk boundary: no fixup pass
+  }
+  GB_TRY(upload(s, &v.row0, h_row0));
+  GB_TRY(upload(s, &v.rows, h_rows));
+  // pass B's segments: one per local row, the cold edges' slot ids in CSR order
+  DevBuf<uint32_t> coff, goffv;
+  GB_TRY(coff.alloc((size_t)n_loc + 1));
+  GB_TRY(goffv.alloc((size_t)n_loc + 1));
+  GB_CUDA(cudaMemcpyAsync(coff.p, lens.p, (size_t)n_loc * 4, cudaMemcpyDeviceToDevice, s));
+  GB_CUDA(cudaMemsetAsync(coff.p + n_loc, 0, 4, s));
+  GB_TRY(scan_exclusive(s, coff.p, (uint64_t)n_loc + 1));
+  k_vb_groups<<<grid_for(n_loc, 256), 256, 0, s>>>(lens.p, n_loc, goffv.p);
+  GB_CUDA(cudaMemsetAsync(goffv.p + n_loc, 0, 4, s));
+  GB_TRY(scan_exclusive(s, goffv.p, (uint64_t)n_loc + 1));
+  uint32_t ngv = 0;
+  GB_CUDA(cudaMemcpyAsync(&ngv, goffv.p + n_loc, 4, cudaMemcpyDeviceToHost, s));
+  GB_CUDA(cudaStreamSynchronize(s));
+  v.NG = ngv;
+  GB_TRY(v.ids.alloc(v.NG, 64));
+  GB_TRY(v.bits.alloc(v.NG / 32 + 8));
+  GB_CUDA(cudaMemsetAsync(v.bits.p, 0, (v.NG / 32 + 8) * 4, s));
+  k_fill_u2<<<grid_for(v.NG + 64, 256), 256, 0, s>>>(v.ids.p, v.NG + 64, make_uint2(B | (B << 16), B | (B << 16)));
+  k_cb_bits<<<grid_for(n_loc, 256), 256, 0, s>>>(goffv.p, n_loc, v.bits.p);
+  // the cold edges sorted by (partition, source): a run of equal keys is one pair, one slot of V
+  const uint32_t Ec = (uint32_t)E;
+  uint32_t NP = 0;
+  DevBuf<uint64_t> akey, akey_alt;
+  DevBuf<uint32_t> aslot, aslot_alt;
+  {
+    DevBuf<uint64_t> keys, keys_alt;
+    DevBuf<uint32_t> idx, idx_alt, erow, rank, pfirst;
+    GB_TRY(keys.alloc(Ec));
+    GB_TRY(keys_alt.alloc(Ec));
+    GB_TRY(idx.alloc(Ec));
+    GB_TRY(idx_alt.alloc(Ec));
+    GB_TRY(erow.alloc(Ec));
+    k_vb_edges<<<grid_for(n_loc, 256), 256, 0, s>>>(lens.p, coff.p, v.row0.p, parts, n_loc, p->slice_meta.p,
+                                                    reinterpret_cast<const uint32_t*>(p->sell.p), keys.p, idx.p, erow.p);
+    cub::DoubleBuffer<uint64_t> kb(keys.p, keys_alt.p);
+    cub::DoubleBuffer<uint32_t> ib(idx.p, idx_alt.p);
+    GB_TRY(sort_pairs(s, kb, ib, Ec, 32 + bits_for(parts)));
+    GB_TRY(rank.alloc(Ec));
+    k_vb_starts<<<grid_for(Ec, 256), 256, 0, s>>>(kb.Current(), Ec, rank.p);
+    GB_TRY(scan_inclusive(s, rank.p, Ec));
+    GB_CUDA(cudaMemcpyAsync(&NP, rank.p + Ec - 1, 4, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaStreamSynchronize(s));
+    GB_TRY(pfirst.alloc((size_t)parts + 1));
+    k_vb_bounds<<<grid_for(parts + 1, 128), 128, 0, s>>>(kb.Current(), rank.p, Ec, 32, parts, NP, pfirst.p);
+    std::vector<uint32_t> h_pfirst(parts + 1);
+    GB_CUDA(cudaMemcpyAsync(h_pfirst.data(), pfirst.p, (size_t)(parts + 1) * 4, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaStreamSynchronize(s));
+    std::vector<uint32_t> h_vbase(parts + 1, 0);
+    for (uint32_t k = 0; k < parts; ++k)
+      h_vbase[k + 1] = h_vbase[k] + (h_pfirst[k + 1] - h_pfirst[k] + VB_ALIGN - 1) / VB_ALIGN * VB_ALIGN;
+    GB_TRY(upload(s, &v.vbase, h_vbase));
+    GB_TRY(v.val.alloc(std::max<uint32_t>(h_vbase[parts], 1)));
+    GB_CUDA(cudaMemsetAsync(v.val.p, 0, (size_t)std::max<uint32_t>(h_vbase[parts], 1) * 4, s));
+    GB_TRY(akey.alloc(NP));
+    GB_TRY(akey_alt.alloc(NP));
+    GB_TRY(aslot.alloc(NP));
+    GB_TRY(aslot_alt.alloc(NP));
+    k_vb_place<<<grid_for(Ec, 256), 256, 0, s>>>(kb.Current(), ib.Current(), rank.p, Ec, erow.p, coff.p, goffv.p,
+                                                 pfirst.p, v.vbase.p, B, reinterpret_cast<uint16_t*>(v.ids.p),
+                                                 akey.p, aslot.p);
+    GB_CUDA(cudaGetLastError());
+    GB_CUDA(cudaStreamSynchronize(s));
+  }
+  // pass A: the pairs by (source block, partition, source); each block's share starts at a multiple of 32
+  const uint32_t nblk = (uint32_t)(((uint64_t)n + B - 1) / B);
+  cub::DoubleBuffer<uint64_t> akb(akey.p, akey_alt.p);
+  cub::DoubleBuffer<uint32_t> asb(aslot.p, aslot_alt.p);
+  GB_TRY(sort_pairs(s, akb, asb, NP, VB_BLK_SHIFT + bits_for(nblk)));
+  DevBuf<uint32_t> run_rank, bfirst, brank, bpos;
+  GB_TRY(run_rank.alloc(NP));
+  k_run_starts<<<grid_for(NP, 256), 256, 0, s>>>(akb.Current(), NP, run_rank.p);
+  GB_TRY(scan_inclusive(s, run_rank.p, NP));
+  GB_CUDA(cudaMemcpyAsync(&v.n_runs, run_rank.p + NP - 1, 4, cudaMemcpyDeviceToHost, s));
+  GB_TRY(bfirst.alloc((size_t)nblk + 1));
+  k_vb_bounds<<<grid_for(nblk + 1, 128), 128, 0, s>>>(akb.Current(), nullptr, NP, VB_BLK_SHIFT, nblk, NP, bfirst.p);
+  std::vector<uint32_t> h_bfirst(nblk + 1);
+  GB_CUDA(cudaMemcpyAsync(h_bfirst.data(), bfirst.p, (size_t)(nblk + 1) * 4, cudaMemcpyDeviceToHost, s));
+  GB_CUDA(cudaStreamSynchronize(s));
+  std::vector<uint32_t> h_brank(nblk, CB_NONE), h_bblk, h_bpos;
+  std::vector<uint2> h_chunks, h_tasks;
+  uint64_t npos = 0;
+  for (uint32_t b = 0; b < nblk; ++b) {
+    const uint32_t cnt = h_bfirst[b + 1] - h_bfirst[b];
+    if (!cnt) continue;
+    const uint32_t j = (uint32_t)h_bblk.size();
+    h_brank[b] = j;
+    h_bblk.push_back(b);
+    h_bpos.push_back((uint32_t)npos);
+    const uint32_t g0 = (uint32_t)(npos / 32), g1 = g0 + (cnt + 31) / 32;
+    const uint32_t c0 = (uint32_t)h_chunks.size();
+    for (uint32_t g = g0; g < g1; g += BIN_CHUNK) h_chunks.push_back(make_uint2(g, std::min(g1, g + BIN_CHUNK)));
+    const uint32_t nc = (uint32_t)h_chunks.size() - c0;
+    for (uint32_t c = 0; c < nc; c += CB_TASK_CHUNKS)
+      h_tasks.push_back(make_uint2(c0 + c, (std::min(nc, c + CB_TASK_CHUNKS) - c) | (j << 8)));
+    npos += (uint64_t)(g1 - g0) * 32;
+    GB_REQUIRE(npos < 0xFFFFFFE0ull, "too many virtual-block pairs (%llu positions)", (unsigned long long)npos);
+  }
+  v.bin_blocks = (uint32_t)h_bblk.size();
+  v.bin_n_tasks = (uint32_t)h_tasks.size();
+  GB_TRY(upload(s, &brank, h_brank));
+  GB_TRY(upload(s, &bpos, h_bpos));
+  GB_TRY(upload(s, &v.bin_blk, h_bblk));
+  GB_TRY(upload(s, &v.bin_chunks, h_chunks));
+  GB_TRY(upload(s, &v.bin_tasks, h_tasks));
+  GB_TRY(v.bin_ids.alloc(npos));
+  GB_CUDA(cudaMemsetAsync(v.bin_ids.p, 0xFF, npos * 2, s));  // BIN_PAD
+  GB_TRY(v.bin_bits.alloc(npos / 32));
+  GB_CUDA(cudaMemsetAsync(v.bin_bits.p, 0, npos / 32 * 4, s));
+  GB_TRY(v.bin_grun.alloc(npos / 32));
+  GB_TRY(v.bin_runs.alloc(v.n_runs));
+  k_bin_place<<<grid_for(NP, 256), 256, 0, s>>>(akb.Current(), asb.Current(), NP, bfirst.p, bpos.p, brank.p,
+                                                run_rank.p, v.bin_ids.p, v.bin_bits.p, v.bin_grun.p, v.bin_runs.p);
+  GB_CUDA(cudaGetLastError());
+  // pass B's chunks and tasks over the virtual blocks (rows [row0[k], row0[k + 1]) each)
+  GB_TRY(cb_chunk_table(s, dev_sms, B, goffv.p, v.row0.p, v.rows.p, parts, v.NG, h_min, v.ids.p, &v.cut));
+  GB_REQUIRE(v.cut.n_fix == 0, "a virtual-block segment is cut by a chunk boundary");
+  GB_TRY(v.partial.alloc(n_loc));
+  GB_CUDA(cudaMemsetAsync(v.partial.p, 0, (size_t)n_loc * 4, s));
+  v.parts = parts;
+  v.pairs = NP;
+  v.edges = E;
+  p->grid_bin = (unsigned)std::min<uint64_t>(v.bin_n_tasks, (uint64_t)dev_sms);
+  p->grid_vb = (unsigned)std::min<uint64_t>(v.cut.n_tasks, (uint64_t)dev_sms);
+  // the SELL slices have served as the build's list of cold edges: k_pr_sell does not run
+  p->sell = DevBuf<uint4>();
+  p->slice_meta = DevBuf<uint2>();
+  p->num_slices = 0;
+  p->vb = true;
+  GB_CUDA(cudaStreamSynchronize(s));
+  return GB_OK;
+}
+
+// Chunks of one column-block stream (KB blocks, block j's segments start at goff[poff[j] ..], NG groups), the
+// bank order of the ids inside them, and every persistent CTA's share of them (tasks).  min_cgrp (empty: none)
+// raises block j's chunk length to at least min_cgrp[j] groups.
+static gb_status cb_chunk_table(cudaStream_t s, int dev_sms, uint32_t B, const uint32_t* goff, const uint32_t* poff,
+                                const uint32_t* nrows, uint32_t KB, uint64_t NG, const std::vector<uint32_t>& min_cgrp,
+                                uint2* ids, CbChunks* out) {
+  // first group of every block's stream
+  DevBuf<uint32_t> gbeg;
+  GB_TRY(gbeg.alloc(KB + 1));
+  k_gather_u32<<<grid_for(KB + 1, 128), 128, 0, s>>>(goff, poff, KB + 1, gbeg.p);
+  std::vector<uint32_t> h_gbeg(KB + 1);
+  GB_CUDA(cudaMemcpyAsync(h_gbeg.data(), gbeg.p, (size_t)(KB + 1) * 4, cudaMemcpyDeviceToHost, s));
+  GB_CUDA(cudaStreamSynchronize(s));
+  // ~8 tasks per SM keep the dynamic schedule level; a task is 32 chunks (one per warp) of 512..2048
+  // groups (fewer, longer chunks = fewer segments cut by chunk boundaries); a thin block is cut into
+  // >= 64 chunks (down to one 64-group step each) so that all warps share it — a lone warp runs at
+  // its dependency latency, ~10x below the SM's throughput
+  uint32_t C = (uint32_t)env_u64("GB_PR_CHUNK", 0);
+  const uint32_t T = std::min<uint32_t>(std::max<uint32_t>((uint32_t)env_u64("GB_PR_TASK_CHUNKS", CB_TASK_CHUNKS), 32u), 128u);
+  if (!C) C = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(NG / ((uint64_t)dev_sms * 8 * T), 16384 / T), 65536 / T);
+  C = std::max<uint32_t>(32u, (C + 31) / 32 * 32);
+  out->chunk_groups = C;
+  std::vector<uint32_t> h_cfirst(KB + 1, 0), h_cgrp(KB, C);
+  std::vector<uint2> h_tasks;
+  for (uint32_t j = 0; j < KB; ++j) {
+    const uint32_t G = h_gbeg[j + 1] - h_gbeg[j];
+    h_cgrp[j] = std::min<uint32_t>(C, std::max<uint32_t>(std::min<uint32_t>(64u, C), (G / 64 + 63) / 64 * 64));
+    if (!min_cgrp.empty()) h_cgrp[j] = std::max(h_cgrp[j], min_cgrp[j]);
+    const uint32_t nc = (G + h_cgrp[j] - 1) / h_cgrp[j];
+    h_cfirst[j + 1] = h_cfirst[j] + nc;
+    for (uint32_t c = 0; c < nc; c += T)
+      h_tasks.push_back(make_uint2(h_cfirst[j] + c, (std::min(nc, c + T) - c) | (j << 8)));
+  }
+  out->n_chunks = h_cfirst[KB];
+  out->n_tasks = (uint32_t)h_tasks.size();
+  GB_TRY(upload(s, &out->tasks, h_tasks));
+  DevBuf<uint32_t> cfirst, cgrp, d_nfix;
+  GB_TRY(upload(s, &cfirst, h_cfirst));
+  GB_TRY(upload(s, &cgrp, h_cgrp));
+  GB_TRY(d_nfix.alloc(2));
+  GB_CUDA(cudaMemsetAsync(d_nfix.p, 0, 8, s));
+  GB_TRY(out->chunks.alloc(out->n_chunks, 1));
+  GB_TRY(out->tail_slot.alloc(out->n_chunks));
+  GB_TRY(out->fix_list.alloc(out->n_chunks));
+  GB_TRY(out->side.alloc((size_t)2 * out->n_chunks + 2));
+  GB_CUDA(cudaMemsetAsync(out->side.p, 0, ((size_t)2 * out->n_chunks + 2) * 8, s));
+  GB_CUDA(cudaMemsetAsync(out->chunks.p + out->n_chunks, 0, sizeof(uint4), s));  // sentinel: ends every fixup walk
+  k_cb_chunks<<<grid_for(out->n_chunks, 128), 128, 0, s>>>(goff, poff, nrows, gbeg.p, cfirst.p, cgrp.p, KB,
+                                                           out->n_chunks, out->chunks.p, out->tail_slot.p,
+                                                           out->fix_list.p, d_nfix.p);
+  k_cb_bank_order<<<grid_for((uint64_t)out->n_chunks * 32, CB_BANK_THREADS), CB_BANK_THREADS, 0, s>>>(
+      out->chunks.p, out->n_chunks, B, ids);
+  GB_CUDA(cudaGetLastError());
+  uint32_t h_fix[2] = {0, 0};
+  GB_CUDA(cudaMemcpyAsync(h_fix, d_nfix.p, 8, cudaMemcpyDeviceToHost, s));
+  GB_CUDA(cudaStreamSynchronize(s));
+  out->n_fix = h_fix[0];
+  out->fix_max_row = h_fix[1];
+  return GB_OK;
+}
+
+// Chunks of the column-block kernel; then the sweep's per-pair and per-row buffers.
 gb_status LayoutBuild::layout_chunks() {
   p->grid_cb = 0;
   if (p->NG) {
-    // first group of every block's stream
-    DevBuf<uint32_t> gbeg;
-    GB_TRY(gbeg.alloc(p->KB + 1));
-    k_gather_u32<<<grid_for(p->KB + 1, 128), 128, 0, s>>>(goff.p, p->poff.p, p->KB + 1, gbeg.p);
-    std::vector<uint32_t> h_gbeg(p->KB + 1);
-    GB_CUDA(cudaMemcpyAsync(h_gbeg.data(), gbeg.p, (size_t)(p->KB + 1) * 4, cudaMemcpyDeviceToHost, s));
-    GB_CUDA(cudaStreamSynchronize(s));
-    // ~8 tasks per SM keep the dynamic schedule level; a task is 32 chunks (one per warp) of 512..2048
-    // groups (fewer, longer chunks = fewer segments cut by chunk boundaries); a thin block is cut into
-    // >= 64 chunks (down to one 64-group step each) so that all warps share it — a lone warp runs at
-    // its dependency latency, ~10x below the SM's throughput
-    uint32_t C = (uint32_t)env_u64("GB_PR_CHUNK", 0);
-    const uint32_t T = std::min<uint32_t>(std::max<uint32_t>((uint32_t)env_u64("GB_PR_TASK_CHUNKS", CB_TASK_CHUNKS), 32u), 128u);
-    if (!C) C = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(p->NG / ((uint64_t)dev_sms * 8 * T), 16384 / T), 65536 / T);
-    C = std::max<uint32_t>(32u, (C + 31) / 32 * 32);
-    p->chunk_groups = C;
-    std::vector<uint32_t> h_cfirst(p->KB + 1, 0), h_cgrp(p->KB, C);
-    std::vector<uint2> h_tasks;
-    for (uint32_t j = 0; j < p->KB; ++j) {
-      const uint32_t G = h_gbeg[j + 1] - h_gbeg[j];
-      h_cgrp[j] = std::min<uint32_t>(C, std::max<uint32_t>(std::min<uint32_t>(64u, C), (G / 64 + 63) / 64 * 64));
-      const uint32_t nc = (G + h_cgrp[j] - 1) / h_cgrp[j];
-      h_cfirst[j + 1] = h_cfirst[j] + nc;
-      for (uint32_t c = 0; c < nc; c += T)
-        h_tasks.push_back(make_uint2(h_cfirst[j] + c, (std::min(nc, c + T) - c) | (j << 8)));
-    }
-    p->n_chunks = h_cfirst[p->KB];
-    p->n_tasks = (uint32_t)h_tasks.size();
+    CbChunks c;
+    GB_TRY(cb_chunk_table(s, dev_sms, B, goff.p, p->poff.p, p->nrows.p, p->KB, p->NG, {}, p->cb_ids.p, &c));
+    p->chunk_groups = c.chunk_groups;
+    p->n_chunks = c.n_chunks;
+    p->n_tasks = c.n_tasks;
+    p->n_fix = c.n_fix;
+    p->fix_max_row = c.fix_max_row;
+    p->chunks = std::move(c.chunks);
+    p->tail_slot = std::move(c.tail_slot);
+    p->fix_list = std::move(c.fix_list);
+    p->side = std::move(c.side);
+    p->tasks = std::move(c.tasks);
     p->grid_cb = (unsigned)std::min<uint64_t>(p->n_tasks, (uint64_t)dev_sms);  // one persistent CTA per SM
-    GB_TRY(upload(s, &p->tasks, h_tasks));
-    DevBuf<uint32_t> cfirst, cgrp;
-    GB_TRY(upload(s, &cfirst, h_cfirst));
-    GB_TRY(upload(s, &cgrp, h_cgrp));
-    GB_TRY(p->chunks.alloc(p->n_chunks, 1));
-    GB_TRY(p->tail_slot.alloc(p->n_chunks));
-    GB_TRY(p->fix_list.alloc(p->n_chunks));
-    GB_TRY(p->side.alloc((size_t)2 * p->n_chunks + 2));
-    GB_CUDA(cudaMemsetAsync(p->side.p, 0, ((size_t)2 * p->n_chunks + 2) * 8, s));
-    GB_CUDA(cudaMemsetAsync(p->chunks.p + p->n_chunks, 0, sizeof(uint4), s));  // sentinel: ends every fixup walk
-    uint32_t* d_nfix = reinterpret_cast<uint32_t*>(counters.p + 3);
-    k_cb_chunks<<<grid_for(p->n_chunks, 128), 128, 0, s>>>(goff.p, p->poff.p, p->nrows.p, gbeg.p, cfirst.p, cgrp.p,
-                                                         p->KB, p->n_chunks, p->chunks.p, p->tail_slot.p,
-                                                         p->fix_list.p, d_nfix);
-    k_cb_bank_order<<<grid_for((uint64_t)p->n_chunks * 32, CB_BANK_THREADS), CB_BANK_THREADS, 0, s>>>(
-        p->chunks.p, p->n_chunks, B, p->cb_ids.p);
-    GB_CUDA(cudaGetLastError());
-    uint32_t h_fix[2] = {0, 0};
-    GB_CUDA(cudaMemcpyAsync(h_fix, d_nfix, 8, cudaMemcpyDeviceToHost, s));
-    GB_CUDA(cudaStreamSynchronize(s));
-    p->n_fix = h_fix[0];
-    p->fix_max_row = h_fix[1];
   } else {
     GB_TRY(p->chunks.alloc(1));
     GB_TRY(p->tail_slot.alloc(1));
@@ -945,12 +1263,13 @@ gb_status LayoutBuild::layout_chunks() {
     GB_TRY(p->side.alloc(2));
     GB_TRY(p->tasks.alloc(1));
   }
-  GB_TRY(p->task_ctr.alloc(std::max<unsigned>(p->grid_cb, 1)));
-  GB_CUDA(cudaMemsetAsync(p->task_ctr.p, 0, (size_t)std::max<unsigned>(p->grid_cb, 1) * 4, s));
+  GB_TRY(p->task_ctr.alloc(std::max<unsigned>(p->task_ranges(), 1)));
+  GB_CUDA(cudaMemsetAsync(p->task_ctr.p, 0, (size_t)std::max<unsigned>(p->task_ranges(), 1) * 4, s));
   GB_TRY(p->partial.alloc(std::max<uint64_t>(p->S, 1)));
   GB_CUDA(cudaMemsetAsync(p->partial.p, 0, std::max<uint64_t>(p->S, 1) * 4, s));
-  GB_TRY(p->rem.alloc(std::max<uint32_t>(p->n_cb, 1)));
-  std::vector<uint32_t> h_kb((p->n_cb + 31) / 32);
+  GB_TRY(p->rem.alloc(std::max<uint32_t>(p->vb ? 1u : p->n_cb, 1)));
+  // k_pr_finish completes the rows below n_cb, or every local row when the virtual blocks run
+  std::vector<uint32_t> h_kb(((p->vb ? p->n_loc : p->n_cb) + 31) / 32);
   for (size_t w = 0; w < h_kb.size(); ++w) h_kb[w] = fin_blocks_of(h_nrows.data(), p->KB, (uint32_t)w * 32);
   GB_TRY(upload(s, &p->fin_kb, h_kb));
   return GB_OK;
@@ -1017,6 +1336,7 @@ gb_status layout_end(LayoutBuild* b, const uint32_t* row_off, const uint32_t* ro
     GB_TRY(b->layout_classify());
     GB_TRY(b->layout_sell());
     GB_TRY(b->layout_fill());
+    GB_TRY(b->layout_vblocks());
     GB_TRY(b->layout_chunks());
     return plan_sweep_shape(b->p, b->h_nrows, b->h_poff, b->dev_sms, b->s);
   }();

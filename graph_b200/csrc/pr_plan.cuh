@@ -35,6 +35,10 @@ constexpr uint32_t CB_ILP = 4;               // 32-edge batches in flight per wa
 // chunk flags (bits 24.. of PrChunk.w)
 constexpr uint32_t CB_HEAD_CONT = 1u, CB_TAIL_CONT = 2u, CB_INTERIOR = 4u;
 
+constexpr uint32_t VB_ALIGN = 32;            // virtual blocks start at multiples of 32 slots of V (128-byte lines)
+constexpr uint16_t BIN_PAD = 0xFFFFu;        // pass A: a position that holds no pair (B < 2^16 - 1)
+constexpr uint32_t BIN_CHUNK = 32;           // pass A: 32-position groups per chunk (1024 pairs, one warp)
+
 // ---- the cyclic deal of 32-row slices over the ranks of the 1-D edge-cut ---------------------------
 struct PrDeal {
   uint32_t P = 1, p = 0;  // rank p of P
@@ -52,6 +56,56 @@ static inline uint32_t deal_count(uint32_t R, uint32_t P, uint32_t p) {
   if (rem && (F % P) == p) c += rem;
   return c;
 }
+
+// The chunks and tasks of one column-block id stream (k_pr_cb's unit of work), as the layout build cuts them
+struct CbChunks {
+  uint32_t chunk_groups = 0, n_chunks = 0, n_tasks = 0, n_fix = 0;
+  uint32_t fix_max_row = 0;     // largest row that owns a segment cut by a chunk boundary
+  DevBuf<uint4> chunks;         // [n_chunks + 1] (g_begin, g_end, row_before, j | flags << 24); a zero sentinel
+  DevBuf<uint32_t> tail_slot;   // [n_chunks] staircase slot of the segment cut by the chunk end
+  DevBuf<double> side;          // [2 n_chunks] head / tail parts of segments cut by chunk boundaries
+  DevBuf<uint32_t> fix_list;    // [n_fix] chunks whose tail segment continues in later chunks
+  DevBuf<uint2> tasks;          // [n_tasks] (first chunk, chunk count | block rank << 8), fattest blocks first
+  uint64_t bytes() const { return chunks.bytes() + tail_slot.bytes() + side.bytes() + fix_list.bytes() + tasks.bytes(); }
+};
+
+// Virtual blocks: the edges that no column-block segment takes (COLD edges) on graphs whose source vector does
+// not fit in L2.  The rows are cut into contiguous PARTITIONS of at most B cold edges; each distinct (source,
+// partition) PAIR owns one slot of the value buffer V (partition-major, by source inside a partition: a
+// partition's slots are one virtual block of at most B entries).  Pass A (k_pr_cb<CB_BIN>) loads each source
+// block into shared memory and writes the values of its pairs to V, run by run; pass B (k_pr_cb<CB_VIRT>) walks a
+// column-block stream over the virtual blocks, with V in place of the source vector, and leaves one partial per
+// local row.  k_pr_finish then completes every local row, and k_pr_sell does not run.
+struct PrVBlocks {
+  uint32_t parts = 0;           // partitions = virtual blocks
+  uint64_t pairs = 0, edges = 0;  // (source, partition) pairs and the cold edges they serve
+  uint32_t bin_blocks = 0, n_runs = 0;
+  DevBuf<uint32_t> vbase;       // [parts + 1] first V slot of each virtual block (multiples of VB_ALIGN)
+  DevBuf<float> val;            // V
+  DevBuf<uint32_t> row0;        // [parts + 1] the partitions' first local rows (pass B's staircase offsets)
+  DevBuf<uint32_t> rows;        // [parts] rows per partition (pass B's row counts)
+  // pass A: the pairs in (source block, partition, source) order, each block's share starting at a multiple of
+  // 32 positions (BIN_PAD in between); a RUN is the pairs of one (block, partition), consecutive slots of V
+  DevBuf<uint16_t> bin_ids;     // block-local source id at every position
+  DevBuf<uint32_t> bin_bits;    // per 32 positions: bit i set <=> position 32 g + i starts a run
+  DevBuf<uint32_t> bin_grun;    // per 32 positions: the run of position 32 g
+  DevBuf<uint2> bin_runs;       // [n_runs] (first position of the run, its first V slot)
+  DevBuf<uint2> bin_chunks;     // [32-position groups g0, g1) of one block: a warp's unit of pass A
+  DevBuf<uint32_t> bin_blk;     // [bin_blocks] source block of each of pass A's block ranks
+  DevBuf<uint2> bin_tasks;      // (first chunk, chunk count | block rank << 8)
+  uint32_t bin_n_tasks = 0;
+  // pass B: one segment per local row (a padding group when the row has no cold edge)
+  uint64_t NG = 0;
+  DevBuf<uint2> ids;            // groups of 4 V-local 16-bit slot ids (pad id = B)
+  DevBuf<uint32_t> bits;        // bit g set <=> group g starts a row's segment
+  DevBuf<float> partial;        // [n_loc] the cold sum of every local row
+  CbChunks cut;
+  uint64_t bytes() const {
+    return vbase.bytes() + val.bytes() + row0.bytes() + rows.bytes() + bin_ids.bytes() + bin_bits.bytes() +
+           bin_grun.bytes() + bin_runs.bytes() + bin_chunks.bytes() + bin_blk.bytes() + bin_tasks.bytes() +
+           ids.bytes() + bits.bytes() + partial.bytes() + cut.bytes();
+  }
+};
 
 struct PrPlan {
   uint32_t n = 0;
@@ -90,6 +144,10 @@ struct PrPlan {
   uint32_t num_slices = 0;
   DevBuf<uint4> sell;         // slice-major, then 4-edge group, then lane
   DevBuf<uint2> slice_meta;   // per slice: (first uint4 index, uint4 groups per lane)
+  // virtual blocks (vb: they take the cold edges, the SELL slices above are empty and k_pr_sell does not run)
+  bool vb = false;
+  PrVBlocks v;
+  unsigned grid_bin = 0, grid_vb = 0;  // persistent CTAs of pass A and pass B
   // state (single-GPU path; the shard API brings its own vectors)
   DevBuf<float> x[2];
   DevBuf<float> scores;
@@ -112,8 +170,10 @@ struct PrPlan {
     return new_id.bytes() + outdeg.bytes() + blk.bytes() + nrows.bytes() + poff.bytes() + cb_ids.bytes() +
            cb_bits.bytes() + partial.bytes() + chunks.bytes() + tail_slot.bytes() + side.bytes() +
            fix_list.bytes() + tasks.bytes() + rem.bytes() + fin_kb.bytes() + sell.bytes() + slice_meta.bytes() + x[0].bytes() +
-           x[1].bytes() + scores.bytes() + block_err.bytes() + err_hist.bytes();
+           x[1].bytes() + scores.bytes() + block_err.bytes() + err_hist.bytes() + v.bytes();
   }
+  // task cursors: k_pr_cb's ranges, then pass A's, then pass B's (the finish kernel resets them all)
+  uint32_t task_ranges() const { return grid_cb + grid_bin + grid_vb; }
 };
 
 // blocks in which local row l owns a segment: the first j with nrows[j] <= l (nrows is non-increasing)

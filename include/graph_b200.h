@@ -453,6 +453,10 @@ typedef struct gb_pr_shard_stats {
   uint32_t chunks, tasks, cut_segments, chunk_groups;
   uint32_t launches_per_sweep;
   uint64_t device_bytes;       /* HBM held by this layout */
+  /* virtual blocks (0 when the SELL kernel takes the edges outside the column blocks instead) */
+  uint32_t vblock_parts;       /* row partitions = virtual blocks */
+  uint64_t vblock_pairs;       /* distinct (source, partition) pairs = slots of the value buffer */
+  uint64_t vblock_edges;       /* edges reduced through the virtual blocks */
 } gb_pr_shard_stats;
 
 /* the reference's own partitioner on the ORIGINAL ids: in_degree_partition (graph_ops.rs:431-439,

@@ -241,6 +241,169 @@ def check(plan, got, in_off, in_tgt):
         int(in_off[int(plan["order"][deal_global(l, plan["P"], plan["p"])])]) for l in range(plan["n_loc"]))
 
 
+# ---- virtual blocks (layout_vblocks in pr_layout.cu, PrVBlocks in pr_plan.cuh) ----------------------------------
+VB_ALIGN = 32
+VB_BLK_SHIFT = 43
+BIN_PAD = 0xFFFF
+
+
+def cold_lens(plan, in_off, in_tgt):
+    """cold edges (those outside every segment: the SELL lane lengths) of every local row, vectorised"""
+    n, B, P, p = plan["n"], plan["B"], plan["P"], plan["p"]
+    in_off = np.asarray(in_off, np.int64)
+    row = np.repeat(np.arange(n, dtype=np.int64), np.diff(in_off))
+    g = plan["new_id"][row]
+    sl = g >> 5
+    l = ((sl // P) << 5) | (g & 31)
+    j = plan["hot_of_blk"][plan["new_id"][np.asarray(in_tgt, np.int64)] // B]
+    nrows = plan["nrows"] if len(plan["nrows"]) else np.zeros(1, np.int64)
+    mine = (sl % P == p) & (g < plan["n_active"])
+    seg = (j >= 0) & (l < nrows[np.maximum(j, 0)])
+    return np.bincount(l[mine & ~seg], minlength=plan["n_loc"])[:plan["n_loc"]]
+
+
+def vb_counts(plan, in_off, in_tgt):
+    """gb_pr_shard_stats' vblock_parts / vblock_pairs / vblock_edges (all 0 when the graph keeps SELL), vectorised"""
+    n, B, P, p = plan["n"], plan["B"], plan["P"], plan["p"]
+    lens = cold_lens(plan, in_off, in_tgt)
+    cut = vb_partitions(lens, B)
+    if cut is None:
+        return dict(vblock_parts=0, vblock_pairs=0, vblock_edges=0)
+    in_off = np.asarray(in_off, np.int64)
+    row = np.repeat(np.arange(n, dtype=np.int64), np.diff(in_off))
+    g = plan["new_id"][row]
+    sl = g >> 5
+    l = ((sl // P) << 5) | (g & 31)
+    s = plan["new_id"][np.asarray(in_tgt, np.int64)]
+    j = plan["hot_of_blk"][s // B]
+    nrows = plan["nrows"] if len(plan["nrows"]) else np.zeros(1, np.int64)
+    cold = (sl % P == p) & (g < plan["n_active"]) & ~((j >= 0) & (l < nrows[np.maximum(j, 0)]))
+    part = np.searchsorted(cut[0], l[cold], side="right") - 1
+    pairs = np.unique((part << 32) | s[cold]).size
+    return dict(vblock_parts=len(cut[1]), vblock_pairs=int(pairs), vblock_edges=int(cold.sum()))
+
+
+def vb_partitions(lens, B):
+    """the greedy cut of the local rows into partitions of at most B cold edges: (first rows + n_loc, longest
+    segment of each partition in groups), or None when the graph keeps SELL (no cold edge, or a row with more
+    than B of them)"""
+    row0, mseg, acc, ms = [0], [], 0, 0
+    for l, d in enumerate(int(x) for x in lens):
+        if d > B:
+            return None
+        if acc + d > B and l > row0[-1]:
+            row0.append(l)
+            mseg.append(ms)
+            acc, ms = 0, 0
+        acc += d
+        ms = max(ms, (d + CB_G - 1) // CB_G if d else 1)
+    if not len(lens) or int(np.sum(lens)) == 0:
+        return None
+    mseg.append(ms)
+    row0.append(len(lens))
+    return np.array(row0, np.int64), np.array(mseg, np.int64)
+
+
+def vblocks(plan, built):
+    """layout_vblocks from the SELL lanes of `built` (build()): partitions, the pairs and V's slots, pass B's
+    segments (k_vb_place) and pass A's positions, run bits, first runs and run table (k_bin_place)."""
+    B, n_loc = plan["B"], plan["n_loc"]
+    lens = np.asarray(built["lens"][:n_loc], np.int64)
+    cut = vb_partitions(lens, B)
+    if cut is None:
+        return None
+    row0, mseg = cut
+    parts = len(mseg)
+    rows = np.repeat(np.arange(n_loc, dtype=np.int64), lens)                  # cold edges by row, CSR order
+    src = np.concatenate([built["sell"][l] for l in range(n_loc)]).astype(np.int64)
+    part = np.searchsorted(row0, rows, side="right") - 1
+    key = (part << 32) | src
+    order = np.argsort(key, kind="stable")                                    # the radix sort of (partition, source)
+    sk = key[order]
+    start = np.r_[True, sk[1:] != sk[:-1]]
+    rank = np.cumsum(start) - 1                                               # pair of every sorted edge
+    NP = int(rank[-1]) + 1
+    pfirst = np.array([rank[i] if i < len(sk) else NP for i in np.searchsorted(sk >> 32, np.arange(parts + 1))])
+    cnt = np.diff(pfirst)
+    vbase = np.concatenate([[0], np.cumsum((cnt + VB_ALIGN - 1) // VB_ALIGN * VB_ALIGN)])
+    # pass B: one segment per local row, V-local slot ids in CSR order, pad id B
+    groups = np.where(lens > 0, (lens + CB_G - 1) // CB_G, 1)
+    goffv = np.concatenate([[0], np.cumsum(groups)])
+    coff = np.concatenate([[0], np.cumsum(lens)])
+    ids = np.full(int(goffv[-1]) * CB_G, B, np.int64)
+    e = order
+    ids[goffv[rows[e]] * CB_G + (e - coff[rows[e]])] = rank - pfirst[sk >> 32]
+    # pass A: the pairs by (source block, partition, source), each block's share at a multiple of 32 positions
+    psrc, ppart = sk[start] & 0xFFFFFFFF, sk[start] >> 32
+    pslot = vbase[ppart] + np.arange(NP) - pfirst[ppart]
+    akey = ((psrc // B) << VB_BLK_SHIFT) | (ppart << 16) | (psrc % B)
+    ao = np.argsort(akey, kind="stable")
+    akey, aslot = akey[ao], pslot[ao]
+    blk = akey >> VB_BLK_SHIFT
+    bcnt = np.bincount(blk, minlength=plan["nblk"])
+    bpos = np.concatenate([[0], np.cumsum((bcnt + 31) // 32 * 32)])
+    bfirst = np.concatenate([[0], np.cumsum(bcnt)])
+    pos = bpos[blk] + np.arange(NP) - bfirst[blk]
+    npos = int(bpos[-1])
+    bin_ids = np.full(npos, BIN_PAD, np.int64)
+    bin_ids[pos] = akey & 0xFFFF
+    rstart = np.r_[True, (akey[1:] >> 16) != (akey[:-1] >> 16)]
+    run = np.cumsum(rstart) - 1
+    bin_bits = np.zeros(npos // 32, np.int64)
+    np.bitwise_or.at(bin_bits, pos[rstart] // 32, 1 << (pos[rstart] % 32))
+    bin_grun = np.zeros(npos // 32, np.int64)
+    first = pos % 32 == 0
+    bin_grun[pos[first] // 32] = run[first]
+    bin_runs = np.stack([pos[rstart], aslot[rstart]], axis=1)
+    pos_blk = np.repeat(np.arange(plan["nblk"]), np.diff(bpos))              # source block of every position
+    return dict(parts=parts, row0=row0, mseg=mseg, vbase=vbase, pairs=NP, edges=int(lens.sum()), lens=lens,
+                goffv=goffv, ids=ids, bin_ids=bin_ids, bin_bits=bin_bits, bin_grun=bin_grun, bin_runs=bin_runs,
+                pos_blk=pos_blk)
+
+
+def vb_pass_a(plan, vb):
+    """pass A (k_pr_cb<CB_BIN> / bin_chunk): the source of every slot of V it writes, and how often it writes it"""
+    B = plan["B"]
+    V = np.full(int(vb["vbase"][-1]), -1, np.int64)
+    writes = np.zeros(len(V), np.int64)
+    for i, sid in enumerate(vb["bin_ids"]):
+        if sid == BIN_PAD:
+            continue
+        g, lane = i // 32, i % 32
+        after = ((2 << lane) - 2) & 0xFFFFFFFF
+        r = int(vb["bin_grun"][g]) + bin(int(vb["bin_bits"][g]) & after).count("1")
+        p0, s0 = vb["bin_runs"][r]
+        slot = int(s0) + i - int(p0)
+        V[slot] = int(vb["pos_blk"][i]) * B + int(sid)
+        writes[slot] += 1
+    return V, writes
+
+
+def check_vblocks(plan, vb, built):
+    """the contract of the two passes: pass A writes every slot of V exactly once (and nothing between the
+    virtual blocks), every cold edge appears exactly once in pass B, and every pass B id resolves to the slot
+    of its edge's source; no virtual block holds more than B slots"""
+    B = plan["B"]
+    V, writes = vb_pass_a(plan, vb)
+    for k in range(vb["parts"]):
+        lo, hi = int(vb["vbase"][k]), int(vb["vbase"][k + 1])
+        used = writes[lo:hi] > 0
+        assert (writes[lo:hi][used] == 1).all(), "pass A writes a slot once"
+        cnt = int(used.sum())
+        assert used[:cnt].all() and cnt <= B, "a virtual block's slots are a prefix of at most B"
+    for l in range(plan["n_loc"]):
+        k = int(np.searchsorted(vb["row0"], l, side="right") - 1)
+        g0, g1 = int(vb["goffv"][l]), int(vb["goffv"][l + 1])
+        d = int(vb["lens"][l])
+        assert g1 - g0 == max(1, (d + CB_G - 1) // CB_G), "one segment per row, ceil(cold / 4) groups, at least one"
+        seg = vb["ids"][g0 * CB_G:g1 * CB_G]
+        assert (seg[d:] == B).all(), "padding = the zero slot"
+        assert (seg[:d] < B).all()
+        assert V[int(vb["vbase"][k]) + seg[:d]].tolist() == built["sell"][l].tolist(), \
+            "pass B's ids resolve to the sources of the row's cold edges, in CSR order"
+    assert vb["edges"] == sum(len(built["sell"][l]) for l in range(plan["n_loc"]))
+
+
 def random_graph(rng, n, m, skew=1.5):
     w = (np.arange(1, n + 1) ** -skew)
     w /= w.sum()
@@ -265,6 +428,9 @@ def main():
                 b = build(plan, in_off, in_tgt, plan["order"])                # resident path: internal order
                 check(plan, a, in_off, in_tgt)
                 assert (a["ids"] == b["ids"]).all() and (a["goff"] == b["goff"]).all()
+                va, vr = vblocks(plan, a), vblocks(plan, b)
+                check_vblocks(plan, va, a)
+                assert all(np.array_equal(va[k], vr[k]) for k in va), "streamed and resident virtual blocks agree"
     print("layout model ok")
 
 
