@@ -90,6 +90,27 @@ __device__ __forceinline__ double warp_sum(double v) {
 }
 
 // ---- sweep kernels (JACOBI) ------------------------------------------------------------------
+// What k_pr_cb's task scheduler reads: the block of each rank, the tasks and this pass's task cursors
+struct CbSched {
+  const uint32_t* blk;  // CbStream::blk (pass A: PrVBlocks::bin_blk)
+  const uint2* tasks;
+  uint32_t n_tasks;
+  uint32_t* task_ctr;
+};
+// What the walker, the fixup of cut segments and k_pr_finish read of a stream (CbStream)
+struct CbWalk {
+  const uint32_t* nrows;
+  const uint32_t* poff;
+  const uint2* ids;
+  const uint32_t* bits;
+  float* partial;
+  const uint4* chunks;
+  uint32_t n_chunks;
+  const uint32_t* tail_slot;
+  double* side;
+  const uint32_t* fix_list;
+  uint32_t n_fix;
+};
 struct PrArgs {
   const uint32_t* outdeg;
   const float* x_cur;
@@ -106,25 +127,13 @@ struct PrArgs {
   uint32_t n_fin;       // rows [0, n_fin) are completed by k_pr_finish (rem[] + partials); rows [n_fin, n_cb) own
                         // segments in at most SELL_FEW blocks and are completed by their k_pr_sell lane
   uint32_t few_kb, few_nrows[SELL_FEW], few_poff[SELL_FEW];  // the first blocks' row prefixes / partial offsets
-  uint32_t fix_in_sell; // k_pr_sell adds the parts of cut segments first (sequential mode: no k_pr_fixup launch)
+  uint32_t fix_in_sell; // k_pr_sell adds the parts of cut segments first (PrPlan::fix_at == PrFix::SELL)
   const uint32_t* fin_kb;  // [ceil(n_cb / 32)] blocks in which the first row of each 32-row group owns a segment
-  // column blocks
-  uint32_t B, KB;
-  const uint32_t* blk;
-  const uint32_t* nrows;
-  const uint32_t* poff;
-  const uint2* cb_ids;
-  const uint32_t* cb_bits;
-  float* partial;
-  const uint4* chunks;
-  uint32_t n_chunks;
-  const uint32_t* tail_slot;
-  double* side;
-  const uint32_t* fix_list;
-  uint32_t n_fix;
-  const uint2* tasks;
-  uint32_t n_tasks, n_task_ranges;
-  uint32_t* task_ctr;
+  // column blocks: the stream a k_pr_cb pass walks, or the hot blocks' (k_pr_fixup, k_pr_sell, k_pr_finish)
+  uint32_t B;
+  CbSched sched;
+  CbWalk walk;
+  uint32_t n_task_ranges;  // all passes' task cursors, from sched.task_ctr of the hot blocks
   float* rem;
   // pass A of the virtual blocks (k_pr_cb<CB_BIN>)
   float* vals;
@@ -206,12 +215,12 @@ __device__ __forceinline__ void cb_emit(const PrArgs& a, uint32_t c, bool is_end
   if (!is_end) return;
   if (SPECIAL) {
     if (q == last && run_continues && !last_step) return;  // carried into the next step
-    if (in_head && cum == 0) a.side[2 * (size_t)c] = tot;                        // tail part of a cut segment
-    else if (q == last && last_step && tail_cont) a.side[2 * (size_t)c + 1] = tot;  // head part of one
-    else a.partial[slot0 + cum] = (float)tot;
+    if (in_head && cum == 0) a.walk.side[2 * (size_t)c] = tot;                        // tail part of a cut segment
+    else if (q == last && last_step && tail_cont) a.walk.side[2 * (size_t)c + 1] = tot;  // head part of one
+    else a.walk.partial[slot0 + cum] = (float)tot;
   } else {
     if (q == last && run_continues) return;  // carried into the next step
-    a.partial[slot0 + cum] = (float)tot;
+    a.walk.partial[slot0 + cum] = (float)tot;
   }
 }
 // A lane's k-th load of a step.  With one load per lane (G = 2) the ids are streamed past L1, so that
@@ -238,12 +247,12 @@ __device__ __forceinline__ void cb_walk(const PrArgs& a, const float* xs, uint32
   const uint32_t g0 = ch.x, g1 = ch.y;
   const uint32_t j = ch.w & 0xFFFFFFu, fl = ch.w >> 24;
   const bool head_cont = SPECIAL && (fl & CB_HEAD_CONT), tail_cont = SPECIAL && (fl & CB_TAIL_CONT);
-  uint32_t slot0 = a.poff[j] + ch.z;  // staircase slot of the row "before" the first segment start
+  uint32_t slot0 = a.walk.poff[j] + ch.z;  // staircase slot of the row "before" the first segment start
   bool in_head = head_cont;
   double carry = 0.0;
   const uint32_t le_mask = 0xFFFFFFFFu >> (31u - lane);
   const uint32_t q0 = G * lane;  // the lane's first position in the step
-  const uint4* ids16 = reinterpret_cast<const uint4*>(a.cb_ids) + NL * lane;  // pairs of groups
+  const uint4* ids16 = reinterpret_cast<const uint4*>(a.walk.ids) + NL * lane;  // pairs of groups
   const uint4 padv = make_uint4(pad2, pad2, pad2, pad2);
   const auto load = [&](uint4(&d)[NL], uint32_t gs) {  // the lane's pairs of the step at gs that start below g1
 #pragma unroll
@@ -262,7 +271,7 @@ __device__ __forceinline__ void cb_walk(const PrArgs& a, const float* xs, uint32
     const uint32_t wi = gs >> 5, sh = gs & 31u;
     uint32_t w[G + 1];
 #pragma unroll
-    for (uint32_t k = 0; k <= G; ++k) w[k] = __ldg(a.cb_bits + wi + k);
+    for (uint32_t k = 0; k <= G; ++k) w[k] = __ldg(a.walk.bits + wi + k);
     const uint32_t nvalid = min(STEP, g1 - gs);
     unsigned long long W[NL];  // segment starts at the step's positions 64 k .. 64 k + 63, inside [g0, g1)
 #pragma unroll
@@ -331,7 +340,7 @@ __device__ __forceinline__ void cb_walk(const PrArgs& a, const float* xs, uint32
   }
 }
 __device__ __forceinline__ void cb_chunk(const PrArgs& a, const float* xs, uint32_t c, uint32_t lane, uint32_t pad2) {
-  const uint4 ch = a.chunks[c];
+  const uint4 ch = a.walk.chunks[c];
   if (ch.x >= ch.y) return;
   const bool special = (ch.w >> 24) & (CB_HEAD_CONT | CB_TAIL_CONT);
   if (cb_step_groups(ch.x, ch.y) == 4) {
@@ -364,18 +373,18 @@ __device__ __forceinline__ void bin_chunk(const PrArgs& a, const float* xs, uint
 // xor tree per batch of 32).  Tiny; runs after k_pr_cb (as k_pr_fixup, or as the prologue of k_pr_sell or of
 // pass A).
 __device__ __forceinline__ void cb_fix_segment(const PrArgs& a, uint32_t c0, uint32_t lane) {
-  double t = a.side[2 * (size_t)c0 + 1];
+  double t = a.walk.side[2 * (size_t)c0 + 1];
   for (uint32_t k0 = c0 + 1;; k0 += 32) {
     const uint32_t k = k0 + lane;
     // the walk ends at the first chunk that is not entirely inside the segment (sentinel chunk after the last)
-    const uint32_t fl = a.chunks[min(k, a.n_chunks)].w >> 24;
-    const bool inside = k < a.n_chunks && (fl & CB_INTERIOR) && (fl & CB_TAIL_CONT);
+    const uint32_t fl = a.walk.chunks[min(k, a.walk.n_chunks)].w >> 24;
+    const bool inside = k < a.walk.n_chunks && (fl & CB_INTERIOR) && (fl & CB_TAIL_CONT);
     const uint32_t stop = __ballot_sync(0xFFFFFFFFu, !inside);
     const uint32_t upto = stop ? (uint32_t)__ffs(stop) - 1 : 31u;  // last lane that contributes
-    t += warp_sum(lane <= upto ? a.side[2 * (size_t)k] : 0.0);
+    t += warp_sum(lane <= upto ? a.walk.side[2 * (size_t)k] : 0.0);
     if (stop) break;
   }
-  if (lane == 0) a.partial[a.tail_slot[c0]] = (float)t;
+  if (lane == 0) a.walk.partial[a.walk.tail_slot[c0]] = (float)t;
 }
 
 // ---- TMA bulk copy of a source block into shared memory (cp.async.bulk + mbarrier) -----------------
@@ -428,9 +437,9 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
   __shared__ __align__(8) unsigned long long s_mbar;
   if (a.ctrl[0] != 0) return;  // tolerance already met by an earlier sweep of this batch
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (KIND == CB_BIN)  // k_pr_cb<CB_MAIN> has finished: no k_pr_fixup launch on this path
-    for (uint32_t i = blockIdx.x * PR_WARPS + warp; i < a.n_fix; i += gridDim.x * PR_WARPS)
-      cb_fix_segment(a, a.fix_list[i], lane);
+  if (KIND == CB_BIN)  // k_pr_cb<CB_MAIN> has finished; walk = the hot blocks' stream (PrFix::PASS_A)
+    for (uint32_t i = blockIdx.x * PR_WARPS + warp; i < a.walk.n_fix; i += gridDim.x * PR_WARPS)
+      cb_fix_segment(a, a.walk.fix_list[i], lane);
   const uint32_t B = a.B;
   const uint32_t pad2 = B | (B << 16);
   const uint32_t R = gridDim.x;  // ranges = CTAs
@@ -447,10 +456,11 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
     if (warp == 0) {
       uint32_t t = CB_NONE;
       for (;;) {
-        const uint32_t lo = (uint32_t)((uint64_t)a.n_tasks * r / R), hi = (uint32_t)((uint64_t)a.n_tasks * (r + 1) / R);
+        const uint32_t lo = (uint32_t)((uint64_t)a.sched.n_tasks * r / R),
+                       hi = (uint32_t)((uint64_t)a.sched.n_tasks * (r + 1) / R);
         uint32_t k = CB_NONE;
         if (lane == 0) {
-          k = lo + atomicAdd(a.task_ctr + r, 1u);
+          k = lo + atomicAdd(a.sched.task_ctr + r, 1u);
           if (k >= hi) k = CB_NONE;
         }
         t = __shfl_sync(0xFFFFFFFFu, k, 0);
@@ -462,8 +472,9 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
           if (q >= R) q -= R;
           bool ok = false;
           if (base + lane < R) {
-            const uint32_t qlo = (uint32_t)((uint64_t)a.n_tasks * q / R), qhi = (uint32_t)((uint64_t)a.n_tasks * (q + 1) / R);
-            ok = *((volatile uint32_t*)(a.task_ctr + q)) < qhi - qlo;
+            const uint32_t qlo = (uint32_t)((uint64_t)a.sched.n_tasks * q / R),
+                           qhi = (uint32_t)((uint64_t)a.sched.n_tasks * (q + 1) / R);
+            ok = *((volatile uint32_t*)(a.sched.task_ctr + q)) < qhi - qlo;
           }
           const uint32_t m = __ballot_sync(0xFFFFFFFFu, ok);
           if (m) found = __shfl_sync(0xFFFFFFFFu, q, __ffs(m) - 1);
@@ -478,11 +489,12 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
     if (threadIdx.x == 0) s_next = PR_THREADS / 32;  // every warp is past its last claim of the previous task
     __syncthreads();
     if (t == CB_NONE) break;
-    const uint2 task = a.tasks[t];  // (first chunk, chunk count | block rank << 8)
+    const uint2 task = a.sched.tasks[t];  // (first chunk, chunk count | block rank << 8)
     const uint32_t j = task.y >> 8;
     if (j != cur_j) {
-      const uint64_t x0 = KIND == CB_VIRT ? (uint64_t)a.blk[j] : (uint64_t)a.blk[j] * B;
-      const uint32_t cnt = KIND == CB_VIRT ? a.blk[j + 1] - a.blk[j] : (uint32_t)min((uint64_t)B, (uint64_t)a.n - x0);
+      const uint64_t x0 = KIND == CB_VIRT ? (uint64_t)a.sched.blk[j] : (uint64_t)a.sched.blk[j] * B;
+      const uint32_t cnt = KIND == CB_VIRT ? a.sched.blk[j + 1] - a.sched.blk[j]
+                                           : (uint32_t)min((uint64_t)B, (uint64_t)a.n - x0);
       if (bulk_ok) {
         const uint32_t bulk = cnt & ~3u;
         if (threadIdx.x == 0) {
@@ -516,7 +528,7 @@ __global__ void k_pr_fixup(const PrArgs a) {
   if (a.ctrl[0] != 0) return;
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
-  for (uint32_t i = gw; i < a.n_fix; i += nw) cb_fix_segment(a, a.fix_list[i], lane);
+  for (uint32_t i = gw; i < a.walk.n_fix; i += nw) cb_fix_segment(a, a.walk.fix_list[i], lane);
 }
 
 // ---- SELL-32 sweep: one lane per row ------------------------------------------------------------
@@ -535,7 +547,7 @@ __global__ void __launch_bounds__(PR_SELL_THREADS, 2) k_pr_sell(const PrArgs a) 
   if (a.fix_in_sell) {
     // segments cut by chunk boundaries (hub rows only: they are completed by k_pr_finish, after this kernel)
     const uint32_t gw0 = blockIdx.x * NW + warp, nw0 = gridDim.x * NW;
-    for (uint32_t i = gw0; i < a.n_fix; i += nw0) cb_fix_segment(a, a.fix_list[i], lane);
+    for (uint32_t i = gw0; i < a.walk.n_fix; i += nw0) cb_fix_segment(a, a.walk.fix_list[i], lane);
   }
   const float* __restrict__ x = a.x_cur;
   double err = 0.0;
@@ -591,7 +603,7 @@ __global__ void __launch_bounds__(PR_SELL_THREADS, 2) k_pr_sell(const PrArgs a) 
 #pragma unroll
     for (uint32_t j = 0; j < SELL_FEW; ++j) {
       part[j] = 0.0f;
-      if (l >= a.n_fin && j < a.few_kb && l < a.few_nrows[j]) part[j] = a.partial[(size_t)a.few_poff[j] + l];
+      if (l >= a.n_fin && j < a.few_kb && l < a.few_nrows[j]) part[j] = a.walk.partial[(size_t)a.few_poff[j] + l];
     }
     float acc = 0.0f;
     for (uint32_t q = 0; q < w4; q += 2) {
@@ -648,7 +660,7 @@ __global__ void __launch_bounds__(PR_FIN_THREADS) k_pr_finish(const PrArgs a) {
   double err = 0.0;
   const uint32_t P = a.deal.P, pp = a.deal.p;
   if (blockIdx.x == 0)  // next sweep's column-block task cursors
-    for (uint32_t i = threadIdx.x; i < a.n_task_ranges; i += PR_FIN_THREADS) a.task_ctr[i] = 0;
+    for (uint32_t i = threadIdx.x; i < a.n_task_ranges; i += PR_FIN_THREADS) a.sched.task_ctr[i] = 0;
   // hub rows (segments in more than FIN_CTA_BLOCKS blocks): one CTA per 32-row group — lane = row,
   // warp w adds blocks w, w + 8, ... (independent coalesced loads), warp 0 adds the 8 sums in order
   __shared__ double part[FIN_WARPS][32];
@@ -661,7 +673,7 @@ __global__ void __launch_bounds__(PR_FIN_THREADS) k_pr_finish(const PrArgs a) {
     double s = 0.0;
 #pragma unroll 8
     for (uint32_t j = warp; j < kb; j += FIN_WARPS)
-      if (l < __ldg(a.nrows + j)) s += (double)a.partial[(size_t)__ldg(a.poff + j) + l];
+      if (l < __ldg(a.walk.nrows + j)) s += (double)a.walk.partial[(size_t)__ldg(a.walk.poff + j) + l];
     part[warp][lane] = s;
     __syncthreads();
     if (warp == 0 && l < a.n_fin) {
@@ -699,8 +711,8 @@ __global__ void __launch_bounds__(PR_FIN_THREADS) k_pr_finish(const PrArgs a) {
     }
 #pragma unroll(FIN_U == 2 ? 16 : 4)
     for (uint32_t j = 0; j < kb; ++j) {
-      const uint32_t nr = __ldg(a.nrows + j);
-      const float* __restrict__ pj = a.partial + __ldg(a.poff + j);
+      const uint32_t nr = __ldg(a.walk.nrows + j);
+      const float* __restrict__ pj = a.walk.partial + __ldg(a.walk.poff + j);
 #pragma unroll
       for (uint32_t u = 0; u < FIN_U; ++u)
         if (l[u] < nr) s[u] += (double)pj[l[u]];
@@ -870,13 +882,14 @@ gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, cons
   // rows with segments in more than SELL_FEW blocks are a prefix (nrows[] is non-increasing): k_pr_finish
   // completes them; all others are completed by their k_pr_sell lane (k_pr_cb is done by then).  With virtual
   // blocks k_pr_finish completes every local row.
-  p->n_fin = p->KB > SELL_FEW ? std::min<uint32_t>(p->n_cb, (h_nrows[SELL_FEW] + 31) / 32 * 32) : 0;
+  p->n_fin = p->hot.KB > SELL_FEW ? std::min<uint32_t>(p->n_cb, (h_nrows[SELL_FEW] + 31) / 32 * 32) : 0;
   if (p->vb) p->n_fin = p->n_loc;
-  for (uint32_t j = 0; j < SELL_FEW && j < p->KB; ++j) {
+  for (uint32_t j = 0; j < SELL_FEW && j < p->hot.KB; ++j) {
     p->few_nrows[j] = h_nrows[j];
     p->few_poff[j] = h_poff[j];
   }
-  p->n_fin_warp = p->KB > FIN_CTA_BLOCKS ? std::min<uint32_t>(p->n_fin, (h_nrows[FIN_CTA_BLOCKS] + 31) / 32 * 32) : 0;
+  p->n_fin_warp =
+      p->hot.KB > FIN_CTA_BLOCKS ? std::min<uint32_t>(p->n_fin, (h_nrows[FIN_CTA_BLOCKS] + 31) / 32 * 32) : 0;
   const uint64_t fin_warps2 = (uint64_t)p->n_fin_warp / 32 * (PR_FIN_THREADS / 32) + (p->n_fin - p->n_fin_warp + 63) / 64;
   const uint64_t fin_warps4 = (uint64_t)p->n_fin_warp / 32 * (PR_FIN_THREADS / 32) + (p->n_fin - p->n_fin_warp + 127) / 128;
   p->fin_u = (fin_warps2 + PR_FIN_THREADS / 32 - 1) / (PR_FIN_THREADS / 32) <= (uint64_t)dev_sms * 8 ? 2 : 4;
@@ -898,10 +911,15 @@ gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, cons
   // the tail rows).
   p->fin_hub_ctas = 0;
   const uint32_t split = (uint32_t)env_u64("GB_PR_FIN_SPLIT", 0);
-  const bool split_pays = want_fin <= (uint64_t)dev_sms * 8 && p->KB > 4 * FIN_CTA_BLOCKS;
+  const bool split_pays = want_fin <= (uint64_t)dev_sms * 8 && p->hot.KB > 4 * FIN_CTA_BLOCKS;
   if (p->n_fin_warp && p->n_fin > p->n_fin_warp && p->grid_fin > p->n_fin_warp / 32 &&
       (split == 1 || (split == 0 && split_pays)))
     p->fin_hub_ctas = p->n_fin_warp / 32;
+  // the kernel that adds the parts of cut segments (PrFix): k_pr_sell only when it completes none of their rows
+  if (!p->hot.n_fix) p->fix_at = PrFix::NONE;
+  else if (p->vb) p->fix_at = PrFix::PASS_A;
+  else if (p->grid_sell && p->hot.fix_max_row < p->n_fin) p->fix_at = PrFix::SELL;
+  else p->fix_at = PrFix::FIXUP;
   const size_t nerr = (size_t)p->grid_sell + p->grid_fin;
   GB_TRY(p->block_err.alloc(nerr));
   GB_CUDA(cudaMemsetAsync(p->block_err.p, 0, nerr * sizeof(double), s));
@@ -912,13 +930,16 @@ gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, cons
   return GB_OK;
 }
 
-// The parts of segments cut by chunk boundaries are added by the first warps of k_pr_sell when every such
-// row is completed later, by k_pr_finish (rows below n_fin).  A row that its k_pr_sell lane completes itself
-// (few hot blocks: small graphs) needs the sum BEFORE that kernel: k_pr_fixup runs in between.
-static bool fix_in_sell(const PrPlan* p) {
-  return p->n_fix && p->grid_sell && p->fix_max_row < p->n_fin;
+// a stream's scheduler and walker groups of PrArgs
+static CbSched sched_of(const CbStream& st, uint32_t* task_ctr) {
+  return CbSched{st.blk.p, st.tasks.p, st.n_tasks, task_ctr};
 }
-static bool fixup_launched(const PrPlan* p) { return p->grid_cb && p->n_fix && !fix_in_sell(p) && !p->vb; }
+static CbWalk walk_of(const CbStream& st) {
+  return CbWalk{st.nrows.p, st.poff.p, st.ids.p, st.bits.p, st.partial.p, st.chunks.p, st.n_chunks,
+                st.tail_slot.p, st.side.p, st.fix_list.p, st.n_fix};
+}
+// the arguments of k_pr_cb<CB_MAIN>, k_pr_fixup, k_pr_sell and k_pr_finish: the hot blocks' stream, for every
+// sweep (the per-sweep fields are set by enqueue_sweep)
 static PrArgs make_args(const PrPlan* p, float base, float damping, double tolerance) {
   PrArgs a{};
   a.outdeg = p->outdeg.p;
@@ -929,31 +950,17 @@ static PrArgs make_args(const PrPlan* p, float base, float damping, double toler
   a.n_fin_warp = p->n_fin_warp;
   a.fin_hub_ctas = p->fin_hub_ctas;
   a.n_fin = p->n_fin;
-  a.few_kb = std::min<uint32_t>(p->KB, SELL_FEW);
+  a.few_kb = std::min<uint32_t>(p->hot.KB, SELL_FEW);
   for (uint32_t j = 0; j < SELL_FEW; ++j) {
     a.few_nrows[j] = p->few_nrows[j];
     a.few_poff[j] = p->few_poff[j];
   }
-  a.fix_in_sell = fix_in_sell(p) ? 1u : 0u;
+  a.fix_in_sell = p->fix_at == PrFix::SELL ? 1u : 0u;
   a.B = p->B;
-  a.KB = p->KB;
-  a.blk = p->blk.p;
-  a.nrows = p->nrows.p;
-  a.poff = p->poff.p;
-  a.cb_ids = p->cb_ids.p;
-  a.cb_bits = p->cb_bits.p;
-  a.partial = p->partial.p;
-  a.chunks = p->chunks.p;
-  a.n_chunks = p->n_chunks;
-  a.tail_slot = p->tail_slot.p;
-  a.side = p->side.p;
-  a.fix_list = p->fix_list.p;
-  a.n_fix = p->n_fix;
-  a.tasks = p->tasks.p;
-  a.n_tasks = p->n_tasks;
-  a.task_ctr = p->task_ctr.p;
+  a.sched = sched_of(p->hot, p->task_ctr.p);
+  a.walk = walk_of(p->hot);
   a.n_task_ranges = p->task_ranges();
-  a.rem = p->vb ? p->v.partial.p : p->rem.p;
+  a.rem = p->vb ? p->v.virt.partial.p : p->rem.p;
   a.fin_kb = p->fin_kb.p;
   a.sell = p->sell.p;
   a.slice_meta = p->slice_meta.p;
@@ -969,44 +976,29 @@ static PrArgs make_args(const PrPlan* p, float base, float damping, double toler
   a.mc_next = nullptr;
   return a;
 }
-// pass A of the virtual blocks: a's source blocks and cut segments, the pass's own tasks and chunks
-static PrArgs bin_args(const PrPlan* p, const PrArgs& a) {
-  PrArgs b = a;
-  b.blk = p->v.bin_blk.p;
-  b.tasks = p->v.bin_tasks.p;
-  b.n_tasks = p->v.bin_n_tasks;
-  b.task_ctr = p->task_ctr.p + p->grid_cb;
-  b.vals = p->v.val.p;
-  b.bin_ids = p->v.bin_ids.p;
-  b.bin_bits = p->v.bin_bits.p;
-  b.bin_grun = p->v.bin_grun.p;
-  b.bin_runs = p->v.bin_runs.p;
-  b.bin_chunks = p->v.bin_chunks.p;
-  return b;
+// pass A of the virtual blocks: its own tasks over x_cur's blocks, and the hot blocks' walker group, whose cut
+// segments its first warps add (PrFix::PASS_A)
+static PrArgs pass_a_args(const PrPlan* p, PrArgs a) {
+  const PrVBlocks& v = p->v;
+  a.sched = CbSched{v.bin_blk.p, v.bin_tasks.p, v.bin_n_tasks, p->task_ctr.p + p->grid_cb};
+  a.vals = v.val.p;
+  a.bin_ids = v.bin_ids.p;
+  a.bin_bits = v.bin_bits.p;
+  a.bin_grun = v.bin_grun.p;
+  a.bin_runs = v.bin_runs.p;
+  a.bin_chunks = v.bin_chunks.p;
+  return a;
 }
-// pass B: the column-block stream of the virtual blocks, over V; partial = the rows' cold sums
-static PrArgs virt_args(const PrPlan* p, const PrArgs& a) {
-  PrArgs b = a;
-  b.x_cur = p->v.val.p;
-  b.blk = p->v.vbase.p;
-  b.poff = p->v.row0.p;
-  b.cb_ids = p->v.ids.p;
-  b.cb_bits = p->v.bits.p;
-  b.partial = p->v.partial.p;
-  b.chunks = p->v.cut.chunks.p;
-  b.n_chunks = p->v.cut.n_chunks;
-  b.tail_slot = p->v.cut.tail_slot.p;
-  b.side = p->v.cut.side.p;
-  b.fix_list = p->v.cut.fix_list.p;
-  b.n_fix = p->v.cut.n_fix;
-  b.tasks = p->v.cut.tasks.p;
-  b.n_tasks = p->v.cut.n_tasks;
-  b.task_ctr = p->task_ctr.p + p->grid_cb + p->grid_bin;
-  return b;
+// pass B: the virtual blocks' stream, over V; its partials are the rows' cold sums (k_pr_finish's rem)
+static PrArgs pass_b_args(const PrPlan* p, PrArgs a) {
+  a.x_cur = p->v.val.p;
+  a.sched = sched_of(p->v.virt, p->task_ctr.p + p->grid_cb + p->grid_bin);
+  a.walk = walk_of(p->v.virt);
+  return a;
 }
 
-// one sweep = column blocks (+ fixup of cut segments), SELL rows, then finish; *launches is advanced by
-// the kernels launched
+// one sweep = column blocks (+ fixup of cut segments), SELL rows or the two virtual-block passes, then finish;
+// *launches is advanced by the kernels launched
 template <bool PEERS>
 static gb_status launch_sweep(const PrPlan* p, const PrArgs& a, cudaStream_t s, uint64_t* launches) {
   cudaEvent_t* ev = nullptr;
@@ -1022,12 +1014,12 @@ static gb_status launch_sweep(const PrPlan* p, const PrArgs& a, cudaStream_t s, 
     *launches += 1;
   }
   if (ev) GB_CUDA(cudaEventRecord(ev[1], s));
-  if (fixup_launched(p)) {
-    k_pr_fixup<<<grid_for((uint64_t)p->n_fix * 32, 128, 296), 128, 0, s>>>(a);
+  if (p->fix_at == PrFix::FIXUP) {
+    k_pr_fixup<<<grid_for((uint64_t)p->hot.n_fix * 32, 128, 296), 128, 0, s>>>(a);
     *launches += 1;
   }
   if (p->vb) {
-    k_pr_cb<CB_BIN><<<p->grid_bin, PR_THREADS, p->smem_cb, s>>>(bin_args(p, a));
+    k_pr_cb<CB_BIN><<<p->grid_bin, PR_THREADS, p->smem_cb, s>>>(pass_a_args(p, a));
     *launches += 1;
   }
   if (ev) GB_CUDA(cudaEventRecord(ev[2], s));
@@ -1036,7 +1028,7 @@ static gb_status launch_sweep(const PrPlan* p, const PrArgs& a, cudaStream_t s, 
     *launches += 1;
   }
   if (p->vb) {
-    k_pr_cb<CB_VIRT><<<p->grid_vb, PR_THREADS, p->smem_cb, s>>>(virt_args(p, a));
+    k_pr_cb<CB_VIRT><<<p->grid_vb, PR_THREADS, p->smem_cb, s>>>(pass_b_args(p, a));
     *launches += 1;
   }
   if (ev) GB_CUDA(cudaEventRecord(ev[3], s));
@@ -1064,13 +1056,26 @@ static gb_status pr_reset(const PrPlan* p, PrStart v, float* x0, float* x1, floa
 static double first_sweep_err(const PrPlan* p, uint64_t sweep_no, PrStart v) {
   return (sweep_no == 1 && p->deal.p == 0) ? (double)(p->n - p->n_active) * fabs((double)(v.base - v.init)) : 0.0;
 }
-// sources without in-edges change exactly once (init/deg -> base/deg): after sweep 1, patch the vector that
-// sweep has just finished reading
-static void pr_fill_inactive(const PrPlan* p, const PrArgs& a, float base, cudaStream_t s, uint64_t* launches) {
-  if (a.sweep_no != 1 || p->n_active >= p->n) return;
-  k_pr_fill_inactive<<<grid_for(p->n - p->n_active, 256), 256, 0, s>>>(p->n, p->n_active, base, p->outdeg.p,
-                                                                     const_cast<float*>(a.x_cur));
-  *launches += 1;
+// Sweep sweep_no, entry `sweep` of a.err_hist, from x_cur into x_next (a: make_args and the caller's vectors).
+// `done` (if any) is recorded after the sweep's kernels.  Sources without in-edges change exactly once
+// (init/deg -> base/deg): after sweep 1, the vector that sweep has just finished reading is patched.
+template <bool PEERS>
+static gb_status enqueue_sweep(const PrPlan* p, PrArgs a, PrStart v, const float* x_cur, float* x_next,
+                               uint32_t sweep, uint64_t sweep_no, cudaEvent_t done, cudaStream_t s,
+                               uint64_t* launches) {
+  a.x_cur = x_cur;
+  a.x_next = x_next;
+  a.sweep = sweep;
+  a.sweep_no = (uint32_t)std::min<uint64_t>(sweep_no, 0xFFFFFFFFull);
+  a.extra_err = first_sweep_err(p, sweep_no, v);
+  GB_TRY(launch_sweep<PEERS>(p, a, s, launches));
+  if (done) GB_CUDA(cudaEventRecord(done, s));
+  if (sweep_no == 1 && p->n_active < p->n) {
+    k_pr_fill_inactive<<<grid_for(p->n - p->n_active, 256), 256, 0, s>>>(p->n, p->n_active, v.base, p->outdeg.p,
+                                                                       const_cast<float*>(x_cur));
+    *launches += 1;
+  }
+  return GB_OK;
 }
 
 // ---- drivers ---------------------------------------------------------------------------------
@@ -1132,11 +1137,6 @@ static gb_status run_jacobi(const gb_graph* g, const gb_page_rank_config* cfg, f
     const uint32_t batch = (uint32_t)std::min<uint64_t>(limit - done, can_stop_early ? 8 : batch_cap);
     for (uint32_t b = 0; b < batch; ++b) {
       const uint64_t sweep_no = done + b + 1;
-      a.x_cur = p->x[(sweep_no - 1) & 1].p;
-      a.x_next = p->x[sweep_no & 1].p;
-      a.sweep = b;
-      a.sweep_no = (uint32_t)std::min<uint64_t>(sweep_no, 0xFFFFFFFFull);
-      a.extra_err = first_sweep_err(p, sweep_no, v);
       cudaEvent_t e0 = nullptr, e1 = nullptr;
       if (profile && ev_used + 2 <= 2 * PR_MAX_PROFILE_EVENTS) {
         while (p->prof_events.size() < ev_used + 2) {
@@ -1149,9 +1149,8 @@ static gb_status run_jacobi(const gb_graph* g, const gb_page_rank_config* cfg, f
         ev_used += 2;
         GB_CUDA(cudaEventRecord(e0, s));
       }
-      GB_TRY(launch_sweep<false>(p, a, s, &g->timing.kernel_launches));
-      if (e1) GB_CUDA(cudaEventRecord(e1, s));
-      pr_fill_inactive(p, a, v.base, s, &g->timing.kernel_launches);
+      GB_TRY(enqueue_sweep<false>(p, a, v, p->x[(sweep_no - 1) & 1].p, p->x[sweep_no & 1].p, b, sweep_no, e1, s,
+                                  &g->timing.kernel_launches));
     }
     GB_CUDA(cudaGetLastError());
     done += batch;
@@ -1197,22 +1196,22 @@ static void plan_stats(const PrPlan* p, gb_pr_shard_stats* stats) {
   stats->local_edges = p->loc_edges;
   stats->block_edges = p->cb_edges;
   stats->block_entries = p->B;
-  stats->hot_blocks = p->KB;
-  stats->segments = p->S;
-  stats->groups = p->NG;
-  stats->chunks = p->n_chunks;
-  stats->tasks = p->n_tasks;
-  stats->cut_segments = p->n_fix;
-  stats->chunk_groups = p->chunk_groups;
-  stats->launches_per_sweep = 1 + (p->grid_cb ? 1 : 0) + (p->grid_sell ? 1 : 0) + (fixup_launched(p) ? 1 : 0) +
-                              (p->vb ? 2 : 0);
+  stats->hot_blocks = p->hot.KB;
+  stats->segments = p->hot.S;
+  stats->groups = p->hot.NG;
+  stats->chunks = p->hot.n_chunks;
+  stats->tasks = p->hot.n_tasks;
+  stats->cut_segments = p->hot.n_fix;
+  stats->chunk_groups = p->hot.chunk_groups;
+  stats->launches_per_sweep = 1 + (p->grid_cb ? 1 : 0) + (p->grid_sell ? 1 : 0) +
+                              (p->fix_at == PrFix::FIXUP ? 1 : 0) + (p->vb ? 2 : 0);
   stats->device_bytes = p->bytes();
-  stats->vblock_parts = p->vb ? p->v.parts : 0;
+  stats->vblock_parts = p->vb ? p->v.virt.KB : 0;
   stats->vblock_pairs = p->vb ? p->v.pairs : 0;
   stats->vblock_edges = p->vb ? p->v.edges : 0;
 }
 static void plan_shape(const PrPlan* p, gb_pr_plan_shape* shape) {
-  shape->hot_blocks = p->KB;
+  shape->hot_blocks = p->hot.KB;
   shape->n_cb = p->n_cb;
   shape->n_fin = p->n_fin;
   shape->n_fin_warp = p->n_fin_warp;
@@ -1222,8 +1221,8 @@ static void plan_shape(const PrPlan* p, gb_pr_plan_shape* shape) {
   shape->grid_sell = p->grid_sell;
   shape->grid_fin = p->grid_fin;
   shape->n_mega = p->n_mega;
-  shape->n_fix = p->n_fix;
-  shape->fix_in_sell = fix_in_sell(p) ? 1u : 0u;
+  shape->n_fix = p->hot.n_fix;
+  shape->fix_in_sell = p->fix_at == PrFix::SELL ? 1u : 0u;
   shape->dual = 0;
   shape->last_hot_block = p->last_hot_block;
 }
@@ -1336,20 +1335,15 @@ gb_status gb_pr_shard_step(const gb_pr_shard* shard, float damping, uint64_t swe
   cudaStream_t s = (cudaStream_t)cuda_stream;
   const gb::PrStart v(p->n, damping);
   gb::PrArgs a = gb::make_args(p, v.base, damping, -1.0 /* the caller owns the stop rule */);
-  a.x_cur = d_x_cur;
-  a.x_next = d_x_next;
   a.scores = d_scores;
   a.n_peers = d_mc_x_next ? 0 : peer_count;
   a.mc_next = d_mc_x_next;
   for (uint32_t i = 0; i < a.n_peers; ++i) a.peer_next[i] = d_peer_x_next[i];
   a.err_hist = d_error;
-  a.sweep = 0;
-  a.sweep_no = (uint32_t)std::min<uint64_t>(sweep_no, 0xFFFFFFFFull);
-  a.extra_err = gb::first_sweep_err(p, sweep_no, v);
   uint64_t launches = 0;
-  if (peer_count || d_mc_x_next) GB_TRY(gb::launch_sweep<true>(p, a, s, &launches));
-  else GB_TRY(gb::launch_sweep<false>(p, a, s, &launches));
-  gb::pr_fill_inactive(p, a, v.base, s, &launches);
+  if (peer_count || d_mc_x_next)
+    GB_TRY(gb::enqueue_sweep<true>(p, a, v, d_x_cur, d_x_next, 0, sweep_no, nullptr, s, &launches));
+  else GB_TRY(gb::enqueue_sweep<false>(p, a, v, d_x_cur, d_x_next, 0, sweep_no, nullptr, s, &launches));
   GB_CUDA(cudaGetLastError());
   return GB_OK;
 }

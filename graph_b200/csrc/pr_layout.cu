@@ -799,16 +799,16 @@ gb_status LayoutBuild::layout_hot_blocks() {
       GB_REQUIRE(S < 0xFFFFFFF0ull, "column-block staircase too large (%llu pairs)", (unsigned long long)S);
     }
     h_poff.push_back((uint32_t)S);
-    p->S = S;
+    p->hot.S = S;
   }
-  p->KB = (uint32_t)h_blk.size();
-  if (p->KB) p->last_hot_block = *std::max_element(h_blk.begin(), h_blk.end());
-  p->n_cb = p->KB ? h_nrows[0] : 0;
+  p->hot.KB = (uint32_t)h_blk.size();
+  if (p->hot.KB) p->last_hot_block = *std::max_element(h_blk.begin(), h_blk.end());
+  p->n_cb = p->hot.KB ? h_nrows[0] : 0;
   if (h_poff.empty()) h_poff.push_back(0);
   GB_TRY(upload(s, &hot_of_blk, h_hot));
-  GB_TRY(upload(s, &p->blk, h_blk));
-  GB_TRY(upload(s, &p->nrows, h_nrows));
-  GB_TRY(upload(s, &p->poff, h_poff));
+  GB_TRY(upload(s, &p->hot.blk, h_blk));
+  GB_TRY(upload(s, &p->hot.nrows, h_nrows));
+  GB_TRY(upload(s, &p->hot.poff, h_poff));
   return GB_OK;
 }
 
@@ -817,11 +817,11 @@ gb_status LayoutBuild::layout_hot_blocks() {
 // record per in-edge; the targets are classified chunk by chunk as they arrive when they stream in from a
 // part (PrSource::feed).  Ends with goff = the first group of every pair.
 gb_status LayoutBuild::layout_classify() {
-  GB_TRY(goff.alloc(p->S + 1));
-  GB_CUDA(cudaMemsetAsync(goff.p, 0, (p->S + 1) * 4, s));
+  GB_TRY(goff.alloc(p->hot.S + 1));
+  GB_CUDA(cudaMemsetAsync(goff.p, 0, (p->hot.S + 1) * 4, s));
   GB_TRY(lens.alloc(std::max<uint32_t>(p->n_loc, 1)));
   n_mega = std::min(n_mega, std::min(p->n_cb, (1u << (32 - CB_MEGA_JBITS)) - 1u));
-  if (p->KB >= (1u << CB_MEGA_JBITS) - 1u) n_mega = 0;
+  if (p->hot.KB >= (1u << CB_MEGA_JBITS) - 1u) n_mega = 0;
   if (n_mega) {
     DevBuf<uint32_t> mdeg;
     GB_TRY(mdeg.alloc(n_mega));
@@ -864,7 +864,7 @@ gb_status LayoutBuild::layout_classify() {
       check_ids_async(s, row_tgt + e0, e1 - e0, n, bad.p);
       if (p->n_cb > n_mega && v1 > v0)
         k_cb_count_rows<<<grid_for((uint64_t)(v1 - v0), 256), 256, 0, s>>>(
-            row_off, row_tgt, p->new_id.p, hot_of_blk.p, p->nrows.p, p->poff.p, p->blk.p, B, v0, v1, n,
+            row_off, row_tgt, p->new_id.p, hot_of_blk.p, p->hot.nrows.p, p->hot.poff.p, p->hot.blk.p, B, v0, v1, n,
             n_mega, p->n_cb, deal, goff.p, rec.p, lens.p, counters.p + 2);
     }
     unsigned int nbad = 0;
@@ -874,7 +874,7 @@ gb_status LayoutBuild::layout_classify() {
     GB_TRY(require_ids("in", nbad, n));
   } else if (p->n_cb > n_mega) {
     k_cb_count<<<grid_for((uint64_t)(p->n_cb - n_mega) * 32, 256), 256, 0, s>>>(
-        row_off, row_tgt, old_of.p, p->new_id.p, hot_of_blk.p, p->nrows.p, p->poff.p, p->blk.p, B,
+        row_off, row_tgt, old_of.p, p->new_id.p, hot_of_blk.p, p->hot.nrows.p, p->hot.poff.p, p->hot.blk.p, B,
         n_mega, p->n_cb, deal, goff.p, rec.p, lens.p, counters.p + 2);
   }
   if (M) {
@@ -885,7 +885,7 @@ gb_status LayoutBuild::layout_classify() {
     GB_TRY(mega_vals.alloc(M));
     GB_TRY(mega_start.alloc(M));
     k_mega_keys<<<grid_for(M, 256), 256, 0, s>>>(row_off, row_tgt, old_of.p, p->new_id.p,
-                                                 hot_of_blk.p, p->nrows.p, B, mega_off.p, n_mega, M, deal,
+                                                 hot_of_blk.p, p->hot.nrows.p, B, mega_off.p, n_mega, M, deal,
                                                  keys_in.p, vals_in.p);
     uint32_t row_bits = 1;
     while ((1u << row_bits) < n_mega) ++row_bits;
@@ -900,20 +900,20 @@ gb_status LayoutBuild::layout_classify() {
       return cub::DeviceScan::InclusiveScan(t, tb, start, start, cub::Max(), (int)M, s);
     }));
     GB_CUDA(cudaMemsetAsync(lens.p, 0, (size_t)n_mega * 4, s));
-    k_mega_counts<<<grid_for(M, 256), 256, 0, s>>>(mega_keys.p, start, M, p->poff.p, goff.p, lens.p,
+    k_mega_counts<<<grid_for(M, 256), 256, 0, s>>>(mega_keys.p, start, M, p->hot.poff.p, goff.p, lens.p,
                                                    counters.p + 2);
     GB_CUDA(cudaGetLastError());
     GB_CUDA(cudaStreamSynchronize(s));  // keys_in / vals_in / tmp / stmp are released here
   }
   if (p->n_loc > p->n_cb)
     k_lens_tail<<<grid_for(p->n_loc - p->n_cb, 256), 256, 0, s>>>(indeg.p, p->n_cb, p->n_loc, deal, lens.p);
-  if (p->S) {
-    k_cb_groups<<<grid_for(p->S, 256), 256, 0, s>>>(goff.p, p->S);
-    GB_TRY(scan_exclusive(s, goff.p, p->S + 1));
+  if (p->hot.S) {
+    k_cb_groups<<<grid_for(p->hot.S, 256), 256, 0, s>>>(goff.p, p->hot.S);
+    GB_TRY(scan_exclusive(s, goff.p, p->hot.S + 1));
     uint32_t ng = 0;
-    GB_CUDA(cudaMemcpyAsync(&ng, goff.p + p->S, 4, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaMemcpyAsync(&ng, goff.p + p->hot.S, 4, cudaMemcpyDeviceToHost, s));
     GB_CUDA(cudaStreamSynchronize(s));
-    p->NG = ng;
+    p->hot.NG = ng;
   }
   unsigned long long h[3] = {0, 0, 0};
   GB_CUDA(cudaMemcpyAsync(h, counters.p, 24, cudaMemcpyDeviceToHost, s));
@@ -947,22 +947,32 @@ gb_status LayoutBuild::layout_sell() {
   return GB_OK;
 }
 
+// A stream's id groups, all of them padding (pad id B) until the fill writes the segments, and its segment-start
+// bits: segment k starts at group goff[k] (S + 1 entries)
+static gb_status cb_stream_ids(cudaStream_t s, uint32_t B, const uint32_t* goff, CbStream* st) {
+  GB_TRY(st->ids.alloc(std::max<uint64_t>(st->NG, 1), 64));
+  GB_TRY(st->bits.alloc(st->NG / 32 + 8));  // a 128-group step reads 5 words from its first
+  GB_CUDA(cudaMemsetAsync(st->bits.p, 0, (st->NG / 32 + 8) * 4, s));
+  if (st->NG) {
+    k_fill_u2<<<grid_for(st->NG + 64, 256), 256, 0, s>>>(st->ids.p, st->NG + 64, make_uint2(B | (B << 16), B | (B << 16)));
+    k_cb_bits<<<grid_for(st->S, 256), 256, 0, s>>>(goff, st->S, st->bits.p);
+  }
+  return GB_OK;
+}
+
 // fill: segments + SELL remainders of the rows below n_cb, whole rows above
 gb_status LayoutBuild::layout_fill() {
-  GB_TRY(p->cb_ids.alloc(std::max<uint64_t>(p->NG, 1), 64));
-  GB_TRY(p->cb_bits.alloc(p->NG / 32 + 8));  // a 128-group step reads 5 words from its first
-  GB_CUDA(cudaMemsetAsync(p->cb_bits.p, 0, (p->NG / 32 + 8) * 4, s));
-  uint16_t* ids = reinterpret_cast<uint16_t*>(p->cb_ids.p);
+  const CbStream& hot = p->hot;
+  GB_TRY(cb_stream_ids(s, B, goff.p, &p->hot));
+  uint16_t* ids = reinterpret_cast<uint16_t*>(hot.ids.p);
   uint32_t* sell = reinterpret_cast<uint32_t*>(p->sell.p);
-  if (p->NG) {
-    k_fill_u2<<<grid_for(p->NG + 64, 256), 256, 0, s>>>(p->cb_ids.p, p->NG + 64, make_uint2(B | (B << 16), B | (B << 16)));
-    k_cb_bits<<<grid_for(p->S, 256), 256, 0, s>>>(goff.p, p->S, p->cb_bits.p);
+  if (hot.NG) {
     if (M)
       k_mega_fill<<<grid_for(M, 256), 256, 0, s>>>(mega_keys.p, mega_vals.p, mega_start.p, M,
-                                                       p->poff.p, p->blk.p, B, goff.p, ids, p->slice_meta.p, sell);
+                                                       hot.poff.p, hot.blk.p, B, goff.p, ids, p->slice_meta.p, sell);
     if (p->n_cb > n_mega)
       k_cb_fill<<<grid_for((uint64_t)(p->n_cb - n_mega) * 32, 256), 256, 0, s>>>(
-          row_off, old_of.p, rec.p, p->poff.p, n_mega, p->n_cb, deal, goff.p, ids, p->slice_meta.p,
+          row_off, old_of.p, rec.p, hot.poff.p, n_mega, p->n_cb, deal, goff.p, ids, p->slice_meta.p,
           sell);
     GB_CUDA(cudaGetLastError());
     GB_CUDA(cudaStreamSynchronize(s));
@@ -976,9 +986,75 @@ gb_status LayoutBuild::layout_fill() {
   return GB_OK;
 }
 
-static gb_status cb_chunk_table(cudaStream_t s, int dev_sms, uint32_t B, const uint32_t* goff, const uint32_t* poff,
-                                const uint32_t* nrows, uint32_t KB, uint64_t NG, const std::vector<uint32_t>& min_cgrp,
-                                uint2* ids, CbChunks* out);
+// The chunk table of stream st (block j's segments start at goff[poff[j]] ..): its chunks, the bank order of the
+// ids inside them, and every persistent CTA's share of them (tasks).  min_cgrp (empty: none) raises block j's
+// chunk length to at least min_cgrp[j] groups.  An empty stream gets one-entry buffers and no task.
+static gb_status cb_chunk_table(cudaStream_t s, int dev_sms, uint32_t B, const uint32_t* goff,
+                                const std::vector<uint32_t>& min_cgrp, CbStream* st) {
+  if (!st->NG) {
+    GB_TRY(st->chunks.alloc(1));
+    GB_TRY(st->tail_slot.alloc(1));
+    GB_TRY(st->fix_list.alloc(1));
+    GB_TRY(st->side.alloc(2));
+    GB_TRY(st->tasks.alloc(1));
+    return GB_OK;
+  }
+  const uint32_t KB = st->KB;
+  // first group of every block's stream
+  DevBuf<uint32_t> gbeg;
+  GB_TRY(gbeg.alloc(KB + 1));
+  k_gather_u32<<<grid_for(KB + 1, 128), 128, 0, s>>>(goff, st->poff.p, KB + 1, gbeg.p);
+  std::vector<uint32_t> h_gbeg(KB + 1);
+  GB_CUDA(cudaMemcpyAsync(h_gbeg.data(), gbeg.p, (size_t)(KB + 1) * 4, cudaMemcpyDeviceToHost, s));
+  GB_CUDA(cudaStreamSynchronize(s));
+  // ~8 tasks per SM keep the dynamic schedule level; a task is 32 chunks (one per warp) of 512..2048
+  // groups (fewer, longer chunks = fewer segments cut by chunk boundaries); a thin block is cut into
+  // >= 64 chunks (down to one 64-group step each) so that all warps share it — a lone warp runs at
+  // its dependency latency, ~10x below the SM's throughput
+  uint32_t C = (uint32_t)env_u64("GB_PR_CHUNK", 0);
+  const uint32_t T = std::min<uint32_t>(std::max<uint32_t>((uint32_t)env_u64("GB_PR_TASK_CHUNKS", CB_TASK_CHUNKS), 32u), 128u);
+  if (!C) C = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(st->NG / ((uint64_t)dev_sms * 8 * T), 16384 / T), 65536 / T);
+  C = std::max<uint32_t>(32u, (C + 31) / 32 * 32);
+  st->chunk_groups = C;
+  std::vector<uint32_t> h_cfirst(KB + 1, 0), h_cgrp(KB, C);
+  std::vector<uint2> h_tasks;
+  for (uint32_t j = 0; j < KB; ++j) {
+    const uint32_t G = h_gbeg[j + 1] - h_gbeg[j];
+    h_cgrp[j] = std::min<uint32_t>(C, std::max<uint32_t>(std::min<uint32_t>(64u, C), (G / 64 + 63) / 64 * 64));
+    if (!min_cgrp.empty()) h_cgrp[j] = std::max(h_cgrp[j], min_cgrp[j]);
+    const uint32_t nc = (G + h_cgrp[j] - 1) / h_cgrp[j];
+    h_cfirst[j + 1] = h_cfirst[j] + nc;
+    for (uint32_t c = 0; c < nc; c += T)
+      h_tasks.push_back(make_uint2(h_cfirst[j] + c, (std::min(nc, c + T) - c) | (j << 8)));
+  }
+  st->n_chunks = h_cfirst[KB];
+  st->n_tasks = (uint32_t)h_tasks.size();
+  GB_TRY(upload(s, &st->tasks, h_tasks));
+  DevBuf<uint32_t> cfirst, cgrp, d_nfix;
+  GB_TRY(upload(s, &cfirst, h_cfirst));
+  GB_TRY(upload(s, &cgrp, h_cgrp));
+  GB_TRY(d_nfix.alloc(2));
+  GB_CUDA(cudaMemsetAsync(d_nfix.p, 0, 8, s));
+  GB_TRY(st->chunks.alloc(st->n_chunks, 1));
+  GB_TRY(st->tail_slot.alloc(st->n_chunks));
+  GB_TRY(st->fix_list.alloc(st->n_chunks));
+  GB_TRY(st->side.alloc((size_t)2 * st->n_chunks + 2));
+  GB_CUDA(cudaMemsetAsync(st->side.p, 0, ((size_t)2 * st->n_chunks + 2) * 8, s));
+  GB_CUDA(cudaMemsetAsync(st->chunks.p + st->n_chunks, 0, sizeof(uint4), s));  // sentinel: ends every fixup walk
+  k_cb_chunks<<<grid_for(st->n_chunks, 128), 128, 0, s>>>(goff, st->poff.p, st->nrows.p, gbeg.p, cfirst.p, cgrp.p, KB,
+                                                          st->n_chunks, st->chunks.p, st->tail_slot.p,
+                                                          st->fix_list.p, d_nfix.p);
+  k_cb_bank_order<<<grid_for((uint64_t)st->n_chunks * 32, CB_BANK_THREADS), CB_BANK_THREADS, 0, s>>>(
+      st->chunks.p, st->n_chunks, B, st->ids.p);
+  GB_CUDA(cudaGetLastError());
+  uint32_t h_fix[2] = {0, 0};
+  GB_CUDA(cudaMemcpyAsync(h_fix, d_nfix.p, 8, cudaMemcpyDeviceToHost, s));
+  GB_CUDA(cudaStreamSynchronize(s));
+  st->n_fix = h_fix[0];
+  st->fix_max_row = h_fix[1];
+  return GB_OK;
+}
+
 constexpr uint64_t VB_L2_FACTOR = 2;  // the virtual blocks run when the source vector exceeds this many L2s
 static uint32_t bits_for(uint64_t count) {  // bits of the largest index below count
   uint32_t b = 1;
@@ -1038,14 +1114,17 @@ gb_status LayoutBuild::layout_vblocks() {
   h_row0.push_back(n_loc);
   if (E == 0 || E >= 0x7FFFFFFFull) return GB_OK;
   PrVBlocks& v = p->v;
+  CbStream& vs = v.virt;  // pass B's stream: one block per partition, one segment per local row
   const uint32_t parts = (uint32_t)h_mseg.size();
+  vs.KB = parts;
+  vs.S = n_loc;
   std::vector<uint32_t> h_rows(parts), h_min(parts);
   for (uint32_t k = 0; k < parts; ++k) {
     h_rows[k] = h_row0[k + 1] - h_row0[k];
     h_min[k] = (h_mseg[k] + 31) / 32 * 32;  // no segment is cut by a chunk boundary: no fixup pass
   }
-  GB_TRY(upload(s, &v.row0, h_row0));
-  GB_TRY(upload(s, &v.rows, h_rows));
+  GB_TRY(upload(s, &vs.poff, h_row0));
+  GB_TRY(upload(s, &vs.nrows, h_rows));
   // pass B's segments: one per local row, the cold edges' slot ids in CSR order
   DevBuf<uint32_t> coff, goffv;
   GB_TRY(coff.alloc((size_t)n_loc + 1));
@@ -1059,12 +1138,8 @@ gb_status LayoutBuild::layout_vblocks() {
   uint32_t ngv = 0;
   GB_CUDA(cudaMemcpyAsync(&ngv, goffv.p + n_loc, 4, cudaMemcpyDeviceToHost, s));
   GB_CUDA(cudaStreamSynchronize(s));
-  v.NG = ngv;
-  GB_TRY(v.ids.alloc(v.NG, 64));
-  GB_TRY(v.bits.alloc(v.NG / 32 + 8));
-  GB_CUDA(cudaMemsetAsync(v.bits.p, 0, (v.NG / 32 + 8) * 4, s));
-  k_fill_u2<<<grid_for(v.NG + 64, 256), 256, 0, s>>>(v.ids.p, v.NG + 64, make_uint2(B | (B << 16), B | (B << 16)));
-  k_cb_bits<<<grid_for(n_loc, 256), 256, 0, s>>>(goffv.p, n_loc, v.bits.p);
+  vs.NG = ngv;
+  GB_TRY(cb_stream_ids(s, B, goffv.p, &vs));
   // the cold edges sorted by (partition, source): a run of equal keys is one pair, one slot of V
   const uint32_t Ec = (uint32_t)E;
   uint32_t NP = 0;
@@ -1078,7 +1153,7 @@ gb_status LayoutBuild::layout_vblocks() {
     GB_TRY(idx.alloc(Ec));
     GB_TRY(idx_alt.alloc(Ec));
     GB_TRY(erow.alloc(Ec));
-    k_vb_edges<<<grid_for(n_loc, 256), 256, 0, s>>>(lens.p, coff.p, v.row0.p, parts, n_loc, p->slice_meta.p,
+    k_vb_edges<<<grid_for(n_loc, 256), 256, 0, s>>>(lens.p, coff.p, vs.poff.p, parts, n_loc, p->slice_meta.p,
                                                     reinterpret_cast<const uint32_t*>(p->sell.p), keys.p, idx.p, erow.p);
     cub::DoubleBuffer<uint64_t> kb(keys.p, keys_alt.p);
     cub::DoubleBuffer<uint32_t> ib(idx.p, idx_alt.p);
@@ -1096,7 +1171,7 @@ gb_status LayoutBuild::layout_vblocks() {
     std::vector<uint32_t> h_vbase(parts + 1, 0);
     for (uint32_t k = 0; k < parts; ++k)
       h_vbase[k + 1] = h_vbase[k] + (h_pfirst[k + 1] - h_pfirst[k] + VB_ALIGN - 1) / VB_ALIGN * VB_ALIGN;
-    GB_TRY(upload(s, &v.vbase, h_vbase));
+    GB_TRY(upload(s, &vs.blk, h_vbase));
     GB_TRY(v.val.alloc(std::max<uint32_t>(h_vbase[parts], 1)));
     GB_CUDA(cudaMemsetAsync(v.val.p, 0, (size_t)std::max<uint32_t>(h_vbase[parts], 1) * 4, s));
     GB_TRY(akey.alloc(NP));
@@ -1104,7 +1179,7 @@ gb_status LayoutBuild::layout_vblocks() {
     GB_TRY(aslot.alloc(NP));
     GB_TRY(aslot_alt.alloc(NP));
     k_vb_place<<<grid_for(Ec, 256), 256, 0, s>>>(kb.Current(), ib.Current(), rank.p, Ec, erow.p, coff.p, goffv.p,
-                                                 pfirst.p, v.vbase.p, B, reinterpret_cast<uint16_t*>(v.ids.p),
+                                                 pfirst.p, vs.blk.p, B, reinterpret_cast<uint16_t*>(vs.ids.p),
                                                  akey.p, aslot.p);
     GB_CUDA(cudaGetLastError());
     GB_CUDA(cudaStreamSynchronize(s));
@@ -1160,15 +1235,14 @@ gb_status LayoutBuild::layout_vblocks() {
                                                 run_rank.p, v.bin_ids.p, v.bin_bits.p, v.bin_grun.p, v.bin_runs.p);
   GB_CUDA(cudaGetLastError());
   // pass B's chunks and tasks over the virtual blocks (rows [row0[k], row0[k + 1]) each)
-  GB_TRY(cb_chunk_table(s, dev_sms, B, goffv.p, v.row0.p, v.rows.p, parts, v.NG, h_min, v.ids.p, &v.cut));
-  GB_REQUIRE(v.cut.n_fix == 0, "a virtual-block segment is cut by a chunk boundary");
-  GB_TRY(v.partial.alloc(n_loc));
-  GB_CUDA(cudaMemsetAsync(v.partial.p, 0, (size_t)n_loc * 4, s));
-  v.parts = parts;
+  GB_TRY(cb_chunk_table(s, dev_sms, B, goffv.p, h_min, &vs));
+  GB_REQUIRE(vs.n_fix == 0, "a virtual-block segment is cut by a chunk boundary");
+  GB_TRY(vs.partial.alloc(n_loc));
+  GB_CUDA(cudaMemsetAsync(vs.partial.p, 0, (size_t)n_loc * 4, s));
   v.pairs = NP;
   v.edges = E;
   p->grid_bin = (unsigned)std::min<uint64_t>(v.bin_n_tasks, (uint64_t)dev_sms);
-  p->grid_vb = (unsigned)std::min<uint64_t>(v.cut.n_tasks, (uint64_t)dev_sms);
+  p->grid_vb = (unsigned)std::min<uint64_t>(vs.n_tasks, (uint64_t)dev_sms);
   // the SELL slices have served as the build's list of cold edges: k_pr_sell does not run
   p->sell = DevBuf<uint4>();
   p->slice_meta = DevBuf<uint2>();
@@ -1178,99 +1252,19 @@ gb_status LayoutBuild::layout_vblocks() {
   return GB_OK;
 }
 
-// Chunks of one column-block stream (KB blocks, block j's segments start at goff[poff[j] ..], NG groups), the
-// bank order of the ids inside them, and every persistent CTA's share of them (tasks).  min_cgrp (empty: none)
-// raises block j's chunk length to at least min_cgrp[j] groups.
-static gb_status cb_chunk_table(cudaStream_t s, int dev_sms, uint32_t B, const uint32_t* goff, const uint32_t* poff,
-                                const uint32_t* nrows, uint32_t KB, uint64_t NG, const std::vector<uint32_t>& min_cgrp,
-                                uint2* ids, CbChunks* out) {
-  // first group of every block's stream
-  DevBuf<uint32_t> gbeg;
-  GB_TRY(gbeg.alloc(KB + 1));
-  k_gather_u32<<<grid_for(KB + 1, 128), 128, 0, s>>>(goff, poff, KB + 1, gbeg.p);
-  std::vector<uint32_t> h_gbeg(KB + 1);
-  GB_CUDA(cudaMemcpyAsync(h_gbeg.data(), gbeg.p, (size_t)(KB + 1) * 4, cudaMemcpyDeviceToHost, s));
-  GB_CUDA(cudaStreamSynchronize(s));
-  // ~8 tasks per SM keep the dynamic schedule level; a task is 32 chunks (one per warp) of 512..2048
-  // groups (fewer, longer chunks = fewer segments cut by chunk boundaries); a thin block is cut into
-  // >= 64 chunks (down to one 64-group step each) so that all warps share it — a lone warp runs at
-  // its dependency latency, ~10x below the SM's throughput
-  uint32_t C = (uint32_t)env_u64("GB_PR_CHUNK", 0);
-  const uint32_t T = std::min<uint32_t>(std::max<uint32_t>((uint32_t)env_u64("GB_PR_TASK_CHUNKS", CB_TASK_CHUNKS), 32u), 128u);
-  if (!C) C = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(NG / ((uint64_t)dev_sms * 8 * T), 16384 / T), 65536 / T);
-  C = std::max<uint32_t>(32u, (C + 31) / 32 * 32);
-  out->chunk_groups = C;
-  std::vector<uint32_t> h_cfirst(KB + 1, 0), h_cgrp(KB, C);
-  std::vector<uint2> h_tasks;
-  for (uint32_t j = 0; j < KB; ++j) {
-    const uint32_t G = h_gbeg[j + 1] - h_gbeg[j];
-    h_cgrp[j] = std::min<uint32_t>(C, std::max<uint32_t>(std::min<uint32_t>(64u, C), (G / 64 + 63) / 64 * 64));
-    if (!min_cgrp.empty()) h_cgrp[j] = std::max(h_cgrp[j], min_cgrp[j]);
-    const uint32_t nc = (G + h_cgrp[j] - 1) / h_cgrp[j];
-    h_cfirst[j + 1] = h_cfirst[j] + nc;
-    for (uint32_t c = 0; c < nc; c += T)
-      h_tasks.push_back(make_uint2(h_cfirst[j] + c, (std::min(nc, c + T) - c) | (j << 8)));
-  }
-  out->n_chunks = h_cfirst[KB];
-  out->n_tasks = (uint32_t)h_tasks.size();
-  GB_TRY(upload(s, &out->tasks, h_tasks));
-  DevBuf<uint32_t> cfirst, cgrp, d_nfix;
-  GB_TRY(upload(s, &cfirst, h_cfirst));
-  GB_TRY(upload(s, &cgrp, h_cgrp));
-  GB_TRY(d_nfix.alloc(2));
-  GB_CUDA(cudaMemsetAsync(d_nfix.p, 0, 8, s));
-  GB_TRY(out->chunks.alloc(out->n_chunks, 1));
-  GB_TRY(out->tail_slot.alloc(out->n_chunks));
-  GB_TRY(out->fix_list.alloc(out->n_chunks));
-  GB_TRY(out->side.alloc((size_t)2 * out->n_chunks + 2));
-  GB_CUDA(cudaMemsetAsync(out->side.p, 0, ((size_t)2 * out->n_chunks + 2) * 8, s));
-  GB_CUDA(cudaMemsetAsync(out->chunks.p + out->n_chunks, 0, sizeof(uint4), s));  // sentinel: ends every fixup walk
-  k_cb_chunks<<<grid_for(out->n_chunks, 128), 128, 0, s>>>(goff, poff, nrows, gbeg.p, cfirst.p, cgrp.p, KB,
-                                                           out->n_chunks, out->chunks.p, out->tail_slot.p,
-                                                           out->fix_list.p, d_nfix.p);
-  k_cb_bank_order<<<grid_for((uint64_t)out->n_chunks * 32, CB_BANK_THREADS), CB_BANK_THREADS, 0, s>>>(
-      out->chunks.p, out->n_chunks, B, ids);
-  GB_CUDA(cudaGetLastError());
-  uint32_t h_fix[2] = {0, 0};
-  GB_CUDA(cudaMemcpyAsync(h_fix, d_nfix.p, 8, cudaMemcpyDeviceToHost, s));
-  GB_CUDA(cudaStreamSynchronize(s));
-  out->n_fix = h_fix[0];
-  out->fix_max_row = h_fix[1];
-  return GB_OK;
-}
-
 // Chunks of the column-block kernel; then the sweep's per-pair and per-row buffers.
 gb_status LayoutBuild::layout_chunks() {
-  p->grid_cb = 0;
-  if (p->NG) {
-    CbChunks c;
-    GB_TRY(cb_chunk_table(s, dev_sms, B, goff.p, p->poff.p, p->nrows.p, p->KB, p->NG, {}, p->cb_ids.p, &c));
-    p->chunk_groups = c.chunk_groups;
-    p->n_chunks = c.n_chunks;
-    p->n_tasks = c.n_tasks;
-    p->n_fix = c.n_fix;
-    p->fix_max_row = c.fix_max_row;
-    p->chunks = std::move(c.chunks);
-    p->tail_slot = std::move(c.tail_slot);
-    p->fix_list = std::move(c.fix_list);
-    p->side = std::move(c.side);
-    p->tasks = std::move(c.tasks);
-    p->grid_cb = (unsigned)std::min<uint64_t>(p->n_tasks, (uint64_t)dev_sms);  // one persistent CTA per SM
-  } else {
-    GB_TRY(p->chunks.alloc(1));
-    GB_TRY(p->tail_slot.alloc(1));
-    GB_TRY(p->fix_list.alloc(1));
-    GB_TRY(p->side.alloc(2));
-    GB_TRY(p->tasks.alloc(1));
-  }
+  CbStream& hot = p->hot;
+  GB_TRY(cb_chunk_table(s, dev_sms, B, goff.p, {}, &hot));
+  p->grid_cb = (unsigned)std::min<uint64_t>(hot.n_tasks, (uint64_t)dev_sms);  // one persistent CTA per SM
   GB_TRY(p->task_ctr.alloc(std::max<unsigned>(p->task_ranges(), 1)));
   GB_CUDA(cudaMemsetAsync(p->task_ctr.p, 0, (size_t)std::max<unsigned>(p->task_ranges(), 1) * 4, s));
-  GB_TRY(p->partial.alloc(std::max<uint64_t>(p->S, 1)));
-  GB_CUDA(cudaMemsetAsync(p->partial.p, 0, std::max<uint64_t>(p->S, 1) * 4, s));
+  GB_TRY(hot.partial.alloc(std::max<uint64_t>(hot.S, 1)));
+  GB_CUDA(cudaMemsetAsync(hot.partial.p, 0, std::max<uint64_t>(hot.S, 1) * 4, s));
   GB_TRY(p->rem.alloc(std::max<uint32_t>(p->vb ? 1u : p->n_cb, 1)));
   // k_pr_finish completes the rows below n_cb, or every local row when the virtual blocks run
   std::vector<uint32_t> h_kb(((p->vb ? p->n_loc : p->n_cb) + 31) / 32);
-  for (size_t w = 0; w < h_kb.size(); ++w) h_kb[w] = fin_blocks_of(h_nrows.data(), p->KB, (uint32_t)w * 32);
+  for (size_t w = 0; w < h_kb.size(); ++w) h_kb[w] = fin_blocks_of(h_nrows.data(), hot.KB, (uint32_t)w * 32);
   GB_TRY(upload(s, &p->fin_kb, h_kb));
   return GB_OK;
 }

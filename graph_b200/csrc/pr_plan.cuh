@@ -57,16 +57,34 @@ static inline uint32_t deal_count(uint32_t R, uint32_t P, uint32_t p) {
   return c;
 }
 
-// The chunks and tasks of one column-block id stream (k_pr_cb's unit of work), as the layout build cuts them
-struct CbChunks {
+// One id stream of k_pr_cb's walker and what its consumers read: KB blocks; block j's local rows [0, nrows[j])
+// own one segment each, row by row, and the segments' partials start at poff[j].  The hot blocks (PrPlan::hot,
+// k_pr_cb<CB_MAIN>) are blocks of the source vector: blk[j] is the source block of hot rank j.  Pass B of the
+// virtual blocks (PrVBlocks::virt, k_pr_cb<CB_VIRT>) walks the slots of V: blk[j] .. blk[j + 1] are virtual
+// block j's slot bounds, poff[j] is partition j's first local row and nrows[j] its row count, so that every
+// local row's partial lands at its own index.
+struct CbStream {
+  uint32_t KB = 0;              // blocks
+  uint64_t S = 0;               // segments = partials = sum of nrows[j]
+  uint64_t NG = 0;              // groups in all blocks
+  DevBuf<uint32_t> blk;         // [KB] hot rank j's source block (pass B: [KB + 1] V slot bounds, multiples of VB_ALIGN)
+  DevBuf<uint32_t> nrows;       // [KB] rows with a segment in block j (non-increasing for the hot blocks)
+  DevBuf<uint32_t> poff;        // [KB + 1] first partial of block j
+  DevBuf<uint2> ids;            // [NG] groups of 4 block-local 16-bit ids (pad id = B)
+  DevBuf<uint32_t> bits;        // [NG/32 + 8] bit g set <=> group g starts a segment
+  DevBuf<float> partial;        // [S] one partial sum per segment
+  // the chunks and tasks (k_pr_cb's unit of work), as cb_chunk_table cuts them
   uint32_t chunk_groups = 0, n_chunks = 0, n_tasks = 0, n_fix = 0;
   uint32_t fix_max_row = 0;     // largest row that owns a segment cut by a chunk boundary
   DevBuf<uint4> chunks;         // [n_chunks + 1] (g_begin, g_end, row_before, j | flags << 24); a zero sentinel
-  DevBuf<uint32_t> tail_slot;   // [n_chunks] staircase slot of the segment cut by the chunk end
+  DevBuf<uint32_t> tail_slot;   // [n_chunks] partial of the segment cut by the chunk end
   DevBuf<double> side;          // [2 n_chunks] head / tail parts of segments cut by chunk boundaries
   DevBuf<uint32_t> fix_list;    // [n_fix] chunks whose tail segment continues in later chunks
   DevBuf<uint2> tasks;          // [n_tasks] (first chunk, chunk count | block rank << 8), fattest blocks first
-  uint64_t bytes() const { return chunks.bytes() + tail_slot.bytes() + side.bytes() + fix_list.bytes() + tasks.bytes(); }
+  uint64_t bytes() const {
+    return blk.bytes() + nrows.bytes() + poff.bytes() + ids.bytes() + bits.bytes() + partial.bytes() + chunks.bytes() +
+           tail_slot.bytes() + side.bytes() + fix_list.bytes() + tasks.bytes();
+  }
 };
 
 // Virtual blocks: the edges that no column-block segment takes (COLD edges) on graphs whose source vector does
@@ -77,13 +95,9 @@ struct CbChunks {
 // column-block stream over the virtual blocks, with V in place of the source vector, and leaves one partial per
 // local row.  k_pr_finish then completes every local row, and k_pr_sell does not run.
 struct PrVBlocks {
-  uint32_t parts = 0;           // partitions = virtual blocks
   uint64_t pairs = 0, edges = 0;  // (source, partition) pairs and the cold edges they serve
   uint32_t bin_blocks = 0, n_runs = 0;
-  DevBuf<uint32_t> vbase;       // [parts + 1] first V slot of each virtual block (multiples of VB_ALIGN)
   DevBuf<float> val;            // V
-  DevBuf<uint32_t> row0;        // [parts + 1] the partitions' first local rows (pass B's staircase offsets)
-  DevBuf<uint32_t> rows;        // [parts] rows per partition (pass B's row counts)
   // pass A: the pairs in (source block, partition, source) order, each block's share starting at a multiple of
   // 32 positions (BIN_PAD in between); a RUN is the pairs of one (block, partition), consecutive slots of V
   DevBuf<uint16_t> bin_ids;     // block-local source id at every position
@@ -94,17 +108,22 @@ struct PrVBlocks {
   DevBuf<uint32_t> bin_blk;     // [bin_blocks] source block of each of pass A's block ranks
   DevBuf<uint2> bin_tasks;      // (first chunk, chunk count | block rank << 8)
   uint32_t bin_n_tasks = 0;
-  // pass B: one segment per local row (a padding group when the row has no cold edge)
-  uint64_t NG = 0;
-  DevBuf<uint2> ids;            // groups of 4 V-local 16-bit slot ids (pad id = B)
-  DevBuf<uint32_t> bits;        // bit g set <=> group g starts a row's segment
-  DevBuf<float> partial;        // [n_loc] the cold sum of every local row
-  CbChunks cut;
+  // pass B: one block per partition (KB = partitions), one segment per local row (a padding group when the row
+  // has no cold edge); its partials are the cold sums of the local rows
+  CbStream virt;
   uint64_t bytes() const {
-    return vbase.bytes() + val.bytes() + row0.bytes() + rows.bytes() + bin_ids.bytes() + bin_bits.bytes() +
-           bin_grun.bytes() + bin_runs.bytes() + bin_chunks.bytes() + bin_blk.bytes() + bin_tasks.bytes() +
-           ids.bytes() + bits.bytes() + partial.bytes() + cut.bytes();
+    return val.bytes() + bin_ids.bytes() + bin_bits.bytes() + bin_grun.bytes() + bin_runs.bytes() +
+           bin_chunks.bytes() + bin_blk.bytes() + bin_tasks.bytes() + virt.bytes();
   }
+};
+
+// Which kernel adds the parts of the hot blocks' segments cut by chunk boundaries: one that runs after k_pr_cb
+// and before the kernel that completes their rows (plan_sweep_shape decides)
+enum class PrFix : uint32_t {
+  NONE,    // no segment is cut
+  FIXUP,   // a k_pr_fixup launch before k_pr_sell: some cut row is completed by its k_pr_sell lane (few hot blocks)
+  SELL,    // k_pr_sell's first warps: every cut row is completed later, by k_pr_finish (rows below n_fin)
+  PASS_A,  // pass A's first warps (virtual blocks): k_pr_finish completes every row
 };
 
 struct PrPlan {
@@ -118,26 +137,12 @@ struct PrPlan {
   uint64_t cb_edges = 0;  // of which served from column blocks
   DevBuf<uint32_t> new_id;    // old id -> internal id
   DevBuf<uint32_t> outdeg;    // out-degree by internal id [n]
-  // column blocks
-  uint32_t B = 0, KB = 0;       // block entries, hot blocks
-  uint64_t S = 0;               // staircase size = sum of nrows[j]
-  uint64_t NG = 0;              // groups in all block streams
-  uint32_t chunk_groups = 0, n_chunks = 0, n_tasks = 0, n_fix = 0;
-  uint32_t fix_max_row = 0;     // largest local row that owns a segment cut by a chunk boundary
+  // column blocks: B entries per block, the hot blocks' stream (the staircase: one partial per (block, row) pair)
+  uint32_t B = 0;
+  CbStream hot;
   uint32_t n_mega = 0;          // local rows [0, n_mega) went through the sort path of the layout build
   uint32_t last_hot_block = CB_NONE;  // largest source block index among the hot blocks
-  DevBuf<uint32_t> blk;         // [KB] source block of hot rank j
-  DevBuf<uint32_t> nrows;       // [KB] local rows [0, nrows[j]) have a segment in block j (non-increasing)
-  DevBuf<uint32_t> poff;        // [KB+1] staircase offsets
-  DevBuf<uint2> cb_ids;         // [NG] groups of 4 block-local 16-bit ids (pad id = B)
-  DevBuf<uint32_t> cb_bits;     // [NG/32 + 8] bit g set <=> group g starts a segment
-  DevBuf<float> partial;        // [S] one partial sum per (block, row) pair
-  DevBuf<uint4> chunks;         // [n_chunks] (g_begin, g_end, row_before, j | flags << 24)
-  DevBuf<uint32_t> tail_slot;   // [n_chunks] staircase slot of the segment cut by the chunk end
-  DevBuf<double> side;          // [2 n_chunks] head / tail parts of segments cut by chunk boundaries
-  DevBuf<uint32_t> fix_list;    // [n_fix] chunks whose tail segment continues in later chunks
-  DevBuf<uint2> tasks;          // [n_tasks] (first chunk, chunk count | block rank << 8), fattest blocks first
-  DevBuf<uint32_t> task_ctr;    // [grid_cb] per-range task cursors (reset by the finish kernel)
+  DevBuf<uint32_t> task_ctr;    // [task_ranges()] per-range task cursors (reset by the finish kernel)
   DevBuf<float> rem;            // [n_cb] SELL remainder sums of the rows that also have segments
   DevBuf<uint32_t> fin_kb;      // [ceil(n_cb / 32)] blocks of the first row of each 32-row group (finish kernel)
   // SELL-32 (all local active rows; rows < n_cb hold only the edges outside their segments)
@@ -157,6 +162,7 @@ struct PrPlan {
   uint32_t fin_hub_ctas = 0; // finish CTAs that take the hub groups (the others take rows [n_fin_warp, n_fin))
   uint32_t n_fin = 0;        // rows [0, n_fin) are completed by k_pr_finish, [n_fin, n_cb) by k_pr_sell
   uint32_t few_nrows[SELL_FEW] = {}, few_poff[SELL_FEW] = {};
+  PrFix fix_at = PrFix::NONE;  // the kernel that adds the parts of the hot blocks' cut segments
   DevBuf<double> block_err;  // per CTA error partials (SELL CTAs, then finish CTAs)
   DevBuf<double> err_hist;   // error of each sweep of the current batch
   DevBuf<uint32_t> ctrl;     // [0] = done flag (sweep number at which tolerance was met), [1] = ticket
@@ -167,10 +173,9 @@ struct PrPlan {
   bool trace = false;
   mutable std::vector<cudaEvent_t> trace_events;  // 5 per traced sweep
   uint64_t bytes() const {
-    return new_id.bytes() + outdeg.bytes() + blk.bytes() + nrows.bytes() + poff.bytes() + cb_ids.bytes() +
-           cb_bits.bytes() + partial.bytes() + chunks.bytes() + tail_slot.bytes() + side.bytes() +
-           fix_list.bytes() + tasks.bytes() + rem.bytes() + fin_kb.bytes() + sell.bytes() + slice_meta.bytes() + x[0].bytes() +
-           x[1].bytes() + scores.bytes() + block_err.bytes() + err_hist.bytes() + v.bytes();
+    return new_id.bytes() + outdeg.bytes() + hot.bytes() + rem.bytes() + fin_kb.bytes() + sell.bytes() +
+           slice_meta.bytes() + x[0].bytes() + x[1].bytes() + scores.bytes() + block_err.bytes() + err_hist.bytes() +
+           v.bytes();
   }
   // task cursors: k_pr_cb's ranges, then pass A's, then pass B's (the finish kernel resets them all)
   uint32_t task_ranges() const { return grid_cb + grid_bin + grid_vb; }

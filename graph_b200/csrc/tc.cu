@@ -270,7 +270,8 @@ static gb_status tc_csr(int device, uint32_t n, const uint32_t* off, const uint3
   gb_tc_csr_info info{};
   info.first_list_chunk = K;
   GB_CUDA(cudaMemsetAsync(t.found.p, 0, (size_t)K * 8, f.check));
-  GB_CUDA(cudaMemsetAsync(t.total.p, 0, 8, t.count));
+  // on the check stream: every count launch, on a lane or on t.count, waits for a checked[] event recorded there
+  GB_CUDA(cudaMemsetAsync(t.total.p, 0, 8, f.check));
   const uint32_t *d_off = f.feed.off.p, *d_tgt = f.feed.tgt.p;
   // chunk k's row-order flag, checked with its ids
   f.per_chunk = [&](uint32_t k) -> gb_status {
