@@ -48,7 +48,8 @@ class PrShardStats(C.Structure):
                 ("groups", C.c_uint64), ("chunks", C.c_uint32), ("tasks", C.c_uint32),
                 ("cut_segments", C.c_uint32), ("chunk_groups", C.c_uint32),
                 ("launches_per_sweep", C.c_uint32), ("device_bytes", C.c_uint64),
-                ("vblock_parts", C.c_uint32), ("vblock_pairs", C.c_uint64), ("vblock_edges", C.c_uint64)]
+                ("vblock_parts", C.c_uint32), ("vblock_pairs", C.c_uint64), ("vblock_edges", C.c_uint64),
+                ("vblock_wide_steps", C.c_uint32)]
 
     def as_dict(self):
         return {k: int(getattr(self, k)) for k, _ in self._fields_}

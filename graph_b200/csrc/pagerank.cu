@@ -140,7 +140,7 @@ struct PrArgs {
   const uint16_t* bin_ids;
   const uint32_t* bin_bits;
   const uint32_t* bin_grun;
-  const uint2* bin_runs;
+  const uint32_t* bin_runs;
   const uint2* bin_chunks;
   // SELL rows
   const uint4* sell;
@@ -352,19 +352,79 @@ __device__ __forceinline__ void cb_chunk(const PrArgs& a, const float* xs, uint3
   }
 }
 
-// Pass A of the virtual blocks, one warp per chunk of 32-position groups of one source block: lane i of group g
-// stores the value of the pair at position 32 g + i to its slot of V.  A run's slots are consecutive, so the
-// stores of a group are coalesced; the run of a position is the group's first run plus the run starts after it.
+// V[slot] = xs[sid] unless sid is BIN_PAD, predicated: a branch per position would split the warp's stores
+__device__ __forceinline__ void bin_store(float* v, uint32_t xs_smem, uint32_t sid) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .f32 x;\n\t"
+      "setp.ne.u32 p, %0, %3;\n\t"
+      "mov.f32 x, 0f00000000;\n\t"
+      "@p ld.shared.f32 x, [%1];\n\t"
+      "@p st.global.f32 [%2], x;\n\t}" ::"r"(sid),
+      "r"(xs_smem + 4 * sid), "l"(v), "n"((uint32_t)BIN_PAD)
+      : "memory");
+}
+// Pass A of the virtual blocks, one warp per chunk of steps of one source block.  In a step of BIN_STEP positions
+// lane L stores the values of positions 32 k + L (k < 8) to their slots of V: slot = position + delta of the
+// position's run.  A run's slots are consecutive, so each of the 8 stores of a step is coalesced.  A step lies in
+// one block's share, so its runs are consecutive from r0, the first run of its first group, and the run of a
+// position is r0 plus the run starts after the step's first position up to it.  Lane L holds the delta of run
+// r0 + L and every lane takes the delta of its run from there by shuffle; a step with more than 32 runs loops over
+// 32-run windows instead.  The loads run ahead of the stores, so that no load waits on another one in the steady
+// state: while step s stores, the ids and start bits of step s + 1 are in flight, and so are its deltas, from its
+// r0, which was loaded during step s - 1.
+template <bool WIDE>
+__device__ __forceinline__ void bin_step(const PrArgs& a, uint32_t xs_smem, uint32_t p0, uint32_t lane, const uint4 id,
+                                         const uint4 b0, const uint4 b1, uint32_t r0, uint32_t d, uint32_t runs) {
+  const uint32_t bits[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+  const uint32_t w[4] = {id.x, id.y, id.z, id.w};
+  const uint32_t upto = 0xFFFFFFFFu >> (31u - lane);  // positions 0 .. lane of a group
+  uint32_t before = 0u - (bits[0] & 1u);  // run starts after the step's first position, before group k
+#pragma unroll
+  for (uint32_t k = 0; k < 8; ++k) {
+    const uint32_t r = before + __popc(bits[k] & upto);  // the position's run - r0
+    before += __popc(bits[k]);
+    uint32_t dk;
+    if (!WIDE) {
+      dk = __shfl_sync(0xFFFFFFFFu, d, r);
+    } else {
+      // a window of 32 runs at a time, the first one in d
+      dk = __shfl_sync(0xFFFFFFFFu, d, r & 31u);
+#pragma unroll 1
+      for (uint32_t w0 = 32; w0 <= runs; w0 += 32) {
+        const uint32_t t = __shfl_sync(0xFFFFFFFFu, __ldg(a.bin_runs + r0 + w0 + lane), (r - w0) & 31u);
+        if (r - w0 < 32) dk = t;
+      }
+    }
+    bin_store(a.vals + (p0 + 32 * k + dk), xs_smem, (w[k / 2] >> (16 * (k & 1))) & 0xFFFFu);
+  }
+}
 __device__ __forceinline__ void bin_chunk(const PrArgs& a, const float* xs, uint32_t c, uint32_t lane) {
-  const uint2 ch = a.bin_chunks[c];
-  const uint32_t after = (2u << lane) - 2u;  // positions 1 .. lane of the group
-#pragma unroll 4
-  for (uint32_t g = ch.x; g < ch.y; ++g) {
-    const uint32_t i = 32 * g + lane;
-    const uint32_t id = __ldg(a.bin_ids + i);
-    if (id == BIN_PAD) continue;
-    const uint2 run = __ldg(a.bin_runs + __ldg(a.bin_grun + g) + __popc(__ldg(a.bin_bits + g) & after));
-    a.vals[run.y + (i - run.x)] = xs[id];
+  constexpr uint32_t GS = BIN_STEP / 32;  // groups per step
+  const uint2 ch = a.bin_chunks[c];       // steps [ch.x, ch.y)
+  const uint32_t* ids = reinterpret_cast<const uint32_t*>(a.bin_ids) + 4 * lane;  // 128 words per step
+  const uint4* bits4 = reinterpret_cast<const uint4*>(a.bin_bits);               // 2 per step
+  const uint32_t xs_smem = (uint32_t)__cvta_generic_to_shared(xs);
+  uint4 id = ld_stream_u4(ids + 128 * (size_t)ch.x);
+  uint4 b0 = __ldg(bits4 + 2 * ch.x), b1 = __ldg(bits4 + 2 * ch.x + 1);
+  uint32_t r0 = __ldg(a.bin_grun + GS * ch.x);
+  uint32_t r0n = ch.x + 1 < ch.y ? __ldg(a.bin_grun + GS * (ch.x + 1)) : 0u;
+  uint32_t d = __ldg(a.bin_runs + r0 + lane);
+  for (uint32_t s = ch.x; s < ch.y; ++s) {
+    uint4 nid = id, nb0 = b0, nb1 = b1;
+    uint32_t nd = d, r0nn = r0n;
+    if (s + 1 < ch.y) {
+      nid = ld_stream_u4(ids + 128 * (size_t)(s + 1));
+      nb0 = __ldg(bits4 + 2 * (s + 1));
+      nb1 = __ldg(bits4 + 2 * (s + 1) + 1);
+      nd = __ldg(a.bin_runs + r0n + lane);
+      if (s + 2 < ch.y) r0nn = __ldg(a.bin_grun + GS * (s + 2));
+    }
+    // runs of the step after its first one: the run starts after its first position
+    const uint32_t runs = __popc(b0.x & ~1u) + __popc(b0.y) + __popc(b0.z) + __popc(b0.w) + __popc(b1.x) +
+                          __popc(b1.y) + __popc(b1.z) + __popc(b1.w);
+    if (runs < 32) bin_step<false>(a, xs_smem, s * BIN_STEP + lane, lane, id, b0, b1, r0, d, runs);
+    else bin_step<true>(a, xs_smem, s * BIN_STEP + lane, lane, id, b0, b1, r0, d, runs);
+    id = nid, b0 = nb0, b1 = nb1, d = nd, r0 = r0n, r0n = r0nn;
   }
 }
 
@@ -1209,6 +1269,7 @@ static void plan_stats(const PrPlan* p, gb_pr_shard_stats* stats) {
   stats->vblock_parts = p->vb ? p->v.virt.KB : 0;
   stats->vblock_pairs = p->vb ? p->v.pairs : 0;
   stats->vblock_edges = p->vb ? p->v.edges : 0;
+  stats->vblock_wide_steps = p->vb ? p->v.wide_steps : 0;
 }
 static void plan_shape(const PrPlan* p, gb_pr_plan_shape* shape) {
   shape->hot_blocks = p->hot.KB;

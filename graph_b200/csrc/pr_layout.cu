@@ -461,23 +461,35 @@ __global__ void k_vb_place(const uint64_t* __restrict__ keys, const uint32_t* __
   }
 }
 // pass A positions: pair i of source block b goes to bpos[b] + (i - bfirst[b]); runs start where (block,
-// partition) changes
+// partition) changes.  The last pair of a block also gives its run to the groups after it up to the end of its
+// step, so that the first runs of a step's groups never decrease.
 __global__ void k_bin_place(const uint64_t* __restrict__ akey, const uint32_t* __restrict__ aslot, uint32_t NP,
                             const uint32_t* __restrict__ bfirst, const uint32_t* __restrict__ bpos,
                             const uint32_t* __restrict__ brank, const uint32_t* __restrict__ run_rank,
                             uint16_t* __restrict__ ids, uint32_t* __restrict__ bits, uint32_t* __restrict__ grun,
-                            uint2* __restrict__ runs) {
+                            uint32_t* __restrict__ runs) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < NP; i += gridDim.x * blockDim.x) {
     const uint64_t key = akey[i];
     const uint32_t b = (uint32_t)(key >> VB_BLK_SHIFT);
     const uint32_t pos = bpos[brank[b]] + (i - bfirst[b]);
     const uint32_t r = run_rank[i] - 1;
-    ids[pos] = (uint16_t)(key & 0xFFFFu);
+    ids[bin_id_index(pos)] = (uint16_t)(key & 0xFFFFu);
     if (i == 0 || (akey[i - 1] >> 16) != (key >> 16)) {
       atomicOr(bits + pos / 32, 1u << (pos % 32));
-      runs[r] = make_uint2(pos, aslot[i]);
+      runs[r] = aslot[i] - pos;
     }
     if (pos % 32 == 0) grun[pos / 32] = r;
+    if (i + 1 == bfirst[b + 1])
+      for (uint32_t g = pos / 32 + 1; g < (pos / BIN_STEP + 1) * (BIN_STEP / 32); ++g) grun[g] = r;
+  }
+}
+// pass A steps whose positions touch more than 32 runs
+__global__ void k_bin_wide(const uint32_t* __restrict__ bits, const uint32_t* __restrict__ grun, uint32_t steps,
+                           uint32_t* __restrict__ count) {
+  constexpr uint32_t GS = BIN_STEP / 32;
+  for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < steps; t += gridDim.x * blockDim.x) {
+    const uint32_t g = GS * t + GS - 1;
+    if (grun[g] + __popc(bits[g] & ~1u) - grun[GS * t] >= 32) atomicAdd(count, 1u);
   }
 }
 __global__ void k_run_starts(const uint64_t* __restrict__ akey, uint32_t NP, uint32_t* __restrict__ flag) {
@@ -1184,7 +1196,7 @@ gb_status LayoutBuild::layout_vblocks() {
     GB_CUDA(cudaGetLastError());
     GB_CUDA(cudaStreamSynchronize(s));
   }
-  // pass A: the pairs by (source block, partition, source); each block's share starts at a multiple of 32
+  // pass A: the pairs by (source block, partition, source); each block's share starts at a step
   const uint32_t nblk = (uint32_t)(((uint64_t)n + B - 1) / B);
   cub::DoubleBuffer<uint64_t> akb(akey.p, akey_alt.p);
   cub::DoubleBuffer<uint32_t> asb(aslot.p, aslot_alt.p);
@@ -1209,14 +1221,14 @@ gb_status LayoutBuild::layout_vblocks() {
     h_brank[b] = j;
     h_bblk.push_back(b);
     h_bpos.push_back((uint32_t)npos);
-    const uint32_t g0 = (uint32_t)(npos / 32), g1 = g0 + (cnt + 31) / 32;
+    const uint32_t s0 = (uint32_t)(npos / BIN_STEP), s1 = s0 + (cnt + BIN_STEP - 1) / BIN_STEP;
     const uint32_t c0 = (uint32_t)h_chunks.size();
-    for (uint32_t g = g0; g < g1; g += BIN_CHUNK) h_chunks.push_back(make_uint2(g, std::min(g1, g + BIN_CHUNK)));
+    for (uint32_t t = s0; t < s1; t += BIN_CHUNK) h_chunks.push_back(make_uint2(t, std::min(s1, t + BIN_CHUNK)));
     const uint32_t nc = (uint32_t)h_chunks.size() - c0;
     for (uint32_t c = 0; c < nc; c += CB_TASK_CHUNKS)
       h_tasks.push_back(make_uint2(c0 + c, (std::min(nc, c + CB_TASK_CHUNKS) - c) | (j << 8)));
-    npos += (uint64_t)(g1 - g0) * 32;
-    GB_REQUIRE(npos < 0xFFFFFFE0ull, "too many virtual-block pairs (%llu positions)", (unsigned long long)npos);
+    npos += (uint64_t)(s1 - s0) * BIN_STEP;
+    GB_REQUIRE(npos <= 0xFFFFFF00ull, "too many virtual-block pairs (%llu positions)", (unsigned long long)npos);
   }
   v.bin_blocks = (uint32_t)h_bblk.size();
   v.bin_n_tasks = (uint32_t)h_tasks.size();
@@ -1230,10 +1242,21 @@ gb_status LayoutBuild::layout_vblocks() {
   GB_TRY(v.bin_bits.alloc(npos / 32));
   GB_CUDA(cudaMemsetAsync(v.bin_bits.p, 0, npos / 32 * 4, s));
   GB_TRY(v.bin_grun.alloc(npos / 32));
-  GB_TRY(v.bin_runs.alloc(v.n_runs));
+  GB_TRY(v.bin_runs.alloc((size_t)v.n_runs + 32));  // a step's 32-run window may reach past the last run
+  GB_CUDA(cudaMemsetAsync(v.bin_runs.p + v.n_runs, 0, 32 * 4, s));
   k_bin_place<<<grid_for(NP, 256), 256, 0, s>>>(akb.Current(), asb.Current(), NP, bfirst.p, bpos.p, brank.p,
                                                 run_rank.p, v.bin_ids.p, v.bin_bits.p, v.bin_grun.p, v.bin_runs.p);
   GB_CUDA(cudaGetLastError());
+  {
+    DevBuf<uint32_t> wide;
+    GB_TRY(wide.alloc(1));
+    GB_CUDA(cudaMemsetAsync(wide.p, 0, 4, s));
+    const uint32_t steps = (uint32_t)(npos / BIN_STEP);
+    k_bin_wide<<<grid_for(steps, 256), 256, 0, s>>>(v.bin_bits.p, v.bin_grun.p, steps, wide.p);
+    GB_CUDA(cudaGetLastError());
+    GB_CUDA(cudaMemcpyAsync(&v.wide_steps, wide.p, 4, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaStreamSynchronize(s));
+  }
   // pass B's chunks and tasks over the virtual blocks (rows [row0[k], row0[k + 1]) each)
   GB_TRY(cb_chunk_table(s, dev_sms, B, goffv.p, h_min, &vs));
   GB_REQUIRE(vs.n_fix == 0, "a virtual-block segment is cut by a chunk boundary");

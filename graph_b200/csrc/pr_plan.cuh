@@ -37,7 +37,13 @@ constexpr uint32_t CB_HEAD_CONT = 1u, CB_TAIL_CONT = 2u, CB_INTERIOR = 4u;
 
 constexpr uint32_t VB_ALIGN = 32;            // virtual blocks start at multiples of 32 slots of V (128-byte lines)
 constexpr uint16_t BIN_PAD = 0xFFFFu;        // pass A: a position that holds no pair (B < 2^16 - 1)
-constexpr uint32_t BIN_CHUNK = 32;           // pass A: 32-position groups per chunk (1024 pairs, one warp)
+constexpr uint32_t BIN_STEP = 256;           // pass A: positions per warp step (8 groups of 32, 8 per lane)
+constexpr uint32_t BIN_CHUNK = 8;            // pass A: steps per chunk (2048 positions, one warp)
+// pass A: where the id of position pos is stored.  Inside a step, position 32 k + L sits at 8 L + k, so that lane L
+// reads its positions L, L + 32, .., L + 224 with one 128-bit load
+__host__ __device__ __forceinline__ uint32_t bin_id_index(uint32_t pos) {
+  return (pos & ~(BIN_STEP - 1)) | (pos & 31u) << 3 | (pos >> 5 & 7u);
+}
 
 // ---- the cyclic deal of 32-row slices over the ranks of the 1-D edge-cut ---------------------------
 struct PrDeal {
@@ -97,14 +103,15 @@ struct CbStream {
 struct PrVBlocks {
   uint64_t pairs = 0, edges = 0;  // (source, partition) pairs and the cold edges they serve
   uint32_t bin_blocks = 0, n_runs = 0;
+  uint32_t wide_steps = 0;      // pass A steps whose positions touch more than 32 runs (the run-window loop)
   DevBuf<float> val;            // V
   // pass A: the pairs in (source block, partition, source) order, each block's share starting at a multiple of
-  // 32 positions (BIN_PAD in between); a RUN is the pairs of one (block, partition), consecutive slots of V
-  DevBuf<uint16_t> bin_ids;     // block-local source id at every position
+  // BIN_STEP positions (BIN_PAD in between); a RUN is the pairs of one (block, partition), consecutive slots of V
+  DevBuf<uint16_t> bin_ids;     // block-local source id of every position, at bin_id_index(position)
   DevBuf<uint32_t> bin_bits;    // per 32 positions: bit i set <=> position 32 g + i starts a run
-  DevBuf<uint32_t> bin_grun;    // per 32 positions: the run of position 32 g
-  DevBuf<uint2> bin_runs;       // [n_runs] (first position of the run, its first V slot)
-  DevBuf<uint2> bin_chunks;     // [32-position groups g0, g1) of one block: a warp's unit of pass A
+  DevBuf<uint32_t> bin_grun;    // per 32 positions: the last run that starts at or before position 32 g
+  DevBuf<uint32_t> bin_runs;    // [n_runs + 32] first V slot - first position of each run (mod 2^32); 32 spare
+  DevBuf<uint2> bin_chunks;     // [steps s0, s1) of one block: a warp's unit of pass A
   DevBuf<uint32_t> bin_blk;     // [bin_blocks] source block of each of pass A's block ranks
   DevBuf<uint2> bin_tasks;      // (first chunk, chunk count | block rank << 8)
   uint32_t bin_n_tasks = 0;

@@ -457,6 +457,8 @@ typedef struct gb_pr_shard_stats {
   uint32_t vblock_parts;       /* row partitions = virtual blocks */
   uint64_t vblock_pairs;       /* distinct (source, partition) pairs = slots of the value buffer */
   uint64_t vblock_edges;       /* edges reduced through the virtual blocks */
+  uint32_t vblock_wide_steps;  /* 256-position steps of the virtual blocks' pass A whose positions fall in more than
+                                  32 runs: every sweep finds their slots through the slower run-window loop */
 } gb_pr_shard_stats;
 
 /* the reference's own partitioner on the ORIGINAL ids: in_degree_partition (graph_ops.rs:431-439,

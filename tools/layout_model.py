@@ -245,6 +245,14 @@ def check(plan, got, in_off, in_tgt):
 VB_ALIGN = 32
 VB_BLK_SHIFT = 43
 BIN_PAD = 0xFFFF
+BIN_STEP = 256   # pass A positions per warp step: 8 groups of 32
+BIN_CHUNK = 8    # pass A steps per chunk
+
+
+def bin_id_index(pos):
+    """where pass A stores the id of position pos: 32 k + L of a step at 8 L + k"""
+    pos = np.asarray(pos, np.int64)
+    return (pos & ~(BIN_STEP - 1)) | (pos & 31) << 3 | (pos >> 5 & 7)
 
 
 def cold_lens(plan, in_off, in_tgt):
@@ -333,7 +341,7 @@ def vblocks(plan, built):
     ids = np.full(int(goffv[-1]) * CB_G, B, np.int64)
     e = order
     ids[goffv[rows[e]] * CB_G + (e - coff[rows[e]])] = rank - pfirst[sk >> 32]
-    # pass A: the pairs by (source block, partition, source), each block's share at a multiple of 32 positions
+    # pass A: the pairs by (source block, partition, source), each block's share starting at a step
     psrc, ppart = sk[start] & 0xFFFFFFFF, sk[start] >> 32
     pslot = vbase[ppart] + np.arange(NP) - pfirst[ppart]
     akey = ((psrc // B) << VB_BLK_SHIFT) | (ppart << 16) | (psrc % B)
@@ -341,42 +349,76 @@ def vblocks(plan, built):
     akey, aslot = akey[ao], pslot[ao]
     blk = akey >> VB_BLK_SHIFT
     bcnt = np.bincount(blk, minlength=plan["nblk"])
-    bpos = np.concatenate([[0], np.cumsum((bcnt + 31) // 32 * 32)])
+    bsteps = (bcnt + BIN_STEP - 1) // BIN_STEP
+    bpos = np.concatenate([[0], np.cumsum(bsteps * BIN_STEP)])
     bfirst = np.concatenate([[0], np.cumsum(bcnt)])
     pos = bpos[blk] + np.arange(NP) - bfirst[blk]
     npos = int(bpos[-1])
     bin_ids = np.full(npos, BIN_PAD, np.int64)
-    bin_ids[pos] = akey & 0xFFFF
+    bin_ids[bin_id_index(pos)] = akey & 0xFFFF
     rstart = np.r_[True, (akey[1:] >> 16) != (akey[:-1] >> 16)]
-    run = np.cumsum(rstart) - 1
     bin_bits = np.zeros(npos // 32, np.int64)
     np.bitwise_or.at(bin_bits, pos[rstart] // 32, 1 << (pos[rstart] % 32))
-    bin_grun = np.zeros(npos // 32, np.int64)
-    first = pos % 32 == 0
-    bin_grun[pos[first] // 32] = run[first]
-    bin_runs = np.stack([pos[rstart], aslot[rstart]], axis=1)
+    # the last run that starts at or before each group's first position
+    bin_grun = np.searchsorted(pos[rstart], np.arange(0, npos, 32), side="right") - 1
+    bin_runs = (aslot[rstart] - pos[rstart]) & 0xFFFFFFFF                     # first slot - first position
     pos_blk = np.repeat(np.arange(plan["nblk"]), np.diff(bpos))              # source block of every position
+    s0 = bpos[:-1] // BIN_STEP
+    bin_chunks = np.array([(t, min(t + BIN_CHUNK, s0[b] + bsteps[b])) for b in np.flatnonzero(bcnt)
+                           for t in range(s0[b], s0[b] + bsteps[b], BIN_CHUNK)], np.int64).reshape(-1, 2)
     return dict(parts=parts, row0=row0, mseg=mseg, vbase=vbase, pairs=NP, edges=int(lens.sum()), lens=lens,
                 goffv=goffv, ids=ids, bin_ids=bin_ids, bin_bits=bin_bits, bin_grun=bin_grun, bin_runs=bin_runs,
-                pos_blk=pos_blk)
+                bin_chunks=bin_chunks, pos_blk=pos_blk, bcnt=bcnt, run_pos=pos[rstart])
 
 
 def vb_pass_a(plan, vb):
-    """pass A (k_pr_cb<CB_BIN> / bin_chunk): the source of every slot of V it writes, and how often it writes it"""
+    """pass A (k_pr_cb<CB_BIN> / bin_chunk), chunk by chunk, step by step, lane by lane: the source of every slot
+    of V it writes, how often it writes it, and the steps that take the run-window loop (more than 32 runs)"""
     B = plan["B"]
     V = np.full(int(vb["vbase"][-1]), -1, np.int64)
     writes = np.zeros(len(V), np.int64)
-    for i, sid in enumerate(vb["bin_ids"]):
-        if sid == BIN_PAD:
-            continue
-        g, lane = i // 32, i % 32
-        after = ((2 << lane) - 2) & 0xFFFFFFFF
-        r = int(vb["bin_grun"][g]) + bin(int(vb["bin_bits"][g]) & after).count("1")
-        p0, s0 = vb["bin_runs"][r]
-        slot = int(s0) + i - int(p0)
-        V[slot] = int(vb["pos_blk"][i]) * B + int(sid)
-        writes[slot] += 1
-    return V, writes
+    wide = []
+    gs = BIN_STEP // 32
+    lanes = np.arange(32)
+    upto = (2 << lanes) - 1                                                   # positions 0 .. lane of a group
+    popc = lambda x: np.array([bin(int(v)).count("1") for v in np.atleast_1d(x)])
+    for s0, s1 in vb["bin_chunks"]:
+        for s in range(int(s0), int(s1)):
+            bits = vb["bin_bits"][gs * s:gs * s + gs]
+            r0 = int(vb["bin_grun"][gs * s])
+            ids = vb["bin_ids"][s * BIN_STEP:(s + 1) * BIN_STEP].reshape(32, 8)  # lane L's 128-bit load
+            runs = int(popc(bits).sum()) - int(bits[0] & 1)                   # run starts after the first position
+            if runs >= 32:
+                wide.append(s)
+            before = -int(bits[0] & 1)
+            for k in range(gs):
+                r = r0 + before + popc(bits[k] & upto)                        # every lane's run
+                before += int(popc(bits[k])[0])
+                p = s * BIN_STEP + 32 * k + lanes
+                slot = (p + vb["bin_runs"][r]) & 0xFFFFFFFF
+                sid = ids[:, k]
+                ok = sid != BIN_PAD
+                V[slot[ok]] = vb["pos_blk"][p[ok]] * B + sid[ok]
+                np.add.at(writes, slot[ok], 1)
+    return V, writes, wide
+
+
+def vb_pass_a_cases(vb):
+    """what a fixture's pass A layout reaches: steps with more than 32 runs, block shares shorter than a step,
+    runs that cross a step boundary and a chunk boundary, and pad positions"""
+    # a run's positions: from its first one to the next run's first or to its block's last pair
+    bcnt = vb["bcnt"][vb["bcnt"] > 0]
+    share = (bcnt + BIN_STEP - 1) // BIN_STEP * BIN_STEP
+    share_end = np.cumsum(share) - share + bcnt                               # one past each block's last pair
+    first = vb["run_pos"]
+    nxt = np.r_[first[1:], np.iinfo(np.int64).max]
+    last = np.minimum(nxt, share_end[np.searchsorted(share_end, first, side="right")]) - 1
+    chunk_start = vb["bin_chunks"][:, 0] * BIN_STEP
+    cross_chunk = np.searchsorted(chunk_start, last, side="right") > np.searchsorted(chunk_start, first, side="right")
+    return dict(short_shares=int((bcnt < BIN_STEP).sum()),
+                step_runs=int((first // BIN_STEP != last // BIN_STEP).sum()),
+                chunk_runs=int(cross_chunk.sum()),
+                pads=int((vb["bin_ids"] == BIN_PAD).sum()))
 
 
 def check_vblocks(plan, vb, built):
@@ -384,7 +426,7 @@ def check_vblocks(plan, vb, built):
     virtual blocks), every cold edge appears exactly once in pass B, and every pass B id resolves to the slot
     of its edge's source; no virtual block holds more than B slots"""
     B = plan["B"]
-    V, writes = vb_pass_a(plan, vb)
+    V, writes, _ = vb_pass_a(plan, vb)
     for k in range(vb["parts"]):
         lo, hi = int(vb["vbase"][k]), int(vb["vbase"][k + 1])
         used = writes[lo:hi] > 0
