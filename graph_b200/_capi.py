@@ -49,7 +49,7 @@ class PrShardStats(C.Structure):
                 ("cut_segments", C.c_uint32), ("chunk_groups", C.c_uint32),
                 ("launches_per_sweep", C.c_uint32), ("device_bytes", C.c_uint64),
                 ("vblock_parts", C.c_uint32), ("vblock_pairs", C.c_uint64), ("vblock_edges", C.c_uint64),
-                ("vblock_wide_steps", C.c_uint32)]
+                ("vblock_wide_steps", C.c_uint32), ("vblock_slots", C.c_uint64), ("vblock_sectors", C.c_uint32)]
 
     def as_dict(self):
         return {k: int(getattr(self, k)) for k, _ in self._fields_}
@@ -159,6 +159,7 @@ SIGNATURES = {
     "gb_in_degree_partition": (C.c_int, [_P, C.c_uint32, _P]),
     "gb_page_rank_plan_info": (C.c_int, [_P, C.POINTER(PrShardStats)]),
     "gb_page_rank_plan_shape": (C.c_int, [_P, C.POINTER(PrPlanShape)]),
+    "gb_page_rank_plan_values": (C.c_int, [_P, C.c_int, _P, C.c_uint64]),
     "gb_page_rank_plan_reset": (C.c_int, [_P]),
     "gb_pr_shard_create": (C.c_int, [_P, C.c_uint32, C.c_uint32, C.POINTER(_P)]),
     "gb_pr_shard_info": (C.c_int, [_P, C.POINTER(PrShardStats)]),

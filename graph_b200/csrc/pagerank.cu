@@ -142,6 +142,7 @@ struct PrArgs {
   const uint32_t* bin_grun;
   const uint32_t* bin_runs;
   const uint2* bin_chunks;
+  uint32_t bin_fill;    // runs start on 32-byte sectors of V: zero each run's pad slots (PrVBlocks::sectors)
   // SELL rows
   const uint4* sell;
   const uint2* slice_meta;
@@ -363,6 +364,16 @@ __device__ __forceinline__ void bin_store(float* v, uint32_t xs_smem, uint32_t s
       "r"(xs_smem + 4 * sid), "l"(v), "n"((uint32_t)BIN_PAD)
       : "memory");
 }
+// V[e .. e rounded up to VB_RUN_ALIGN) = 0: the pad slots after a run, with at most one 4-, one 8- and one 16-byte
+// store, so that the run's last 32-byte sector is written whole in the step that stores the run's last value
+__device__ __forceinline__ void bin_fill_pad(float* v, uint32_t e) {
+  if (e & 1u) v[e++] = 0.0f;
+  if (e & 2u) {
+    *reinterpret_cast<float2*>(v + e) = make_float2(0.0f, 0.0f);
+    e += 2;
+  }
+  if (e & 4u) *reinterpret_cast<float4*>(v + e) = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+}
 // Pass A of the virtual blocks, one warp per chunk of steps of one source block.  In a step of BIN_STEP positions
 // lane L stores the values of positions 32 k + L (k < 8) to their slots of V: slot = position + delta of the
 // position's run.  A run's slots are consecutive, so each of the 8 stores of a step is coalesced.  A step lies in
@@ -372,13 +383,23 @@ __device__ __forceinline__ void bin_store(float* v, uint32_t xs_smem, uint32_t s
 // 32-run windows instead.  The loads run ahead of the stores, so that no load waits on another one in the steady
 // state: while step s stores, the ids and start bits of step s + 1 are in flight, and so are its deltas, from its
 // r0, which was loaded during step s - 1.
-template <bool WIDE>
+// FILL (sector-aligned runs): the lane of a run's last position also zeroes the run's pad slots.  A run ends where
+// the next position starts a run (nbit: the first position of the next step) or is a pad; the pads of a step
+// follow its valid positions, so the step's last valid position is where they begin.
+template <bool WIDE, bool FILL>
 __device__ __forceinline__ void bin_step(const PrArgs& a, uint32_t xs_smem, uint32_t p0, uint32_t lane, const uint4 id,
-                                         const uint4 b0, const uint4 b1, uint32_t r0, uint32_t d, uint32_t runs) {
-  const uint32_t bits[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+                                         const uint4 b0, const uint4 b1, uint32_t nbit, uint32_t r0, uint32_t d,
+                                         uint32_t runs) {
+  const uint32_t bits[9] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w, nbit};
   const uint32_t w[4] = {id.x, id.y, id.z, id.w};
   const uint32_t upto = 0xFFFFFFFFu >> (31u - lane);  // positions 0 .. lane of a group
   uint32_t before = 0u - (bits[0] & 1u);  // run starts after the step's first position, before group k
+  uint32_t nvalid = 0;                    // FILL: the step's positions that hold a pair
+  if (FILL) {
+#pragma unroll
+    for (uint32_t k = 0; k < 8; ++k)
+      nvalid += __popc(__ballot_sync(0xFFFFFFFFu, ((w[k / 2] >> (16 * (k & 1))) & 0xFFFFu) != BIN_PAD));
+  }
 #pragma unroll
   for (uint32_t k = 0; k < 8; ++k) {
     const uint32_t r = before + __popc(bits[k] & upto);  // the position's run - r0
@@ -395,9 +416,17 @@ __device__ __forceinline__ void bin_step(const PrArgs& a, uint32_t xs_smem, uint
         if (r - w0 < 32) dk = t;
       }
     }
-    bin_store(a.vals + (p0 + 32 * k + dk), xs_smem, (w[k / 2] >> (16 * (k & 1))) & 0xFFFFu);
+    const uint32_t sid = (w[k / 2] >> (16 * (k & 1))) & 0xFFFFu;
+    bin_store(a.vals + (p0 + 32 * k + dk), xs_smem, sid);
+    if (FILL) {
+      const uint32_t q = 32 * k + lane;  // the position in the step
+      const bool last = sid != BIN_PAD && (((__funnelshift_rc(bits[k], bits[k + 1], lane + 1) & 1u) != 0) ||
+                                           (q + 1 == nvalid && nvalid < BIN_STEP));
+      if (last) bin_fill_pad(a.vals, p0 + 32 * k + dk + 1);
+    }
   }
 }
+template <bool FILL>
 __device__ __forceinline__ void bin_chunk(const PrArgs& a, const float* xs, uint32_t c, uint32_t lane) {
   constexpr uint32_t GS = BIN_STEP / 32;  // groups per step
   const uint2 ch = a.bin_chunks[c];       // steps [ch.x, ch.y)
@@ -419,11 +448,13 @@ __device__ __forceinline__ void bin_chunk(const PrArgs& a, const float* xs, uint
       nd = __ldg(a.bin_runs + r0n + lane);
       if (s + 2 < ch.y) r0nn = __ldg(a.bin_grun + GS * (s + 2));
     }
+    // FILL: the start bits of the next step's first 32 positions (past the last step: a run start)
+    const uint32_t nbit = !FILL ? 0u : s + 1 < ch.y ? nb0.x : __ldg(a.bin_bits + 8 * (s + 1));
     // runs of the step after its first one: the run starts after its first position
     const uint32_t runs = __popc(b0.x & ~1u) + __popc(b0.y) + __popc(b0.z) + __popc(b0.w) + __popc(b1.x) +
                           __popc(b1.y) + __popc(b1.z) + __popc(b1.w);
-    if (runs < 32) bin_step<false>(a, xs_smem, s * BIN_STEP + lane, lane, id, b0, b1, r0, d, runs);
-    else bin_step<true>(a, xs_smem, s * BIN_STEP + lane, lane, id, b0, b1, r0, d, runs);
+    if (runs < 32) bin_step<false, FILL>(a, xs_smem, s * BIN_STEP + lane, lane, id, b0, b1, nbit, r0, d, runs);
+    else bin_step<true, FILL>(a, xs_smem, s * BIN_STEP + lane, lane, id, b0, b1, nbit, r0, d, runs);
     id = nid, b0 = nb0, b1 = nb1, d = nd, r0 = r0n, r0n = r0nn;
   }
 }
@@ -575,7 +606,10 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
     // a warp starts with chunk `warp` of the task and claims further ones from the CTA's counter
     const uint32_t nchunks = task.y & 0xFFu;
     for (uint32_t k = warp; k < nchunks;) {
-      if (KIND == CB_BIN) bin_chunk(a, xs, task.x + k, lane);
+      if (KIND == CB_BIN) {
+        if (a.bin_fill) bin_chunk<true>(a, xs, task.x + k, lane);
+        else bin_chunk<false>(a, xs, task.x + k, lane);
+      }
       else cb_chunk(a, xs, task.x + k, lane, pad2);
       uint32_t nx = 0;
       if (lane == 0) nx = atomicAdd(&s_next, 1u);
@@ -929,14 +963,41 @@ __global__ void __launch_bounds__(32) k_pr_exact(const uint32_t* __restrict__ in
   }
 }
 
+// The dynamic shared memory k_pr_cb<KIND> can take on `device`: the per-block opt-in limit less its static
+// shared memory
+template <uint32_t KIND>
+static gb_status cb_smem_limit(int device, size_t* bytes) {
+  int optin = 0;
+  GB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+  cudaFuncAttributes fa{};
+  GB_CUDA(cudaFuncGetAttributes(&fa, k_pr_cb<KIND>));
+  *bytes = (size_t)optin - fa.sharedSizeBytes;
+  return GB_OK;
+}
+// cudaFuncAttributeMaxDynamicSharedMemorySize belongs to the kernel, for the whole process, and every plan's
+// launches need it at least as large as their own shared memory (smem_cb, smem_vb).  So it is set to the
+// device's limit, not to the plan's size: a plan built later (another B, another window of V) never lowers it
+// below what an earlier plan, still cached, launches with.
+template <uint32_t KIND>
+static gb_status cb_smem_ceiling(int device, size_t need) {
+  size_t lim = 0;
+  GB_TRY(cb_smem_limit<KIND>(device, &lim));
+  GB_REQUIRE(need <= lim, "k_pr_cb needs %zu bytes of shared memory, the device allows %zu", need, lim);
+  GB_CUDA(cudaFuncSetAttribute(k_pr_cb<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lim));
+  return GB_OK;
+}
+
 // ---- launch shapes: the last stage of the layout build --------------------------------------------
 gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, const std::vector<uint32_t>& h_poff,
                            int dev_sms, cudaStream_t s) {
   p->trace = (uint32_t)env_u64("GB_PR_TRACE", 0) != 0;
   p->smem_cb = ((size_t)p->B + 4) * sizeof(float);
-  GB_CUDA(cudaFuncSetAttribute(k_pr_cb<CB_MAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cb));
-  GB_CUDA(cudaFuncSetAttribute(k_pr_cb<CB_VIRT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cb));
-  GB_CUDA(cudaFuncSetAttribute(k_pr_cb<CB_BIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_cb));
+  p->smem_vb = p->vb ? ((size_t)p->v.window + 4) * sizeof(float) : p->smem_cb;
+  int dev = 0;
+  GB_CUDA(cudaGetDevice(&dev));
+  GB_TRY(cb_smem_ceiling<CB_MAIN>(dev, p->smem_cb));
+  GB_TRY(cb_smem_ceiling<CB_VIRT>(dev, p->smem_vb));
+  GB_TRY(cb_smem_ceiling<CB_BIN>(dev, p->smem_cb));
   const uint64_t want_sell = ((uint64_t)p->num_slices + PR_SELL_THREADS / 32 - 1) / (PR_SELL_THREADS / 32);
   p->grid_sell = (unsigned)std::min<uint64_t>(want_sell, (uint64_t)dev_sms * 2);
   // rows with segments in more than SELL_FEW blocks are a prefix (nrows[] is non-increasing): k_pr_finish
@@ -987,6 +1048,18 @@ gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, cons
   GB_TRY(p->ctrl.alloc(2));
   GB_CUDA(cudaMemsetAsync(p->ctrl.p, 0, 8, s));
   GB_CUDA(cudaStreamSynchronize(s));
+  return GB_OK;
+}
+
+gb_status pr_vb_window(int device, uint32_t* window) {
+  size_t lim = 0;
+  GB_TRY(cb_smem_limit<CB_VIRT>(device, &lim));
+  uint32_t W = (uint32_t)(lim / sizeof(float) - 4) / VB_ALIGN * VB_ALIGN;
+  // pass B's ids are 16-bit: every V-local slot and the pad id W itself stay below 0xFFFF
+  W = std::min<uint32_t>(W, 0xFFFFu & ~(VB_ALIGN - 1));
+  const uint64_t force = env_u64("GB_PR_VB_WINDOW", 0);
+  if (force) W = (uint32_t)std::min<uint64_t>(W, force / VB_ALIGN * VB_ALIGN);
+  *window = W;
   return GB_OK;
 }
 
@@ -1047,11 +1120,14 @@ static PrArgs pass_a_args(const PrPlan* p, PrArgs a) {
   a.bin_grun = v.bin_grun.p;
   a.bin_runs = v.bin_runs.p;
   a.bin_chunks = v.bin_chunks.p;
+  a.bin_fill = v.sectors ? 1u : 0u;
   return a;
 }
-// pass B: the virtual blocks' stream, over V; its partials are the rows' cold sums (k_pr_finish's rem)
+// pass B: the virtual blocks' stream, over V, in blocks of its window; its partials are the rows' cold sums
+// (k_pr_finish's rem)
 static PrArgs pass_b_args(const PrPlan* p, PrArgs a) {
   a.x_cur = p->v.val.p;
+  a.B = p->v.window;
   a.sched = sched_of(p->v.virt, p->task_ctr.p + p->grid_cb + p->grid_bin);
   a.walk = walk_of(p->v.virt);
   return a;
@@ -1088,7 +1164,7 @@ static gb_status launch_sweep(const PrPlan* p, const PrArgs& a, cudaStream_t s, 
     *launches += 1;
   }
   if (p->vb) {
-    k_pr_cb<CB_VIRT><<<p->grid_vb, PR_THREADS, p->smem_cb, s>>>(pass_b_args(p, a));
+    k_pr_cb<CB_VIRT><<<p->grid_vb, PR_THREADS, p->smem_vb, s>>>(pass_b_args(p, a));
     *launches += 1;
   }
   if (ev) GB_CUDA(cudaEventRecord(ev[3], s));
@@ -1270,6 +1346,8 @@ static void plan_stats(const PrPlan* p, gb_pr_shard_stats* stats) {
   stats->vblock_pairs = p->vb ? p->v.pairs : 0;
   stats->vblock_edges = p->vb ? p->v.edges : 0;
   stats->vblock_wide_steps = p->vb ? p->v.wide_steps : 0;
+  stats->vblock_slots = p->vb ? p->v.slots : 0;
+  stats->vblock_sectors = p->vb && p->v.sectors ? 1u : 0u;
 }
 static void plan_shape(const PrPlan* p, gb_pr_plan_shape* shape) {
   shape->hot_blocks = p->hot.KB;
@@ -1459,6 +1537,24 @@ gb_status gb_page_rank_plan_info(const gb_graph* g, gb_pr_shard_stats* stats) {
   std::lock_guard<std::mutex> lock(g->mu);
   GB_TRY(gb::ensure_plan(g));
   gb::plan_stats(g->pr_plan, stats);
+  return GB_OK;
+}
+
+gb_status gb_page_rank_plan_values(const gb_graph* g, int poison, float* values, uint64_t count) {
+  GB_REQUIRE(g, "NULL argument");
+  if (g->kind != GB_KIND_DIRECTED) return gb::fail(GB_ERR_UNSUPPORTED, "page rank needs a directed graph");
+  gb::DeviceGuard guard(g->device);
+  std::lock_guard<std::mutex> lock(g->mu);
+  GB_TRY(gb::ensure_plan(g));
+  const gb::PrVBlocks& v = g->pr_plan->v;
+  GB_REQUIRE(g->pr_plan->vb, "the layout has no virtual blocks");
+  GB_REQUIRE(count == v.slots, "count %llu is not the value buffer's %llu slots", (unsigned long long)count,
+             (unsigned long long)v.slots);
+  if (poison) {
+    GB_CUDA(cudaMemsetAsync(v.val.p, 0xFF, v.slots * sizeof(float), 0));
+    GB_CUDA(cudaStreamSynchronize(0));
+  }
+  if (values) GB_CUDA(cudaMemcpy(values, v.val.p, v.slots * sizeof(float), cudaMemcpyDeviceToHost));
   return GB_OK;
 }
 

@@ -440,18 +440,51 @@ __global__ void k_vb_bounds(const uint64_t* __restrict__ keys, const uint32_t* _
     first[k] = lo < E ? (rank ? rank[lo] - 1 : lo) : total;
   }
 }
+// Sector-aligned slots of V.  A run is the pairs of one source block inside one partition (the sorted keys are
+// (partition, source), so a run is where neither the partition nor source / B changes).  flag[pair] = 1 where a
+// run starts; its inclusive scan is every pair's run rank
+__global__ void k_vb_run_flags(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ rank, uint32_t E,
+                               uint32_t B, uint32_t* __restrict__ flag) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < E; i += gridDim.x * blockDim.x) {
+    const uint64_t key = keys[i];
+    if (i > 0 && keys[i - 1] == key) continue;
+    const uint64_t prev = i > 0 ? keys[i - 1] : 0;
+    flag[rank[i] - 1] = i == 0 || (prev >> 32) != (key >> 32) || (uint32_t)prev / B != (uint32_t)key / B ? 1u : 0u;
+  }
+}
+// rfirst[r] = first pair of run r
+__global__ void k_vb_run_first(const uint32_t* __restrict__ rrank, uint32_t NP, uint32_t* __restrict__ rfirst) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < NP; i += gridDim.x * blockDim.x)
+    if (i == 0 || rrank[i] != rrank[i - 1]) rfirst[rrank[i] - 1] = i;
+}
+// every run's length rounded up to VB_RUN_ALIGN slots (its exclusive scan: each run's first slot)
+__global__ void k_vb_run_slots(const uint32_t* __restrict__ rfirst, uint32_t NR, uint32_t NP, uint32_t* __restrict__ len) {
+  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < NR; r += gridDim.x * blockDim.x)
+    len[r] = ((r + 1 < NR ? rfirst[r + 1] : NP) - rfirst[r] + VB_RUN_ALIGN - 1) / VB_RUN_ALIGN * VB_RUN_ALIGN;
+}
+// the run rank of every pair becomes its slot: its run's first slot + its place in the run
+__global__ void k_vb_run_pos(uint32_t* __restrict__ rrank, uint32_t NP, const uint32_t* __restrict__ rfirst,
+                             const uint32_t* __restrict__ roff) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < NP; i += gridDim.x * blockDim.x) {
+    const uint32_t r = rrank[i] - 1;
+    rrank[i] = roff[r] + (i - rfirst[r]);
+  }
+}
 // every cold edge (sorted by pair): its V-local slot id into its row's segment of pass B; the first edge of every
 // pair also leaves the pair's pass A key (source block << 43 | partition << 16 | block-local source) and V slot
 constexpr uint32_t VB_BLK_SHIFT = 43;
+// every pair's slot: gpos[pair] when the runs start on sectors, else the pair itself (packed), minus first[k], the
+// slot of partition k's first pair
 __global__ void k_vb_place(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ idx,
                            const uint32_t* __restrict__ rank, uint32_t E, const uint32_t* __restrict__ erow,
                            const uint32_t* __restrict__ coff, const uint32_t* __restrict__ goffv,
-                           const uint32_t* __restrict__ pfirst, const uint32_t* __restrict__ vbase, uint32_t B,
-                           uint16_t* __restrict__ ids, uint64_t* __restrict__ akey, uint32_t* __restrict__ aslot) {
+                           const uint32_t* __restrict__ gpos, const uint32_t* __restrict__ first,
+                           const uint32_t* __restrict__ vbase, uint32_t B, uint16_t* __restrict__ ids,
+                           uint64_t* __restrict__ akey, uint32_t* __restrict__ aslot) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < E; i += gridDim.x * blockDim.x) {
     const uint64_t key = keys[i];
     const uint32_t k = (uint32_t)(key >> 32), src = (uint32_t)key;
-    const uint32_t pair = rank[i] - 1, slot = pair - pfirst[k];
+    const uint32_t pair = rank[i] - 1, slot = (gpos ? gpos[pair] : pair) - first[k];
     const uint32_t e = idx[i], l = erow[e];
     ids[(uint64_t)goffv[l] * CB_G + (e - coff[l])] = (uint16_t)slot;
     if (i == 0 || keys[i - 1] != key) {
@@ -1151,7 +1184,6 @@ gb_status LayoutBuild::layout_vblocks() {
   GB_CUDA(cudaMemcpyAsync(&ngv, goffv.p + n_loc, 4, cudaMemcpyDeviceToHost, s));
   GB_CUDA(cudaStreamSynchronize(s));
   vs.NG = ngv;
-  GB_TRY(cb_stream_ids(s, B, goffv.p, &vs));
   // the cold edges sorted by (partition, source): a run of equal keys is one pair, one slot of V
   const uint32_t Ec = (uint32_t)E;
   uint32_t NP = 0;
@@ -1180,9 +1212,47 @@ gb_status LayoutBuild::layout_vblocks() {
     std::vector<uint32_t> h_pfirst(parts + 1);
     GB_CUDA(cudaMemcpyAsync(h_pfirst.data(), pfirst.p, (size_t)(parts + 1) * 4, cudaMemcpyDeviceToHost, s));
     GB_CUDA(cudaStreamSynchronize(s));
+    // the slots with every run on a 32-byte sector (PrVBlocks::sectors), kept when every padded partition fits in
+    // pass B's largest window; else the packed slots (the pair itself) and a window of B
+    uint32_t W = 0;
+    GB_TRY(pr_vb_window(src.device, &W));
+    // every pair's padded slot (NP + 1 words: the total last) in the sort's spare key buffer (2 Ec words, free
+    // once the keys are sorted), so that the build's peak memory does not grow; every partition's first slot
+    uint32_t* gpos = reinterpret_cast<uint32_t*>(kb.Alternate());
+    DevBuf<uint32_t> gfirst;
+    std::vector<uint32_t> h_first = h_pfirst;
+    {
+      DevBuf<uint32_t> rfirst, roff;
+      k_vb_run_flags<<<grid_for(Ec, 256), 256, 0, s>>>(kb.Current(), rank.p, Ec, B, gpos);
+      GB_TRY(scan_inclusive(s, gpos, NP));
+      uint32_t NR = 0;
+      GB_CUDA(cudaMemcpyAsync(&NR, gpos + NP - 1, 4, cudaMemcpyDeviceToHost, s));
+      GB_CUDA(cudaStreamSynchronize(s));
+      if ((uint64_t)NP + (uint64_t)(VB_RUN_ALIGN - 1) * NR < 0x7FFFFFFFull) {
+        GB_TRY(rfirst.alloc(NR));
+        GB_TRY(roff.alloc((size_t)NR + 1));
+        k_vb_run_first<<<grid_for(NP, 256), 256, 0, s>>>(gpos, NP, rfirst.p);
+        k_vb_run_slots<<<grid_for(NR, 256), 256, 0, s>>>(rfirst.p, NR, NP, roff.p);
+        GB_CUDA(cudaMemsetAsync(roff.p + NR, 0, 4, s));
+        GB_TRY(scan_exclusive(s, roff.p, (uint64_t)NR + 1));
+        k_vb_run_pos<<<grid_for(NP, 256), 256, 0, s>>>(gpos, NP, rfirst.p, roff.p);
+        GB_CUDA(cudaMemcpyAsync(gpos + NP, roff.p + NR, 4, cudaMemcpyDeviceToDevice, s));
+        GB_TRY(gfirst.alloc((size_t)parts + 1));
+        k_gather_u32<<<grid_for(parts + 1, 128), 128, 0, s>>>(gpos, pfirst.p, parts + 1, gfirst.p);
+        GB_CUDA(cudaGetLastError());
+        std::vector<uint32_t> h_gfirst(parts + 1);
+        GB_CUDA(cudaMemcpyAsync(h_gfirst.data(), gfirst.p, (size_t)(parts + 1) * 4, cudaMemcpyDeviceToHost, s));
+        GB_CUDA(cudaStreamSynchronize(s));
+        v.sectors = true;
+        for (uint32_t k = 0; k < parts; ++k) v.sectors = v.sectors && h_gfirst[k + 1] - h_gfirst[k] <= W;
+        if (v.sectors) h_first = h_gfirst;
+      }
+    }
+    v.window = v.sectors ? W : B;
     std::vector<uint32_t> h_vbase(parts + 1, 0);
     for (uint32_t k = 0; k < parts; ++k)
-      h_vbase[k + 1] = h_vbase[k] + (h_pfirst[k + 1] - h_pfirst[k] + VB_ALIGN - 1) / VB_ALIGN * VB_ALIGN;
+      h_vbase[k + 1] = h_vbase[k] + (h_first[k + 1] - h_first[k] + VB_ALIGN - 1) / VB_ALIGN * VB_ALIGN;
+    v.slots = h_vbase[parts];
     GB_TRY(upload(s, &vs.blk, h_vbase));
     GB_TRY(v.val.alloc(std::max<uint32_t>(h_vbase[parts], 1)));
     GB_CUDA(cudaMemsetAsync(v.val.p, 0, (size_t)std::max<uint32_t>(h_vbase[parts], 1) * 4, s));
@@ -1190,9 +1260,10 @@ gb_status LayoutBuild::layout_vblocks() {
     GB_TRY(akey_alt.alloc(NP));
     GB_TRY(aslot.alloc(NP));
     GB_TRY(aslot_alt.alloc(NP));
+    GB_TRY(cb_stream_ids(s, v.window, goffv.p, &vs));
     k_vb_place<<<grid_for(Ec, 256), 256, 0, s>>>(kb.Current(), ib.Current(), rank.p, Ec, erow.p, coff.p, goffv.p,
-                                                 pfirst.p, vs.blk.p, B, reinterpret_cast<uint16_t*>(vs.ids.p),
-                                                 akey.p, aslot.p);
+                                                 v.sectors ? gpos : nullptr, v.sectors ? gfirst.p : pfirst.p,
+                                                 vs.blk.p, B, reinterpret_cast<uint16_t*>(vs.ids.p), akey.p, aslot.p);
     GB_CUDA(cudaGetLastError());
     GB_CUDA(cudaStreamSynchronize(s));
   }
@@ -1239,8 +1310,9 @@ gb_status LayoutBuild::layout_vblocks() {
   GB_TRY(upload(s, &v.bin_tasks, h_tasks));
   GB_TRY(v.bin_ids.alloc(npos));
   GB_CUDA(cudaMemsetAsync(v.bin_ids.p, 0xFF, npos * 2, s));  // BIN_PAD
-  GB_TRY(v.bin_bits.alloc(npos / 32));
-  GB_CUDA(cudaMemsetAsync(v.bin_bits.p, 0, npos / 32 * 4, s));
+  GB_TRY(v.bin_bits.alloc(npos / 32 + BIN_STEP / 32));
+  GB_CUDA(cudaMemsetAsync(v.bin_bits.p, 0, (npos / 32 + BIN_STEP / 32) * 4, s));
+  GB_CUDA(cudaMemsetAsync(v.bin_bits.p + npos / 32, 1, 1, s));  // the step after the last one starts a run
   GB_TRY(v.bin_grun.alloc(npos / 32));
   GB_TRY(v.bin_runs.alloc((size_t)v.n_runs + 32));  // a step's 32-run window may reach past the last run
   GB_CUDA(cudaMemsetAsync(v.bin_runs.p + v.n_runs, 0, 32 * 4, s));
@@ -1258,7 +1330,7 @@ gb_status LayoutBuild::layout_vblocks() {
     GB_CUDA(cudaStreamSynchronize(s));
   }
   // pass B's chunks and tasks over the virtual blocks (rows [row0[k], row0[k + 1]) each)
-  GB_TRY(cb_chunk_table(s, dev_sms, B, goffv.p, h_min, &vs));
+  GB_TRY(cb_chunk_table(s, dev_sms, v.window, goffv.p, h_min, &vs));
   GB_REQUIRE(vs.n_fix == 0, "a virtual-block segment is cut by a chunk boundary");
   GB_TRY(vs.partial.alloc(n_loc));
   GB_CUDA(cudaMemsetAsync(vs.partial.p, 0, (size_t)n_loc * 4, s));

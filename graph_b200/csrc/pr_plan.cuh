@@ -36,6 +36,7 @@ constexpr uint32_t CB_ILP = 4;               // 32-edge batches in flight per wa
 constexpr uint32_t CB_HEAD_CONT = 1u, CB_TAIL_CONT = 2u, CB_INTERIOR = 4u;
 
 constexpr uint32_t VB_ALIGN = 32;            // virtual blocks start at multiples of 32 slots of V (128-byte lines)
+constexpr uint32_t VB_RUN_ALIGN = 8;         // runs of V start at multiples of 8 slots (32-byte sectors) and fill them
 constexpr uint16_t BIN_PAD = 0xFFFFu;        // pass A: a position that holds no pair (B < 2^16 - 1)
 constexpr uint32_t BIN_STEP = 256;           // pass A: positions per warp step (8 groups of 32, 8 per lane)
 constexpr uint32_t BIN_CHUNK = 8;            // pass A: steps per chunk (2048 positions, one warp)
@@ -76,7 +77,7 @@ struct CbStream {
   DevBuf<uint32_t> blk;         // [KB] hot rank j's source block (pass B: [KB + 1] V slot bounds, multiples of VB_ALIGN)
   DevBuf<uint32_t> nrows;       // [KB] rows with a segment in block j (non-increasing for the hot blocks)
   DevBuf<uint32_t> poff;        // [KB + 1] first partial of block j
-  DevBuf<uint2> ids;            // [NG] groups of 4 block-local 16-bit ids (pad id = B)
+  DevBuf<uint2> ids;            // [NG] groups of 4 block-local 16-bit ids (pad id = B; pass B: its window)
   DevBuf<uint32_t> bits;        // [NG/32 + 8] bit g set <=> group g starts a segment
   DevBuf<float> partial;        // [S] one partial sum per segment
   // the chunks and tasks (k_pr_cb's unit of work), as cb_chunk_table cuts them
@@ -96,7 +97,13 @@ struct CbStream {
 // Virtual blocks: the edges that no column-block segment takes (COLD edges) on graphs whose source vector does
 // not fit in L2.  The rows are cut into contiguous PARTITIONS of at most B cold edges; each distinct (source,
 // partition) PAIR owns one slot of the value buffer V (partition-major, by source inside a partition: a
-// partition's slots are one virtual block of at most B entries).  Pass A (k_pr_cb<CB_BIN>) loads each source
+// partition's slots are one virtual block).  The pairs of one source block inside one partition are a RUN of
+// consecutive slots.  With `sectors`, every run starts at a multiple of VB_RUN_ALIGN slots and is followed by pad
+// slots up to the next one, which pass A zeroes in the step that stores the run's last value: every 32-byte
+// sector of V is then written whole by one warp, and none is left half-written in L2 to be read back from HBM
+// when it is evicted.  A padded virtual block may then hold more than B slots; pass B's window (its shared-memory
+// block, pad id and zero slot) is the largest that fits.  Without `sectors` (some padded partition would not fit
+// in that window) the runs are packed and pass B's window is B.  Pass A (k_pr_cb<CB_BIN>) loads each source
 // block into shared memory and writes the values of its pairs to V, run by run; pass B (k_pr_cb<CB_VIRT>) walks a
 // column-block stream over the virtual blocks, with V in place of the source vector, and leaves one partial per
 // local row.  k_pr_finish then completes every local row, and k_pr_sell does not run.
@@ -104,11 +111,15 @@ struct PrVBlocks {
   uint64_t pairs = 0, edges = 0;  // (source, partition) pairs and the cold edges they serve
   uint32_t bin_blocks = 0, n_runs = 0;
   uint32_t wide_steps = 0;      // pass A steps whose positions touch more than 32 runs (the run-window loop)
+  bool sectors = false;         // runs start on 32-byte sectors and pass A zeroes their pad slots
+  uint32_t window = 0;          // pass B's block: V slots of its shared-memory block, and its pad id
+  uint64_t slots = 0;           // V's length
   DevBuf<float> val;            // V
   // pass A: the pairs in (source block, partition, source) order, each block's share starting at a multiple of
   // BIN_STEP positions (BIN_PAD in between); a RUN is the pairs of one (block, partition), consecutive slots of V
   DevBuf<uint16_t> bin_ids;     // block-local source id of every position, at bin_id_index(position)
-  DevBuf<uint32_t> bin_bits;    // per 32 positions: bit i set <=> position 32 g + i starts a run
+  DevBuf<uint32_t> bin_bits;    // per 32 positions: bit i set <=> position 32 g + i starts a run; then one step
+                                // whose first position starts a run (the end of the last one)
   DevBuf<uint32_t> bin_grun;    // per 32 positions: the last run that starts at or before position 32 g
   DevBuf<uint32_t> bin_runs;    // [n_runs + 32] first V slot - first position of each run (mod 2^32); 32 spare
   DevBuf<uint2> bin_chunks;     // [steps s0, s1) of one block: a warp's unit of pass A
@@ -173,7 +184,8 @@ struct PrPlan {
   DevBuf<double> block_err;  // per CTA error partials (SELL CTAs, then finish CTAs)
   DevBuf<double> err_hist;   // error of each sweep of the current batch
   DevBuf<uint32_t> ctrl;     // [0] = done flag (sweep number at which tolerance was met), [1] = ticket
-  size_t smem_cb = 0;
+  size_t smem_cb = 0;        // k_pr_cb<CB_MAIN> and pass A: a source block and its zero slot
+  size_t smem_vb = 0;        // pass B: its window of V and the zero slot
   std::vector<cudaEvent_t> prof_events;
   // GB_PR_TRACE=1 (diagnostics): CUDA events between the kernels of every sweep; averages are printed
   // to stderr when the layout is released
@@ -287,5 +299,10 @@ gb_status pr_csr_shards(const std::vector<int>& devs, uint32_t V, uint32_t n, co
 // h_nrows / h_poff: the staircase (nrows[], poff[]) as the layout build holds it on the host.
 gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, const std::vector<uint32_t>& h_poff,
                            int dev_sms, cudaStream_t s);
+// The largest window of V pass B can take on `device` (a multiple of VB_ALIGN slots): its shared-memory block,
+// the zero slot and k_pr_cb's static shared memory within the per-block opt-in limit, and below 0xFFFF, since
+// pass B's ids and pad id are 16-bit (58048 slots on an H100).
+// GB_PR_VB_WINDOW (tests): a smaller window, in slots.
+gb_status pr_vb_window(int device, uint32_t* window);
 
 }  // namespace gb

@@ -459,6 +459,8 @@ typedef struct gb_pr_shard_stats {
   uint64_t vblock_edges;       /* edges reduced through the virtual blocks */
   uint32_t vblock_wide_steps;  /* 256-position steps of the virtual blocks' pass A whose positions fall in more than
                                   32 runs: every sweep finds their slots through the slower run-window loop */
+  uint64_t vblock_slots;       /* length of the value buffer, pad slots included */
+  uint32_t vblock_sectors;     /* 1: every run of the value buffer starts on a 32-byte sector and fills its last one */
 } gb_pr_shard_stats;
 
 /* the reference's own partitioner on the ORIGINAL ids: in_degree_partition (graph_ops.rs:431-439,
@@ -490,6 +492,10 @@ typedef struct gb_pr_plan_shape {
   uint32_t last_hot_block;     /* largest source block index among the hot blocks (0xFFFFFFFF: none) */
 } gb_pr_plan_shape;
 gb_status gb_page_rank_plan_shape(const gb_graph* graph, gb_pr_plan_shape* shape);
+/* Diagnostics (tests): the virtual blocks' value buffer of the single-GPU JACOBI plan (built on first use),
+ * count = its vblock_slots.  poison != 0 first sets every slot to the bit pattern 0xFFFFFFFF (a NaN), so that a
+ * later sweep shows which slots pass A writes; values (unless NULL) receives the buffer. */
+gb_status gb_page_rank_plan_values(const gb_graph* graph, int poison, float* values, uint64_t count);
 gb_status gb_pr_shard_plan_shape(const gb_pr_shard* shard, gb_pr_plan_shape* shape);
 /* fills the full initial vectors (n floats each, internal order) on this rank: d_x0 = init/outdeg,
  * the constant part of d_x1; d_scores = init for own rows, 0 for the others (rows without in-edges:

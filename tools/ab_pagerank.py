@@ -11,7 +11,8 @@ What it runs, alternating the trees wherever a number is compared:
     RMAT-25 one with --dump-outputs;
   * bench.py at RMAT-22 and RMAT-24 (the SELL path), once per tree;
 and writes every bench line, the trace lines and a summary (OUT/ab.json): the GTEPS and e2e of every run, the
-kernel times, and whether the two trees' dumped scores are bit-identical at each scale."""
+kernel times, and whether the two trees' dumped scores are bit-identical at each scale (if not, their largest
+relative difference)."""
 from __future__ import annotations
 
 import argparse
@@ -82,6 +83,8 @@ def main():
         try:
             x, y = (np.load(out / f"dump{scale}_{t}" / "scores.npy") for t in trees)
             same[scale] = bool(np.array_equal(x, y))
+            if not same[scale]:  # reordered sums: how far apart, relative to the base tree's scores
+                same[scale] = {"max_rel_diff": float(np.max(np.abs(y.astype(np.float64) - x) / np.abs(x)))}
         except OSError as e:
             same[scale] = f"missing: {e}"
     kern = {}

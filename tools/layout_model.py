@@ -243,6 +243,8 @@ def check(plan, got, in_off, in_tgt):
 
 # ---- virtual blocks (layout_vblocks in pr_layout.cu, PrVBlocks in pr_plan.cuh) ----------------------------------
 VB_ALIGN = 32
+VB_RUN_ALIGN = 8     # with sectors, runs of V start at multiples of 8 slots (32-byte sectors) and fill them
+VB_WINDOW = 58048    # pr_vb_window on an H100: (227 KB opt-in - 128 B static) / 4 - the zero slot, to 32 slots
 VB_BLK_SHIFT = 43
 BIN_PAD = 0xFFFF
 BIN_STEP = 256   # pass A positions per warp step: 8 groups of 32
@@ -312,9 +314,12 @@ def vb_partitions(lens, B):
     return np.array(row0, np.int64), np.array(mseg, np.int64)
 
 
-def vblocks(plan, built):
+def vblocks(plan, built, window=VB_WINDOW):
     """layout_vblocks from the SELL lanes of `built` (build()): partitions, the pairs and V's slots, pass B's
-    segments (k_vb_place) and pass A's positions, run bits, first runs and run table (k_bin_place)."""
+    segments (k_vb_place) and pass A's positions, run bits, first runs and run table (k_bin_place).  `window` is
+    pass B's largest window (pr_vb_window; GB_PR_VB_WINDOW lowers it).  Every run (the pairs of one source block
+    inside one partition) starts at a multiple of VB_RUN_ALIGN slots and is padded to one (sectors), unless a
+    padded partition would exceed the window: then the whole graph keeps the packed slots and a window of B."""
     B, n_loc = plan["B"], plan["n_loc"]
     lens = np.asarray(built["lens"][:n_loc], np.int64)
     cut = vb_partitions(lens, B)
@@ -332,18 +337,29 @@ def vblocks(plan, built):
     rank = np.cumsum(start) - 1                                               # pair of every sorted edge
     NP = int(rank[-1]) + 1
     pfirst = np.array([rank[i] if i < len(sk) else NP for i in np.searchsorted(sk >> 32, np.arange(parts + 1))])
-    cnt = np.diff(pfirst)
-    vbase = np.concatenate([[0], np.cumsum((cnt + VB_ALIGN - 1) // VB_ALIGN * VB_ALIGN)])
-    # pass B: one segment per local row, V-local slot ids in CSR order, pad id B
+    psrc, ppart = sk[start] & 0xFFFFFFFF, sk[start] >> 32
+    # sector slots (k_vb_run_flags .. k_vb_run_pos): a run starts where the partition or source / B changes
+    vrun = np.r_[True, (ppart[1:] != ppart[:-1]) | (psrc[1:] // B != psrc[:-1] // B)]
+    rfirst = np.flatnonzero(vrun)
+    rlen = np.diff(np.r_[rfirst, NP])
+    roff = np.concatenate([[0], np.cumsum((rlen + VB_RUN_ALIGN - 1) // VB_RUN_ALIGN * VB_RUN_ALIGN)])
+    rid = np.cumsum(vrun) - 1
+    gpos = np.r_[roff[rid] + np.arange(NP) - rfirst[rid], roff[-1]]
+    gfirst = gpos[pfirst]
+    sectors = bool((np.diff(gfirst) <= window).all()) and NP + (VB_RUN_ALIGN - 1) * len(rfirst) < 0x7FFFFFFF
+    slot_of = gpos[:NP] if sectors else np.arange(NP)
+    first = gfirst if sectors else pfirst
+    win = window if sectors else B
+    vbase = np.concatenate([[0], np.cumsum((np.diff(first) + VB_ALIGN - 1) // VB_ALIGN * VB_ALIGN)])
+    # pass B: one segment per local row, V-local slot ids in CSR order, pad id = its window
     groups = np.where(lens > 0, (lens + CB_G - 1) // CB_G, 1)
     goffv = np.concatenate([[0], np.cumsum(groups)])
     coff = np.concatenate([[0], np.cumsum(lens)])
-    ids = np.full(int(goffv[-1]) * CB_G, B, np.int64)
+    ids = np.full(int(goffv[-1]) * CB_G, win, np.int64)
     e = order
-    ids[goffv[rows[e]] * CB_G + (e - coff[rows[e]])] = rank - pfirst[sk >> 32]
+    ids[goffv[rows[e]] * CB_G + (e - coff[rows[e]])] = slot_of[rank] - first[sk >> 32]
     # pass A: the pairs by (source block, partition, source), each block's share starting at a step
-    psrc, ppart = sk[start] & 0xFFFFFFFF, sk[start] >> 32
-    pslot = vbase[ppart] + np.arange(NP) - pfirst[ppart]
+    pslot = vbase[ppart] + slot_of - first[ppart]
     akey = ((psrc // B) << VB_BLK_SHIFT) | (ppart << 16) | (psrc % B)
     ao = np.argsort(akey, kind="stable")
     akey, aslot = akey[ao], pslot[ao]
@@ -368,16 +384,24 @@ def vblocks(plan, built):
                            for t in range(s0[b], s0[b] + bsteps[b], BIN_CHUNK)], np.int64).reshape(-1, 2)
     return dict(parts=parts, row0=row0, mseg=mseg, vbase=vbase, pairs=NP, edges=int(lens.sum()), lens=lens,
                 goffv=goffv, ids=ids, bin_ids=bin_ids, bin_bits=bin_bits, bin_grun=bin_grun, bin_runs=bin_runs,
-                bin_chunks=bin_chunks, pos_blk=pos_blk, bcnt=bcnt, run_pos=pos[rstart])
+                bin_chunks=bin_chunks, pos_blk=pos_blk, bcnt=bcnt, run_pos=pos[rstart], pos=pos, aslot=aslot,
+                run_of=np.cumsum(rstart) - 1, slots=int(vbase[-1]), sectors=sectors, window=win,
+                vrun_slot=vbase[ppart[rfirst]] + roff[:-1] - gfirst[ppart[rfirst]] if sectors else None,
+                vrun_len=rlen)
 
 
-def vb_pass_a(plan, vb):
+def vb_pass_a(plan, vb, fills=None):
     """pass A (k_pr_cb<CB_BIN> / bin_chunk), chunk by chunk, step by step, lane by lane: the source of every slot
-    of V it writes, how often it writes it, and the steps that take the run-window loop (more than 32 runs)"""
+    of V it writes, how often it writes it, and the steps that take the run-window loop (more than 32 runs).  With
+    sectors the lane of a run's last position also zeroes the run's pad slots (bin_fill_pad): each is counted in
+    `writes` and marked -2 in V, and `fills` (a dict, when given) counts the fills by where the run ends: at a
+    step's last position (step_end; chunk_end when that is also its chunk's), before pads (share_end), in a wide
+    step (wide)."""
     B = plan["B"]
     V = np.full(int(vb["vbase"][-1]), -1, np.int64)
     writes = np.zeros(len(V), np.int64)
     wide = []
+    bits_all = np.r_[vb["bin_bits"], 1, np.zeros(BIN_STEP // 32 - 1, np.int64)]   # the step after the last: a start
     gs = BIN_STEP // 32
     lanes = np.arange(32)
     upto = (2 << lanes) - 1                                                   # positions 0 .. lane of a group
@@ -400,6 +424,25 @@ def vb_pass_a(plan, vb):
                 ok = sid != BIN_PAD
                 V[slot[ok]] = vb["pos_blk"][p[ok]] * B + sid[ok]
                 np.add.at(writes, slot[ok], 1)
+                if not vb["sectors"]:
+                    continue
+                nvalid = int((ids != BIN_PAD).sum())
+                nxt = bits_all[gs * s + k + 1]                                # bits[k + 1], or the next step's
+                q = 32 * k + lanes
+                nstart = np.where(lanes < 31, (int(bits[k]) >> np.minimum(lanes + 1, 31)) & 1, int(nxt) & 1)
+                last = ok & ((nstart == 1) | ((q + 1 == nvalid) & (nvalid < BIN_STEP)))
+                for L in np.flatnonzero(last):
+                    e = int(slot[L]) + 1
+                    pad = np.arange(e, (e + VB_RUN_ALIGN - 1) // VB_RUN_ALIGN * VB_RUN_ALIGN)
+                    V[pad] = -2
+                    np.add.at(writes, pad, 1)
+                    if fills is not None:
+                        end = q[L] == BIN_STEP - 1
+                        key = "share_end" if nstart[L] == 0 else "chunk_end" if end and s + 1 == s1 else \
+                            "step_end" if end else "inside"
+                        fills[key] = fills.get(key, 0) + 1
+                        if runs >= 32:
+                            fills["wide"] = fills.get("wide", 0) + 1
     return V, writes, wide
 
 
@@ -424,23 +467,41 @@ def vb_pass_a_cases(vb):
 def check_vblocks(plan, vb, built):
     """the contract of the two passes: pass A writes every slot of V exactly once (and nothing between the
     virtual blocks), every cold edge appears exactly once in pass B, and every pass B id resolves to the slot
-    of its edge's source; no virtual block holds more than B slots"""
+    of its edge's source; position + delta is every pair's slot.  Packed: a virtual block's slots are a prefix of
+    at most B.  Sectors: every run starts at a multiple of VB_RUN_ALIGN slots, its pad slots up to the next one
+    are zeroed (so every sector a run touches is written whole), and no virtual block exceeds the window."""
     B = plan["B"]
     V, writes, _ = vb_pass_a(plan, vb)
+    W = vb["window"]
+    slot = (vb["pos"] + vb["bin_runs"][vb["run_of"]]) % (1 << 32)
+    assert (slot == vb["aslot"]).all(), "position + delta = the pair's slot"
+    if vb["sectors"]:
+        rs, rl = vb["vrun_slot"], vb["vrun_len"]
+        assert (rs % VB_RUN_ALIGN == 0).all(), "runs start on a sector"
+        pad = np.zeros(len(V) + 1, np.int64)
+        np.add.at(pad, rs + rl, 1)
+        np.add.at(pad, (rs + rl + VB_RUN_ALIGN - 1) // VB_RUN_ALIGN * VB_RUN_ALIGN, -1)
+        want_pad = np.cumsum(pad)[:-1] > 0
+        assert ((V == -2) == want_pad).all(), "pass A zeroes exactly the runs' pad slots"
+    else:
+        assert W == B
     for k in range(vb["parts"]):
         lo, hi = int(vb["vbase"][k]), int(vb["vbase"][k + 1])
+        assert hi - lo <= max(W, (B + VB_ALIGN - 1) // VB_ALIGN * VB_ALIGN), "a virtual block fits in pass B's window"
         used = writes[lo:hi] > 0
         assert (writes[lo:hi][used] == 1).all(), "pass A writes a slot once"
         cnt = int(used.sum())
-        assert used[:cnt].all() and cnt <= B, "a virtual block's slots are a prefix of at most B"
+        assert used[:cnt].all(), "a virtual block's slots are a prefix"
+        assert vb["sectors"] or cnt <= B, "a packed virtual block holds at most B slots"
     for l in range(plan["n_loc"]):
         k = int(np.searchsorted(vb["row0"], l, side="right") - 1)
         g0, g1 = int(vb["goffv"][l]), int(vb["goffv"][l + 1])
         d = int(vb["lens"][l])
         assert g1 - g0 == max(1, (d + CB_G - 1) // CB_G), "one segment per row, ceil(cold / 4) groups, at least one"
         seg = vb["ids"][g0 * CB_G:g1 * CB_G]
-        assert (seg[d:] == B).all(), "padding = the zero slot"
-        assert (seg[:d] < B).all()
+        assert (seg[d:] == W).all(), "padding = the zero slot"
+        assert (seg[:d] < W).all()
+        assert (V[int(vb["vbase"][k]) + seg[:d]] >= 0).all(), "pass B never names a pad slot"
         assert V[int(vb["vbase"][k]) + seg[:d]].tolist() == built["sell"][l].tolist(), \
             "pass B's ids resolve to the sources of the row's cold edges, in CSR order"
     assert vb["edges"] == sum(len(built["sell"][l]) for l in range(plan["n_loc"]))
