@@ -55,9 +55,12 @@ void free_pr_plan(PrPlan* p) {
         cudaEventElapsedTime(&ms, p->trace_events[5 * i + k], p->trace_events[5 * i + k + 1]);
         acc[k] += ms;
       }
-    fprintf(stderr, p->vb ? "[gb trace] shard %u/%u, %zu sweeps: k_pr_cb %.4f  pass A %.4f  pass B %.4f  k_pr_finish %.4f ms\n"
-                          : "[gb trace] shard %u/%u, %zu sweeps: k_pr_cb %.4f  k_pr_fixup %.4f  k_pr_sell %.4f  k_pr_finish %.4f ms\n",
-            p->deal.p, p->deal.P, sweeps, acc[0] / sweeps, acc[1] / sweeps, acc[2] / sweeps, acc[3] / sweeps);
+    if (p->vb)  // nothing runs between the fused k_pr_cb and pass B
+      fprintf(stderr, "[gb trace] shard %u/%u, %zu sweeps: k_pr_cb with pass A %.4f  pass B %.4f  k_pr_finish %.4f ms\n",
+              p->deal.p, p->deal.P, sweeps, acc[0] / sweeps, acc[2] / sweeps, acc[3] / sweeps);
+    else
+      fprintf(stderr, "[gb trace] shard %u/%u, %zu sweeps: k_pr_cb %.4f  k_pr_fixup %.4f  k_pr_sell %.4f  k_pr_finish %.4f ms\n",
+              p->deal.p, p->deal.P, sweeps, acc[0] / sweeps, acc[1] / sweeps, acc[2] / sweeps, acc[3] / sweeps);
   }
   for (cudaEvent_t e : p->trace_events) cudaEventDestroy(e);
   for (cudaEvent_t e : p->prof_events) cudaEventDestroy(e);
@@ -78,6 +81,13 @@ __device__ __forceinline__ uint2 ld_stream_u2(const uint2* p) {
   asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
   return r;
 }
+// a fused task of k_pr_cb<CB_FUSED>, read afresh wherever it is needed (an L1 hit): a coherent load in volatile
+// asm, so that the compiler cannot merge the reads into one value that would live (and spill) across the walks
+__device__ __forceinline__ uint4 ld_task(const uint4* p) {
+  uint4 r;
+  asm volatile("ld.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
+  return r;
+}
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);
@@ -92,9 +102,9 @@ __device__ __forceinline__ double warp_sum(double v) {
 // ---- sweep kernels (JACOBI) ------------------------------------------------------------------
 // What k_pr_cb's task scheduler reads: the block of each rank, the tasks and this pass's task cursors
 struct CbSched {
-  const uint32_t* blk;  // CbStream::blk (pass A: PrVBlocks::bin_blk)
+  const uint32_t* blk;  // CbStream::blk (CB_FUSED: unused, its tasks name their source block)
   const uint2* tasks;
-  uint32_t n_tasks;
+  uint32_t n_tasks;     // CB_FUSED: PrVBlocks::n_tasks (the tasks are PrArgs::fused_tasks)
   uint32_t* task_ctr;
 };
 // What the walker, the fixup of cut segments and k_pr_finish read of a stream (CbStream)
@@ -133,9 +143,11 @@ struct PrArgs {
   uint32_t B;
   CbSched sched;
   CbWalk walk;
+  CbWalk fix;              // pass B: the hot blocks' stream, whose cut segments its first warps add (PrFix::PASS_B)
   uint32_t n_task_ranges;  // all passes' task cursors, from sched.task_ctr of the hot blocks
   float* rem;
-  // pass A of the virtual blocks (k_pr_cb<CB_BIN>)
+  // pass A of the virtual blocks (k_pr_cb<CB_FUSED>)
+  const uint4* fused_tasks;  // PrVBlocks::tasks
   float* vals;
   const uint16_t* bin_ids;
   const uint32_t* bin_bits;
@@ -462,20 +474,20 @@ __device__ __forceinline__ void bin_chunk(const PrArgs& a, const float* xs, uint
 // Segments cut by chunk boundaries (segments longer than a chunk): one warp per segment adds its parts
 // in a fixed order — the head part of the first chunk, then lanes over the following chunks (a fixed
 // xor tree per batch of 32).  Tiny; runs after k_pr_cb (as k_pr_fixup, or as the prologue of k_pr_sell or of
-// pass A).
-__device__ __forceinline__ void cb_fix_segment(const PrArgs& a, uint32_t c0, uint32_t lane) {
-  double t = a.walk.side[2 * (size_t)c0 + 1];
+// pass B).  w = the hot blocks' stream.
+__device__ __forceinline__ void cb_fix_segment(const CbWalk& w, uint32_t c0, uint32_t lane) {
+  double t = w.side[2 * (size_t)c0 + 1];
   for (uint32_t k0 = c0 + 1;; k0 += 32) {
     const uint32_t k = k0 + lane;
     // the walk ends at the first chunk that is not entirely inside the segment (sentinel chunk after the last)
-    const uint32_t fl = a.walk.chunks[min(k, a.walk.n_chunks)].w >> 24;
-    const bool inside = k < a.walk.n_chunks && (fl & CB_INTERIOR) && (fl & CB_TAIL_CONT);
+    const uint32_t fl = w.chunks[min(k, w.n_chunks)].w >> 24;
+    const bool inside = k < w.n_chunks && (fl & CB_INTERIOR) && (fl & CB_TAIL_CONT);
     const uint32_t stop = __ballot_sync(0xFFFFFFFFu, !inside);
     const uint32_t upto = stop ? (uint32_t)__ffs(stop) - 1 : 31u;  // last lane that contributes
-    t += warp_sum(lane <= upto ? a.walk.side[2 * (size_t)k] : 0.0);
+    t += warp_sum(lane <= upto ? w.side[2 * (size_t)k] : 0.0);
     if (stop) break;
   }
-  if (lane == 0) a.walk.partial[a.walk.tail_slot[c0]] = (float)t;
+  if (lane == 0) w.partial[w.tail_slot[c0]] = (float)t;
 }
 
 // ---- TMA bulk copy of a source block into shared memory (cp.async.bulk + mbarrier) -----------------
@@ -516,10 +528,12 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
 // thin blocks are (a purely static split leaves thin blocks at single-warp latency, one global cursor reloads the
 // block for every task).  Claiming the next task one task ahead (to hide the atomic's
 // round trip) was measured and dropped: a claimed task cannot be stolen, which costs more at the tail.
-// KIND: CB_MAIN = the column blocks of x_cur; CB_BIN = pass A of the virtual blocks (the same loads of x_cur,
-// bin_chunk per chunk; its first warps also add the cut segments of CB_MAIN); CB_VIRT = pass B (block j is
-// V[blk[j] .. blk[j + 1]), the column-block walker as in CB_MAIN).
-constexpr uint32_t CB_MAIN = 0, CB_VIRT = 1, CB_BIN = 2;
+// KIND: CB_MAIN = the column blocks of x_cur; CB_FUSED = the same, with pass A of the virtual blocks: a task
+// holds a source block's hot chunks and its pass-A chunks (PrVBlocks::tasks), interleaved so that the warps of a
+// CTA stream ids through cb_chunk and scatter values through bin_chunk at the same time, from one load of the
+// block; CB_VIRT = pass B (block j is V[blk[j] .. blk[j + 1]), the column-block walker as in CB_MAIN; its first
+// warps add the cut segments of the hot blocks, which CB_FUSED has finished).
+constexpr uint32_t CB_MAIN = 0, CB_VIRT = 1, CB_FUSED = 2;
 template <uint32_t KIND>
 __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
   extern __shared__ __align__(128) float smem[];
@@ -528,9 +542,9 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
   __shared__ __align__(8) unsigned long long s_mbar;
   if (a.ctrl[0] != 0) return;  // tolerance already met by an earlier sweep of this batch
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (KIND == CB_BIN)  // k_pr_cb<CB_MAIN> has finished; walk = the hot blocks' stream (PrFix::PASS_A)
-    for (uint32_t i = blockIdx.x * PR_WARPS + warp; i < a.walk.n_fix; i += gridDim.x * PR_WARPS)
-      cb_fix_segment(a, a.walk.fix_list[i], lane);
+  if (KIND == CB_VIRT)  // k_pr_cb<CB_FUSED> has finished (PrFix::PASS_B; n_fix = 0 otherwise)
+    for (uint32_t i = blockIdx.x * PR_WARPS + warp; i < a.fix.n_fix; i += gridDim.x * PR_WARPS)
+      cb_fix_segment(a.fix, a.fix.fix_list[i], lane);
   const uint32_t B = a.B;
   const uint32_t pad2 = B | (B << 16);
   const uint32_t R = gridDim.x;  // ranges = CTAs
@@ -580,10 +594,14 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
     if (threadIdx.x == 0) s_next = PR_THREADS / 32;  // every warp is past its last claim of the previous task
     __syncthreads();
     if (t == CB_NONE) break;
-    const uint2 task = a.sched.tasks[t];  // (first chunk, chunk count | block rank << 8)
-    const uint32_t j = task.y >> 8;
+    // (first chunk, chunk count | block rank << 8); CB_FUSED: (first hot chunk, first pass-A chunk, hot chunks |
+    // pass-A chunks << 8, source block)
+    const uint2 task = KIND == CB_FUSED ? make_uint2(0u, 0u) : a.sched.tasks[t];
+    const uint32_t j = KIND == CB_FUSED ? ld_task(a.fused_tasks + t).w : task.y >> 8;
     if (j != cur_j) {
-      const uint64_t x0 = KIND == CB_VIRT ? (uint64_t)a.sched.blk[j] : (uint64_t)a.sched.blk[j] * B;
+      const uint64_t x0 = KIND == CB_VIRT    ? (uint64_t)a.sched.blk[j]
+                          : KIND == CB_FUSED ? (uint64_t)j * B
+                                             : (uint64_t)a.sched.blk[j] * B;
       const uint32_t cnt = KIND == CB_VIRT ? a.sched.blk[j + 1] - a.sched.blk[j]
                                            : (uint32_t)min((uint64_t)B, (uint64_t)a.n - x0);
       if (bulk_ok) {
@@ -603,14 +621,24 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
       cur_j = j;
       __syncthreads();
     }
-    // a warp starts with chunk `warp` of the task and claims further ones from the CTA's counter
-    const uint32_t nchunks = task.y & 0xFFu;
+    // a warp starts with chunk `warp` of the task and claims further ones from the CTA's counter.  CB_FUSED: the
+    // task's chunks alternate hot, pass A, hot, .. while both kinds last, then the rest of the longer kind; the
+    // task is read again for every chunk, so that none of it stays live across a walk (the walkers use every
+    // register of the 64 that one 1024-thread CTA per SM leaves)
+    const uint32_t nchunks = KIND == CB_FUSED ? CB_NONE : task.y & 0xFFu;  // CB_FUSED leaves the loop below
     for (uint32_t k = warp; k < nchunks;) {
-      if (KIND == CB_BIN) {
-        if (a.bin_fill) bin_chunk<true>(a, xs, task.x + k, lane);
-        else bin_chunk<false>(a, xs, task.x + k, lane);
+      if constexpr (KIND == CB_FUSED) {
+        const uint4 ft = ld_task(a.fused_tasks + t);
+        const uint32_t n_hot = ft.z & 0xFFu, n_bin = ft.z >> 8, pairs = min(n_hot, n_bin);
+        if (k >= n_hot + n_bin) break;
+        const bool hot = k < 2 * pairs ? (k & 1u) == 0 : n_hot > n_bin;
+        const uint32_t i = k < 2 * pairs ? k >> 1 : k - pairs;
+        if (hot) cb_chunk(a, xs, ft.x + i, lane, pad2);
+        else if (a.bin_fill) bin_chunk<true>(a, xs, ft.y + i, lane);
+        else bin_chunk<false>(a, xs, ft.y + i, lane);
+      } else {
+        cb_chunk(a, xs, task.x + k, lane, pad2);
       }
-      else cb_chunk(a, xs, task.x + k, lane, pad2);
       uint32_t nx = 0;
       if (lane == 0) nx = atomicAdd(&s_next, 1u);
       k = __shfl_sync(0xFFFFFFFFu, nx, 0);
@@ -622,7 +650,7 @@ __global__ void k_pr_fixup(const PrArgs a) {
   if (a.ctrl[0] != 0) return;
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
-  for (uint32_t i = gw; i < a.walk.n_fix; i += nw) cb_fix_segment(a, a.walk.fix_list[i], lane);
+  for (uint32_t i = gw; i < a.walk.n_fix; i += nw) cb_fix_segment(a.walk, a.walk.fix_list[i], lane);
 }
 
 // ---- SELL-32 sweep: one lane per row ------------------------------------------------------------
@@ -641,7 +669,7 @@ __global__ void __launch_bounds__(PR_SELL_THREADS, 2) k_pr_sell(const PrArgs a) 
   if (a.fix_in_sell) {
     // segments cut by chunk boundaries (hub rows only: they are completed by k_pr_finish, after this kernel)
     const uint32_t gw0 = blockIdx.x * NW + warp, nw0 = gridDim.x * NW;
-    for (uint32_t i = gw0; i < a.walk.n_fix; i += nw0) cb_fix_segment(a, a.walk.fix_list[i], lane);
+    for (uint32_t i = gw0; i < a.walk.n_fix; i += nw0) cb_fix_segment(a.walk, a.walk.fix_list[i], lane);
   }
   const float* __restrict__ x = a.x_cur;
   double err = 0.0;
@@ -997,7 +1025,7 @@ gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, cons
   GB_CUDA(cudaGetDevice(&dev));
   GB_TRY(cb_smem_ceiling<CB_MAIN>(dev, p->smem_cb));
   GB_TRY(cb_smem_ceiling<CB_VIRT>(dev, p->smem_vb));
-  GB_TRY(cb_smem_ceiling<CB_BIN>(dev, p->smem_cb));
+  GB_TRY(cb_smem_ceiling<CB_FUSED>(dev, p->smem_cb));
   const uint64_t want_sell = ((uint64_t)p->num_slices + PR_SELL_THREADS / 32 - 1) / (PR_SELL_THREADS / 32);
   p->grid_sell = (unsigned)std::min<uint64_t>(want_sell, (uint64_t)dev_sms * 2);
   // rows with segments in more than SELL_FEW blocks are a prefix (nrows[] is non-increasing): k_pr_finish
@@ -1038,7 +1066,7 @@ gb_status plan_sweep_shape(PrPlan* p, const std::vector<uint32_t>& h_nrows, cons
     p->fin_hub_ctas = p->n_fin_warp / 32;
   // the kernel that adds the parts of cut segments (PrFix): k_pr_sell only when it completes none of their rows
   if (!p->hot.n_fix) p->fix_at = PrFix::NONE;
-  else if (p->vb) p->fix_at = PrFix::PASS_A;
+  else if (p->vb) p->fix_at = PrFix::PASS_B;
   else if (p->grid_sell && p->hot.fix_max_row < p->n_fin) p->fix_at = PrFix::SELL;
   else p->fix_at = PrFix::FIXUP;
   const size_t nerr = (size_t)p->grid_sell + p->grid_fin;
@@ -1109,11 +1137,11 @@ static PrArgs make_args(const PrPlan* p, float base, float damping, double toler
   a.mc_next = nullptr;
   return a;
 }
-// pass A of the virtual blocks: its own tasks over x_cur's blocks, and the hot blocks' walker group, whose cut
-// segments its first warps add (PrFix::PASS_A)
-static PrArgs pass_a_args(const PrPlan* p, PrArgs a) {
+// k_pr_cb<CB_FUSED>: the hot blocks' walker and pass A of the virtual blocks, over the fused tasks
+static PrArgs fused_args(const PrPlan* p, PrArgs a) {
   const PrVBlocks& v = p->v;
-  a.sched = CbSched{v.bin_blk.p, v.bin_tasks.p, v.bin_n_tasks, p->task_ctr.p + p->grid_cb};
+  a.sched = CbSched{nullptr, nullptr, v.n_tasks, p->task_ctr.p};
+  a.fused_tasks = v.tasks.p;
   a.vals = v.val.p;
   a.bin_ids = v.bin_ids.p;
   a.bin_bits = v.bin_bits.p;
@@ -1124,17 +1152,19 @@ static PrArgs pass_a_args(const PrPlan* p, PrArgs a) {
   return a;
 }
 // pass B: the virtual blocks' stream, over V, in blocks of its window; its partials are the rows' cold sums
-// (k_pr_finish's rem)
+// (k_pr_finish's rem).  Its first warps add the hot blocks' cut segments (PrFix::PASS_B).
 static PrArgs pass_b_args(const PrPlan* p, PrArgs a) {
   a.x_cur = p->v.val.p;
   a.B = p->v.window;
-  a.sched = sched_of(p->v.virt, p->task_ctr.p + p->grid_cb + p->grid_bin);
+  a.sched = sched_of(p->v.virt, p->task_ctr.p + p->grid_cb);
   a.walk = walk_of(p->v.virt);
+  a.fix = walk_of(p->hot);
+  if (p->fix_at != PrFix::PASS_B) a.fix.n_fix = 0;
   return a;
 }
 
-// one sweep = column blocks (+ fixup of cut segments), SELL rows or the two virtual-block passes, then finish;
-// *launches is advanced by the kernels launched
+// one sweep = column blocks (+ fixup of cut segments) and SELL rows, or column blocks fused with pass A of the
+// virtual blocks and pass B; then finish.  *launches is advanced by the kernels launched
 template <bool PEERS>
 static gb_status launch_sweep(const PrPlan* p, const PrArgs& a, cudaStream_t s, uint64_t* launches) {
   cudaEvent_t* ev = nullptr;
@@ -1146,16 +1176,13 @@ static gb_status launch_sweep(const PrPlan* p, const PrArgs& a, cudaStream_t s, 
     GB_CUDA(cudaEventRecord(ev[0], s));
   }
   if (p->grid_cb) {
-    k_pr_cb<CB_MAIN><<<p->grid_cb, PR_THREADS, p->smem_cb, s>>>(a);
+    if (p->vb) k_pr_cb<CB_FUSED><<<p->grid_cb, PR_THREADS, p->smem_cb, s>>>(fused_args(p, a));
+    else k_pr_cb<CB_MAIN><<<p->grid_cb, PR_THREADS, p->smem_cb, s>>>(a);
     *launches += 1;
   }
   if (ev) GB_CUDA(cudaEventRecord(ev[1], s));
   if (p->fix_at == PrFix::FIXUP) {
     k_pr_fixup<<<grid_for((uint64_t)p->hot.n_fix * 32, 128, 296), 128, 0, s>>>(a);
-    *launches += 1;
-  }
-  if (p->vb) {
-    k_pr_cb<CB_BIN><<<p->grid_bin, PR_THREADS, p->smem_cb, s>>>(pass_a_args(p, a));
     *launches += 1;
   }
   if (ev) GB_CUDA(cudaEventRecord(ev[2], s));
@@ -1336,11 +1363,11 @@ static void plan_stats(const PrPlan* p, gb_pr_shard_stats* stats) {
   stats->segments = p->hot.S;
   stats->groups = p->hot.NG;
   stats->chunks = p->hot.n_chunks;
-  stats->tasks = p->hot.n_tasks;
+  stats->tasks = p->vb ? p->v.n_tasks : p->hot.n_tasks;  // k_pr_cb's tasks (CB_FUSED's with virtual blocks)
   stats->cut_segments = p->hot.n_fix;
   stats->chunk_groups = p->hot.chunk_groups;
   stats->launches_per_sweep = 1 + (p->grid_cb ? 1 : 0) + (p->grid_sell ? 1 : 0) +
-                              (p->fix_at == PrFix::FIXUP ? 1 : 0) + (p->vb ? 2 : 0);
+                              (p->fix_at == PrFix::FIXUP ? 1 : 0) + (p->vb ? 1 : 0);
   stats->device_bytes = p->bytes();
   stats->vblock_parts = p->vb ? p->v.virt.KB : 0;
   stats->vblock_pairs = p->vb ? p->v.pairs : 0;

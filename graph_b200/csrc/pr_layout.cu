@@ -726,6 +726,7 @@ struct LayoutBuild {
   uint32_t n_mega = 0;  // local rows [0, n_mega) take the sort path of the build
   uint32_t M = 0;       // their in-edges
   std::vector<uint32_t> h_nrows, h_poff;  // the staircase on the host
+  std::vector<uint3> h_bin_range;  // virtual blocks: [source block] pass A's chunks (first, count) and steps
   DevBuf<uint32_t> old_of;  // internal id -> original id
   DevBuf<uint32_t> indeg;   // in-degree by internal id [n + 1]
   DevBuf<unsigned long long> counters;  // [0] active rows, [1] local edges, [2] edges in segments, [3] fix count
@@ -742,6 +743,7 @@ struct LayoutBuild {
   gb_status layout_fill();
   gb_status layout_vblocks();
   gb_status layout_chunks();
+  gb_status layout_fused_tasks();
 };
 
 // permutation (in-degree descending, then out-degree descending, then id), the active rows (a prefix of
@@ -1282,32 +1284,26 @@ gb_status LayoutBuild::layout_vblocks() {
   std::vector<uint32_t> h_bfirst(nblk + 1);
   GB_CUDA(cudaMemcpyAsync(h_bfirst.data(), bfirst.p, (size_t)(nblk + 1) * 4, cudaMemcpyDeviceToHost, s));
   GB_CUDA(cudaStreamSynchronize(s));
-  std::vector<uint32_t> h_brank(nblk, CB_NONE), h_bblk, h_bpos;
-  std::vector<uint2> h_chunks, h_tasks;
+  std::vector<uint32_t> h_brank(nblk, CB_NONE), h_bpos;
+  std::vector<uint2> h_chunks;
+  h_bin_range.assign(nblk, make_uint3(0, 0, 0));
   uint64_t npos = 0;
   for (uint32_t b = 0; b < nblk; ++b) {
     const uint32_t cnt = h_bfirst[b + 1] - h_bfirst[b];
     if (!cnt) continue;
-    const uint32_t j = (uint32_t)h_bblk.size();
-    h_brank[b] = j;
-    h_bblk.push_back(b);
+    h_brank[b] = (uint32_t)h_bpos.size();
     h_bpos.push_back((uint32_t)npos);
     const uint32_t s0 = (uint32_t)(npos / BIN_STEP), s1 = s0 + (cnt + BIN_STEP - 1) / BIN_STEP;
     const uint32_t c0 = (uint32_t)h_chunks.size();
     for (uint32_t t = s0; t < s1; t += BIN_CHUNK) h_chunks.push_back(make_uint2(t, std::min(s1, t + BIN_CHUNK)));
-    const uint32_t nc = (uint32_t)h_chunks.size() - c0;
-    for (uint32_t c = 0; c < nc; c += CB_TASK_CHUNKS)
-      h_tasks.push_back(make_uint2(c0 + c, (std::min(nc, c + CB_TASK_CHUNKS) - c) | (j << 8)));
+    h_bin_range[b] = make_uint3(c0, (uint32_t)h_chunks.size() - c0, s1 - s0);
     npos += (uint64_t)(s1 - s0) * BIN_STEP;
     GB_REQUIRE(npos <= 0xFFFFFF00ull, "too many virtual-block pairs (%llu positions)", (unsigned long long)npos);
   }
-  v.bin_blocks = (uint32_t)h_bblk.size();
-  v.bin_n_tasks = (uint32_t)h_tasks.size();
+  v.bin_blocks = (uint32_t)h_bpos.size();
   GB_TRY(upload(s, &brank, h_brank));
   GB_TRY(upload(s, &bpos, h_bpos));
-  GB_TRY(upload(s, &v.bin_blk, h_bblk));
   GB_TRY(upload(s, &v.bin_chunks, h_chunks));
-  GB_TRY(upload(s, &v.bin_tasks, h_tasks));
   GB_TRY(v.bin_ids.alloc(npos));
   GB_CUDA(cudaMemsetAsync(v.bin_ids.p, 0xFF, npos * 2, s));  // BIN_PAD
   GB_TRY(v.bin_bits.alloc(npos / 32 + BIN_STEP / 32));
@@ -1336,7 +1332,6 @@ gb_status LayoutBuild::layout_vblocks() {
   GB_CUDA(cudaMemsetAsync(vs.partial.p, 0, (size_t)n_loc * 4, s));
   v.pairs = NP;
   v.edges = E;
-  p->grid_bin = (unsigned)std::min<uint64_t>(v.bin_n_tasks, (uint64_t)dev_sms);
   p->grid_vb = (unsigned)std::min<uint64_t>(vs.n_tasks, (uint64_t)dev_sms);
   // the SELL slices have served as the build's list of cold edges: k_pr_sell does not run
   p->sell = DevBuf<uint4>();
@@ -1347,11 +1342,79 @@ gb_status LayoutBuild::layout_vblocks() {
   return GB_OK;
 }
 
-// Chunks of the column-block kernel; then the sweep's per-pair and per-row buffers.
+// x_cur block loads of a k_pr_cb pass whose R persistent CTAs drain the static ranges of a task list whose task t
+// runs on source block blk[t], before any stealing (GB_PR_TRACE)
+static uint64_t range_block_loads(const std::vector<uint32_t>& blk, uint64_t R) {
+  uint64_t loads = 0;
+  for (uint64_t r = 0; r < R; ++r)
+    for (uint64_t t = blk.size() * r / R, hi = blk.size() * (r + 1) / R; t < hi; ++t)
+      loads += t == blk.size() * r / R || blk[t] != blk[t - 1];
+  return loads;
+}
+
+// The fused pass's tasks (PrVBlocks::tasks): every source block with hot chunks or pass-A chunks, fattest first
+// by the bytes its chunks stream (8 per hot group; per pass-A position a 2-byte id and a 4-byte value), and the
+// block's i-th hot task (as cb_chunk_table cut them) with its i-th run of CB_TASK_CHUNKS pass-A chunks.
+gb_status LayoutBuild::layout_fused_tasks() {
+  CbStream& hot = p->hot;
+  PrVBlocks& v = p->v;
+  std::vector<uint2> h_hot_tasks(hot.n_tasks);
+  std::vector<uint4> h_hot_chunks(hot.n_chunks);
+  std::vector<uint32_t> h_blk(hot.KB);
+  if (hot.n_tasks) {
+    GB_CUDA(cudaMemcpyAsync(h_hot_tasks.data(), hot.tasks.p, (size_t)hot.n_tasks * 8, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaMemcpyAsync(h_hot_chunks.data(), hot.chunks.p, (size_t)hot.n_chunks * 16, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaMemcpyAsync(h_blk.data(), hot.blk.p, (size_t)hot.KB * 4, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaStreamSynchronize(s));
+  }
+  const uint32_t nblk = (uint32_t)h_bin_range.size();
+  std::vector<uint64_t> bytes(nblk, 0);
+  std::vector<std::vector<uint2>> hot_of(nblk);  // a source block's hot tasks, in order
+  std::vector<uint32_t> old_hot_blk, old_bin_blk;
+  for (const uint2 t : h_hot_tasks) {
+    const uint32_t b = h_blk[t.y >> 8];
+    hot_of[b].push_back(t);
+    old_hot_blk.push_back(b);
+    for (uint32_t c = t.x; c < t.x + (t.y & 0xFFu); ++c) bytes[b] += 8ull * (h_hot_chunks[c].y - h_hot_chunks[c].x);
+  }
+  std::vector<uint32_t> order;
+  for (uint32_t b = 0; b < nblk; ++b) {
+    bytes[b] += 6ull * BIN_STEP * h_bin_range[b].z;
+    for (uint32_t c = 0; c < h_bin_range[b].y; c += CB_TASK_CHUNKS) old_bin_blk.push_back(b);
+    if (bytes[b]) order.push_back(b);
+  }
+  std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return bytes[x] > bytes[y]; });
+  std::vector<uint4> h_tasks;
+  std::vector<uint32_t> task_blk;
+  for (const uint32_t b : order) {
+    const uint3 r = h_bin_range[b];
+    const uint32_t nt = std::max<uint32_t>((uint32_t)hot_of[b].size(), (r.y + CB_TASK_CHUNKS - 1) / CB_TASK_CHUNKS);
+    for (uint32_t i = 0; i < nt; ++i) {
+      const uint2 ht = i < hot_of[b].size() ? hot_of[b][i] : make_uint2(0, 0);
+      const uint32_t a0 = std::min(r.y, i * CB_TASK_CHUNKS), na = std::min(r.y - a0, CB_TASK_CHUNKS);
+      h_tasks.push_back(make_uint4(ht.x, r.x + a0, (ht.y & 0xFFu) | na << 8, b));
+      task_blk.push_back(b);
+    }
+  }
+  v.n_tasks = (uint32_t)h_tasks.size();
+  GB_TRY(upload(s, &v.tasks, h_tasks));
+  p->grid_cb = (unsigned)std::min<uint64_t>(v.n_tasks, (uint64_t)dev_sms);
+  if (env_u64("GB_PR_TRACE", 0))
+    fprintf(stderr, "[gb trace] shard %u/%u: x_cur block loads per sweep before stealing: fused k_pr_cb %llu (k_pr_cb "
+            "%llu + pass A %llu as separate passes)\n", deal.p, deal.P,
+            (unsigned long long)range_block_loads(task_blk, p->grid_cb),
+            (unsigned long long)range_block_loads(old_hot_blk, std::min<uint64_t>(old_hot_blk.size(), dev_sms)),
+            (unsigned long long)range_block_loads(old_bin_blk, std::min<uint64_t>(old_bin_blk.size(), dev_sms)));
+  return GB_OK;
+}
+
+// Chunks of the column-block kernel (and with virtual blocks, the fused pass's tasks); then the sweep's per-pair
+// and per-row buffers.
 gb_status LayoutBuild::layout_chunks() {
   CbStream& hot = p->hot;
   GB_TRY(cb_chunk_table(s, dev_sms, B, goff.p, {}, &hot));
   p->grid_cb = (unsigned)std::min<uint64_t>(hot.n_tasks, (uint64_t)dev_sms);  // one persistent CTA per SM
+  if (p->vb) GB_TRY(layout_fused_tasks());
   GB_TRY(p->task_ctr.alloc(std::max<unsigned>(p->task_ranges(), 1)));
   GB_CUDA(cudaMemsetAsync(p->task_ctr.p, 0, (size_t)std::max<unsigned>(p->task_ranges(), 1) * 4, s));
   GB_TRY(hot.partial.alloc(std::max<uint64_t>(hot.S, 1)));

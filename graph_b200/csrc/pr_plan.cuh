@@ -103,10 +103,12 @@ struct CbStream {
 // sector of V is then written whole by one warp, and none is left half-written in L2 to be read back from HBM
 // when it is evicted.  A padded virtual block may then hold more than B slots; pass B's window (its shared-memory
 // block, pad id and zero slot) is the largest that fits.  Without `sectors` (some padded partition would not fit
-// in that window) the runs are packed and pass B's window is B.  Pass A (k_pr_cb<CB_BIN>) loads each source
-// block into shared memory and writes the values of its pairs to V, run by run; pass B (k_pr_cb<CB_VIRT>) walks a
-// column-block stream over the virtual blocks, with V in place of the source vector, and leaves one partial per
-// local row.  k_pr_finish then completes every local row, and k_pr_sell does not run.
+// in that window) the runs are packed and pass B's window is B.  Pass A writes the values of each source block's
+// pairs to V, run by run, from the block in shared memory; it runs inside k_pr_cb<CB_FUSED>, whose tasks carry a
+// source block's hot chunks and its pass-A chunks side by side, so that the block is loaded once for both.  Pass
+// B (k_pr_cb<CB_VIRT>) walks a column-block stream over the virtual blocks, with V in place of the source
+// vector, and leaves one partial per local row.  k_pr_finish then completes every local row, and k_pr_sell does
+// not run.
 struct PrVBlocks {
   uint64_t pairs = 0, edges = 0;  // (source, partition) pairs and the cold edges they serve
   uint32_t bin_blocks = 0, n_runs = 0;
@@ -123,15 +125,18 @@ struct PrVBlocks {
   DevBuf<uint32_t> bin_grun;    // per 32 positions: the last run that starts at or before position 32 g
   DevBuf<uint32_t> bin_runs;    // [n_runs + 32] first V slot - first position of each run (mod 2^32); 32 spare
   DevBuf<uint2> bin_chunks;     // [steps s0, s1) of one block: a warp's unit of pass A
-  DevBuf<uint32_t> bin_blk;     // [bin_blocks] source block of each of pass A's block ranks
-  DevBuf<uint2> bin_tasks;      // (first chunk, chunk count | block rank << 8)
-  uint32_t bin_n_tasks = 0;
+  // k_pr_cb<CB_FUSED>'s tasks over the union of the hot blocks and pass A's source blocks, fattest blocks first
+  // (bytes of ids and values), a block's tasks consecutive: (first hot chunk, first pass-A chunk, hot chunks |
+  // pass-A chunks << 8, source block).  Task i of a block holds the block's i-th run of up to CB_TASK_CHUNKS hot
+  // chunks (hot.tasks cuts them) and its i-th run of up to CB_TASK_CHUNKS pass-A chunks; either may be empty.
+  DevBuf<uint4> tasks;
+  uint32_t n_tasks = 0;
   // pass B: one block per partition (KB = partitions), one segment per local row (a padding group when the row
   // has no cold edge); its partials are the cold sums of the local rows
   CbStream virt;
   uint64_t bytes() const {
     return val.bytes() + bin_ids.bytes() + bin_bits.bytes() + bin_grun.bytes() + bin_runs.bytes() +
-           bin_chunks.bytes() + bin_blk.bytes() + bin_tasks.bytes() + virt.bytes();
+           bin_chunks.bytes() + tasks.bytes() + virt.bytes();
   }
 };
 
@@ -141,7 +146,7 @@ enum class PrFix : uint32_t {
   NONE,    // no segment is cut
   FIXUP,   // a k_pr_fixup launch before k_pr_sell: some cut row is completed by its k_pr_sell lane (few hot blocks)
   SELL,    // k_pr_sell's first warps: every cut row is completed later, by k_pr_finish (rows below n_fin)
-  PASS_A,  // pass A's first warps (virtual blocks): k_pr_finish completes every row
+  PASS_B,  // pass B's first warps (virtual blocks): k_pr_finish completes every row
 };
 
 struct PrPlan {
@@ -170,11 +175,11 @@ struct PrPlan {
   // virtual blocks (vb: they take the cold edges, the SELL slices above are empty and k_pr_sell does not run)
   bool vb = false;
   PrVBlocks v;
-  unsigned grid_bin = 0, grid_vb = 0;  // persistent CTAs of pass A and pass B
+  unsigned grid_vb = 0;      // persistent CTAs of pass B
   // state (single-GPU path; the shard API brings its own vectors)
   DevBuf<float> x[2];
   DevBuf<float> scores;
-  unsigned grid_cb = 0, grid_sell = 0, grid_fin = 1;
+  unsigned grid_cb = 0, grid_sell = 0, grid_fin = 1;  // grid_cb: k_pr_cb<CB_MAIN>, or <CB_FUSED> (vb)
   uint32_t n_fin_warp = 0;   // rows [0, n_fin_warp) own segments in more than FIN_CTA_BLOCKS blocks
   uint32_t fin_u = 4;        // finish: row groups per warp iteration (template argument of k_pr_finish)
   uint32_t fin_hub_ctas = 0; // finish CTAs that take the hub groups (the others take rows [n_fin_warp, n_fin))
@@ -184,7 +189,7 @@ struct PrPlan {
   DevBuf<double> block_err;  // per CTA error partials (SELL CTAs, then finish CTAs)
   DevBuf<double> err_hist;   // error of each sweep of the current batch
   DevBuf<uint32_t> ctrl;     // [0] = done flag (sweep number at which tolerance was met), [1] = ticket
-  size_t smem_cb = 0;        // k_pr_cb<CB_MAIN> and pass A: a source block and its zero slot
+  size_t smem_cb = 0;        // k_pr_cb<CB_MAIN> and <CB_FUSED>: a source block and its zero slot
   size_t smem_vb = 0;        // pass B: its window of V and the zero slot
   std::vector<cudaEvent_t> prof_events;
   // GB_PR_TRACE=1 (diagnostics): CUDA events between the kernels of every sweep; averages are printed
@@ -196,8 +201,8 @@ struct PrPlan {
            slice_meta.bytes() + x[0].bytes() + x[1].bytes() + scores.bytes() + block_err.bytes() + err_hist.bytes() +
            v.bytes();
   }
-  // task cursors: k_pr_cb's ranges, then pass A's, then pass B's (the finish kernel resets them all)
-  uint32_t task_ranges() const { return grid_cb + grid_bin + grid_vb; }
+  // task cursors: k_pr_cb's ranges, then pass B's (the finish kernel resets them all)
+  uint32_t task_ranges() const { return grid_cb + grid_vb; }
 };
 
 // blocks in which local row l owns a segment: the first j with nrows[j] <= l (nrows is non-increasing)

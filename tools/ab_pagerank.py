@@ -91,8 +91,11 @@ def main():
     for r in runs:
         for l in r["trace"]:
             m = re.search(r"k_pr_cb ([\d.]+)\s+pass A ([\d.]+)\s+pass B ([\d.]+)\s+k_pr_finish ([\d.]+)", l)
-            if m:
+            if m:  # k_pr_cb and pass A as two launches
                 kern[r["tag"]] = dict(zip(("k_pr_cb", "pass_a", "pass_b", "k_pr_finish"), map(float, m.groups())))
+            m = re.search(r"k_pr_cb with pass A ([\d.]+)\s+pass B ([\d.]+)\s+k_pr_finish ([\d.]+)", l)
+            if m:  # pass A inside k_pr_cb's tasks
+                kern[r["tag"]] = dict(zip(("k_pr_cb_with_pass_a", "pass_b", "k_pr_finish"), map(float, m.groups())))
     summary = {"card": card.strip(), "bit_identical_scores": same, "kernel_ms": kern,
                "runs": [{k: r.get(k) for k in ("tag", "tree", "exit", "value", "e2e", "verified")} for r in runs]}
     (out / "ab.json").write_text(json.dumps(summary, indent=1))

@@ -391,7 +391,7 @@ def vblocks(plan, built, window=VB_WINDOW):
 
 
 def vb_pass_a(plan, vb, fills=None):
-    """pass A (k_pr_cb<CB_BIN> / bin_chunk), chunk by chunk, step by step, lane by lane: the source of every slot
+    """pass A (bin_chunk in k_pr_cb<CB_FUSED>), chunk by chunk, step by step, lane by lane: the source of every slot
     of V it writes, how often it writes it, and the steps that take the run-window loop (more than 32 runs).  With
     sectors the lane of a run's last position also zeroes the run's pad slots (bin_fill_pad): each is counted in
     `writes` and marked -2 in V, and `fills` (a dict, when given) counts the fills by where the run ends: at a
@@ -505,6 +505,80 @@ def check_vblocks(plan, vb, built):
         assert V[int(vb["vbase"][k]) + seg[:d]].tolist() == built["sell"][l].tolist(), \
             "pass B's ids resolve to the sources of the row's cold edges, in CSR order"
     assert vb["edges"] == sum(len(built["sell"][l]) for l in range(plan["n_loc"]))
+
+
+# ---- k_pr_cb's chunks and tasks (cb_chunk_table, layout_fused_tasks in pr_layout.cu) ----------------------------
+CB_TASK_CHUNKS = 32
+
+
+def _cb_cut(goff_j, nr, gend, q, C):
+    """cb_cut of k_cb_chunks: where a chunk boundary aimed at group q of a block lands -> (group, row, the boundary
+    lies inside a segment longer than C)"""
+    if q >= gend:
+        return gend, nr, False
+    lo = int(np.searchsorted(goff_j, q, side="right")) - 1
+    s0 = int(goff_j[lo])
+    s1 = int(goff_j[lo + 1]) if lo + 1 < nr else gend
+    if s0 == q:
+        return q, lo, False
+    if s1 - s0 > C:
+        return q, lo, True
+    return s1, lo + 1, False
+
+
+def hot_chunks(plan, goff, sms=H100_SMS, T=CB_TASK_CHUNKS):
+    """cb_chunk_table of the hot blocks' stream: the chunks (g0, g1, hot rank j) in block order, the tasks (first
+    chunk, chunks, j) of up to T consecutive chunks of one block, and n_fix, the chunks whose end cuts a segment
+    that goes on past the next chunk's start (the fix list of k_pr_fixup / pass B)"""
+    NG = int(goff[-1])
+    if NG == 0:
+        return [], [], 0
+    gbeg = goff[plan["poff"]]
+    C = min(max(NG // (sms * 8 * T), 16384 // T), 65536 // T)
+    C = max(32, (C + 31) // 32 * 32)
+    chunks, tasks, n_fix = [], [], 0
+    for j in range(plan["KB"]):
+        g0, g1, nr = int(gbeg[j]), int(gbeg[j + 1]), int(plan["nrows"][j])
+        Cj = min(C, max(min(64, C), ((g1 - g0) // 64 + 63) // 64 * 64))
+        nc = (g1 - g0 + Cj - 1) // Cj
+        goff_j = goff[plan["poff"][j]:plan["poff"][j] + nr]
+        c0 = len(chunks)
+        for k in range(nc):
+            a = _cb_cut(goff_j, nr, g1, g0 + k * Cj, Cj)
+            b = (g1, nr, False) if k + 1 == nc else _cb_cut(goff_j, nr, g1, g0 + (k + 1) * Cj, Cj)
+            interior = a[2] and (b[1] if b[2] else b[1] - 1) == a[1]
+            n_fix += b[2] and not interior
+            chunks.append((a[0], b[0], j))
+        tasks += [(c0 + c, min(nc, c + T) - c, j) for c in range(0, nc, T)]
+    return chunks, tasks, n_fix
+
+
+def fused_tasks(plan, goff, vb, sms=H100_SMS):
+    """layout_fused_tasks: k_pr_cb<CB_FUSED>'s tasks (first hot chunk, hot chunks, first pass-A chunk, pass-A
+    chunks, source block).  Source blocks with hot or pass-A chunks, fattest first by the bytes their chunks stream
+    (8 per hot group, 6 per pass-A position: a 2-byte id and a 4-byte value), ties by block; task i of a block
+    takes the block's i-th hot task and its i-th run of CB_TASK_CHUNKS pass-A chunks.  Also returns the hot
+    chunks and tasks and n_fix (hot_chunks)."""
+    chunks, htasks, n_fix = hot_chunks(plan, goff, sms)
+    nblk = plan["nblk"]
+    nbytes = np.zeros(nblk, np.int64)
+    hot_of = [[] for _ in range(nblk)]
+    for t in htasks:
+        b = int(plan["blk"][t[2]])
+        hot_of[b].append(t)
+        nbytes[b] += sum(8 * (chunks[c][1] - chunks[c][0]) for c in range(t[0], t[0] + t[1]))
+    bin_blk = vb["pos_blk"][vb["bin_chunks"][:, 0] * BIN_STEP]
+    a_first = np.searchsorted(bin_blk, np.arange(nblk))
+    a_count = np.bincount(bin_blk, minlength=nblk)
+    nbytes += 6 * BIN_STEP * ((vb["bcnt"] + BIN_STEP - 1) // BIN_STEP)
+    tasks = []
+    for b in sorted(np.flatnonzero(nbytes), key=lambda b: -nbytes[b]):
+        na_all = int(a_count[b])
+        for i in range(max(len(hot_of[b]), (na_all + CB_TASK_CHUNKS - 1) // CB_TASK_CHUNKS)):
+            h0, nh = hot_of[b][i][:2] if i < len(hot_of[b]) else (0, 0)
+            a0 = min(na_all, i * CB_TASK_CHUNKS)
+            tasks.append((h0, nh, int(a_first[b]) + a0, min(na_all - a0, CB_TASK_CHUNKS), int(b)))
+    return dict(tasks=tasks, hot_chunks=chunks, hot_tasks=htasks, n_fix=n_fix, bin_blk=bin_blk)
 
 
 def random_graph(rng, n, m, skew=1.5):
