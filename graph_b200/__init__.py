@@ -20,7 +20,8 @@ from . import _capi
 from ._capi import GraphB200Error, check, lib
 
 __all__ = ["DiGraph", "Graph", "Layout", "FileFormat", "PageRankResult", "WccResult",
-           "TriangleCountResult", "SsspResult", "PageRankConfig", "WccConfig", "DeltaSteppingConfig",
+           "TriangleCountResult", "SsspResult", "LabelStats", "NodeLabelIndex", "NeighborLabelFrequencies",
+           "NeighborLabelFrequency", "PageRankConfig", "WccConfig", "DeltaSteppingConfig",
            "GraphB200Error", "device_count", "set_device", "write_graph500", "wcc_csr",
            "triangle_count_csr", "sssp_csr"]
 
@@ -145,6 +146,8 @@ class FileFormat:
     Graph500 = _Enum("FileFormat", "Graph500", 0)
     EdgeList = _Enum("FileFormat", "EdgeList", 1)
     Binary = _Enum("FileFormat", "Binary", 2)  # SerializeGraphOp's file (input/binary.rs); see serialize()
+    # node-labelled .graph file (input/dotgraph.rs); load() drops the labels, load_labeled() keeps them
+    DotGraph = _Enum("FileFormat", "DotGraph", 3)
 
 
 def _layout_value(layout) -> int:
@@ -237,13 +240,86 @@ class SsspResult:
         return f'SsspResult {{ distances: "[... {len(self._distances)} values]", took: {_took(self.micros)} }}'
 
 
+# ---- structures over a labelled graph (crates/builder/src/input/dotgraph.rs) ------------------------
+class LabelStats:
+    """LabelStats (dotgraph.rs:213-219): max_degree is the largest degree of the graph, label_count the number
+    of distinct labels, label_frequency a dict label -> number of nodes."""
+
+    def __init__(self, max_degree, label_count, max_label, max_label_frequency, label_frequency):
+        self.max_degree, self.label_count, self.max_label = max_degree, label_count, max_label
+        self.max_label_frequency, self.label_frequency = max_label_frequency, label_frequency
+
+    def __repr__(self):
+        return (f"LabelStats {{ max_degree: {self.max_degree}, label_count: {self.label_count}, "
+                f"max_label: {self.max_label}, max_label_frequency: {self.max_label_frequency} }}")
+
+
+class NodeLabelIndex:
+    """NodeLabelIndex (dotgraph.rs:430-532): a CSR with max_label + 1 rows; nodes(label) lists the nodes with that
+    label, ascending (read-only)."""
+
+    def __init__(self, offsets, nodes):
+        offsets.flags.writeable = False
+        nodes.flags.writeable = False
+        self.offsets, self._nodes = offsets, nodes
+
+    def nodes(self, label: int) -> np.ndarray:
+        if not 0 <= label < len(self.offsets) - 1:
+            raise IndexError(f"label {label} out of range for an index of {len(self.offsets) - 1} labels")
+        return self._nodes[self.offsets[label]:self.offsets[label + 1]]
+
+
+class NeighborLabelFrequency:
+    """NeighborLabelFrequency (dotgraph.rs:337-365): the labels of one node's neighbours and how often each
+    occurs.  get(label) is None for a label that does not occur; iteration yields (label, count) pairs, labels
+    ascending."""
+
+    def __init__(self, labels, counts):
+        self._labels, self._counts = labels, counts
+
+    def get(self, label: int):
+        i = int(np.searchsorted(self._labels, label))
+        if i < len(self._labels) and int(self._labels[i]) == label:
+            return int(self._counts[i])
+        return None
+
+    def __len__(self):
+        return len(self._labels)
+
+    def is_empty(self) -> bool:
+        return len(self._labels) == 0
+
+    def __iter__(self):
+        return zip(self._labels.tolist(), self._counts.tolist())
+
+    iter = __iter__
+
+
+class NeighborLabelFrequencies:
+    """NeighborLabelFrequencies (dotgraph.rs:367-427) as a pair CSR: node u's (label, count) pairs are
+    labels / counts[offsets[u]:offsets[u + 1]], labels ascending.  `micros` is the call's time, `device_ms` the
+    CUDA-event time of its device work."""
+
+    def __init__(self, offsets, labels, counts, micros=0, device_ms=0.0):
+        for a in (offsets, labels, counts):
+            a.flags.writeable = False
+        self.offsets, self.labels, self.counts = offsets, labels, counts
+        self.micros, self.device_ms = micros, device_ms
+
+    def neighbor_frequency(self, node: int) -> NeighborLabelFrequency:
+        if not 0 <= node < len(self.offsets) - 1:
+            raise IndexError(f"node {node} out of range for a graph with {len(self.offsets) - 1} nodes")
+        a, b = int(self.offsets[node]), int(self.offsets[node + 1])
+        return NeighborLabelFrequency(self.labels[a:b], self.counts[a:b])
+
+
 # ---- input files (crates/builder/src/input/{graph500,edgelist}.rs) --------------------------------
 # DiGraph.load / Graph.load stream the file to the device and parse it there (csrc/load.cu).  The host
 # readers below (csrc/io.cu) give the same edges; they serve the Flight server's weighted undirected graphs
 # and are the reference the device loader is tested against.
 def _load_args(path, file_format, layout):
     """(path bytes, format value, layout value) for gb_*_load_u32; raises what opening the file raises."""
-    if file_format in (FileFormat.Graph500, FileFormat.EdgeList, FileFormat.Binary):
+    if file_format in (FileFormat.Graph500, FileFormat.EdgeList, FileFormat.Binary, FileFormat.DotGraph):
         fmt = file_format.value
     else:
         raise TypeError(f"unknown file format {file_format!r}")
@@ -330,6 +406,19 @@ def _ptr(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+def _node_values(values, node_count: int) -> np.ndarray:
+    """The labels of from_numpy(node_values=...): one u32 per node; their number is the node count."""
+    v = np.asarray(values)
+    if v.ndim != 1 or len(v) == 0:
+        raise ValueError("node_values must be a non-empty 1-D array with one label per node")
+    if v.dtype != np.uint32:
+        if not np.issubdtype(v.dtype, np.integer) or v.min() < 0 or v.max() > 0xFFFFFFFF:
+            raise TypeError("node values must be 32-bit unsigned integers")
+    if node_count and node_count != len(v):
+        raise ValueError(f"node_count {node_count} differs from the {len(v)} node values")
+    return np.ascontiguousarray(v, dtype=np.uint32)
+
+
 def _torch_edges(src, dst, weights):
     """Device u32 id tensors (narrowed and range-checked on the device), the weights, and torch's current
     stream on the graph's device, for gb_*_from_device_edges_u32."""
@@ -405,7 +494,10 @@ class _Handle:
 
     def _views_alive(self) -> bool:
         # a numpy view keeps a reference to its base array
-        for off, tgt in self._host.values():
+        for key, entry in self._host.items():
+            if key == "labels":
+                continue
+            off, tgt = entry
             if sys.getrefcount(tgt) > 3:  # tuple entry + loop variable + getrefcount argument
                 return True
         return False
@@ -449,6 +541,26 @@ class _Handle:
         info = _capi.LoadInfo()
         check(lib.gb_graph_load_info(self._g, C.byref(info)))
         return info.as_dict()
+
+    def node_values(self) -> np.ndarray:
+        """NodeValues of a labelled graph: one label per node (read-only).  A graph without labels raises
+        ValueError."""
+        if "labels" not in self._host:
+            labels = np.empty(self.node_count(), np.uint32)
+            check(lib.gb_graph_node_values(self._g, _ptr(labels)))
+            labels.flags.writeable = False
+            self._host["labels"] = labels
+        return self._host["labels"]
+
+    def node_value(self, node: int) -> int:
+        """NodeValues::node_value (csr.rs:64-76)."""
+        labels = self.node_values()
+        if not 0 <= node < len(labels):
+            raise IndexError(f"node {node} out of range for a graph with {len(labels)} nodes")
+        return int(labels[node])
+
+    def has_node_values(self) -> bool:
+        return lib.gb_graph_node_values(self._g, None) == _capi.GB_OK
 
     def serialize(self, path) -> None:
         """SerializeGraphOp::serialize (graph_ops.rs:232-238): writes the graph as the binary file that
@@ -495,6 +607,13 @@ class DiGraph(_Handle):
         return _construct(DiGraph, lib.gb_digraph_load_u32, _device, *_load_args(path, file_format, layout), 0)
 
     @staticmethod
+    def load_labeled(path, layout=None) -> "DiGraph":
+        """A DotGraph (.graph) file as DirectedCsrGraph<u32, u32>: node_count = N, one label per node
+        (input/dotgraph.rs; GraphBuilder::file_format(DotGraphInput)).  Parsed on the device when large."""
+        p, _, lay = _load_args(path, FileFormat.DotGraph, layout)
+        return _construct(DiGraph, lib.gb_digraph_load_labeled_u32, _device, p, lay)
+
+    @staticmethod
     def load_weighted(path, layout=None, file_format=FileFormat.EdgeList) -> "DiGraph":
         """Weighted text edge list `<src> <dst> <f32>`, or a binary file with Target<NI, f32> records
         (DirectedCsrGraph<u32, (), f32>, for sssp)."""
@@ -512,8 +631,16 @@ class DiGraph(_Handle):
                           stream.cuda_stream)
 
     @staticmethod
-    def from_numpy(arr, layout=None, weights=None, node_count: int = 0) -> "DiGraph":
+    def from_numpy(arr, layout=None, weights=None, node_count: int = 0, node_values=None) -> "DiGraph":
+        """node_values: one u32 label per node (GraphBuilder::edges(..).node_values(..), builder.rs:388, 425);
+        the node count is then their number."""
         src, dst = _edges_from_numpy(arr)
+        if node_values is not None:
+            if weights is not None:
+                raise ValueError("a graph with node values carries no edge weights")
+            labels = _node_values(node_values, node_count)
+            return _construct(DiGraph, lib.gb_digraph_from_edges_labeled_u32, _device, _ptr(src), _ptr(dst), len(src),
+                              _ptr(labels), len(labels), _layout_value(layout))
         w = None if weights is None else np.ascontiguousarray(weights, dtype=np.float32)
         if w is not None and len(w) != len(src):
             raise ValueError("weights must have one entry per edge")
@@ -676,6 +803,12 @@ class Graph(_Handle):
         return _construct(Graph, lib.gb_graph_load_u32, _device, *_load_args(path, file_format, layout))
 
     @staticmethod
+    def load_labeled(path, layout=None) -> "Graph":
+        """A DotGraph (.graph) file as UndirectedCsrGraph<u32, u32>: node_count = N, one label per node."""
+        p, _, lay = _load_args(path, FileFormat.DotGraph, layout)
+        return _construct(Graph, lib.gb_graph_load_labeled_u32, _device, p, lay)
+
+    @staticmethod
     def from_torch(src, dst, node_count: int = 0, layout=None) -> "Graph":
         """From contiguous 1-D int32 / int64 CUDA tensors on the graph's device, without a host copy."""
         s, d, _, m, stream = _torch_edges(src, dst, None)
@@ -683,8 +816,13 @@ class Graph(_Handle):
                           int(node_count), _layout_value(layout), stream.cuda_stream)
 
     @staticmethod
-    def from_numpy(arr, layout=None, node_count: int = 0) -> "Graph":
+    def from_numpy(arr, layout=None, node_count: int = 0, node_values=None) -> "Graph":
+        """node_values: one u32 label per node; the node count is then their number."""
         src, dst = _edges_from_numpy(arr)
+        if node_values is not None:
+            labels = _node_values(node_values, node_count)
+            return _construct(Graph, lib.gb_graph_from_edges_labeled_u32, _device, _ptr(src), _ptr(dst), len(src),
+                              _ptr(labels), len(labels), _layout_value(layout))
         return Graph._from_edges(src, dst, node_count, layout)
 
     @staticmethod
@@ -725,6 +863,39 @@ class Graph(_Handle):
         _, micros = _timed(go)
         self._host.clear()
         self.load_micros += micros
+
+    def label_stats(self) -> LabelStats:
+        """LabelStats::from_graph (dotgraph.rs:220-313) of a labelled graph."""
+        st = _capi.LabelStatsInfo()
+        check(lib.gb_label_stats(self._g, C.byref(st), None, None))
+        labels = np.empty(st.label_count, np.uint32)
+        counts = np.empty(st.label_count, np.uint64)
+        check(lib.gb_label_stats(self._g, C.byref(st), _ptr(labels), _ptr(counts)))
+        return LabelStats(int(st.max_degree), int(st.label_count), int(st.max_label), int(st.max_label_frequency),
+                          dict(zip(labels.tolist(), counts.tolist())))
+
+    def node_label_index(self) -> NodeLabelIndex:
+        """NodeLabelIndex::from_stats(node_count, &label_stats, node_value) (dotgraph.rs:430-532)."""
+        max_label = C.c_uint32(0)
+        check(lib.gb_node_label_index(self._g, C.byref(max_label), None, None))
+        offsets = np.empty(max_label.value + 2, np.uint32)
+        nodes = np.empty(self.node_count(), np.uint32)
+        check(lib.gb_node_label_index(self._g, None, _ptr(offsets), _ptr(nodes)))
+        return NodeLabelIndex(offsets, nodes)
+
+    def neighbor_label_frequencies(self) -> NeighborLabelFrequencies:
+        """NeighborLabelFrequencies::from_graph (dotgraph.rs:367-427), computed on the device."""
+        cap = int(self._info.target_count)
+        offsets = np.empty(self.node_count() + 1, np.uint32)
+        labels = np.empty(max(cap, 1), np.uint32)
+        counts = np.empty(max(cap, 1), np.uint32)
+
+        def go():
+            check(lib.gb_neighbor_label_frequencies(self._g, _ptr(offsets), _ptr(labels), _ptr(counts)))
+        _, micros = _timed(go)
+        pairs = int(offsets[-1])
+        return NeighborLabelFrequencies(offsets, labels[:pairs].copy(), counts[:pairs].copy(), micros,
+                                        self.last_timing()["total_ms"])
 
     def global_triangle_count(self) -> TriangleCountResult:
         """global_triangle_count(&graph) (triangle_count.rs:22-86)."""

@@ -95,6 +95,11 @@ class SsspCsrInfo(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class LabelStatsInfo(C.Structure):
+    _fields_ = [("max_degree", C.c_uint32), ("max_label", C.c_uint32), ("label_count", C.c_uint64),
+                ("max_label_frequency", C.c_uint64)]
+
+
 class GraphB200Error(RuntimeError):
     """CUDA / allocation failure inside libgraph_b200."""
 
@@ -125,6 +130,16 @@ SIGNATURES = {
     "gb_digraph_load_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
     "gb_graph_load_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.c_int, C.POINTER(_P)]),
     "gb_graph_load_info": (C.c_int, [_P, C.POINTER(LoadInfo)]),
+    "gb_digraph_load_labeled_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.POINTER(_P)]),
+    "gb_graph_load_labeled_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.POINTER(_P)]),
+    "gb_digraph_from_edges_labeled_u32": (C.c_int, [C.c_int, _P, _P, C.c_uint64, _P, C.c_uint32, C.c_int,
+                                                    C.POINTER(_P)]),
+    "gb_graph_from_edges_labeled_u32": (C.c_int, [C.c_int, _P, _P, C.c_uint64, _P, C.c_uint32, C.c_int,
+                                                  C.POINTER(_P)]),
+    "gb_graph_node_values": (C.c_int, [_P, _P]),
+    "gb_label_stats": (C.c_int, [_P, C.POINTER(LabelStatsInfo), _P, _P]),
+    "gb_node_label_index": (C.c_int, [_P, C.POINTER(C.c_uint32), _P, _P]),
+    "gb_neighbor_label_frequencies": (C.c_int, [_P, _P, _P, _P]),
     "gb_digraph_from_device_edges_u32": (C.c_int, [C.c_int, _P, _P, _P, C.c_uint64, C.c_uint32, C.c_int, _P,
                                                    C.POINTER(_P)]),
     "gb_graph_from_device_edges_u32": (C.c_int, [C.c_int, _P, _P, C.c_uint64, C.c_uint32, C.c_int, _P,

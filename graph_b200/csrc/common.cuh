@@ -16,6 +16,7 @@
 
 #include "../../include/graph_b200.h"
 #include "csr_split.h"
+#include "dotgraph_line.h"
 
 namespace gb {
 
@@ -309,6 +310,9 @@ struct gb_graph {
   mutable gb::PrPlan* pr_plan = nullptr;  // lazily built PageRank layout (pagerank.cu)
   mutable gb_timing timing{};
   gb_load_info load{};  // filled by gb_[di]graph_load_u32 (load.cu)
+  // NodeValues of a labelled twin (one u32 label per node), NULL otherwise.  Only labels.cu reads them;
+  // to_undirected copies them and make_degree_ordered leaves them where they are (graph_ops.rs:511-538).
+  gb::DevBuf<uint32_t> labels;
 };
 
 namespace gb {
@@ -363,6 +367,18 @@ gb_status graph_from_device_arrays(int device, gb_graph_kind kind, const uint32_
 // k-th occurrence of t in out-row s.  Fails when the in-CSR is not the transpose of the out-CSR.  Runs on the
 // graph's stream; the caller holds g->mu.
 gb_status in_csr_values(const gb_graph* g, DevBuf<float>* in_w);
+
+// ---- DotGraph files (io.cu; grammar in dotgraph_line.h) ----
+// The header from the first bytes of the file: its whole first line, or the whole file when it has no '\n'.
+gb_status dot_read_header(const char* text, uint64_t len, DotHeader* h);
+// The node and edge lines of a whole file in host memory: labels[N], src[M], dst[M].  A NULL labels (or src, and
+// with it dst) skips those stores: the lines are still checked.
+gb_status dot_read_host(const char* text, uint64_t len, const DotHeader& h, uint32_t* labels, uint32_t* src,
+                        uint32_t* dst);
+// The failure of a DotGraph read: `code` on 1-based line `line`, or DOT_MISSING with `have` of h.lines lines.
+gb_status dot_fail(uint32_t code, uint64_t line, const DotHeader& h, uint64_t have);
+// Copies n labels (host or device memory, by `kind`) into g->labels on g's stream and waits for the copy.
+gb_status attach_labels(gb_graph* g, const uint32_t* labels, cudaMemcpyKind kind);
 
 // the devices of a communicator, in its order (multi.cu); peer access among them is enabled
 const std::vector<int>& comm_devices(const gb_comm* c);

@@ -655,6 +655,29 @@ static gb_status graph_from_host_edges(int device, gb_graph_kind kind, const uin
   return GB_OK;
 }
 
+gb_status attach_labels(gb_graph* g, const uint32_t* labels, cudaMemcpyKind kind) {
+  GB_TRY(g->labels.alloc(g->n));
+  GB_CUDA(cudaMemcpyAsync(g->labels.p, labels, (size_t)g->n * 4, kind, g->stream));
+  GB_CUDA(cudaStreamSynchronize(g->stream));
+  return GB_OK;
+}
+
+// GraphBuilder::edges(..).node_values(..) (builder.rs:388, 425): node_count = the number of labels
+static gb_status graph_from_host_edges_labeled(int device, gb_graph_kind kind, const uint32_t* src,
+                                               const uint32_t* dst, uint64_t m, const uint32_t* labels,
+                                               uint32_t label_count, gb_layout layout, gb_graph** out) {
+  GB_REQUIRE(out != nullptr, "graph out-pointer is NULL");
+  GB_REQUIRE(labels != nullptr, "labels is NULL");
+  GB_REQUIRE(label_count > 0, "a labelled graph needs at least one node (label_count = 0)");
+  gb_graph* raw = nullptr;
+  GB_TRY(graph_from_host_edges(device, kind, src, dst, nullptr, m, label_count, layout, &raw));
+  GraphPtr g(raw);
+  DeviceGuard guard(device);
+  GB_TRY(attach_labels(g.get(), labels, cudaMemcpyHostToDevice));
+  *out = g.release();
+  return GB_OK;
+}
+
 static gb_status require_device_array(const void* p, int device, const char* what) {
   cudaPointerAttributes a{};
   if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
@@ -832,6 +855,29 @@ gb_status gb_graph_from_edges_u32(int device, const uint32_t* src, const uint32_
   return graph_from_host_edges(device, GB_KIND_UNDIRECTED, src, dst, nullptr, m, n, layout, graph);
 }
 
+gb_status gb_digraph_from_edges_labeled_u32(int device, const uint32_t* src, const uint32_t* dst, uint64_t m,
+                                            const uint32_t* labels, uint32_t label_count, gb_layout layout,
+                                            gb_graph** graph) {
+  return graph_from_host_edges_labeled(device, GB_KIND_DIRECTED, src, dst, m, labels, label_count, layout, graph);
+}
+
+gb_status gb_graph_from_edges_labeled_u32(int device, const uint32_t* src, const uint32_t* dst, uint64_t m,
+                                          const uint32_t* labels, uint32_t label_count, gb_layout layout,
+                                          gb_graph** graph) {
+  return graph_from_host_edges_labeled(device, GB_KIND_UNDIRECTED, src, dst, m, labels, label_count, layout, graph);
+}
+
+gb_status gb_graph_node_values(const gb_graph* g, uint32_t* labels) {
+  GB_REQUIRE(g != nullptr, "NULL graph");
+  if (!g->labels.p) return fail(GB_ERR_UNSUPPORTED, "the graph has no node values (it was built without labels)");
+  if (!labels) return GB_OK;
+  DeviceGuard guard(g->device);
+  std::lock_guard<std::mutex> lock(g->mu);
+  GB_CUDA(cudaMemcpyAsync(labels, g->labels.p, (size_t)g->n * 4, cudaMemcpyDeviceToHost, g->stream));
+  GB_CUDA(cudaStreamSynchronize(g->stream));
+  return GB_OK;
+}
+
 gb_status gb_digraph_from_device_edges_u32(int device, const uint32_t* d_src, const uint32_t* d_dst,
                                            const float* d_weights, uint64_t m, uint32_t n, gb_layout layout,
                                            void* stream, gb_graph** graph) {
@@ -904,6 +950,7 @@ gb_status gb_graph_free(gb_graph* g) {
   if (g->pr_plan) free_pr_plan(g->pr_plan);
   g->out = DevCsr();
   g->in = DevCsr();
+  g->labels = DevBuf<uint32_t>();
   if (g->ev_begin) cudaEventDestroy(g->ev_begin);
   if (g->ev_end) cudaEventDestroy(g->ev_end);
   if (g->stream) cudaStreamDestroy(g->stream);
@@ -923,7 +970,7 @@ gb_status gb_graph_get_info(const gb_graph* g, gb_graph_info* info) {
   info->edge_count = (g->kind == GB_KIND_UNDIRECTED) ? g->out.len / 2 : g->out.len;
   info->has_weights = g->out.w.p != nullptr;
   info->device = g->device;
-  info->device_bytes = g->out.bytes() + g->in.bytes() + pr_plan_bytes(g->pr_plan);
+  info->device_bytes = g->out.bytes() + g->in.bytes() + g->labels.bytes() + pr_plan_bytes(g->pr_plan);
   return GB_OK;
 }
 
@@ -992,12 +1039,14 @@ gb_status gb_to_undirected(const gb_graph* dg, gb_layout layout, gb_graph** grap
   if (m) k_expand_rows<<<grid_for((uint64_t)dg->n * 32, 256), 256, 0, g->stream>>>(dg->out.off.p, dg->n, rows.p);
   GB_CUDA(cudaGetLastError());
   GB_TRY(build_graph_csrs(g.get(), rows.p, dg->out.tgt.p, nullptr, m, layout));
+  if (dg->labels.p) GB_TRY(attach_labels(g.get(), dg->labels.p, cudaMemcpyDeviceToDevice));  // csr.rs:400
   *graph = g.release();
   return GB_OK;
 }
 
 // make_degree_ordered: graph_ops.rs:511-638.  (degree, id) pairs sorted descending (:555), so
-// ties give the larger old id the smaller new id; rows rewritten and sorted ascending (:629).
+// ties give the larger old id the smaller new id; rows rewritten and sorted ascending (:629).  Like the
+// reference's swap_csr (:511-538) it leaves a labelled twin's labels where they are: not permuted.
 gb_status gb_make_degree_ordered(gb_graph* g) {
   GB_REQUIRE(g != nullptr, "NULL graph");
   if (g->kind != GB_KIND_UNDIRECTED)

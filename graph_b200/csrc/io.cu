@@ -2,6 +2,8 @@
 //
 //   Graph500 packed edges   crates/builder/src/input/graph500.rs:63-127
 //   text edge lists         crates/builder/src/input/edgelist.rs:181-279
+//   DotGraph (.graph)       crates/builder/src/input/dotgraph.rs:136-203 (one thread: the device loader
+//                           takes every file it is worth splitting)
 //
 // Like the reference the work is split into one contiguous chunk per hardware thread (edgelist.rs:
 // 186-212 cuts at line boundaries); unlike it the chunks are written at prefix offsets, so the edge
@@ -35,6 +37,53 @@ static void parallel_chunks(unsigned threads, F&& body) {
   pool.reserve(threads);
   for (unsigned t = 0; t < threads; ++t) pool.emplace_back([&body, t] { body(t); });
   for (auto& th : pool) th.join();
+}
+
+// the end of the line that starts at p: the position of its '\n', or len
+static uint64_t line_end(const char* text, uint64_t p, uint64_t len) {
+  const void* nl = std::memchr(text + p, '\n', len - p);
+  return nl ? (uint64_t)(static_cast<const char*>(nl) - text) : len;
+}
+
+gb_status dot_fail(uint32_t code, uint64_t line, const DotHeader& h, uint64_t have) {
+  if (code == DOT_MISSING) {
+    if (have == 0) return fail(GB_ERR_INVALID, "DotGraph file is empty: the header line \"t N M\" is missing");
+    return fail(GB_ERR_INVALID, "DotGraph file ends after %llu lines; its header declares 1 + %u node + %u edge lines",
+                (unsigned long long)have, h.nodes, h.edges);
+  }
+  return fail(GB_ERR_INVALID, "DotGraph line %llu: %s", (unsigned long long)line, dot_error_text(code));
+}
+
+gb_status dot_read_header(const char* text, uint64_t len, DotHeader* h) {
+  if (len == 0) return dot_fail(DOT_MISSING, 0, *h, 0);
+  const uint64_t eol = line_end(text, 0, len);
+  uint32_t v[2];
+  if (const uint32_t code = dot_line(text, 0, eol, 2, v)) return dot_fail(code, 1, *h, 0);
+  h->nodes = v[0];
+  h->edges = v[1];
+  h->lines = 1 + (uint64_t)v[0] + v[1];
+  h->body = eol < len ? eol + 1 : len;
+  return GB_OK;
+}
+
+gb_status dot_read_host(const char* text, uint64_t len, const DotHeader& h, uint32_t* labels, uint32_t* src,
+                        uint32_t* dst) {
+  uint64_t p = h.body;
+  for (uint64_t line = 1; line < h.lines; ++line) {  // 0-based: the header is line 0
+    if (p >= len) return dot_fail(DOT_MISSING, 0, h, line);
+    const uint64_t eol = line_end(text, p, len);
+    uint32_t v[3];
+    const bool node = line <= h.nodes;
+    if (const uint32_t code = dot_line(text, p, eol, node ? 3 : 2, v)) return dot_fail(code, line + 1, h, 0);
+    if (node) {
+      if (labels) labels[line - 1] = v[1];
+    } else if (src) {
+      src[line - 1 - h.nodes] = v[0];
+      dst[line - 1 - h.nodes] = v[1];
+    }
+    p = eol < len ? eol + 1 : len;
+  }
+  return GB_OK;
 }
 
 }  // namespace gb

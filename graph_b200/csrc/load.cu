@@ -24,6 +24,9 @@
 //   declines are listed (file offset, edge index) and re-parsed on the host with gb::parse_line.  Both build
 //   the graph from the device arrays (graph_from_device_arrays), so it is the one the host readers followed by
 //   gb_[di]graph_from_edges_u32 give.
+//   DotGraph: the text pipeline above, with the line index of every line.  The host reads the header "t N M" first;
+//   k_load_parse_dotgraph sends line 1..N to labels[line - 1] and line N+1..N+M to src / dst[line - 1 - N]
+//   (dotgraph_line.h), ignores the lines after them, and keeps the smallest (line, error) pair it meets.
 //   Binary: the host preads the headers (bin_parse gives the section table) and every chunk is cut against the
 //   table.  u32 sections without values go from the pinned buffer straight into their CSR array; a chunk that
 //   meets another section is staged with the bytes of the element it cuts carried in front, and k_bin_split
@@ -130,6 +133,50 @@ __global__ void __launch_bounds__(LOAD_BLOCK) k_load_parse_text(const uint4* __r
     if (pos + j + 1 < len) parse(pos + j + 1, e);
   }
   if (__syncthreads_or(wide) && threadIdx.x == 0) atomicOr(&ctr->wide, 1u);
+}
+
+// DotGraph lines (dotgraph_line.h), found as k_load_parse_text finds them; line_base = lines of the earlier chunks,
+// with the header as line 0.  The first error (smallest line) is kept as line << 3 | code in *first_error.  A NULL
+// labels (or src, and with it dst) skips those stores.
+__global__ void __launch_bounds__(LOAD_BLOCK) k_load_parse_dotgraph(const uint4* __restrict__ buf, uint64_t len,
+                                                                    const uint32_t* __restrict__ incl,
+                                                                    uint64_t line_base, uint32_t nodes,
+                                                                    uint64_t lines, uint32_t* __restrict__ labels,
+                                                                    uint32_t* __restrict__ src,
+                                                                    uint32_t* __restrict__ dst,
+                                                                    unsigned long long* __restrict__ first_error) {
+  using Scan = cub::BlockScan<uint32_t, LOAD_BLOCK>;
+  __shared__ typename Scan::TempStorage tmp;
+  const uint64_t i = (uint64_t)blockIdx.x * LOAD_BLOCK + threadIdx.x;
+  const uint64_t pos = 16 * i;
+  uint32_t m = newline_mask(buf[i], pos, len);
+  uint32_t before;
+  Scan(tmp).ExclusiveSum((uint32_t)__popc(m), before);
+  uint64_t line = line_base + (blockIdx.x ? incl[blockIdx.x - 1] : 0u) + before;
+  const char* text = reinterpret_cast<const char*>(buf);
+  auto parse = [&](uint64_t start, uint64_t ln) {
+    if (ln == 0 || ln >= lines) return;
+    uint64_t eol = start;
+    while (eol < len && text[eol] != '\n') ++eol;
+    uint32_t v[3];
+    const bool node = ln <= nodes;
+    const uint32_t code = dot_line(text, start, eol, node ? 3 : 2, v);
+    if (code) {
+      atomicMin(first_error, (unsigned long long)(ln << 3 | code));
+    } else if (node) {
+      if (labels) labels[ln - 1] = v[1];
+    } else if (src) {
+      src[ln - 1 - nodes] = v[0];
+      dst[ln - 1 - nodes] = v[1];
+    }
+  };
+  if (i == 0 && len > 0) parse(0, line_base);
+  while (m) {
+    const int j = __ffs(m) - 1;
+    m &= m - 1;
+    ++line;
+    if (pos + j + 1 < len) parse(pos + j + 1, line);
+  }
 }
 
 // PackedEdge{v0_low, v1_low, high} (graph500.rs:111-127): 4 records = 48 bytes = three 128-bit loads per
@@ -488,13 +535,15 @@ static gb_status grow(DevBuf<T>& b, uint64_t need, uint64_t want, uint64_t keep,
 struct LoadedEdges {
   DevBuf<uint32_t> src, dst;
   DevBuf<float> w;
+  DevBuf<uint32_t> labels;  // DotGraph: [N]
   uint64_t m = 0;
   uint32_t n = 0;  // 0: max id + 1
 };
 
 static gb_status load_file(int device, const InputFile& f, gb_file_format format, bool want_value,
-                           LoadedEdges* out, gb_load_info* info) {
+                           const DotHeader& dot, LoadedEdges* out, gb_load_info* info) {
   const bool g500 = format == GB_FORMAT_GRAPH500;
+  const bool dotgraph = format == GB_FORMAT_DOTGRAPH;
   ChunkReader rd(f.fd, device);
   const uint64_t m500 = f.bytes / 12;
   rd.plan(g500 ? 12 * m500 : f.bytes, g500 ? 48 : 1);  // Graph500: whole 4-record groups, a partial tail ignored
@@ -525,6 +574,11 @@ static gb_status load_file(int device, const InputFile& f, gb_file_format format
   if (g500) {
     GB_TRY(out->src.alloc(m500));
     GB_TRY(out->dst.alloc(m500));
+  }
+  DevBuf<unsigned long long> dot_error;  // line << 3 | code of the first bad line
+  if (dotgraph) {  // the caller allocated the arrays it wants filled
+    GB_TRY(dot_error.alloc(1));
+    GB_CUDA(cudaMemsetAsync(dot_error.p, 0xFF, 8, sp.work));
   }
 
   // what prepare() leaves for run(): the device chunk and where it starts in the file
@@ -591,6 +645,15 @@ static gb_status load_file(int device, const InputFile& f, gb_file_format format
     if (tiles) {
       GB_CUDA(cudaStreamSynchronize(sp.work));
       const uint64_t lines = hsmall[0] + (sg.ends_with_newline ? 0 : 1);
+      if (dotgraph) {
+        k_load_parse_dotgraph<<<(unsigned)tiles, LOAD_BLOCK, 0, sp.work>>>(d, sg.len, counts.p, m, dot.nodes,
+                                                                          dot.lines, out->labels.p, out->src.p,
+                                                                          out->dst.p, dot_error.p);
+        GB_CUDA(cudaGetLastError());
+        m += lines;
+        GB_CUDA(cudaEventRecord(st.parsed[r], sp.work));
+        continue;
+      }
       // size the arrays for the whole file from the lines per byte seen so far
       const uint64_t through = std::min(rd.read_end, (k + 1) * rd.chunk);
       const uint64_t est = (uint64_t)((double)(m + lines) * (double)rd.read_end / (double)through * 1.02) + 1024;
@@ -616,6 +679,18 @@ static gb_status load_file(int device, const InputFile& f, gb_file_format format
   GB_CUDA(cudaStreamSynchronize(sp.work));
   GB_REQUIRE(hc.wide == 0, g500 ? "Graph500 node id does not fit 32 bits" : "edge list node id does not fit 32 bits");
   if (g500) m = m500;
+  if (dotgraph) {
+    unsigned long long first = 0;
+    GB_CUDA(cudaMemcpyAsync(&first, dot_error.p, 8, cudaMemcpyDeviceToHost, sp.work));
+    GB_CUDA(cudaStreamSynchronize(sp.work));
+    if (first != ~0ull) return dot_fail((uint32_t)(first & 7), (first >> 3) + 1, dot, 0);
+    if (m < dot.lines) return dot_fail(DOT_MISSING, 0, dot, m);
+    out->m = dot.edges;
+    info->edges = dot.edges;
+    info->h2d_bytes = st.h2d;
+    GB_CUDA(cudaStreamSynchronize(sp.copy));
+    return GB_OK;
+  }
 
   // declined values: re-read each line and parse it with the host reader's own function
   if (hc.declined) {
@@ -837,6 +912,81 @@ static gb_status load_on_host(int device, gb_graph_kind kind, const InputFile& f
   return GB_OK;
 }
 
+// A labelled graph has N nodes, one per label (csr.rs:554-562 asserts that every edge id is below it); an unlabelled
+// one has max edge id + 1 (csr.rs:577-587), N only counting the node lines to skip.
+static gb_status dot_require_nodes(const DotHeader& h, bool labeled) {
+  GB_REQUIRE(!labeled || h.nodes > 0, "a labelled DotGraph needs at least one node line; the header declares N = 0");
+  return GB_OK;
+}
+// A read without stores (dot_fits false) always meets a bad or missing line and fails first, so this guards a case
+// that cannot arise: such a file never reaches the graph build.
+static gb_status dot_require_fits(const DotHeader& h, bool fits) {
+  GB_REQUIRE(fits, "DotGraph file is too short for the 1 + %u node + %u edge lines its header declares", h.nodes,
+             h.edges);
+  return GB_OK;
+}
+
+// a small DotGraph file: the host reader, then the upload of gb_[di]graph_from_edges[_labeled]_u32
+static gb_status load_dotgraph_on_host(int device, gb_graph_kind kind, const InputFile& f, gb_layout layout,
+                                       bool labeled, gb_graph** graph, gb_load_info* info) {
+  std::unique_ptr<char[]> bytes;
+  GB_TRY(f.read_all(&bytes));
+  DotHeader h;
+  GB_TRY(dot_read_header(bytes.get(), f.bytes, &h));
+  const bool fits = dot_fits(h, f.bytes);
+  std::vector<uint32_t> labels, src, dst;
+  try {
+    if (fits) labels.resize(labeled ? h.nodes : 0), src.resize(h.edges), dst.resize(h.edges);
+  } catch (const std::bad_alloc&) {
+    return fail(GB_ERR_OOM, "host allocation for %u labels and %u edges failed", h.nodes, h.edges);
+  }
+  GB_TRY(dot_read_host(bytes.get(), f.bytes, h, fits && labeled ? labels.data() : nullptr, fits ? src.data() : nullptr,
+                       fits ? dst.data() : nullptr));
+  GB_TRY(dot_require_fits(h, fits));
+  GB_TRY(dot_require_nodes(h, labeled));
+  if (labeled && kind == GB_KIND_DIRECTED)
+    GB_TRY(gb_digraph_from_edges_labeled_u32(device, src.data(), dst.data(), h.edges, labels.data(), h.nodes, layout,
+                                             graph));
+  else if (labeled)
+    GB_TRY(gb_graph_from_edges_labeled_u32(device, src.data(), dst.data(), h.edges, labels.data(), h.nodes, layout,
+                                           graph));
+  else if (kind == GB_KIND_DIRECTED)
+    GB_TRY(gb_digraph_from_edges_u32(device, src.data(), dst.data(), nullptr, h.edges, 0, layout, graph));
+  else
+    GB_TRY(gb_graph_from_edges_u32(device, src.data(), dst.data(), h.edges, 0, layout, graph));
+  info->edges = h.edges;
+  info->h2d_bytes = 8ull * h.edges + (labeled ? 4ull * h.nodes : 0);
+  return GB_OK;
+}
+
+// a larger DotGraph file (or any, with GB_LOAD_CHUNK_BYTES): the header on the host, the lines on the device
+static gb_status load_dotgraph_streamed(int device, gb_graph_kind kind, const InputFile& f, gb_layout layout,
+                                        bool labeled, gb_graph** graph, gb_load_info* info) {
+  // the first line, as the host reader sees it in the whole file
+  std::string head;
+  for (uint64_t want = std::min<uint64_t>(f.bytes, 4096);; want = std::min(f.bytes, 2 * want)) {
+    head.resize(want);
+    if (want && !pread_all(f.fd, &head[0], want, 0)) return fail(GB_ERR_INVALID, "reading %s failed", f.path);
+    if (want == f.bytes || std::memchr(head.data(), '\n', want)) break;
+  }
+  DotHeader h;
+  GB_TRY(dot_read_header(head.data(), head.size(), &h));
+  const bool fits = dot_fits(h, f.bytes);
+  LoadedEdges e;
+  if (fits) {
+    GB_TRY(e.src.alloc(h.edges));
+    GB_TRY(e.dst.alloc(h.edges));
+    if (labeled) GB_TRY(e.labels.alloc(h.nodes));
+  }
+  GB_TRY(load_file(device, f, GB_FORMAT_DOTGRAPH, false, h, &e, info));
+  GB_TRY(dot_require_fits(h, fits));
+  GB_TRY(dot_require_nodes(h, labeled));
+  GB_TRY(graph_from_device_arrays(device, kind, e.src.p, e.dst.p, nullptr, h.edges, labeled ? h.nodes : 0, layout,
+                                  nullptr, graph));
+  if (labeled) (*graph)->labels = std::move(e.labels);  // parsed on the device, so not part of h2d_bytes
+  return GB_OK;
+}
+
 // a small binary file: gb_binary_decode, then the upload of gb_[di]graph_from_csr_u32
 static gb_status load_binary_on_host(int device, gb_graph_kind kind, const InputFile& f, bool want_value,
                                      gb_graph** graph, gb_load_info* info) {
@@ -893,6 +1043,8 @@ struct TempFile {
 // interleaved on the device first)
 static gb_status serialize_graph(const gb_graph* g, const char* path) {
   GB_REQUIRE(g && path, "NULL argument");
+  if (g->labels.p)
+    return fail(GB_ERR_UNSUPPORTED, "a labelled graph cannot be serialized: NodeValues payloads are not written");
   GB_REQUIRE(g->out.tgt.p != nullptr, "this handle holds no out targets (page-rank-only twin) and cannot be serialized");
   DeviceGuard guard(g->device);
   std::lock_guard<std::mutex> lock(g->mu);
@@ -971,12 +1123,14 @@ static gb_status serialize_graph(const gb_graph* g, const char* path) {
 }
 
 static gb_status load_graph(int device, gb_graph_kind kind, const char* path, gb_file_format format,
-                            gb_layout layout, int with_values, gb_graph** graph) {
+                            gb_layout layout, int with_values, bool labeled, gb_graph** graph) {
   GB_REQUIRE(graph != nullptr, "graph out-pointer is NULL");
   GB_REQUIRE(path != nullptr, "path is NULL");
-  GB_REQUIRE(format == GB_FORMAT_GRAPH500 || format == GB_FORMAT_EDGE_LIST || format == GB_FORMAT_BINARY,
+  GB_REQUIRE(format == GB_FORMAT_GRAPH500 || format == GB_FORMAT_EDGE_LIST || format == GB_FORMAT_BINARY ||
+                 format == GB_FORMAT_DOTGRAPH,
              "unknown file format %d", (int)format);
-  GB_REQUIRE(!with_values || format != GB_FORMAT_GRAPH500, "only edge lists and binary files carry edge values");
+  GB_REQUIRE(!with_values || format == GB_FORMAT_EDGE_LIST || format == GB_FORMAT_BINARY,
+             "only edge lists and binary files carry edge values");
   GB_TRY(check_layout(layout));
   GB_TRY(require_device(device));
   DeviceGuard guard(device);
@@ -985,14 +1139,17 @@ static gb_status load_graph(int device, gb_graph_kind kind, const char* path, gb
   gb_load_info info{};
   info.file_bytes = f.bytes;
   const bool on_host = env_chunk_bytes() == 0 && f.bytes < LOAD_DEVICE_MIN_BYTES;
-  if (format == GB_FORMAT_BINARY) {
+  if (format == GB_FORMAT_DOTGRAPH) {
+    if (on_host) GB_TRY(load_dotgraph_on_host(device, kind, f, layout, labeled, graph, &info));
+    else GB_TRY(load_dotgraph_streamed(device, kind, f, layout, labeled, graph, &info));
+  } else if (format == GB_FORMAT_BINARY) {
     if (on_host) GB_TRY(load_binary_on_host(device, kind, f, with_values != 0, graph, &info));
     else GB_TRY(load_binary_streamed(device, kind, f, with_values != 0, graph, &info));
   } else if (on_host) {
     GB_TRY(load_on_host(device, kind, f, format, layout, with_values != 0, graph, &info));
   } else {
     LoadedEdges e;
-    GB_TRY(load_file(device, f, format, with_values != 0, &e, &info));
+    GB_TRY(load_file(device, f, format, with_values != 0, DotHeader{}, &e, &info));
     GB_TRY(graph_from_device_arrays(device, kind, e.src.p, e.dst.p, with_values ? e.w.p : nullptr, e.m, e.n, layout,
                                     nullptr, graph));
   }
@@ -1006,12 +1163,20 @@ extern "C" {
 
 gb_status gb_digraph_load_u32(int device, const char* path, gb_file_format format, gb_layout layout,
                               int with_values, gb_graph** graph) {
-  return gb::load_graph(device, GB_KIND_DIRECTED, path, format, layout, with_values, graph);
+  return gb::load_graph(device, GB_KIND_DIRECTED, path, format, layout, with_values, false, graph);
 }
 
 gb_status gb_graph_load_u32(int device, const char* path, gb_file_format format, gb_layout layout,
                             gb_graph** graph) {
-  return gb::load_graph(device, GB_KIND_UNDIRECTED, path, format, layout, 0, graph);
+  return gb::load_graph(device, GB_KIND_UNDIRECTED, path, format, layout, 0, false, graph);
+}
+
+gb_status gb_digraph_load_labeled_u32(int device, const char* path, gb_layout layout, gb_graph** graph) {
+  return gb::load_graph(device, GB_KIND_DIRECTED, path, GB_FORMAT_DOTGRAPH, layout, 0, true, graph);
+}
+
+gb_status gb_graph_load_labeled_u32(int device, const char* path, gb_layout layout, gb_graph** graph) {
+  return gb::load_graph(device, GB_KIND_UNDIRECTED, path, GB_FORMAT_DOTGRAPH, layout, 0, true, graph);
 }
 
 gb_status gb_graph_serialize(const gb_graph* graph, const char* path) { return gb::serialize_graph(graph, path); }

@@ -206,7 +206,11 @@ gb_status gb_binary_decode(const void* bytes, uint64_t len, gb_graph_kind kind, 
 typedef enum gb_file_format {
   GB_FORMAT_GRAPH500 = 0,  /* packed 12-byte records; node_count = edges / 16 */
   GB_FORMAT_EDGE_LIST = 1, /* text "<src> <dst>[ <f32>]"; node_count = max id + 1 */
-  GB_FORMAT_BINARY = 2     /* SerializeGraphOp's file (see gb_binary_decode): the CSRs as stored */
+  GB_FORMAT_BINARY = 2,    /* SerializeGraphOp's file (see gb_binary_decode): the CSRs as stored */
+  GB_FORMAT_DOTGRAPH = 3   /* node-labelled .graph file (input/dotgraph.rs:136-203); see gb_digraph_load_labeled_u32.
+                              Loaded by gb_[di]graph_load_u32 it gives the unlabelled DirectedCsrGraph<NI, ()> /
+                              UndirectedCsrGraph<NI, ()> (csr.rs:577-587, 781-791): node_count = max edge id + 1, as
+                              for an edge list, and the N node lines are only skipped. */
 } gb_file_format;
 /* with_values: read the third column of an edge list as f32 edge values (Graph500 has none).
  * A binary file's rows are kept byte for byte: `layout` is checked and otherwise ignored, as the reference
@@ -226,6 +230,65 @@ gb_status gb_graph_load_u32(int device, const char* path, gb_file_format format,
  * (s, t) edges.  The file is written to a temporary file in the same directory, which is renamed over
  * `path` on success and removed on failure.  GB_ERR_INVALID for a gb_digraph_for_page_rank_u32 twin. */
 gb_status gb_graph_serialize(const gb_graph* graph, const char* path);
+
+/* ---- node-labelled graphs (crates/builder/src/input/dotgraph.rs) ----------------------------------------------
+ * A labelled twin carries one u32 label per node (NodeValues::node_value, csr.rs:64-76) beside its CSRs: the
+ * DirectedCsrGraph<u32, u32> / UndirectedCsrGraph<u32, u32> the reference builds from a DotGraph file or from
+ * GraphBuilder::edges(..).node_values(..).  Its node_count is the number of labels, and every edge id must be
+ * below it (the reference asserts it, csr.rs:554-562); the CSRs are those gb_[di]graph_from_edges_u32 builds from
+ * the same edges with that node_count, byte for byte.  gb_to_undirected copies the labels (csr.rs:400).
+ * CAUTION: gb_make_degree_ordered relabels the CSR and, like the reference (graph_ops.rs:511-538, which swaps the
+ * CSR and leaves node_values alone), does NOT permute the labels: afterwards label[v] is the label of the node
+ * that had old id v, not of the node now called v.  gb_graph_serialize refuses a labelled twin
+ * (GB_ERR_UNSUPPORTED): NodeValues payloads are not written.
+ *
+ * DotGraph file (dotgraph.rs:136-203): the header line "t N M", then N node lines "v <id> <label> <degree>" in id
+ * order (the id and degree are skipped, the label kept), then M edge lines "e <src> <dst>" (kept in file order);
+ * lines after them are not read.  Each line's first 2 bytes are skipped unread (so `n` tags load too), numbers are
+ * leading ASCII digits and exactly one byte separates them.  GB_ERR_INVALID, with a message naming the line, for:
+ * fewer than 1 + N + M lines, a number without digits, bytes between the last number and the line end (a '\r'
+ * included), a number >= 2^32; the last line may lack its '\n'.  Loading follows gb_[di]graph_load_u32: files
+ * below 64 MiB are read on the host, larger ones (or any, with GB_LOAD_CHUNK_BYTES) are parsed on the device
+ * after the host has read the header; both give the same graph and the same errors and messages. */
+gb_status gb_digraph_load_labeled_u32(int device, const char* path, gb_layout layout, gb_graph** graph);
+gb_status gb_graph_load_labeled_u32(int device, const char* path, gb_layout layout, gb_graph** graph);
+/* GraphBuilder::edges(..).node_values(..).build() (builder.rs:388, 425): node_count = label_count >= 1 */
+gb_status gb_digraph_from_edges_labeled_u32(int device, const uint32_t* src, const uint32_t* dst, uint64_t edge_count,
+                                            const uint32_t* labels, uint32_t label_count, gb_layout layout,
+                                            gb_graph** graph);
+gb_status gb_graph_from_edges_labeled_u32(int device, const uint32_t* src, const uint32_t* dst, uint64_t edge_count,
+                                          const uint32_t* labels, uint32_t label_count, gb_layout layout,
+                                          gb_graph** graph);
+/* NodeValues::node_value for every node (csr.rs:64-76): labels receives node_count entries.  labels == NULL only
+ * asks whether the twin has labels: GB_OK, or GB_ERR_UNSUPPORTED. */
+gb_status gb_graph_node_values(const gb_graph* graph, uint32_t* labels);
+
+/* LabelStats::from_graph (dotgraph.rs:220-313), on an undirected labelled twin.  max_degree is the largest CSR
+ * degree (not the file's degree column); label_count the number of DISTINCT labels (DotGraph::label_count means
+ * max_label + 1 instead).  labels / counts may be NULL; if given they receive label_count entries, the labels
+ * ascending and counts[i] the frequency of labels[i] (the label_frequency map). */
+typedef struct gb_label_stats_info {  /* not gb_label_stats: C gives a typedef and a function one name space */
+  uint32_t max_degree;
+  uint32_t max_label;
+  uint64_t label_count;
+  uint64_t max_label_frequency;
+} gb_label_stats_info;
+gb_status gb_label_stats(const gb_graph* graph, gb_label_stats_info* stats, uint32_t* labels, uint64_t* counts);
+/* NodeLabelIndex::from_stats (dotgraph.rs:430-532): a CSR with max_label + 1 rows; row l lists the nodes labelled l,
+ * ascending.  *max_label (unless NULL) receives the largest label; offsets then need max_label + 2 entries and nodes
+ * node_count.  With offsets and nodes both NULL the call only finds the largest label (one reduction), so a caller
+ * sizes the arrays with one call and fills them with a second. */
+gb_status gb_node_label_index(const gb_graph* graph, uint32_t* max_label, uint32_t* offsets, uint32_t* nodes);
+/* NeighborLabelFrequencies::from_graph (dotgraph.rs:367-427): for every node u, the pairs (label, count) of the
+ * labels in u's CSR row, duplicates and self-loops counted as listed (a self-loop puts u into its row twice).
+ * A pair CSR: offsets has node_count + 1 entries, labels and counts the pairs of u at [offsets[u], offsets[u+1]),
+ * labels ascending within each node.  labels and counts need capacity target_count (gb_graph_info), which bounds
+ * the number of pairs. */
+gb_status gb_neighbor_label_frequencies(const gb_graph* graph, uint32_t* offsets, uint32_t* labels, uint32_t* counts);
+/* The three structures above fail with GB_ERR_UNSUPPORTED on a directed twin or a twin without labels.  Each leaves
+ * in gb_graph_last_timing the CUDA-event time of its device work, from its first kernel to its last (the copies of
+ * the results to the host not included). */
+
 /* Statistics of the load that created the graph (all zero for graphs made otherwise). */
 typedef struct gb_load_info {
   uint64_t file_bytes;     /* size of the file */

@@ -42,7 +42,8 @@ enum class CsrLayout { Unsorted = GB_LAYOUT_UNSORTED, Sorted = GB_LAYOUT_SORTED,
 
 // input formats of `GraphBuilder::file_format(..).path(..)` (builder.rs:283-361; input/graph500.rs, input/edgelist.rs)
 // Binary: the file of SerializeGraphOp (input/binary.rs), loaded as stored by gb_[di]graph_load_u32
-enum class FileFormat { Graph500, EdgeList, Binary };
+// DotGraph: the node-labelled .graph file (input/dotgraph.rs), built as a labelled twin by gb_[di]graph_load_labeled_u32
+enum class FileFormat { Graph500, EdgeList, Binary, DotGraph };
 
 // crates/algos/src/page_rank.rs:14-56
 struct PageRankConfig {
@@ -86,12 +87,15 @@ class CsrGraphBase {
   explicit CsrGraphBase(gb_graph* g) : g_(g) {}
   CsrGraphBase(const CsrGraphBase&) = delete;
   CsrGraphBase& operator=(const CsrGraphBase&) = delete;
-  CsrGraphBase(CsrGraphBase&& o) noexcept : g_(o.g_), host_(std::move(o.host_)) { o.g_ = nullptr; }
+  CsrGraphBase(CsrGraphBase&& o) noexcept : g_(o.g_), host_(std::move(o.host_)), labels_(std::move(o.labels_)) {
+    o.g_ = nullptr;
+  }
   CsrGraphBase& operator=(CsrGraphBase&& o) noexcept {
     if (this != &o) {
       reset();
       g_ = o.g_;
       host_ = std::move(o.host_);
+      labels_ = std::move(o.labels_);
       o.g_ = nullptr;
     }
     return *this;
@@ -103,6 +107,15 @@ class CsrGraphBase {
   gb_graph* handle() const { return g_; }
   // SerializeGraphOp::serialize, graph_ops.rs:232-238 (NI = u32)
   void serialize(const std::string& path) const { detail::check(gb_graph_serialize(g_, path.c_str())); }
+  // NodeValues::node_value, csr.rs:64-76 (labelled graphs; throws graph::Error on a graph without labels)
+  std::uint32_t node_value(std::uint32_t node) const {
+    if (labels_.empty()) {
+      labels_.resize(node_count());
+      detail::check(gb_graph_node_values(g_, labels_.data()));
+    }
+    if (node >= labels_.size()) throw std::out_of_range("node id out of range");
+    return labels_[node];
+  }
 
  protected:
   struct HostCsr {
@@ -135,6 +148,36 @@ class CsrGraphBase {
   }
   gb_graph* g_ = nullptr;
   mutable std::array<HostCsr, 3> host_;
+  mutable std::vector<std::uint32_t> labels_;
+};
+
+// LabelStats (dotgraph.rs:213-219); label_frequency as (label, count) pairs, labels ascending
+struct LabelStats {
+  std::uint32_t max_degree = 0;
+  std::size_t label_count = 0;
+  std::uint32_t max_label = 0;
+  std::size_t max_label_frequency = 0;
+  std::vector<std::pair<std::uint32_t, std::uint64_t>> label_frequency;
+};
+
+// NodeLabelIndex (dotgraph.rs:430-532): nodes(label) lists the nodes with that label, ascending
+struct NodeLabelIndex {
+  std::vector<std::uint32_t> offsets, node_ids;
+  std::pair<const std::uint32_t*, const std::uint32_t*> nodes(std::uint32_t label) const {
+    if (offsets.empty() || label >= offsets.size() - 1) throw std::out_of_range("label out of range");
+    return {node_ids.data() + offsets[label], node_ids.data() + offsets[label + 1]};
+  }
+};
+
+// NeighborLabelFrequencies (dotgraph.rs:367-427) as a pair CSR; get(node, label) is 0 for an absent label
+struct NeighborLabelFrequencies {
+  std::vector<std::uint32_t> offsets, labels, counts;
+  std::size_t len(std::uint32_t node) const { return offsets.at(node + 1) - offsets.at(node); }
+  std::size_t get(std::uint32_t node, std::uint32_t label) const {
+    for (std::uint32_t i = offsets.at(node); i < offsets.at(node + 1); ++i)
+      if (labels[i] == label) return counts[i];
+    return 0;
+  }
 };
 
 class UndirectedCsrGraph;
@@ -156,9 +199,40 @@ class UndirectedCsrGraph : public CsrGraphBase {
   using CsrGraphBase::CsrGraphBase;
   std::uint32_t degree(std::uint32_t n) const { auto r = row(GB_CSR_UNDIRECTED, n); return static_cast<std::uint32_t>(r.second - r.first); }
   std::pair<const std::uint32_t*, const std::uint32_t*> neighbors(std::uint32_t n) const { return row(GB_CSR_UNDIRECTED, n); }
-  void make_degree_ordered() {  // RelabelByDegreeOp, graph_ops.rs:173
+  void make_degree_ordered() {  // RelabelByDegreeOp, graph_ops.rs:173 (labels are not permuted: graph_b200.h)
     detail::check(gb_make_degree_ordered(g_));
     for (auto& h : host_) h = HostCsr{};
+  }
+  LabelStats label_stats() const {  // LabelStats::from_graph, dotgraph.rs:220-313
+    gb_label_stats_info st{};
+    detail::check(gb_label_stats(g_, &st, nullptr, nullptr));
+    std::vector<std::uint32_t> labels(st.label_count);
+    std::vector<std::uint64_t> counts(st.label_count);
+    detail::check(gb_label_stats(g_, &st, labels.data(), counts.data()));
+    LabelStats out{st.max_degree, static_cast<std::size_t>(st.label_count), st.max_label,
+                   static_cast<std::size_t>(st.max_label_frequency), {}};
+    for (std::size_t i = 0; i < labels.size(); ++i) out.label_frequency.emplace_back(labels[i], counts[i]);
+    return out;
+  }
+  NodeLabelIndex node_label_index() const {  // NodeLabelIndex::from_stats, dotgraph.rs:430-532
+    std::uint32_t max_label = 0;
+    detail::check(gb_node_label_index(g_, &max_label, nullptr, nullptr));
+    NodeLabelIndex idx;
+    idx.offsets.resize(static_cast<std::size_t>(max_label) + 2);
+    idx.node_ids.resize(node_count());
+    detail::check(gb_node_label_index(g_, nullptr, idx.offsets.data(), idx.node_ids.data()));
+    return idx;
+  }
+  NeighborLabelFrequencies neighbor_label_frequencies() const {  // dotgraph.rs:367-427
+    const gb_graph_info i = info();
+    NeighborLabelFrequencies f;
+    f.offsets.resize(static_cast<std::size_t>(i.node_count) + 1);
+    f.labels.resize(i.target_count ? i.target_count : 1);
+    f.counts.resize(i.target_count ? i.target_count : 1);
+    detail::check(gb_neighbor_label_frequencies(g_, f.offsets.data(), f.labels.data(), f.counts.data()));
+    f.labels.resize(f.offsets.back());
+    f.counts.resize(f.offsets.back());
+    return f;
   }
 };
 
@@ -184,6 +258,8 @@ class GraphBuilder {
     return *this;
   }
   GraphBuilder& node_count(std::uint32_t n) { n_ = n; return *this; }
+  // GraphBuilder::node_values (builder.rs:388, 425): one label per node; the node count is their number
+  GraphBuilder& node_values(const std::vector<std::uint32_t>& labels) { labels_ = labels; return *this; }
   // file_format(format).path(p): read the file with the library's native readers (csrc/io.cu)
   GraphBuilder& file_format(FileFormat f) { format_ = f; return *this; }
   // read the third column of a text edge list as f32 edge values (the reference selects this through
@@ -194,7 +270,9 @@ class GraphBuilder {
     if (!in) throw Error(GB_ERR_INVALID, "cannot open " + p);  // Error::IoError, lib.rs:276-281
     src_.clear(); dst_.clear(); w_.clear();
     binary_path_.clear();
-    if (format_ == FileFormat::Binary) {  // the CSRs are read as stored at build time (csr.rs:636-656)
+    labels_.clear();
+    // Binary: the CSRs are read as stored at build time (csr.rs:636-656); DotGraph: loaded as a labelled graph
+    if (format_ == FileFormat::Binary || format_ == FileFormat::DotGraph) {
       binary_path_ = p;
       return *this;
     }
@@ -225,9 +303,19 @@ class GraphBuilder {
   const std::vector<float>& pending_values() const { return w_; }
   DirectedCsrGraph build_directed() const {
     gb_graph* g = nullptr;
+    if (!binary_path_.empty() && format_ == FileFormat::DotGraph) {
+      detail::check(gb_digraph_load_labeled_u32(device_, binary_path_.c_str(), static_cast<gb_layout>(layout_), &g));
+      return DirectedCsrGraph(g);
+    }
     if (!binary_path_.empty()) {
       detail::check(gb_digraph_load_u32(device_, binary_path_.c_str(), GB_FORMAT_BINARY, static_cast<gb_layout>(layout_),
                                         with_values_ ? 1 : 0, &g));
+      return DirectedCsrGraph(g);
+    }
+    if (!labels_.empty()) {
+      detail::check(gb_digraph_from_edges_labeled_u32(device_, src_.data(), dst_.data(), src_.size(), labels_.data(),
+                                                      static_cast<std::uint32_t>(labels_.size()),
+                                                      static_cast<gb_layout>(layout_), &g));
       return DirectedCsrGraph(g);
     }
     detail::check(gb_digraph_from_edges_u32(device_, src_.data(), dst_.data(), w_.empty() ? nullptr : w_.data(), src_.size(), n_,
@@ -236,8 +324,18 @@ class GraphBuilder {
   }
   UndirectedCsrGraph build_undirected() const {
     gb_graph* g = nullptr;
+    if (!binary_path_.empty() && format_ == FileFormat::DotGraph) {
+      detail::check(gb_graph_load_labeled_u32(device_, binary_path_.c_str(), static_cast<gb_layout>(layout_), &g));
+      return UndirectedCsrGraph(g);
+    }
     if (!binary_path_.empty()) {
       detail::check(gb_graph_load_u32(device_, binary_path_.c_str(), GB_FORMAT_BINARY, static_cast<gb_layout>(layout_), &g));
+      return UndirectedCsrGraph(g);
+    }
+    if (!labels_.empty()) {
+      detail::check(gb_graph_from_edges_labeled_u32(device_, src_.data(), dst_.data(), src_.size(), labels_.data(),
+                                                    static_cast<std::uint32_t>(labels_.size()),
+                                                    static_cast<gb_layout>(layout_), &g));
       return UndirectedCsrGraph(g);
     }
     detail::check(gb_graph_from_edges_u32(device_, src_.data(), dst_.data(), src_.size(), n_, static_cast<gb_layout>(layout_), &g));
@@ -250,8 +348,8 @@ class GraphBuilder {
   bool with_values_ = false;
   int device_ = 0;
   std::uint32_t n_ = 0;
-  std::string binary_path_;  // set by path(..) for FileFormat::Binary
-  std::vector<std::uint32_t> src_, dst_;
+  std::string binary_path_;  // set by path(..) for FileFormat::Binary and FileFormat::DotGraph
+  std::vector<std::uint32_t> src_, dst_, labels_;
   std::vector<float> w_;
 };
 
