@@ -179,6 +179,7 @@ SIGNATURES = {
     "gb_pr_shard_create": (C.c_int, [_P, C.c_uint32, C.c_uint32, C.POINTER(_P)]),
     "gb_pr_shard_info": (C.c_int, [_P, C.POINTER(PrShardStats)]),
     "gb_pr_shard_plan_shape": (C.c_int, [_P, C.POINTER(PrPlanShape)]),
+    "gb_pr_shard_plan_values": (C.c_int, [_P, C.c_int, _P, C.c_uint64]),
     "gb_pr_shard_init": (C.c_int, [_P, C.c_float, _P, _P, _P, _P]),
     "gb_pr_shard_step": (C.c_int, [_P, C.c_float, C.c_uint64, _P, _P, _P, C.c_uint32, _P, _P, _P, _P]),
     "gb_pr_shard_sync": (C.c_int, [_P, C.c_uint64, _P, _P, _P, _P, C.c_uint32, _P]),

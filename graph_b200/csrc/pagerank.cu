@@ -1392,6 +1392,19 @@ static void plan_shape(const PrPlan* p, gb_pr_plan_shape* shape) {
   shape->dual = 0;
   shape->last_hot_block = p->last_hot_block;
 }
+// the value buffer V of a plan's virtual blocks: poison it with 0xFFFFFFFF, and / or copy it to the host
+static gb_status plan_values(const PrPlan* p, int poison, float* values, uint64_t count) {
+  const PrVBlocks& v = p->v;
+  GB_REQUIRE(p->vb, "the layout has no virtual blocks");
+  GB_REQUIRE(count == v.slots, "count %llu is not the value buffer's %llu slots", (unsigned long long)count,
+             (unsigned long long)v.slots);
+  if (poison) {
+    GB_CUDA(cudaMemsetAsync(v.val.p, 0xFF, v.slots * sizeof(float), 0));
+    GB_CUDA(cudaStreamSynchronize(0));
+  }
+  if (values) GB_CUDA(cudaMemcpy(values, v.val.p, v.slots * sizeof(float), cudaMemcpyDeviceToHost));
+  return GB_OK;
+}
 
 gb_status page_rank_impl(const gb_graph* g, const gb_page_rank_config* cfg, float* d_scores, float* h_scores,
                          uint64_t* ran, double* error) {
@@ -1573,16 +1586,13 @@ gb_status gb_page_rank_plan_values(const gb_graph* g, int poison, float* values,
   gb::DeviceGuard guard(g->device);
   std::lock_guard<std::mutex> lock(g->mu);
   GB_TRY(gb::ensure_plan(g));
-  const gb::PrVBlocks& v = g->pr_plan->v;
-  GB_REQUIRE(g->pr_plan->vb, "the layout has no virtual blocks");
-  GB_REQUIRE(count == v.slots, "count %llu is not the value buffer's %llu slots", (unsigned long long)count,
-             (unsigned long long)v.slots);
-  if (poison) {
-    GB_CUDA(cudaMemsetAsync(v.val.p, 0xFF, v.slots * sizeof(float), 0));
-    GB_CUDA(cudaStreamSynchronize(0));
-  }
-  if (values) GB_CUDA(cudaMemcpy(values, v.val.p, v.slots * sizeof(float), cudaMemcpyDeviceToHost));
-  return GB_OK;
+  return gb::plan_values(g->pr_plan, poison, values, count);
+}
+
+gb_status gb_pr_shard_plan_values(const gb_pr_shard* shard, int poison, float* values, uint64_t count) {
+  GB_REQUIRE(shard, "NULL argument");
+  gb::DeviceGuard guard(shard->device);
+  return gb::plan_values(shard->plan, poison, values, count);
 }
 
 gb_status gb_pr_shard_plan_shape(const gb_pr_shard* shard, gb_pr_plan_shape* shape) {

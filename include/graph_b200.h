@@ -559,6 +559,9 @@ gb_status gb_page_rank_plan_shape(const gb_graph* graph, gb_pr_plan_shape* shape
  * count = its vblock_slots.  poison != 0 first sets every slot to the bit pattern 0xFFFFFFFF (a NaN), so that a
  * later sweep shows which slots pass A writes; values (unless NULL) receives the buffer. */
 gb_status gb_page_rank_plan_values(const gb_graph* graph, int poison, float* values, uint64_t count);
+/* the same for a shard's plan, which a caller drives from vectors of its own choosing (gb_pr_shard_step); the
+ * copy waits for the legacy default stream only: synchronize the shard's stream first */
+gb_status gb_pr_shard_plan_values(const gb_pr_shard* shard, int poison, float* values, uint64_t count);
 gb_status gb_pr_shard_plan_shape(const gb_pr_shard* shard, gb_pr_plan_shape* shape);
 /* fills the full initial vectors (n floats each, internal order) on this rank: d_x0 = init/outdeg,
  * the constant part of d_x1; d_scores = init for own rows, 0 for the others (rows without in-edges:
