@@ -315,8 +315,7 @@ class NeighborLabelFrequencies:
 
 # ---- input files (crates/builder/src/input/{graph500,edgelist}.rs) --------------------------------
 # DiGraph.load / Graph.load stream the file to the device and parse it there (csrc/load.cu).  The host
-# readers below (csrc/io.cu) give the same edges; they serve the Flight server's weighted undirected graphs
-# and are the reference the device loader is tested against.
+# readers below (csrc/io.cu) give the same edges; they are the reference the device loader is tested against.
 def _load_args(path, file_format, layout):
     """(path bytes, format value, layout value) for gb_*_load_u32; raises what opening the file raises."""
     if file_format in (FileFormat.Graph500, FileFormat.EdgeList, FileFormat.Binary, FileFormat.DotGraph):
@@ -713,9 +712,11 @@ class DiGraph(_Handle):
         """(offsets, targets) host arrays of the out or in CSR (read-only)."""
         return self._mirror(_capi.CSR_OUT if which == "out" else _capi.CSR_IN)
 
-    def to_undirected(self, layout=None) -> "Graph":
-        """New, unrelated undirected graph (graph_ops.rs:229; csr.rs:391-464)."""
-        return _construct(Graph, lib.gb_to_undirected, self._g, _layout_value(layout))
+    def to_undirected(self, layout=None, *, weights=False) -> "Graph":
+        """New, unrelated undirected graph (graph_ops.rs:229; csr.rs:391-464).  weights=True keeps the out-CSR's
+        f32 values (UndirectedCsrGraph<u32, (), f32>) and needs a weighted digraph."""
+        fn = lib.gb_to_undirected_weighted if weights else lib.gb_to_undirected
+        return _construct(Graph, fn, self._g, _layout_value(layout))
 
     def in_degree_partition(self, parts: int) -> list:
         """graph_ops.rs:431-439 — ranges as [(start, end), ...]"""
@@ -794,7 +795,10 @@ class Graph(_Handle):
     (csr.rs:658-661; Python surface graph_mate.pyi:120-168)."""
 
     @staticmethod
-    def _from_edges(src, dst, node_count, layout) -> "Graph":
+    def _from_edges(src, dst, node_count, layout, weights=None) -> "Graph":
+        if weights is not None:
+            return _construct(Graph, lib.gb_graph_from_weighted_edges_u32, _device, _ptr(src), _ptr(dst),
+                              _ptr(weights), len(src), node_count, _layout_value(layout))
         return _construct(Graph, lib.gb_graph_from_edges_u32, _device, _ptr(src), _ptr(dst), len(src), node_count,
                           _layout_value(layout))
 
@@ -809,21 +813,42 @@ class Graph(_Handle):
         return _construct(Graph, lib.gb_graph_load_labeled_u32, _device, p, lay)
 
     @staticmethod
-    def from_torch(src, dst, node_count: int = 0, layout=None) -> "Graph":
-        """From contiguous 1-D int32 / int64 CUDA tensors on the graph's device, without a host copy."""
-        s, d, _, m, stream = _torch_edges(src, dst, None)
+    def load_weighted(path, layout=None, file_format=FileFormat.EdgeList) -> "Graph":
+        """Weighted text edge list `<src> <dst> <f32>`, or a binary file with Target<NI, f32> records, as
+        UndirectedCsrGraph<u32, (), f32> (the reference's `loading --undirected --weighted`)."""
+        if file_format is FileFormat.Graph500:
+            raise ValueError("Graph500 files carry no edge values")
+        if file_format is FileFormat.DotGraph:
+            raise ValueError("DotGraph files carry no edge values")
+        return _construct(Graph, lib.gb_graph_load_weighted_u32, _device, *_load_args(path, file_format, layout))
+
+    @staticmethod
+    def from_torch(src, dst, node_count: int = 0, layout=None, weights=None) -> "Graph":
+        """From contiguous 1-D int32 / int64 CUDA tensors on the graph's device, without a host copy.  weights:
+        one float32 value per edge on the same device, for UndirectedCsrGraph<u32, (), f32>."""
+        s, d, w, m, stream = _torch_edges(src, dst, weights)
+        if w is not None:
+            return _construct(Graph, lib.gb_graph_from_device_weighted_edges_u32, _device, s.data_ptr(),
+                              d.data_ptr(), w.data_ptr(), m, int(node_count), _layout_value(layout),
+                              stream.cuda_stream)
         return _construct(Graph, lib.gb_graph_from_device_edges_u32, _device, s.data_ptr(), d.data_ptr(), m,
                           int(node_count), _layout_value(layout), stream.cuda_stream)
 
     @staticmethod
-    def from_numpy(arr, layout=None, node_count: int = 0, node_values=None) -> "Graph":
-        """node_values: one u32 label per node; the node count is then their number."""
+    def from_numpy(arr, layout=None, node_count: int = 0, node_values=None, weights=None) -> "Graph":
+        """node_values: one u32 label per node; the node count is then their number.  weights: one f32 value
+        per edge, which both entries of the edge carry (UndirectedCsrGraph<u32, (), f32>)."""
         src, dst = _edges_from_numpy(arr)
         if node_values is not None:
+            if weights is not None:
+                raise ValueError("a graph with node values carries no edge weights")
             labels = _node_values(node_values, node_count)
             return _construct(Graph, lib.gb_graph_from_edges_labeled_u32, _device, _ptr(src), _ptr(dst), len(src),
                               _ptr(labels), len(labels), _layout_value(layout))
-        return Graph._from_edges(src, dst, node_count, layout)
+        w = None if weights is None else np.ascontiguousarray(weights, dtype=np.float32)
+        if w is not None and (w.ndim != 1 or len(w) != len(src)):
+            raise ValueError("weights must have one entry per edge")
+        return Graph._from_edges(src, dst, node_count, layout, w)
 
     @staticmethod
     def from_pandas(df, layout=None) -> "Graph":
@@ -851,6 +876,16 @@ class Graph(_Handle):
 
     def csr(self):
         return self._mirror(_capi.CSR_UNDIRECTED)
+
+    def weights(self) -> np.ndarray:
+        """f32 edge values aligned with the csr() targets (SoA twin of Target<u32, f32>); a graph without values
+        raises ValueError."""
+        ln = C.c_uint64(0)
+        check(lib.gb_graph_csr_len(self._g, _capi.CSR_UNDIRECTED, C.byref(ln)))
+        off = np.empty(self.node_count() + 1, np.uint32)
+        w = np.empty(ln.value, np.float32)
+        check(lib.gb_graph_copy_csr(self._g, _capi.CSR_UNDIRECTED, _ptr(off), None, _ptr(w)))
+        return w
 
     def make_degree_ordered(self) -> None:
         """Relabel by descending degree, in place (graph_ops.rs:173, 511-638)."""

@@ -118,6 +118,8 @@ SIGNATURES = {
     "gb_graph_from_csr_u32": (C.c_int, [C.c_int, C.c_uint32, _P, _P, C.POINTER(_P)]),
     "gb_digraph_from_edges_u32": (C.c_int, [C.c_int, _P, _P, _P, C.c_uint64, C.c_uint32, C.c_int, C.POINTER(_P)]),
     "gb_graph_from_edges_u32": (C.c_int, [C.c_int, _P, _P, C.c_uint64, C.c_uint32, C.c_int, C.POINTER(_P)]),
+    "gb_graph_from_weighted_edges_u32": (C.c_int, [C.c_int, _P, _P, _P, C.c_uint64, C.c_uint32, C.c_int,
+                                                   C.POINTER(_P)]),
     "gb_digraph_rmat": (C.c_int, [C.c_int, C.c_uint32, C.c_uint32, C.c_uint64, C.c_int, C.c_int, C.POINTER(_P)]),
     "gb_graph_rmat": (C.c_int, [C.c_int, C.c_uint32, C.c_uint32, C.c_uint64, C.c_int, C.POINTER(_P)]),
     "gb_rmat_edges": (C.c_int, [C.c_int, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint64, _P, _P]),
@@ -129,6 +131,7 @@ SIGNATURES = {
     "gb_graph_serialize": (C.c_int, [_P, C.c_char_p]),
     "gb_digraph_load_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
     "gb_graph_load_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.c_int, C.POINTER(_P)]),
+    "gb_graph_load_weighted_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.c_int, C.POINTER(_P)]),
     "gb_graph_load_info": (C.c_int, [_P, C.POINTER(LoadInfo)]),
     "gb_digraph_load_labeled_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.POINTER(_P)]),
     "gb_graph_load_labeled_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.POINTER(_P)]),
@@ -144,6 +147,8 @@ SIGNATURES = {
                                                    C.POINTER(_P)]),
     "gb_graph_from_device_edges_u32": (C.c_int, [C.c_int, _P, _P, C.c_uint64, C.c_uint32, C.c_int, _P,
                                                  C.POINTER(_P)]),
+    "gb_graph_from_device_weighted_edges_u32": (C.c_int, [C.c_int, _P, _P, _P, C.c_uint64, C.c_uint32, C.c_int,
+                                                          _P, C.POINTER(_P)]),
     "gb_ids_to_u32": (C.c_int, [C.c_int, _P, C.c_int, C.c_uint64, _P, _P]),
     "gb_graph_free": (C.c_int, [_P]),
     "gb_graph_get_info": (C.c_int, [_P, C.POINTER(GraphInfo)]),
@@ -152,6 +157,7 @@ SIGNATURES = {
     "gb_graph_stream": (_P, [_P]),
     "gb_graph_last_timing": (C.c_int, [_P, C.POINTER(Timing)]),
     "gb_to_undirected": (C.c_int, [_P, C.c_int, C.POINTER(_P)]),
+    "gb_to_undirected_weighted": (C.c_int, [_P, C.c_int, C.POINTER(_P)]),
     "gb_make_degree_ordered": (C.c_int, [_P]),
     "gb_page_rank": (C.c_int, [_P, C.POINTER(PageRankConfig), _P, C.POINTER(C.c_uint64), C.POINTER(C.c_double)]),
     "gb_page_rank_device": (C.c_int, [_P, C.POINTER(PageRankConfig), _P, C.POINTER(C.c_uint64), C.POINTER(C.c_double)]),

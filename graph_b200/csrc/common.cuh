@@ -345,9 +345,10 @@ gb_status check_layout(gb_layout layout);
 
 // CSR construction on device (graph.cu)
 // rows/cols: device arrays of `count` entries, only read. Builds `csr` with the given layout; n rows.
-// w may be null.
+// w may be null.  It holds one value per entry when w_period is 0; otherwise w_period values that entries j and
+// j + w_period share (an undirected build's two passes over one edge list, count = 2 * w_period).
 gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, const uint32_t* d_cols,
-                           const float* d_w, uint64_t count, gb_layout layout, DevCsr* csr);
+                           const float* d_w, uint64_t count, gb_layout layout, DevCsr* csr, uint64_t w_period = 0);
 gb_status new_graph(int device, gb_graph_kind kind, uint32_t n, GraphPtr* out);
 // Uploads a host CSR on stream s and checks it: require_host_csr on the host, the offsets monotone and the
 // targets below n on the device.  offsets_only uploads the offsets alone (degrees); w may be NULL.  Returns

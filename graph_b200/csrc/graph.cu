@@ -109,6 +109,26 @@ __global__ void k_gather(const T* __restrict__ src, const uint32_t* __restrict__
     dst[i] = src[idx[i]];
 }
 
+// The values of an undirected build: its 2m entries are the outgoing pass (entry j < m is edge j) and the incoming
+// pass (entry j >= m is edge j - m), so both entries of an edge read its one value and no doubled array exists.
+__global__ void k_gather_mirrored(const float* __restrict__ w, const uint32_t* __restrict__ idx, uint64_t count,
+                                  uint64_t m, float* __restrict__ dst) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
+       i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t j = idx[i];
+    dst[i] = w[j < m ? j : j - m];
+  }
+}
+
+// out[i] = the value of the entry the sort moved to position i (w_period: see build_csr_device)
+static void gather_values(cudaStream_t s, const float* d_w, uint64_t w_period, const uint32_t* order, uint64_t count,
+                          float* out) {
+  if (w_period)
+    k_gather_mirrored<<<grid_for(count, 256), 256, 0, s>>>(d_w, order, count, w_period, out);
+  else
+    k_gather<float><<<grid_for(count, 256), 256, 0, s>>>(d_w, order, count, out);
+}
+
 // Deduplicated layout (csr.rs:897-948): keep the first of each run of equal (row,target) keys and
 // drop entries whose target is the row itself.
 __global__ void k_dedup_flags(const uint64_t* __restrict__ keys, uint64_t count, uint32_t bits,
@@ -183,7 +203,7 @@ __global__ void k_relabel_keys(const uint32_t* __restrict__ rows, const uint32_t
 
 // ---- CSR build -----------------------------------------------------------------------------
 gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, const uint32_t* d_cols,
-                           const float* d_w, uint64_t count, gb_layout layout, DevCsr* csr) {
+                           const float* d_w, uint64_t count, gb_layout layout, DevCsr* csr, uint64_t w_period) {
   GB_REQUIRE(count < 0xFFFFFFFFull, "CSR with %llu entries does not fit u32 offsets (csr.rs:124)",
              (unsigned long long)count);
   const uint32_t bits = bits_for(n);
@@ -218,7 +238,7 @@ gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, c
     k_gather<uint32_t><<<grid_for(count, blk), blk, 0, s>>>(d_cols, vb.Current(), count, csr->tgt.p);
     if (d_w) {
       GB_TRY(csr->w.alloc(count, 8));
-      k_gather<float><<<grid_for(count, blk), blk, 0, s>>>(d_w, vb.Current(), count, csr->w.p);
+      gather_values(s, d_w, w_period, vb.Current(), count, csr->w.p);
     }
     GB_TRY(offsets_from_sorted(s, RowOfArr{kb.Current()}, count, n, csr->off.p));
     GB_CUDA(cudaGetLastError());
@@ -286,7 +306,7 @@ gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, c
     k_unpack_targets<<<grid_for(out_count, blk), blk, 0, s>>>(sorted, out_count, bits, csr->tgt.p);
     if (d_w) {
       GB_TRY(csr->w.alloc(out_count, 8));
-      k_gather<float><<<grid_for(out_count, blk), blk, 0, s>>>(d_w, order, out_count, csr->w.p);
+      gather_values(s, d_w, w_period, order, out_count, csr->w.p);
     }
   } else if (d_w) {
     GB_TRY(csr->w.alloc(0, 8));
@@ -567,7 +587,8 @@ static gb_status build_graph_csrs(gb_graph* g, const uint32_t* d_src, const uint
     GB_TRY(build_csr_device(s, g->n, d_src, d_dst, d_w, m, layout, &g->out));
     GB_TRY(build_csr_device(s, g->n, d_dst, d_src, nullptr, m, layout, &g->in));
   } else {
-    // one CSR holding both directions: outgoing pass first, then incoming (csr.rs:154-172)
+    // one CSR holding both directions: outgoing pass first, then incoming (csr.rs:154-172); both entries of an
+    // edge carry its value, read from d_w by the sort's index payload (k_gather_mirrored)
     DevBuf<uint32_t> rows, cols;
     GB_TRY(rows.alloc(2 * m));
     GB_TRY(cols.alloc(2 * m));
@@ -577,7 +598,7 @@ static gb_status build_graph_csrs(gb_graph* g, const uint32_t* d_src, const uint
       GB_CUDA(cudaMemcpyAsync(cols.p, d_dst, m * 4, cudaMemcpyDeviceToDevice, s));
       GB_CUDA(cudaMemcpyAsync(cols.p + m, d_src, m * 4, cudaMemcpyDeviceToDevice, s));
     }
-    GB_TRY(build_csr_device(s, g->n, rows.p, cols.p, nullptr, 2 * m, layout, &g->out));
+    GB_TRY(build_csr_device(s, g->n, rows.p, cols.p, d_w, 2 * m, layout, &g->out, m));
   }
   // an Unsorted build keeps the edge-list order inside each row, which may or may not be ascending
   g->row_order = (layout == GB_LAYOUT_UNSORTED) ? RowOrder::Unknown : RowOrder::Sorted;
@@ -855,6 +876,15 @@ gb_status gb_graph_from_edges_u32(int device, const uint32_t* src, const uint32_
   return graph_from_host_edges(device, GB_KIND_UNDIRECTED, src, dst, nullptr, m, n, layout, graph);
 }
 
+// UndirectedCsrGraph<u32, (), f32>: `weights` may be NULL only without edges, which still gives a twin with values
+gb_status gb_graph_from_weighted_edges_u32(int device, const uint32_t* src, const uint32_t* dst, const float* weights,
+                                           uint64_t m, uint32_t n, gb_layout layout, gb_graph** graph) {
+  static const float no_values = 0.0f;  // never read: it only marks the empty twin as one with values
+  GB_REQUIRE(m == 0 || weights != nullptr, "weights is NULL");
+  return graph_from_host_edges(device, GB_KIND_UNDIRECTED, src, dst, weights ? weights : &no_values, m, n, layout,
+                               graph);
+}
+
 gb_status gb_digraph_from_edges_labeled_u32(int device, const uint32_t* src, const uint32_t* dst, uint64_t m,
                                             const uint32_t* labels, uint32_t label_count, gb_layout layout,
                                             gb_graph** graph) {
@@ -888,6 +918,16 @@ gb_status gb_digraph_from_device_edges_u32(int device, const uint32_t* d_src, co
 gb_status gb_graph_from_device_edges_u32(int device, const uint32_t* d_src, const uint32_t* d_dst, uint64_t m,
                                          uint32_t n, gb_layout layout, void* stream, gb_graph** graph) {
   return graph_from_device_arrays(device, GB_KIND_UNDIRECTED, d_src, d_dst, nullptr, m, n, layout,
+                                  static_cast<cudaStream_t>(stream), graph);
+}
+
+gb_status gb_graph_from_device_weighted_edges_u32(int device, const uint32_t* d_src, const uint32_t* d_dst,
+                                                  const float* d_weights, uint64_t m, uint32_t n, gb_layout layout,
+                                                  void* stream, gb_graph** graph) {
+  GB_REQUIRE(m == 0 || d_weights != nullptr, "d_weights is NULL");
+  // without edges nothing is read from the device: the host constructor gives the same empty twin with values
+  if (m == 0) return gb_graph_from_weighted_edges_u32(device, nullptr, nullptr, nullptr, 0, n, layout, graph);
+  return graph_from_device_arrays(device, GB_KIND_UNDIRECTED, d_src, d_dst, d_weights, m, n, layout,
                                   static_cast<cudaStream_t>(stream), graph);
 }
 
@@ -1022,13 +1062,15 @@ gb_status gb_graph_last_timing(const gb_graph* g, gb_timing* t) {
 }
 
 // to_undirected: csr.rs:391-464 — every out-edge (u, v) of the directed graph becomes an edge of a
-// fresh UndirectedCsrGraph, fed in out-CSR order.
-gb_status gb_to_undirected(const gb_graph* dg, gb_layout layout, gb_graph** graph) {
+// fresh UndirectedCsrGraph, fed in out-CSR order; with `weighted` each carries its out-CSR value (ToUndirectedOp
+// keeps EV, csr.rs:391-406), read from out.w as it stands.
+static gb_status to_undirected(const gb_graph* dg, gb_layout layout, bool weighted, gb_graph** graph) {
   GB_REQUIRE(dg && graph, "NULL argument");
   if (dg->kind != GB_KIND_DIRECTED) return fail(GB_ERR_UNSUPPORTED, "to_undirected needs a directed graph");
   GB_TRY(check_layout(layout));
   uint64_t m = dg->out.len;
   GB_REQUIRE(m == 0 || dg->out.tgt.p != nullptr, "this handle holds no out targets (page-rank-only twin)");
+  GB_REQUIRE(!weighted || dg->out.w.p != nullptr, "to_undirected_weighted needs a digraph with edge values");
   GB_REQUIRE(2 * m < 0xFFFFFFFFull, "undirected twin would exceed u32 offsets");
   DeviceGuard guard(dg->device);
   GraphPtr g;
@@ -1038,10 +1080,18 @@ gb_status gb_to_undirected(const gb_graph* dg, gb_layout layout, gb_graph** grap
   GB_TRY(rows.alloc(m));
   if (m) k_expand_rows<<<grid_for((uint64_t)dg->n * 32, 256), 256, 0, g->stream>>>(dg->out.off.p, dg->n, rows.p);
   GB_CUDA(cudaGetLastError());
-  GB_TRY(build_graph_csrs(g.get(), rows.p, dg->out.tgt.p, nullptr, m, layout));
+  GB_TRY(build_graph_csrs(g.get(), rows.p, dg->out.tgt.p, weighted ? dg->out.w.p : nullptr, m, layout));
   if (dg->labels.p) GB_TRY(attach_labels(g.get(), dg->labels.p, cudaMemcpyDeviceToDevice));  // csr.rs:400
   *graph = g.release();
   return GB_OK;
+}
+
+gb_status gb_to_undirected(const gb_graph* dg, gb_layout layout, gb_graph** graph) {
+  return to_undirected(dg, layout, false, graph);
+}
+
+gb_status gb_to_undirected_weighted(const gb_graph* dg, gb_layout layout, gb_graph** graph) {
+  return to_undirected(dg, layout, true, graph);
 }
 
 // make_degree_ordered: graph_ops.rs:511-638.  (degree, id) pairs sorted descending (:555), so
@@ -1053,6 +1103,10 @@ gb_status gb_make_degree_ordered(gb_graph* g) {
     return fail(GB_ERR_UNSUPPORTED, "make_degree_ordered is defined for undirected graphs (graph_ops.rs:240-253)");
   DeviceGuard guard(g->device);
   std::lock_guard<std::mutex> lock(g->mu);
+  if (g->out.w.p)  // the graph is left as it is: no value is dropped or moved
+    return fail(GB_ERR_UNSUPPORTED,
+                "make_degree_ordered needs EV: Ord (relabel_by_degree, graph_ops.rs:511-520), and f32 edge values are "
+                "not Ord: a weighted undirected graph cannot be relabelled");
   cudaStream_t s = g->stream;
   const uint32_t n = g->n;
   const uint64_t len = g->out.len;

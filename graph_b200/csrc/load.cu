@@ -799,7 +799,7 @@ static gb_status load_binary_streamed(int device, gb_graph_kind kind, const Inpu
     GB_TRY(d.off.alloc((size_t)l.n + 1));
     GB_TRY(d.tgt.alloc(l.entries, 8));
     GB_CUDA(cudaMemsetAsync(d.tgt.p + l.entries, 0, 8 * 4, sp.work));
-    if (c == 0 && want_value) GB_TRY(d.w.alloc(l.entries, 8));  // only a digraph's out-CSR keeps values
+    if (c == 0 && want_value) GB_TRY(d.w.alloc(l.entries, 8));  // the out-CSR or the undirected CSR; no in-CSR values
     BinSection o, t;
     o.pos = l.csr[c].off_pos, o.count = (uint64_t)l.n + 1, o.stride = l.id_bytes, o.ids = d.off.p;
     t.pos = l.csr[c].rec_pos, t.count = l.entries, t.stride = l.rec_bytes, t.ids = d.tgt.p, t.w = d.w.p;
@@ -905,6 +905,8 @@ static gb_status load_on_host(int device, gb_graph_kind kind, const InputFile& f
   if (kind == GB_KIND_DIRECTED)
     GB_TRY(gb_digraph_from_edges_u32(device, src.data(), dst.data(), want_value ? w.data() : nullptr, m, n, layout,
                                      graph));
+  else if (want_value)
+    GB_TRY(gb_graph_from_weighted_edges_u32(device, src.data(), dst.data(), w.data(), m, n, layout, graph));
   else
     GB_TRY(gb_graph_from_edges_u32(device, src.data(), dst.data(), m, n, layout, graph));
   info->edges = m;
@@ -1040,7 +1042,7 @@ struct TempFile {
 };
 
 // SerializeGraphOp::serialize (headers from host memory, arrays from device memory; Target<u32, f32> records are
-// interleaved on the device first)
+// interleaved on the device first: a weighted digraph's out- and in-CSR, a weighted undirected twin's one CSR)
 static gb_status serialize_graph(const gb_graph* g, const char* path) {
   GB_REQUIRE(g && path, "NULL argument");
   if (g->labels.p)
@@ -1048,11 +1050,11 @@ static gb_status serialize_graph(const gb_graph* g, const char* path) {
   GB_REQUIRE(g->out.tgt.p != nullptr, "this handle holds no out targets (page-rank-only twin) and cannot be serialized");
   DeviceGuard guard(g->device);
   std::lock_guard<std::mutex> lock(g->mu);
-  const bool values = g->kind == GB_KIND_DIRECTED && g->out.w.p != nullptr;
+  const bool values = g->out.w.p != nullptr;
   const BinLayout l = bin_layout_u32(g->kind, g->n, g->out.len, values);
   const DevCsr* csr[2] = {&g->out, &g->in};
   DevBuf<float> in_w;
-  if (values) GB_TRY(in_csr_values(g, &in_w));
+  if (values && g->kind == GB_KIND_DIRECTED) GB_TRY(in_csr_values(g, &in_w));
   struct Piece {
     uint64_t pos, len;
     const void* src;
@@ -1169,6 +1171,11 @@ gb_status gb_digraph_load_u32(int device, const char* path, gb_file_format forma
 gb_status gb_graph_load_u32(int device, const char* path, gb_file_format format, gb_layout layout,
                             gb_graph** graph) {
   return gb::load_graph(device, GB_KIND_UNDIRECTED, path, format, layout, 0, false, graph);
+}
+
+gb_status gb_graph_load_weighted_u32(int device, const char* path, gb_file_format format, gb_layout layout,
+                                     gb_graph** graph) {
+  return gb::load_graph(device, GB_KIND_UNDIRECTED, path, format, layout, 1, false, graph);
 }
 
 gb_status gb_digraph_load_labeled_u32(int device, const char* path, gb_layout layout, gb_graph** graph) {

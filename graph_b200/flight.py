@@ -91,9 +91,7 @@ class B200Engine:
             fmt = gb.FileFormat.Graph500 if file_format == "Graph500" else gb.FileFormat.EdgeList
             return "directed", gb.DiGraph.load(path, self._layout(layout), fmt)
         if weighted:
-            # no algorithm of the front end reads the values of an undirected graph: the twin keeps none
-            src, dst, _w = gb._read_edge_list(path, with_values=True)
-            return "undirected+weighted", gb.Graph.from_numpy(np.stack([src, dst], 1), self._layout(layout))
+            return "undirected+weighted", gb.Graph.load_weighted(path, self._layout(layout))
         fmt = gb.FileFormat.Graph500 if file_format == "Graph500" else gb.FileFormat.EdgeList
         return "undirected", gb.Graph.load(path, self._layout(layout), fmt)
 
@@ -120,7 +118,8 @@ class B200Engine:
         g.make_degree_ordered()
 
     def to_undirected(self, g, layout: str):
-        return g.to_undirected(self._layout(layout))
+        # a "directed+weighted" twin becomes an "undirected+weighted" one with its values (server.rs:390-391)
+        return g.to_undirected(self._layout(layout), weights=bool(g._info.has_weights))
 
 
 class GraphFlightServer(fl.FlightServerBase):

@@ -77,7 +77,8 @@ typedef struct gb_graph_info {
   uint32_t node_count;    /* Graph::node_count  lib.rs:315-321 */
   uint64_t edge_count;    /* Graph::edge_count: directed = |out targets|; undirected = |targets|/2 (csr.rs:687-689) */
   uint64_t target_count;  /* entries in the out (or undirected) targets array */
-  uint32_t has_weights;   /* 1 if the out-CSR carries f32 edge values (Target<u32,f32>, graph/mod.rs:6-10) */
+  uint32_t has_weights;   /* 1 if the out-CSR (undirected: the CSR) carries f32 edge values (Target<u32,f32>,
+                             graph/mod.rs:6-10) */
   int32_t device;         /* CUDA device ordinal the arrays live on */
   uint64_t device_bytes;  /* HBM held by this handle */
 } gb_graph_info;
@@ -156,6 +157,16 @@ gb_status gb_digraph_from_edges_u32(int device, const uint32_t* src, const uint3
 gb_status gb_graph_from_edges_u32(int device, const uint32_t* src, const uint32_t* dst,
                                   uint64_t edge_count, uint32_t node_count, gb_layout layout,
                                   gb_graph** graph);
+/* UndirectedCsrGraph<u32, (), f32> (csr.rs:124-221 with Direction::Undirected): edge (s, t, w) puts Target(t, w)
+ * in row s and Target(s, w) in row t; a self-loop (u, u, w) puts u into row u twice, with w both times.  Offsets
+ * and targets are those gb_graph_from_edges_u32 builds from the same edges, byte for byte, in every layout.
+ * Values follow their entries: UNSORTED keeps the single-thread order (outgoing pass, then incoming pass, each in
+ * edge-list order); SORTED orders each row by target, equal targets keeping that order; DEDUPLICATED keeps the
+ * value of the first entry of each run of equal targets in that order and drops self-loops (csr.rs:897-948).
+ * weights (edge_count values) may be NULL only when edge_count == 0; the twin still has values (none). */
+gb_status gb_graph_from_weighted_edges_u32(int device, const uint32_t* src, const uint32_t* dst, const float* weights,
+                                           uint64_t edge_count, uint32_t node_count, gb_layout layout,
+                                           gb_graph** graph);
 
 /* Synthetic R-MAT / Graph500-style graph generated on device (a,b,c,d = .57,.19,.19,.05,
  * n = 2^scale, m = edge_factor * n, ids scrambled, duplicates and self-loops kept); the same
@@ -216,13 +227,24 @@ typedef enum gb_file_format {
  * A binary file's rows are kept byte for byte: `layout` is checked and otherwise ignored, as the reference
  * ignores it (csr.rs:650), and the row order is left unknown, as after gb_graph_from_csr_u32.  with_values
  * = 1 needs a file with values; with 0 they are dropped, and so are the in-CSR values (the device keeps
- * none) and an undirected file's values.  The streamed path DMAs u32 sections without values straight into
- * the CSR arrays and narrows / splits the others on the device. */
+ * none).  gb_graph_load_u32 drops an undirected file's values; gb_graph_load_weighted_u32 keeps them.  The
+ * streamed path DMAs u32 sections without values straight into the CSR arrays and narrows / splits the others
+ * on the device. */
 gb_status gb_digraph_load_u32(int device, const char* path, gb_file_format format, gb_layout layout,
                               int with_values, gb_graph** graph);
 gb_status gb_graph_load_u32(int device, const char* path, gb_file_format format, gb_layout layout,
                             gb_graph** graph);
+/* UndirectedCsrGraph<u32, (), f32> from a file: gb_digraph_load_u32 with with_values = 1, for the undirected
+ * twin (the reference's `loading --undirected --weighted`, crates/app/src/loading.rs:47-48).  An edge list is
+ * built as gb_graph_from_weighted_edges_u32 builds its edges (host reader below 64 MiB, streamed above or with
+ * GB_LOAD_CHUNK_BYTES); a binary file with Target<NI, f32> records keeps its rows and values byte for byte,
+ * including records whose two entries of an edge disagree.  GB_ERR_INVALID for Graph500 and DotGraph files and
+ * for a binary file without values. */
+gb_status gb_graph_load_weighted_u32(int device, const char* path, gb_file_format format, gb_layout layout,
+                                     gb_graph** graph);
 /* SerializeGraphOp::serialize (graph_ops.rs:232-238): writes the graph as a binary file with NI = "u32";
+ * a weighted undirected twin writes Target<u32,f32> records for its CSR (csr.rs:810-839), so
+ * save(gb_graph_load_weighted_u32(f)) is byte-equal to a u32 file f;
  * a weighted digraph writes Target<u32,f32> records for both CSRs, the in-CSR value of the k-th occurrence
  * of s in in-row t being that of the k-th occurrence of t in out-row s (for every graph built here the
  * value of the same edge; the in-CSR must be the transpose of the out-CSR).  So save(load(f)) is byte-equal
@@ -308,6 +330,10 @@ gb_status gb_digraph_from_device_edges_u32(int device, const uint32_t* d_src, co
 gb_status gb_graph_from_device_edges_u32(int device, const uint32_t* d_src, const uint32_t* d_dst,
                                          uint64_t edge_count, uint32_t node_count, gb_layout layout,
                                          void* stream, gb_graph** graph);
+/* gb_graph_from_weighted_edges_u32 from device arrays; d_weights may be NULL only when edge_count == 0 */
+gb_status gb_graph_from_device_weighted_edges_u32(int device, const uint32_t* d_src, const uint32_t* d_dst,
+                                                  const float* d_weights, uint64_t edge_count, uint32_t node_count,
+                                                  gb_layout layout, void* stream, gb_graph** graph);
 /* Narrows device ids (int32 when id_bytes == 4, int64 when 8) to uint32 on the device; any id outside
  * [0, 2^32) is GB_ERR_INVALID.  Enqueued on `stream`, waited for before returning. */
 gb_status gb_ids_to_u32(int device, const void* d_ids, int id_bytes, uint64_t count, uint32_t* d_out,
@@ -316,7 +342,9 @@ gb_status gb_ids_to_u32(int device, const void* d_ids, int id_bytes, uint64_t co
 gb_status gb_graph_free(gb_graph* graph);
 gb_status gb_graph_get_info(const gb_graph* graph, gb_graph_info* info);
 /* copy a CSR back to the host (neighbour views of the host mirror: csr.rs:97-117).
- * offsets: node_count+1 entries; targets: target_count entries; weights may be NULL. */
+ * offsets: node_count+1 entries; targets: target_count entries; weights may be NULL.  weights receives the
+ * values of a weighted digraph's GB_CSR_OUT or of a weighted undirected twin's GB_CSR_UNDIRECTED (aligned with
+ * the targets); GB_ERR_INVALID for a CSR without values. */
 gb_status gb_graph_copy_csr(const gb_graph* graph, gb_csr_which which, uint32_t* offsets,
                             uint32_t* targets, float* weights);
 /* number of entries in the chosen CSR's targets array */
@@ -326,10 +354,16 @@ void* gb_graph_stream(const gb_graph* graph);
 gb_status gb_graph_last_timing(const gb_graph* graph, gb_timing* timing);
 
 /* ---- graph ops ----------------------------------------------------------------------------- */
-/* ToUndirectedOp::to_undirected (graph_ops.rs:229, csr.rs:391-464) */
+/* ToUndirectedOp::to_undirected (graph_ops.rs:229, csr.rs:391-464); the twin has no values */
 gb_status gb_to_undirected(const gb_graph* digraph, gb_layout layout, gb_graph** graph);
+/* to_undirected keeping EV = f32 (csr.rs:391-406): the out-CSR's entries are fed in CSR order with their values,
+ * as gb_graph_from_weighted_edges_u32 builds them; offsets and targets equal gb_to_undirected's.  Needs a weighted
+ * digraph (GB_ERR_INVALID otherwise, and for a gb_digraph_for_page_rank_u32 twin). */
+gb_status gb_to_undirected_weighted(const gb_graph* digraph, gb_layout layout, gb_graph** graph);
 /* RelabelByDegreeOp::make_degree_ordered (graph_ops.rs:173,250-252,511-638): new id = rank in
- * (degree, old id) DESCENDING; rows rewritten and re-sorted.  Undirected graphs only. */
+ * (degree, old id) DESCENDING; rows rewritten and re-sorted.  Undirected graphs without edge values only: the
+ * reference's relabel_by_degree needs EV: Ord (graph_ops.rs:511-520) and f32 is not Ord, so a weighted
+ * undirected twin gets GB_ERR_UNSUPPORTED and is left unchanged. */
 gb_status gb_make_degree_ordered(gb_graph* graph);
 
 /* ---- algorithms ---------------------------------------------------------------------------- */
@@ -453,7 +487,9 @@ gb_status gb_sssp_csr_info(gb_sssp_csr_stats* info);
 
 /* global_triangle_count(&graph) -> u64                      triangle_count.rs:22-86
  * Any row order, as the reference counts it.  The first call on a graph whose rows are not known to be
- * sorted (an Unsorted build, gb_graph_from_csr_u32) checks them once and caches the answer. */
+ * sorted (an Unsorted build, gb_graph_from_csr_u32) checks them once and caches the answer.  It also counts a
+ * weighted undirected twin, whose targets are those of the unweighted build, and ignores its values; this goes
+ * beyond the reference, which implements UndirectedNeighbors for EV = () only (csr.rs:704). */
 gb_status gb_triangle_count(const gb_graph* graph, uint64_t* triangles);
 
 /* global_triangle_count (triangle_count.rs:22-86) of a HOST undirected CSR, with no twin kept: the number

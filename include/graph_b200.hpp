@@ -191,6 +191,8 @@ class DirectedCsrGraph : public CsrGraphBase {
   std::pair<const std::uint32_t*, const std::uint32_t*> out_neighbors(std::uint32_t n) const { return row(GB_CSR_OUT, n); }
   std::pair<const std::uint32_t*, const std::uint32_t*> in_neighbors(std::uint32_t n) const { return row(GB_CSR_IN, n); }
   inline UndirectedCsrGraph to_undirected(CsrLayout layout = CsrLayout::Unsorted) const;  // graph_ops.rs:229
+  // to_undirected keeping the f32 values (csr.rs:391-406): UndirectedCsrGraph<u32, (), f32>; needs a weighted digraph
+  inline UndirectedCsrGraph to_undirected_weighted(CsrLayout layout = CsrLayout::Unsorted) const;
 };
 
 // UndirectedCsrGraph<u32>, csr.rs:658-661; traits :682-725
@@ -199,9 +201,26 @@ class UndirectedCsrGraph : public CsrGraphBase {
   using CsrGraphBase::CsrGraphBase;
   std::uint32_t degree(std::uint32_t n) const { auto r = row(GB_CSR_UNDIRECTED, n); return static_cast<std::uint32_t>(r.second - r.first); }
   std::pair<const std::uint32_t*, const std::uint32_t*> neighbors(std::uint32_t n) const { return row(GB_CSR_UNDIRECTED, n); }
+  // UndirectedNeighborsWithValues::neighbors_with_values (csr.rs:715-725) of a graph with f32 values; throws
+  // graph::Error on a graph without values
+  std::pair<const Target*, const Target*> neighbors_with_values(std::uint32_t n) const {
+    const HostCsr& h = mirror(GB_CSR_UNDIRECTED);
+    if (n >= node_count()) throw std::out_of_range("node id out of range");
+    if (!values_read_) {
+      std::vector<float> w(h.tgt.size());
+      std::vector<std::uint32_t> off(h.off.size());
+      detail::check(gb_graph_copy_csr(g_, GB_CSR_UNDIRECTED, off.data(), nullptr, w.data()));
+      targets_.resize(h.tgt.size());
+      for (std::size_t i = 0; i < w.size(); ++i) targets_[i] = Target{h.tgt[i], w[i]};
+      values_read_ = true;
+    }
+    return {targets_.data() + h.off[n], targets_.data() + h.off[n + 1]};
+  }
   void make_degree_ordered() {  // RelabelByDegreeOp, graph_ops.rs:173 (labels are not permuted: graph_b200.h)
     detail::check(gb_make_degree_ordered(g_));
     for (auto& h : host_) h = HostCsr{};
+    targets_.clear();
+    values_read_ = false;
   }
   LabelStats label_stats() const {  // LabelStats::from_graph, dotgraph.rs:220-313
     gb_label_stats_info st{};
@@ -234,11 +253,21 @@ class UndirectedCsrGraph : public CsrGraphBase {
     f.counts.resize(f.offsets.back());
     return f;
   }
+
+ private:
+  mutable std::vector<Target> targets_;  // host AoS copy for neighbors_with_values, read once
+  mutable bool values_read_ = false;
 };
 
 inline UndirectedCsrGraph DirectedCsrGraph::to_undirected(CsrLayout layout) const {
   gb_graph* u = nullptr;
   detail::check(gb_to_undirected(g_, static_cast<gb_layout>(layout), &u));
+  return UndirectedCsrGraph(u);
+}
+
+inline UndirectedCsrGraph DirectedCsrGraph::to_undirected_weighted(CsrLayout layout) const {
+  gb_graph* u = nullptr;
+  detail::check(gb_to_undirected_weighted(g_, static_cast<gb_layout>(layout), &u));
   return UndirectedCsrGraph(u);
 }
 
@@ -249,11 +278,13 @@ class GraphBuilder {
   GraphBuilder& device(int d) { device_ = d; return *this; }
   GraphBuilder& edges(const std::vector<std::pair<std::uint32_t, std::uint32_t>>& e) {
     src_.clear(); dst_.clear(); w_.clear();
+    values_ = false;
     for (auto& p : e) { src_.push_back(p.first); dst_.push_back(p.second); }
     return *this;
   }
   GraphBuilder& edges_with_values(const std::vector<std::tuple<std::uint32_t, std::uint32_t, float>>& e) {
     src_.clear(); dst_.clear(); w_.clear();
+    values_ = true;
     for (auto& t : e) { src_.push_back(std::get<0>(t)); dst_.push_back(std::get<1>(t)); w_.push_back(std::get<2>(t)); }
     return *this;
   }
@@ -271,6 +302,8 @@ class GraphBuilder {
     src_.clear(); dst_.clear(); w_.clear();
     binary_path_.clear();
     labels_.clear();
+    // a file read with with_values() holds values when its format has them (a binary file's are checked at build)
+    values_ = with_values_ && (format_ == FileFormat::EdgeList || format_ == FileFormat::Binary);
     // Binary: the CSRs are read as stored at build time (csr.rs:636-656); DotGraph: loaded as a labelled graph
     if (format_ == FileFormat::Binary || format_ == FileFormat::DotGraph) {
       binary_path_ = p;
@@ -341,11 +374,26 @@ class GraphBuilder {
     detail::check(gb_graph_from_edges_u32(device_, src_.data(), dst_.data(), src_.size(), n_, static_cast<gb_layout>(layout_), &g));
     return UndirectedCsrGraph(g);
   }
+  // UndirectedCsrGraph<u32, (), f32> (the reference's EV = f32 undirected build, csr.rs:124-221): from
+  // edges_with_values(..), or from a file read with with_values() (edge list or Binary); both entries of an edge
+  // carry its value.  Throws graph::Error when the builder holds no values.
+  UndirectedCsrGraph build_undirected_weighted() const {
+    if (!values_) throw Error(GB_ERR_INVALID, "build_undirected_weighted needs edges_with_values(..) or a file read with with_values()");
+    gb_graph* g = nullptr;
+    if (!binary_path_.empty()) {
+      detail::check(gb_graph_load_weighted_u32(device_, binary_path_.c_str(), GB_FORMAT_BINARY, static_cast<gb_layout>(layout_), &g));
+      return UndirectedCsrGraph(g);
+    }
+    detail::check(gb_graph_from_weighted_edges_u32(device_, src_.data(), dst_.data(), w_.data(), src_.size(), n_,
+                                                   static_cast<gb_layout>(layout_), &g));
+    return UndirectedCsrGraph(g);
+  }
 
  private:
   CsrLayout layout_ = CsrLayout::Unsorted;  // CsrLayout::default()
   FileFormat format_ = FileFormat::EdgeList;
   bool with_values_ = false;
+  bool values_ = false;  // the pending edges (or file) carry f32 values
   int device_ = 0;
   std::uint32_t n_ = 0;
   std::string binary_path_;  // set by path(..) for FileFormat::Binary and FileFormat::DotGraph
