@@ -11,6 +11,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 import sys
+import threading
 import time
 from pathlib import Path
 
@@ -23,7 +24,7 @@ __all__ = ["DiGraph", "Graph", "Layout", "FileFormat", "PageRankResult", "WccRes
            "TriangleCountResult", "SsspResult", "LabelStats", "NodeLabelIndex", "NeighborLabelFrequencies",
            "NeighborLabelFrequency", "PageRankConfig", "WccConfig", "DeltaSteppingConfig",
            "GraphB200Error", "device_count", "set_device", "write_graph500", "wcc_csr",
-           "triangle_count_csr", "sssp_csr"]
+           "triangle_count_csr", "sssp_csr", "DirectedALGraph", "UndirectedALGraph"]
 
 _device = 0
 
@@ -940,6 +941,284 @@ class Graph(_Handle):
             check(lib.gb_triangle_count(self._g, C.byref(tri)))
         _, micros = _timed(go)
         return TriangleCountResult(int(tri.value), micros)
+
+
+# ---- adjacency-list graphs (crates/builder/src/graph/adj_list.rs) ----------------------------------------
+def _batch_arrays(src, dst, values, with_values: bool):
+    """Host edge arrays of add_edges as contiguous uint32 / float32."""
+    s = np.asarray(src)
+    d = np.asarray(dst)
+    for a in (s, d):
+        if a.ndim != 1:
+            raise ValueError("src and dst must be 1-D arrays")
+        if a.dtype != np.uint32 and (not np.issubdtype(a.dtype, np.integer)
+                                     or (a.size and (a.min() < 0 or a.max() > 0xFFFFFFFF))):
+            raise TypeError("node ids must be 32-bit unsigned integers")
+    if len(s) != len(d):
+        raise ValueError("src and dst must have the same length")
+    w = None
+    if with_values:
+        if values is None:
+            raise ValueError("the graph carries edge values: add_edges needs values")
+        w = np.ascontiguousarray(values, dtype=np.float32)
+        if w.ndim != 1 or len(w) != len(s):
+            raise ValueError("values must have one entry per edge")
+    elif values is not None:
+        raise ValueError("the graph carries no edge values")
+    return np.ascontiguousarray(s, np.uint32), np.ascontiguousarray(d, np.uint32), w
+
+
+class _ALGraph:
+    """Owns a gb_algraph*: adjacency lists on the device that take new edges.  Neighbour accessors return owned
+    copies, because rows move when edges are added.  The algorithms run on a snapshot (to_graph()) that is kept
+    until the next add_edges."""
+    _KIND = _capi.KIND_DIRECTED
+    _SNAPSHOT = None  # DiGraph / Graph
+
+    def __init__(self, raw_ptr, load_micros=0, layout=None, values=False):
+        self._g = raw_ptr
+        self.load_micros = int(load_micros)
+        self.layout = layout
+        self._values = bool(values)
+        self._lock = threading.Lock()
+        self._version = 0
+        self._snap = (None, None)
+
+    def __del__(self):
+        g, self._g = getattr(self, "_g", None), None
+        if g:
+            try:
+                lib.gb_algraph_free(g)
+            except Exception:  # interpreter shutdown
+                pass
+
+    # -- construction --
+    @classmethod
+    def _make(cls, fn, *args, layout=None, values=False):
+        out = C.c_void_p()
+        _, micros = _timed(lambda: check(fn(*args, C.byref(out))))
+        return cls(out, micros, layout if layout is not None else Layout.Unsorted, values)
+
+    @classmethod
+    def from_numpy(cls, arr, layout=None, weights=None, node_count: int = 0):
+        """From an (m, 2) array of edges (DirectedALGraph / UndirectedALGraph From<(E, CsrLayout)>, adj_list.rs:
+        406-450, 559-595); weights: one f32 value per edge (EV = f32).  node_count 0 means max id + 1."""
+        src, dst = _edges_from_numpy(arr)
+        w = None if weights is None else np.ascontiguousarray(weights, dtype=np.float32)
+        if w is not None and (w.ndim != 1 or len(w) != len(src)):
+            raise ValueError("weights must have one entry per edge")
+        return cls._make(lib.gb_algraph_from_edges_u32, _device, cls._KIND, _ptr(src), _ptr(dst), _ptr(w), len(src),
+                         int(node_count), _layout_value(layout), int(w is not None), layout=layout,
+                         values=w is not None)
+
+    @classmethod
+    def from_torch(cls, src, dst, weights=None, node_count: int = 0, layout=None):
+        """From contiguous 1-D CUDA tensors on the graph's device (ids int32 or int64, weights float32)."""
+        s, d, w, m, stream = _torch_edges(src, dst, weights)
+        return cls._make(lib.gb_algraph_from_device_edges_u32, _device, cls._KIND, s.data_ptr(), d.data_ptr(),
+                         None if w is None else w.data_ptr(), m, int(node_count), _layout_value(layout),
+                         int(w is not None), stream.cuda_stream, layout=layout, values=w is not None)
+
+    @classmethod
+    def load(cls, path, layout=None, file_format=FileFormat.Graph500):
+        """A Graph500 or text edge-list file, streamed to the device and parsed there."""
+        p, fmt, lay = _load_args(path, file_format, layout)
+        return cls._make(lib.gb_algraph_load_u32, _device, cls._KIND, p, fmt, lay, 0, layout=layout)
+
+    @classmethod
+    def load_weighted(cls, path, layout=None):
+        """A weighted text edge list `<src> <dst> <f32>` (EV = f32)."""
+        p, fmt, lay = _load_args(path, FileFormat.EdgeList, layout)
+        return cls._make(lib.gb_algraph_load_u32, _device, cls._KIND, p, fmt, lay, 1, layout=layout, values=True)
+
+    # -- accessors --
+    def _info(self):
+        info = _capi.GraphInfo()
+        check(lib.gb_algraph_get_info(self._g, C.byref(info)))
+        return info
+
+    def node_count(self) -> int:
+        return int(self._info().node_count)
+
+    def edge_count(self) -> int:
+        return int(self._info().edge_count)
+
+    def device_bytes(self) -> int:
+        return int(self._info().device_bytes)
+
+    def has_values(self) -> bool:
+        return self._values
+
+    def load_info(self) -> dict:
+        info = _capi.LoadInfo()
+        check(lib.gb_algraph_load_info(self._g, C.byref(info)))
+        return info.as_dict()
+
+    def last_batch(self) -> dict:
+        """What the last add_edges did: entries inserted, rows touched and moved, compactions, device times."""
+        info = _capi.AlBatchInfo()
+        check(lib.gb_algraph_last_batch(self._g, C.byref(info)))
+        return info.as_dict()
+
+    def _degree(self, which: int, node: int) -> int:
+        ln = C.c_uint32(0)
+        self._check_node(node)
+        check(lib.gb_algraph_copy_row(self._g, which, node, 0, None, None, C.byref(ln)))
+        return int(ln.value)
+
+    def _check_node(self, node: int) -> None:
+        n = self.node_count()
+        if not 0 <= node < n:
+            raise IndexError(f"node {node} out of range for a graph with {n} nodes")
+
+    def _row(self, which: int, node: int, with_values: bool = False):
+        if with_values and not self._values:
+            raise ValueError("the graph carries no edge values")
+        cap = self._degree(which, node)
+        while True:  # another thread may add edges between the two calls
+            tgt = np.empty(cap, np.uint32)
+            val = np.empty(cap, np.float32) if with_values else None
+            ln = C.c_uint32(0)
+            check(lib.gb_algraph_copy_row(self._g, which, node, cap, _ptr(tgt), _ptr(val), C.byref(ln)))
+            if ln.value <= cap:
+                n = int(ln.value)
+                return (tgt[:n], val[:n]) if with_values else tgt[:n]
+            cap = int(ln.value)
+
+    def _csr(self, which: int, with_values: bool = False):
+        """(offsets, targets[, values]) of one list as a compacted CSR."""
+        if with_values and not self._values:
+            raise ValueError("the graph carries no edge values")
+        off = np.empty(self.node_count() + 1, np.uint32)
+        count = C.c_uint64(0)
+        check(lib.gb_algraph_copy_csr(self._g, which, 0, _ptr(off), None, None, C.byref(count)))
+        while True:  # the arrays are filled only when they can hold the list as it is at the call
+            m = int(count.value)
+            tgt = np.empty(max(m, 1), np.uint32)
+            val = np.empty(max(m, 1), np.float32) if with_values else None
+            check(lib.gb_algraph_copy_csr(self._g, which, m, _ptr(off), _ptr(tgt), _ptr(val), C.byref(count)))
+            if int(count.value) <= m:
+                k = int(count.value)
+                return (off, tgt[:k], val[:k]) if with_values else (off, tgt[:k])
+
+    # -- mutation --
+    def add_edge(self, source: int, target: int, value=None) -> None:
+        """EdgeMutation::add_edge / EdgeMutationWithValues::add_edge_with_value (adj_list.rs:381-404, 534-557).
+        A missing node raises ValueError: node "<id>" does not exist in the graph."""
+        if (value is None) == self._values:
+            raise ValueError("add_edge needs a value exactly when the graph carries edge values")
+        for x in (source, target):
+            if not 0 <= int(x) <= 0xFFFFFFFF:
+                raise ValueError(f'node "{int(x)}" does not exist in the graph')
+        self.add_edges([source], [target], None if value is None else [value])
+
+    def add_edges(self, src, dst, values=None) -> None:
+        """len(src) add_edge calls in array order, as one device batch: all or nothing.  numpy arrays (or lists)
+        or CUDA tensors on the graph's device (ids int32 / int64, values float32)."""
+        try:
+            import torch
+            on_device = isinstance(src, torch.Tensor)
+        except ImportError:
+            on_device = False
+        if on_device:
+            if (values is None) == self._values:
+                raise ValueError("add_edges needs values exactly when the graph carries edge values")
+            s, d, w, m, stream = _torch_edges(src, dst, values)
+            check(lib.gb_algraph_add_device_edges_u32(self._g, s.data_ptr(), d.data_ptr(),
+                                                      None if w is None else w.data_ptr(), m, stream.cuda_stream))
+        else:
+            s, d, w = _batch_arrays(src, dst, values, self._values)
+            check(lib.gb_algraph_add_edges_u32(self._g, _ptr(s), _ptr(d), _ptr(w), len(s)))
+        with self._lock:
+            self._version += 1
+            self._snap = (None, None)
+
+    # -- snapshot and algorithms --
+    def to_graph(self):
+        """A fresh, immutable DiGraph / Graph with this graph's rows (and out values), byte for byte."""
+        return _construct(self._SNAPSHOT, lib.gb_algraph_to_graph, self._g)
+
+    def _snapshot(self):
+        with self._lock:
+            version, snap = self._snap
+            if snap is None or version != self._version:
+                snap = self.to_graph()
+                self._snap = (self._version, snap)
+            return snap
+
+    def __repr__(self):
+        return f"{type(self).__name__} {{ node_count: {self.node_count()}, edge_count: {self.edge_count()} }}"
+
+
+class DirectedALGraph(_ALGraph):
+    """Device twin of DirectedALGraph<u32, (), EV> (crates/builder/src/graph/adj_list.rs:279-450), EV = () or
+    f32: an out-list and an in-list that take new edges."""
+    _KIND = _capi.KIND_DIRECTED
+    _SNAPSHOT = DiGraph
+
+    def out_degree(self, node: int) -> int:
+        return self._degree(_capi.CSR_OUT, node)
+
+    def in_degree(self, node: int) -> int:
+        return self._degree(_capi.CSR_IN, node)
+
+    def out_neighbors(self, node: int) -> np.ndarray:
+        return self._row(_capi.CSR_OUT, node)
+
+    def in_neighbors(self, node: int) -> np.ndarray:
+        return self._row(_capi.CSR_IN, node)
+
+    def out_neighbors_with_values(self, node: int):
+        """(targets, values) of out-row `node` (DirectedNeighborsWithValues, adj_list.rs:355-369)."""
+        return self._row(_capi.CSR_OUT, node, True)
+
+    def in_neighbors_with_values(self, node: int):
+        return self._row(_capi.CSR_IN, node, True)
+
+    def csr(self, which: str = "out", with_values: bool = False):
+        return self._csr(_capi.CSR_OUT if which == "out" else _capi.CSR_IN, with_values)
+
+    def page_rank(self, *, max_iterations: int = PageRankConfig.DEFAULT_MAX_ITERATIONS,
+                  tolerance: float = PageRankConfig.DEFAULT_TOLERANCE,
+                  damping_factor: float = PageRankConfig.DEFAULT_DAMPING_FACTOR, mode: str = "auto") -> PageRankResult:
+        """DiGraph.page_rank on the snapshot."""
+        return self._snapshot().page_rank(max_iterations=max_iterations, tolerance=tolerance,
+                                          damping_factor=damping_factor, mode=mode)
+
+    def wcc(self, *, chunk_size: int = WccConfig.DEFAULT_CHUNK_SIZE,
+            neighbor_rounds: int = WccConfig.DEFAULT_NEIGHBOR_ROUNDS,
+            sampling_size: int = WccConfig.DEFAULT_SAMPLING_SIZE) -> WccResult:
+        """DiGraph.wcc on the snapshot."""
+        return self._snapshot().wcc(chunk_size=chunk_size, neighbor_rounds=neighbor_rounds,
+                                    sampling_size=sampling_size)
+
+    def delta_stepping(self, *, start_node: int, delta: float) -> SsspResult:
+        """DiGraph.delta_stepping on the snapshot; needs f32 edge values."""
+        return self._snapshot().delta_stepping(start_node=start_node, delta=delta)
+
+
+class UndirectedALGraph(_ALGraph):
+    """Device twin of UndirectedALGraph<u32, (), EV> (adj_list.rs:452-595), EV = () or f32: one list that takes
+    new edges."""
+    _KIND = _capi.KIND_UNDIRECTED
+    _SNAPSHOT = Graph
+
+    def degree(self, node: int) -> int:
+        return self._degree(_capi.CSR_UNDIRECTED, node)
+
+    def neighbors(self, node: int) -> np.ndarray:
+        return self._row(_capi.CSR_UNDIRECTED, node)
+
+    def neighbors_with_values(self, node: int):
+        """(targets, values) of row `node` (UndirectedNeighborsWithValues, adj_list.rs:512-522)."""
+        return self._row(_capi.CSR_UNDIRECTED, node, True)
+
+    def csr(self, with_values: bool = False):
+        return self._csr(_capi.CSR_UNDIRECTED, with_values)
+
+    def global_triangle_count(self) -> TriangleCountResult:
+        """Graph.global_triangle_count on the snapshot."""
+        return self._snapshot().global_triangle_count()
 
 
 def _page_rank_csr_arrays(in_offsets, in_targets, out_offsets, what: str):

@@ -100,6 +100,16 @@ class LabelStatsInfo(C.Structure):
                 ("max_label_frequency", C.c_uint64)]
 
 
+class AlBatchInfo(C.Structure):
+    _fields_ = [("edges", C.c_uint64), ("inserted", C.c_uint64), ("touched_rows", C.c_uint64),
+                ("relocated_rows", C.c_uint64), ("compactions", C.c_uint64), ("total_compactions", C.c_uint64),
+                ("pool_entries", C.c_uint64), ("pool_used", C.c_uint64), ("total_ms", C.c_double),
+                ("compaction_ms", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class GraphB200Error(RuntimeError):
     """CUDA / allocation failure inside libgraph_b200."""
 
@@ -200,6 +210,20 @@ SIGNATURES = {
     "gb_page_rank_csr_multi_u32": (C.c_int, [_P, C.c_uint32, _P, _P, _P, C.POINTER(PageRankConfig), _P,
                                              C.POINTER(C.c_uint64), C.POINTER(C.c_double)]),
     "gb_pr_shards_csr_u32": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P, _P, _P, C.POINTER(_P)]),
+    "gb_algraph_from_edges_u32": (C.c_int, [C.c_int, C.c_int, _P, _P, _P, C.c_uint64, C.c_uint32, C.c_int, C.c_int,
+                                            C.POINTER(_P)]),
+    "gb_algraph_from_device_edges_u32": (C.c_int, [C.c_int, C.c_int, _P, _P, _P, C.c_uint64, C.c_uint32, C.c_int,
+                                                   C.c_int, _P, C.POINTER(_P)]),
+    "gb_algraph_load_u32": (C.c_int, [C.c_int, C.c_int, C.c_char_p, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
+    "gb_algraph_load_info": (C.c_int, [_P, C.POINTER(LoadInfo)]),
+    "gb_algraph_add_edges_u32": (C.c_int, [_P, _P, _P, _P, C.c_uint64]),
+    "gb_algraph_add_device_edges_u32": (C.c_int, [_P, _P, _P, _P, C.c_uint64, _P]),
+    "gb_algraph_last_batch": (C.c_int, [_P, C.POINTER(AlBatchInfo)]),
+    "gb_algraph_get_info": (C.c_int, [_P, C.POINTER(GraphInfo)]),
+    "gb_algraph_copy_row": (C.c_int, [_P, C.c_int, C.c_uint32, C.c_uint32, _P, _P, C.POINTER(C.c_uint32)]),
+    "gb_algraph_copy_csr": (C.c_int, [_P, C.c_int, C.c_uint64, _P, _P, _P, C.POINTER(C.c_uint64)]),
+    "gb_algraph_to_graph": (C.c_int, [_P, C.POINTER(_P)]),
+    "gb_algraph_free": (C.c_int, [_P]),
 }
 
 

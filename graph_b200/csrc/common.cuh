@@ -346,9 +346,26 @@ gb_status check_layout(gb_layout layout);
 // CSR construction on device (graph.cu)
 // rows/cols: device arrays of `count` entries, only read. Builds `csr` with the given layout; n rows.
 // w may be null.  It holds one value per entry when w_period is 0; otherwise w_period values that entries j and
-// j + w_period share (an undirected build's two passes over one edge list, count = 2 * w_period).
+// j + w_period share (an undirected build's two passes over one edge list, count = 2 * w_period).  With w_pairs
+// entries 2i and 2i + 1 share w[i] instead (an adjacency list's interleaved undirected stream).  keep_self_loops
+// makes Deduplicated keep entries whose target is their row, as the adjacency lists do (adj_list.rs:260-263).
 gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, const uint32_t* d_cols,
-                           const float* d_w, uint64_t count, gb_layout layout, DevCsr* csr, uint64_t w_period = 0);
+                           const float* d_w, uint64_t count, gb_layout layout, DevCsr* csr, uint64_t w_period = 0,
+                           bool keep_self_loops = false, bool w_pairs = false);
+// Checks device edge arrays on s: *n == 0 becomes the largest id + 1, otherwise every id must be below *n.
+gb_status check_edge_ids(cudaStream_t s, const uint32_t* d_src, const uint32_t* d_dst, uint64_t m, uint32_t* n);
+// GB_ERR_INVALID unless p is device (or managed) memory of `device`
+gb_status require_device_array(const void* p, int device, const char* what);
+// Edge arrays read from a file on the device (load.cu): Graph500 or text edge list through the pinned-ring
+// pipeline, in file order.  n is edges / 16 for Graph500 and 0 (max id + 1) for an edge list.
+struct EdgeArrays {
+  DevBuf<uint32_t> src, dst;
+  DevBuf<float> w;
+  uint64_t m = 0;
+  uint32_t n = 0;
+  gb_load_info info{};
+};
+gb_status load_edge_arrays(int device, const char* path, gb_file_format format, bool with_values, EdgeArrays* out);
 gb_status new_graph(int device, gb_graph_kind kind, uint32_t n, GraphPtr* out);
 // Uploads a host CSR on stream s and checks it: require_host_csr on the host, the offsets monotone and the
 // targets below n on the device.  offsets_only uploads the offsets alone (degrees); w may be NULL.  Returns

@@ -120,24 +120,35 @@ __global__ void k_gather_mirrored(const float* __restrict__ w, const uint32_t* _
   }
 }
 
-// out[i] = the value of the entry the sort moved to position i (w_period: see build_csr_device)
-static void gather_values(cudaStream_t s, const float* d_w, uint64_t w_period, const uint32_t* order, uint64_t count,
-                          float* out) {
-  if (w_period)
+// The values of an interleaved build (an adjacency list's undirected rows): entries 2i and 2i + 1 are the two
+// entries of edge i, which read its one value.
+__global__ void k_gather_pairs(const float* __restrict__ w, const uint32_t* __restrict__ idx, uint64_t count,
+                               float* __restrict__ dst) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
+       i += (uint64_t)gridDim.x * blockDim.x)
+    dst[i] = w[idx[i] >> 1];
+}
+
+// out[i] = the value of the entry the sort moved to position i (w_period, w_pairs: see build_csr_device)
+static void gather_values(cudaStream_t s, const float* d_w, uint64_t w_period, bool w_pairs, const uint32_t* order,
+                          uint64_t count, float* out) {
+  if (w_pairs)
+    k_gather_pairs<<<grid_for(count, 256), 256, 0, s>>>(d_w, order, count, out);
+  else if (w_period)
     k_gather_mirrored<<<grid_for(count, 256), 256, 0, s>>>(d_w, order, count, w_period, out);
   else
     k_gather<float><<<grid_for(count, 256), 256, 0, s>>>(d_w, order, count, out);
 }
 
 // Deduplicated layout (csr.rs:897-948): keep the first of each run of equal (row,target) keys and
-// drop entries whose target is the row itself.
+// drop entries whose target is the row itself, unless keep_self_loops (adj_list.rs:260-263 only dedups).
 __global__ void k_dedup_flags(const uint64_t* __restrict__ keys, uint64_t count, uint32_t bits,
-                              uint8_t* __restrict__ flags) {
+                              bool keep_self_loops, uint8_t* __restrict__ flags) {
   uint64_t mask = (bits >= 32) ? 0xFFFFFFFFull : ((1ull << bits) - 1ull);
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
        i += (uint64_t)gridDim.x * blockDim.x) {
     uint64_t k = keys[i];
-    bool keep = (i == 0 || keys[i - 1] != k) && ((uint32_t)(k >> bits) != (uint32_t)(k & mask));
+    bool keep = (i == 0 || keys[i - 1] != k) && (keep_self_loops || (uint32_t)(k >> bits) != (uint32_t)(k & mask));
     flags[i] = keep ? 1 : 0;
   }
 }
@@ -203,7 +214,8 @@ __global__ void k_relabel_keys(const uint32_t* __restrict__ rows, const uint32_t
 
 // ---- CSR build -----------------------------------------------------------------------------
 gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, const uint32_t* d_cols,
-                           const float* d_w, uint64_t count, gb_layout layout, DevCsr* csr, uint64_t w_period) {
+                           const float* d_w, uint64_t count, gb_layout layout, DevCsr* csr, uint64_t w_period,
+                           bool keep_self_loops, bool w_pairs) {
   GB_REQUIRE(count < 0xFFFFFFFFull, "CSR with %llu entries does not fit u32 offsets (csr.rs:124)",
              (unsigned long long)count);
   const uint32_t bits = bits_for(n);
@@ -238,7 +250,7 @@ gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, c
     k_gather<uint32_t><<<grid_for(count, blk), blk, 0, s>>>(d_cols, vb.Current(), count, csr->tgt.p);
     if (d_w) {
       GB_TRY(csr->w.alloc(count, 8));
-      gather_values(s, d_w, w_period, vb.Current(), count, csr->w.p);
+      gather_values(s, d_w, w_period, w_pairs, vb.Current(), count, csr->w.p);
     }
     GB_TRY(offsets_from_sorted(s, RowOfArr{kb.Current()}, count, n, csr->off.p));
     GB_CUDA(cudaGetLastError());
@@ -279,7 +291,7 @@ gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, c
     DevBuf<uint64_t> d_num;
     GB_TRY(flags.alloc(count));
     GB_TRY(d_num.alloc(1));
-    k_dedup_flags<<<grid_for(count, blk), blk, 0, s>>>(sorted, count, bits, flags.p);
+    k_dedup_flags<<<grid_for(count, blk), blk, 0, s>>>(sorted, count, bits, keep_self_loops, flags.p);
     DevBuf<uint8_t> sel_tmp;
     GB_TRY(cub_call(sel_tmp, [&](void* t, size_t& tb) {
       return cub::DeviceSelect::Flagged(t, tb, sorted, flags.p, spare, d_num.p, (int64_t)count, s);
@@ -306,7 +318,7 @@ gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, c
     k_unpack_targets<<<grid_for(out_count, blk), blk, 0, s>>>(sorted, out_count, bits, csr->tgt.p);
     if (d_w) {
       GB_TRY(csr->w.alloc(out_count, 8));
-      gather_values(s, d_w, w_period, order, out_count, csr->w.p);
+      gather_values(s, d_w, w_period, w_pairs, order, out_count, csr->w.p);
     }
   } else if (d_w) {
     GB_TRY(csr->w.alloc(0, 8));
@@ -627,20 +639,18 @@ static gb_status check_edge_args(gb_graph_kind kind, const uint32_t* src, const 
   return GB_OK;
 }
 
-// Checks device edge arrays on g's stream, then builds g's CSRs from them.  g->n == 0 is inferred as the
-// largest id + 1 (Edges::max_node_id + 1, edgelist.rs:84-90); otherwise every id must be below g->n.
-static gb_status build_from_edges(gb_graph* g, const uint32_t* d_src, const uint32_t* d_dst, const float* d_w,
-                                  uint64_t m, gb_layout layout) {
-  cudaStream_t s = g->stream;
-  const bool infer = g->n == 0;
+// Checks device edge arrays on stream s.  *n == 0 is inferred as the largest id + 1 (Edges::max_node_id + 1,
+// edgelist.rs:84-90); otherwise every id must be below *n.
+gb_status check_edge_ids(cudaStream_t s, const uint32_t* d_src, const uint32_t* d_dst, uint64_t m, uint32_t* n) {
+  const bool infer = *n == 0;
   DevBuf<unsigned int> scratch;
   GB_TRY(scratch.alloc(1));
   GB_CUDA(cudaMemsetAsync(scratch.p, 0, 4, s));
   if (infer) {
     k_max_ids<<<grid_for(m, 256), 256, 0, s>>>(d_src, d_dst, m, scratch.p);
   } else {
-    check_ids_async(s, d_src, m, g->n, scratch.p);
-    check_ids_async(s, d_dst, m, g->n, scratch.p);
+    check_ids_async(s, d_src, m, *n, scratch.p);
+    check_ids_async(s, d_dst, m, *n, scratch.p);
   }
   unsigned int h = 0;
   GB_CUDA(cudaMemcpyAsync(&h, scratch.p, 4, cudaMemcpyDeviceToHost, s));
@@ -648,10 +658,17 @@ static gb_status build_from_edges(gb_graph* g, const uint32_t* d_src, const uint
   GB_CUDA(cudaGetLastError());
   if (infer) {
     GB_REQUIRE(h < 0xFFFFFFFFu, "node id 2^32-1 leaves no room for node_count");
-    g->n = h + 1;
+    *n = h + 1;
   } else {
-    GB_REQUIRE(h == 0, "%u edge endpoints are >= node_count %u", h, g->n);
+    GB_REQUIRE(h == 0, "%u edge endpoints are >= node_count %u", h, *n);
   }
+  return GB_OK;
+}
+
+// Checks device edge arrays on g's stream (check_edge_ids, with g->n), then builds g's CSRs from them.
+static gb_status build_from_edges(gb_graph* g, const uint32_t* d_src, const uint32_t* d_dst, const float* d_w,
+                                  uint64_t m, gb_layout layout) {
+  GB_TRY(check_edge_ids(g->stream, d_src, d_dst, m, &g->n));
   return build_graph_csrs(g, d_src, d_dst, d_w, m, layout);
 }
 
@@ -699,7 +716,7 @@ static gb_status graph_from_host_edges_labeled(int device, gb_graph_kind kind, c
   return GB_OK;
 }
 
-static gb_status require_device_array(const void* p, int device, const char* what) {
+gb_status require_device_array(const void* p, int device, const char* what) {
   cudaPointerAttributes a{};
   if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
     cudaGetLastError();

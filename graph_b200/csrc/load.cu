@@ -1159,6 +1159,31 @@ static gb_status load_graph(int device, gb_graph_kind kind, const char* path, gb
   return GB_OK;
 }
 
+// The edges of a Graph500 or edge-list file on the device, for a graph that is not built by build_csr_device
+// alone (the adjacency lists of adj_list.cu).  Always the streamed pipeline: the edge arrays it fills are what the
+// caller keeps, so the host readers' upload would only add a copy.
+gb_status load_edge_arrays(int device, const char* path, gb_file_format format, bool with_values, EdgeArrays* out) {
+  GB_REQUIRE(path != nullptr, "path is NULL");
+  GB_REQUIRE(format == GB_FORMAT_GRAPH500 || format == GB_FORMAT_EDGE_LIST,
+             "adjacency lists load Graph500 and edge-list files, not format %d", (int)format);
+  GB_REQUIRE(!with_values || format == GB_FORMAT_EDGE_LIST, "only edge lists carry edge values");
+  GB_TRY(require_device(device));
+  DeviceGuard guard(device);
+  InputFile f;
+  GB_TRY(f.open(path));
+  out->info = gb_load_info{};
+  out->info.file_bytes = f.bytes;
+  LoadedEdges e;
+  GB_TRY(load_file(device, f, format, with_values, DotHeader{}, &e, &out->info));
+  out->src = std::move(e.src);
+  out->dst = std::move(e.dst);
+  out->w = std::move(e.w);
+  out->m = e.m;
+  out->n = e.n;
+  out->info.edges = e.m;
+  return GB_OK;
+}
+
 }  // namespace gb
 
 extern "C" {

@@ -17,7 +17,8 @@
  *   - all calls return gb_status; on failure gb_last_error() holds a
  *     thread-local message.  Nothing unwinds or aborts across the ABI.
  *   - a gb_graph is immutable after creation except gb_make_degree_ordered,
- *     which relabels it in place (graph_ops.rs:173).
+ *     which relabels it in place (graph_ops.rs:173).  Graphs that take new
+ *     edges are a separate handle, gb_algraph (adjacency lists, below).
  *   - threads: calls on distinct handles may run concurrently.  Calls on one
  *     handle serialise on its lock, gb_make_degree_ordered included; other
  *     calls see the graph either before or after the relabelling.  The one
@@ -27,6 +28,9 @@
  *     PageRank calls (gb_page_rank_multi, gb_page_rank_csr_multi_u32).  The
  *     statistics of the one-shot calls (gb_sssp_csr_info,
  *     gb_triangle_count_csr_info) are thread-local, like gb_last_error().
+ *     A gb_algraph has a lock of its own: calls on one serialise, a batch of
+ *     gb_algraph_add_*edges_u32 is atomic, and every other call sees the
+ *     graph before or after it.
  *   - there is NO CPU fallback: if no CUDA device is usable every graph
  *     constructor fails with GB_ERR_CUDA.
  */
@@ -365,6 +369,98 @@ gb_status gb_to_undirected_weighted(const gb_graph* digraph, gb_layout layout, g
  * reference's relabel_by_degree needs EV: Ord (graph_ops.rs:511-520) and f32 is not Ord, so a weighted
  * undirected twin gets GB_ERR_UNSUPPORTED and is left unchanged. */
 gb_status gb_make_degree_ordered(gb_graph* graph);
+
+/* ---- adjacency-list graphs (crates/builder/src/graph/adj_list.rs) ----------------------------------------------
+ * An opaque gb_algraph is the device twin of DirectedALGraph<u32, (), EV> (adj_list.rs:279-450: an out-list and an
+ * in-list) or UndirectedALGraph<u32, (), EV> (:452-595: one list), EV = () or f32.  Unlike a gb_graph it takes new
+ * edges (EdgeMutation::add_edge / EdgeMutationWithValues::add_edge_with_value, lib.rs:415-456).  Its rows are those
+ * of the reference's single-thread run:
+ *   - construction (AdjacencyList::from, adj_list.rs:216-277): node_count as for the CSR builds (max id + 1, an
+ *     explicit count, or edges / 16 for Graph500).  Directed UNSORTED rows list entries in edge-list order, as the
+ *     CSR twin's do.  Undirected UNSORTED rows interleave the directions edge by edge: edge (s, t) pushes t into
+ *     row s and then s into row t (for edges (0,1),(1,2) row 1 is [0, 2], the CSR twin's is [2, 0]); a self-loop
+ *     (u, u) puts u into row u twice.  SORTED rows are ascending, equal targets in UNSORTED order.  DEDUPLICATED
+ *     rows are sorted with one entry per target, the first in UNSORTED order, and KEEP self-loops (adj_list.rs:
+ *     260-263 only sorts and dedups; the CSR build also drops them).
+ *   - add_edge(s, t[, v]) (adj_list.rs:381-404, :534-557, apply_layout :81-94): directed, Target(t, v) goes into
+ *     out-row s and Target(s, v) into in-row t; undirected, into row s and then row t (a self-loop inserts u
+ *     twice).  UNSORTED appends; SORTED inserts after the entries with an equal target; DEDUPLICATED inserts only
+ *     a target the row does not hold (the first value wins; an undirected self-loop adds u once).
+ *   - edge_count: directed, the out-list's entries; undirected, the list's entries / 2 (adj_list.rs:484-486).
+ *     gb_graph_info's target_count is the out (or undirected) list's entries, device_bytes the pools and rows.
+ * Threads: every call on a gb_algraph holds the handle's lock, so calls on one handle serialise, a batch is atomic
+ * and readers see the graph before or after it.  gb_algraph_free needs exclusive access.
+ * A batch allocates everything it needs for every list (a digraph's two) before it changes any, so a batch refused
+ * for a missing node, an overflow or a failed allocation leaves the graph as it was; only a CUDA error while the
+ * lists are written (a broken context) can leave it part-way.
+ * Storage and growth: DESIGN.md §10. */
+typedef struct gb_algraph gb_algraph;
+
+/* What the last gb_algraph_add_*edges_u32 call did (all zero before the first). */
+typedef struct gb_algraph_batch_info {
+  uint64_t edges;             /* edges in the batch */
+  uint64_t inserted;          /* entries inserted over all lists (DEDUPLICATED: those not dropped) */
+  uint64_t touched_rows;      /* rows that received entries, over all lists */
+  uint64_t relocated_rows;    /* of which outgrew their capacity and moved */
+  uint64_t compactions;       /* pools this batch rebuilt compacted */
+  uint64_t total_compactions; /* pools rebuilt since the graph was made */
+  uint64_t pool_entries;      /* capacity of the target pools after the batch, over all lists */
+  uint64_t pool_used;         /* of which handed out to rows */
+  double total_ms;            /* CUDA-event time of the batch's device work, from the id check on, compactions included */
+  double compaction_ms;       /* of which the compactions */
+} gb_algraph_batch_info;
+
+/* DirectedALGraph / UndirectedALGraph `From<(E, CsrLayout)>` (adj_list.rs:406-450, :559-595) from host edges.
+ * node_count == 0 means max id + 1.  with_values != 0 makes EV = f32: weights holds edge_count values (NULL only
+ * without edges).  The lists are built on the device by build_csr_device's radix sort. */
+gb_status gb_algraph_from_edges_u32(int device, gb_graph_kind kind, const uint32_t* src, const uint32_t* dst,
+                                    const float* weights, uint64_t edge_count, uint32_t node_count, gb_layout layout,
+                                    int with_values, gb_algraph** graph);
+/* the same from DEVICE arrays on `device` (not kept), after the work already enqueued on `stream` */
+gb_status gb_algraph_from_device_edges_u32(int device, gb_graph_kind kind, const uint32_t* d_src,
+                                           const uint32_t* d_dst, const float* d_weights, uint64_t edge_count,
+                                           uint32_t node_count, gb_layout layout, int with_values, void* stream,
+                                           gb_algraph** graph);
+/* From a GB_FORMAT_GRAPH500 (node_count = edges / 16, graph500.rs:74) or GB_FORMAT_EDGE_LIST file (with_values: the
+ * third column as f32), streamed through the pinned-ring loader of gb_[di]graph_load_u32 (the reference's CLI
+ * `--graph adjacency-list`, crates/app/src/runner.rs:93-99).  gb_algraph_load_info gives the load's statistics. */
+gb_status gb_algraph_load_u32(int device, gb_graph_kind kind, const char* path, gb_file_format format,
+                              gb_layout layout, int with_values, gb_algraph** graph);
+gb_status gb_algraph_load_info(const gb_algraph* graph, gb_load_info* info);
+/* Batched add_edge_with_value (adj_list.rs:381-404, :534-557): leaves exactly the rows edge_count add_edge calls in
+ * array order leave, in every layout.  weights: edge_count values for a graph with values, ignored otherwise.  All
+ * or nothing: when an endpoint is >= node_count the call fails with GB_ERR_INVALID and a message that names the
+ * first such edge and its missing node, the source first (`node "3" does not exist in the graph ...`, lib.rs:300),
+ * and nothing is inserted.  A batch that would bring a list to 2^32 - 1 entries or more, or that holds 2^31 list
+ * entries or more (an undirected edge makes two), is refused the same way before anything is read or allocated.
+ * The work grows with the batch and the lengths of the rows it touches, except for a pool compaction (DESIGN.md
+ * §10), which gb_algraph_last_batch reports apart. */
+gb_status gb_algraph_add_edges_u32(gb_algraph* graph, const uint32_t* src, const uint32_t* dst, const float* weights,
+                                   uint64_t edge_count);
+/* the same from DEVICE arrays, after the work already enqueued on `stream` */
+gb_status gb_algraph_add_device_edges_u32(gb_algraph* graph, const uint32_t* d_src, const uint32_t* d_dst,
+                                          const float* d_weights, uint64_t edge_count, void* stream);
+gb_status gb_algraph_last_batch(const gb_algraph* graph, gb_algraph_batch_info* info);
+/* Graph::node_count / edge_count (adj_list.rs:311-322, :475-487) and the rest of gb_graph_info */
+gb_status gb_algraph_get_info(const gb_algraph* graph, gb_graph_info* info);
+/* One row as a copy (AdjacencyList::targets / targets_with_values, adj_list.rs:152-214; the degree is *len):
+ * which = GB_CSR_OUT / GB_CSR_IN (directed) or GB_CSR_UNDIRECTED.  *len receives the row's length; the first
+ * min(len, capacity) targets (and values, unless NULL) are copied. */
+gb_status gb_algraph_copy_row(const gb_algraph* graph, gb_csr_which which, uint32_t node, uint32_t capacity,
+                              uint32_t* targets, float* values, uint32_t* len);
+/* One list as a compacted CSR: offsets receives node_count + 1 entries and *count the list's entries.  targets and
+ * values (either may be NULL) receive *count entries when *count <= capacity and are left untouched otherwise, so a
+ * caller that sized them from an earlier call, before another thread's batch landed, calls again with the new
+ * count; offsets and *count always describe the same state of the list as the targets copied with them. */
+gb_status gb_algraph_copy_csr(const gb_algraph* graph, gb_csr_which which, uint64_t capacity, uint32_t* offsets,
+                              uint32_t* targets, float* values, uint64_t* count);
+/* Snapshot: a fresh, immutable gb_graph whose CSRs are the lists' rows byte for byte, with the out (or undirected)
+ * list's values.  Its row order is known sorted for SORTED and DEDUPLICATED lists.  Every gb_graph entry then works
+ * on it (gb_page_rank, gb_wcc, gb_sssp, gb_triangle_count, gb_to_undirected, gb_graph_serialize, the accessors):
+ * the reference's algorithms are generic over the traits both graph types implement, so their results are defined
+ * by the rows alone.  gb_graph_last_timing of the snapshot holds the CUDA-event time of the copy. */
+gb_status gb_algraph_to_graph(const gb_algraph* graph, gb_graph** snapshot);
+gb_status gb_algraph_free(gb_algraph* graph);
 
 /* ---- algorithms ---------------------------------------------------------------------------- */
 /* page_rank(&graph, config) -> (Vec<f32>, usize, f64)     page_rank.rs:58-111

@@ -271,6 +271,116 @@ inline UndirectedCsrGraph DirectedCsrGraph::to_undirected_weighted(CsrLayout lay
   return UndirectedCsrGraph(u);
 }
 
+// Adjacency-list graphs, crates/builder/src/graph/adj_list.rs: DirectedALGraph<u32, (), EV> and
+// UndirectedALGraph<u32, (), EV> with EV = () or f32.  They take new edges (EdgeMutation::add_edge,
+// EdgeMutationWithValues::add_edge_with_value, lib.rs:415-456); a missing node throws graph::Error with the
+// reference's message (`node "3" does not exist in the graph ...`).  Neighbours are returned as copies, since rows
+// move when edges are added.  to_csr() snapshots the rows into an immutable CSR graph, on which the algorithms run.
+class ALGraphBase {
+ public:
+  explicit ALGraphBase(gb_algraph* g = nullptr) : g_(g) {}
+  ALGraphBase(const ALGraphBase&) = delete;
+  ALGraphBase& operator=(const ALGraphBase&) = delete;
+  ALGraphBase(ALGraphBase&& o) noexcept : g_(o.g_) { o.g_ = nullptr; }
+  ALGraphBase& operator=(ALGraphBase&& o) noexcept {
+    if (this != &o) {
+      if (g_) gb_algraph_free(g_);
+      g_ = o.g_;
+      o.g_ = nullptr;
+    }
+    return *this;
+  }
+  ~ALGraphBase() {
+    if (g_) gb_algraph_free(g_);
+  }
+  std::uint32_t node_count() const { return info().node_count; }  // adj_list.rs:311-322, :475-487
+  std::uint64_t edge_count() const { return info().edge_count; }
+  gb_algraph* handle() const { return g_; }
+  // len(src) add_edge calls in order, as one device batch: all or nothing
+  void add_edges(const std::vector<std::uint32_t>& src, const std::vector<std::uint32_t>& dst,
+                 const std::vector<float>& values = {}) {
+    if (src.size() != dst.size()) throw Error(GB_ERR_INVALID, "src and dst must have the same length");
+    if (!values.empty() && values.size() != src.size()) throw Error(GB_ERR_INVALID, "values must have one entry per edge");
+    detail::check(gb_algraph_add_edges_u32(g_, src.data(), dst.data(), values.empty() ? nullptr : values.data(),
+                                           src.size()));
+  }
+  void add_edge(std::uint32_t source, std::uint32_t target) { add_edges({source}, {target}); }
+  void add_edge_with_value(std::uint32_t source, std::uint32_t target, float value) {
+    add_edges({source}, {target}, {value});
+  }
+
+ protected:
+  gb_graph_info info() const {
+    gb_graph_info i{};
+    detail::check(gb_algraph_get_info(g_, &i));
+    return i;
+  }
+  std::uint32_t degree_of(gb_csr_which which, std::uint32_t node) const {
+    std::uint32_t len = 0;
+    detail::check(gb_algraph_copy_row(g_, which, node, 0, nullptr, nullptr, &len));
+    return len;
+  }
+  std::vector<std::uint32_t> row(gb_csr_which which, std::uint32_t node) const {
+    std::vector<std::uint32_t> t;
+    std::uint32_t len = degree_of(which, node);
+    for (;;) {  // another thread may add edges between the two calls
+      t.resize(len);
+      std::uint32_t got = 0;
+      detail::check(gb_algraph_copy_row(g_, which, node, len, t.data(), nullptr, &got));
+      if (got <= len) {
+        t.resize(got);
+        return t;
+      }
+      len = got;
+    }
+  }
+  std::vector<Target> row_with_values(gb_csr_which which, std::uint32_t node) const {
+    std::vector<std::uint32_t> t;
+    std::vector<float> w;
+    std::uint32_t len = degree_of(which, node);
+    for (;;) {
+      t.resize(len);
+      w.resize(len);
+      std::uint32_t got = 0;
+      detail::check(gb_algraph_copy_row(g_, which, node, len, t.data(), w.data(), &got));
+      if (got <= len) break;
+      len = got;
+    }
+    std::vector<Target> out(t.size());
+    for (std::size_t i = 0; i < t.size(); ++i) out[i] = Target{t[i], w[i]};
+    return out;
+  }
+  gb_graph* snapshot() const {
+    gb_graph* s = nullptr;
+    detail::check(gb_algraph_to_graph(g_, &s));
+    return s;
+  }
+  gb_algraph* g_ = nullptr;
+};
+
+// DirectedALGraph, adj_list.rs:279-450
+class DirectedALGraph : public ALGraphBase {
+ public:
+  using ALGraphBase::ALGraphBase;
+  std::uint32_t out_degree(std::uint32_t n) const { return degree_of(GB_CSR_OUT, n); }
+  std::uint32_t in_degree(std::uint32_t n) const { return degree_of(GB_CSR_IN, n); }
+  std::vector<std::uint32_t> out_neighbors(std::uint32_t n) const { return row(GB_CSR_OUT, n); }
+  std::vector<std::uint32_t> in_neighbors(std::uint32_t n) const { return row(GB_CSR_IN, n); }
+  std::vector<Target> out_neighbors_with_values(std::uint32_t n) const { return row_with_values(GB_CSR_OUT, n); }
+  std::vector<Target> in_neighbors_with_values(std::uint32_t n) const { return row_with_values(GB_CSR_IN, n); }
+  DirectedCsrGraph to_csr() const { return DirectedCsrGraph(snapshot()); }
+};
+
+// UndirectedALGraph, adj_list.rs:452-595
+class UndirectedALGraph : public ALGraphBase {
+ public:
+  using ALGraphBase::ALGraphBase;
+  std::uint32_t degree(std::uint32_t n) const { return degree_of(GB_CSR_UNDIRECTED, n); }
+  std::vector<std::uint32_t> neighbors(std::uint32_t n) const { return row(GB_CSR_UNDIRECTED, n); }
+  std::vector<Target> neighbors_with_values(std::uint32_t n) const { return row_with_values(GB_CSR_UNDIRECTED, n); }
+  UndirectedCsrGraph to_csr() const { return UndirectedCsrGraph(snapshot()); }
+};
+
 // GraphBuilder, crates/builder/src/builder.rs:123-539 (the in-memory edge-list states)
 class GraphBuilder {
  public:
@@ -388,8 +498,21 @@ class GraphBuilder {
                                                    static_cast<gb_layout>(layout_), &g));
     return UndirectedCsrGraph(g);
   }
+  // DirectedALGraph / UndirectedALGraph from the pending edges (adj_list.rs:406-450, :559-595): with values
+  // (EV = f32) when the builder holds them (edges_with_values(..), or an edge list read with with_values()).
+  // Graph500 and edge-list files; Binary and DotGraph files and node values have no adjacency-list form here.
+  DirectedALGraph build_directed_al() const { return DirectedALGraph(build_al(GB_KIND_DIRECTED)); }
+  UndirectedALGraph build_undirected_al() const { return UndirectedALGraph(build_al(GB_KIND_UNDIRECTED)); }
 
  private:
+  gb_algraph* build_al(gb_graph_kind kind) const {
+    if (!binary_path_.empty() || !labels_.empty())
+      throw Error(GB_ERR_UNSUPPORTED, "adjacency-list graphs are built from edges, Graph500 or edge-list files");
+    gb_algraph* g = nullptr;
+    detail::check(gb_algraph_from_edges_u32(device_, kind, src_.data(), dst_.data(), values_ ? w_.data() : nullptr,
+                                            src_.size(), n_, static_cast<gb_layout>(layout_), values_ ? 1 : 0, &g));
+    return g;
+  }
   CsrLayout layout_ = CsrLayout::Unsorted;  // CsrLayout::default()
   FileFormat format_ = FileFormat::EdgeList;
   bool with_values_ = false;
@@ -486,6 +609,17 @@ inline std::uint64_t global_triangle_count(const UndirectedCsrGraph& g) {
 }
 // relabel_graph(&mut graph)                                    triangle_count.rs:12-20
 inline void relabel_graph(UndirectedCsrGraph& g) { g.make_degree_ordered(); }
+
+// The algorithms on adjacency-list graphs: the reference's are generic over the traits both storage types
+// implement, so they run here on a snapshot of the rows (to_csr()), whose results the rows alone define.
+inline std::tuple<std::vector<float>, std::size_t, double> page_rank(const DirectedALGraph& g, PageRankConfig c) {
+  return page_rank(g.to_csr(), c);
+}
+inline Components wcc_afforest(const DirectedALGraph& g, WccConfig c = {}) { return wcc_afforest(g.to_csr(), c); }
+inline std::vector<float> delta_stepping(const DirectedALGraph& g, DeltaSteppingConfig c) {
+  return delta_stepping(g.to_csr(), c);
+}
+inline std::uint64_t global_triangle_count(const UndirectedALGraph& g) { return global_triangle_count(g.to_csr()); }
 
 }  // namespace prelude
 }  // namespace graph
