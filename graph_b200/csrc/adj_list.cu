@@ -39,12 +39,6 @@ struct AlList {
   uint64_t bytes() const { return start.bytes() + len.bytes() + cap.bytes() + tgt.bytes() + w.bytes(); }
 };
 
-static inline uint32_t al_bits(uint32_t n) {  // bits of a row id (graph.cu's bits_for)
-  uint32_t b = 1;
-  while (b < 32 && (1ull << b) < n) ++b;
-  return b;
-}
-
 }  // namespace gb
 
 struct gb_algraph {
@@ -287,10 +281,6 @@ __global__ void k_al_narrow(const uint64_t* __restrict__ a, uint64_t count, uint
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------
-static gb_status excl_scan(cudaStream_t s, DevBuf<uint8_t>& tmp, uint64_t* a, uint64_t count) {
-  return cub_call(tmp, [&](void* t, size_t& tb) { return cub::DeviceScan::ExclusiveSum(t, tb, a, a, (int64_t)count, s); });
-}
-
 static gb_status d2h(cudaStream_t s, void* host, const void* dev, size_t bytes) {
   GB_CUDA(cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, s));
   GB_CUDA(cudaStreamSynchronize(s));
@@ -302,7 +292,7 @@ static gb_status len_prefix(cudaStream_t s, const AlList& L, uint32_t n, DevBuf<
   DevBuf<uint8_t> tmp;
   GB_TRY(prefix->alloc((size_t)n + 1));
   k_al_widen<<<grid_for((uint64_t)n + 1, 256), 256, 0, s>>>(L.len.p, n, prefix->p);
-  GB_TRY(excl_scan(s, tmp, prefix->p, (uint64_t)n + 1));
+  GB_TRY(exclusive_sum(s, tmp, prefix->p, (int64_t)n + 1));
   GB_TRY(d2h(s, total, prefix->p + n, 8));
   return GB_OK;
 }
@@ -348,11 +338,14 @@ static gb_status list_from_csr(cudaStream_t s, uint32_t n, DevCsr& csr, bool val
   return GB_OK;
 }
 
-// AdjacencyList::from for every list of g (adj_list.rs:216-277), from device edges whose ids are checked
+// Checks device edge arrays on g's stream (check_edge_ids, with g->n), then AdjacencyList::from for every list of g
+// (adj_list.rs:216-277); d_w is read only when g carries values
 static gb_status build_lists(gb_algraph* g, const uint32_t* d_src, const uint32_t* d_dst, const float* d_w,
                              uint64_t m) {
   cudaStream_t s = g->stream;
   const gb_layout lay = g->layout;
+  GB_TRY(check_edge_ids(s, d_src, d_dst, m, &g->n));
+  if (!g->values) d_w = nullptr;
   if (g->kind == GB_KIND_DIRECTED) {
     DevCsr out, in;
     GB_TRY(build_csr_device(s, g->n, d_src, d_dst, d_w, m, lay, &out, 0, true));
@@ -392,20 +385,6 @@ static gb_status new_algraph(int device, gb_graph_kind kind, gb_layout layout, b
   return GB_OK;
 }
 
-static gb_status check_al_args(gb_graph_kind kind, const void* src, const void* dst, const void* w, uint64_t m,
-                               uint32_t n, gb_layout layout, int with_values, gb_algraph** out) {
-  GB_REQUIRE(out != nullptr, "graph out-pointer is NULL");
-  GB_REQUIRE(kind == GB_KIND_DIRECTED || kind == GB_KIND_UNDIRECTED, "bad graph kind %d", (int)kind);
-  GB_REQUIRE(m == 0 || (src && dst), "edge arrays are NULL");
-  GB_REQUIRE(m == 0 || !with_values || w, "weights is NULL");
-  GB_TRY(check_layout(layout));
-  const uint64_t entries = (kind == GB_KIND_UNDIRECTED) ? 2 * m : m;
-  GB_REQUIRE(m < AL_MAX_ENTRIES && entries < AL_MAX_ENTRIES, "edge count %llu does not fit u32 offsets",
-             (unsigned long long)m);
-  GB_REQUIRE(n != 0 || m > 0, "cannot infer node_count from an empty edge list");
-  return GB_OK;
-}
-
 // builds an adjacency-list graph from device edge arrays, after work enqueued on `caller`
 static gb_status algraph_from_device(int device, gb_graph_kind kind, const uint32_t* d_src, const uint32_t* d_dst,
                                      const float* d_w, uint64_t m, uint32_t n, gb_layout layout, bool values,
@@ -413,14 +392,8 @@ static gb_status algraph_from_device(int device, gb_graph_kind kind, const uint3
   AlPtr g(nullptr, al_free);
   GB_TRY(new_algraph(device, kind, layout, values, n, &g));
   DevBufStreamScope scope(g->stream);
-  cudaEvent_t ready;
-  GB_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
-  cudaError_t e = cudaEventRecord(ready, caller);
-  if (e == cudaSuccess) e = cudaStreamWaitEvent(g->stream, ready, 0);
-  cudaEventDestroy(ready);
-  GB_CUDA(e);
-  GB_TRY(check_edge_ids(g->stream, d_src, d_dst, m, &g->n));
-  GB_TRY(build_lists(g.get(), d_src, d_dst, values ? d_w : nullptr, m));
+  GB_TRY(wait_on_stream(g->stream, caller));
+  GB_TRY(build_lists(g.get(), d_src, d_dst, d_w, m));
   *out = g.release();
   return GB_OK;
 }
@@ -442,7 +415,7 @@ struct AlStep {
 static gb_status prepare_list(gb_algraph* g, const AlList& L, const uint32_t* d_src, const uint32_t* d_dst,
                               const float* d_w, uint64_t b, bool reversed, AlStep& st, gb_algraph_batch_info* info) {
   cudaStream_t s = g->stream;
-  const uint32_t n = g->n, bits = al_bits(n);
+  const uint32_t n = g->n, bits = bits_for(n);
   const bool pairs = g->kind == GB_KIND_UNDIRECTED;
   const bool sorted = g->layout != GB_LAYOUT_UNSORTED;
   const uint64_t B = pairs ? 2 * b : b;
@@ -530,7 +503,8 @@ static gb_status prepare_list(gb_algraph* g, const AlList& L, const uint32_t* d_
   p.dst = a + 6 * R1;
   p.rcap = rcap.p;
   k_al_plan<<<grid_for(R1, blk), blk, 0, s>>>(U.p, C.p, R, L.start.p, L.len.p, L.cap.p, p, moved.p);
-  for (uint64_t* x : {p.run_off, p.ex_off, p.sc_off, p.tail_off, p.cp_off}) GB_TRY(excl_scan(s, tmp, x, R1));
+  for (uint64_t* x : {p.run_off, p.ex_off, p.sc_off, p.tail_off, p.cp_off})
+    GB_TRY(exclusive_sum(s, tmp, x, (int64_t)R1));
   uint64_t &ex_total = st.ex_total, &sc_total = st.sc_total, &tail_total = st.tail_total, &cp_total = st.cp_total;
   unsigned long long nmoved = 0;
   GB_CUDA(cudaMemcpyAsync(&ex_total, p.ex_off + R, 8, cudaMemcpyDeviceToHost, s));
@@ -554,7 +528,7 @@ static gb_status prepare_list(gb_algraph* g, const AlList& L, const uint32_t* d_
     GB_TRY(st.caps.alloc((size_t)n + 1));
     k_al_widen<<<grid_for((uint64_t)n + 1, blk), blk, 0, s>>>(L.cap.p, n, st.caps.p);
     k_al_set_caps<<<grid_for(R, blk), blk, 0, s>>>(U.p, R, p.rcap, st.caps.p);
-    GB_TRY(excl_scan(s, tmp, st.caps.p, (uint64_t)n + 1));
+    GB_TRY(exclusive_sum(s, tmp, st.caps.p, (int64_t)n + 1));
     GB_TRY(d2h(s, &st.cap_total, st.caps.p + n, 8));
     GB_TRY(len_prefix(s, L, n, &st.live, &st.live_total));
     st.pool = 2 * st.cap_total + AL_MIN_TAIL;
@@ -704,29 +678,24 @@ extern "C" {
 gb_status gb_algraph_from_edges_u32(int device, gb_graph_kind kind, const uint32_t* src, const uint32_t* dst,
                                     const float* weights, uint64_t edge_count, uint32_t node_count, gb_layout layout,
                                     int with_values, gb_algraph** graph) {
-  GB_TRY(check_al_args(kind, src, dst, weights, edge_count, node_count, layout, with_values, graph));
+  GB_TRY(check_edge_args(kind, src, dst, weights, edge_count, node_count, layout, with_values != 0, graph));
   GB_TRY(require_device(device));
   DeviceGuard guard(device);
-  const uint64_t m = edge_count;
-  DevBuf<uint32_t> d_src, d_dst;
-  DevBuf<float> d_w;
-  GB_TRY(d_src.alloc(m));
-  GB_TRY(d_dst.alloc(m));
-  if (with_values) GB_TRY(d_w.alloc(m));
-  if (m) {
-    GB_CUDA(cudaMemcpy(d_src.p, src, m * 4, cudaMemcpyHostToDevice));
-    GB_CUDA(cudaMemcpy(d_dst.p, dst, m * 4, cudaMemcpyHostToDevice));
-    if (with_values) GB_CUDA(cudaMemcpy(d_w.p, weights, m * 4, cudaMemcpyHostToDevice));
-  }
-  return algraph_from_device(device, kind, d_src.p, d_dst.p, d_w.p, m, node_count, layout, with_values != 0,
-                             cudaStreamLegacy, graph);
+  AlPtr g(nullptr, al_free);
+  GB_TRY(new_algraph(device, kind, layout, with_values != 0, node_count, &g));
+  DevBufStreamScope scope(g->stream);
+  EdgeArrays e;
+  GB_TRY(upload_edges(g->stream, src, dst, with_values ? weights : nullptr, edge_count, &e));
+  GB_TRY(build_lists(g.get(), e.src.p, e.dst.p, e.w.p, edge_count));
+  *graph = g.release();
+  return GB_OK;
 }
 
 gb_status gb_algraph_from_device_edges_u32(int device, gb_graph_kind kind, const uint32_t* d_src,
                                            const uint32_t* d_dst, const float* d_weights, uint64_t edge_count,
                                            uint32_t node_count, gb_layout layout, int with_values, void* stream,
                                            gb_algraph** graph) {
-  GB_TRY(check_al_args(kind, d_src, d_dst, d_weights, edge_count, node_count, layout, with_values, graph));
+  GB_TRY(check_edge_args(kind, d_src, d_dst, d_weights, edge_count, node_count, layout, with_values != 0, graph));
   GB_TRY(require_device(device));
   DeviceGuard guard(device);
   if (edge_count) {
@@ -746,7 +715,7 @@ gb_status gb_algraph_load_u32(int device, gb_graph_kind kind, const char* path, 
   EdgeArrays e;
   GB_TRY(load_edge_arrays(device, path, format, with_values != 0, &e));
   DeviceGuard guard(device);
-  GB_TRY(check_al_args(kind, e.src.p, e.dst.p, e.w.p, e.m, e.n, layout, with_values, graph));
+  GB_TRY(check_edge_args(kind, e.src.p, e.dst.p, e.w.p, e.m, e.n, layout, with_values != 0, graph));
   GB_TRY(algraph_from_device(device, kind, e.src.p, e.dst.p, e.w.p, e.m, e.n, layout, with_values != 0, nullptr,
                              graph));
   (*graph)->load = e.info;
@@ -760,20 +729,9 @@ gb_status gb_algraph_add_edges_u32(gb_algraph* g, const uint32_t* src, const uin
   std::lock_guard<std::mutex> lock(g->mu);
   GB_TRY(check_batch(g, src, dst, weights, edge_count));
   DevBufStreamScope scope(g->stream);
-  const uint64_t b = edge_count;
-  DevBuf<uint32_t> d_src, d_dst;
-  DevBuf<float> d_w;
-  if (b) {
-    GB_TRY(d_src.alloc(b));
-    GB_TRY(d_dst.alloc(b));
-    GB_CUDA(cudaMemcpyAsync(d_src.p, src, b * 4, cudaMemcpyHostToDevice, g->stream));
-    GB_CUDA(cudaMemcpyAsync(d_dst.p, dst, b * 4, cudaMemcpyHostToDevice, g->stream));
-    if (g->values) {
-      GB_TRY(d_w.alloc(b));
-      GB_CUDA(cudaMemcpyAsync(d_w.p, weights, b * 4, cudaMemcpyHostToDevice, g->stream));
-    }
-  }
-  return add_edges_locked(g, d_src.p, d_dst.p, d_w.p, b);
+  EdgeArrays e;
+  if (edge_count) GB_TRY(upload_edges(g->stream, src, dst, g->values ? weights : nullptr, edge_count, &e));
+  return add_edges_locked(g, e.src.p, e.dst.p, e.w.p, edge_count);
 }
 
 gb_status gb_algraph_add_device_edges_u32(gb_algraph* g, const uint32_t* d_src, const uint32_t* d_dst,
@@ -788,12 +746,7 @@ gb_status gb_algraph_add_device_edges_u32(gb_algraph* g, const uint32_t* d_src, 
     if (g->values) GB_TRY(require_device_array(d_weights, g->device, "d_weights"));
   }
   DevBufStreamScope scope(g->stream);
-  cudaEvent_t ready;
-  GB_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
-  cudaError_t e = cudaEventRecord(ready, static_cast<cudaStream_t>(stream));
-  if (e == cudaSuccess) e = cudaStreamWaitEvent(g->stream, ready, 0);
-  cudaEventDestroy(ready);
-  GB_CUDA(e);
+  GB_TRY(wait_on_stream(g->stream, static_cast<cudaStream_t>(stream)));
   return add_edges_locked(g, d_src, d_dst, d_weights, edge_count);
 }
 

@@ -276,6 +276,27 @@ gb_status cub_call(DevBuf<uint8_t>& tmp, Call&& call, size_t headroom = 1) {
   return GB_OK;
 }
 
+// CUB's in-place prefix sums and its radix pair sort over bits [0, end_bit), enqueued on s through cub_call; N, the
+// count's type, is CUB's offset type.  For the translation units that include CUB first: an include of CUB emits a
+// kernel into its translation unit, so this header does not pull it in.
+#ifdef CUB_VERSION
+template <typename T, typename N>
+gb_status exclusive_sum(cudaStream_t s, DevBuf<uint8_t>& tmp, T* a, N count) {
+  return cub_call(tmp, [&](void* t, size_t& tb) { return cub::DeviceScan::ExclusiveSum(t, tb, a, a, count, s); });
+}
+template <typename T, typename N>
+gb_status inclusive_sum(cudaStream_t s, DevBuf<uint8_t>& tmp, T* a, N count) {
+  return cub_call(tmp, [&](void* t, size_t& tb) { return cub::DeviceScan::InclusiveSum(t, tb, a, a, count, s); });
+}
+template <typename K, typename V, typename N>
+gb_status sort_pairs(cudaStream_t s, DevBuf<uint8_t>& tmp, cub::DoubleBuffer<K>& k, cub::DoubleBuffer<V>& v, N count,
+                     int end_bit) {
+  return cub_call(tmp, [&](void* t, size_t& tb) {
+    return cub::DeviceRadixSort::SortPairs(t, tb, k, v, count, 0, end_bit, s);
+  });
+}
+#endif
+
 // ---- device CSR ----------------------------------------------------------------------------
 // offsets[n+1] u32, targets[len] u32 (+8 entries of zeroed slack for 128-bit loads), optional
 // SoA weights[len] f32 (the host API exposes the reference's 8-byte AoS Target{u32,f32}).
@@ -356,8 +377,9 @@ gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, c
 gb_status check_edge_ids(cudaStream_t s, const uint32_t* d_src, const uint32_t* d_dst, uint64_t m, uint32_t* n);
 // GB_ERR_INVALID unless p is device (or managed) memory of `device`
 gb_status require_device_array(const void* p, int device, const char* what);
-// Edge arrays read from a file on the device (load.cu): Graph500 or text edge list through the pinned-ring
-// pipeline, in file order.  n is edges / 16 for Graph500 and 0 (max id + 1) for an edge list.
+// Edge arrays on the device: read from a file (load.cu: Graph500 or text edge list through the pinned-ring
+// pipeline, in file order; n is edges / 16 for Graph500 and 0 (max id + 1) for an edge list), or copied from the
+// host (upload_edges).
 struct EdgeArrays {
   DevBuf<uint32_t> src, dst;
   DevBuf<float> w;
@@ -366,6 +388,16 @@ struct EdgeArrays {
   gb_load_info info{};
 };
 gb_status load_edge_arrays(int device, const char* path, gb_file_format format, bool with_values, EdgeArrays* out);
+// Copies m host edges into out->src, out->dst on stream s, and their values into out->w when w is not NULL (out->w
+// is allocated then even for m = 0, which marks a build with values).  Returns once the copies are enqueued.
+gb_status upload_edges(cudaStream_t s, const uint32_t* src, const uint32_t* dst, const float* w, uint64_t m,
+                       EdgeArrays* out);
+// The argument checks of every edge-list constructor, in this order: out, the kind, the edge arrays, the weights
+// (with_values only), the layout, the u32 offset limit (2m entries when undirected) and n = 0 without edges.
+gb_status check_edge_args(gb_graph_kind kind, const void* src, const void* dst, const void* w, uint64_t m, uint32_t n,
+                          gb_layout layout, bool with_values, const void* out);
+// Makes stream s wait for the work enqueued on `caller` so far (a caller's producer work comes first).
+gb_status wait_on_stream(cudaStream_t s, cudaStream_t caller);
 gb_status new_graph(int device, gb_graph_kind kind, uint32_t n, GraphPtr* out);
 // Uploads a host CSR on stream s and checks it: require_host_csr on the host, the offsets monotone and the
 // targets below n on the device.  offsets_only uploads the offsets alone (degrees); w may be NULL.  Returns
@@ -408,5 +440,29 @@ inline unsigned grid_for(uint64_t items, unsigned block, unsigned max_blocks = H
   if (b < 1) b = 1;
   if (b > max_blocks) b = max_blocks;
   return static_cast<unsigned>(b);
+}
+
+// bits of the largest id below n (at least 1, at most 32): the width of a field of a packed sort key
+inline uint32_t bits_for(uint64_t n) {
+  uint32_t b = 1;
+  while (b < 32 && (1ull << b) < n) ++b;
+  return b;
+}
+
+// The library is built without -rdc, so a kernel launched from several translation units lives here; templates,
+// so that a translation unit that does not launch one emits nothing.
+template <typename T>
+__global__ void k_iota(T* __restrict__ a, uint64_t count) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
+       i += (uint64_t)gridDim.x * blockDim.x)
+    a[i] = (T)i;
+}
+
+template <typename T>
+__global__ void k_gather(const T* __restrict__ src, const uint32_t* __restrict__ idx, uint64_t count,
+                         T* __restrict__ dst) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
+       i += (uint64_t)gridDim.x * blockDim.x)
+    dst[i] = src[idx[i]];
 }
 }  // namespace gb

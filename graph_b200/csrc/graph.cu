@@ -38,24 +38,12 @@ gb_status fail(gb_status st, const char* fmt, ...) {
 static std::atomic<bool> g_profiling{false};
 bool profiling_on() { return g_profiling.load(std::memory_order_relaxed); }
 
-static inline uint32_t bits_for(uint32_t n) {
-  uint32_t b = 1;
-  while (b < 32 && (1ull << b) < n) ++b;
-  return b;
-}
-
 // ---- kernels -------------------------------------------------------------------------------
 __global__ void k_pack_keys(const uint32_t* __restrict__ rows, const uint32_t* __restrict__ cols,
                             uint64_t count, uint32_t bits, uint64_t* __restrict__ keys) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
        i += (uint64_t)gridDim.x * blockDim.x)
     keys[i] = ((uint64_t)rows[i] << bits) | cols[i];
-}
-
-__global__ void k_iota(uint32_t* __restrict__ a, uint64_t count) {
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
-       i += (uint64_t)gridDim.x * blockDim.x)
-    a[i] = (uint32_t)i;
 }
 
 // offsets from a row-sorted sequence: the end of each non-empty row's run is marked at
@@ -99,14 +87,6 @@ __global__ void k_unpack_targets(const uint64_t* __restrict__ keys, uint64_t cou
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
        i += (uint64_t)gridDim.x * blockDim.x)
     tgt[i] = (uint32_t)(keys[i] & mask);
-}
-
-template <typename T>
-__global__ void k_gather(const T* __restrict__ src, const uint32_t* __restrict__ idx, uint64_t count,
-                         T* __restrict__ dst) {
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
-       i += (uint64_t)gridDim.x * blockDim.x)
-    dst[i] = src[idx[i]];
 }
 
 // The values of an undirected build: its 2m entries are the outgoing pass (entry j < m is edge j) and the incoming
@@ -242,9 +222,7 @@ gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, c
     cub::DoubleBuffer<uint32_t> kb(rows_copy.p, keys_alt.p);
     cub::DoubleBuffer<uint32_t> vb(idx.p, idx_alt.p);
     DevBuf<uint8_t> tmp;
-    GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
-      return cub::DeviceRadixSort::SortPairs(t, tb, kb, vb, count, 0, (int)bits, s);
-    }));
+    GB_TRY(sort_pairs(s, tmp, kb, vb, count, (int)bits));
     GB_TRY(csr->tgt.alloc(count, 8));
     GB_CUDA(cudaMemsetAsync(csr->tgt.p + count, 0, 8 * 4, s));
     k_gather<uint32_t><<<grid_for(count, blk), blk, 0, s>>>(d_cols, vb.Current(), count, csr->tgt.p);
@@ -272,9 +250,7 @@ gb_status build_csr_device(cudaStream_t s, uint32_t n, const uint32_t* d_rows, c
     GB_TRY(idx_alt.alloc(count));
     k_iota<<<grid_for(count, blk), blk, 0, s>>>(idx.p, count);
     cub::DoubleBuffer<uint32_t> vb(idx.p, idx_alt.p);
-    GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
-      return cub::DeviceRadixSort::SortPairs(t, tb, kb, vb, count, 0, (int)(2 * bits), s);
-    }));
+    GB_TRY(sort_pairs(s, tmp, kb, vb, count, (int)(2 * bits)));
     order = vb.Current();
   } else {
     GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
@@ -627,15 +603,41 @@ __global__ void k_max_ids(const uint32_t* __restrict__ a, const uint32_t* __rest
   if ((threadIdx.x & 31) == 0) atomicMax(mx, v);
 }
 
-// the argument checks of the host and the device edge paths
-static gb_status check_edge_args(gb_graph_kind kind, const uint32_t* src, const uint32_t* dst, uint64_t m,
-                                 uint32_t n, gb_layout layout, gb_graph** out) {
+gb_status check_edge_args(gb_graph_kind kind, const void* src, const void* dst, const void* w, uint64_t m, uint32_t n,
+                          gb_layout layout, bool with_values, const void* out) {
   GB_REQUIRE(out != nullptr, "graph out-pointer is NULL");
+  GB_REQUIRE(kind == GB_KIND_DIRECTED || kind == GB_KIND_UNDIRECTED, "bad graph kind %d", (int)kind);
   GB_REQUIRE(m == 0 || (src && dst), "edge arrays are NULL");
+  GB_REQUIRE(m == 0 || !with_values || w, "weights is NULL");
   GB_TRY(check_layout(layout));
-  uint64_t cap = (kind == GB_KIND_UNDIRECTED) ? 2 * m : m;
-  GB_REQUIRE(cap < 0xFFFFFFFFull, "edge count %llu does not fit u32 offsets", (unsigned long long)m);
+  const uint64_t entries = (kind == GB_KIND_UNDIRECTED) ? 2 * m : m;
+  GB_REQUIRE(m < 0xFFFFFFFFull && entries < 0xFFFFFFFFull, "edge count %llu does not fit u32 offsets",
+             (unsigned long long)m);
   GB_REQUIRE(n != 0 || m > 0, "cannot infer node_count from an empty edge list");
+  return GB_OK;
+}
+
+gb_status upload_edges(cudaStream_t s, const uint32_t* src, const uint32_t* dst, const float* w, uint64_t m,
+                       EdgeArrays* out) {
+  GB_TRY(out->src.alloc(m));
+  GB_TRY(out->dst.alloc(m));
+  if (w) GB_TRY(out->w.alloc(m));
+  out->m = m;
+  if (m) {
+    GB_CUDA(cudaMemcpyAsync(out->src.p, src, m * 4, cudaMemcpyHostToDevice, s));
+    GB_CUDA(cudaMemcpyAsync(out->dst.p, dst, m * 4, cudaMemcpyHostToDevice, s));
+    if (w) GB_CUDA(cudaMemcpyAsync(out->w.p, w, m * 4, cudaMemcpyHostToDevice, s));
+  }
+  return GB_OK;
+}
+
+gb_status wait_on_stream(cudaStream_t s, cudaStream_t caller) {
+  cudaEvent_t ready;
+  GB_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
+  cudaError_t e = cudaEventRecord(ready, caller);
+  if (e == cudaSuccess) e = cudaStreamWaitEvent(s, ready, 0);
+  cudaEventDestroy(ready);
+  GB_CUDA(e);
   return GB_OK;
 }
 
@@ -675,20 +677,12 @@ static gb_status build_from_edges(gb_graph* g, const uint32_t* d_src, const uint
 static gb_status graph_from_host_edges(int device, gb_graph_kind kind, const uint32_t* src,
                                        const uint32_t* dst, const float* w, uint64_t m, uint32_t n,
                                        gb_layout layout, gb_graph** out) {
-  GB_TRY(check_edge_args(kind, src, dst, m, n, layout, out));
+  GB_TRY(check_edge_args(kind, src, dst, w, m, n, layout, false, out));
   GraphPtr g;
   GB_TRY(new_graph(device, kind, n, &g));
-  DevBuf<uint32_t> d_src, d_dst;
-  DevBuf<float> d_w;
-  GB_TRY(d_src.alloc(m));
-  GB_TRY(d_dst.alloc(m));
-  if (w) GB_TRY(d_w.alloc(m));
-  if (m) {
-    GB_CUDA(cudaMemcpyAsync(d_src.p, src, m * 4, cudaMemcpyHostToDevice, g->stream));
-    GB_CUDA(cudaMemcpyAsync(d_dst.p, dst, m * 4, cudaMemcpyHostToDevice, g->stream));
-    if (w) GB_CUDA(cudaMemcpyAsync(d_w.p, w, m * 4, cudaMemcpyHostToDevice, g->stream));
-  }
-  GB_TRY(build_from_edges(g.get(), d_src.p, d_dst.p, d_w.p, m, layout));
+  EdgeArrays e;
+  GB_TRY(upload_edges(g->stream, src, dst, w, m, &e));
+  GB_TRY(build_from_edges(g.get(), e.src.p, e.dst.p, e.w.p, m, layout));
   *out = g.release();
   return GB_OK;
 }
@@ -730,7 +724,7 @@ gb_status require_device_array(const void* p, int device, const char* what) {
 gb_status graph_from_device_arrays(int device, gb_graph_kind kind, const uint32_t* d_src, const uint32_t* d_dst,
                                    const float* d_w, uint64_t m, uint32_t n, gb_layout layout, cudaStream_t caller,
                                    gb_graph** out) {
-  GB_TRY(check_edge_args(kind, d_src, d_dst, m, n, layout, out));
+  GB_TRY(check_edge_args(kind, d_src, d_dst, d_w, m, n, layout, false, out));
   GraphPtr g;
   GB_TRY(new_graph(device, kind, n, &g));
   if (m) {
@@ -738,13 +732,7 @@ gb_status graph_from_device_arrays(int device, gb_graph_kind kind, const uint32_
     GB_TRY(require_device_array(d_dst, device, "d_dst"));
     if (d_w) GB_TRY(require_device_array(d_w, device, "d_weights"));
   }
-  // the caller's producer work comes first
-  cudaEvent_t ready;
-  GB_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
-  cudaError_t e = cudaEventRecord(ready, caller);
-  if (e == cudaSuccess) e = cudaStreamWaitEvent(g->stream, ready, 0);
-  cudaEventDestroy(ready);
-  GB_CUDA(e);
+  GB_TRY(wait_on_stream(g->stream, caller));
   GB_TRY(build_from_edges(g.get(), d_src, d_dst, d_w, m, layout));
   *out = g.release();
   return GB_OK;

@@ -29,11 +29,6 @@ constexpr unsigned FULL_MASK = 0xFFFFFFFFu;
 
 static int label_bits(uint32_t max_label) { return max_label ? 32 - __builtin_clz(max_label) : 1; }
 
-__global__ void k_iota_u32(uint32_t* __restrict__ a, uint64_t count) {
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count; i += (uint64_t)gridDim.x * blockDim.x)
-    a[i] = (uint32_t)i;
-}
-
 __global__ void k_max_degree(const uint32_t* __restrict__ off, uint32_t n, unsigned int* __restrict__ mx) {
   uint32_t d = 0;
   for (uint64_t v = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; v < n; v += (uint64_t)gridDim.x * blockDim.x)
@@ -256,7 +251,7 @@ static gb_status sort_by_label(const gb_graph* g, DevBuf<uint8_t>& tmp, uint32_t
   GB_TRY(iota.alloc(n));
   GB_TRY(keys->alloc(n));
   GB_TRY(nodes->alloc(n));
-  k_iota_u32<<<grid_for(n, 256), 256, 0, s>>>(iota.p, n);
+  k_iota<<<grid_for(n, 256), 256, 0, s>>>(iota.p, n);
   GB_CUDA(cudaGetLastError());
   const int bits = label_bits(max_label);
   GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
@@ -406,9 +401,7 @@ static gb_status neighbor_label_frequencies(const gb_graph* g, uint32_t* offsets
     GB_TRY(seg.alloc((uint64_t)hubs + 1));
     k_hub_degrees<<<grid_for(hubs, 256), 256, 0, s>>>(rows.p, hubs, off, seg.p);
     GB_CUDA(cudaGetLastError());
-    GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
-      return cub::DeviceScan::ExclusiveSum(t, tb, seg.p, seg.p, (int64_t)hubs + 1, s);
-    }));
+    GB_TRY(exclusive_sum(s, tmp, seg.p, (int64_t)hubs + 1));
     uint32_t hub_entries = 0;
     GB_CUDA(cudaMemcpyAsync(&hub_entries, seg.p + hubs, 4, cudaMemcpyDeviceToHost, s));
     GB_CUDA(cudaStreamSynchronize(s));

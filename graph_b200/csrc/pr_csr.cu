@@ -200,9 +200,7 @@ gb_status pr_csr_plans(const std::vector<int>& devs, uint32_t V, uint32_t n, con
       GB_TRY(k.loc_off.alloc((size_t)n + 1));
       k_pr_owned_deg<<<grid_for((uint64_t)n + 1, 256), 256, 0, k.s>>>(k.in_off.p, new_id, n, U, r, k.loc_off.p);
       DevBuf<uint8_t> tmp;
-      GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
-        return cub::DeviceScan::ExclusiveSum(t, tb, k.loc_off.p, k.loc_off.p, (int)(n + 1), k.s);
-      }));
+      GB_TRY(exclusive_sum(k.s, tmp, k.loc_off.p, (int)(n + 1)));
       uint32_t total = 0;
       GB_CUDA(cudaMemcpyAsync(&total, k.loc_off.p + n, 4, cudaMemcpyDeviceToHost, k.s));
       GB_CUDA(cudaStreamSynchronize(k.s));

@@ -534,11 +534,6 @@ __global__ void k_vb_groups(const uint32_t* __restrict__ lens, uint32_t n_loc, u
     g[l] = lens[l] ? (lens[l] + CB_G - 1) / CB_G : 1u;  // a row without cold edges keeps one padding group
 }
 
-__global__ void k_gather_u32(const uint32_t* __restrict__ src, const uint32_t* __restrict__ idx, uint32_t count,
-                             uint32_t* __restrict__ dst) {
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) dst[i] = src[idx[i]];
-}
-
 // Chunks: block j's stream [gbeg[j], gbeg[j+1]) is cut every C_j groups; a cut inside a segment moves to
 // the segment's end unless the segment is longer than C_j groups, in which case the cut stays and both
 // neighbours handle a PART of it (side buffer + fixup), so no warp ever owns more than 2 C_j groups.
@@ -691,14 +686,6 @@ __global__ void __launch_bounds__(CB_BANK_THREADS) k_cb_bank_order(const uint4* 
 // The degrees (order, hot blocks, staircase) come from the PrSource's full offsets; the rows' edges from the
 // row source (row_off, row_tgt) given to layout_end, which for a resident twin is its in-CSR.
 template <typename T>
-static gb_status scan_exclusive(cudaStream_t s, T* data, uint64_t count) {
-  GB_REQUIRE(count < (1ull << 31), "scan of %llu items is too long", (unsigned long long)count);
-  DevBuf<uint8_t> tmp;
-  GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) { return cub::DeviceScan::ExclusiveSum(t, tb, data, data, (int)count, s); }));
-  GB_CUDA(cudaStreamSynchronize(s));
-  return GB_OK;
-}
-template <typename T>
 static gb_status upload(cudaStream_t s, DevBuf<T>* dst, const std::vector<T>& src, size_t pad = 0) {
   GB_TRY(dst->alloc(std::max<size_t>(src.size(), 1), pad));
   if (!src.empty()) GB_CUDA(cudaMemcpyAsync(dst->p, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice, s));
@@ -760,7 +747,7 @@ gb_status LayoutBuild::layout_order() {
     cub::DoubleBuffer<uint64_t> kb(keys.p, keys_alt.p);
     cub::DoubleBuffer<uint32_t> vb(ids.p, ids_alt.p);
     DevBuf<uint8_t> tmp;
-    GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) { return cub::DeviceRadixSort::SortPairs(t, tb, kb, vb, (int)n, 0, 64, s); }));
+    GB_TRY(sort_pairs(s, tmp, kb, vb, (int)n, 64));
     GB_TRY(p->new_id.alloc(n));
     GB_TRY(p->outdeg.alloc(n));
     GB_TRY(indeg.alloc((size_t)n + 1));
@@ -934,8 +921,7 @@ gb_status LayoutBuild::layout_classify() {
     k_mega_keys<<<grid_for(M, 256), 256, 0, s>>>(row_off, row_tgt, old_of.p, p->new_id.p,
                                                  hot_of_blk.p, p->hot.nrows.p, B, mega_off.p, n_mega, M, deal,
                                                  keys_in.p, vals_in.p);
-    uint32_t row_bits = 1;
-    while ((1u << row_bits) < n_mega) ++row_bits;
+    const uint32_t row_bits = bits_for(n_mega);
     uint32_t* start = mega_start.p;
     DevBuf<uint8_t> tmp, stmp;
     GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
@@ -956,7 +942,10 @@ gb_status LayoutBuild::layout_classify() {
     k_lens_tail<<<grid_for(p->n_loc - p->n_cb, 256), 256, 0, s>>>(indeg.p, p->n_cb, p->n_loc, deal, lens.p);
   if (p->hot.S) {
     k_cb_groups<<<grid_for(p->hot.S, 256), 256, 0, s>>>(goff.p, p->hot.S);
-    GB_TRY(scan_exclusive(s, goff.p, p->hot.S + 1));
+    GB_REQUIRE(p->hot.S + 1 < (1ull << 31), "scan of %llu items is too long", (unsigned long long)p->hot.S + 1);
+    DevBuf<uint8_t> tmp;
+    GB_TRY(exclusive_sum(s, tmp, goff.p, (int)(p->hot.S + 1)));
+    GB_CUDA(cudaStreamSynchronize(s));
     uint32_t ng = 0;
     GB_CUDA(cudaMemcpyAsync(&ng, goff.p + p->hot.S, 4, cudaMemcpyDeviceToHost, s));
     GB_CUDA(cudaStreamSynchronize(s));
@@ -979,7 +968,12 @@ gb_status LayoutBuild::layout_sell() {
   GB_TRY(bases.alloc(p->num_slices));
   k_sell_widths<<<grid_for((uint64_t)p->num_slices * 32, 256), 256, 0, s>>>(lens.p, p->n_loc, p->num_slices, units.p);
   GB_CUDA(cudaMemcpyAsync(bases.p, units.p, (size_t)p->num_slices * 4, cudaMemcpyDeviceToDevice, s));
-  GB_TRY(scan_exclusive(s, bases.p, p->num_slices));
+  GB_REQUIRE(p->num_slices < (1ull << 31), "scan of %llu items is too long", (unsigned long long)p->num_slices);
+  {
+    DevBuf<uint8_t> tmp;
+    GB_TRY(exclusive_sum(s, tmp, bases.p, (int)p->num_slices));
+    GB_CUDA(cudaStreamSynchronize(s));
+  }
   uint32_t last_base = 0, last_units = 0;
   GB_CUDA(cudaMemcpyAsync(&last_base, bases.p + p->num_slices - 1, 4, cudaMemcpyDeviceToHost, s));
   GB_CUDA(cudaMemcpyAsync(&last_units, units.p + p->num_slices - 1, 4, cudaMemcpyDeviceToHost, s));
@@ -1050,7 +1044,7 @@ static gb_status cb_chunk_table(cudaStream_t s, int dev_sms, uint32_t B, const u
   // first group of every block's stream
   DevBuf<uint32_t> gbeg;
   GB_TRY(gbeg.alloc(KB + 1));
-  k_gather_u32<<<grid_for(KB + 1, 128), 128, 0, s>>>(goff, st->poff.p, KB + 1, gbeg.p);
+  k_gather<<<grid_for(KB + 1, 128), 128, 0, s>>>(goff, st->poff.p, KB + 1, gbeg.p);
   std::vector<uint32_t> h_gbeg(KB + 1);
   GB_CUDA(cudaMemcpyAsync(h_gbeg.data(), gbeg.p, (size_t)(KB + 1) * 4, cudaMemcpyDeviceToHost, s));
   GB_CUDA(cudaStreamSynchronize(s));
@@ -1103,27 +1097,6 @@ static gb_status cb_chunk_table(cudaStream_t s, int dev_sms, uint32_t B, const u
 }
 
 constexpr uint64_t VB_L2_FACTOR = 2;  // the virtual blocks run when the source vector exceeds this many L2s
-static uint32_t bits_for(uint64_t count) {  // bits of the largest index below count
-  uint32_t b = 1;
-  while ((1ull << b) < count) ++b;
-  return b;
-}
-template <typename K, typename V>
-static gb_status sort_pairs(cudaStream_t s, cub::DoubleBuffer<K>& k, cub::DoubleBuffer<V>& v, uint32_t count,
-                            uint32_t end_bit) {
-  DevBuf<uint8_t> tmp;
-  GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
-    return cub::DeviceRadixSort::SortPairs(t, tb, k, v, (int)count, 0, (int)end_bit, s);
-  }));
-  GB_CUDA(cudaStreamSynchronize(s));
-  return GB_OK;
-}
-static gb_status scan_inclusive(cudaStream_t s, uint32_t* data, uint32_t count) {
-  DevBuf<uint8_t> tmp;
-  GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) { return cub::DeviceScan::InclusiveSum(t, tb, data, data, (int)count, s); }));
-  GB_CUDA(cudaStreamSynchronize(s));
-  return GB_OK;
-}
 
 // Virtual blocks (PrVBlocks) in place of the SELL slices, when the source vector is well past L2: there a SELL
 // gather of a cold edge is mostly a 32-byte sector from HBM for a 4-byte value, while the two passes stream ids
@@ -1178,10 +1151,16 @@ gb_status LayoutBuild::layout_vblocks() {
   GB_TRY(goffv.alloc((size_t)n_loc + 1));
   GB_CUDA(cudaMemcpyAsync(coff.p, lens.p, (size_t)n_loc * 4, cudaMemcpyDeviceToDevice, s));
   GB_CUDA(cudaMemsetAsync(coff.p + n_loc, 0, 4, s));
-  GB_TRY(scan_exclusive(s, coff.p, (uint64_t)n_loc + 1));
-  k_vb_groups<<<grid_for(n_loc, 256), 256, 0, s>>>(lens.p, n_loc, goffv.p);
-  GB_CUDA(cudaMemsetAsync(goffv.p + n_loc, 0, 4, s));
-  GB_TRY(scan_exclusive(s, goffv.p, (uint64_t)n_loc + 1));
+  GB_REQUIRE((uint64_t)n_loc + 1 < (1ull << 31), "scan of %llu items is too long", (unsigned long long)n_loc + 1);
+  {
+    DevBuf<uint8_t> tmp;  // the two scans are of the same size
+    GB_TRY(exclusive_sum(s, tmp, coff.p, (int)(n_loc + 1)));
+    GB_CUDA(cudaStreamSynchronize(s));
+    k_vb_groups<<<grid_for(n_loc, 256), 256, 0, s>>>(lens.p, n_loc, goffv.p);
+    GB_CUDA(cudaMemsetAsync(goffv.p + n_loc, 0, 4, s));
+    GB_TRY(exclusive_sum(s, tmp, goffv.p, (int)(n_loc + 1)));
+    GB_CUDA(cudaStreamSynchronize(s));
+  }
   uint32_t ngv = 0;
   GB_CUDA(cudaMemcpyAsync(&ngv, goffv.p + n_loc, 4, cudaMemcpyDeviceToHost, s));
   GB_CUDA(cudaStreamSynchronize(s));
@@ -1203,10 +1182,18 @@ gb_status LayoutBuild::layout_vblocks() {
                                                     reinterpret_cast<const uint32_t*>(p->sell.p), keys.p, idx.p, erow.p);
     cub::DoubleBuffer<uint64_t> kb(keys.p, keys_alt.p);
     cub::DoubleBuffer<uint32_t> ib(idx.p, idx_alt.p);
-    GB_TRY(sort_pairs(s, kb, ib, Ec, 32 + bits_for(parts)));
+    {
+      DevBuf<uint8_t> tmp;
+      GB_TRY(sort_pairs(s, tmp, kb, ib, (int)Ec, (int)(32 + bits_for(parts))));
+      GB_CUDA(cudaStreamSynchronize(s));
+    }
     GB_TRY(rank.alloc(Ec));
     k_vb_starts<<<grid_for(Ec, 256), 256, 0, s>>>(kb.Current(), Ec, rank.p);
-    GB_TRY(scan_inclusive(s, rank.p, Ec));
+    {
+      DevBuf<uint8_t> tmp;
+      GB_TRY(inclusive_sum(s, tmp, rank.p, (int)Ec));
+      GB_CUDA(cudaStreamSynchronize(s));
+    }
     GB_CUDA(cudaMemcpyAsync(&NP, rank.p + Ec - 1, 4, cudaMemcpyDeviceToHost, s));
     GB_CUDA(cudaStreamSynchronize(s));
     GB_TRY(pfirst.alloc((size_t)parts + 1));
@@ -1226,7 +1213,11 @@ gb_status LayoutBuild::layout_vblocks() {
     {
       DevBuf<uint32_t> rfirst, roff;
       k_vb_run_flags<<<grid_for(Ec, 256), 256, 0, s>>>(kb.Current(), rank.p, Ec, B, gpos);
-      GB_TRY(scan_inclusive(s, gpos, NP));
+      {
+        DevBuf<uint8_t> tmp;
+        GB_TRY(inclusive_sum(s, tmp, gpos, (int)NP));
+        GB_CUDA(cudaStreamSynchronize(s));
+      }
       uint32_t NR = 0;
       GB_CUDA(cudaMemcpyAsync(&NR, gpos + NP - 1, 4, cudaMemcpyDeviceToHost, s));
       GB_CUDA(cudaStreamSynchronize(s));
@@ -1236,11 +1227,16 @@ gb_status LayoutBuild::layout_vblocks() {
         k_vb_run_first<<<grid_for(NP, 256), 256, 0, s>>>(gpos, NP, rfirst.p);
         k_vb_run_slots<<<grid_for(NR, 256), 256, 0, s>>>(rfirst.p, NR, NP, roff.p);
         GB_CUDA(cudaMemsetAsync(roff.p + NR, 0, 4, s));
-        GB_TRY(scan_exclusive(s, roff.p, (uint64_t)NR + 1));
+        GB_REQUIRE((uint64_t)NR + 1 < (1ull << 31), "scan of %llu items is too long", (unsigned long long)NR + 1);
+        {
+          DevBuf<uint8_t> tmp;
+          GB_TRY(exclusive_sum(s, tmp, roff.p, (int)(NR + 1)));
+          GB_CUDA(cudaStreamSynchronize(s));
+        }
         k_vb_run_pos<<<grid_for(NP, 256), 256, 0, s>>>(gpos, NP, rfirst.p, roff.p);
         GB_CUDA(cudaMemcpyAsync(gpos + NP, roff.p + NR, 4, cudaMemcpyDeviceToDevice, s));
         GB_TRY(gfirst.alloc((size_t)parts + 1));
-        k_gather_u32<<<grid_for(parts + 1, 128), 128, 0, s>>>(gpos, pfirst.p, parts + 1, gfirst.p);
+        k_gather<<<grid_for(parts + 1, 128), 128, 0, s>>>(gpos, pfirst.p, parts + 1, gfirst.p);
         GB_CUDA(cudaGetLastError());
         std::vector<uint32_t> h_gfirst(parts + 1);
         GB_CUDA(cudaMemcpyAsync(h_gfirst.data(), gfirst.p, (size_t)(parts + 1) * 4, cudaMemcpyDeviceToHost, s));
@@ -1273,11 +1269,19 @@ gb_status LayoutBuild::layout_vblocks() {
   const uint32_t nblk = (uint32_t)(((uint64_t)n + B - 1) / B);
   cub::DoubleBuffer<uint64_t> akb(akey.p, akey_alt.p);
   cub::DoubleBuffer<uint32_t> asb(aslot.p, aslot_alt.p);
-  GB_TRY(sort_pairs(s, akb, asb, NP, VB_BLK_SHIFT + bits_for(nblk)));
+  {
+    DevBuf<uint8_t> tmp;
+    GB_TRY(sort_pairs(s, tmp, akb, asb, (int)NP, (int)(VB_BLK_SHIFT + bits_for(nblk))));
+    GB_CUDA(cudaStreamSynchronize(s));
+  }
   DevBuf<uint32_t> run_rank, bfirst, brank, bpos;
   GB_TRY(run_rank.alloc(NP));
   k_run_starts<<<grid_for(NP, 256), 256, 0, s>>>(akb.Current(), NP, run_rank.p);
-  GB_TRY(scan_inclusive(s, run_rank.p, NP));
+  {
+    DevBuf<uint8_t> tmp;
+    GB_TRY(inclusive_sum(s, tmp, run_rank.p, (int)NP));
+    GB_CUDA(cudaStreamSynchronize(s));
+  }
   GB_CUDA(cudaMemcpyAsync(&v.n_runs, run_rank.p + NP - 1, 4, cudaMemcpyDeviceToHost, s));
   GB_TRY(bfirst.alloc((size_t)nblk + 1));
   k_vb_bounds<<<grid_for(nblk + 1, 128), 128, 0, s>>>(akb.Current(), nullptr, NP, VB_BLK_SHIFT, nblk, NP, bfirst.p);
