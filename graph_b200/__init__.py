@@ -147,7 +147,8 @@ class FileFormat:
     Graph500 = _Enum("FileFormat", "Graph500", 0)
     EdgeList = _Enum("FileFormat", "EdgeList", 1)
     Binary = _Enum("FileFormat", "Binary", 2)  # SerializeGraphOp's file (input/binary.rs); see serialize()
-    # node-labelled .graph file (input/dotgraph.rs); load() drops the labels, load_labeled() keeps them
+    # node-labelled .graph file (input/dotgraph.rs); load() drops the labels, load_labeled() keeps them.
+    # load_labeled(file_format=Binary) reads the labelled binary file that serialize_labeled() writes.
     DotGraph = _Enum("FileFormat", "DotGraph", 3)
 
 
@@ -382,6 +383,39 @@ def _decode_binary(data: bytes, directed: bool, with_values: bool = False):
     return (*csrs[0], w, *csrs[1]) if directed else csrs[0]
 
 
+def _decode_binary_labeled(data: bytes, directed: bool, label_bytes: int = 4, with_values: bool = False):
+    """The host decoder of labelled binary graph files (gb_binary_decode_labeled): the labels, then what
+    _decode_binary returns.  label_bytes is NV's width (4: u32, 8: u64 / usize), which the file does not state."""
+    raw = np.frombuffer(data, np.uint8)
+    kind = _capi.KIND_DIRECTED if directed else _capi.KIND_UNDIRECTED
+    n, m, hv = C.c_uint32(0), C.c_uint64(0), C.c_int(0)
+    args = (_ptr(raw) if raw.size else None, raw.size, kind, label_bytes, C.byref(n), C.byref(m), C.byref(hv))
+    check(lib.gb_binary_decode_labeled(*args, None, None, None, None, None, None))
+    if with_values and not hv.value:
+        raise ValueError("the binary graph file holds no edge values")
+    labels = np.empty(n.value, np.uint32)
+    csrs = [(np.empty(n.value + 1, np.uint32), np.empty(m.value, np.uint32)) for _ in range(2 if directed else 1)]
+    w = np.empty(m.value, np.float32) if with_values else None
+    inc = csrs[1] if directed else (None, None)
+    check(lib.gb_binary_decode_labeled(*args, _ptr(labels), _ptr(csrs[0][0]), _ptr(csrs[0][1]), _ptr(w),
+                                       _ptr(inc[0]), _ptr(inc[1])))
+    return (labels, *csrs[0], w, *csrs[1]) if directed else (labels, *csrs[0])
+
+
+def _load_labeled(cls, dot_fn, binary_fn, path, layout, file_format, label_bytes):
+    """load_labeled: a DotGraph file through dot_fn, or a binary file with NodeValues of label_bytes each through
+    binary_fn."""
+    if file_format is FileFormat.Binary:
+        p, _, lay = _load_args(path, file_format, layout)
+        return _construct(cls, binary_fn, _device, p, lay, int(label_bytes))
+    if file_format is not FileFormat.DotGraph:
+        raise ValueError(f"labelled graphs load from DotGraph or Binary files, not {file_format!r}")
+    if label_bytes != 4:
+        raise ValueError("label_bytes is the width of a binary file's node values; a DotGraph file's labels are u32")
+    p, _, lay = _load_args(path, FileFormat.DotGraph, layout)
+    return _construct(cls, dot_fn, _device, p, lay)
+
+
 def _check_host_csr(off: np.ndarray, tgt: np.ndarray, what: str) -> None:
     """The C side reads off[n] and copies off[n] targets: reject arrays that are too short here."""
     if off.ndim != 1 or len(off) < 2:
@@ -569,6 +603,13 @@ class _Handle:
         under a temporary name and renamed over it."""
         check(lib.gb_graph_serialize(self._g, os.fsencode(os.fspath(path))))
 
+    def serialize_labeled(self, path) -> None:
+        """SerializeGraphOp::serialize of a labelled graph (DirectedCsrGraph<u32, u32> / UndirectedCsrGraph<u32,
+        u32>): NodeValues<u32>, then the CSRs as serialize() writes them, without edge values.  The file loads
+        with `load_labeled(path, file_format=FileFormat.Binary)`.  After make_degree_ordered() the labels are
+        written as stored, which are not permuted.  A graph without labels raises ValueError."""
+        check(lib.gb_graph_serialize_labeled(self._g, os.fsencode(os.fspath(path))))
+
     def __repr__(self):
         return (f"{type(self).__name__} {{ node_count: {self.node_count()}, edge_count: {self.edge_count()}, "
                 f"load_took: {_took(self.load_micros)} }}")
@@ -607,11 +648,13 @@ class DiGraph(_Handle):
         return _construct(DiGraph, lib.gb_digraph_load_u32, _device, *_load_args(path, file_format, layout), 0)
 
     @staticmethod
-    def load_labeled(path, layout=None) -> "DiGraph":
+    def load_labeled(path, layout=None, file_format=FileFormat.DotGraph, label_bytes: int = 4) -> "DiGraph":
         """A DotGraph (.graph) file as DirectedCsrGraph<u32, u32>: node_count = N, one label per node
-        (input/dotgraph.rs; GraphBuilder::file_format(DotGraphInput)).  Parsed on the device when large."""
-        p, _, lay = _load_args(path, FileFormat.DotGraph, layout)
-        return _construct(DiGraph, lib.gb_digraph_load_labeled_u32, _device, p, lay)
+        (input/dotgraph.rs; GraphBuilder::file_format(DotGraphInput)).  Parsed on the device when large.
+        FileFormat.Binary: the file serialize_labeled() writes, or a DirectedCsrGraph<NI, NV> file of the reference
+        with NV of label_bytes (4: u32, 8: u64 / usize, narrowed); its rows are kept as stored."""
+        return _load_labeled(DiGraph, lib.gb_digraph_load_labeled_u32, lib.gb_digraph_load_labeled_binary_u32, path,
+                             layout, file_format, label_bytes)
 
     @staticmethod
     def load_weighted(path, layout=None, file_format=FileFormat.EdgeList) -> "DiGraph":
@@ -808,10 +851,11 @@ class Graph(_Handle):
         return _construct(Graph, lib.gb_graph_load_u32, _device, *_load_args(path, file_format, layout))
 
     @staticmethod
-    def load_labeled(path, layout=None) -> "Graph":
-        """A DotGraph (.graph) file as UndirectedCsrGraph<u32, u32>: node_count = N, one label per node."""
-        p, _, lay = _load_args(path, FileFormat.DotGraph, layout)
-        return _construct(Graph, lib.gb_graph_load_labeled_u32, _device, p, lay)
+    def load_labeled(path, layout=None, file_format=FileFormat.DotGraph, label_bytes: int = 4) -> "Graph":
+        """A DotGraph (.graph) file as UndirectedCsrGraph<u32, u32>: node_count = N, one label per node.
+        FileFormat.Binary: a labelled binary file, as DiGraph.load_labeled reads one."""
+        return _load_labeled(Graph, lib.gb_graph_load_labeled_u32, lib.gb_graph_load_labeled_binary_u32, path, layout,
+                             file_format, label_bytes)
 
     @staticmethod
     def load_weighted(path, layout=None, file_format=FileFormat.EdgeList) -> "Graph":

@@ -149,6 +149,11 @@ SIGNATURES = {
                                                     C.POINTER(_P)]),
     "gb_graph_from_edges_labeled_u32": (C.c_int, [C.c_int, _P, _P, C.c_uint64, _P, C.c_uint32, C.c_int,
                                                   C.POINTER(_P)]),
+    "gb_digraph_load_labeled_binary_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.c_uint32, C.POINTER(_P)]),
+    "gb_graph_load_labeled_binary_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.c_uint32, C.POINTER(_P)]),
+    "gb_graph_serialize_labeled": (C.c_int, [_P, C.c_char_p]),
+    "gb_binary_decode_labeled": (C.c_int, [_P, C.c_uint64, C.c_int, C.c_uint32, C.POINTER(C.c_uint32),
+                                           C.POINTER(C.c_uint64), C.POINTER(C.c_int), _P, _P, _P, _P, _P, _P]),
     "gb_graph_node_values": (C.c_int, [_P, _P]),
     "gb_label_stats": (C.c_int, [_P, C.POINTER(LabelStatsInfo), _P, _P]),
     "gb_node_label_index": (C.c_int, [_P, C.POINTER(C.c_uint32), _P, _P]),

@@ -4,7 +4,11 @@
 // SerializeGraphOp / DeserializeGraphOp (crates/builder/src/graph_ops.rs:232-238) write, little-endian, with
 // usize = 8 bytes:
 //
-//   NodeValues (csr.rs:334-341; NV = (), so no payload)   [usize n]
+//   NodeValues (csr.rs:334-341)                         [usize n][NV x n]
+//                                                       NV = (): no payload; a labelled graph's NV = u32 (4 B) or
+//                                                       u64 / usize (8 B).  The file does not say which: the
+//                                                       caller gives NV's width, and the first CSR header starts
+//                                                       at 8 + n * width.
 //   per CSR (directed: csr_out, csr_inc; undirected: csr), Csr::serialize csr.rs:252-266:
 //     [usize L][L bytes: type name of NI, "u32" | "u64" | "usize"]
 //     [NI node_count][NI entries]                       entries = targets.len() (undirected: 2m)
@@ -37,7 +41,8 @@ struct BinCsr {
 
 struct BinLayout {
   gb_graph_kind kind = GB_KIND_DIRECTED;
-  uint32_t id_bytes = 4;   // 4: "u32", 8: "u64" / "usize"
+  uint32_t label_bytes = 0;  // NodeValues width: 0 (NV = ()), 4 or 8; the labels start at byte BIN_USIZE
+  uint32_t id_bytes = 4;     // 4: "u32", 8: "u64" / "usize"
   uint32_t rec_bytes = 4;  // id_bytes without values; 8 (u32,f32) or 16 (u64,f32: 4 padding bytes) with
   bool values = false;
   uint32_t n = 0;
@@ -61,10 +66,13 @@ inline BinCsr bin_csr_at(uint64_t header, uint64_t name_len, uint32_t id_bytes, 
   return c;
 }
 
-// the file this library writes: NI = u32, records with values when `values`
-inline BinLayout bin_layout_u32(gb_graph_kind kind, uint32_t n, uint64_t entries, bool values) {
+// the file this library writes: NI = u32, records with values when `values`, and n labels of label_bytes each
+// in front of the CSRs when label_bytes is not 0
+inline BinLayout bin_layout_u32(gb_graph_kind kind, uint32_t n, uint64_t entries, bool values,
+                                uint32_t label_bytes = 0) {
   BinLayout l;
   l.kind = kind;
+  l.label_bytes = label_bytes;
   l.id_bytes = 4;
   l.rec_bytes = values ? bin_value_rec_bytes(4) : 4;
   l.values = values;
@@ -72,7 +80,7 @@ inline BinLayout bin_layout_u32(gb_graph_kind kind, uint32_t n, uint64_t entries
   l.entries = entries;
   l.ncsr = kind == GB_KIND_DIRECTED ? 2 : 1;
   l.name = "u32";
-  uint64_t pos = BIN_USIZE;
+  uint64_t pos = BIN_USIZE + (uint64_t)n * label_bytes;
   for (unsigned c = 0; c < l.ncsr; ++c) {
     l.csr[c] = bin_csr_at(pos, 3, 4, n, entries, l.rec_bytes);
     pos = l.csr[c].end;
@@ -81,11 +89,12 @@ inline BinLayout bin_layout_u32(gb_graph_kind kind, uint32_t n, uint64_t entries
   return l;
 }
 
-// the header bytes in front of CSR c's offsets (with the NodeValues count in front of the first)
+// the header bytes in front of CSR c's offsets (with the NodeValues count in front of the first when there is
+// no payload between them; a labelled file's count and labels are written apart)
 inline std::string bin_header_bytes(const BinLayout& l, unsigned c) {
   std::string h;
   auto put = [&](uint64_t v, unsigned bytes) { h.append(reinterpret_cast<const char*>(&v), bytes); };
-  if (c == 0) put(l.n, BIN_USIZE);
+  if (c == 0 && l.label_bytes == 0) put(l.n, BIN_USIZE);
   put(l.name.size(), BIN_USIZE);
   h += l.name;
   put(l.n, l.id_bytes);
@@ -139,6 +148,19 @@ BinHeader bin_read_header(Read& read, uint64_t size, uint64_t pos) {
 
 inline gb_status bin_eof() { return fail(GB_ERR_INVALID, "binary graph file: unexpected end of file"); }
 
+// NV's width, which a labelled file does not state
+inline gb_status bin_check_label_bytes(uint32_t label_bytes) {
+  GB_REQUIRE(label_bytes == 4 || label_bytes == 8,
+             "label_bytes must be 4 (NV = u32) or 8 (NV = u64 / usize), not %u", label_bytes);
+  return GB_OK;
+}
+
+// an 8-byte label of 2^32 or more; `node` is the smallest such node
+inline gb_status bin_label_wide(uint64_t node) {
+  return fail(GB_ERR_INVALID, "binary graph file: the node value of node %llu does not fit 32 bits",
+              (unsigned long long)node);
+}
+
 inline gb_status bin_header_error(const BinHeader& h) {
   if (h.err == 1) return bin_eof();
   std::string shown;  // Error::InvalidIdType, lib.rs:297-298
@@ -150,12 +172,17 @@ inline gb_status bin_header_error(const BinHeader& h) {
 // Walks the headers of a file of `size` bytes that should hold a graph of kind `want`, and fills the section
 // table.  Checks everything the headers decide: type names, the NodeValues count (lib.rs:295), node_count > 0,
 // counts that fit 32 bits, equal csr_out / csr_inc counts, the graph kind, and that the sections end exactly
-// at the end of the file.  The offsets and targets themselves are checked by the callers.
+// at the end of the file.  The offsets and targets themselves, and the labels, are checked by the callers.
+// label_bytes is NV's width (0: NV = (), no payload; 4 or 8, checked by the caller).  The NodeValues count is
+// outside input: it places the first CSR header only once the file is known to hold the n labels in front of
+// it, so an absurd count ends the file instead of sizing anything.
 template <typename Read>
-gb_status bin_parse(Read read, uint64_t size, gb_graph_kind want, BinLayout* l) {
+gb_status bin_parse(Read read, uint64_t size, gb_graph_kind want, BinLayout* l, uint32_t label_bytes = 0) {
   uint64_t nv = 0;
   if (!bin_get(read, size, 0, BIN_USIZE, &nv)) return bin_eof();
-  const BinHeader h = bin_read_header(read, size, BIN_USIZE);
+  if (label_bytes && nv > (size - BIN_USIZE) / label_bytes) return bin_eof();
+  const uint64_t base = BIN_USIZE + nv * label_bytes;  // the first CSR header
+  const BinHeader h = bin_read_header(read, size, base);
   if (h.err) return bin_header_error(h);
   const uint32_t w = h.id_bytes;
   GB_REQUIRE(h.n <= 0xFFFFFFFFull, "binary graph file: node_count %llu does not fit 32 bits",
@@ -166,10 +193,11 @@ gb_status bin_parse(Read read, uint64_t size, gb_graph_kind want, BinLayout* l) 
              (unsigned long long)h.entries);
   const uint32_t cand[2] = {w, bin_value_rec_bytes(w)};
   BinCsr first[2];
-  for (int i = 0; i < 2; ++i) first[i] = bin_csr_at(BIN_USIZE, h.name_len, w, h.n, h.entries, cand[i]);
+  for (int i = 0; i < 2; ++i) first[i] = bin_csr_at(base, h.name_len, w, h.n, h.entries, cand[i]);
   if (first[0].rec_pos > size) return bin_eof();  // inside the header or the offsets
 
   l->kind = want;
+  l->label_bytes = label_bytes;
   l->id_bytes = w;
   l->n = (uint32_t)h.n;
   l->entries = h.entries;

@@ -189,28 +189,41 @@ gb_status gb_edge_list_parse(const char* text, uint64_t len, uint32_t* src, uint
   return GB_OK;
 }
 
-// Binary graph files (binary_format.h): the section table from the headers, then the offsets and targets
-// checked and narrowed to u32 on the host.  In-CSR values are never returned (device graphs hold none).
-gb_status gb_binary_decode(const void* bytes, uint64_t len, gb_graph_kind kind, uint32_t* node_count,
-                           uint64_t* entries, int* has_values, uint32_t* out_offsets, uint32_t* out_targets,
-                           float* out_values, uint32_t* in_offsets, uint32_t* in_targets) {
+}  // extern "C"
+
+namespace gb {
+
+// Binary graph files (binary_format.h): the section table from the headers, then the labels (label_bytes != 0),
+// the offsets and targets checked and narrowed to u32 on the host.  In-CSR values are never returned (device graphs
+// hold none).
+static gb_status binary_decode(const void* bytes, uint64_t len, gb_graph_kind kind, uint32_t label_bytes,
+                               uint32_t* node_count, uint64_t* entries, int* has_values, uint32_t* labels,
+                               uint32_t* out_offsets, uint32_t* out_targets, float* out_values, uint32_t* in_offsets,
+                               uint32_t* in_targets) {
   GB_REQUIRE(node_count && entries && has_values, "NULL argument");
   GB_REQUIRE(kind == GB_KIND_DIRECTED || kind == GB_KIND_UNDIRECTED, "unknown graph kind %d", (int)kind);
   GB_REQUIRE(bytes || len == 0, "NULL bytes");
   const uint8_t* base = static_cast<const uint8_t*>(bytes);
-  gb::BinLayout l;
-  GB_TRY(gb::bin_parse([&](uint64_t pos, void* dst, uint64_t n) { return std::memcpy(dst, base + pos, n), true; },
-                       len, kind, &l));
+  BinLayout l;
+  GB_TRY(bin_parse([&](uint64_t pos, void* dst, uint64_t n) { return std::memcpy(dst, base + pos, n), true; }, len,
+                   kind, &l, label_bytes));
   *node_count = l.n;
   *entries = l.entries;
   *has_values = l.values ? 1 : 0;
   if (!out_offsets) return GB_OK;
+  GB_REQUIRE(labels || label_bytes == 0, "labels is NULL");
   GB_REQUIRE(out_targets || l.entries == 0, "out_targets is NULL");
   GB_REQUIRE(!out_values || l.values, "the file holds no edge values");
   GB_REQUIRE(kind == GB_KIND_UNDIRECTED || (in_offsets && (in_targets || l.entries == 0)), "in-CSR arrays are NULL");
   const uint64_t n = l.n, m = l.entries, w = l.id_bytes, rec = l.rec_bytes;
+  for (uint64_t v = 0; v < n && label_bytes; ++v) {  // the labels first: they come first in the file
+    uint64_t x = 0;
+    std::memcpy(&x, base + BIN_USIZE + v * label_bytes, label_bytes);
+    if (x > 0xFFFFFFFFull) return bin_label_wide(v);
+    labels[v] = (uint32_t)x;
+  }
   for (unsigned c = 0; c < l.ncsr; ++c) {
-    const char* what = gb::bin_csr_name(l, c);
+    const char* what = bin_csr_name(l, c);
     uint32_t* off = c == 0 ? out_offsets : in_offsets;
     uint32_t* tgt = c == 0 ? out_targets : in_targets;
     float* val = c == 0 ? out_values : nullptr;
@@ -226,28 +239,53 @@ gb_status gb_binary_decode(const void* bytes, uint64_t len, gb_graph_kind kind, 
       off[v] = id_at(l.csr[c].off_pos + v * w);
       if (v && off[v] < off[v - 1]) ++decreasing;
     }
-    const unsigned T = gb::io_threads(m);
+    const unsigned T = io_threads(m);
     std::vector<uint64_t> big_t(T, 0);
     std::vector<int> wide_t(T, 0);
-    gb::parallel_chunks(T, [&](unsigned t) {
+    parallel_chunks(T, [&](unsigned t) {
+      uint64_t nbig = 0;  // counted in registers: big_t[t] and wide_t[t] of the threads share cache lines
+      bool nwide = false;
       for (uint64_t i = m * t / T, e = m * (t + 1) / T; i < e; ++i) {
         const uint8_t* r = base + l.csr[c].rec_pos + i * rec;
         uint64_t v = 0;
         std::memcpy(&v, r, w);
-        wide_t[t] |= v > 0xFFFFFFFFull;
-        big_t[t] += v >= n;
+        nwide |= v > 0xFFFFFFFFull;
+        nbig += v >= n;
         tgt[i] = (uint32_t)v;
         if (val) std::memcpy(val + i, r + w, 4);
       }
+      big_t[t] = nbig;
+      wide_t[t] = nwide;
     });
     for (unsigned t = 0; t < T; ++t) big += big_t[t], wide |= wide_t[t] != 0;
     GB_REQUIRE(!wide, "binary graph file: %s holds an id or offset that does not fit 32 bits", what);
     GB_REQUIRE(off[0] == 0, "%s offsets[0] must be 0", what);
-    GB_TRY(gb::require_monotone(what, decreasing));
+    GB_TRY(require_monotone(what, decreasing));
     GB_REQUIRE(off[n] == m, "%s offsets end at %u, not at its %llu entries", what, off[n], (unsigned long long)m);
-    GB_TRY(gb::require_ids(what, big, l.n));
+    GB_TRY(require_ids(what, big, l.n));
   }
   return GB_OK;
+}
+
+}  // namespace gb
+
+extern "C" {
+
+gb_status gb_binary_decode(const void* bytes, uint64_t len, gb_graph_kind kind, uint32_t* node_count,
+                           uint64_t* entries, int* has_values, uint32_t* out_offsets, uint32_t* out_targets,
+                           float* out_values, uint32_t* in_offsets, uint32_t* in_targets) {
+  return gb::binary_decode(bytes, len, kind, 0, node_count, entries, has_values, nullptr, out_offsets, out_targets,
+                           out_values, in_offsets, in_targets);
+}
+
+// the NodeValues payload of label_bytes (4 or 8) per node in front of the CSRs; 8-byte labels are narrowed
+gb_status gb_binary_decode_labeled(const void* bytes, uint64_t len, gb_graph_kind kind, uint32_t label_bytes,
+                                   uint32_t* node_count, uint64_t* entries, int* has_values, uint32_t* labels,
+                                   uint32_t* out_offsets, uint32_t* out_targets, float* out_values,
+                                   uint32_t* in_offsets, uint32_t* in_targets) {
+  GB_TRY(gb::bin_check_label_bytes(label_bytes));
+  return gb::binary_decode(bytes, len, kind, label_bytes, node_count, entries, has_values, labels, out_offsets,
+                           out_targets, out_values, in_offsets, in_targets);
 }
 
 }  // extern "C"

@@ -30,7 +30,9 @@
 //   Binary: the host preads the headers (bin_parse gives the section table) and every chunk is cut against the
 //   table.  u32 sections without values go from the pinned buffer straight into their CSR array; a chunk that
 //   meets another section is staged with the bytes of the element it cuts carried in front, and k_bin_split
-//   narrows the ids and splits the records.
+//   narrows the ids and splits the records.  A labelled file's NodeValues are one more section: 4-byte labels go
+//   straight into the label array, 8-byte ones are narrowed by k_bin_split, which keeps the smallest node whose
+//   label does not fit 32 bits.
 //   Writer: the file is pieces of host and device memory; chunk k + 1 is copied from the device into the ring
 //   while chunk k is written with pwrite to a temporary file, which is then renamed over the destination.
 #include <fcntl.h>
@@ -222,20 +224,31 @@ __device__ __forceinline__ uint32_t load_u32_at(const uint8_t* base, uint64_t po
 
 // Binary files: elements [first, first + count) of a section staged in buf, whose byte 0 is file byte buf_off.
 // Element e starts at file byte sec + e * stride with an id of id_bytes (u64 ids are narrowed; a high word
-// that is not 0 sets *wide), followed by an f32 value that goes to w[e] when w is not NULL.
+// that is not 0 sets *wide), followed by an f32 value that goes to w[e] when w is not NULL.  With first_wide
+// (the labels, whose elements number below 2^32) the smallest such e goes to *first_wide instead of the flag.
 __global__ void k_bin_split(const uint8_t* __restrict__ buf, uint64_t buf_off, uint64_t sec, uint32_t stride,
                             uint32_t id_bytes, uint64_t first, uint64_t count, uint32_t* __restrict__ ids,
-                            float* __restrict__ w, unsigned int* __restrict__ wide) {
+                            float* __restrict__ w, unsigned int* __restrict__ wide,
+                            unsigned int* __restrict__ first_wide) {
   bool big = false;
+  unsigned int lo = 0xFFFFFFFFu;  // the first e of this thread with a high word (its e ascend)
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
        i += (uint64_t)gridDim.x * blockDim.x) {
     const uint64_t e = first + i;
     const uint64_t pos = sec + e * stride - buf_off;
     ids[e] = load_u32_at(buf, pos);
-    if (id_bytes == 8) big |= load_u32_at(buf, pos + 4) != 0;
+    if (id_bytes == 8 && load_u32_at(buf, pos + 4) != 0) {
+      if (!big) lo = (unsigned int)e;
+      big = true;
+    }
     if (w) w[e] = __uint_as_float(load_u32_at(buf, pos + id_bytes));
   }
-  if (__any_sync(0xFFFFFFFFu, big) && (threadIdx.x & 31) == 0) atomicOr(wide, 1u);
+  if (first_wide) {
+    lo = __reduce_min_sync(0xFFFFFFFFu, lo);
+    if (lo != 0xFFFFFFFFu && (threadIdx.x & 31) == 0) atomicMin(first_wide, lo);
+  } else if (__any_sync(0xFFFFFFFFu, big) && (threadIdx.x & 31) == 0) {
+    atomicOr(wide, 1u);
+  }
 }
 
 // Target<u32, f32> records (8 bytes, #[repr(C)]) from the SoA arrays, for the writer
@@ -730,14 +743,15 @@ static gb_status load_file(int device, const InputFile& f, gb_file_format format
   return GB_OK;
 }
 
-// The CSR arrays a binary file's section fills.  Elements of `stride` bytes start at file byte `pos`; a u32
-// section without values (stride 4) is DMA'd straight into `ids`, the others are staged and split by
-// k_bin_split.
+// The CSR (or label) arrays a binary file's section fills.  Elements of `stride` bytes start at file byte `pos`
+// with an id (or label) of `width` bytes; a u32 section without values (stride 4) is DMA'd straight into `ids`,
+// the others are staged and split by k_bin_split.  first_wide: see k_bin_split (NULL: the `wide` flag).
 struct BinSection {
   uint64_t pos = 0, count = 0;
-  uint32_t stride = 0;
+  uint32_t stride = 0, width = 0;
   uint32_t* ids = nullptr;
   float* w = nullptr;
+  unsigned int* first_wide = nullptr;
   bool direct() const { return stride == 4; }
   uint64_t end() const { return pos + count * stride; }
 };
@@ -776,13 +790,14 @@ static gb_status check_loaded_csrs(gb_graph* g, const BinLayout& l, DevCsr* cons
   return GB_OK;
 }
 
-// Binary graph files streamed into the CSR arrays.  A staged chunk carries at most 15 bytes of a cut element
-// in front, and k_bin_split decodes the elements that end inside the chunk.
+// Binary graph files streamed into the CSR arrays (and the label array, for label_bytes != 0).  A staged chunk
+// carries at most 15 bytes of a cut element in front, and k_bin_split decodes the elements that end inside the
+// chunk.
 static gb_status load_binary_streamed(int device, gb_graph_kind kind, const InputFile& f, bool want_value,
-                                      gb_graph** graph, gb_load_info* info) {
+                                      uint32_t label_bytes, gb_graph** graph, gb_load_info* info) {
   BinLayout l;
   GB_TRY(bin_parse([&](uint64_t pos, void* dst, uint64_t n) { return pread_all(f.fd, static_cast<char*>(dst), n, pos); },
-                   f.bytes, kind, &l));
+                   f.bytes, kind, &l, label_bytes));
   GB_REQUIRE(!want_value || l.values, "the binary graph file holds no edge values");
   GraphPtr g;
   GB_TRY(new_graph(device, kind, l.n, &g));
@@ -793,6 +808,16 @@ static gb_status load_binary_streamed(int device, gb_graph_kind kind, const Inpu
   DevBufStreamScope scope(sp.work);
   DevCsr* csr[2] = {&g->out, &g->in};
   std::vector<BinSection> secs;
+  DevBuf<unsigned int> label_wide;  // the smallest node whose 8-byte label does not fit 32 bits, or ~0
+  if (label_bytes) {
+    GB_TRY(g->labels.alloc(l.n));
+    GB_TRY(label_wide.alloc(1));
+    GB_CUDA(cudaMemsetAsync(label_wide.p, 0xFF, 4, sp.work));
+    BinSection s;
+    s.pos = BIN_USIZE, s.count = l.n, s.stride = s.width = label_bytes, s.ids = g->labels.p;
+    s.first_wide = label_wide.p;
+    secs.push_back(s);
+  }
   for (unsigned c = 0; c < l.ncsr; ++c) {
     DevCsr& d = *csr[c];
     d.len = l.entries;
@@ -801,8 +826,9 @@ static gb_status load_binary_streamed(int device, gb_graph_kind kind, const Inpu
     GB_CUDA(cudaMemsetAsync(d.tgt.p + l.entries, 0, 8 * 4, sp.work));
     if (c == 0 && want_value) GB_TRY(d.w.alloc(l.entries, 8));  // the out-CSR or the undirected CSR; no in-CSR values
     BinSection o, t;
-    o.pos = l.csr[c].off_pos, o.count = (uint64_t)l.n + 1, o.stride = l.id_bytes, o.ids = d.off.p;
-    t.pos = l.csr[c].rec_pos, t.count = l.entries, t.stride = l.rec_bytes, t.ids = d.tgt.p, t.w = d.w.p;
+    o.pos = l.csr[c].off_pos, o.count = (uint64_t)l.n + 1, o.stride = o.width = l.id_bytes, o.ids = d.off.p;
+    t.pos = l.csr[c].rec_pos, t.count = l.entries, t.stride = l.rec_bytes, t.width = l.id_bytes, t.ids = d.tgt.p;
+    t.w = d.w.p;
     secs.push_back(o);
     if (t.count) secs.push_back(t);
   }
@@ -856,8 +882,8 @@ static gb_status load_binary_streamed(int device, gb_graph_kind kind, const Inpu
       const uint64_t last = std::min(s.count, (b - s.pos) / s.stride);  // elements that end by b
       if (last <= first) continue;
       k_bin_split<<<grid_for(last - first, 256), 256, 0, sp.work>>>(st.dbuf[r].p, staged_off[r], s.pos, s.stride,
-                                                                      l.id_bytes, first, last - first, s.ids, s.w,
-                                                                      wide.p);
+                                                                      s.width, first, last - first, s.ids, s.w,
+                                                                      wide.p, s.first_wide);
       GB_CUDA(cudaGetLastError());
     }
     GB_CUDA(cudaEventRecord(st.parsed[r], sp.work));
@@ -869,6 +895,12 @@ static gb_status load_binary_streamed(int device, gb_graph_kind kind, const Inpu
     GB_TRY(split(k));
   }
   GB_CUDA(cudaStreamSynchronize(sp.copy));
+  if (label_bytes == 8) {  // the labels first, as gb_binary_decode_labeled checks them
+    unsigned int first = 0;
+    GB_CUDA(cudaMemcpyAsync(&first, label_wide.p, 4, cudaMemcpyDeviceToHost, sp.work));
+    GB_CUDA(cudaStreamSynchronize(sp.work));
+    if (first != 0xFFFFFFFFu) return bin_label_wide(first);
+  }
   GB_TRY(check_loaded_csrs(g.get(), l, csr, wide.p, sp.work));
   info->edges = kind == GB_KIND_DIRECTED ? l.entries : l.entries / 2;
   info->h2d_bytes = st.h2d;
@@ -989,32 +1021,42 @@ static gb_status load_dotgraph_streamed(int device, gb_graph_kind kind, const In
   return GB_OK;
 }
 
-// a small binary file: gb_binary_decode, then the upload of gb_[di]graph_from_csr_u32
+// a small binary file: gb_binary_decode (gb_binary_decode_labeled, for label_bytes != 0), then the upload of
+// gb_[di]graph_from_csr_u32 and of the labels
 static gb_status load_binary_on_host(int device, gb_graph_kind kind, const InputFile& f, bool want_value,
-                                     gb_graph** graph, gb_load_info* info) {
+                                     uint32_t label_bytes, gb_graph** graph, gb_load_info* info) {
   std::unique_ptr<char[]> bytes;
   GB_TRY(f.read_all(&bytes));
   const uint64_t len = f.bytes;
   uint32_t n = 0;
   uint64_t m = 0;
   int has_values = 0;
-  GB_TRY(gb_binary_decode(bytes.get(), len, kind, &n, &m, &has_values, nullptr, nullptr, nullptr, nullptr, nullptr));
+  if (label_bytes)
+    GB_TRY(gb_binary_decode_labeled(bytes.get(), len, kind, label_bytes, &n, &m, &has_values, nullptr, nullptr,
+                                    nullptr, nullptr, nullptr, nullptr));
+  else
+    GB_TRY(gb_binary_decode(bytes.get(), len, kind, &n, &m, &has_values, nullptr, nullptr, nullptr, nullptr, nullptr));
   GB_REQUIRE(!want_value || has_values, "the binary graph file holds no edge values");
   const unsigned ncsr = kind == GB_KIND_DIRECTED ? 2 : 1;
-  std::vector<uint32_t> off[2], tgt[2];
+  std::vector<uint32_t> off[2], tgt[2], labels(label_bytes ? n : 0);
   std::vector<float> w(want_value ? m : 0);
   for (unsigned c = 0; c < ncsr; ++c) off[c].resize((size_t)n + 1), tgt[c].resize(m);
-  GB_TRY(gb_binary_decode(bytes.get(), len, kind, &n, &m, &has_values, off[0].data(), tgt[0].data(),
-                          want_value ? w.data() : nullptr, off[1].data(), tgt[1].data()));
+  if (label_bytes)
+    GB_TRY(gb_binary_decode_labeled(bytes.get(), len, kind, label_bytes, &n, &m, &has_values, labels.data(),
+                                    off[0].data(), tgt[0].data(), nullptr, off[1].data(), tgt[1].data()));
+  else
+    GB_TRY(gb_binary_decode(bytes.get(), len, kind, &n, &m, &has_values, off[0].data(), tgt[0].data(),
+                            want_value ? w.data() : nullptr, off[1].data(), tgt[1].data()));
   GraphPtr g;
   GB_TRY(new_graph(device, kind, n, &g));
   GB_TRY(upload_host_csr(g->stream, n, off[0].data(), tgt[0].data(), want_value ? w.data() : nullptr, &g->out,
                          kind == GB_KIND_DIRECTED ? "csr_out" : "csr"));
   if (kind == GB_KIND_DIRECTED)
     GB_TRY(upload_host_csr(g->stream, n, off[1].data(), tgt[1].data(), nullptr, &g->in, "csr_inc"));
+  if (label_bytes) GB_TRY(attach_labels(g.get(), labels.data(), cudaMemcpyHostToDevice));
   *graph = g.release();
   info->edges = kind == GB_KIND_DIRECTED ? m : m / 2;
-  info->h2d_bytes = ncsr * (((uint64_t)n + 1) * 4 + m * 4) + (want_value ? m * 4 : 0);
+  info->h2d_bytes = ncsr * (((uint64_t)n + 1) * 4 + m * 4) + (want_value ? m * 4 : 0) + (label_bytes ? 4ull * n : 0);
   return GB_OK;
 }
 
@@ -1042,16 +1084,19 @@ struct TempFile {
 };
 
 // SerializeGraphOp::serialize (headers from host memory, arrays from device memory; Target<u32, f32> records are
-// interleaved on the device first: a weighted digraph's out- and in-CSR, a weighted undirected twin's one CSR)
-static gb_status serialize_graph(const gb_graph* g, const char* path) {
+// interleaved on the device first: a weighted digraph's out- and in-CSR, a weighted undirected twin's one CSR).
+// `labeled`: NodeValues<u32> in front of the CSRs, the count from host memory and the labels from device memory.
+static gb_status serialize_graph(const gb_graph* g, const char* path, bool labeled) {
   GB_REQUIRE(g && path, "NULL argument");
-  if (g->labels.p)
+  if (g->labels.p && !labeled)
     return fail(GB_ERR_UNSUPPORTED, "a labelled graph cannot be serialized: NodeValues payloads are not written");
   GB_REQUIRE(g->out.tgt.p != nullptr, "this handle holds no out targets (page-rank-only twin) and cannot be serialized");
+  if (labeled && !g->labels.p)
+    return fail(GB_ERR_UNSUPPORTED, "the graph has no node values to write (it was built without labels)");
   DeviceGuard guard(g->device);
   std::lock_guard<std::mutex> lock(g->mu);
-  const bool values = g->out.w.p != nullptr;
-  const BinLayout l = bin_layout_u32(g->kind, g->n, g->out.len, values);
+  const bool values = !labeled && g->out.w.p != nullptr;  // a labelled twin's records carry no values
+  const BinLayout l = bin_layout_u32(g->kind, g->n, g->out.len, values, labeled ? 4 : 0);
   const DevCsr* csr[2] = {&g->out, &g->in};
   DevBuf<float> in_w;
   if (values && g->kind == GB_KIND_DIRECTED) GB_TRY(in_csr_values(g, &in_w));
@@ -1061,11 +1106,16 @@ static gb_status serialize_graph(const gb_graph* g, const char* path) {
     bool device;
   };
   std::vector<Piece> pieces;
+  const uint64_t count = g->n;  // NodeValues' [usize n]
+  if (labeled) {
+    pieces.push_back({0, BIN_USIZE, &count, false});
+    pieces.push_back({BIN_USIZE, (uint64_t)g->n * 4, g->labels.p, true});
+  }
   std::string headers[2];
   DevBuf<uint2> records[2];
   for (unsigned c = 0; c < l.ncsr; ++c) {
     headers[c] = bin_header_bytes(l, c);
-    pieces.push_back({c == 0 ? 0 : l.csr[c].header, headers[c].size(), headers[c].data(), false});
+    pieces.push_back({c == 0 && !labeled ? 0 : l.csr[c].header, headers[c].size(), headers[c].data(), false});
     pieces.push_back({l.csr[c].off_pos, ((uint64_t)l.n + 1) * 4, csr[c]->off.p, true});
     if (!l.entries) continue;
     if (values) {
@@ -1124,8 +1174,10 @@ static gb_status serialize_graph(const gb_graph* g, const char* path) {
   return GB_OK;
 }
 
+// label_bytes: NV's width in a labelled binary file
 static gb_status load_graph(int device, gb_graph_kind kind, const char* path, gb_file_format format,
-                            gb_layout layout, int with_values, bool labeled, gb_graph** graph) {
+                            gb_layout layout, int with_values, bool labeled, gb_graph** graph,
+                            uint32_t label_bytes = 0) {
   GB_REQUIRE(graph != nullptr, "graph out-pointer is NULL");
   GB_REQUIRE(path != nullptr, "path is NULL");
   GB_REQUIRE(format == GB_FORMAT_GRAPH500 || format == GB_FORMAT_EDGE_LIST || format == GB_FORMAT_BINARY ||
@@ -1134,6 +1186,8 @@ static gb_status load_graph(int device, gb_graph_kind kind, const char* path, gb
   GB_REQUIRE(!with_values || format == GB_FORMAT_EDGE_LIST || format == GB_FORMAT_BINARY,
              "only edge lists and binary files carry edge values");
   GB_TRY(check_layout(layout));
+  if (labeled && format == GB_FORMAT_BINARY) GB_TRY(bin_check_label_bytes(label_bytes));
+  else label_bytes = 0;
   GB_TRY(require_device(device));
   DeviceGuard guard(device);
   InputFile f;
@@ -1145,8 +1199,8 @@ static gb_status load_graph(int device, gb_graph_kind kind, const char* path, gb
     if (on_host) GB_TRY(load_dotgraph_on_host(device, kind, f, layout, labeled, graph, &info));
     else GB_TRY(load_dotgraph_streamed(device, kind, f, layout, labeled, graph, &info));
   } else if (format == GB_FORMAT_BINARY) {
-    if (on_host) GB_TRY(load_binary_on_host(device, kind, f, with_values != 0, graph, &info));
-    else GB_TRY(load_binary_streamed(device, kind, f, with_values != 0, graph, &info));
+    if (on_host) GB_TRY(load_binary_on_host(device, kind, f, with_values != 0, label_bytes, graph, &info));
+    else GB_TRY(load_binary_streamed(device, kind, f, with_values != 0, label_bytes, graph, &info));
   } else if (on_host) {
     GB_TRY(load_on_host(device, kind, f, format, layout, with_values != 0, graph, &info));
   } else {
@@ -1211,7 +1265,23 @@ gb_status gb_graph_load_labeled_u32(int device, const char* path, gb_layout layo
   return gb::load_graph(device, GB_KIND_UNDIRECTED, path, GB_FORMAT_DOTGRAPH, layout, 0, true, graph);
 }
 
-gb_status gb_graph_serialize(const gb_graph* graph, const char* path) { return gb::serialize_graph(graph, path); }
+gb_status gb_digraph_load_labeled_binary_u32(int device, const char* path, gb_layout layout, uint32_t label_bytes,
+                                             gb_graph** graph) {
+  return gb::load_graph(device, GB_KIND_DIRECTED, path, GB_FORMAT_BINARY, layout, 0, true, graph, label_bytes);
+}
+
+gb_status gb_graph_load_labeled_binary_u32(int device, const char* path, gb_layout layout, uint32_t label_bytes,
+                                           gb_graph** graph) {
+  return gb::load_graph(device, GB_KIND_UNDIRECTED, path, GB_FORMAT_BINARY, layout, 0, true, graph, label_bytes);
+}
+
+gb_status gb_graph_serialize(const gb_graph* graph, const char* path) {
+  return gb::serialize_graph(graph, path, false);
+}
+
+gb_status gb_graph_serialize_labeled(const gb_graph* graph, const char* path) {
+  return gb::serialize_graph(graph, path, true);
+}
 
 gb_status gb_graph_load_info(const gb_graph* g, gb_load_info* info) {
   GB_REQUIRE(g && info, "NULL argument");

@@ -254,7 +254,9 @@ gb_status gb_graph_load_weighted_u32(int device, const char* path, gb_file_forma
  * value of the same edge; the in-CSR must be the transpose of the out-CSR).  So save(load(f)) is byte-equal
  * to f for files written here, and for a foreign weighted file up to the order of the values among parallel
  * (s, t) edges.  The file is written to a temporary file in the same directory, which is renamed over
- * `path` on success and removed on failure.  GB_ERR_INVALID for a gb_digraph_for_page_rank_u32 twin. */
+ * `path` on success and removed on failure.  GB_ERR_INVALID for a gb_digraph_for_page_rank_u32 twin.
+ * GB_ERR_UNSUPPORTED for a labelled twin, so that an unlabelled file never silently loses the labels: write
+ * those with gb_graph_serialize_labeled. */
 gb_status gb_graph_serialize(const gb_graph* graph, const char* path);
 
 /* ---- node-labelled graphs (crates/builder/src/input/dotgraph.rs) ----------------------------------------------
@@ -266,7 +268,7 @@ gb_status gb_graph_serialize(const gb_graph* graph, const char* path);
  * CAUTION: gb_make_degree_ordered relabels the CSR and, like the reference (graph_ops.rs:511-538, which swaps the
  * CSR and leaves node_values alone), does NOT permute the labels: afterwards label[v] is the label of the node
  * that had old id v, not of the node now called v.  gb_graph_serialize refuses a labelled twin
- * (GB_ERR_UNSUPPORTED): NodeValues payloads are not written.
+ * (GB_ERR_UNSUPPORTED); gb_graph_serialize_labeled writes it with its NodeValues.
  *
  * DotGraph file (dotgraph.rs:136-203): the header line "t N M", then N node lines "v <id> <label> <degree>" in id
  * order (the id and degree are skipped, the label kept), then M edge lines "e <src> <dst>" (kept in file order);
@@ -278,6 +280,35 @@ gb_status gb_graph_serialize(const gb_graph* graph, const char* path);
  * after the host has read the header; both give the same graph and the same errors and messages. */
 gb_status gb_digraph_load_labeled_u32(int device, const char* path, gb_layout layout, gb_graph** graph);
 gb_status gb_graph_load_labeled_u32(int device, const char* path, gb_layout layout, gb_graph** graph);
+/* DirectedCsrGraph<u32, NV> / UndirectedCsrGraph<u32, NV> from a binary file with a NodeValues payload
+ * (csr.rs:334-360, 606-656, 810-851): [usize n][NV x n], then the CSRs as gb_digraph_load_u32 reads them.
+ * label_bytes is NV's size and is not in the file: 4 (u32) or 8 (u64 / usize, narrowed to u32).
+ * `layout` is checked and otherwise ignored, as in the unlabelled binary load: rows are kept byte for byte and
+ * their order is left unknown.  A file whose records carry f32 values loads with the values dropped (a labelled
+ * twin has none), as gb_graph_load_u32 drops them.  The NodeValues count n places the first CSR header at
+ * 8 + n * label_bytes; it sizes nothing until the file is known to hold that many labels, so an absurd count
+ * fails with the end-of-file message and allocates nothing.  GB_ERR_INVALID, with the same message on the host
+ * path (below 64 MiB) and the streamed path (above, or with GB_LOAD_CHUNK_BYTES), for: label_bytes other than 4
+ * or 8; a NodeValues count that differs from the CSRs' node_count; an 8-byte label of 2^32 or more (the message
+ * names the smallest such node); and everything gb_binary_decode rejects.  The streamed path DMAs 4-byte labels
+ * straight into the twin's label array and narrows 8-byte ones on the device; gb_load_info.h2d_bytes counts
+ * them. */
+gb_status gb_digraph_load_labeled_binary_u32(int device, const char* path, gb_layout layout, uint32_t label_bytes,
+                                             gb_graph** graph);
+gb_status gb_graph_load_labeled_binary_u32(int device, const char* path, gb_layout layout, uint32_t label_bytes,
+                                           gb_graph** graph);
+/* SerializeGraphOp::serialize of a labelled twin: NodeValues<u32> ([usize n][u32 x n]), then what
+ * gb_graph_serialize writes, with NI = u32 and records without values.  It takes the handle's lock and writes
+ * through a temporary file renamed over `path`, as gb_graph_serialize does.  GB_ERR_UNSUPPORTED for a twin
+ * without labels, GB_ERR_INVALID for a gb_digraph_for_page_rank_u32 twin; no file is left in either case.
+ * CAUTION: after gb_make_degree_ordered it writes the labels as stored, which are not permuted (see above). */
+gb_status gb_graph_serialize_labeled(const gb_graph* graph, const char* path);
+/* the host decoder of those files: gb_binary_decode plus the labels (node_count entries, which labels needs
+ * whenever out_offsets is given); label_bytes as above */
+gb_status gb_binary_decode_labeled(const void* bytes, uint64_t len, gb_graph_kind kind, uint32_t label_bytes,
+                                   uint32_t* node_count, uint64_t* entries, int* has_values, uint32_t* labels,
+                                   uint32_t* out_offsets, uint32_t* out_targets, float* out_values,
+                                   uint32_t* in_offsets, uint32_t* in_targets);
 /* GraphBuilder::edges(..).node_values(..).build() (builder.rs:388, 425): node_count = label_count >= 1 */
 gb_status gb_digraph_from_edges_labeled_u32(int device, const uint32_t* src, const uint32_t* dst, uint64_t edge_count,
                                             const uint32_t* labels, uint32_t label_count, gb_layout layout,

@@ -107,6 +107,11 @@ class CsrGraphBase {
   gb_graph* handle() const { return g_; }
   // SerializeGraphOp::serialize, graph_ops.rs:232-238 (NI = u32)
   void serialize(const std::string& path) const { detail::check(gb_graph_serialize(g_, path.c_str())); }
+  // the same for a labelled graph (NI = u32, NV = u32): NodeValues, then the CSRs; throws graph::Error on a graph
+  // without labels.  build_[un]directed_labeled() reads the file back.
+  void serialize_labeled(const std::string& path) const {
+    detail::check(gb_graph_serialize_labeled(g_, path.c_str()));
+  }
   // NodeValues::node_value, csr.rs:64-76 (labelled graphs; throws graph::Error on a graph without labels)
   std::uint32_t node_value(std::uint32_t node) const {
     if (labels_.empty()) {
@@ -498,6 +503,21 @@ class GraphBuilder {
                                                    static_cast<gb_layout>(layout_), &g));
     return UndirectedCsrGraph(g);
   }
+  // DirectedCsrGraph<u32, NV> / UndirectedCsrGraph<u32, NV> from file_format(FileFormat::Binary).path(p), as
+  // build::<DirectedCsrGraph<u32, u32>>() reads a binary file: NodeValues of label_bytes each (4: u32, 8: u64 /
+  // usize, narrowed), then the CSRs as stored.  Throws graph::Error for any other source.
+  DirectedCsrGraph build_directed_labeled(std::uint32_t label_bytes = 4) const {
+    gb_graph* g = nullptr;
+    detail::check(gb_digraph_load_labeled_binary_u32(device_, labeled_binary_path().c_str(),
+                                                     static_cast<gb_layout>(layout_), label_bytes, &g));
+    return DirectedCsrGraph(g);
+  }
+  UndirectedCsrGraph build_undirected_labeled(std::uint32_t label_bytes = 4) const {
+    gb_graph* g = nullptr;
+    detail::check(gb_graph_load_labeled_binary_u32(device_, labeled_binary_path().c_str(),
+                                                   static_cast<gb_layout>(layout_), label_bytes, &g));
+    return UndirectedCsrGraph(g);
+  }
   // DirectedALGraph / UndirectedALGraph from the pending edges (adj_list.rs:406-450, :559-595): with values
   // (EV = f32) when the builder holds them (edges_with_values(..), or an edge list read with with_values()).
   // Graph500 and edge-list files; Binary and DotGraph files and node values have no adjacency-list form here.
@@ -505,6 +525,11 @@ class GraphBuilder {
   UndirectedALGraph build_undirected_al() const { return UndirectedALGraph(build_al(GB_KIND_UNDIRECTED)); }
 
  private:
+  const std::string& labeled_binary_path() const {
+    if (binary_path_.empty() || format_ != FileFormat::Binary)
+      throw Error(GB_ERR_INVALID, "build_directed_labeled / build_undirected_labeled read file_format(FileFormat::Binary).path(p)");
+    return binary_path_;
+  }
   gb_algraph* build_al(gb_graph_kind kind) const {
     if (!binary_path_.empty() || !labels_.empty())
       throw Error(GB_ERR_UNSUPPORTED, "adjacency-list graphs are built from edges, Graph500 or edge-list files");

@@ -3,7 +3,7 @@ and DotGraph (.graph) loads, beside the numpy restatement of the reference the t
 (tests/dotgraph_restatement.py).  That restatement is vectorised numpy (its reader a Python loop), not the
 reference's Rust, so its times are a CPU point of comparison, not the reference's numbers.
 
-    python tools/bench_labels.py [--runs 5] [--nlf-scales 22,24] [--cpu-max-scale 22] [--json out.json]
+    python tools/bench_labels.py [--runs 5] [--nlf-scales 22,24] [--cpu-max-scale 22] [--load-only] [--json out.json]
 
 Workloads:
   - label_stats and node_label_index on the graph of the reference's Criterion bench
@@ -11,7 +11,10 @@ Workloads:
     1e5 (the reference's sizes), 2^24 and 2^26;
   - neighbor_label_frequencies on undirected Sorted RMAT graphs (edge factor 16) with labels uniform in 0..42;
   - .graph loads of an RMAT-18 file (below 64 MiB, so read by the host reader unless GB_LOAD_CHUNK_BYTES selects
-    the device parser) and of an RMAT-20 file (parsed on the device).
+    the device parser) and of an RMAT-20 file (parsed on the device);
+  - the same two graphs saved with serialize_labeled and loaded back with load_labeled(file_format=Binary): the
+    RMAT-18 file on the host path and the streamed path, the RMAT-20 file (above 64 MiB) on the streamed path, beside
+    the pread floor of the file (tools/bench_load.py: 4 threads reading it into pinned memory, no device work).
 Times: each structure reports the CUDA-event time of its device work (gb_graph_last_timing: first kernel to last,
 the copies of the results to the host excluded) and the host time of the whole call; the achieved bandwidth of
 neighbor_label_frequencies is computed over the device time from the compulsory bytes
@@ -38,6 +41,7 @@ sys.path.insert(0, str(ROOT / "tests"))
 import graph_b200 as gb  # noqa: E402
 import oracle  # noqa: E402
 import dotgraph_restatement as dot  # noqa: E402
+from bench_load import pread_floor  # noqa: E402
 
 
 def timed(fn, runs):
@@ -130,7 +134,7 @@ def write_dotgraph(path, scale):
     return n, len(src)
 
 
-def bench_load(rows, runs, tmp):
+def bench_load(rows, runs, tmp, pinned):
     for scale, paths in ((18, ("host", "device")), (20, ("device",))):
         path = Path(tmp) / f"rmat{scale}.graph"
         n, m = write_dotgraph(path, scale)
@@ -151,7 +155,35 @@ def bench_load(rows, runs, tmp):
                 row["python_read_ms"] = (time.perf_counter() - t0) * 1e3
                 row["match"] = g.node_values().tobytes() == want.labels.tobytes()
             emit(rows, row)
-            del g
+            if which != paths[-1]:
+                del g
+        bench_binary(rows, runs, path.with_suffix(".bin"), g, scale, paths, pinned)
+        del g
+
+
+def bench_binary(rows, runs, path, g, scale, paths, pinned):
+    """save_labeled of the DotGraph twin g, then load_labeled of that binary file on each path"""
+    _, save_ms = timed(lambda: g.serialize_labeled(path), runs)
+    size = path.stat().st_size
+    emit(rows, {"bench": "save_labeled", "scale": scale, "file_bytes": size, "ms": save_ms,
+                "file_gb_per_s": size / save_ms / 1e6})
+    path.read_bytes()  # warm page cache
+    floor = min(pread_floor(path, pinned) for _ in range(runs)) * 1e3
+    for which in paths:
+        if which == "device" and size < (64 << 20):
+            os.environ["GB_LOAD_CHUNK_BYTES"] = str(64 << 20)
+        else:
+            os.environ.pop("GB_LOAD_CHUNK_BYTES", None)
+        h, ms = timed(lambda: gb.Graph.load_labeled(path, file_format=gb.FileFormat.Binary), runs)
+        os.environ.pop("GB_LOAD_CHUNK_BYTES", None)
+        info = h.load_info()
+        emit(rows, {"bench": "load_labeled binary", "scale": scale, "path": which, "file_bytes": size,
+                    "ms": ms, "file_gb_per_s": size / ms / 1e6, "pread_floor_ms": floor, "over_floor": ms / floor,
+                    "chunks": info["chunks"], "h2d_bytes": info["h2d_bytes"],
+                    "match": (h.node_values().tobytes() == g.node_values().tobytes()
+                              and all(a.tobytes() == b.tobytes() for a, b in zip(h.csr(), g.csr())))})
+        del h
+    path.unlink()
 
 
 def main():
@@ -161,6 +193,7 @@ def main():
     ap.add_argument("--cpu-max-scale", type=int, default=22, help="largest RMAT scale the numpy restatement runs")
     ap.add_argument("--cpu-max-nodes", type=int, default=1 << 24, help="largest stats workload the numpy code runs")
     ap.add_argument("--skip-load", action="store_true")
+    ap.add_argument("--load-only", action="store_true", help="only the DotGraph and binary file rows")
     ap.add_argument("--json", default=None)
     a = ap.parse_args()
     if gb.device_count() == 0:
@@ -169,11 +202,14 @@ def main():
                           capture_output=True, text=True).stdout.strip()
     rows = []
     emit(rows, {"device": info})
-    bench_stats(rows, a.runs, [1000, 10000, 100000, 1 << 24, 1 << 26], a.cpu_max_nodes)
-    bench_nlf(rows, a.runs, [int(s) for s in a.nlf_scales.split(",") if s], a.cpu_max_scale)
+    if not a.load_only:
+        bench_stats(rows, a.runs, [1000, 10000, 100000, 1 << 24, 1 << 26], a.cpu_max_nodes)
+        bench_nlf(rows, a.runs, [int(s) for s in a.nlf_scales.split(",") if s], a.cpu_max_scale)
     if not a.skip_load:
+        import torch  # the pinned buffer of the pread floor
+        pinned = torch.empty(4 * (64 << 20), dtype=torch.uint8, pin_memory=True)
         with tempfile.TemporaryDirectory() as tmp:
-            bench_load(rows, a.runs, tmp)
+            bench_load(rows, a.runs, tmp, pinned)
     if a.json:
         Path(a.json).parent.mkdir(parents=True, exist_ok=True)
         Path(a.json).write_text(json.dumps(rows, indent=1))
