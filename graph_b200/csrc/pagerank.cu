@@ -534,11 +534,64 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
 // block; CB_VIRT = pass B (block j is V[blk[j] .. blk[j + 1]), the column-block walker as in CB_MAIN; its first
 // warps add the cut segments of the hot blocks, which CB_FUSED has finished).
 constexpr uint32_t CB_MAIN = 0, CB_VIRT = 1, CB_FUSED = 2;
+
+// the next task of a CTA that drains range r (whole warp): from r's cursor, else from the first range after r that
+// has tasks left, which becomes r.  CB_NONE when every range is drained.
+__device__ __forceinline__ uint32_t cb_claim_task(const CbSched& s, uint32_t& r, uint32_t lane) {
+  const uint32_t R = gridDim.x;  // ranges = CTAs
+  for (;;) {
+    const uint32_t lo = (uint32_t)((uint64_t)s.n_tasks * r / R), hi = (uint32_t)((uint64_t)s.n_tasks * (r + 1) / R);
+    uint32_t k = CB_NONE;
+    if (lane == 0) {
+      k = lo + atomicAdd(s.task_ctr + r, 1u);
+      if (k >= hi) k = CB_NONE;
+    }
+    const uint32_t t = __shfl_sync(0xFFFFFFFFu, k, 0);
+    if (t != CB_NONE) return t;
+    // this range is drained: the lanes probe the other ranges' cursors 32 at a time (plain loads)
+    uint32_t found = CB_NONE;
+    for (uint32_t base = 1; base < R && found == CB_NONE; base += 32) {
+      uint32_t q = r + base + lane;
+      if (q >= R) q -= R;
+      bool ok = false;
+      if (base + lane < R) {
+        const uint32_t qlo = (uint32_t)((uint64_t)s.n_tasks * q / R), qhi = (uint32_t)((uint64_t)s.n_tasks * (q + 1) / R);
+        ok = *((volatile uint32_t*)(s.task_ctr + q)) < qhi - qlo;
+      }
+      const uint32_t m = __ballot_sync(0xFFFFFFFFu, ok);
+      if (m) found = __shfl_sync(0xFFFFFFFFu, q, __ffs(m) - 1);
+    }
+    if (found == CB_NONE) return CB_NONE;  // every range is drained
+    r = found;
+  }
+}
+// the block of task t: a source block (CB_FUSED), else a block rank of the stream
+template <uint32_t KIND>
+__device__ __forceinline__ uint32_t cb_task_block(const PrArgs& a, uint32_t t) {
+  return KIND == CB_FUSED ? ld_task(a.fused_tasks + t).w : a.sched.tasks[t].y >> 8;
+}
+
+// Inside a block the chunks of the CTA's tasks FLOW: s_flow = (task << 32 | next chunk) is the one cursor, and a
+// warp claims a chunk with one shared atomicAdd, which gives it the task and the chunk's index in it together
+// (CB_FUSED: hot, pass A, hot, .. while both kinds last, then the rest of the longer kind).  The warp that draws
+// the last index, n - 1, of an n-chunk task claims the CTA's next task before it walks that chunk (cb_claim_task:
+// only once the current task has no chunk left to hand out, so a claimed task is taken up by the next warp that
+// finishes a chunk and is not withheld from stealing for longer; the claim's round trip overlaps the walk).  If
+// that task is in the block in shared memory, the warp swaps it into s_flow with index 0 and the warps go on
+// without waiting; otherwise it leaves the task in s_task and CB_NONE in s_flow, and every warp leaves the flow
+// when it draws CB_NONE (the claiming warp after its chunk).  A warp that draws an index past n - 1 waits until
+// s_flow names another task.  Ordering rules:
+//  * a task and its chunk index come from one atomic on s_flow: no warp reads a task that is not published;
+//  * s_range (the range being drained) is written by a claimer before its atomicExch on s_flow, behind a
+//    __threadfence_block, and read by the next claimer after its atomicAdd, behind another: the claims are ordered;
+//  * the block is replaced only between two __syncthreads, which a warp reaches only after it drew CB_NONE, i.e.
+//    with no chunk of the block left; s_task is read after the first and s_flow is reset before the second.
 template <uint32_t KIND>
 __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
   extern __shared__ __align__(128) float smem[];
   float* xs = smem;  // B entries of x_cur + one zero slot (the pad id)
-  __shared__ uint32_t s_task, s_next;
+  __shared__ uint32_t s_task, s_range;
+  __shared__ __align__(8) unsigned long long s_flow;
   __shared__ __align__(8) unsigned long long s_mbar;
   if (a.ctrl[0] != 0) return;  // tolerance already met by an earlier sweep of this batch
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -547,101 +600,100 @@ __global__ void __launch_bounds__(PR_THREADS, 1) k_pr_cb(const PrArgs a) {
       cb_fix_segment(a.fix, a.fix.fix_list[i], lane);
   const uint32_t B = a.B;
   const uint32_t pad2 = B | (B << 16);
-  const uint32_t R = gridDim.x;  // ranges = CTAs
   const uint32_t mbar = (uint32_t)__cvta_generic_to_shared(&s_mbar);
   const uint32_t xs_smem = (uint32_t)__cvta_generic_to_shared(xs);
   const bool bulk_ok = (reinterpret_cast<uintptr_t>(a.x_cur) & 15u) == 0;  // cp.async.bulk moves 16-byte units
   uint32_t phase = 0;
   if (threadIdx.x == 0) mbar_init(mbar, 1);
   if (threadIdx.x < 4) xs[B + threadIdx.x] = 0.0f;  // the pad id's zero slot: never overwritten
-  uint32_t cur_j = CB_NONE;
-  uint32_t r = blockIdx.x;  // range being drained (warp 0 keeps it)
-  __syncthreads();  // mbarrier + zero slot are set up
+  if (warp == 0) {
+    uint32_t r = blockIdx.x;
+    const uint32_t t = cb_claim_task(a.sched, r, lane);
+    if (lane == 0) s_task = t, s_range = r;
+  }
   for (;;) {
-    if (warp == 0) {
-      uint32_t t = CB_NONE;
-      for (;;) {
-        const uint32_t lo = (uint32_t)((uint64_t)a.sched.n_tasks * r / R),
-                       hi = (uint32_t)((uint64_t)a.sched.n_tasks * (r + 1) / R);
-        uint32_t k = CB_NONE;
-        if (lane == 0) {
-          k = lo + atomicAdd(a.sched.task_ctr + r, 1u);
-          if (k >= hi) k = CB_NONE;
-        }
-        t = __shfl_sync(0xFFFFFFFFu, k, 0);
-        if (t != CB_NONE) break;
-        // this range is drained: the lanes probe the other ranges' cursors 32 at a time (plain loads)
-        uint32_t found = CB_NONE;
-        for (uint32_t base = 1; base < R && found == CB_NONE; base += 32) {
-          uint32_t q = r + base + lane;
-          if (q >= R) q -= R;
-          bool ok = false;
-          if (base + lane < R) {
-            const uint32_t qlo = (uint32_t)((uint64_t)a.sched.n_tasks * q / R),
-                           qhi = (uint32_t)((uint64_t)a.sched.n_tasks * (q + 1) / R);
-            ok = *((volatile uint32_t*)(a.sched.task_ctr + q)) < qhi - qlo;
-          }
-          const uint32_t m = __ballot_sync(0xFFFFFFFFu, ok);
-          if (m) found = __shfl_sync(0xFFFFFFFFu, q, __ffs(m) - 1);
-        }
-        if (found == CB_NONE) break;  // every range is drained
-        r = found;
+    __syncthreads();  // s_task is set, and every warp has left the flow of the previous block
+    const uint32_t t0 = s_task;
+    if (t0 == CB_NONE) break;
+    const uint32_t j = cb_task_block<KIND>(a, t0);
+    const uint64_t x0 = KIND == CB_VIRT    ? (uint64_t)a.sched.blk[j]
+                        : KIND == CB_FUSED ? (uint64_t)j * B
+                                           : (uint64_t)a.sched.blk[j] * B;
+    const uint32_t cnt = KIND == CB_VIRT ? a.sched.blk[j + 1] - a.sched.blk[j]
+                                         : (uint32_t)min((uint64_t)B, (uint64_t)a.n - x0);
+    if (bulk_ok) {
+      const uint32_t bulk = cnt & ~3u;
+      if (threadIdx.x == 0) {
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the block's old contents were read through the generic proxy
+        mbar_expect_tx(mbar, bulk * 4u);
+        for (uint32_t off = 0; off < bulk; off += 4096u)  // 16 KB pieces
+          bulk_g2s(xs_smem + off * 4u, a.x_cur + x0 + off, min(4096u, bulk - off) * 4u, mbar);
       }
-      if (lane == 0) s_task = t;
+      if (threadIdx.x >= 32 && threadIdx.x - 32 < cnt - bulk) xs[bulk + threadIdx.x - 32] = a.x_cur[x0 + bulk + threadIdx.x - 32];
+      mbar_wait(mbar, phase);
+      phase ^= 1u;
+    } else {
+      for (uint32_t i = threadIdx.x; i < cnt; i += PR_THREADS) xs[i] = a.x_cur[x0 + i];
     }
-    __syncthreads();  // also: every warp is done with the previous task's block
-    const uint32_t t = s_task;
-    if (threadIdx.x == 0) s_next = PR_THREADS / 32;  // every warp is past its last claim of the previous task
+    if (threadIdx.x == 0) s_flow = (unsigned long long)t0 << 32;
     __syncthreads();
-    if (t == CB_NONE) break;
-    // (first chunk, chunk count | block rank << 8); CB_FUSED: (first hot chunk, first pass-A chunk, hot chunks |
-    // pass-A chunks << 8, source block)
-    const uint2 task = KIND == CB_FUSED ? make_uint2(0u, 0u) : a.sched.tasks[t];
-    const uint32_t j = KIND == CB_FUSED ? ld_task(a.fused_tasks + t).w : task.y >> 8;
-    if (j != cur_j) {
-      const uint64_t x0 = KIND == CB_VIRT    ? (uint64_t)a.sched.blk[j]
-                          : KIND == CB_FUSED ? (uint64_t)j * B
-                                             : (uint64_t)a.sched.blk[j] * B;
-      const uint32_t cnt = KIND == CB_VIRT ? a.sched.blk[j + 1] - a.sched.blk[j]
-                                           : (uint32_t)min((uint64_t)B, (uint64_t)a.n - x0);
-      if (bulk_ok) {
-        const uint32_t bulk = cnt & ~3u;
-        if (threadIdx.x == 0) {
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the block's old contents were read through the generic proxy
-          mbar_expect_tx(mbar, bulk * 4u);
-          for (uint32_t off = 0; off < bulk; off += 4096u)  // 16 KB pieces
-            bulk_g2s(xs_smem + off * 4u, a.x_cur + x0 + off, min(4096u, bulk - off) * 4u, mbar);
-        }
-        if (threadIdx.x >= 32 && threadIdx.x - 32 < cnt - bulk) xs[bulk + threadIdx.x - 32] = a.x_cur[x0 + bulk + threadIdx.x - 32];
-        mbar_wait(mbar, phase);
-        phase ^= 1u;
-      } else {
-        for (uint32_t i = threadIdx.x; i < cnt; i += PR_THREADS) xs[i] = a.x_cur[x0 + i];
-      }
-      cur_j = j;
-      __syncthreads();
-    }
-    // a warp starts with chunk `warp` of the task and claims further ones from the CTA's counter.  CB_FUSED: the
-    // task's chunks alternate hot, pass A, hot, .. while both kinds last, then the rest of the longer kind; the
-    // task is read again for every chunk, so that none of it stays live across a walk (the walkers use every
-    // register of the 64 that one 1024-thread CTA per SM leaves)
-    const uint32_t nchunks = KIND == CB_FUSED ? CB_NONE : task.y & 0xFFu;  // CB_FUSED leaves the loop below
-    for (uint32_t k = warp; k < nchunks;) {
+    // the flow of block j.  The task is read again for every chunk, so that none of it stays live across a walk
+    // (the walkers use every register of the 64 that one 1024-thread CTA per SM leaves)
+    for (;;) {
+      unsigned long long f = 0;
+      if (lane == 0) f = atomicAdd(&s_flow, 1ull);
+      f = __shfl_sync(0xFFFFFFFFu, f, 0);
+      const uint32_t t = (uint32_t)(f >> 32), k = (uint32_t)f;
+      if (t == CB_NONE) break;
+      // (first chunk, chunk count | block rank << 8); CB_FUSED: (first hot chunk, first pass-A chunk, hot chunks |
+      // pass-A chunks << 8, source block)
+      uint32_t n;
       if constexpr (KIND == CB_FUSED) {
-        const uint4 ft = ld_task(a.fused_tasks + t);
-        const uint32_t n_hot = ft.z & 0xFFu, n_bin = ft.z >> 8, pairs = min(n_hot, n_bin);
-        if (k >= n_hot + n_bin) break;
-        const bool hot = k < 2 * pairs ? (k & 1u) == 0 : n_hot > n_bin;
-        const uint32_t i = k < 2 * pairs ? k >> 1 : k - pairs;
-        if (hot) cb_chunk(a, xs, ft.x + i, lane, pad2);
-        else if (a.bin_fill) bin_chunk<true>(a, xs, ft.y + i, lane);
-        else bin_chunk<false>(a, xs, ft.y + i, lane);
+        const uint32_t z = ld_task(a.fused_tasks + t).z;
+        n = (z & 0xFFu) + (z >> 8);
       } else {
-        cb_chunk(a, xs, task.x + k, lane, pad2);
+        n = a.sched.tasks[t].y & 0xFFu;
       }
-      uint32_t nx = 0;
-      if (lane == 0) nx = atomicAdd(&s_next, 1u);
-      k = __shfl_sync(0xFFFFFFFFu, nx, 0);
+      if (k >= max(n, 1u)) {  // past the task's chunks: wait until the claiming warp has swapped the next task in
+        uint32_t cur = t;
+        while (cur == t) {
+          __nanosleep(64);
+          if (lane == 0) cur = (uint32_t)(*(volatile unsigned long long*)&s_flow >> 32);
+          cur = __shfl_sync(0xFFFFFFFFu, cur, 0);
+        }
+        continue;
+      }
+      bool leave = false;
+      if (k + 1 == max(n, 1u)) {  // the task's last chunk: none is left to hand out, so claim the CTA's next task
+        uint32_t r = 0;
+        if (lane == 0) {
+          __threadfence_block();
+          r = *(volatile uint32_t*)&s_range;
+        }
+        r = __shfl_sync(0xFFFFFFFFu, r, 0);
+        const uint32_t nt = cb_claim_task(a.sched, r, lane);
+        leave = nt == CB_NONE || cb_task_block<KIND>(a, nt) != j;
+        if (lane == 0) {
+          *(volatile uint32_t*)&s_range = r;
+          if (leave) s_task = nt;
+          __threadfence_block();
+          atomicExch(&s_flow, (unsigned long long)(leave ? CB_NONE : nt) << 32);
+        }
+      }
+      if (k < n) {
+        if constexpr (KIND == CB_FUSED) {
+          const uint4 ft = ld_task(a.fused_tasks + t);
+          const uint32_t n_hot = ft.z & 0xFFu, n_bin = ft.z >> 8, pairs = min(n_hot, n_bin);
+          const bool hot = k < 2 * pairs ? (k & 1u) == 0 : n_hot > n_bin;
+          const uint32_t i = k < 2 * pairs ? k >> 1 : k - pairs;
+          if (hot) cb_chunk(a, xs, ft.x + i, lane, pad2);
+          else if (a.bin_fill) bin_chunk<true>(a, xs, ft.y + i, lane);
+          else bin_chunk<false>(a, xs, ft.y + i, lane);
+        } else {
+          cb_chunk(a, xs, a.sched.tasks[t].x + k, lane, pad2);
+        }
+      }
+      if (leave) break;
     }
   }
 }
