@@ -5,8 +5,9 @@
 // pageable memory and their result is uploaded.  Larger files go through a ring of pinned buffers
 // (PinnedRing): chunk k of the file travels through buffer k % ring.  On a load, one reader thread per buffer
 // preads the chunks that map to it (ChunkReader), a copy stream moves each chunk to the device slot's staging
-// buffer (DeviceStaging), and kernels on a work stream decode it.  On a save the copy stream fills the buffers
-// from device memory and the host writes them out.  Ordering rules:
+// buffer (DeviceStaging), and kernels on a work stream decode it; stream_file runs that loop, and one decoder per
+// format below says what each chunk stages and decodes.  On a save the copy stream fills the buffers from device
+// memory and the host writes them out.  Ordering rules:
 //   - a pinned buffer is refilled only after the copy out of it has completed (its `copied` event);
 //   - a device staging buffer is overwritten or reallocated only after the kernels that read it have completed
 //     (its `parsed` event);
@@ -303,6 +304,16 @@ struct InputFile {
     if (bytes && !pread_all(fd, out->get(), bytes, 0)) return fail(GB_ERR_INVALID, "reading %s failed", path);
     return GB_OK;
   }
+  // the bytes from `off` on through the next '\n' (or to the end of the file), read in pieces that start at
+  // `piece` bytes and double until one holds the '\n'
+  gb_status read_line(uint64_t off, uint64_t piece, std::string* out) const {
+    for (;; piece *= 2) {
+      const uint64_t n = std::min(piece, bytes - off);
+      out->resize(n);
+      if (!pread_all(fd, &(*out)[0], n, off)) return fail(GB_ERR_INVALID, "reading %s failed", path);
+      if (n == bytes - off || std::memchr(out->data(), '\n', n)) return GB_OK;
+    }
+  }
 };
 
 struct PinnedBuf {
@@ -486,17 +497,19 @@ struct ChunkReader : PinnedRing {
   }
 };
 
-// The device side of a streamed load: per ring slot a staging buffer and the event recorded behind the kernels
-// that read it.  Chunks reach the device on sp.copy and are decoded on sp.work.  Declare it inside the
+// The device side of a streamed load: per ring slot a staging buffer, what it holds, and the event recorded behind
+// the kernels that read it.  Chunks reach the device on sp.copy and are decoded on sp.work.  Declare it inside the
 // DevBufStreamScope of sp.work.
 struct DeviceStaging {
   ChunkReader& rd;
   StreamPair& sp;
   std::vector<DevBuf<uint8_t>> dbuf;  // [ring]: LOAD_TILE bytes of slack, as the text kernels read whole tiles
+  std::vector<uint64_t> off, len;     // [ring]: dbuf[r] holds len bytes from file byte off (len 0: none staged)
   std::vector<cudaEvent_t> parsed;    // [ring]
   uint64_t h2d = 0;                   // bytes copied to the device
 
-  DeviceStaging(ChunkReader& r, StreamPair& s) : rd(r), sp(s), dbuf(r.ring), parsed(r.ring, nullptr) {}
+  DeviceStaging(ChunkReader& r, StreamPair& s)
+      : rd(r), sp(s), dbuf(r.ring), off(r.ring, 0), len(r.ring, 0), parsed(r.ring, nullptr) {}
   gb_status create_events() {
     for (cudaEvent_t& e : parsed) GB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     return GB_OK;
@@ -514,22 +527,24 @@ struct DeviceStaging {
   gb_status stage(uint64_t k, const char* carry, uint64_t cl, uint64_t body) {
     const unsigned r = (unsigned)(k % rd.ring);
     char* data = rd.data(r);
-    const uint64_t len = cl + body;
-    if (dbuf[r].n < len + LOAD_TILE) {
+    const uint64_t n = cl + body;
+    if (dbuf[r].n < n + LOAD_TILE) {
       GB_CUDA(cudaEventSynchronize(parsed[r]));
       DevBuf<uint8_t> nb;
-      GB_TRY(nb.alloc(std::max<uint64_t>(len, rd.chunk + LOAD_CARRY_RESERVE) + LOAD_TILE));
+      GB_TRY(nb.alloc(std::max<uint64_t>(n, rd.chunk + LOAD_CARRY_RESERVE) + LOAD_TILE));
       dbuf[r] = std::move(nb);
     }
     GB_CUDA(cudaStreamWaitEvent(sp.copy, parsed[r], 0));
     if (cl <= LOAD_CARRY_RESERVE) {
       std::memcpy(data - cl, carry, cl);
-      GB_CUDA(cudaMemcpyAsync(dbuf[r].p, data - cl, len, cudaMemcpyHostToDevice, sp.copy));
+      GB_CUDA(cudaMemcpyAsync(dbuf[r].p, data - cl, n, cudaMemcpyHostToDevice, sp.copy));
     } else {
       GB_CUDA(cudaMemcpyAsync(dbuf[r].p, carry, cl, cudaMemcpyHostToDevice, sp.copy));
       if (body) GB_CUDA(cudaMemcpyAsync(dbuf[r].p + cl, data, body, cudaMemcpyHostToDevice, sp.copy));
     }
-    h2d += len;
+    off[r] = k * rd.chunk - cl;
+    len[r] = n;
+    h2d += n;
     return GB_OK;
   }
 };
@@ -545,21 +560,35 @@ static gb_status grow(DevBuf<T>& b, uint64_t need, uint64_t want, uint64_t keep,
   return GB_OK;
 }
 
-struct LoadedEdges {
-  DevBuf<uint32_t> src, dst;
-  DevBuf<float> w;
-  DevBuf<uint32_t> labels;  // DotGraph: [N]
-  uint64_t m = 0;
-  uint32_t n = 0;  // 0: max id + 1
+// Chunk k of a streamed read: file bytes [a, b).  In a decoder's stage() they are in pinned memory at `data`; in
+// its before() and after(), `dev` holds the len bytes that stage() sent to the device, from file byte `off`.
+struct Chunk {
+  uint64_t k, a, b;
+  bool last;
+  const char* data;
+  const uint8_t* dev;
+  uint64_t off, len;
 };
 
-static gb_status load_file(int device, const InputFile& f, gb_file_format format, bool want_value,
-                           const DotHeader& dot, LoadedEdges* out, gb_load_info* info) {
-  const bool g500 = format == GB_FORMAT_GRAPH500;
-  const bool dotgraph = format == GB_FORMAT_DOTGRAPH;
+// The streamed read of a file, for every format: its first `bytes` in chunks of whole `unit`s (PinnedRing::plan),
+// chunk k + 1 staged on sp.copy while chunk k is decoded on sp.work.  The Decoder is built here from sp.work and
+// `args` (its leading fields) and supplies:
+//   begin()        its arrays and counters, before the first chunk;
+//   stage(c, st)   from chunk k's pinned bytes: st.stage of the carried bytes and a body, and direct copies on
+//                  sp.copy (counted in st.h2d);
+//   before(c)      the work it issues on sp.work before chunk k + 1 is prepared;
+//   after(c)       the work it issues after that.  A chunk that staged nothing has neither;
+//   finish(info)   its checks and results, once every chunk is decoded and sp.copy has drained.
+// Destruction runs in reverse order of declaration, and the order matters:
+//   - the decoder goes first, inside the DevBufStreamScope, so its arrays, like every array grown and replaced
+//     during the read, are released in stream order on sp.work;
+//   - ~DeviceStaging drains sp.copy before the staging buffers are freed;
+//   - ~ChunkReader joins the reader threads before ~PinnedRing hands the pinned buffers back to PinnedRingCache.
+template <typename Decoder, typename... Args>
+static gb_status stream_file(int device, const InputFile& f, uint64_t bytes, uint64_t unit, gb_load_info* info,
+                             Args&&... args) {
   ChunkReader rd(f.fd, device);
-  const uint64_t m500 = f.bytes / 12;
-  rd.plan(g500 ? 12 * m500 : f.bytes, g500 ? 48 : 1);  // Graph500: whole 4-record groups, a partial tail ignored
+  rd.plan(bytes, unit);
   info->chunks = rd.nchunks;
   if (rd.nchunks == 0) return GB_OK;  // empty: gb_*_from_device_edges reports it
 
@@ -570,178 +599,235 @@ static gb_status load_file(int device, const InputFile& f, gb_file_format format
   DevBufStreamScope scope(sp.work);
   DeviceStaging st(rd, sp);
   GB_TRY(st.create_events());
+  Decoder dec{sp.work, std::forward<Args>(args)...};
+  GB_TRY(dec.begin());
 
-  const unsigned R = rd.ring;
-  DevBuf<LoadCounters> ctr;
-  GB_TRY(ctr.alloc(1));
-  GB_CUDA(cudaMemsetAsync(ctr.p, 0, sizeof(LoadCounters), sp.work));
-  PinnedBuf small;  // [0] = '\n' in the chunk, [1] = declined so far
-  GB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&small.p), 64, cudaHostAllocDefault));
-  uint32_t* hsmall = reinterpret_cast<uint32_t*>(small.p);
-
-  DevBuf<uint32_t> counts;  // per-tile '\n' counts, scanned in place
-  DevBuf<uint8_t> scan_tmp;
-  DevBuf<uint64_t> dec_off;
-  DevBuf<uint32_t> dec_edge;
-  uint64_t m = 0;
-  if (g500) {
-    GB_TRY(out->src.alloc(m500));
-    GB_TRY(out->dst.alloc(m500));
-  }
-  DevBuf<unsigned long long> dot_error;  // line << 3 | code of the first bad line
-  if (dotgraph) {  // the caller allocated the arrays it wants filled
-    GB_TRY(dot_error.alloc(1));
-    GB_CUDA(cudaMemsetAsync(dot_error.p, 0xFF, 8, sp.work));
-  }
-
-  // what prepare() leaves for run(): the device chunk and where it starts in the file
-  struct Staged {
-    uint64_t len = 0, file_off = 0;
-    bool ends_with_newline = true;
+  auto chunk = [&](uint64_t k) {
+    const unsigned r = (unsigned)(k % rd.ring);
+    const uint64_t a = k * rd.chunk;
+    return Chunk{k, a, a + rd.chunk_bytes(k), k + 1 == rd.nchunks, rd.data(r), st.dbuf[r].p, st.off[r], st.len[r]};
   };
-  std::vector<Staged> staged(R);
-  std::string carry;  // text: the bytes after the last '\n' so far
-
-  // waits for chunk k's bytes, moves them (with the carried line in front) to the device on the copy stream
+  // waits for chunk k's bytes and lets the decoder move them to the device on the copy stream
   auto prepare = [&](uint64_t k) -> gb_status {
-    const unsigned r = (unsigned)(k % R);
     GB_TRY(rd.wait_filled(k));
-    const char* data = rd.data(r);
-    const uint64_t n = rd.chunk_bytes(k);
-    const bool last = k + 1 == rd.nchunks;
-    uint64_t body = n;  // bytes of this chunk that go to the device now
-    std::string next_carry;
-    if (!g500 && !last) {
-      const void* nl = memrchr(data, '\n', n);
-      body = nl ? (uint64_t)(static_cast<const char*>(nl) - data) + 1 : 0;
-      if (!nl) next_carry = carry;
-      next_carry.append(data + body, n - body);
-    }
-    const uint64_t cl = (!g500 && (body || last)) ? carry.size() : 0;  // carried bytes that go in front
-    Staged& sg = staged[r];
-    sg.len = cl + body;
-    sg.file_off = k * rd.chunk - cl;
-    sg.ends_with_newline = sg.len == 0 || (body ? data[body - 1] == '\n' : carry.back() == '\n');
-    if (sg.len) GB_TRY(st.stage(k, carry.data(), cl, body));
-    GB_TRY(rd.release(k, sp));
-    if (!g500) carry.swap(next_carry);
-    return GB_OK;
+    st.len[k % rd.ring] = 0;
+    GB_TRY(dec.stage(chunk(k), st));
+    return rd.release(k, sp);
   };
-
   GB_TRY(prepare(0));
   for (uint64_t k = 0; k < rd.nchunks; ++k) {
-    const unsigned r = (unsigned)(k % R);
-    const Staged sg = staged[r];
-    const uint4* d = reinterpret_cast<const uint4*>(st.dbuf[r].p);
-    if (g500) {
-      if (k + 1 < rd.nchunks) GB_TRY(prepare(k + 1));
-      const uint64_t nrec = sg.len / 12;
-      if (nrec) {
-        k_load_graph500<<<grid_for((nrec + 3) / 4, 256), 256, 0, sp.work>>>(d, nrec, k * rd.chunk / 12, out->src.p,
-                                                                             out->dst.p, ctr.p);
-        GB_CUDA(cudaGetLastError());
-      }
-      GB_CUDA(cudaEventRecord(st.parsed[r], sp.work));
-      continue;
-    }
-    const uint64_t tiles = (sg.len + LOAD_TILE - 1) / LOAD_TILE;
-    if (tiles) {
-      GB_TRY(grow(counts, tiles, 2 * tiles, 0, sp.work));
-      k_load_count_lines<<<(unsigned)tiles, LOAD_BLOCK, 0, sp.work>>>(d, sg.len, counts.p);
-      GB_TRY(cub_call(scan_tmp, [&](void* t, size_t& tb) {
-        return cub::DeviceScan::InclusiveSum(t, tb, counts.p, counts.p, (int)tiles, sp.work);
-      }, 2));
-      GB_CUDA(cudaMemcpyAsync(hsmall, counts.p + tiles - 1, 4, cudaMemcpyDeviceToHost, sp.work));
-      GB_CUDA(cudaMemcpyAsync(hsmall + 1, &ctr.p->declined, 4, cudaMemcpyDeviceToHost, sp.work));
-    }
+    const Chunk c = chunk(k);
+    if (c.len) GB_TRY(dec.before(c));
     if (k + 1 < rd.nchunks) GB_TRY(prepare(k + 1));  // the next chunk crosses the bus meanwhile
-    if (tiles) {
-      GB_CUDA(cudaStreamSynchronize(sp.work));
-      const uint64_t lines = hsmall[0] + (sg.ends_with_newline ? 0 : 1);
-      if (dotgraph) {
-        k_load_parse_dotgraph<<<(unsigned)tiles, LOAD_BLOCK, 0, sp.work>>>(d, sg.len, counts.p, m, dot.nodes,
-                                                                          dot.lines, out->labels.p, out->src.p,
-                                                                          out->dst.p, dot_error.p);
-        GB_CUDA(cudaGetLastError());
-        m += lines;
-        GB_CUDA(cudaEventRecord(st.parsed[r], sp.work));
-        continue;
-      }
-      // size the arrays for the whole file from the lines per byte seen so far
-      const uint64_t through = std::min(rd.read_end, (k + 1) * rd.chunk);
-      const uint64_t est = (uint64_t)((double)(m + lines) * (double)rd.read_end / (double)through * 1.02) + 1024;
-      const uint64_t want = std::max(est, out->src.n + out->src.n / 2);
-      GB_TRY(grow(out->src, m + lines, want, m, sp.work));
-      GB_TRY(grow(out->dst, m + lines, want, m, sp.work));
-      if (want_value) {
-        GB_TRY(grow(out->w, m + lines, want, m, sp.work));
-        const uint64_t declined = hsmall[1];
-        GB_TRY(grow(dec_off, declined + lines, 2 * (declined + lines), declined, sp.work));
-        GB_TRY(grow(dec_edge, declined + lines, 2 * (declined + lines), declined, sp.work));
-      }
-      k_load_parse_text<<<(unsigned)tiles, LOAD_BLOCK, 0, sp.work>>>(d, sg.len, counts.p, m, sg.file_off,
-                                                                    want_value ? 1 : 0, out->src.p, out->dst.p,
-                                                                    out->w.p, ctr.p, dec_off.p, dec_edge.p);
-      GB_CUDA(cudaGetLastError());
-      m += lines;
+    if (c.len) {
+      GB_TRY(dec.after(c));
+      GB_CUDA(cudaEventRecord(st.parsed[k % rd.ring], sp.work));
     }
-    GB_CUDA(cudaEventRecord(st.parsed[r], sp.work));
   }
-  LoadCounters hc{};
-  GB_CUDA(cudaMemcpyAsync(&hc, ctr.p, sizeof hc, cudaMemcpyDeviceToHost, sp.work));
-  GB_CUDA(cudaStreamSynchronize(sp.work));
-  GB_REQUIRE(hc.wide == 0, g500 ? "Graph500 node id does not fit 32 bits" : "edge list node id does not fit 32 bits");
-  if (g500) m = m500;
-  if (dotgraph) {
-    unsigned long long first = 0;
-    GB_CUDA(cudaMemcpyAsync(&first, dot_error.p, 8, cudaMemcpyDeviceToHost, sp.work));
-    GB_CUDA(cudaStreamSynchronize(sp.work));
-    if (first != ~0ull) return dot_fail((uint32_t)(first & 7), (first >> 3) + 1, dot, 0);
-    if (m < dot.lines) return dot_fail(DOT_MISSING, 0, dot, m);
-    out->m = dot.edges;
-    info->edges = dot.edges;
-    info->h2d_bytes = st.h2d;
-    GB_CUDA(cudaStreamSynchronize(sp.copy));
+  GB_CUDA(cudaStreamSynchronize(sp.copy));
+  info->h2d_bytes = st.h2d;
+  return dec.finish(info);
+}
+
+// Graph500 files, into arrays of m edges allocated up front
+struct Graph500Decoder {
+  cudaStream_t s;
+  uint64_t m;  // records: a partial one at the end of the file is ignored
+  EdgeArrays* out;
+  DevBuf<LoadCounters> ctr;
+
+  gb_status begin() {
+    GB_TRY(ctr.alloc(1));
+    GB_CUDA(cudaMemsetAsync(ctr.p, 0, sizeof(LoadCounters), s));
+    GB_TRY(out->src.alloc(m));
+    GB_TRY(out->dst.alloc(m));
     return GB_OK;
   }
-
-  // declined values: re-read each line and parse it with the host reader's own function
-  if (hc.declined) {
-    std::vector<uint64_t> off(hc.declined);
-    std::vector<uint32_t> edge(hc.declined);
-    GB_CUDA(cudaMemcpyAsync(off.data(), dec_off.p, hc.declined * 8ull, cudaMemcpyDeviceToHost, sp.work));
-    GB_CUDA(cudaMemcpyAsync(edge.data(), dec_edge.p, hc.declined * 4ull, cudaMemcpyDeviceToHost, sp.work));
-    GB_CUDA(cudaStreamSynchronize(sp.work));
-    std::vector<float> val(hc.declined);
-    std::string line;
-    for (uint64_t i = 0; i < hc.declined; ++i) {
-      uint64_t want = 256;
-      for (;;) {
-        const uint64_t n = std::min(want, f.bytes - off[i]);
-        line.resize(n);
-        if (!pread_all(f.fd, &line[0], n, off[i])) return fail(GB_ERR_INVALID, "reading %s failed", f.path);
-        if (n == f.bytes - off[i] || std::memchr(line.data(), '\n', n)) break;
-        want *= 2;
-      }
-      uint64_t s, t;
-      gb::parse_line(line.data(), 0, line.size(), 1, &s, &t, &val[i]);
-    }
-    DevBuf<float> dval;
-    GB_TRY(dval.alloc(hc.declined));
-    GB_CUDA(cudaMemcpyAsync(dval.p, val.data(), hc.declined * 4ull, cudaMemcpyHostToDevice, sp.work));
-    k_load_patch<<<grid_for(hc.declined, 256), 256, 0, sp.work>>>(dec_edge.p, dval.p, hc.declined, out->w.p);
+  gb_status stage(const Chunk& c, DeviceStaging& st) { return st.stage(c.k, "", 0, c.b - c.a); }
+  gb_status before(const Chunk&) { return GB_OK; }
+  gb_status after(const Chunk& c) {
+    const uint64_t nrec = c.len / 12;  // >= 1: the file's first 12 m bytes are read
+    k_load_graph500<<<grid_for((nrec + 3) / 4, 256), 256, 0, s>>>(reinterpret_cast<const uint4*>(c.dev), nrec,
+                                                                   c.a / 12, out->src.p, out->dst.p, ctr.p);
     GB_CUDA(cudaGetLastError());
-    GB_CUDA(cudaStreamSynchronize(sp.work));
-    st.h2d += hc.declined * 4ull;
+    return GB_OK;
   }
-  out->m = m;
-  out->n = g500 ? (uint32_t)std::min<uint64_t>(m500 / 16, 0xFFFFFFFFull) : 0;  // graph500.rs:74
-  info->edges = m;
-  info->fallback_lines = hc.declined;
-  info->h2d_bytes = st.h2d;
-  GB_CUDA(cudaStreamSynchronize(sp.copy));
-  return GB_OK;
-}
+  gb_status finish(gb_load_info* info) {
+    LoadCounters hc{};
+    GB_CUDA(cudaMemcpyAsync(&hc, ctr.p, sizeof hc, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaStreamSynchronize(s));
+    GB_REQUIRE(hc.wide == 0, "Graph500 node id does not fit 32 bits");
+    out->m = m;
+    out->n = (uint32_t)std::min<uint64_t>(m / 16, 0xFFFFFFFFull);  // graph500.rs:74
+    info->edges = m;
+    return GB_OK;
+  }
+};
+
+// The line-tile stage of the text formats: a chunk staged up to its last '\n' (the last chunk whole) with the
+// carried bytes in front, then the tile counts and their scan into the tile bases the parse kernels take.
+struct LineTiles {
+  std::string carry;        // the bytes after the last '\n' so far
+  bool open_end = false;    // the file's last byte is not a '\n': its last line has none
+  DevBuf<uint32_t> counts;  // per-tile '\n' counts, scanned in place
+  DevBuf<uint8_t> scan_tmp;
+  PinnedBuf small;  // [0] = '\n' in the chunk; [1] is the edge-list decoder's
+  uint32_t* host = nullptr;
+
+  static uint64_t tiles(const Chunk& c) { return (c.len + LOAD_TILE - 1) / LOAD_TILE; }
+  gb_status begin() {
+    GB_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&small.p), 64, cudaHostAllocDefault));
+    host = reinterpret_cast<uint32_t*>(small.p);
+    return GB_OK;
+  }
+  gb_status stage(const Chunk& c, DeviceStaging& st) {
+    const uint64_t n = c.b - c.a;
+    uint64_t body = n;  // bytes of this chunk that go to the device now
+    if (c.last) {
+      open_end = c.data[n - 1] != '\n';
+    } else {
+      const void* nl = memrchr(c.data, '\n', n);
+      body = nl ? (uint64_t)(static_cast<const char*>(nl) - c.data) + 1 : 0;
+    }
+    if (body) {
+      GB_TRY(st.stage(c.k, carry.data(), carry.size(), body));
+      carry.clear();
+    }
+    carry.append(c.data + body, n - body);
+    return GB_OK;
+  }
+  // enqueues the tile counts of the staged chunk, their scan and the copy of its '\n' count to host[0]
+  gb_status count(const Chunk& c, cudaStream_t s) {
+    const uint64_t t = tiles(c);
+    GB_TRY(grow(counts, t, 2 * t, 0, s));
+    k_load_count_lines<<<(unsigned)t, LOAD_BLOCK, 0, s>>>(reinterpret_cast<const uint4*>(c.dev), c.len, counts.p);
+    GB_TRY(cub_call(scan_tmp, [&](void* tmp, size_t& tb) {
+      return cub::DeviceScan::InclusiveSum(tmp, tb, counts.p, counts.p, (int)t, s);
+    }, 2));
+    GB_CUDA(cudaMemcpyAsync(host, counts.p + t - 1, 4, cudaMemcpyDeviceToHost, s));
+    return GB_OK;
+  }
+  // the lines of the staged chunk, once host[0] has arrived
+  uint64_t lines(const Chunk& c) const { return host[0] + (c.last && open_end ? 1 : 0); }
+};
+
+// Text edge lists, into arrays that grow as the lines come; the values the device parser declines are re-read
+// on the host and patched in by k_load_patch once every chunk is parsed.
+struct EdgeListDecoder {
+  cudaStream_t s;
+  const InputFile& f;
+  bool want_value;
+  EdgeArrays* out;
+  LineTiles text;
+  DevBuf<LoadCounters> ctr;
+  DevBuf<uint64_t> dec_off;
+  DevBuf<uint32_t> dec_edge;
+  uint64_t m = 0;  // edges so far
+
+  gb_status begin() {
+    GB_TRY(ctr.alloc(1));
+    GB_CUDA(cudaMemsetAsync(ctr.p, 0, sizeof(LoadCounters), s));
+    return text.begin();
+  }
+  gb_status stage(const Chunk& c, DeviceStaging& st) { return text.stage(c, st); }
+  gb_status before(const Chunk& c) {
+    GB_TRY(text.count(c, s));
+    GB_CUDA(cudaMemcpyAsync(text.host + 1, &ctr.p->declined, 4, cudaMemcpyDeviceToHost, s));
+    return GB_OK;
+  }
+  gb_status after(const Chunk& c) {
+    GB_CUDA(cudaStreamSynchronize(s));
+    const uint64_t lines = text.lines(c);
+    // size the arrays for the whole file from the lines per byte seen so far
+    const uint64_t est = (uint64_t)((double)(m + lines) * (double)f.bytes / (double)c.b * 1.02) + 1024;
+    const uint64_t want = std::max(est, out->src.n + out->src.n / 2);
+    GB_TRY(grow(out->src, m + lines, want, m, s));
+    GB_TRY(grow(out->dst, m + lines, want, m, s));
+    if (want_value) {
+      GB_TRY(grow(out->w, m + lines, want, m, s));
+      const uint64_t declined = text.host[1];
+      GB_TRY(grow(dec_off, declined + lines, 2 * (declined + lines), declined, s));
+      GB_TRY(grow(dec_edge, declined + lines, 2 * (declined + lines), declined, s));
+    }
+    k_load_parse_text<<<(unsigned)LineTiles::tiles(c), LOAD_BLOCK, 0, s>>>(
+        reinterpret_cast<const uint4*>(c.dev), c.len, text.counts.p, m, c.off, want_value ? 1 : 0, out->src.p,
+        out->dst.p, out->w.p, ctr.p, dec_off.p, dec_edge.p);
+    GB_CUDA(cudaGetLastError());
+    m += lines;
+    return GB_OK;
+  }
+  gb_status finish(gb_load_info* info) {
+    LoadCounters hc{};
+    GB_CUDA(cudaMemcpyAsync(&hc, ctr.p, sizeof hc, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaStreamSynchronize(s));
+    GB_REQUIRE(hc.wide == 0, "edge list node id does not fit 32 bits");
+    // declined values: re-read each line and parse it with the host reader's own function
+    if (hc.declined) {
+      std::vector<uint64_t> off(hc.declined);
+      std::vector<uint32_t> edge(hc.declined);
+      GB_CUDA(cudaMemcpyAsync(off.data(), dec_off.p, hc.declined * 8ull, cudaMemcpyDeviceToHost, s));
+      GB_CUDA(cudaMemcpyAsync(edge.data(), dec_edge.p, hc.declined * 4ull, cudaMemcpyDeviceToHost, s));
+      GB_CUDA(cudaStreamSynchronize(s));
+      std::vector<float> val(hc.declined);
+      std::string line;
+      for (uint64_t i = 0; i < hc.declined; ++i) {
+        GB_TRY(f.read_line(off[i], 256, &line));
+        uint64_t src, dst;
+        gb::parse_line(line.data(), 0, line.size(), 1, &src, &dst, &val[i]);
+      }
+      DevBuf<float> dval;
+      GB_TRY(dval.alloc(hc.declined));
+      GB_CUDA(cudaMemcpyAsync(dval.p, val.data(), hc.declined * 4ull, cudaMemcpyHostToDevice, s));
+      k_load_patch<<<grid_for(hc.declined, 256), 256, 0, s>>>(dec_edge.p, dval.p, hc.declined, out->w.p);
+      GB_CUDA(cudaGetLastError());
+      GB_CUDA(cudaStreamSynchronize(s));
+      info->h2d_bytes += hc.declined * 4ull;
+    }
+    out->m = m;
+    out->n = 0;  // max id + 1
+    info->edges = m;
+    info->fallback_lines = hc.declined;
+    return GB_OK;
+  }
+};
+
+// DotGraph files after the header h, which the host has read.  The arrays are the caller's, NULL where they are
+// not wanted or the file cannot hold the lines h declares (dot_fits).
+struct DotGraphDecoder {
+  cudaStream_t s;
+  const DotHeader& h;
+  uint32_t *labels, *src, *dst;
+  LineTiles text;
+  DevBuf<unsigned long long> first_error;  // line << 3 | code of the first bad line
+  uint64_t line = 0;  // lines so far, the header included
+
+  gb_status begin() {
+    GB_TRY(text.begin());
+    GB_TRY(first_error.alloc(1));
+    GB_CUDA(cudaMemsetAsync(first_error.p, 0xFF, 8, s));
+    return GB_OK;
+  }
+  gb_status stage(const Chunk& c, DeviceStaging& st) { return text.stage(c, st); }
+  gb_status before(const Chunk& c) { return text.count(c, s); }
+  gb_status after(const Chunk& c) {
+    GB_CUDA(cudaStreamSynchronize(s));
+    k_load_parse_dotgraph<<<(unsigned)LineTiles::tiles(c), LOAD_BLOCK, 0, s>>>(
+        reinterpret_cast<const uint4*>(c.dev), c.len, text.counts.p, line, h.nodes, h.lines, labels, src, dst,
+        first_error.p);
+    GB_CUDA(cudaGetLastError());
+    line += text.lines(c);
+    return GB_OK;
+  }
+  gb_status finish(gb_load_info* info) {
+    unsigned long long first = 0;
+    GB_CUDA(cudaMemcpyAsync(&first, first_error.p, 8, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaStreamSynchronize(s));
+    if (first != ~0ull) return dot_fail((uint32_t)(first & 7), (first >> 3) + 1, h, 0);
+    if (line < h.lines) return dot_fail(DOT_MISSING, 0, h, line);
+    info->edges = h.edges;
+    return GB_OK;
+  }
+};
 
 // The CSR (or label) arrays a binary file's section fills.  Elements of `stride` bytes start at file byte `pos`
 // with an id (or label) of `width` bytes; a u32 section without values (stride 4) is DMA'd straight into `ids`,
@@ -790,123 +876,94 @@ static gb_status check_loaded_csrs(gb_graph* g, const BinLayout& l, DevCsr* cons
   return GB_OK;
 }
 
-// Binary graph files streamed into the CSR arrays (and the label array, for label_bytes != 0).  A staged chunk
+// Binary graph files, into the CSR arrays of g (and its label array, for a labelled layout l).  A staged chunk
 // carries at most 15 bytes of a cut element in front, and k_bin_split decodes the elements that end inside the
 // chunk.
-static gb_status load_binary_streamed(int device, gb_graph_kind kind, const InputFile& f, bool want_value,
-                                      uint32_t label_bytes, gb_graph** graph, gb_load_info* info) {
-  BinLayout l;
-  GB_TRY(bin_parse([&](uint64_t pos, void* dst, uint64_t n) { return pread_all(f.fd, static_cast<char*>(dst), n, pos); },
-                   f.bytes, kind, &l, label_bytes));
-  GB_REQUIRE(!want_value || l.values, "the binary graph file holds no edge values");
-  GraphPtr g;
-  GB_TRY(new_graph(device, kind, l.n, &g));
-
-  StreamPair sp;
-  GB_CUDA(cudaStreamCreateWithFlags(&sp.copy, cudaStreamNonBlocking));
-  GB_CUDA(cudaStreamCreateWithFlags(&sp.work, cudaStreamNonBlocking));
-  DevBufStreamScope scope(sp.work);
-  DevCsr* csr[2] = {&g->out, &g->in};
+struct BinaryDecoder {
+  cudaStream_t s;
+  gb_graph* g;
+  const BinLayout& l;
+  bool want_value;
   std::vector<BinSection> secs;
+  DevBuf<unsigned int> wide;        // an id or offset does not fit 32 bits
   DevBuf<unsigned int> label_wide;  // the smallest node whose 8-byte label does not fit 32 bits, or ~0
-  if (label_bytes) {
-    GB_TRY(g->labels.alloc(l.n));
-    GB_TRY(label_wide.alloc(1));
-    GB_CUDA(cudaMemsetAsync(label_wide.p, 0xFF, 4, sp.work));
-    BinSection s;
-    s.pos = BIN_USIZE, s.count = l.n, s.stride = s.width = label_bytes, s.ids = g->labels.p;
-    s.first_wide = label_wide.p;
-    secs.push_back(s);
-  }
-  for (unsigned c = 0; c < l.ncsr; ++c) {
-    DevCsr& d = *csr[c];
-    d.len = l.entries;
-    GB_TRY(d.off.alloc((size_t)l.n + 1));
-    GB_TRY(d.tgt.alloc(l.entries, 8));
-    GB_CUDA(cudaMemsetAsync(d.tgt.p + l.entries, 0, 8 * 4, sp.work));
-    if (c == 0 && want_value) GB_TRY(d.w.alloc(l.entries, 8));  // the out-CSR or the undirected CSR; no in-CSR values
-    BinSection o, t;
-    o.pos = l.csr[c].off_pos, o.count = (uint64_t)l.n + 1, o.stride = o.width = l.id_bytes, o.ids = d.off.p;
-    t.pos = l.csr[c].rec_pos, t.count = l.entries, t.stride = l.rec_bytes, t.width = l.id_bytes, t.ids = d.tgt.p;
-    t.w = d.w.p;
-    secs.push_back(o);
-    if (t.count) secs.push_back(t);
-  }
+  std::string carry;                // bytes of the staged element that the next chunk completes
 
-  ChunkReader rd(f.fd, device);
-  rd.plan(f.bytes);
-  info->chunks = rd.nchunks;
-  GB_TRY(rd.start());
-  DeviceStaging st(rd, sp);
-  GB_TRY(st.create_events());
-  const unsigned R = rd.ring;
-  DevBuf<unsigned int> wide;
-  GB_TRY(wide.alloc(1));
-  GB_CUDA(cudaMemsetAsync(wide.p, 0, 4, sp.work));
-
-  std::vector<uint64_t> staged_off(R, 0);  // file byte of st.dbuf[r][0], or ~0: the chunk was not staged
-  std::string carry;                       // bytes of the staged element that the next chunk completes
-  auto prepare = [&](uint64_t k) -> gb_status {
-    const unsigned r = (unsigned)(k % R);
-    GB_TRY(rd.wait_filled(k));
-    const char* data = rd.data(r);
-    const uint64_t a = k * rd.chunk, len = rd.chunk_bytes(k), b = a + len;
-    bool stage = false;
-    for (const BinSection& s : secs) stage |= !s.direct() && s.pos < b && s.end() > a;
-    const uint64_t cl = stage ? carry.size() : 0;
-    staged_off[r] = stage ? a - cl : ~0ull;
-    if (stage) GB_TRY(st.stage(k, carry.data(), cl, len));
-    for (const BinSection& s : secs) {
-      if (!s.direct()) continue;
-      const uint64_t x = std::max(a, s.pos), y = std::min(b, s.end());
+  gb_status begin() {
+    if (l.label_bytes) {
+      GB_TRY(g->labels.alloc(l.n));
+      GB_TRY(label_wide.alloc(1));
+      GB_CUDA(cudaMemsetAsync(label_wide.p, 0xFF, 4, s));
+      BinSection sec;
+      sec.pos = BIN_USIZE, sec.count = l.n, sec.stride = sec.width = l.label_bytes, sec.ids = g->labels.p;
+      sec.first_wide = label_wide.p;
+      secs.push_back(sec);
+    }
+    DevCsr* csr[2] = {&g->out, &g->in};
+    for (unsigned c = 0; c < l.ncsr; ++c) {
+      DevCsr& d = *csr[c];
+      d.len = l.entries;
+      GB_TRY(d.off.alloc((size_t)l.n + 1));
+      GB_TRY(d.tgt.alloc(l.entries, 8));
+      GB_CUDA(cudaMemsetAsync(d.tgt.p + l.entries, 0, 8 * 4, s));
+      if (c == 0 && want_value) GB_TRY(d.w.alloc(l.entries, 8));  // the out-CSR or the undirected CSR; no in-CSR values
+      BinSection o, t;
+      o.pos = l.csr[c].off_pos, o.count = (uint64_t)l.n + 1, o.stride = o.width = l.id_bytes, o.ids = d.off.p;
+      t.pos = l.csr[c].rec_pos, t.count = l.entries, t.stride = l.rec_bytes, t.width = l.id_bytes, t.ids = d.tgt.p;
+      t.w = d.w.p;
+      secs.push_back(o);
+      if (t.count) secs.push_back(t);
+    }
+    GB_TRY(wide.alloc(1));
+    GB_CUDA(cudaMemsetAsync(wide.p, 0, 4, s));
+    return GB_OK;
+  }
+  gb_status stage(const Chunk& c, DeviceStaging& st) {
+    bool staged = false;
+    for (const BinSection& sec : secs) staged |= !sec.direct() && sec.pos < c.b && sec.end() > c.a;
+    if (staged) GB_TRY(st.stage(c.k, carry.data(), carry.size(), c.b - c.a));
+    for (const BinSection& sec : secs) {
+      if (!sec.direct()) continue;
+      const uint64_t x = std::max(c.a, sec.pos), y = std::min(c.b, sec.end());
       if (x >= y) continue;
-      GB_CUDA(cudaMemcpyAsync(reinterpret_cast<char*>(s.ids) + (x - s.pos), data + (x - a), y - x,
-                              cudaMemcpyHostToDevice, sp.copy));
+      GB_CUDA(cudaMemcpyAsync(reinterpret_cast<char*>(sec.ids) + (x - sec.pos), c.data + (x - c.a), y - x,
+                              cudaMemcpyHostToDevice, st.sp.copy));
       st.h2d += y - x;
     }
     carry.clear();
-    for (const BinSection& s : secs)
-      if (!s.direct() && s.pos < b && s.end() > b) {
-        const uint64_t cut = (b - s.pos) % s.stride;  // bytes of the element that begins before b
-        carry.assign(data + (len - cut), cut);
+    for (const BinSection& sec : secs)
+      if (!sec.direct() && sec.pos < c.b && sec.end() > c.b) {
+        const uint64_t cut = (c.b - sec.pos) % sec.stride;  // bytes of the element that begins before b
+        carry.assign(c.data + (c.b - c.a - cut), cut);
       }
-    return rd.release(k, sp);
-  };
-  auto split = [&](uint64_t k) -> gb_status {
-    const unsigned r = (unsigned)(k % R);
-    if (staged_off[r] == ~0ull) return GB_OK;
-    const uint64_t a = k * rd.chunk, b = a + rd.chunk_bytes(k);
-    for (const BinSection& s : secs) {
-      if (s.direct() || s.pos >= b || s.end() <= a) continue;
-      const uint64_t first = a > s.pos ? (a - s.pos) / s.stride : 0;  // the first element that ends after a
-      const uint64_t last = std::min(s.count, (b - s.pos) / s.stride);  // elements that end by b
+    return GB_OK;
+  }
+  gb_status before(const Chunk&) { return GB_OK; }
+  gb_status after(const Chunk& c) {
+    for (const BinSection& sec : secs) {
+      if (sec.direct() || sec.pos >= c.b || sec.end() <= c.a) continue;
+      const uint64_t first = c.a > sec.pos ? (c.a - sec.pos) / sec.stride : 0;  // the first element that ends after a
+      const uint64_t last = std::min(sec.count, (c.b - sec.pos) / sec.stride);   // elements that end by b
       if (last <= first) continue;
-      k_bin_split<<<grid_for(last - first, 256), 256, 0, sp.work>>>(st.dbuf[r].p, staged_off[r], s.pos, s.stride,
-                                                                      s.width, first, last - first, s.ids, s.w,
-                                                                      wide.p, s.first_wide);
+      k_bin_split<<<grid_for(last - first, 256), 256, 0, s>>>(c.dev, c.off, sec.pos, sec.stride, sec.width, first,
+                                                             last - first, sec.ids, sec.w, wide.p, sec.first_wide);
       GB_CUDA(cudaGetLastError());
     }
-    GB_CUDA(cudaEventRecord(st.parsed[r], sp.work));
     return GB_OK;
-  };
-  GB_TRY(prepare(0));
-  for (uint64_t k = 0; k < rd.nchunks; ++k) {
-    if (k + 1 < rd.nchunks) GB_TRY(prepare(k + 1));  // the next chunk crosses the bus meanwhile
-    GB_TRY(split(k));
   }
-  GB_CUDA(cudaStreamSynchronize(sp.copy));
-  if (label_bytes == 8) {  // the labels first, as gb_binary_decode_labeled checks them
-    unsigned int first = 0;
-    GB_CUDA(cudaMemcpyAsync(&first, label_wide.p, 4, cudaMemcpyDeviceToHost, sp.work));
-    GB_CUDA(cudaStreamSynchronize(sp.work));
-    if (first != 0xFFFFFFFFu) return bin_label_wide(first);
+  gb_status finish(gb_load_info* info) {
+    if (l.label_bytes == 8) {  // the labels first, as gb_binary_decode_labeled checks them
+      unsigned int first = 0;
+      GB_CUDA(cudaMemcpyAsync(&first, label_wide.p, 4, cudaMemcpyDeviceToHost, s));
+      GB_CUDA(cudaStreamSynchronize(s));
+      if (first != 0xFFFFFFFFu) return bin_label_wide(first);
+    }
+    DevCsr* csr[2] = {&g->out, &g->in};
+    GB_TRY(check_loaded_csrs(g, l, csr, wide.p, s));
+    info->edges = l.kind == GB_KIND_DIRECTED ? l.entries : l.entries / 2;
+    return GB_OK;
   }
-  GB_TRY(check_loaded_csrs(g.get(), l, csr, wide.p, sp.work));
-  info->edges = kind == GB_KIND_DIRECTED ? l.entries : l.entries / 2;
-  info->h2d_bytes = st.h2d;
-  *graph = g.release();
-  return GB_OK;
-}
+};
 
 // Below these sizes the fixed costs of the pipeline (threads, streams, pinned ring) exceed what it saves, and
 // the host readers are faster (H100 80GB HBM3, 400 W; tools/bench_load.py).  GB_LOAD_CHUNK_BYTES, when
@@ -944,6 +1001,24 @@ static gb_status load_on_host(int device, gb_graph_kind kind, const InputFile& f
   info->edges = m;
   info->h2d_bytes = m * (want_value ? 12 : 8);
   return GB_OK;
+}
+
+// the edges of a Graph500 or edge-list file, parsed on the device into out
+static gb_status stream_edges(int device, const InputFile& f, gb_file_format format, bool want_value,
+                              EdgeArrays* out, gb_load_info* info) {
+  if (format == GB_FORMAT_GRAPH500)
+    return stream_file<Graph500Decoder>(device, f, 12 * (f.bytes / 12), 48, info, f.bytes / 12, out);
+  return stream_file<EdgeListDecoder>(device, f, f.bytes, 1, info, f, want_value, out);
+}
+
+// a larger Graph500 or edge-list file (or any, with GB_LOAD_CHUNK_BYTES): parsed on the device, then
+// gb_[di]graph_from_device_edges_u32's build
+static gb_status load_edges_streamed(int device, gb_graph_kind kind, const InputFile& f, gb_file_format format,
+                                     gb_layout layout, bool want_value, gb_graph** graph, gb_load_info* info) {
+  EdgeArrays e;
+  GB_TRY(stream_edges(device, f, format, want_value, &e, info));
+  return graph_from_device_arrays(device, kind, e.src.p, e.dst.p, want_value ? e.w.p : nullptr, e.m, e.n, layout,
+                                  nullptr, graph);
 }
 
 // A labelled graph has N nodes, one per label (csr.rs:554-562 asserts that every edge id is below it); an unlabelled
@@ -998,26 +1073,22 @@ static gb_status load_dotgraph_streamed(int device, gb_graph_kind kind, const In
                                         bool labeled, gb_graph** graph, gb_load_info* info) {
   // the first line, as the host reader sees it in the whole file
   std::string head;
-  for (uint64_t want = std::min<uint64_t>(f.bytes, 4096);; want = std::min(f.bytes, 2 * want)) {
-    head.resize(want);
-    if (want && !pread_all(f.fd, &head[0], want, 0)) return fail(GB_ERR_INVALID, "reading %s failed", f.path);
-    if (want == f.bytes || std::memchr(head.data(), '\n', want)) break;
-  }
+  GB_TRY(f.read_line(0, 4096, &head));
   DotHeader h;
   GB_TRY(dot_read_header(head.data(), head.size(), &h));
   const bool fits = dot_fits(h, f.bytes);
-  LoadedEdges e;
+  DevBuf<uint32_t> src, dst, labels;
   if (fits) {
-    GB_TRY(e.src.alloc(h.edges));
-    GB_TRY(e.dst.alloc(h.edges));
-    if (labeled) GB_TRY(e.labels.alloc(h.nodes));
+    GB_TRY(src.alloc(h.edges));
+    GB_TRY(dst.alloc(h.edges));
+    if (labeled) GB_TRY(labels.alloc(h.nodes));
   }
-  GB_TRY(load_file(device, f, GB_FORMAT_DOTGRAPH, false, h, &e, info));
+  GB_TRY(stream_file<DotGraphDecoder>(device, f, f.bytes, 1, info, h, labels.p, src.p, dst.p));
   GB_TRY(dot_require_fits(h, fits));
   GB_TRY(dot_require_nodes(h, labeled));
-  GB_TRY(graph_from_device_arrays(device, kind, e.src.p, e.dst.p, nullptr, h.edges, labeled ? h.nodes : 0, layout,
-                                  nullptr, graph));
-  if (labeled) (*graph)->labels = std::move(e.labels);  // parsed on the device, so not part of h2d_bytes
+  GB_TRY(graph_from_device_arrays(device, kind, src.p, dst.p, nullptr, h.edges, labeled ? h.nodes : 0, layout, nullptr,
+                                  graph));
+  if (labeled) (*graph)->labels = std::move(labels);  // parsed on the device, so not part of h2d_bytes
   return GB_OK;
 }
 
@@ -1057,6 +1128,21 @@ static gb_status load_binary_on_host(int device, gb_graph_kind kind, const Input
   *graph = g.release();
   info->edges = kind == GB_KIND_DIRECTED ? m : m / 2;
   info->h2d_bytes = ncsr * (((uint64_t)n + 1) * 4 + m * 4) + (want_value ? m * 4 : 0) + (label_bytes ? 4ull * n : 0);
+  return GB_OK;
+}
+
+// a larger binary file (or any, with GB_LOAD_CHUNK_BYTES): the headers on the host, the sections streamed into the
+// CSR arrays (and the label array, for label_bytes != 0)
+static gb_status load_binary_streamed(int device, gb_graph_kind kind, const InputFile& f, bool want_value,
+                                      uint32_t label_bytes, gb_graph** graph, gb_load_info* info) {
+  BinLayout l;
+  GB_TRY(bin_parse([&](uint64_t pos, void* dst, uint64_t n) { return pread_all(f.fd, static_cast<char*>(dst), n, pos); },
+                   f.bytes, kind, &l, label_bytes));
+  GB_REQUIRE(!want_value || l.values, "the binary graph file holds no edge values");
+  GraphPtr g;
+  GB_TRY(new_graph(device, kind, l.n, &g));
+  GB_TRY(stream_file<BinaryDecoder>(device, f, f.bytes, 1, info, g.get(), l, want_value));
+  *graph = g.release();
   return GB_OK;
 }
 
@@ -1201,13 +1287,9 @@ static gb_status load_graph(int device, gb_graph_kind kind, const char* path, gb
   } else if (format == GB_FORMAT_BINARY) {
     if (on_host) GB_TRY(load_binary_on_host(device, kind, f, with_values != 0, label_bytes, graph, &info));
     else GB_TRY(load_binary_streamed(device, kind, f, with_values != 0, label_bytes, graph, &info));
-  } else if (on_host) {
-    GB_TRY(load_on_host(device, kind, f, format, layout, with_values != 0, graph, &info));
   } else {
-    LoadedEdges e;
-    GB_TRY(load_file(device, f, format, with_values != 0, DotHeader{}, &e, &info));
-    GB_TRY(graph_from_device_arrays(device, kind, e.src.p, e.dst.p, with_values ? e.w.p : nullptr, e.m, e.n, layout,
-                                    nullptr, graph));
+    if (on_host) GB_TRY(load_on_host(device, kind, f, format, layout, with_values != 0, graph, &info));
+    else GB_TRY(load_edges_streamed(device, kind, f, format, layout, with_values != 0, graph, &info));
   }
   (*graph)->load = info;
   return GB_OK;
@@ -1227,15 +1309,7 @@ gb_status load_edge_arrays(int device, const char* path, gb_file_format format, 
   GB_TRY(f.open(path));
   out->info = gb_load_info{};
   out->info.file_bytes = f.bytes;
-  LoadedEdges e;
-  GB_TRY(load_file(device, f, format, with_values, DotHeader{}, &e, &out->info));
-  out->src = std::move(e.src);
-  out->dst = std::move(e.dst);
-  out->w = std::move(e.w);
-  out->m = e.m;
-  out->n = e.n;
-  out->info.edges = e.m;
-  return GB_OK;
+  return stream_edges(device, f, format, with_values, out, &out->info);
 }
 
 }  // namespace gb
