@@ -23,7 +23,7 @@ from ._capi import GraphB200Error, check, lib
 __all__ = ["DiGraph", "Graph", "Layout", "FileFormat", "PageRankResult", "WccResult",
            "TriangleCountResult", "SsspResult", "LabelStats", "NodeLabelIndex", "NeighborLabelFrequencies",
            "NeighborLabelFrequency", "PageRankConfig", "WccConfig", "DeltaSteppingConfig",
-           "GraphB200Error", "device_count", "set_device", "write_graph500", "wcc_csr",
+           "GraphB200Error", "device_count", "set_device", "write_graph500", "wcc_csr", "wcc_file", "wcc_file_info",
            "triangle_count_csr", "sssp_csr", "DirectedALGraph", "UndirectedALGraph"]
 
 _device = 0
@@ -1317,6 +1317,42 @@ def wcc_csr(offsets, targets, *, chunk_size: int = WccConfig.DEFAULT_CHUNK_SIZE,
     the labels instead of a new array; it is left untouched when the call fails."""
     return _wcc_csr_call(lib.gb_wcc_csr_u32, _device, offsets, targets, chunk_size, neighbor_rounds,
                          sampling_size, out)
+
+
+def wcc_file(path, file_format=FileFormat.Graph500, *, chunk_size: int = WccConfig.DEFAULT_CHUNK_SIZE,
+             neighbor_rounds: int = WccConfig.DEFAULT_NEIGHBOR_ROUNDS,
+             sampling_size: int = WccConfig.DEFAULT_SAMPLING_SIZE) -> WccResult:
+    """wcc of a graph file in one pass, without building the graph (gb_wcc_file_u32): the file is read as
+    DiGraph.load(path, file_format=file_format) reads it, and each chunk's edges are linked on the device as soon as
+    they are decoded, so no edge array or CSR is ever held and Graph500, edge-list and DotGraph files of 2^32 - 1
+    edges or more are accepted.  The labels are those of DiGraph.load(...).wcc() (the minimum node id of each
+    component), and every other file fails as the load fails, with FileNotFoundError or the same ValueError.  The
+    config is checked and otherwise ignored; wcc_file_info() describes the call."""
+    p, fmt, _ = _load_args(path, file_format, None)
+    cfg = _capi.WccConfig(int(chunk_size), int(neighbor_rounds), int(sampling_size))
+    h = C.c_void_p()
+
+    def go():
+        check(lib.gb_wcc_file_u32(_device, p, fmt, C.byref(cfg), C.byref(h)))
+        try:
+            n = C.c_uint32(0)
+            check(lib.gb_components_node_count(h, C.byref(n)))
+            comp = np.empty(n.value, np.uint32)
+            check(lib.gb_components_copy(h, _ptr(comp)))
+        finally:
+            lib.gb_components_free(h)
+        return comp
+    comp, micros = _timed(go)
+    return WccResult(comp, micros)
+
+
+def wcc_file_info() -> dict:
+    """Statistics of the calling thread's last wcc_file (all zero after a failed call): file_bytes, chunks, edges,
+    h2d_bytes, device_bytes (the most the call held on the device at once), node_count and total_ms (CUDA-event time
+    from the first copy to the last link)."""
+    info = _capi.WccFileStats()
+    check(lib.gb_wcc_file_info(C.byref(info)))
+    return info.as_dict()
 
 
 def triangle_count_csr(offsets, targets) -> TriangleCountResult:

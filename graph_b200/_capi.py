@@ -95,6 +95,15 @@ class SsspCsrInfo(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class WccFileStats(C.Structure):
+    _fields_ = [("file_bytes", C.c_uint64), ("chunks", C.c_uint64), ("edges", C.c_uint64),
+                ("h2d_bytes", C.c_uint64), ("device_bytes", C.c_uint64), ("node_count", C.c_uint32),
+                ("reserved", C.c_uint32), ("total_ms", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_ if k != "reserved"}
+
+
 class LabelStatsInfo(C.Structure):
     _fields_ = [("max_degree", C.c_uint32), ("max_label", C.c_uint32), ("label_count", C.c_uint64),
                 ("max_label_frequency", C.c_uint64)]
@@ -182,6 +191,11 @@ SIGNATURES = {
     "gb_wcc": (C.c_int, [_P, C.POINTER(WccConfig), _P]),
     "gb_wcc_device": (C.c_int, [_P, C.POINTER(WccConfig), _P]),
     "gb_wcc_csr_u32": (C.c_int, [C.c_int, C.c_uint32, _P, _P, C.POINTER(WccConfig), _P]),
+    "gb_wcc_file_u32": (C.c_int, [C.c_int, C.c_char_p, C.c_int, C.POINTER(WccConfig), C.POINTER(_P)]),
+    "gb_components_node_count": (C.c_int, [_P, C.POINTER(C.c_uint32)]),
+    "gb_components_copy": (C.c_int, [_P, _P]),
+    "gb_components_free": (C.c_int, [_P]),
+    "gb_wcc_file_info": (C.c_int, [C.POINTER(WccFileStats)]),
     "gb_wcc_shard_phase": (C.c_int, [_P, C.POINTER(WccConfig), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                      C.c_int, _P, _P, _P]),
     "gb_wcc_sample_label": (C.c_int, [_P, C.POINTER(WccConfig), _P, C.POINTER(C.c_uint32), C.POINTER(C.c_int), _P]),

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
@@ -76,16 +77,39 @@ struct DevBufStreamScope {
   DevBufStreamScope(const DevBufStreamScope&) = delete;
   DevBufStreamScope& operator=(const DevBufStreamScope&) = delete;
 };
+// The device bytes one call holds: while a DevBufTally is open on a thread, every DevBuf that thread allocates is
+// counted in `now` until it is released, and `peak` keeps the most held at once.  A buffer that outlives the call
+// leaves the tally first (DevBuf::untally).
+struct DevBufTally {
+  uint64_t now = 0, peak = 0;
+  DevBufTally* prev;
+  static DevBufTally*& slot() {
+    static thread_local DevBufTally* open = nullptr;
+    return open;
+  }
+  DevBufTally() : prev(slot()) { slot() = this; }
+  ~DevBufTally() { slot() = prev; }
+  DevBufTally(const DevBufTally&) = delete;
+  DevBufTally& operator=(const DevBufTally&) = delete;
+};
 template <typename T>
 struct DevBuf {
   T* p = nullptr;
   size_t n = 0;
+  DevBufTally* tally = nullptr;  // counts the block's `held` bytes
+  size_t held = 0;
   DevBuf() = default;
   DevBuf(const DevBuf&) = delete;
   DevBuf& operator=(const DevBuf&) = delete;
-  DevBuf(DevBuf&& o) noexcept : p(o.p), n(o.n) { o.p = nullptr; o.n = 0; }
+  DevBuf(DevBuf&& o) noexcept : p(o.p), n(o.n), tally(o.tally), held(o.held) {
+    o.p = nullptr; o.n = 0; o.tally = nullptr; o.held = 0;
+  }
   DevBuf& operator=(DevBuf&& o) noexcept {
-    if (this != &o) { release(); p = o.p; n = o.n; o.p = nullptr; o.n = 0; }
+    if (this != &o) {
+      release();
+      p = o.p; n = o.n; tally = o.tally; held = o.held;
+      o.p = nullptr; o.n = 0; o.tally = nullptr; o.held = 0;
+    }
     return *this;
   }
   ~DevBuf() { release(); }
@@ -96,8 +120,14 @@ struct DevBuf {
       else cudaDeviceSynchronize();
       cudaFreeAsync(p, cudaStreamLegacy);
     }
+    untally();
     p = nullptr;
     n = 0;
+  }
+  void untally() {
+    if (tally) tally->now -= held;
+    tally = nullptr;
+    held = 0;
   }
   // allocates count elements (+ pad elements of slack so 128-bit loads may overrun the tail)
   gb_status alloc(size_t count, size_t pad = 0) {
@@ -114,6 +144,11 @@ struct DevBuf {
                   "cudaMallocAsync(%zu bytes) failed: %s", bytes, cudaGetErrorString(e));
     }
     n = count;
+    if ((tally = DevBufTally::slot())) {
+      held = bytes;
+      tally->now += bytes;
+      tally->peak = std::max(tally->peak, tally->now);
+    }
     return GB_OK;
   }
   size_t bytes() const { return n * sizeof(T); }
@@ -429,6 +464,21 @@ gb_status dot_read_host(const char* text, uint64_t len, const DotHeader& h, uint
 gb_status dot_fail(uint32_t code, uint64_t line, const DotHeader& h, uint64_t have);
 // Copies n labels (host or device memory, by `kind`) into g->labels on g's stream and waits for the copy.
 gb_status attach_labels(gb_graph* g, const uint32_t* labels, cudaMemcpyKind kind);
+
+// ---- union-find links for the WCC of a graph file (wcc.cu; load.cu decodes the chunks) ----
+// Every link hooks the higher root under the lower, so after cc_compress_async parent[v] is the minimum node id of
+// v's component, as gb_wcc gives.  All of them enqueue on s.
+// parent[v] = v for v in [from, to)
+void cc_init_async(cudaStream_t s, uint32_t* parent, uint64_t from, uint64_t to);
+// links src[i] with dst[i] for i < count; a pair with an endpoint >= n is not linked, and *bad counts its endpoints
+// >= n (the count check_edge_ids makes)
+void cc_link_pairs_async(cudaStream_t s, const uint32_t* src, const uint32_t* dst, uint64_t count, uint32_t n,
+                         uint32_t* parent, unsigned int* bad);
+// links every edge [e0, e0 + len) of a device CSR of n rows whose offsets are checked (off[0] == 0, monotone,
+// off[n] == entries): tgt holds those edges' targets with 8 entries of slack; *bad counts the targets >= n
+void cc_link_csr_async(cudaStream_t s, const uint32_t* off, uint32_t n, const uint32_t* tgt, uint32_t e0,
+                       uint32_t len, uint32_t* parent, unsigned int* bad);
+void cc_compress_async(cudaStream_t s, uint32_t* parent, uint32_t n);
 
 // the devices of a communicator, in its order (multi.cu); peer access among them is enabled
 const std::vector<int>& comm_devices(const gb_comm* c);

@@ -36,6 +36,8 @@
 //   label does not fit 32 bits.
 //   Writer: the file is pieces of host and device memory; chunk k + 1 is copied from the device into the ring
 //   while chunk k is written with pwrite to a temporary file, which is then renamed over the destination.
+//   WCC of a file (gb_wcc_file_u32): the same decoders, given a WccSink, decode each chunk into per-chunk scratch
+//   instead of whole-file arrays and hand it to the sink, which links it into a parent array (DESIGN.md §11).
 #include <fcntl.h>
 #include <sys/stat.h>
 #include <unistd.h>
@@ -53,6 +55,13 @@
 #include "common.cuh"
 #include "edgelist_line.h"
 #include "edgelist_scan.h"
+
+// the labels of a gb_wcc_file_u32 call, on the device that computed them
+struct gb_components {
+  int device = 0;
+  uint32_t n = 0;
+  gb::DevBuf<uint32_t> labels;
+};
 
 namespace gb {
 
@@ -570,6 +579,148 @@ struct Chunk {
   uint64_t off, len;
 };
 
+// The consumer of decoded chunks behind gb_wcc_file_u32.  A decoder given one puts each chunk's edges into its
+// scratch instead of whole-file arrays (src / dst pairs, or a binary chunk's targets in src) and hands them over in
+// after(); they are linked into parent[] on the work stream s, behind the decode.  One scratch serves every chunk:
+// chunk k's links run on s before the decode of chunk k + 1 overwrites it.  With no node_count up front (edge lists,
+// DotGraph, Graph500 files of fewer than 16 records) it is the largest id so far + 1: each chunk's largest id is
+// read back before its links, and parent[] grows by doubling with an identity tail.
+struct WccSink {
+  cudaStream_t s = nullptr;
+  bool infer = true;          // node_count = max id + 1
+  uint64_t n = 0, cap = 0;    // nodes so far, parent entries (the identity past n)
+  bool max_id = false;        // an id 2^32 - 1 was read: no node_count fits
+  bool stop = false;          // the read fails anyway: no more links
+  DevBuf<uint32_t> parent;
+  DevBuf<uint32_t> src, dst;  // one chunk's pairs; src holds a binary chunk's targets
+  DevBuf<unsigned int> bad;   // pairs: [0] endpoints >= n; binary: [c] targets >= n of CSR c
+  DevBuf<uint32_t> mx;        // the chunk's largest src and dst
+  DevBuf<uint8_t> tmp;
+  uint32_t host[3] = {0, 0, 0};
+  cudaEvent_t begin = nullptr, end = nullptr;
+  double total_ms = 0.0;
+  // binary files: the offsets of the out- and in-CSR, and their checks (check_loaded_csrs's), made before the first
+  // link searches them
+  DevCsr csr[2];
+  bool checked[2] = {false, false};
+  uint32_t off_first[2] = {0, 0}, off_last[2] = {0, 0};
+  unsigned int off_bad[2] = {0, 0};
+
+  ~WccSink() {
+    if (begin) cudaEventDestroy(begin);
+    if (end) cudaEventDestroy(end);
+  }
+  // fixed_n: the file's node_count, or 0 when it is the largest id + 1
+  gb_status start(cudaStream_t stream, uint64_t fixed_n) {
+    s = stream;
+    GB_CUDA(cudaEventCreate(&begin));
+    GB_CUDA(cudaEventCreate(&end));
+    GB_TRY(bad.alloc(2));
+    GB_CUDA(cudaMemsetAsync(bad.p, 0, 8, s));
+    GB_TRY(mx.alloc(2));
+    infer = fixed_n == 0;
+    if (!infer) {
+      GB_TRY(parent.alloc(fixed_n));
+      cc_init_async(s, parent.p, 0, fixed_n);
+      n = cap = fixed_n;
+    }
+    return GB_OK;
+  }
+  // in a decoder's stage(): the timed section starts with chunk 0's first copy
+  gb_status staging(const Chunk& c, cudaStream_t copy) {
+    if (c.k == 0) GB_CUDA(cudaEventRecord(begin, copy));
+    return GB_OK;
+  }
+  // room for `count` pairs (count targets when !pairs), with 8 entries of slack; a power of two, so that the
+  // size follows the chunk size and not the file
+  gb_status scratch(uint64_t count, bool pairs = true) {
+    uint64_t want = 1024;
+    while (want < count + 8) want *= 2;
+    if (src.n < count + 8) GB_TRY(src.alloc(want));
+    if (pairs && dst.n < count + 8) GB_TRY(dst.alloc(want));
+    return GB_OK;
+  }
+  // links the `count` pairs the decoder has put into src / dst; d_stop: the decoder's flag of an error that fails
+  // the read, read back with the largest id
+  gb_status link_pairs(uint64_t count, const unsigned int* d_stop) {
+    if (stop || count == 0) return GB_OK;
+    if (infer) {
+      GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) { return cub::DeviceReduce::Max(t, tb, src.p, mx.p, count, s); }));
+      GB_TRY(cub_call(tmp, [&](void* t, size_t& tb) {
+        return cub::DeviceReduce::Max(t, tb, dst.p, mx.p + 1, count, s);
+      }));
+      host[2] = 0;
+      GB_CUDA(cudaMemcpyAsync(host, mx.p, 8, cudaMemcpyDeviceToHost, s));
+      if (d_stop) GB_CUDA(cudaMemcpyAsync(host + 2, d_stop, 4, cudaMemcpyDeviceToHost, s));
+      GB_CUDA(cudaStreamSynchronize(s));
+      const uint32_t hi = std::max(host[0], host[1]);
+      max_id = hi == 0xFFFFFFFFu;
+      if (host[2] || max_id) {
+        stop = true;
+        return GB_OK;
+      }
+      if (hi + 1ull > cap) {
+        const uint64_t want = std::min<uint64_t>(std::max<uint64_t>(hi + 1ull, 2 * cap), 0xFFFFFFFFull);
+        GB_TRY(grow(parent, hi + 1ull, want, cap, s));
+        cc_init_async(s, parent.p, cap, parent.n);
+        cap = parent.n;
+      }
+      n = std::max<uint64_t>(n, hi + 1ull);
+    }
+    cc_link_pairs_async(s, src.p, dst.p, count, (uint32_t)n, parent.p, bad.p);
+    GB_CUDA(cudaGetLastError());
+    return GB_OK;
+  }
+  // after the decoder's own checks: those of gb_[di]graph_from_device_edges_u32 on m edges (check_edge_args but
+  // for the u32 offset limit, then check_edge_ids), and the labels
+  gb_status finish_pairs(uint64_t m) {
+    GB_REQUIRE(!infer || m > 0, "cannot infer node_count from an empty edge list");
+    if (infer) {
+      GB_REQUIRE(!max_id, "node id 2^32-1 leaves no room for node_count");
+    } else {
+      GB_CUDA(cudaMemcpyAsync(host, bad.p, 4, cudaMemcpyDeviceToHost, s));
+      GB_CUDA(cudaStreamSynchronize(s));
+      GB_REQUIRE(host[0] == 0, "%u edge endpoints are >= node_count %u", host[0], (uint32_t)n);
+    }
+    return finish();
+  }
+  // CSR c's offsets (all on the device): off[0], off[n] and the decreasing rows
+  gb_status check_offsets(unsigned c, uint32_t rows) {
+    if (checked[c]) return GB_OK;
+    GB_CUDA(cudaMemsetAsync(mx.p, 0, 4, s));
+    check_monotone_async(s, csr[c].off.p, rows, reinterpret_cast<unsigned int*>(mx.p));
+    GB_CUDA(cudaGetLastError());
+    GB_CUDA(cudaMemcpyAsync(&off_bad[c], mx.p, 4, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaMemcpyAsync(&off_first[c], csr[c].off.p, 4, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaMemcpyAsync(&off_last[c], csr[c].off.p + rows, 4, cudaMemcpyDeviceToHost, s));
+    GB_CUDA(cudaStreamSynchronize(s));
+    checked[c] = true;
+    return GB_OK;
+  }
+  // the targets [e0, e0 + count) of CSR c, which the decoder has put into src; not linked when c's offsets fail
+  // their checks (the read fails on them, and the row searches need them)
+  gb_status link_targets(unsigned c, const BinLayout& l, uint64_t e0, uint64_t count) {
+    GB_TRY(check_offsets(c, l.n));
+    if (off_first[c] != 0 || off_bad[c] != 0 || off_last[c] != l.entries) return GB_OK;
+    cc_link_csr_async(s, csr[c].off.p, l.n, src.p, (uint32_t)e0, (uint32_t)count, parent.p, bad.p + c);
+    GB_CUDA(cudaGetLastError());
+    return GB_OK;
+  }
+  // the final compress; the scratch goes, parent[] stays for the caller
+  gb_status finish() {
+    cc_compress_async(s, parent.p, (uint32_t)n);
+    GB_CUDA(cudaGetLastError());
+    GB_CUDA(cudaEventRecord(end, s));
+    GB_CUDA(cudaStreamSynchronize(s));
+    float ms = 0.0f;
+    GB_CUDA(cudaEventElapsedTime(&ms, begin, end));
+    total_ms = ms;
+    src.release(), dst.release(), bad.release(), mx.release(), tmp.release();
+    csr[0] = DevCsr(), csr[1] = DevCsr();
+    return GB_OK;
+  }
+};
+
 // The streamed read of a file, for every format: its first `bytes` in chunks of whole `unit`s (PinnedRing::plan),
 // chunk k + 1 staged on sp.copy while chunk k is decoded on sp.work.  The Decoder is built here from sp.work and
 // `args` (its leading fields) and supplies:
@@ -629,24 +780,37 @@ static gb_status stream_file(int device, const InputFile& f, uint64_t bytes, uin
   return dec.finish(info);
 }
 
-// Graph500 files, into arrays of m edges allocated up front
+// Graph500 files, into arrays of m edges allocated up front, or chunk by chunk into the pairs of a WccSink
 struct Graph500Decoder {
   cudaStream_t s;
   uint64_t m;  // records: a partial one at the end of the file is ignored
   EdgeArrays* out;
+  WccSink* wcc = nullptr;  // instead of out
   DevBuf<LoadCounters> ctr;
 
+  static uint32_t nodes(uint64_t m) { return (uint32_t)std::min<uint64_t>(m / 16, 0xFFFFFFFFull); }  // graph500.rs:74
   gb_status begin() {
     GB_TRY(ctr.alloc(1));
     GB_CUDA(cudaMemsetAsync(ctr.p, 0, sizeof(LoadCounters), s));
+    if (wcc) return wcc->start(s, nodes(m));
     GB_TRY(out->src.alloc(m));
     GB_TRY(out->dst.alloc(m));
     return GB_OK;
   }
-  gb_status stage(const Chunk& c, DeviceStaging& st) { return st.stage(c.k, "", 0, c.b - c.a); }
+  gb_status stage(const Chunk& c, DeviceStaging& st) {
+    if (wcc) GB_TRY(wcc->staging(c, st.sp.copy));
+    return st.stage(c.k, "", 0, c.b - c.a);
+  }
   gb_status before(const Chunk&) { return GB_OK; }
   gb_status after(const Chunk& c) {
     const uint64_t nrec = c.len / 12;  // >= 1: the file's first 12 m bytes are read
+    if (wcc) {
+      GB_TRY(wcc->scratch(nrec));
+      k_load_graph500<<<grid_for((nrec + 3) / 4, 256), 256, 0, s>>>(reinterpret_cast<const uint4*>(c.dev), nrec, 0,
+                                                                     wcc->src.p, wcc->dst.p, ctr.p);
+      GB_CUDA(cudaGetLastError());
+      return wcc->link_pairs(nrec, &ctr.p->wide);
+    }
     k_load_graph500<<<grid_for((nrec + 3) / 4, 256), 256, 0, s>>>(reinterpret_cast<const uint4*>(c.dev), nrec,
                                                                    c.a / 12, out->src.p, out->dst.p, ctr.p);
     GB_CUDA(cudaGetLastError());
@@ -657,9 +821,10 @@ struct Graph500Decoder {
     GB_CUDA(cudaMemcpyAsync(&hc, ctr.p, sizeof hc, cudaMemcpyDeviceToHost, s));
     GB_CUDA(cudaStreamSynchronize(s));
     GB_REQUIRE(hc.wide == 0, "Graph500 node id does not fit 32 bits");
-    out->m = m;
-    out->n = (uint32_t)std::min<uint64_t>(m / 16, 0xFFFFFFFFull);  // graph500.rs:74
     info->edges = m;
+    if (wcc) return wcc->finish_pairs(m);
+    out->m = m;
+    out->n = nodes(m);
     return GB_OK;
   }
 };
@@ -718,6 +883,7 @@ struct EdgeListDecoder {
   const InputFile& f;
   bool want_value;
   EdgeArrays* out;
+  WccSink* wcc = nullptr;  // instead of out (without values)
   LineTiles text;
   DevBuf<LoadCounters> ctr;
   DevBuf<uint64_t> dec_off;
@@ -727,9 +893,13 @@ struct EdgeListDecoder {
   gb_status begin() {
     GB_TRY(ctr.alloc(1));
     GB_CUDA(cudaMemsetAsync(ctr.p, 0, sizeof(LoadCounters), s));
+    if (wcc) GB_TRY(wcc->start(s, 0));
     return text.begin();
   }
-  gb_status stage(const Chunk& c, DeviceStaging& st) { return text.stage(c, st); }
+  gb_status stage(const Chunk& c, DeviceStaging& st) {
+    if (wcc) GB_TRY(wcc->staging(c, st.sp.copy));
+    return text.stage(c, st);
+  }
   gb_status before(const Chunk& c) {
     GB_TRY(text.count(c, s));
     GB_CUDA(cudaMemcpyAsync(text.host + 1, &ctr.p->declined, 4, cudaMemcpyDeviceToHost, s));
@@ -738,6 +908,15 @@ struct EdgeListDecoder {
   gb_status after(const Chunk& c) {
     GB_CUDA(cudaStreamSynchronize(s));
     const uint64_t lines = text.lines(c);
+    if (wcc) {
+      GB_TRY(wcc->scratch(lines));
+      k_load_parse_text<<<(unsigned)LineTiles::tiles(c), LOAD_BLOCK, 0, s>>>(
+          reinterpret_cast<const uint4*>(c.dev), c.len, text.counts.p, 0, c.off, 0, wcc->src.p, wcc->dst.p, nullptr,
+          ctr.p, nullptr, nullptr);
+      GB_CUDA(cudaGetLastError());
+      m += lines;
+      return wcc->link_pairs(lines, &ctr.p->wide);
+    }
     // size the arrays for the whole file from the lines per byte seen so far
     const uint64_t est = (uint64_t)((double)(m + lines) * (double)f.bytes / (double)c.b * 1.02) + 1024;
     const uint64_t want = std::max(est, out->src.n + out->src.n / 2);
@@ -761,6 +940,10 @@ struct EdgeListDecoder {
     GB_CUDA(cudaMemcpyAsync(&hc, ctr.p, sizeof hc, cudaMemcpyDeviceToHost, s));
     GB_CUDA(cudaStreamSynchronize(s));
     GB_REQUIRE(hc.wide == 0, "edge list node id does not fit 32 bits");
+    if (wcc) {
+      info->edges = m;
+      return wcc->finish_pairs(m);
+    }
     // declined values: re-read each line and parse it with the host reader's own function
     if (hc.declined) {
       std::vector<uint64_t> off(hc.declined);
@@ -797,6 +980,7 @@ struct DotGraphDecoder {
   cudaStream_t s;
   const DotHeader& h;
   uint32_t *labels, *src, *dst;
+  WccSink* wcc = nullptr;  // instead of the arrays (labels not kept)
   LineTiles text;
   DevBuf<unsigned long long> first_error;  // line << 3 | code of the first bad line
   uint64_t line = 0;  // lines so far, the header included
@@ -805,12 +989,36 @@ struct DotGraphDecoder {
     GB_TRY(text.begin());
     GB_TRY(first_error.alloc(1));
     GB_CUDA(cudaMemsetAsync(first_error.p, 0xFF, 8, s));
+    if (wcc) GB_TRY(wcc->start(s, 0));
     return GB_OK;
   }
-  gb_status stage(const Chunk& c, DeviceStaging& st) { return text.stage(c, st); }
+  gb_status stage(const Chunk& c, DeviceStaging& st) {
+    if (wcc) GB_TRY(wcc->staging(c, st.sp.copy));
+    return text.stage(c, st);
+  }
   gb_status before(const Chunk& c) { return text.count(c, s); }
   gb_status after(const Chunk& c) {
     GB_CUDA(cudaStreamSynchronize(s));
+    if (wcc) {
+      // the chunk's edge lines N + 1 + e, e in [e0, e1), go to the pairs; a bad line leaves its pair (0, 0)
+      const uint64_t first_edge_line = (uint64_t)h.nodes + 1, lines = text.lines(c);
+      const uint64_t a = std::max(line, first_edge_line), b = std::min(line + lines, first_edge_line + h.edges);
+      const uint64_t e0 = a - first_edge_line, count = b > a ? b - a : 0;
+      uint32_t *ps = nullptr, *pd = nullptr;
+      if (count) {
+        GB_TRY(wcc->scratch(count));
+        GB_CUDA(cudaMemsetAsync(wcc->src.p, 0, count * 4, s));
+        GB_CUDA(cudaMemsetAsync(wcc->dst.p, 0, count * 4, s));
+        ps = wcc->src.p - e0;  // the kernel stores edge e at src[e]
+        pd = wcc->dst.p - e0;
+      }
+      k_load_parse_dotgraph<<<(unsigned)LineTiles::tiles(c), LOAD_BLOCK, 0, s>>>(
+          reinterpret_cast<const uint4*>(c.dev), c.len, text.counts.p, line, h.nodes, h.lines, nullptr, ps, pd,
+          first_error.p);
+      GB_CUDA(cudaGetLastError());
+      line += lines;
+      return wcc->link_pairs(count, nullptr);
+    }
     k_load_parse_dotgraph<<<(unsigned)LineTiles::tiles(c), LOAD_BLOCK, 0, s>>>(
         reinterpret_cast<const uint4*>(c.dev), c.len, text.counts.p, line, h.nodes, h.lines, labels, src, dst,
         first_error.p);
@@ -825,6 +1033,7 @@ struct DotGraphDecoder {
     if (first != ~0ull) return dot_fail((uint32_t)(first & 7), (first >> 3) + 1, h, 0);
     if (line < h.lines) return dot_fail(DOT_MISSING, 0, h, line);
     info->edges = h.edges;
+    if (wcc) return wcc->finish_pairs(h.edges);
     return GB_OK;
   }
 };
@@ -832,20 +1041,38 @@ struct DotGraphDecoder {
 // The CSR (or label) arrays a binary file's section fills.  Elements of `stride` bytes start at file byte `pos`
 // with an id (or label) of `width` bytes; a u32 section without values (stride 4) is DMA'd straight into `ids`,
 // the others are staged and split by k_bin_split.  first_wide: see k_bin_split (NULL: the `wide` flag).
+// A section whose targets a WccSink links (link = its CSR) is always staged: its chunks are split into the sink's
+// scratch and linked there.
 struct BinSection {
   uint64_t pos = 0, count = 0;
   uint32_t stride = 0, width = 0;
   uint32_t* ids = nullptr;
   float* w = nullptr;
   unsigned int* first_wide = nullptr;
-  bool direct() const { return stride == 4; }
+  int link = -1;
+  bool direct() const { return stride == 4 && link < 0; }
   uint64_t end() const { return pos + count * stride; }
 };
 
+// check_loaded_csrs's verdicts on CSR c: its offsets' first and last entries and decreasing rows, then its targets
+// >= n
+static gb_status bin_csr_verdict(const BinLayout& l, unsigned c, uint32_t first, unsigned int bad_rows, uint32_t last,
+                                 unsigned int bad_targets) {
+  const char* what = bin_csr_name(l, c);
+  GB_REQUIRE(first == 0, "%s offsets[0] must be 0", what);
+  GB_TRY(require_monotone(what, bad_rows));
+  GB_REQUIRE(last == l.entries, "%s offsets end at %u, not at its %llu entries", what, last,
+             (unsigned long long)l.entries);
+  return require_ids(what, bad_targets, l.n);
+}
+static gb_status bin_wide_verdict(unsigned int wide) {
+  GB_REQUIRE(wide == 0, "binary graph file: an id or offset does not fit 32 bits");
+  return GB_OK;
+}
+
 // the checks of gb_binary_decode on the device arrays: offsets[0] == 0, monotone, offsets[n] == entries, targets
 // below n; `wide` is the flag of the narrowing kernel
-static gb_status check_loaded_csrs(gb_graph* g, const BinLayout& l, DevCsr* const* csr, unsigned int* d_wide,
-                                   cudaStream_t s) {
+static gb_status check_loaded_csrs(const BinLayout& l, DevCsr* const* csr, unsigned int* d_wide, cudaStream_t s) {
   DevBuf<unsigned int> bad;  // per CSR: [2c] targets >= n, [2c + 1] decreasing rows
   DevBuf<uint32_t> ends;     // per CSR: offsets[0], offsets[n]
   GB_TRY(bad.alloc(4));
@@ -864,26 +1091,21 @@ static gb_status check_loaded_csrs(gb_graph* g, const BinLayout& l, DevCsr* cons
   GB_CUDA(cudaMemcpyAsync(h + 4, d_wide, 4, cudaMemcpyDeviceToHost, s));
   GB_CUDA(cudaMemcpyAsync(e, ends.p, 16, cudaMemcpyDeviceToHost, s));
   GB_CUDA(cudaStreamSynchronize(s));
-  GB_REQUIRE(h[4] == 0, "binary graph file: an id or offset does not fit 32 bits");
-  for (unsigned c = 0; c < l.ncsr; ++c) {
-    const char* what = bin_csr_name(l, c);
-    GB_REQUIRE(e[2 * c] == 0, "%s offsets[0] must be 0", what);
-    GB_TRY(require_monotone(what, h[2 * c + 1]));
-    GB_REQUIRE(e[2 * c + 1] == l.entries, "%s offsets end at %u, not at its %llu entries", what, e[2 * c + 1],
-               (unsigned long long)l.entries);
-    GB_TRY(require_ids(what, h[2 * c], g->n));
-  }
+  GB_TRY(bin_wide_verdict(h[4]));
+  for (unsigned c = 0; c < l.ncsr; ++c) GB_TRY(bin_csr_verdict(l, c, e[2 * c], h[2 * c + 1], e[2 * c + 1], h[2 * c]));
   return GB_OK;
 }
 
 // Binary graph files, into the CSR arrays of g (and its label array, for a labelled layout l).  A staged chunk
 // carries at most 15 bytes of a cut element in front, and k_bin_split decodes the elements that end inside the
-// chunk.
+// chunk.  With a WccSink (g NULL, l directed without labels) the offsets go into the sink's CSRs and each chunk's
+// targets into its scratch, where they are linked.
 struct BinaryDecoder {
   cudaStream_t s;
   gb_graph* g;
   const BinLayout& l;
   bool want_value;
+  WccSink* wcc = nullptr;
   std::vector<BinSection> secs;
   DevBuf<unsigned int> wide;        // an id or offset does not fit 32 bits
   DevBuf<unsigned int> label_wide;  // the smallest node whose 8-byte label does not fit 32 bits, or ~0
@@ -899,26 +1121,31 @@ struct BinaryDecoder {
       sec.first_wide = label_wide.p;
       secs.push_back(sec);
     }
-    DevCsr* csr[2] = {&g->out, &g->in};
     for (unsigned c = 0; c < l.ncsr; ++c) {
-      DevCsr& d = *csr[c];
+      DevCsr& d = *csr(c);
       d.len = l.entries;
       GB_TRY(d.off.alloc((size_t)l.n + 1));
-      GB_TRY(d.tgt.alloc(l.entries, 8));
-      GB_CUDA(cudaMemsetAsync(d.tgt.p + l.entries, 0, 8 * 4, s));
+      if (!wcc) {
+        GB_TRY(d.tgt.alloc(l.entries, 8));
+        GB_CUDA(cudaMemsetAsync(d.tgt.p + l.entries, 0, 8 * 4, s));
+      }
       if (c == 0 && want_value) GB_TRY(d.w.alloc(l.entries, 8));  // the out-CSR or the undirected CSR; no in-CSR values
       BinSection o, t;
       o.pos = l.csr[c].off_pos, o.count = (uint64_t)l.n + 1, o.stride = o.width = l.id_bytes, o.ids = d.off.p;
       t.pos = l.csr[c].rec_pos, t.count = l.entries, t.stride = l.rec_bytes, t.width = l.id_bytes, t.ids = d.tgt.p;
       t.w = d.w.p;
+      if (wcc) t.link = (int)c;
       secs.push_back(o);
       if (t.count) secs.push_back(t);
     }
     GB_TRY(wide.alloc(1));
     GB_CUDA(cudaMemsetAsync(wide.p, 0, 4, s));
+    if (wcc) return wcc->start(s, l.n);
     return GB_OK;
   }
+  DevCsr* csr(unsigned c) const { return wcc ? &wcc->csr[c] : c == 0 ? &g->out : &g->in; }
   gb_status stage(const Chunk& c, DeviceStaging& st) {
+    if (wcc) GB_TRY(wcc->staging(c, st.sp.copy));
     bool staged = false;
     for (const BinSection& sec : secs) staged |= !sec.direct() && sec.pos < c.b && sec.end() > c.a;
     if (staged) GB_TRY(st.stage(c.k, carry.data(), carry.size(), c.b - c.a));
@@ -945,6 +1172,16 @@ struct BinaryDecoder {
       const uint64_t first = c.a > sec.pos ? (c.a - sec.pos) / sec.stride : 0;  // the first element that ends after a
       const uint64_t last = std::min(sec.count, (c.b - sec.pos) / sec.stride);   // elements that end by b
       if (last <= first) continue;
+      if (sec.link >= 0) {
+        // elements [first, last) as elements [0, last - first) of a section that starts `first` elements later
+        GB_TRY(wcc->scratch(last - first, false));
+        k_bin_split<<<grid_for(last - first, 256), 256, 0, s>>>(c.dev, c.off, sec.pos + first * sec.stride, sec.stride,
+                                                               sec.width, 0, last - first, wcc->src.p, nullptr, wide.p,
+                                                               nullptr);
+        GB_CUDA(cudaGetLastError());
+        GB_TRY(wcc->link_targets((unsigned)sec.link, l, first, last - first));
+        continue;
+      }
       k_bin_split<<<grid_for(last - first, 256), 256, 0, s>>>(c.dev, c.off, sec.pos, sec.stride, sec.width, first,
                                                              last - first, sec.ids, sec.w, wide.p, sec.first_wide);
       GB_CUDA(cudaGetLastError());
@@ -958,9 +1195,21 @@ struct BinaryDecoder {
       GB_CUDA(cudaStreamSynchronize(s));
       if (first != 0xFFFFFFFFu) return bin_label_wide(first);
     }
-    DevCsr* csr[2] = {&g->out, &g->in};
-    GB_TRY(check_loaded_csrs(g, l, csr, wide.p, s));
     info->edges = l.kind == GB_KIND_DIRECTED ? l.entries : l.entries / 2;
+    if (wcc) {  // check_loaded_csrs's verdicts, on the checks made along the way
+      unsigned int h[3] = {0, 0, 0};
+      GB_CUDA(cudaMemcpyAsync(h, wide.p, 4, cudaMemcpyDeviceToHost, s));
+      GB_CUDA(cudaMemcpyAsync(h + 1, wcc->bad.p, 8, cudaMemcpyDeviceToHost, s));
+      GB_CUDA(cudaStreamSynchronize(s));
+      GB_TRY(bin_wide_verdict(h[0]));
+      for (unsigned c = 0; c < l.ncsr; ++c) {
+        GB_TRY(wcc->check_offsets(c, l.n));
+        GB_TRY(bin_csr_verdict(l, c, wcc->off_first[c], wcc->off_bad[c], wcc->off_last[c], h[1 + c]));
+      }
+      return wcc->finish();
+    }
+    DevCsr* csr[2] = {&g->out, &g->in};
+    GB_TRY(check_loaded_csrs(l, csr, wide.p, s));
     return GB_OK;
   }
 };
@@ -1312,7 +1561,66 @@ gb_status load_edge_arrays(int device, const char* path, gb_file_format format, 
   return stream_edges(device, f, format, with_values, out, &out->info);
 }
 
+thread_local gb_wcc_file_stats wcc_file_last{};  // behind gb_wcc_file_info
+
+// gb_wcc_file_u32: the file as load_graph(device, GB_KIND_DIRECTED, path, format, GB_LAYOUT_UNSORTED, 0) reads it
+// on its streamed path, every decoded chunk handed to a WccSink.  The checks come in the load's order.
+static gb_status wcc_file(int device, const char* path, gb_file_format format, const gb_wcc_config* cfg,
+                          gb_components** out) {
+  wcc_file_last = gb_wcc_file_stats{};
+  GB_REQUIRE(out != nullptr, "components out-pointer is NULL");
+  GB_REQUIRE(cfg != nullptr, "config is NULL");  // chunk_size / neighbor_rounds / sampling_size: labels unchanged
+  GB_REQUIRE(path != nullptr, "path is NULL");
+  GB_REQUIRE(format == GB_FORMAT_GRAPH500 || format == GB_FORMAT_EDGE_LIST || format == GB_FORMAT_BINARY ||
+                 format == GB_FORMAT_DOTGRAPH,
+             "unknown file format %d", (int)format);
+  GB_TRY(require_device(device));
+  DeviceGuard guard(device);
+  InputFile f;
+  GB_TRY(f.open(path));
+  DevBufTally tally;
+  WccSink sink;
+  gb_load_info info{};
+  info.file_bytes = f.bytes;
+  if (format == GB_FORMAT_GRAPH500) {
+    GB_TRY(stream_file<Graph500Decoder>(device, f, 12 * (f.bytes / 12), 48, &info, f.bytes / 12, nullptr, &sink));
+  } else if (format == GB_FORMAT_EDGE_LIST) {
+    GB_TRY(stream_file<EdgeListDecoder>(device, f, f.bytes, 1, &info, f, false, nullptr, &sink));
+  } else if (format == GB_FORMAT_DOTGRAPH) {
+    std::string head;
+    GB_TRY(f.read_line(0, 4096, &head));
+    DotHeader h;
+    GB_TRY(dot_read_header(head.data(), head.size(), &h));
+    GB_TRY(stream_file<DotGraphDecoder>(device, f, f.bytes, 1, &info, h, nullptr, nullptr, nullptr, &sink));
+    GB_TRY(dot_require_fits(h, dot_fits(h, f.bytes)));
+  } else {
+    BinLayout l;
+    GB_TRY(bin_parse([&](uint64_t pos, void* dst, uint64_t n) { return pread_all(f.fd, static_cast<char*>(dst), n, pos); },
+                     f.bytes, GB_KIND_DIRECTED, &l));
+    GB_TRY(stream_file<BinaryDecoder>(device, f, f.bytes, 1, &info, nullptr, l, false, &sink));
+  }
+  // an empty Graph500 or edge-list file streams no chunk (the load's build reports it)
+  GB_REQUIRE(info.chunks > 0, "cannot infer node_count from an empty edge list");
+  std::unique_ptr<gb_components> c(new (std::nothrow) gb_components());
+  GB_REQUIRE(c != nullptr, "host allocation failed");
+  c->device = device;
+  c->n = (uint32_t)sink.n;
+  c->labels = std::move(sink.parent);
+  c->labels.untally();  // the handle outlives the call
+  gb_wcc_file_stats& w = wcc_file_last;
+  w.file_bytes = info.file_bytes;
+  w.chunks = info.chunks;
+  w.edges = info.edges;
+  w.h2d_bytes = info.h2d_bytes;
+  w.device_bytes = tally.peak;
+  w.node_count = c->n;
+  w.total_ms = sink.total_ms;
+  *out = c.release();
+  return GB_OK;
+}
+
 }  // namespace gb
+
 
 extern "C" {
 
@@ -1360,6 +1668,37 @@ gb_status gb_graph_serialize_labeled(const gb_graph* graph, const char* path) {
 gb_status gb_graph_load_info(const gb_graph* g, gb_load_info* info) {
   GB_REQUIRE(g && info, "NULL argument");
   *info = g->load;
+  return GB_OK;
+}
+
+gb_status gb_wcc_file_u32(int device, const char* path, gb_file_format format, const gb_wcc_config* config,
+                          gb_components** out) {
+  return gb::wcc_file(device, path, format, config, out);
+}
+
+gb_status gb_components_node_count(const gb_components* c, uint32_t* node_count) {
+  GB_REQUIRE(c && node_count, "NULL argument");
+  *node_count = c->n;
+  return GB_OK;
+}
+
+gb_status gb_components_copy(const gb_components* c, uint32_t* labels) {
+  GB_REQUIRE(c && labels, "NULL argument");
+  gb::DeviceGuard guard(c->device);
+  GB_CUDA(cudaMemcpy(labels, c->labels.p, (size_t)c->n * 4, cudaMemcpyDeviceToHost));
+  return GB_OK;
+}
+
+gb_status gb_components_free(gb_components* c) {
+  if (!c) return GB_OK;
+  gb::DeviceGuard guard(c->device);
+  delete c;
+  return GB_OK;
+}
+
+gb_status gb_wcc_file_info(gb_wcc_file_stats* info) {
+  GB_REQUIRE(info != nullptr, "info is NULL");
+  *info = gb::wcc_file_last;
   return GB_OK;
 }
 

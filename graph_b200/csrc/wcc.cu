@@ -273,6 +273,46 @@ __global__ void k_cc_merge_halving(uint32_t* parent, const uint32_t* __restrict_
   }
 }
 
+// ---- the WCC of a graph file (gb_wcc_file_u32, load.cu): links of decoded chunks ---------------------------
+__global__ void k_cc_init_range(uint32_t* parent, uint64_t from, uint64_t to) {
+  for (uint64_t v = from + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; v < to;
+       v += (uint64_t)gridDim.x * blockDim.x)
+    parent[v] = (uint32_t)v;
+}
+
+// One chunk's (src, dst) pairs, linked with link_halving: a file may list a path in id order, and af_link would then
+// walk chains as long as the chunk.  A pair with an endpoint >= n is not linked; its endpoints >= n are counted.
+__global__ void __launch_bounds__(256) k_cc_link_pairs(const uint32_t* __restrict__ src,
+                                                       const uint32_t* __restrict__ dst, uint64_t count, uint32_t n,
+                                                       uint32_t* parent, unsigned int* bad) {
+  unsigned int nbad = 0;
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < count;
+       i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t u = src[i], v = dst[i];
+    const unsigned int out = (u >= n ? 1u : 0u) + (v >= n ? 1u : 0u);
+    if (out) nbad += out;
+    else link_halving(parent, u, v);
+  }
+  nbad = __reduce_add_sync(0xFFFFFFFFu, nbad);
+  if ((threadIdx.x & 31) == 0 && nbad) atomicAdd(bad, nbad);
+}
+
+void cc_init_async(cudaStream_t s, uint32_t* parent, uint64_t from, uint64_t to) {
+  if (to > from) k_cc_init_range<<<grid_for(to - from, 256), 256, 0, s>>>(parent, from, to);
+}
+void cc_link_pairs_async(cudaStream_t s, const uint32_t* src, const uint32_t* dst, uint64_t count, uint32_t n,
+                         uint32_t* parent, unsigned int* bad) {
+  if (count) k_cc_link_pairs<<<grid_for(count, 256), 256, 0, s>>>(src, dst, count, n, parent, bad);
+}
+void cc_link_csr_async(cudaStream_t s, const uint32_t* off, uint32_t n, const uint32_t* tgt, uint32_t e0,
+                       uint32_t len, uint32_t* parent, unsigned int* bad) {
+  if (len)
+    k_cc_link_edges<<<grid_for(len, LINK_TILE * (256 / 32)), 256, 0, s>>>(off, n, 0, tgt, e0, len, n, parent, bad);
+}
+void cc_compress_async(cudaStream_t s, uint32_t* parent, uint32_t n) {
+  k_cc_compress<<<grid_for(n, 256), 256, 0, s>>>(parent, n);
+}
+
 static gb_status wcc_impl(const gb_graph* g, const gb_wcc_config* cfg, uint32_t* d_comp, uint32_t* h_comp) {
   GB_REQUIRE(g && cfg, "NULL argument");
   if (g->kind != GB_KIND_DIRECTED)

@@ -544,6 +544,40 @@ gb_status gb_wcc_device(const gb_graph* graph, const gb_wcc_config* config, uint
 gb_status gb_wcc_csr_u32(int device, uint32_t node_count, const uint32_t* offsets, const uint32_t* targets,
                          const gb_wcc_config* config, uint32_t* components);
 
+/* wcc(&GraphBuilder::new().file_format(F).path(p).build::<DirectedCsrGraph<u32>>()) in one pass over the file, with
+ * no twin, no CSR and no edge arrays: the file is read exactly as gb_digraph_load_u32(device, path, format,
+ * GB_LAYOUT_UNSORTED, 0, ...) reads it (every format, every file size through the streamed pipeline, chunks of
+ * GB_LOAD_CHUNK_BYTES when set), and every chunk's edges are linked into a parent array on the device as soon as
+ * they are decoded, while the next chunk crosses the bus.
+ *   - Result: the load's node_count, and per node the minimum node id of its component, bit-equal to gb_wcc on the
+ *     loaded twin.  A binary file's out- and in-CSR are both linked, as gb_wcc links both lists.
+ *   - Failures: where the load fails, with its status and message, with one exception: Graph500, edge-list and
+ *     DotGraph files of 2^32 - 1 edges or more are accepted (nothing stores an edge offset).  Binary files keep
+ *     the load's limits.  config is checked and otherwise ignored, as by gb_wcc_csr_u32.
+ *   - Device memory: the parent array (4 bytes per node; an edge list's grows by doubling as larger ids come), the
+ *     pipeline's staging buffers, one chunk of decoded pairs, and for a binary file its offsets sections
+ *     (4(n + 1) bytes each); nothing grows with the edge count.
+ * *out receives a handle that keeps the labels on the device until gb_components_free. */
+typedef struct gb_components gb_components;
+gb_status gb_wcc_file_u32(int device, const char* path, gb_file_format format, const gb_wcc_config* config,
+                          gb_components** out);
+gb_status gb_components_node_count(const gb_components* components, uint32_t* node_count);
+/* node_count labels into host memory */
+gb_status gb_components_copy(const gb_components* components, uint32_t* labels);
+gb_status gb_components_free(gb_components* components);
+/* Statistics of the calling thread's last gb_wcc_file_u32 (all zero after a failed call).  The struct is not
+ * called gb_wcc_file_info: C gives a typedef and a function one name space. */
+typedef struct gb_wcc_file_stats {
+  uint64_t file_bytes;   /* size of the file */
+  uint64_t chunks;       /* pinned buffers the file was streamed through */
+  uint64_t edges;        /* edges read (a binary directed file: its entries) */
+  uint64_t h2d_bytes;    /* bytes copied host -> device */
+  uint64_t device_bytes; /* peak bytes the call held on the device */
+  uint32_t node_count, reserved;
+  double total_ms;       /* CUDA-event time from the first copy to the last link */
+} gb_wcc_file_stats;
+gb_status gb_wcc_file_info(gb_wcc_file_stats* info);
+
 /* Multi-GPU WCC (1-D cut by vertex range, one process per GPU; the caller owns the exchange of the
  * parent arrays, e.g. an NCCL all-gather).  The phases of wcc() (wcc.rs:158-183) restricted to the rank's
  * vertices [vertex_begin, vertex_end) over a FULL parent[n] on every rank:

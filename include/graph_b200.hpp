@@ -596,6 +596,25 @@ inline Components wcc_baseline_csr(std::uint32_t node_count, const std::uint32_t
   detail::check(gb_wcc_csr_u32(device, node_count, offsets, targets, &cfg, out.ids.data()));
   return out;
 }
+// wcc(&GraphBuilder::new().file_format(format).path(path).build::<DirectedCsrGraph<u32>>()) in one pass over the
+// file, without building the graph (gb_wcc_file_u32): each chunk's edges are linked on the device as they are
+// decoded.  The labels of wcc_afforest on the loaded graph; throws graph::Error where the load fails, except that
+// Graph500, edge-list and DotGraph files of 2^32 - 1 edges or more are accepted.
+inline Components wcc_file(const std::string& path, FileFormat format, WccConfig c = {}, int device = 0) {
+  gb_wcc_config cfg{c.chunk_size, c.neighbor_rounds, c.sampling_size};
+  gb_components* h = nullptr;
+  detail::check(gb_wcc_file_u32(device, path.c_str(), static_cast<gb_file_format>(format), &cfg, &h));
+  struct Free {
+    gb_components* h;
+    ~Free() { gb_components_free(h); }
+  } free_h{h};
+  std::uint32_t n = 0;
+  detail::check(gb_components_node_count(h, &n));
+  Components out;
+  out.ids.resize(n);
+  detail::check(gb_components_copy(h, out.ids.data()));
+  return out;
+}
 // global_triangle_count of a host undirected CSR (same layout), streamed to the device in row-aligned chunks and
 // counted as they land, without a resident twin (gb_triangle_count_csr_u32); the number global_triangle_count
 // gives on UndirectedCsrGraph::from_csr of the same arrays
